@@ -1,11 +1,12 @@
 #!/usr/bin/env python
-"""bench.py -- PVNet per-image inference hot path on B200: images/sec (480x640, K=9),
+"""bench.py -- PVNet per-image inference hot path on H100: images/sec (480x640, K=9),
 backbone (Resnet18_8s) + RANSAC vote (ransac_voting_layer_v3).
 
     python bench.py --gpus N --steps K --warmup W            # our arm
     python bench.py --impl reference --gpus N --steps K ...  # the reference's CPU path (rank 0)
     torchrun --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
     python bench.py --config 4 | --config 5                  # another BASELINE config as the headline
+    python bench.py ... --dump-outputs DIR                   # also write the last timed step's results as .npy
 
 One "step" = one batch of 16 synthetic 480x640 images per GPU (BASELINE config 2, the headline at
 every N so that the per-GPU work is fixed -- "weak" scaling):
@@ -22,11 +23,17 @@ the same process at the same N, so a 1/2/4/8 run yields config 4's scaling as we
 Prints ONE JSON line (rank 0).  `value` = device-resident inputs; `e2e` = the same step
 through the public API (PoseKeypointPipeline) from pinned HOST buffers -- raw uint8 HWC images,
 normalised on the device -- with the H2D of the image batch and the D2H of the keypoints (and
-covariances) inside the timed region.  Also: `roofline` of the dominant kernel (the tcgen05
+covariances) inside the timed region.  Also: `roofline` of the dominant kernel (the wgmma
 convolutions, timed per layer with CUDA events inside this process), `roofline_vote` (the voting
 layer timed in place: tests/s, FP32-issue fraction, algorithmic HBM GB/s), `cpu_baseline` (the same
 workload on the host cores: the reference graph under torch CPU + the oracle port of the voting
 kernels, bounded sample), `clocks`, `gpu_launches`.
+
+--dump-outputs DIR writes what the last timed device-resident step returned to its caller:
+DIR/keypoints.npy [batch,K,2] float32 (and DIR/covariance.npy [batch,K,2,2] float32 with the
+covariance configs); under torchrun the batch gathered from every rank, written by rank 0; with
+--impl reference the host path's keypoints [1,K,2].  Inputs, weights and the in-kernel sampling are seeded, so two builds run
+with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -46,10 +53,6 @@ if ROOT not in sys.path:
 
 H, W, K_KP, HYP, BATCH = 480, 640, 9, 256, 16
 THRESH = 0.99
-VOTE_ISSUE_SLOTS_PER_TEST = 5.0   # k_vote3's sweep in SASS: 160 instructions per 32 tests = 2 FFMA2 + FADD + LEA.HI + 1/2 FMNMX3
-#                                   per test + 12 LDS.128 + 4 loop instructions; also its FMA-pipe cycles (FFMA2 = 2)
-VOTE_MICRO_CYCLES_PER_TEST = 7.17  # that mix alone, in registers, at the kernel's 4 resident warps per sub-partition
-#                                    (profiles/r02_micro_vote_mix.txt row 16; 6.32 at 6 warps): what the SM sustains
 
 # BASELINE.json configs that bench.py can run as the headline (per-GPU batch: weak scaling)
 CONFIGS = {
@@ -86,7 +89,7 @@ def _rank_world():
 
 # ----------------------------------------------------------------------------- clocks
 class ClockSampler:
-    """nvidia-smi sampling during the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi sampling during the timed region (SM clock and throttle reasons under load)."""
 
     def __init__(self, gpu_index):
         self.gpu = gpu_index
@@ -176,23 +179,9 @@ def make_step(torch, net, with_cov=False):
 
 
 # ----------------------------------------------------------------------------- roofline
-def _ncu_traffic():
-    """DRAM bytes (read+write) of the conv launches of one step from the committed ncu --set full
-    capture; NOT measured in this run (the profiler cannot run inside the timed process)."""
-    for name in ("r02_conv_dram_traffic.json", "r01_conv_dram_traffic.json"):
-        try:
-            d = json.load(open(os.path.join(ROOT, "profiles", name)))
-            return {"dram_bytes_per_step": d["bytes_per_step"], "source": d["source"], "measured": False,
-                    "note": f"constant read from profiles/{name} (one ncu --set full capture of the same step), "
-                            "not re-measured by this run"}
-        except Exception:
-            continue
-    return None
-
-
 def conv_roofline(torch, net, x, peaks, k=K_KP):
     """Per-stage device time of one forward pass, CUDA events recorded on the launch stream
-    between the single-kernel stages; aggregates the tcgen05 convolution launches."""
+    between the single-kernel stages; aggregates the wgmma convolution launches."""
     import ctypes
 
     from pvnet_b200 import _native
@@ -232,27 +221,26 @@ def conv_roofline(torch, net, x, peaks, k=K_KP):
     gflop_img = GFLOP_PER_IMAGE + 0.039 * (k - K_KP)               # SURVEY App. B: +0.039 GFLOP per extra keypoint
     flops = gflop_img * 1e9 * b
     achieved = flops / (conv_ms * 1e-3) / 1e12
-    bf16 = peaks.get("bf16_tflops_sustained") or peaks.get("bf16_tflops") or 1590.0
+    # dense TF32 = half the dense BF16 rate; fallback: the H100 SXM data sheet's 989 TFLOP/s BF16 (a card at 700 W)
+    bf16 = peaks.get("bf16_tflops_sustained") or peaks.get("bf16_tflops") or 989.0
     peak = bf16 / 2.0
     stages = [{"stage": nm, "ms": round(float(t), 4)} for nm, t in zip(names, ms)]
     return {
-        "bound": "tensor", "kernel": "k_conv_tap_p + k_conv_col (tcgen05.mma kind::tf32; every conv of the network incl. "
+        "bound": "tensor", "kernel": "k_conv_tap + k_conv_col (wgmma tf32; every conv of the network incl. "
                                      "stem and fused 1x1 head)",
         "achieved": round(achieved, 2), "peak": round(peak, 1), "unit": "TFLOP/s", "frac": round(achieved / peak, 4),
-        "peak_source": ("MEASURED_PEAKS.json bf16_tflops_sustained / 2 (tcgen05 tf32 = half the bf16 rate)"
-                        if "bf16_tflops_sustained" in peaks else "fallback 1590/2"),
+        "peak_source": ("MEASURED_PEAKS.json bf16_tflops_sustained / 2 (tf32 = half the bf16 rate)"
+                        if "bf16_tflops_sustained" in peaks else "H100 SXM data sheet 989/2 (not a measured rate)"),
         "algorithmic_gflop_per_launch_set": round(flops / 1e9, 1), "conv_ms_per_step": round(conv_ms, 3),
         "backbone_ms_per_step": round(backbone_ms, 3),
         "frac_whole_backbone": round(flops / (backbone_ms * 1e-3) / 1e12 / peak, 4),
-        "traffic": _ncu_traffic(),
     }, stages
 
 
 def vote_roofline(torch, pipe, x, peaks, clocks, cfg):
     """The voting layer timed in place (CUDA events around the public call on the launch stream, 20
-    back-to-back repetitions after 5 warm ones, median): inlier tests per second, the fraction of the
-    FP32-issue roof (tests x instructions per test / (SMs x 128 lanes x clock)) and the algorithmic
-    HBM rate B_alg / t against the measured copy bandwidth (SURVEY.md section 8d)."""
+    back-to-back repetitions after 5 warm ones, median): inlier tests per second and the algorithmic
+    HBM rate B_alg / t against the HBM bandwidth (SURVEY.md section 8d)."""
     from pvnet_b200 import ransac_voting_gpu as rv
     net = pipe.net
     out, mask = net.forward_native(x, with_mask=True, mask_dtype=torch.uint8, pixel_major=True)     # as pipe.step does
@@ -279,27 +267,18 @@ def vote_roofline(torch, pipe, x, peaks, clocks, cfg):
     torch.cuda.synchronize()
     ms = float(np.median([e0.elapsed_time(e1) for e0, e1 in evs]))
     tests = float(tn.sum()) * k * (hn + hnt + 1)                    # +1: the winner's vote of the refit
-    clk = ((clocks or {}).get("sm_mhz") or 1900.0) * 1e6
-    sms = torch.cuda.get_device_properties(x.device).multi_processor_count
-    issue_roof = sms * 128 * clk / VOTE_ISSUE_SLOTS_PER_TEST
-    micro_roof = sms * 128 * clk / VOTE_MICRO_CYCLES_PER_TEST
     b_alg = b * (h * w * 1 + k * 24 + (hn + hnt) * k * 8) + float(tn.sum()) * k * 8
-    hbm = peaks.get("hbm_gbs") or 6575.0
+    hbm = peaks.get("hbm_gbs") or 3350.0            # fallback: the H100 SXM data sheet's HBM3 bandwidth
     return {
         "kernel": "k_vote3 inside pvnet_ransac_voting_pipeline (whole layer timed: compaction, gather, hypotheses, "
                   "vote, refit" + (", covariance)" if cov else ")"),
         "layer_ms": round(ms, 4), "tests": int(tests), "tests_per_s": round(tests / (ms * 1e-3), 1),
-        "issue_slots_per_test": VOTE_ISSUE_SLOTS_PER_TEST, "micro_cycles_per_32_tests": VOTE_MICRO_CYCLES_PER_TEST,
-        "sm_clock_mhz": round(clk / 1e6, 1),
-        "issue_frac": round(tests / (ms * 1e-3) / issue_roof, 4),
-        "micro_frac": round(tests / (ms * 1e-3) / micro_roof, 4), "bound": "fp32 issue",
+        "bound": "fp32 issue",
         "alg_bytes": int(b_alg), "alg_hbm_gbs": round(b_alg / (ms * 1e-3) / 1e9, 2),
         "alg_hbm_frac": round(b_alg / (ms * 1e-3) / 1e9 / hbm, 5), "hbm_peak_gbs": hbm,
         "fg_px_per_image": round(float(tn.mean()), 1),
         "note": "whole layer timed (10 launches); FP32-issue bound by construction (SURVEY 8d): the [hn,K,tn] inlier tensor the "
-                "reference streams through HBM never exists here; issue_frac = tests/s over SMs x 128 lanes x clock / 5.0 slots, "
-                "micro_frac = over what the instruction mix alone sustains in a register-only microbenchmark at the same "
-                "occupancy; the kernel's own ncu DRAM bytes (1.00x its algorithmic bytes) are in profiles/r02_ncu_vote.md",
+                "reference streams through HBM never exists here",
     }
 
 
@@ -356,19 +335,21 @@ def run_reference_arm(args):
     if rank != 0:
         return
     step, cores = _cpu_path()
-    for _ in range(max(1, min(args.warmup, 2))):
+    for _ in range(args.warmup):
         step()
-    steps = max(1, min(args.steps, 5))
+    steps = args.steps
     t0 = time.perf_counter()
     for _ in range(steps):
-        step()
+        last = step()
     dt = time.perf_counter() - t0
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, last)
     val = steps / dt
     line = {
         "impl": "reference", "metric": "images/sec (480x640, K=9) backbone+vote", "value": round(val, 4),
         "unit": "images/sec", "n_gpus": args.gpus, "steps": steps, "warmup": args.warmup,
         "ms_per_step": round(dt / steps * 1e3, 2), "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-        "dtype": "f32", "data": "synthetic",
+        "dtype": "f32", "data": "synthetic", "gpu": None,
         "config": {"workload": "BASELINE config 2 shape, 1 image/step on the host: Resnet18_8s(18,2) eval forward "
                                "(torch CPU, reference graph) + ransac_voting_layer_v3(256 hyp, thresh 0.99, 20000 fg px)"},
         "cpu_baseline": {"value": round(val, 4), "unit": "images/sec", "cores": cores, "kind": "port",
@@ -382,7 +363,7 @@ def run_reference_arm(args):
 def measure(torch, dist, pd, pipe, xs, hosts, batch, k, steps, warmup, world, sampler=None, rank=0):
     """One configuration, two ways: K steps on device-resident inputs, and the same K steps through
     PoseKeypointPipeline.run from pinned host buffers.  Returns per-rank (ms_device, ms_e2e, launches,
-    clocks or None)."""
+    clocks or None, the last timed device-resident step's result)."""
     from pvnet_b200 import _native
     with_cov = pipe.with_cov
 
@@ -416,8 +397,9 @@ def measure(torch, dist, pd, pipe, xs, hosts, batch, k, steps, warmup, world, sa
         _native.launch_count_reset()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
+        last = None
         for i in range(steps):
-            full_step(xs[i % 3])
+            last = full_step(xs[i % 3])
         e1.record()
         barrier()
         launches = _native.launch_count()
@@ -438,7 +420,28 @@ def measure(torch, dist, pd, pipe, xs, hosts, batch, k, steps, warmup, world, sa
         barrier()
         ms_e2e = f0.elapsed_time(f1)
         clocks = sampler.stop() if (sampler is not None and rank == 0) else None
-    return ms_dev, ms_e2e, launches, clocks
+    return ms_dev, ms_e2e, launches, clocks, last
+
+
+def dump_outputs(d, result):
+    """The arrays the device-resident step hands its caller, as float32 .npy files under d."""
+    os.makedirs(d, exist_ok=True)
+    kp, cov = result if isinstance(result, tuple) else (result, None)
+    f32 = lambda a: (a.float().cpu().numpy() if hasattr(a, "cpu") else np.asarray(a, np.float32))   # noqa: E731
+    np.save(os.path.join(d, "keypoints.npy"), f32(kp))
+    if cov is not None:
+        np.save(os.path.join(d, "covariance.npy"), f32(cov))
+
+
+def gpu_identity(index):
+    """Name, power limit and maximum SM clock of the GPU the numbers were measured on (nvidia-smi)."""
+    try:
+        out = subprocess.run(["nvidia-smi", f"--id={index}", "--query-gpu=name,power.limit,clocks.max.sm",
+                              "--format=csv,noheader,nounits"], capture_output=True, text=True, timeout=30).stdout
+        name, pl, clk = (v.strip() for v in out.strip().splitlines()[0].split(","))
+        return {"name": name, "power_limit_w": float(pl), "sm_max_mhz": float(clk)}
+    except Exception as e:                  # the number still stands; say why its context is missing
+        return {"name": None, "error": str(e)[:200]}
 
 
 def main():
@@ -453,7 +456,11 @@ def main():
     ap.add_argument("--with-cov", action="store_true", help="same as --config 4")
     ap.add_argument("--e2e-input", default="u8", choices=["u8", "f32"],
                     help="host buffers of the e2e arm: raw uint8 HWC images normalised on the device, or float32 NCHW")
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help="write the last timed step's keypoints (and covariances) to DIR as float32 .npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     args.warmup = max(args.warmup, 3)
     if args.with_cov:
         args.config = 4
@@ -481,7 +488,7 @@ def main():
     cfg = CONFIGS[args.config]
     k, batch = cfg["k"], cfg["batch"]
     net = build_model(torch, dev, k)
-    # 3 rotating input batches (3 x 59 MB of activations-in > 126 MB L2); different per rank.  Raw uint8 HWC
+    # 3 rotating input batches (3 x 59 MB of activations-in > 50 MB L2); different per rank.  Raw uint8 HWC
     # images on the host (what a decoder yields); the device-resident arm gets the same images already
     # normalised to float32 NCHW (ToTensor + Normalize, tools/demo.py:89-95).
     rng = np.random.default_rng(1000 * args.config + 17 * rank)
@@ -494,8 +501,14 @@ def main():
     fg = calibrate_foreground(torch, net, xs[0], cfg["fg"])
 
     pipe = make_pipe(net, cfg)
-    ms_total, ms_e2e, launches, clocks = measure(torch, dist, pd, pipe, xs, hosts, batch, k, args.steps, args.warmup, world,
-                                                 ClockSampler(local), rank)
+    ms_total, ms_e2e, launches, clocks, last = measure(torch, dist, pd, pipe, xs, hosts, batch, k, args.steps, args.warmup,
+                                                       world, ClockSampler(local), rank)
+    if args.dump_outputs:
+        if world > 1:       # every rank receives the gathered batch (rank order); rank 0 writes it
+            last = tuple(pd.gather_results(t, batch * world) for t in last) if isinstance(last, tuple) \
+                else pd.gather_results(last, batch * world)
+        if rank == 0:
+            dump_outputs(args.dump_outputs, last)
     extra = None
     if args.config == 2:                             # config 4's per-GPU workload in the same process, same N
         pipe4 = make_pipe(net, CONFIGS[4])
@@ -527,13 +540,14 @@ def main():
             "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
             "ms_per_step": round(ms_total / args.steps, 4), "higher_is_better": True, "scaling": "weak",
             "vs_baseline": None, "dtype": "tf32 (fp32 storage, fp32 accumulate; vote fp32/fp64)", "data": "synthetic",
+            "gpu": gpu_identity(local),
             "config": {"workload": cfg["name"],
                        "global_batch": batch * world, "parallelism": f"batch-sharded dp{world}",
                        "fg_px_per_image": round(fg, 1), "rng": "device (in-kernel Philox)",
                        "weights": "random-init, BN stats randomised",
                        "e2e_input": ("uint8 HWC images, normalised on the device" if args.e2e_input == "u8"
                                      else "float32 NCHW"),
-                       "l2": "3 rotating input batches and a ~3.7 GB activation working set per step, both > 126 MB L2"},
+                       "l2": "3 rotating input batches and a ~3.7 GB activation working set per step, both > 50 MB L2"},
             "e2e": {"value": round(images / (ms_e2e * 1e-3), 2), "unit": "images/sec",
                     "h2d_bytes_per_step": in_bytes, "d2h_bytes_per_step": d2h(cfg["cov"] is not None)},
             "gpu_launches": int(launches),

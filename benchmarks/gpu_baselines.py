@@ -1,4 +1,4 @@
-"""GPU-vs-GPU baselines on the same B200 (BASELINE.md section 4): what the REFERENCE's own CUDA path costs for
+"""GPU-vs-GPU baselines on the same GPU (BASELINE.md section 4): what the REFERENCE's own CUDA path costs for
 the work bench.py times, next to ours, same inputs, CUDA events / synchronize brackets.
 
  (i)  voting: oracle/ref_cuda.layer_v3 (+ layer_cov_with_mean) = the reference's kernels (compiled verbatim

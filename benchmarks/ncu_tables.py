@@ -1,15 +1,15 @@
-"""Turn ncu reports captured on the GPU box into the markdown / JSON summaries under profiles/.
+"""Turn ncu reports into markdown / JSON summaries.
 
-  python benchmarks/ncu_tables.py conv  gpurun_out/conv_full.ncu-rep   profiles/r01_ncu_conv_final.md profiles/r01_conv_dram_traffic.json
-  python benchmarks/ncu_tables.py list  gpurun_out/launches.csv        profiles/r01_ncu_launches_final.md
-  python benchmarks/ncu_tables.py vote  gpurun_out/vote_full.ncu-rep   profiles/r01_ncu_vote_final.md
-  python benchmarks/ncu_tables.py top   gpurun_out/conv_full.ncu-rep   <kernel index> [n]     (hottest source lines)
+  python benchmarks/ncu_tables.py conv  out/conv_full.ncu-rep   conv.md conv_dram_traffic.json
+  python benchmarks/ncu_tables.py list  out/launches.csv        launches.md
+  python benchmarks/ncu_tables.py vote  out/vote_full.ncu-rep   vote.md
+  python benchmarks/ncu_tables.py top   out/conv_full.ncu-rep   <kernel index> [n]     (hottest source lines)
 
 Captures (see the header each table carries):
   conv: ncu --profile-from-start off --set full --clock-control none --import-source on
-        -k regex:"k_conv_tap_p|k_conv_col|k_conv_tc" -c 25 -o gpurun_out/conv_full python benchmarks/profile_step.py 1
+        -k regex:"k_conv_tap|k_conv_col" -c 25 -o out/conv_full python benchmarks/profile_step.py 1
   list: ncu --profile-from-start off --metrics gpu__time_duration.sum --clock-control none --csv
-        --log-file gpurun_out/launches.csv python benchmarks/profile_step.py 2
+        --log-file out/launches.csv python benchmarks/profile_step.py 2
 """
 import csv
 import json
@@ -61,7 +61,7 @@ def conv(rep, md, js, batch=16):
     gm = _gmac()
     lines = ["# ncu --set full, all 25 tensor-core conv launches (stem .. convraw.0 + fused head) of one bench step (batch 16, 480x640)", "",
              "`ncu --profile-from-start off --set full --clock-control none --import-source on -k "
-             "regex:\"k_conv_tap_p|k_conv_col|k_conv_tc\" -c 25 python benchmarks/profile_step.py 1`"
+             "regex:\"k_conv_tap|k_conv_col\" -c 25 python benchmarks/profile_step.py 1`"
              " -> `python benchmarks/ncu_tables.py conv ...`", "",
              "Times are under the profiler (serialised, cold): use shares. TFLOP/s = 2*GMAC*16 / time.", "",
              "`tensor pipe %` = the MMA sub-pipe doing math (max of the sm__*tensor*pct metrics); `tc active %` = "

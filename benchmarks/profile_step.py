@@ -2,7 +2,7 @@
 warm-up step happen BEFORE cudaProfilerStart, so run ncu with `--profile-from-start off`:
 
   ncu --profile-from-start off --metrics gpu__time_duration.sum --clock-control none \
-      --csv --log-file gpurun_out/launches.csv python benchmarks/profile_step.py 2
+      --csv --log-file out/launches.csv python benchmarks/profile_step.py 2
 """
 import os
 import sys

@@ -1,4 +1,4 @@
-"""BASELINE config 3: voting-only sweep on one B200 -- foreground pixel count x hypotheses,
+"""BASELINE config 3: voting-only sweep on one GPU -- foreground pixel count x hypotheses,
 K=9, max_num=10**9 (no subsampling).  Times pvnet_ransac_voting_v3 (whole layer: compaction
 + gather + hypotheses + vote + refit), with CUDA events on the launch
 stream; prints one JSON line per point.  Inputs are flushed from L2 between iterations by
@@ -20,7 +20,9 @@ def main():
     K = 9
     b = int(os.environ.get("SWEEP_BATCH", "4"))
     flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
-    sm_clock = 1.9e9
+    props = torch.cuda.get_device_properties(dev)
+    sm_clock = props.clock_rate * 1e3 if hasattr(props, "clock_rate") else 1.98e9     # maximum SM clock, Hz
+    sms = props.multi_processor_count
     pts = os.environ.get("SWEEP_POINTS")          # e.g. "10000:512,150000:2048"
     want = None if not pts else {(int(a), int(b_)) for a, b_ in (p.split(":") for p in pts.split(","))}
     for n in (1000, 10000, 50000, 150000):
@@ -52,7 +54,7 @@ def main():
             print(json.dumps(dict(n_fg=n, hn=hn, batch=b, ms=round(ms, 4), images_per_s=round(b / ms * 1e3, 1),
                                   gtests_per_s=round(tests / ms / 1e6, 2),
                                   alg_GBps=round(b_alg / ms / 1e6, 2),
-                                  issue_frac_at_8=round(tests * 8 / (148 * 128 * sm_clock) / (ms * 1e-3), 3))),
+                                  issue_frac_at_8=round(tests * 8 / (sms * 128 * sm_clock) / (ms * 1e-3), 3))),
                   flush=True)
 
 

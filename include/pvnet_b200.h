@@ -1,5 +1,5 @@
 /*
- * pvnet_b200.h -- C ABI of libpvnet_b200.so: the B200 (sm_100a) implementation of
+ * pvnet_b200.h -- C ABI of libpvnet_b200.so: the H100 (sm_90a) implementation of
  * PVNet's per-image inference hot path (voting layer + Resnet18_8s backbone).
  *
  * Boundary rules (SURVEY.md §8b):
@@ -261,7 +261,7 @@ PVNET_API void pvnet_launch_count_reset(void);
 
 /* -------------------------------------------------------------------- backbone */
 
-/* One NHWC convolution on the tcgen05 tensor cores (TF32 inputs, fp32 accumulate), the
+/* One NHWC convolution on the Hopper tensor cores (wgmma, TF32 inputs, fp32 accumulate), the
  * building block of Resnet18_8s (lib/networks/resnet.py:28-35,54-70; model_repository.py:22-58):
  *
  *   out[n,y,x,out_co+co] = act( bias[co] + res[n,y,x,res_co+co]
@@ -289,17 +289,12 @@ PVNET_API int pvnet_conv2d_nhwc(const float *in, int in_cs, int in_co, int Cin,
  * Cout <= 64 whose weights fit in shared memory, per-tap kernel otherwise), 1 = per-tap kernel
  * only, 2 = column kernel (error if the layer is not eligible). */
 PVNET_API int pvnet_conv_set_mode(int mode);
-/* Test hook: how the per-tap kernel runs 256-channel weight tiles.  0 (default) = single CTAs;
- * 1 = 2-CTA clusters with TMA multicast of the weight tile; 2 = 2-CTA clusters issuing
- * tcgen05.mma.cta_group::2 (each CTA holds half of the weight tile). */
+/* Test hook: 1 = the per-tap kernel runs as clusters of two CTAs on adjacent M tiles that share each
+ * weight tile through TMA multicast; 0 (default) = single CTAs. */
 PVNET_API int pvnet_conv_set_multicast(int on);
-/* Test hook: 1 (default) runs single-CTA tiles of the per-tap kernel on its persistent variant
- * (continuous TMA ring, two TMEM accumulator stages); 0 = one tile per CTA. */
+/* Test hook: 1 (default) runs the per-tap kernel persistent (one CTA per SM looping over the
+ * output tiles, continuous TMA ring); 0 = one tile per CTA. */
 PVNET_API int pvnet_conv_set_persistent(int on);
-/* Test hook / tuning knob: epilogue warp sets of the fused-head column kernel (convraw.0) in plans built
- * afterwards.  1 = one set of four warps (default), 2 = two sets alternating tiles (measured no faster: the
- * launch is tensor-pipe bound), 0 = default (environment variable PVNET_HEAD_EPI, else 1). */
-PVNET_API int pvnet_conv_set_head_epilogue_sets(int sets);
 
 /* Resnet18_8s.forward (lib/networks/model_repository.py:64-80), eval mode, whole batch.
  *
@@ -338,10 +333,9 @@ PVNET_API int pvnet_backbone_set_conv(pvnet_backbone_t *m, int slot, const float
 PVNET_API int pvnet_backbone_set_output_layout(pvnet_backbone_t *m, int pixel_major);
 /* The last decoder upsampling, F.interpolate(x2s_up, scale_factor=2, mode='bilinear', align_corners=True)
  * (model_repository.py:75), can run inside convraw.0's operand loader: the full-resolution
- * [b,h,w,s2dim] tensor is then never written, the output is bit-identical.  on = 1 selects the fused
- * form with the interpolation on convraw.0's epilogue warps (two CTAs per SM), 2 the form with eight
- * dedicated interpolation warps (one CTA per SM, four-tile operand ring), 0 the separate upsampling
- * launch, -1 = default (environment variable PVNET_FUSE_UP; see DESIGN.md section 5 for the measurements). */
+ * [b,h,w,s2dim] tensor is then never written, the output is bit-identical.  on != 0 selects the fused
+ * form (the producer warps of convraw.0 interpolate into its operand stages), 0 the separate upsampling
+ * launch, -1 = default (environment variable PVNET_FUSE_UP, else the separate launch). */
 PVNET_API int pvnet_backbone_set_fused_upsample(pvnet_backbone_t *m, int on);
 PVNET_API int pvnet_backbone_workspace_bytes(const pvnet_backbone_t *m, int b, int h, int w, size_t *bytes);
 PVNET_API int pvnet_backbone_forward(pvnet_backbone_t *m, const float *image_nchw, int b, int h, int w,

@@ -2,7 +2,7 @@
 (same rules as oracle/pvnet_oracle.py: imported by tests/, smoke() and bench.py's CPU legs only).
 
 Restates, in numpy/scipy, what the reference computes after the voting layers (paths relative to
-/root/reference):
+the reference project):
 
   covariance -> weights  inv(sqrtm(cov)), zeros for cov[0,0] < 1e-6 or NaN     lib/utils/evaluation_utils.py:170-181
   4 most confident points  argsort(wxx + wxy)[-4:] (sic)                         lib/utils/extend_utils/extend_utils.py:84
@@ -20,8 +20,8 @@ is "the local minimiser of the cost above reached from the P3P pose" up to Ceres
 scipy.optimize.least_squares(method="lm") at tight tolerances, i.e. it returns the minimiser itself.
 PARITY PIN: the reference ships no test for this stage; pinned by (1) the known-answer pose of
 data/demo (cat_pose.npy reprojects cat_points_3d onto the fixture's keypoints: tests/golden/pnp_cases.npz,
-made by tests/golden/make_golden_pnp.py), (2) OpenCV's own P3P and iterative PnP, run in the authoring
-container when the fixtures were generated, (3) first-order optimality of the returned pose.
+made by tests/golden/make_golden_pnp.py), (2) OpenCV's own P3P and iterative PnP, run when generating
+the fixtures, (3) first-order optimality of the returned pose.
 Ceres itself never ran: for the weighted cases parity with the reference BINARY is unpinned.
 """
 from __future__ import annotations

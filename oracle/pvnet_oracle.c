@@ -6,7 +6,7 @@
  * cpu_baseline / --impl reference legs use it, and only as the checker or the
  * timed CPU baseline -- never as the product path.
  *
- * What is restated (paths relative to /root/reference):
+ * What is restated (paths relative to the reference project):
  *   pvo_generate_hypothesis   lib/ransac_voting_gpu_layer/src/ransac_voting_kernel.cu:11-49
  *   pvo_voting_for_hypothesis lib/ransac_voting_gpu_layer/src/ransac_voting_kernel.cu:88-126
  *   pvo_generate_hypothesis_vp / pvo_voting_for_hypothesis_vp
@@ -17,14 +17,14 @@
  *
  * Floating point.  The reference .cu is built by nvcc with its defaults
  * (-fmad=true, -prec-div=true, -prec-sqrt=true).  The exact rounding sequence
- * below was read off the SASS nvcc 12.9 emits for sm_100a (see DESIGN.md,
+ * below was read off the SASS nvcc 12.9 emits (see DESIGN.md,
  * "FP sequence"):  individually rounded FP32 mul/add, single-rounding fmaf where
  * ptxas contracted, correctly rounded sqrtf and '/', and the `< 1e-6` tests
  * done after promotion to double.  x86-64 fmaf/sqrtf/'/' are correctly rounded,
  * so built with -ffp-contract=off this file is bit-exact to the GPU kernels.
  *
  * Parity pin: tests/test_gpu_reference_layer.py runs the reference .cu itself
- * (compiled verbatim into oracle/_ref by oracle/Makefile) on the GPU box and
+ * (compiled verbatim into oracle/_ref by oracle/Makefile) on the GPU and
  * checks it against these functions bit for bit.
  */
 #include <math.h>
@@ -67,7 +67,7 @@ PVO_API void pvo_generate_hypothesis(const float *direct, const float *coords,
             const float s1 = fmaf(d1y, cx1, -(d1x * cy1));
             const float s0 = fmaf(d0y, cx0, -(d0x * cy0));
             const float y = fmaf(d1y, s0, -(d0y * s1)) / det_y;
-            const float x = fmaf(d0x, s1, -(d1x * s0)) / det_x;
+            const float x = fmaf(-d1x, s0, d0x * s1) / det_x;
             hypo[(hi * vn + vi) * 2] = x;
             hypo[(hi * vn + vi) * 2 + 1] = y;
         }
@@ -136,7 +136,7 @@ PVO_API void pvo_vote_counts(const float *direct, const float *coords,
 }
 
 /* ransac_voting_kernel.cu:170-230.  hypo [hn,vn,3] homogeneous intersection of the two pixels' lines;
- * rounding sequence as nvcc compiles the reference (SASS, sm_100a): see exact_vp_hypothesis in
+ * rounding sequence as nvcc compiles the reference (SASS): see exact_vp_hypothesis in
  * pvnet_b200/csrc/vote.cu for the line-by-line mapping. */
 PVO_API void pvo_generate_hypothesis_vp(const float *direct, const float *coords, const int32_t *idxs,
                                         float *hypo, int tn, int vn, int hn)

@@ -6,7 +6,7 @@ timed CPU baseline.  Nothing under ``pvnet_b200/`` imports it; the product path
 fails loudly when its CUDA library is missing.
 
 It restates, in numpy + the C kernels of ``pvnet_oracle.c``, what these reference
-functions compute (paths relative to /root/reference):
+functions compute (paths relative to the reference project):
 
   ransac_voting_layer_v3                    lib/ransac_voting_gpu_layer/ransac_voting_gpu.py:514-598
   estimate_voting_distribution_with_mean    lib/ransac_voting_gpu_layer/ransac_voting_gpu.py:333-406
@@ -24,7 +24,7 @@ Parity pin.  The reference has no test suite and no golden vectors (SURVEY.md §
 The oracle is pinned two ways: (1) the analytic known-answer fixture derived from
 the reference's ``data/demo`` (tests/golden/demo_cat.npz, made by
 tests/golden/make_golden.py): voting on the exact vector field must return the
-projected keypoints; (2) on the GPU box the reference's own CUDA kernels, compiled
+projected keypoints; (2) on the GPU the reference's own CUDA kernels, compiled
 verbatim into ``oracle/_ref``, are run against the C kernels here bit for bit
 (tests/test_gpu_reference_layer.py).
 """

@@ -1,6 +1,6 @@
-"""The reference's own CUDA voting layer, run on the GPU box -- TEST INFRASTRUCTURE ONLY.
+"""The reference's own CUDA voting layer, run on the GPU -- TEST INFRASTRUCTURE ONLY.
 
-`oracle/_ref/libpvnet_refcuda.so` is /root/reference/lib/ransac_voting_gpu_layer/src/
+`oracle/_ref/libpvnet_refcuda.so` is the reference project's lib/ransac_voting_gpu_layer/src/
 ransac_voting_kernel.cu compiled verbatim (oracle/Makefile, target `ref`) plus our C shim
 (oracle/ref_shim.cu).  This module binds it with ctypes and re-states, with the torch
 ops the reference uses and in the reference's order, the Python orchestration of

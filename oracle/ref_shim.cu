@@ -1,7 +1,7 @@
 // ref_shim.cu -- OUR C-ABI shim around the reference's CUDA voting launchers.
 //
 // TEST INFRASTRUCTURE ONLY (see oracle/pvnet_oracle.c header).  It is compiled by
-// oracle/Makefile together with /root/reference/lib/ransac_voting_gpu_layer/src/
+// oracle/Makefile together with the reference project's lib/ransac_voting_gpu_layer/src/
 // ransac_voting_kernel.cu -- taken verbatim from where it lies, never copied --
 // into oracle/_ref/libpvnet_refcuda.so.  The reference's own binding
 // (ransac_voting.cpp) does not compile against torch 2.11 (THCState, bare

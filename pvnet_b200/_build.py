@@ -1,7 +1,7 @@
-"""Builds pvnet_b200/_lib/libpvnet_b200.so in-tree with nvcc for sm_100a.
+"""Builds pvnet_b200/_lib/libpvnet_b200.so in-tree with nvcc for sm_90a (H100).
 
-nvcc cross-compiles without a GPU, so this runs in the authoring container; the
-resulting .so is git-ignored but travels to the GPU box with the repo snapshot.
+nvcc cross-compiles without a GPU; the resulting .so (git-ignored) is loaded from the
+source tree.
 """
 from __future__ import annotations
 
@@ -18,7 +18,7 @@ INCLUDE = os.path.join(os.path.dirname(HERE), "include")
 
 NVCC_FLAGS = [
     "-std=c++17", "-O3", "-lineinfo",
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden",
     "-Xptxas", "-v", "-Xptxas", "-warn-spills",
 ]
@@ -56,7 +56,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         if p.returncode != 0:
             sys.stderr.write(out)
             raise RuntimeError(f"nvcc failed on {src}")
-    cmd = [nvcc, "-shared", "-o", LIB + ".tmp", *objs, "-ldl"]
+    cmd = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-o", LIB + ".tmp", *objs, "-ldl"]
     subprocess.check_call(cmd)
     os.replace(LIB + ".tmp", LIB)
     with open(os.path.join(LIBDIR, "build.log"), "w") as f:

@@ -67,7 +67,6 @@ SIGNATURES = {
     "pvnet_conv_set_mode": (c_int, [c_int]),
     "pvnet_conv_set_multicast": (c_int, [c_int]),
     "pvnet_conv_set_persistent": (c_int, [c_int]),
-    "pvnet_conv_set_head_epilogue_sets": (c_int, [c_int]),
     "pvnet_backbone_create": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_void_p)]),
     "pvnet_backbone_destroy": (None, [c_void_p]),
     "pvnet_backbone_num_convs": (c_int, []),

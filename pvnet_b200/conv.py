@@ -23,13 +23,8 @@ def set_mode(mode: int):
 
 
 def set_multicast(mode: int):
-    """Test hook (pvnet_conv_set_multicast): 0 single CTA (default), 1 2-CTA weight multicast, 2 cta_group::2."""
+    """Test hook (pvnet_conv_set_multicast): 0 single CTAs (default), 1 two-CTA clusters with weight multicast."""
     _native.check(_native.lib().pvnet_conv_set_multicast(int(mode)), "pvnet_conv_set_multicast")
-
-
-def set_head_epilogue_sets(sets: int):
-    """Test hook (pvnet_conv_set_head_epilogue_sets): epilogue warp sets of the fused-head kernel, 0 = default."""
-    _native.check(_native.lib().pvnet_conv_set_head_epilogue_sets(int(sets)), "pvnet_conv_set_head_epilogue_sets")
 
 
 def set_persistent(on: bool):

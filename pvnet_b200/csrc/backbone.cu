@@ -1,6 +1,6 @@
 // backbone.cu -- Resnet18_8s.forward (lib/networks/model_repository.py:64-80 over
 // lib/networks/resnet.py:200-220) as one launch sequence on the caller's stream:
-// 25 tcgen05 convolutions (conv_tc.cu) + stem / max-pool / 3 upsamplings / image packing /
+// 25 wgmma convolutions (conv_tc.cu, conv_col.cu) + stem / max-pool / 3 upsamplings / image packing /
 // head (backbone_aux.cu).  Eval mode only: BatchNorm is folded into the packed weights by
 // the host layer (pvnet_b200/model_repository.py).  Activations are NHWC fp32 (TF32-rounded
 // where they feed a tensor-core conv); every torch.cat of the decoder is replaced by
@@ -46,10 +46,8 @@ struct pvnet_backbone {
     bool up2_fused = false;              // the current plan has no separate 1/2 -> 1 upsampling launch
 };
 
-// default of the fused 1/2 -> 1 upsampling (tuning knob PVNET_FUSE_UP, read once): OFF.  Measured on B200
-// (DESIGN.md section 5, profiles/r02_ncu_convraw_fused.md): bit-identical output, but the interpolation runs on
-// convraw.0's epilogue warps, whose per-tile chain (three TMEM round trips + the head MMA) is already as long
-// as the tile's MMAs -- 0.77 ms fused against 0.43 + 0.17 ms for the two separate launches.
+// default of the fused 1/2 -> 1 upsampling (tuning knob PVNET_FUSE_UP, read once): OFF.  Both forms compute the
+// same bits; the separate k_upsample2x launch is the default.
 static int env_fuse_up()
 {
     static const int v = [] {
@@ -222,7 +220,6 @@ int build_plans(pvnet_backbone *m, const Buffers &B, int b, int h, int w)
             const int want = m->fuse_up < 0 ? env_fuse_up() : m->fuse_up;
             if (want != 0 && m->s2 == 32 && m->raw == 32 && m->seg_dim + m->ver_dim <= 32) {
                 draw.up_src = B.U2;
-                draw.up_mode = want == 2 ? 2 : 1;
                 m->up2_fused = true;
             }
         }
@@ -272,7 +269,7 @@ int pvnet_backbone_set_output_layout(pvnet_backbone_t *m, int pixel_major)
 int pvnet_backbone_set_fused_upsample(pvnet_backbone_t *m, int on)
 {
     PV_CHECK_ARG(m, "null handle");
-    m->fuse_up = on < 0 ? -1 : (on == 2 ? 2 : (on ? 1 : 0));
+    m->fuse_up = on < 0 ? -1 : (on ? 1 : 0);
     m->p_ws = nullptr;   // replan
     return PVNET_OK;
 }

@@ -1,4 +1,4 @@
-// common.cuh -- shared host/device helpers for libpvnet_b200.so (sm_100a only).
+// common.cuh -- shared host/device helpers for libpvnet_b200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdarg>

@@ -1,25 +1,22 @@
 // conv_col.cu -- persistent, weights-resident 3x3 convolution for the narrow layers
-// (Cout <= 64: layer1.*, conv2s.0, convraw.0 of lib/networks/model_repository.py:22-58).
+// (Cout <= 64: layer1.*, conv2s.0, convraw.0 of lib/networks/model_repository.py:22-58, and the stem in its
+// space-to-depth 4x4 form), on the Hopper tensor cores (wgmma, sm_90a).
 //
-// Why a second kernel: with N <= 64 output channels a 128-pixel tile does too little math
-// per byte for the per-tap kernel (conv_tc.cu) -- ncu showed those launches L2-throughput
-// bound (62-71 %) with the tensor pipe 7-20 % active, because each of the 9 taps re-reads the
-// 128-pixel A tile and every CTA re-reads all weights.  Here:
+// Why a second kernel: with N <= 64 output channels a 128-pixel tile does too little math per byte
+// for the per-tap kernel (conv_tc.cu), which re-reads the 128-pixel A tile for each of the 9 taps
+// and the weights in every CTA.  Here:
 //   * ALL weights of the layer (<= 147 KB) are loaded into shared memory once per CTA, and the
-//     CTA is persistent over output tiles (grid = resident CTAs, static round-robin);
-//   * "halo box": for each channel chunk ONE TMA box of (TH+2d) x (TW+2d) pixels is loaded and
-//     all KH x KW taps are operand-descriptor offsets into it.  The tile is 16 rows x 8 pixels, so
-//     an 8-row descriptor group is one tile row and the group stride (SBO) is the box pitch
-//     (TW+2d rows); tcgen05 applies the 128/64/32-byte swizzle to ABSOLUTE shared-memory address
-//     bits -- the same function TMA used when it wrote the box -- so start addresses and group
-//     strides need not be multiples of the 1024-byte swizzle repeat (verified on B200 by
-//     benchmarks/micro/desc_offset.cu).  A traffic drops from 9x (per-tap kernel) and 3.75x (one
-//     box per kernel column, the previous scheme) to (TH+2)(TW+2)/(TH*TW) = 1.41x;
-//   * two TMEM accumulator stages: the epilogue of tile i overlaps the MMAs of tile i+1; with
-//     EPI = 2 two epilogue warp sets alternate tiles (short-K layers are epilogue-bound);
-//   * TMA-store epilogue shared with conv_tc.cu (conv_tc.cuh: epi_activate / epi_stage / ...);
-//   * optional fused head (convraw.3 1x1 + bias + argmax, exact fp32) in the epilogue, writing
-//     the reference's NCHW output directly -- the [b,H,W,32] intermediate never exists.
+//     CTA is persistent over output tiles (grid = one CTA per SM, static round-robin);
+//   * "halo box": for each channel chunk ONE TMA box of (TH+KH-1) x (TW+KH-1) pixels is loaded and
+//     all KH x KW taps read from it: A traffic is (TH+2)(TW+2)/(TH*TW) = 1.41x the tile instead of 9x.
+//     A tap's operand rows start anywhere in the box, so the consumer warpgroups gather the A
+//     fragments into registers (undoing the box's swizzle) and issue register-A wgmma; the weights
+//     are shared-memory descriptor operands;
+//   * optional fused head (convraw.3 1x1 + bias + argmax) in the epilogue: the activated 128 x 32 tile
+//     is already in the register layout of a wgmma A operand, so the head is one more MMA, and the
+//     reference's NCHW output is written directly -- the [b,H,W,32] intermediate never exists;
+//   * optional fused bilinear x2 upsampling of convraw.0's first input (the producer warps interpolate
+//     it into the operand stages instead of TMA loading it).
 #include "conv_tc.cuh"
 #include "ptx.cuh"
 
@@ -30,21 +27,20 @@
 namespace pvnet {
 
 int g_conv_mode = 0;
-int g_head_epi = 0;     // test hook: epilogue warp sets of the fused-head kernel (0 = PVNET_HEAD_EPI / default 1)
 
 namespace {
 
 constexpr int COL_TH = 16, COL_TW = 8;
+constexpr int COL_THREADS = 384;       // consumer warpgroups 0 and 1 (64 tile pixels each), producer warpgroup 2
 constexpr int HEAD_MAX = 64;
 
 struct ColGeom {
     int Ho, Wo, tiles_x, tiles_y, total_tiles;
-    int dil, cin_chunks, cin_pad;
+    int cin_chunks, cin_pad;
     int split_chunk;        // chunks >= split_chunk are read through the second source map (== cin_chunks: none)
-    int KW, KH, pad_l, pad_t;   // taps and how many of them lie left of / above the output pixel
-    int BN;                 // == Cout (<= 64)
+    int pad_l, pad_t;       // how many taps lie left of / above the output pixel
     int stages;
-    int resident;           // 1: all weights loaded once per CTA; 0: the KH weight tiles ride in each stage
+    int resident;           // 1: all weights loaded once per CTA; 0: the KH*KH weight tiles ride in each stage
     int out_cs, out_co, res_cs, res_co;
     int act, round_out;
     // fused head
@@ -57,10 +53,10 @@ struct ColUp {
     const float *src;       // half-resolution source [b,h,w,cs], dense
     int h, w, cs;
     float sy, sx;           // ATen's align_corners scale (in-1)/(out-1)
-    unsigned zero;          // always 0; opaque to the compiler (see up_fill_chunk)
+    unsigned zero;          // always 0; opaque to the compiler (see up_fill_rows)
 };
 
-// Fused upsampling (UP variant of the kernel): epilogue warp q interpolates channel chunk q (8 channels)
+// Fused upsampling (UP variant of the kernel): producer warp q interpolates channel chunk q (8 channels)
 // of one tile's halo box -- (COL_TH+2) x (COL_TW+2) full-resolution pixels, zero outside the image like
 // the TMA box it replaces -- straight into the operand stage, in the 32-byte-swizzled layout TMA would
 // have written (16-byte half `hf` of box row rr sits at rr*32 + ((hf ^ (rr>>2 & 1)) << 4): address bit 4
@@ -122,8 +118,8 @@ __device__ __forceinline__ void up_fill_rows(const float *base, unsigned rstride
                     wc = __shfl_sync(0xffffffffu, wc_l, i);
         const int e = (i >> 1) - S0;
         // Rounding to tf32 (nearest, ties away -- cvt.rna.tf32, what k_upsample2x stores): add half an ulp of
-        // the 10-bit mantissa; the 13 low bits that remain are ignored by the tensor core (kind::tf32 reads the
-        // upper 19 bits), so they need not be cleared.  Exactly the values the separate launch feeds the MMA.
+        // the 10-bit mantissa; the 13 low bits that remain are cleared when the MMA operand is gathered (see
+        // k_conv_col), so the MMA sees exactly the values the separate launch feeds it.
         float4 o;
         o.x = __uint_as_float(__float_as_uint(lerp3(wa, t[e].x, wb, t[e + 1].x, wc, t[e + 2].x)) + 0x1000u);
         o.y = __uint_as_float(__float_as_uint(lerp3(wa, t[e].y, wb, t[e + 1].y, wc, t[e + 2].y)) + 0x1000u);
@@ -134,31 +130,7 @@ __device__ __forceinline__ void up_fill_rows(const float *base, unsigned rstride
     }
 }
 
-// L2 prefetch of the source lines a later up_fill_chunk of the same warp will read (same addresses; no data comes
-// back, so no registers are held): ncu showed the dedicated interpolation warps waiting ~2k cycles per load batch --
-// half of the 157 MB source has left the L2 by the time convraw.0 runs.  One 16-byte half per 32-byte sector suffices.
-__device__ __forceinline__ void up_prefetch_chunk(const ColUp &u, const ColGeom &g, int img, int y0, int x0, int q, int lane)
-{
-    constexpr int PITCH = COL_TW + 2, NSLOT = COL_TH / 2 + 3;
-    if (lane >= 2 * PITCH || (lane & 1)) return;
-    const int xc = min(max(x0 - 1 + (lane >> 1), 0), g.Wo - 1);
-    const int xlo = (int)(u.sx * (float)xc);
-    const int xhi = min(xlo + 1, u.w - 1);
-    const int R0 = (y0 >> 1) - 2;
-    const float *base = u.src + (size_t)img * u.h * u.w * u.cs + q * 8;
-    const unsigned rstride = (unsigned)u.w * (unsigned)u.cs;
-    const unsigned olo = (unsigned)xlo * (unsigned)u.cs, ohi = (unsigned)xhi * (unsigned)u.cs;
-#pragma unroll
-    for (int j = 1; j < NSLOT; ++j) {
-        const unsigned ro = (unsigned)min(max(R0 + j, 0), u.h - 1) * rstride;
-        asm volatile("prefetch.global.L2 [%0];" ::"l"(base + (ro + olo)));
-        asm volatile("prefetch.global.L2 [%0];" ::"l"(base + (ro + ohi)));
-    }
-}
-
-// PARTS = 1: the whole column at once (20 loads in flight, ~130 registers); PARTS = 2: rows 0-8, then rows 9-17
-// (12 + 14 loads, for the 112-register variant with dedicated interpolation warps).
-template <int PARTS>
+// The whole column at once (20 loads in flight).
 __device__ __forceinline__ void up_fill_chunk(const ColUp &u, const ColGeom &g, int img, int y0, int x0, int q, int lane,
                                               uint32_t stage_addr)
 {
@@ -194,442 +166,271 @@ __device__ __forceinline__ void up_fill_chunk(const ColUp &u, const ColGeom &g, 
     const unsigned rstride = (unsigned)u.w * (unsigned)u.cs;      // 32-bit element offsets inside one image
     const unsigned olo = (unsigned)xlo * (unsigned)u.cs, ohi = (unsigned)xhi * (unsigned)u.cs;
     const uint32_t sbase = stage_addr + (uint32_t)(c * 32);   // box row rr = i*PITCH + c sits at rr*32 + ((hf ^ bit 2 of rr) << 4)
-    if (PARTS == 1) {
-        up_fill_rows<0, ROWS>(base, rstride, olo, ohi, R0, u.h, act, vx, w1x_, u.zero, wa_l, wb_l, wc_l, sbase, c, hf);
-    } else {
-        up_fill_rows<0, ROWS / 2>(base, rstride, olo, ohi, R0, u.h, act, vx, w1x_, u.zero, wa_l, wb_l, wc_l, sbase, c, hf);
-        up_fill_rows<ROWS / 2, ROWS>(base, rstride, olo, ohi, R0, u.h, act, vx, w1x_, u.zero, wa_l, wb_l, wc_l, sbase, c, hf);
-    }
+    up_fill_rows<0, ROWS>(base, rstride, olo, ohi, R0, u.h, act, vx, w1x_, u.zero, wa_l, wb_l, wc_l, sbase, c, hf);
 }
 
 
-// EPI = number of epilogue warp sets (4 warps each).  ncu showed the stem and layer1 launches
-// epilogue-bound (epilogue warps never wait on tfull; 39 % of samples on the residual load): with
-// EPI = 2 the sets alternate tiles, one per TMEM accumulator stage.
-// UP (with HEAD, KC = 8, 4 interpolated chunks + 1 TMA chunk per tile, ring = 2 tiles): the first
-// split_chunk chunks of every tile are produced by the epilogue warps (up_fill_chunk) instead of TMA.
-// Epilogue warp q fills chunk q of tile it+2 between the two halves of tile it's epilogue (after the
-// activated tile went back to TMEM, while the head MMA is pending), into stage ((it+2)&1)*5 + q; its
-// empty barrier completed with tile it's MMAs, which the warp has already seen through tfull.
-// UP = 2: one CTA per SM, EPI = 2, and EIGHT more warps that only interpolate (warp 10 + 4*s + q: chunk q of the
-// tiles of parity s), running ahead of the MMAs through a ring of four tiles; the epilogue warps do no filling.
-constexpr int UP_WARPS = 8;
-template <int KC, bool HEAD, int KH, int EPI, int UP = 0>
-__global__ void __launch_bounds__(64 + 128 * EPI + (UP == 2 ? 32 * UP_WARPS : 0), ((EPI == 2 && !HEAD) || UP == 2) ? 1 : 2)
+
+// BN = Cout (32 or 64); KC channels per chunk (rows of KC*4 bytes, swizzled by the same amount).
+template <int KC, bool HEAD, int KH, bool UP, int BN>
+__global__ void __launch_bounds__(COL_THREADS, 1)
     k_conv_col(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
-               const __grid_constant__ CUtensorMap tmB,
-               const __grid_constant__ CUtensorMap tmH, const __grid_constant__ CUtensorMap tmO, const ColGeom g,
+               const __grid_constant__ CUtensorMap tmB, const __grid_constant__ ColGeom g,
                const float *__restrict__ bias, const float *__restrict__ res, float *__restrict__ out,
                const float *__restrict__ head_w, const float *__restrict__ head_b, float *__restrict__ head_out,
                void *__restrict__ mask, const ColUp up)
 {
-    static_assert(UP == 0 || (HEAD && KC == 8 && KH == 3), "fused upsampling: convraw.0 form only");
-    static_assert(UP != 2 || EPI == 2, "dedicated interpolation warps come with two epilogue sets");
+    static_assert(!UP || (HEAD && KC == 8 && KH == 3), "fused upsampling: convraw.0 form only");
+    static_assert(!HEAD || BN == 32, "fused head: 32 input channels");
     constexpr int ROWB = KC * 4;                       // bytes per K-major row
+    constexpr int B_TILE = BN * ROWB;                  // one [BN][KC] weight tile (a multiple of 1024 bytes)
+    constexpr int PITCH = COL_TW + KH - 1;             // box pitch in pixels (= shared-memory rows)
+    constexpr int A_BOX = (COL_TH + KH - 1) * PITCH * ROWB;
+    constexpr int A_BYTES = (A_BOX + 1023) & ~1023;    // stages stay 1024-byte aligned
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    const int b_tile = g.BN * ROWB;                    // one [BN][KC] weight tile
-    const int n_btiles = g.KW * KH * g.cin_chunks;
-    constexpr int PITCH = COL_TW + KH - 1;             // box pitch in pixels (= shared-memory rows); dilation 1 only
-    constexpr int a_box = (COL_TH + KH - 1) * PITCH * ROWB;
-    constexpr int a_bytes = (a_box + 1023) & ~1023;    // stages stay 1024-byte aligned
-    const int stage_bytes = a_bytes + (g.resident ? 0 : KH * KH * b_tile);
+    const int n_btiles = KH * KH * g.cin_chunks;
+    const int stage_bytes = A_BYTES + (g.resident ? 0 : KH * KH * B_TILE);
     uint8_t *sB = smem;
-    uint8_t *sA = smem + (g.resident ? (size_t)n_btiles * b_tile : 0);
-    // HEAD: head weights [32][32], 4 KB.  otherwise: one 128-pixel x 32-channel output staging tile
-    // (128B-swizzled rows) for the TMA store of the epilogue, 16 KB
-    uint8_t *sHB = sA + (size_t)g.stages * stage_bytes;
-    uint64_t *bars = reinterpret_cast<uint64_t *>(sHB + (HEAD ? 4096 : 32768));
-    uint64_t *wfull = bars;
-    uint64_t *full = bars + 1;
+    uint8_t *sA = smem + (g.resident ? (size_t)n_btiles * B_TILE : 0);
+    uint8_t *sH = sA + (size_t)g.stages * stage_bytes;            // HEAD: head weights, 32 x 32, 128-byte swizzle
+    uint64_t *wfull = reinterpret_cast<uint64_t *>(sH + (HEAD ? 4096 : 0));
+    uint64_t *full = wfull + 1;
     uint64_t *empty = full + g.stages;
-    uint64_t *tfull = empty + g.stages;               // [2]
-    uint64_t *tempty = tfull + 2;                     // [2]
-    uint64_t *a2full = tempty + 2;                    // [2] HEAD: activated tile written back to TMEM
-    uint64_t *d2full = a2full + 2;                    // [2] HEAD: 1x1 head MMAs done
-    uint64_t *hfull = d2full + 2;                     // HEAD: head weights landed
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(hfull + 1);
-    float *s_bias = reinterpret_cast<float *>((reinterpret_cast<uintptr_t>(tmem_slot + 4) + 15) & ~uintptr_t(15));  // [64]
-    float *s_head = s_bias + 64;                                                                              // [head_cout*33]
+    float *s_bias = reinterpret_cast<float *>(empty + g.stages);  // [BN]
+    float *s_head = s_bias + 64;                                  // [32]
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    uint32_t tmem_cols = 32;
-    while (tmem_cols < (uint32_t)(2 * g.BN)) tmem_cols <<= 1;
-    if (HEAD) tmem_cols = 256;      // acc[2] | A2[2] | D2[2], 32 columns each
-
-    if (warp == 0 && lane == 0) {
-        ptx::prefetch_tensormap(&tmA);
-        ptx::prefetch_tensormap(&tmB);
+    if (threadIdx.x == 0) {
         ptx::mbar_init(wfull, 1);
         for (int s = 0; s < g.stages; ++s) {
             ptx::mbar_init(&full[s], 1);
-            ptx::mbar_init(&empty[s], 1);
+            ptx::mbar_init(&empty[s], 8);              // one arrive per consumer warp
         }
-        for (int s = 0; s < 2; ++s) {
-            ptx::mbar_init(&tfull[s], 1);
-            ptx::mbar_init(&tempty[s], 4);             // one arrive per epilogue warp
-            ptx::mbar_init(&a2full[s], 4);
-            ptx::mbar_init(&d2full[s], 1);
-        }
-        ptx::mbar_init(hfull, 1);
         ptx::fence_barrier_init();
     }
-    if (warp == 1) {
-        ptx::tmem_alloc(tmem_slot, tmem_cols);
-        ptx::tmem_relinquish();
+    for (int i = threadIdx.x; i < BN; i += blockDim.x) s_bias[i] = bias[i];
+    if (HEAD) {
+        for (int i = threadIdx.x; i < 32; i += blockDim.x) s_head[i] = i < g.head_cout ? head_b[i] : 0.f;
+        // convraw.3 weights [cout][32] as the B operand of the head MMA, rows >= cout zero.  K is stored permuted
+        // within each group of 8 (position p < 4 holds channel 2p, position p >= 4 channel 2(p-4)+1): the order in
+        // which the accumulator fragment of the 3x3 conv hands its channels to the A fragment of the head MMA.
+        for (int i = threadIdx.x; i < 32 * 32; i += blockDim.x) {
+            const int n = i >> 5, p = i & 31, q = p & 7;
+            const int k = (p & ~7) + (q < 4 ? 2 * q : 2 * (q - 4) + 1);
+            const float v = n < g.head_cout ? head_w[n * 32 + k] : 0.f;
+            *reinterpret_cast<float *>(sH + ptx::swizzle_off((uint32_t)(n * 128 + p * 4), 128)) = v;
+        }
+        ptx::fence_proxy_async();                      // generic stores -> read by the MMA (async proxy)
     }
-    for (int i = threadIdx.x; i < g.BN; i += blockDim.x) s_bias[i] = bias[i];
-    if (HEAD)
-        for (int i = threadIdx.x; i < g.head_cout; i += blockDim.x) s_head[i] = head_b[i];
-    ptx::tc_fence_before();
     __syncthreads();
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     const int tiles_per_img = g.tiles_x * g.tiles_y;
-    const int kb_per_tile = g.cin_chunks;
 
-    if (warp == 0) {
-        if (lane == 0) {
-            if (HEAD) {      // convraw.3 weights [cout][32] -> K-major 32x32 tile (rows >= cout zero-filled)
-                ptx::mbar_arrive_expect_tx(hfull, 4096u);
-                ptx::tma_load_2d(sHB, &tmH, hfull, 0, 0);
-            }
-            // all weights, once: tile t = (cc*KH + kh)*KW + kw <- packed [Cout][kh][kw][cin]
-            if (g.resident) {
-                ptx::mbar_arrive_expect_tx(wfull, (uint32_t)(n_btiles * b_tile));
-                for (int cc = 0; cc < g.cin_chunks; ++cc)
-                    for (int t = 0; t < KH * KH; ++t)
-                        ptx::tma_load_2d(sB + (size_t)(cc * KH * KH + t) * b_tile, &tmB, wfull,
-                                         t * g.cin_pad + cc * KC, 0);
-            }
-            int s = 0;
-            uint32_t ph = 0;
-            const uint32_t tx_bytes = (uint32_t)(a_box + (g.resident ? 0 : KH * KH * b_tile));
-            for (int tile = blockIdx.x; tile < g.total_tiles; tile += gridDim.x) {
-                const int img = tile / tiles_per_img;
-                const int trem = tile - img * tiles_per_img;
-                const int tyi = trem / g.tiles_x, txi = trem - tyi * g.tiles_x;
-                const int y0 = tyi * COL_TH, x0 = txi * COL_TW;
-                for (int cc = 0; cc < g.cin_chunks; ++cc) {
-                    if (UP != 0 && cc < g.split_chunk) {     // filled by the epilogue / interpolation warps
-                        if (++s == g.stages) {
-                            s = 0;
-                            ph ^= 1u;
-                        }
-                        continue;
-                    }
-                    ptx::mbar_wait(&empty[s], ph ^ 1u);
-                    ptx::mbar_arrive_expect_tx(&full[s], tx_bytes);
-                    uint8_t *st = sA + (size_t)s * stage_bytes;
-                    if (cc < g.split_chunk)
-                        ptx::tma_load_4d(st, &tmA, &full[s], cc * KC, x0 - g.pad_l, y0 - g.pad_t, img);
-                    else
-                        ptx::tma_load_4d(st, &tmA2, &full[s], (cc - g.split_chunk) * KC, x0 - g.pad_l, y0 - g.pad_t, img);
-                    if (!g.resident)
-                        for (int t = 0; t < KH * KH; ++t)
-                            ptx::tma_load_2d(st + a_bytes + (size_t)t * b_tile, &tmB, &full[s],
-                                             t * g.cin_pad + cc * KC, 0);
-                    if (++s == g.stages) {
-                        s = 0;
-                        ph ^= 1u;
-                    }
-                }
-            }
+    if (warp >= 8) {
+        // producer warpgroup: warp 8 lane 0 issues the TMA loads; with UP, warp 8 + q also interpolates chunk q
+        const int pw = warp - 8;
+        if (pw == 0 && lane == 0 && g.resident) {
+            // all weights, once: tile t = cc*KH*KH + kh*KH + kw <- packed [Cout][kh][kw][cin]
+            ptx::mbar_arrive_expect_tx(wfull, (uint32_t)(n_btiles * B_TILE));
+            for (int cc = 0; cc < g.cin_chunks; ++cc)
+                for (int t = 0; t < KH * KH; ++t)
+                    ptx::tma_load_2d(sB + (size_t)(cc * KH * KH + t) * B_TILE, &tmB, wfull, t * g.cin_pad + cc * KC, 0);
         }
-    } else if (warp == 1) {
-        {   // the whole warp runs the loop converged (warp-uniform values stay in uniform registers,
-            // no R2UR per MMA); one elected lane issues
-            const uint32_t idesc = ptx::make_idesc_tf32(128, g.BN);
-            if (g.resident) ptx::mbar_wait(wfull, 0);
-            // The issuing thread is the bottleneck of narrow tiles (hardware floor 40-48 cycles per
-            // N<=64 MMA, benchmarks/micro/mma_rate.cu), so the loop is kept to a handful of
-            // instructions per MMA: descriptors are a constant plus a 16-byte-unit offset, the
-            // (kh, k) nest is fully unrolled, stage/phase are running counters.
-            const uint64_t dbase = ptx::make_kmajor_desc(0, ROWB);
-            // A: 8-row groups are tile rows, one box pitch apart
-            const uint64_t abase = (dbase & ~(0x3fffull << 32)) | ((uint64_t)((uint32_t)(PITCH * ROWB) >> 4) << 32);
-            const uint32_t hidesc = ptx::make_idesc_tf32(128, 32);
-            constexpr uint32_t a_kh = (uint32_t)(PITCH * ROWB) >> 4, a_kw = (uint32_t)ROWB >> 4;   // compile-time tap offsets
-            const uint32_t b_t = (uint32_t)b_tile >> 4;
-            const uint32_t sA_u = ptx::smem_u32(sA), sB_u = ptx::smem_u32(sB);
-            int s = 0;
-            uint32_t ph = 0, it = 0;
-            for (int tile = blockIdx.x; tile < g.total_tiles; tile += gridDim.x, ++it) {
-                const uint32_t as = it & 1u;
-                ptx::mbar_wait(&tempty[as], ((it >> 1) & 1u) ^ 1u);
-                ptx::tc_fence_after();
-                const uint32_t tacc = tmem_base + as * (uint32_t)g.BN;
-                uint32_t bres = sB_u;
-                for (int kb = 0; kb < kb_per_tile; ++kb) {
-                    ptx::mbar_wait(&full[s], ph);
-                    ptx::tc_fence_after();
-                    const uint32_t a0 = sA_u + (uint32_t)s * (uint32_t)stage_bytes;
-                    const uint32_t b0 = g.resident ? bres : a0 + (uint32_t)a_bytes;
-                    const uint64_t ad = abase + (uint64_t)(a0 >> 4);
-                    const uint64_t bd = dbase + (uint64_t)(b0 >> 4);
-                    if (ptx::elect_one()) {
-#pragma unroll
-                        for (int kh = 0; kh < KH; ++kh) {
-#pragma unroll
-                            for (int kw = 0; kw < KH; ++kw) {
-#pragma unroll
-                                for (int k = 0; k < KC / 8; ++k)
-                                    ptx::mma_tf32_ss(tacc, ad + (uint64_t)(kh * a_kh + kw * a_kw + 2 * k),
-                                                     bd + (uint64_t)((kh * KH + kw) * b_t + 2 * k), idesc,
-                                                     (kb | kh | kw | k) != 0 ? 1u : 0u);
-                            }
-                        }
-                        ptx::mma_commit(&empty[s]);
-                    }
-                    __syncwarp();
-                    bres += (uint32_t)(KH * KH * b_tile);
-                    if (++s == g.stages) {
-                        s = 0;
-                        ph ^= 1u;
-                    }
-                }
-                if (ptx::elect_one()) ptx::mma_commit(&tfull[as]);
-                __syncwarp();
-                if (HEAD && it > 0) {
-                    // 1x1 head of the PREVIOUS tile: D2 = leaky(acc) [TMEM, written back by the epilogue
-                    // warps] x Whead^T [smem]; issued after this tile's MMAs so the tensor pipe never waits
-                    const uint32_t hs = (it - 1) & 1u;
-                    if (it == 1) ptx::mbar_wait(hfull, 0);
-                    ptx::mbar_wait(&a2full[hs], ((it - 1) >> 1) & 1u);
-                    ptx::tc_fence_after();
-                    if (ptx::elect_one()) {
-                        const uint64_t hd = ptx::make_kmajor_desc(ptx::smem_u32(sHB), 128);   // head tile: 128-byte rows whatever KC is
-#pragma unroll
-                        for (int k = 0; k < 4; ++k)
-                            ptx::mma_tf32_ts(tmem_base + 128u + hs * 32u, tmem_base + 64u + hs * 32u + 8u * k,
-                                             hd + (uint64_t)(2 * k), hidesc, k != 0 ? 1u : 0u);
-                        ptx::mma_commit(&d2full[hs]);
-                    }
-                    __syncwarp();
-                }
-            }
-            if (HEAD && it > 0) {    // head of the last tile
-                const uint32_t hs = (it - 1) & 1u;
-                if (it == 1) ptx::mbar_wait(hfull, 0);
-                ptx::mbar_wait(&a2full[hs], ((it - 1) >> 1) & 1u);
-                ptx::tc_fence_after();
-                if (ptx::elect_one()) {
-                    const uint64_t hd = ptx::make_kmajor_desc(ptx::smem_u32(sHB), 128);   // head tile: 128-byte rows whatever KC is
-#pragma unroll
-                    for (int k = 0; k < 4; ++k)
-                        ptx::mma_tf32_ts(tmem_base + 128u + hs * 32u, tmem_base + 64u + hs * 32u + 8u * k,
-                                         hd + (uint64_t)(2 * k), hidesc, k != 0 ? 1u : 0u);
-                    ptx::mma_commit(&d2full[hs]);
-                }
-                __syncwarp();
-            }
-        }
-    } else if (UP == 2 && warp >= 2 + 4 * EPI) {
-        // dedicated interpolation warps: set s = tiles of parity s, chunk q; ring slot = tile index mod ring tiles
-        const int iw = warp - (2 + 4 * EPI), iset = iw >> 2, q = iw & 3;
-        const uint32_t ring_tiles = (uint32_t)(g.stages / g.cin_chunks);
-        uint32_t it = (uint32_t)iset;
-        for (int tile = blockIdx.x + iset * gridDim.x; tile < g.total_tiles; tile += 2 * gridDim.x, it += 2) {
+        if (!UP && pw != 0) return;
+        int s = 0;
+        uint32_t ph = 0;
+        const uint32_t tx_bytes = (uint32_t)(A_BOX + (g.resident ? 0 : KH * KH * B_TILE));
+        for (int tile = blockIdx.x; tile < g.total_tiles; tile += gridDim.x) {
             const int img = tile / tiles_per_img;
             const int trem = tile - img * tiles_per_img;
             const int tyi = trem / g.tiles_x, txi = trem - tyi * g.tiles_x;
-            const uint32_t use = it / ring_tiles;
-            const uint32_t sj = (it - use * ring_tiles) * (uint32_t)g.cin_chunks + (uint32_t)q;
-            {   // this warp's next tile: its source lines start moving into L2 now
-                const int tile_n = tile + 2 * (int)gridDim.x;
-                if (tile_n < g.total_tiles) {
-                    const int img_n = tile_n / tiles_per_img;
-                    const int trem_n = tile_n - img_n * tiles_per_img;
-                    const int tyn = trem_n / g.tiles_x, txn = trem_n - tyn * g.tiles_x;
-                    up_prefetch_chunk(up, g, img_n, tyn * COL_TH, txn * COL_TW, q, lane);
-                }
-            }
-            ptx::mbar_wait(&empty[sj], (use & 1u) ^ 1u);
-            up_fill_chunk<2>(up, g, img, tyi * COL_TH, txi * COL_TW, q, lane, ptx::smem_u32(sA) + sj * (uint32_t)stage_bytes);
-            ptx::fence_proxy_async();       // generic-proxy stores -> visible to the MMA's async-proxy reads
-            __syncwarp();
-            if (lane == 0) ptx::mbar_arrive(&full[sj]);
-        }
-    } else {
-        const int q = warp & 3;
-        const int m = q * 32 + lane;
-        const int ty = m / COL_TW, tx = m - ty * COL_TW;
-        const int epi_set = (warp - 2) >> 2;                     // 0, or 1 when EPI == 2
-        // staging: 32 KB = 4 warps x 2 buffers x 4 KB (EPI 1) or 2 sets x 4 warps x 1 buffer (EPI 2)
-        const uint32_t stage_u = ptx::smem_u32(sHB) + (uint32_t)epi_set * 16384u + (uint32_t)q * (EPI == 2 ? 4096u : 8192u);
-        uint32_t nstore = 0;
-        uint32_t it = (uint32_t)epi_set;
-        // UP: this warp's chunk q of the CTA's itj-th tile -> stage (itj&1)*chunks + q (the ring holds two tiles)
-        auto up_fill = [&](int tile_j, uint32_t itj) {
-            const int img_j = tile_j / tiles_per_img;
-            const int trem_j = tile_j - img_j * tiles_per_img;
-            const int tyj = trem_j / g.tiles_x, txj = trem_j - tyj * g.tiles_x;
-            const uint32_t sj = (itj & 1u) * (uint32_t)g.cin_chunks + (uint32_t)q;
-            ptx::mbar_wait(&empty[sj], ((itj >> 1) & 1u) ^ 1u);
-            up_fill_chunk<1>(up, g, img_j, tyj * COL_TH, txj * COL_TW, q, lane,
-                          ptx::smem_u32(sA) + sj * (uint32_t)stage_bytes);
-            ptx::fence_proxy_async();       // generic-proxy stores -> visible to the MMA's async-proxy reads
-            __syncwarp();
-            if (lane == 0) ptx::mbar_arrive(&full[sj]);
-        };
-        if constexpr (UP == 1) {
-            // the first two tiles of the CTA (EPI = 2: each set fills the one it will finish)
-            for (int p = 0; p < 2; ++p) {
-                const int tile_p = (int)blockIdx.x + p * (int)gridDim.x;
-                if ((EPI == 1 || p == epi_set) && tile_p < g.total_tiles) up_fill(tile_p, (uint32_t)p);
-            }
-        }
-        for (int tile = blockIdx.x + epi_set * gridDim.x; tile < g.total_tiles; tile += EPI * gridDim.x, it += EPI) {
-            const uint32_t as = it & 1u;
-            const int img = tile / tiles_per_img;
-            const int trem = tile - img * tiles_per_img;
-            const int tyi = trem / g.tiles_x, txi = trem - tyi * g.tiles_x;
-            const int y = tyi * COL_TH + ty, x = txi * COL_TW + tx;
-            const bool valid = (y < g.Ho) && (x < g.Wo);
-            const size_t pix = ((size_t)img * g.Ho + y) * g.Wo + x;
-            // Residual: fetched COALESCED (load i of lane l = pixel 4i + l/8 of this warp, 16-byte
-            // chunk l%8: four full 128-byte lines per instruction instead of 32 strided sectors) and
-            // handed to the pixel-owning lanes through this warp's rows of the staging tile. The first
-            // 32 channels are issued before waiting for the accumulator so the latency overlaps the MMAs.
-            float4 rpre[8];
-            const float *rbase = nullptr;
-            if (res != nullptr) {
-                rbase = res + (((size_t)img * g.Ho + tyi * COL_TH) * g.Wo + txi * COL_TW) * g.res_cs + g.res_co;
-                res_fetch8<COL_TW>(rpre, rbase, q, lane, tyi * COL_TH, txi * COL_TW, g.Ho, g.Wo, g.res_cs);
-            }
-            ptx::mbar_wait(&tfull[as], (it >> 1) & 1u);
-            ptx::tc_fence_after();
-            const uint32_t tacc = tmem_base + ((uint32_t)(q * 32) << 16) + as * (uint32_t)g.BN;
-            for (int c0 = 0; c0 < g.BN; c0 += 32) {
-                uint32_t r[32];
-                ptx::tmem_ld_32x32b_x32(tacc + (uint32_t)c0, r);
-                ptx::tmem_ld_wait();
-                if (c0 + 32 >= g.BN) {
-                    // accumulators are in registers: hand the TMEM stage back to the MMA warp
-                    ptx::tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) ptx::mbar_arrive(&tempty[as]);
-                }
-                float v[32];
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {      // bias from shared memory: 8 broadcast LDS.128 instead of 32 LDG
-                    const float4 bv = reinterpret_cast<const float4 *>(s_bias + c0)[j];
-                    v[4 * j] = __uint_as_float(r[4 * j]) + bv.x;
-                    v[4 * j + 1] = __uint_as_float(r[4 * j + 1]) + bv.y;
-                    v[4 * j + 2] = __uint_as_float(r[4 * j + 2]) + bv.z;
-                    v[4 * j + 3] = __uint_as_float(r[4 * j + 3]) + bv.w;
-                }
-                // staging buffer of this chunk: the store issued two chunks ago has left it
-                const uint32_t buf = stage_u + (EPI == 2 ? 0u : (nstore & 1u) * 4096u);
-                if (!HEAD) {
+            const int y0 = tyi * COL_TH, x0 = txi * COL_TW;
+            for (int cc = 0; cc < g.cin_chunks; ++cc) {
+                uint8_t *st = sA + (size_t)s * stage_bytes;
+                if (UP && cc < g.split_chunk) {
+                    if (pw == cc) {
+                        ptx::mbar_wait(&empty[s], ph ^ 1u);
+                        up_fill_chunk(up, g, img, y0, x0, cc, lane, ptx::smem_u32(st));
+                        // generic-proxy stores into a stage that a later round refills by TMA (async proxy)
+                        ptx::fence_proxy_async();
+                        __syncwarp();
+                        if (lane == 0) ptx::mbar_arrive(&full[s]);
+                    }
+                } else if (pw == 0) {
                     if (lane == 0) {
-                        if (EPI == 2) ptx::tma_store_wait_read();
-                        else ptx::tma_store_wait_read1();
+                        ptx::mbar_wait(&empty[s], ph ^ 1u);
+                        ptx::mbar_arrive_expect_tx(&full[s], tx_bytes);
+                        if (cc < g.split_chunk)
+                            ptx::tma_load_4d(st, &tmA, &full[s], cc * KC, x0 - g.pad_l, y0 - g.pad_t, img);
+                        else
+                            ptx::tma_load_4d(st, &tmA2, &full[s], (cc - g.split_chunk) * KC, x0 - g.pad_l, y0 - g.pad_t, img);
+                        if (!g.resident)
+                            for (int t = 0; t < KH * KH; ++t)
+                                ptx::tma_load_2d(st + A_BYTES + (size_t)t * B_TILE, &tmB, &full[s], t * g.cin_pad + cc * KC, 0);
                     }
                     __syncwarp();
-                    if (res != nullptr) {
-                        epi_add_residual(v, rpre, buf, lane);
-                        if (c0 + 32 < g.BN)
-                            res_fetch8<COL_TW>(rpre, rbase + c0 + 32, q, lane, tyi * COL_TH, txi * COL_TW, g.Ho, g.Wo, g.res_cs);
-                    }
                 }
-                epi_activate(v, g.act, g.round_out);
-                if (HEAD) {
-                    // convraw.3 (model_repository.py:57) on the tensor cores: the activated tile goes
-                    // back to TMEM as the A operand of a 128x32x32 MMA issued by the MMA warp, then
-                    // bias + torch.argmax over the seg channels + NCHW stores happen here.
-                    uint32_t a2[32];
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) a2[j] = __float_as_uint(ptx::round_tf32(v[j]));
-                    ptx::tmem_st_32x32b_x32(tmem_base + ((uint32_t)(q * 32) << 16) + 64u + as * 32u, a2);
-                    ptx::tmem_st_wait();
-                    ptx::tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) ptx::mbar_arrive(&a2full[as]);
-                    if constexpr (UP == 1) {
-                        const int tile_n = tile + 2 * (int)gridDim.x;
-                        if (tile_n < g.total_tiles) up_fill(tile_n, it + 2u);
-                    }
-                    ptx::mbar_wait(&d2full[as], (it >> 1) & 1u);
-                    ptx::tc_fence_after();
-                    uint32_t d2[32];
-                    ptx::tmem_ld_32x32b_x32(tmem_base + ((uint32_t)(q * 32) << 16) + 128u + as * 32u, d2);
-                    ptx::tmem_ld_wait();
-                    if (valid) {
-                        const size_t npix = (size_t)g.Ho * g.Wo;
-                        float best = -INFINITY;
-                        int best_c = 0;
-                        if (g.head_nhwc) {
-                            // pixel-major record [cout] per pixel (what the voting layer's gather reads as one
-                            // contiguous piece): 16-byte stores, scalar tail when cout is not a multiple of 4
-                            float *o = head_out + pix * (size_t)g.head_cout;
-                            float val[32];
-#pragma unroll
-                            for (int co = 0; co < 32; ++co) {
-                                val[co] = __uint_as_float(d2[co]) + (co < g.head_cout ? s_head[co] : 0.f);
-                                if (co < g.head_seg && val[co] > best) {
-                                    best = val[co];
-                                    best_c = co;
-                                }
-                            }
-#pragma unroll
-                            for (int c4 = 0; c4 < 32; c4 += 4) {
-                                if (c4 + 4 <= g.head_cout)
-                                    *reinterpret_cast<float4 *>(o + c4) = make_float4(val[c4], val[c4 + 1], val[c4 + 2], val[c4 + 3]);
-                                else
-                                    for (int co = c4; co < c4 + 4; ++co)
-                                        if (co < g.head_cout) o[co] = val[co];
-                            }
-                        } else {
-                            float *o = head_out + (size_t)img * g.head_cout * npix + (size_t)y * g.Wo + x;
-#pragma unroll
-                            for (int co = 0; co < 32; ++co) {
-                                if (co < g.head_cout) {
-                                    const float val = __uint_as_float(d2[co]) + s_head[co];
-                                    o[(size_t)co * npix] = val;
-                                    if (co < g.head_seg && val > best) {
-                                        best = val;
-                                        best_c = co;
-                                    }
-                                }
-                            }
-                        }
-                        if (mask) {
-                            if (g.mask_esz == 8) reinterpret_cast<long long *>(mask)[pix] = best_c;
-                            else reinterpret_cast<unsigned char *>(mask)[pix] = (unsigned char)best_c;
-                        }
-                    }
-                } else {
-                    // Stores go through shared memory and one TMA box per warp and 32 channels: a thread
-                    // owns a pixel, so direct 16-byte stores hit 32 different 256..768-byte-strided
-                    // records per instruction (LSU-transaction bound).
-                    epi_stage(v, buf, lane);
-                    ptx::fence_proxy_async();
-                    __syncwarp();
-                    if (lane == 0) {
-                        ptx::tma_store_4d_u32(&tmO, buf, c0, txi * COL_TW, tyi * COL_TH + q * (32 / COL_TW), img);
-                        ptx::tma_store_commit();
-                    }
-                    ++nstore;
+                if (++s == g.stages) {
+                    s = 0;
+                    ph ^= 1u;
                 }
             }
         }
-        if (!HEAD && lane == 0) ptx::tma_store_wait_all();      // every issuing lane drains its own bulk groups
+        return;
     }
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        ptx::tc_fence_after();
-        ptx::tmem_dealloc(tmem_base, tmem_cols);
+
+    // consumer warpgroup wg: tile rows [8 wg, 8 wg + 8); this thread's A rows are tile pixels
+    // (8 wg + 2 wq, g8) and (8 wg + 2 wq + 1, g8), i.e. box rows rr0 and rr0 + PITCH at tap (0, 0)
+    const int wg = warp >> 2, wq = warp & 3;
+    const int g8 = lane >> 2, t4 = lane & 3;
+    const uint32_t rr0 = (uint32_t)((8 * wg + 2 * wq) * PITCH + g8);
+    const uint32_t sA_u = ptx::smem_u32(sA), sB_u = ptx::smem_u32(sB);
+    if (g.resident) ptx::mbar_wait(wfull, 0);
+    int s = 0;
+    uint32_t ph = 0;
+    for (int tile = blockIdx.x; tile < g.total_tiles; tile += gridDim.x) {
+        float acc[BN / 2];
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+        for (int cc = 0; cc < g.cin_chunks; ++cc) {
+            ptx::mbar_wait(&full[s], ph);
+            const uint32_t a0 = sA_u + (uint32_t)s * (uint32_t)stage_bytes;
+            const uint32_t b0 = g.resident ? sB_u + (uint32_t)(cc * KH * KH * B_TILE) : a0 + (uint32_t)A_BYTES;
+            // taps in groups of TG (a whole tap row for the narrow chunks, one tap for 32-channel chunks: register
+            // budget): gather the group's A fragments (tf32: the low 13 bits cleared), then TG * KC/8 MMAs
+            constexpr int TG = KC == 32 ? 1 : KH;
+#pragma unroll
+            for (int t0 = 0; t0 < KH * KH; t0 += TG) {
+                uint32_t a[TG][KC / 8][4];
+#pragma unroll
+                for (int u = 0; u < TG; ++u)
+#pragma unroll
+                    for (int ks = 0; ks < KC / 8; ++ks)
+#pragma unroll
+                        for (int f = 0; f < 4; ++f) {
+                            const int kh = (t0 + u) / KH, kw = (t0 + u) % KH;
+                            const uint32_t rr = rr0 + (uint32_t)((kh + (f & 1)) * PITCH + kw);
+                            const uint32_t off = rr * ROWB + (uint32_t)((8 * ks + t4 + 4 * (f >> 1)) * 4);
+                            uint32_t v;
+                            asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(a0 + ptx::swizzle_off(off, ROWB)));
+                            a[u][ks][f] = v & 0xFFFFE000u;
+                        }
+                ptx::wgmma_fence();
+#pragma unroll
+                for (int u = 0; u < TG; ++u) {
+                    const uint64_t bd = ptx::make_kmajor_desc(b0 + (uint32_t)((t0 + u) * B_TILE), ROWB);
+#pragma unroll
+                    for (int ks = 0; ks < KC / 8; ++ks)
+                        ptx::Wgmma<BN>::rs(acc, a[u][ks], bd + (uint64_t)(2 * ks), (cc | (t0 + u) | ks) != 0 ? 1u : 0u);
+                }
+                ptx::wgmma_commit();
+                ptx::wgmma_wait<0>();
+                ptx::fence_regs(acc);
+            }
+            __syncwarp();
+            if (lane == 0) ptx::mbar_arrive(&empty[s]);
+            if (++s == g.stages) {
+                s = 0;
+                ph ^= 1u;
+            }
+        }
+
+        const int img = tile / tiles_per_img;
+        const int trem = tile - img * tiles_per_img;
+        const int tyi = trem / g.tiles_x, txi = trem - tyi * g.tiles_x;
+        const int ty = 8 * wg + 2 * wq;
+        if constexpr (!HEAD) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int y = tyi * COL_TH + ty + h, x = txi * COL_TW + g8;
+                if (y >= g.Ho || x >= g.Wo) continue;
+                const size_t pix = ((size_t)img * g.Ho + y) * g.Wo + x;
+                float *optr = out + pix * g.out_cs + g.out_co;
+                const float *rptr = res ? res + pix * g.res_cs + g.res_co : nullptr;
+#pragma unroll
+                for (int j = 0; j < BN / 8; ++j) {
+                    const int c = 8 * j + 2 * t4;
+                    float2 v = make_float2(acc[4 * j + 2 * h] + s_bias[c], acc[4 * j + 2 * h + 1] + s_bias[c + 1]);
+                    if (rptr) {
+                        const float2 rv = __ldg(reinterpret_cast<const float2 *>(rptr + c));
+                        v.x += rv.x;
+                        v.y += rv.y;
+                    }
+                    v.x = epi_act(v.x, g.act, g.round_out);
+                    v.y = epi_act(v.y, g.act, g.round_out);
+                    *reinterpret_cast<float2 *>(optr + c) = v;
+                }
+            }
+        } else {
+            // convraw.3 (model_repository.py:57): the activated, tf32-rounded tile is the A operand of a
+            // 128 x 32 x 32 MMA against the head weights; accumulator entry (row, 8j+2t+e) is K position
+            // 8j+t+4e of step j, matching the permuted B rows written above.
+            uint32_t a2[4][4];
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+#pragma unroll
+                for (int f = 0; f < 4; ++f) {
+                    const int r = 4 * j + ((f & 1) << 1) + (f >> 1);      // f: (row g, k t), (g+8, t), (g, t+4), (g+8, t+4)
+                    const int c = 8 * j + 2 * t4 + (f >> 1);
+                    a2[j][f] = __float_as_uint(ptx::round_tf32(epi_act(acc[r] + s_bias[c], g.act, g.round_out)));
+                }
+            float hacc[16];
+#pragma unroll
+            for (int i = 0; i < 16; ++i) hacc[i] = 0.f;
+            const uint64_t hd = ptx::make_kmajor_desc(ptx::smem_u32(sH), 128);
+            ptx::wgmma_fence();
+#pragma unroll
+            for (int j = 0; j < 4; ++j) ptx::Wgmma<32>::rs(hacc, a2[j], hd + (uint64_t)(2 * j), j != 0 ? 1u : 0u);
+            ptx::wgmma_commit();
+            ptx::wgmma_wait<0>();
+            ptx::fence_regs(hacc);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int y = tyi * COL_TH + ty + h, x = txi * COL_TW + g8;
+                const bool valid = y < g.Ho && x < g.Wo;
+                const size_t pix = ((size_t)img * g.Ho + y) * g.Wo + x;
+                const size_t npix = (size_t)g.Ho * g.Wo;
+                float best = -INFINITY;
+                int best_c = 0;
+#pragma unroll
+                for (int j = 0; j < 4; ++j)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const int co = 8 * j + 2 * t4 + e;
+                        const float val = hacc[4 * j + 2 * h + e] + s_head[co];
+                        if (co < g.head_seg && val > best) {
+                            best = val;
+                            best_c = co;
+                        }
+                        if (valid && co < g.head_cout) {
+                            if (g.head_nhwc) head_out[pix * (size_t)g.head_cout + co] = val;
+                            else head_out[((size_t)img * g.head_cout + co) * npix + (size_t)y * g.Wo + x] = val;
+                        }
+                    }
+                // torch.argmax over the four lanes of the pixel: the largest value, the lowest channel among equals
+#pragma unroll
+                for (int o = 1; o < 4; o <<= 1) {
+                    const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+                    const int oc = __shfl_xor_sync(0xffffffffu, best_c, o);
+                    if (ob > best || (ob == best && oc < best_c)) {
+                        best = ob;
+                        best_c = oc;
+                    }
+                }
+                if (valid && mask && t4 == 0) {
+                    if (g.mask_esz == 8) reinterpret_cast<long long *>(mask)[pix] = best_c;
+                    else reinterpret_cast<unsigned char *>(mask)[pix] = (unsigned char)best_c;
+                }
+            }
+        }
     }
 }
 
 struct ColPlan {
-    CUtensorMap tmA, tmA2, tmB, tmH, tmO;
+    CUtensorMap tmA, tmA2, tmB;
     ColGeom g;
-    int kc, head, epi;
-    int up_mode;            // 0 none, 1 epilogue warps interpolate, 2 dedicated interpolation warps
-    ColUp up;
+    int kc, ksize, head, up, bn;
+    ColUp cup;
     unsigned grid;
     size_t smem;
     const float *bias, *res;
@@ -640,24 +441,37 @@ struct ColPlan {
 constexpr size_t SMEM_LIMIT = 227 * 1024;
 
 // K-chunk: 128-byte rows when Cin is a multiple of 32, 64-byte rows for the 16-channel stem, else
-// 32-byte rows (Cin=40: measured 0.73 ms vs 1.12 ms with zero-padded 128-byte rows).
+// 32-byte rows (Cin=40: 8-channel chunks instead of zero-padded 32-channel ones).
 int col_kc(int Cin) { return Cin % 32 == 0 ? 32 : (Cin == 16 ? 16 : 8); }
 int col_cin_pad(int Cin) { return Cin == 16 ? 16 : (Cin + 31) / 32 * 32; }   // packing of the weights
 
-size_t col_smem(int kc, int ksize, int cin_chunks, int bn, int dil, int stages, int head_cout, bool resident = true)
+size_t col_smem(int kc, int ksize, int cin_chunks, int bn, int stages, bool head, bool resident)
 {
     const size_t rowb = (size_t)kc * 4;
-    const size_t a_box = (size_t)(COL_TH + (ksize - 1) * dil) * (COL_TW + (ksize - 1) * dil) * rowb;
+    const size_t a_box = (size_t)(COL_TH + ksize - 1) * (COL_TW + ksize - 1) * rowb;
     const size_t a = (a_box + 1023) & ~(size_t)1023, bt = (size_t)bn * rowb;
     return 1024 + (resident ? (size_t)ksize * ksize * cin_chunks * bt : 0) +
-           (size_t)stages * (a + (resident ? 0 : (size_t)ksize * ksize * bt)) +
-           (size_t)(1 + 2 * stages + 4 + 5) * 8 + 16 + (size_t)(64 + 64) * 4 + 64 + (head_cout ? 4096 : 32768);
+           (size_t)stages * (a + (resident ? 0 : (size_t)ksize * ksize * bt)) + (head ? 4096 : 0) +
+           (size_t)(1 + 2 * stages) * 8 + (64 + 32) * 4;
 }
 
-template <int KC, bool HEAD, int KH, int EPI>
-cudaError_t set_attr()
+template <int KC, bool HEAD, int KH, bool UP, int BN>
+int col_launch(const ColPlan &p, cudaStream_t s)
 {
-    return cudaFuncSetAttribute(k_conv_col<KC, HEAD, KH, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_LIMIT);
+    // the instantiation must be the plan's: weight boxes, barrier byte counts and stores are sized by BN
+    if (p.bn != BN || p.kc != KC || p.ksize != KH || p.head != (HEAD ? 1 : 0) || p.up != (UP ? 1 : 0)) {
+        set_error("conv(col): no kernel instantiation for this plan (Cout %d, chunk %d, ksize %d)", p.bn, p.kc, p.ksize);
+        return PVNET_E_STATE;
+    }
+    auto fn = k_conv_col<KC, HEAD, KH, UP, BN>;
+    const cudaError_t attr_err = ensure_max_smem((const void *)fn, (int)SMEM_LIMIT);
+    PV_CUDA(attr_err);
+    const HeadDesc &h = p.hd;
+    fn<<<p.grid, COL_THREADS, p.smem, s>>>(p.tmA, p.tmA2, p.tmB, p.g, p.bias, p.res, p.out, p.head ? h.w : nullptr,
+                                           p.head ? h.bias : nullptr, p.head ? h.out_nchw : nullptr,
+                                           p.head ? h.mask : nullptr, p.cup);
+    PV_LAUNCHED("k_conv_col");
+    return PVNET_OK;
 }
 
 }  // namespace
@@ -671,7 +485,7 @@ bool conv_col_eligible(const ConvDesc &d)
     const int kc = col_kc(cin);
     if (d.Cin % kc != 0 || d.Cin2 % kc != 0) return false;
     if ((d.ksize == 4) != (kc == 16)) return false;   // instantiated: 4x4 taps with 16 channels, 3x3 otherwise
-    return col_smem(kc, d.ksize, (cin + kc - 1) / kc, d.Cout, d.dilation, 2, HEAD_MAX, false) <= SMEM_LIMIT;
+    return col_smem(kc, d.ksize, (cin + kc - 1) / kc, d.Cout, 2, true, false) <= SMEM_LIMIT;
 }
 
 size_t conv_col_plan_size() { return sizeof(ColPlan); }
@@ -690,34 +504,17 @@ int conv_col_plan_at(const ConvDesc &d, const HeadDesc *head, void *storage)
     PV_CHECK_ARG(!head || (d.Cout == 32 && col_kc(d.Cin + d.Cin2) != 16 && head->cout >= 1 && head->cout <= 32 && head->w && head->bias &&
                            head->out_nchw && (!head->mask || head->mask_esz == 1 || head->mask_esz == 8)),
                  "conv(col): bad fused-head description");
-    int kc = col_kc(d.Cin + d.Cin2);
-    // Half chunks (tuning knob PVNET_COL_HALF_CHUNKS=1, default off): a 3x3 layer with 144 KB of resident weights
-    // (layer1.*, conv2s.0) has room for only TWO 23 KB stages of 32 channels; the same bytes as four 12 KB stages of
-    // 16 channels (64-byte rows) keep three box requests in flight instead of one.  Measured: conv2s.0 0.357 against
-    // 0.329 ms, layer1 unchanged -- these launches are not waiting for their operand boxes (tensor pipe at the N<=64
-    // shared-memory floor), the extra barrier round per 18 MMAs only costs.
-    static const int env_half = [] {
-        const char *e = getenv("PVNET_COL_HALF_CHUNKS");
-        return e ? atoi(e) : 0;
-    }();
-    if (env_half && kc == 32 && d.ksize == 3 && !head &&
-        col_smem(32, 3, (d.Cin + d.Cin2) / 32, d.Cout, d.dilation, 3, 0, true) > SMEM_LIMIT &&
-        col_smem(32, 3, (d.Cin + d.Cin2) / 32, d.Cout, d.dilation, 2, 0, true) <= SMEM_LIMIT &&
-        col_smem(16, 3, (d.Cin + d.Cin2) / 16, d.Cout, d.dilation, 4, 0, true) <= SMEM_LIMIT)
-        kc = 16;
+    const int kc = col_kc(d.Cin + d.Cin2);
     ColGeom &g = p->g;
-    g.KW = g.KH = d.ksize;
     g.pad_l = g.pad_t = d.ksize == 4 ? 2 : 1;
     g.Ho = d.H;
     g.Wo = d.W;
     g.tiles_x = (d.W + COL_TW - 1) / COL_TW;
     g.tiles_y = (d.H + COL_TH - 1) / COL_TH;
     g.total_tiles = g.tiles_x * g.tiles_y * d.b;
-    g.dil = d.dilation;
     g.cin_chunks = (d.Cin + d.Cin2) / kc;
     g.split_chunk = d.in2 ? d.Cin / kc : g.cin_chunks;
     g.cin_pad = col_cin_pad(d.Cin + d.Cin2);   // weights are packed [Cout][KH][KW][cin_pad], zero padded
-    g.BN = d.Cout;
     g.out_cs = d.out_cs;
     g.out_co = d.out_co;
     g.res_cs = d.res_cs;
@@ -728,61 +525,50 @@ int conv_col_plan_at(const ConvDesc &d, const HeadDesc *head, void *storage)
     g.head_seg = head ? head->seg_dim : 0;
     g.mask_esz = head ? head->mask_esz : 0;
     g.head_nhwc = 0;
-    p->up.src = d.up_src;
-    p->up.h = d.H / 2;
-    p->up.w = d.W / 2;
-    p->up.cs = d.Cin;
-    p->up.sy = (float)(p->up.h - 1) / (float)(2 * p->up.h - 1);   // launch_upsample2x's scales
-    p->up.sx = (float)(p->up.w - 1) / (float)(2 * p->up.w - 1);
-    p->up.zero = 0;
-    p->up_mode = d.up_src ? (d.up_mode == 2 ? 2 : 1) : 0;
+    p->cup.src = d.up_src;
+    p->cup.h = d.H / 2;
+    p->cup.w = d.W / 2;
+    p->cup.cs = d.Cin;
+    p->cup.sy = (float)(p->cup.h - 1) / (float)(2 * p->cup.h - 1);   // launch_upsample2x's scales
+    p->cup.sx = (float)(p->cup.w - 1) / (float)(2 * p->cup.w - 1);
+    p->cup.zero = 0;
     // Resident weights whenever at least 2 A stages (one channel chunk with all its taps each) still
-    // fit next to them; otherwise the KH*KW weight tiles of a chunk travel with its A box.  Two CTAs
-    // per SM when the footprint allows.
+    // fit next to them; otherwise the KH*KW weight tiles of a chunk travel with its A box.
+    const bool hd = head != nullptr;
     int stages = 8;
     bool resident = true;
-    while (stages > 2 && col_smem(kc, d.ksize, g.cin_chunks, g.BN, g.dil, stages, g.head_cout, true) > SMEM_LIMIT)
-        --stages;
-    static const int min_res_stages = [] {
-        const char *e = getenv("PVNET_COL_RESIDENT_MIN_STAGES");   // tuning knob, default 2
-        return e ? atoi(e) : 2;
-    }();
-    if (stages < min_res_stages || col_smem(kc, d.ksize, g.cin_chunks, g.BN, g.dil, stages, g.head_cout, true) > SMEM_LIMIT) {
+    while (stages > 2 && col_smem(kc, d.ksize, g.cin_chunks, d.Cout, stages, hd, true) > SMEM_LIMIT) --stages;
+    if (col_smem(kc, d.ksize, g.cin_chunks, d.Cout, stages, hd, true) > SMEM_LIMIT) {
         resident = false;
         stages = 8;
-        while (stages > 2 &&
-               col_smem(kc, d.ksize, g.cin_chunks, g.BN, g.dil, stages, g.head_cout, false) > SMEM_LIMIT)
-            --stages;
+        while (stages > 2 && col_smem(kc, d.ksize, g.cin_chunks, d.Cout, stages, hd, false) > SMEM_LIMIT) --stages;
     }
-    if (d.up_src) {     // the ring is exactly two tiles: stage = (tile parity) * chunks + chunk (dedicated warps: four tiles)
-        stages = (d.up_mode == 2 ? 4 : 2) * g.cin_chunks;
-        PV_CHECK_ARG(resident && col_smem(kc, d.ksize, g.cin_chunks, g.BN, g.dil, stages, g.head_cout, true) <= SMEM_LIMIT,
-                     "conv(col): fused upsampling does not fit in shared memory");
-    }
+    PV_CHECK_ARG(!d.up_src || resident, "conv(col): fused upsampling needs resident weights");
     g.stages = stages;
     g.resident = resident ? 1 : 0;
-    p->smem = col_smem(kc, d.ksize, g.cin_chunks, g.BN, g.dil, stages, g.head_cout, resident);
+    p->smem = col_smem(kc, d.ksize, g.cin_chunks, d.Cout, stages, hd, resident);
     p->kc = kc;
-    p->head = head ? 1 : 0;
+    p->ksize = d.ksize;
+    p->bn = d.Cout;
+    p->head = hd ? 1 : 0;
+    p->up = d.up_src ? 1 : 0;
     if (head) p->hd = *head;
     if (!d.up_src) {
         const float *base = d.in + d.in_co;
         cuuint64_t dims[4] = {(cuuint64_t)d.Cin, (cuuint64_t)d.W, (cuuint64_t)d.H, (cuuint64_t)d.b};
         cuuint64_t strides[3] = {(cuuint64_t)d.in_cs * 4, (cuuint64_t)d.W * d.in_cs * 4,
                                  (cuuint64_t)d.H * d.W * d.in_cs * 4};
-        cuuint32_t box[4] = {(cuuint32_t)kc, (cuuint32_t)(COL_TW + (d.ksize - 1) * d.dilation),
-                             (cuuint32_t)(COL_TH + (d.ksize - 1) * d.dilation), 1};
+        cuuint32_t box[4] = {(cuuint32_t)kc, (cuuint32_t)(COL_TW + d.ksize - 1), (cuuint32_t)(COL_TH + d.ksize - 1), 1};
         int rc = tma_encode(&p->tmA, base, 4, dims, strides, box, kc * 4);
         if (rc) return rc;
+        p->tmA2 = p->tmA;
     }
-    if (!d.up_src) p->tmA2 = p->tmA;
     if (d.in2) {
         PV_CHECK_ARG(d.in2_cs % 4 == 0 && d.in2_co % 4 == 0 && d.Cin2 > 0, "conv(col): second source stride/offset alignment");
         cuuint64_t dims[4] = {(cuuint64_t)d.Cin2, (cuuint64_t)d.W, (cuuint64_t)d.H, (cuuint64_t)d.b};
         cuuint64_t strides[3] = {(cuuint64_t)d.in2_cs * 4, (cuuint64_t)d.W * d.in2_cs * 4,
                                  (cuuint64_t)d.H * d.W * d.in2_cs * 4};
-        cuuint32_t box[4] = {(cuuint32_t)kc, (cuuint32_t)(COL_TW + (d.ksize - 1) * d.dilation),
-                             (cuuint32_t)(COL_TH + (d.ksize - 1) * d.dilation), 1};
+        cuuint32_t box[4] = {(cuuint32_t)kc, (cuuint32_t)(COL_TW + d.ksize - 1), (cuuint32_t)(COL_TH + d.ksize - 1), 1};
         int rc = tma_encode(&p->tmA2, d.in2 + d.in2_co, 4, dims, strides, box, kc * 4);
         if (rc) return rc;
         if (d.up_src) p->tmA = p->tmA2;     // the first source is interpolated in the kernel, not read by TMA
@@ -794,46 +580,8 @@ int conv_col_plan_at(const ConvDesc &d, const HeadDesc *head, void *storage)
         int rc = tma_encode(&p->tmB, d.w, 2, dims, strides, box, kc * 4);
         if (rc) return rc;
     }
-    if (!head) {     // output slice [b,H,W,out_cs] at out_co, stored by TMA in boxes {32 ch, TW, TH, 1}
-        cuuint64_t dims[4] = {(cuuint64_t)d.Cout, (cuuint64_t)d.W, (cuuint64_t)d.H, (cuuint64_t)d.b};
-        cuuint64_t strides[3] = {(cuuint64_t)d.out_cs * 4, (cuuint64_t)d.W * d.out_cs * 4,
-                                 (cuuint64_t)d.H * d.W * d.out_cs * 4};
-        cuuint32_t box[4] = {32, (cuuint32_t)COL_TW, (cuuint32_t)(32 / COL_TW), 1};     // one epilogue warp: 32 pixels
-        int rc = tma_encode(&p->tmO, d.out + d.out_co, 4, dims, strides, box, 128);
-        if (rc) return rc;
-    } else {
-        p->tmO = p->tmA;
-    }
-    if (head) {      // convraw.3 weights [cout][32] fp32, read as a 32x32 K-major tile (rows beyond cout: zero fill)
-        PV_CHECK_ARG((uintptr_t)head->w % 16 == 0, "conv(col): head weights must be 16-byte aligned");
-        cuuint64_t dims[2] = {32, (cuuint64_t)head->cout};
-        cuuint64_t strides[1] = {128};
-        cuuint32_t box[2] = {32, 32};
-        int rc = tma_encode(&p->tmH, head->w, 2, dims, strides, box, 128);
-        if (rc) return rc;
-    } else {
-        p->tmH = p->tmB;
-    }
-    const int per_sm = (int)(SMEM_LIMIT / p->smem) >= 2 ? 2 : 1;
-    static const int env_epi = [] {
-        const char *e = getenv("PVNET_COL_EPI");       // tuning knob: 1 forces a single epilogue warp set
-        return e ? atoi(e) : 2;
-    }();
-    // Two epilogue warp sets (alternating tiles, one per TMEM accumulator stage; the 32 KB of staging
-    // are then 8 single buffers instead of 4 double ones) when the CTA is alone on its SM anyway and
-    // the variant exists: the short-K layers are epilogue-bound (ncu: stem tensor pipe 40 %).
-    p->epi = (env_epi == 2 && !head && kc != 8 && per_sm == 1) ? 2 : 1;
-    // Fused head (convraw.0), tuning knob PVNET_HEAD_EPI=2: two epilogue warp sets alternating tiles (set s owns
-    // TMEM stage s, the EPI = 2 protocol) with two CTAs per SM still resident at 96 registers per thread.
-    // Measured no gain (0.449 against 0.429 ms): the launch is bound by the tensor pipe (sm__pipe_tc_cycles_active
-    // 75 %: 45 N=32 MMAs per tile at the 40-cycle shared-memory operand floor), not by its epilogue.  Default 1.
-    static const int env_head_epi = [] {
-        const char *e = getenv("PVNET_HEAD_EPI");
-        return e ? atoi(e) : 1;
-    }();
-    if (head && kc == 8 && (g_head_epi ? g_head_epi : env_head_epi) == 2) p->epi = 2;
-    if (p->up_mode == 2) p->epi = 2;
-    long long grid = (long long)sm_count() * (p->up_mode == 2 ? 1 : per_sm);
+    PV_CHECK_ARG(!head || (uintptr_t)head->w % 16 == 0, "conv(col): head weights must be 16-byte aligned");
+    long long grid = (long long)sm_count();
     if (grid > g.total_tiles) grid = g.total_tiles;
     p->grid = (unsigned)grid;
     p->bias = d.bias;
@@ -855,49 +603,18 @@ void conv_col_set_head_ptrs(void *storage, float *out_nchw, void *mask, int mask
 int conv_col_launch_at(const void *storage, cudaStream_t s)
 {
     const ColPlan &p = *static_cast<const ColPlan *>(storage);
-    const void *fn = p.up_mode == 2 ? (const void *)k_conv_col<8, true, 3, 2, 2>
-                     : p.up_mode == 1 ? (p.epi == 2 ? (const void *)k_conv_col<8, true, 3, 2, 1> : (const void *)k_conv_col<8, true, 3, 1, 1>)
-                     : (p.kc == 32 && !p.head) ? (p.epi == 2 ? (const void *)k_conv_col<32, false, 3, 2> : (const void *)k_conv_col<32, false, 3, 1>)
-                     : (p.kc == 16 && !p.head && p.g.KH == 3) ? (p.epi == 2 ? (const void *)k_conv_col<16, false, 3, 2> : (const void *)k_conv_col<16, false, 3, 1>)
-                     : (p.kc == 16 && !p.head) ? (p.epi == 2 ? (const void *)k_conv_col<16, false, 4, 2> : (const void *)k_conv_col<16, false, 4, 1>)
-                     : (p.kc == 8 && !p.head) ? (const void *)k_conv_col<8, false, 3, 1>
-                     : p.kc == 32 ? (const void *)k_conv_col<32, true, 3, 1>
-                     : p.epi == 2 ? (const void *)k_conv_col<8, true, 3, 2> : (const void *)k_conv_col<8, true, 3, 1>;
-    const cudaError_t attr_err = ensure_max_smem(fn, (int)SMEM_LIMIT);
-    PV_CUDA(attr_err);
-    const HeadDesc &h = p.hd;
-#define COL_LAUNCH(KC_, HEAD_, KH_, EPI_, UP_)                                                                    \
-    k_conv_col<KC_, HEAD_, KH_, EPI_, UP_><<<p.grid, 64 + 128 * EPI_ + (UP_ == 2 ? 32 * UP_WARPS : 0), p.smem, s>>>(p.tmA, p.tmA2, p.tmB, p.tmH, p.tmO, p.g, p.bias, p.res, p.out,      \
-                                                                p.head ? h.w : nullptr, p.head ? h.bias : nullptr, \
-                                                                p.head ? h.out_nchw : nullptr, p.head ? h.mask : nullptr, p.up)
-    if (p.up_mode == 2) COL_LAUNCH(8, true, 3, 2, 2);
-    else if (p.up_mode == 1 && p.epi == 2) COL_LAUNCH(8, true, 3, 2, 1);
-    else if (p.up_mode == 1) COL_LAUNCH(8, true, 3, 1, 1);
-    else if (p.kc == 32 && !p.head && p.epi == 2) COL_LAUNCH(32, false, 3, 2, 0);
-    else if (p.kc == 32 && !p.head) COL_LAUNCH(32, false, 3, 1, 0);
-    else if (p.kc == 16 && !p.head && p.g.KH == 3 && p.epi == 2) COL_LAUNCH(16, false, 3, 2, 0);
-    else if (p.kc == 16 && !p.head && p.g.KH == 3) COL_LAUNCH(16, false, 3, 1, 0);
-    else if (p.kc == 16 && !p.head && p.epi == 2) COL_LAUNCH(16, false, 4, 2, 0);
-    else if (p.kc == 16 && !p.head) COL_LAUNCH(16, false, 4, 1, 0);
-    else if (p.kc == 8 && !p.head) COL_LAUNCH(8, false, 3, 1, 0);
-    else if (p.kc == 32) COL_LAUNCH(32, true, 3, 1, 0);
-    else if (p.epi == 2) COL_LAUNCH(8, true, 3, 2, 0);
-    else COL_LAUNCH(8, true, 3, 1, 0);
-#undef COL_LAUNCH
-    PV_LAUNCHED("k_conv_col");
-    return PVNET_OK;
+    if (p.up) return col_launch<8, true, 3, true, 32>(p, s);
+    if (p.head) return p.kc == 32 ? col_launch<32, true, 3, false, 32>(p, s) : col_launch<8, true, 3, false, 32>(p, s);
+    const bool n64 = p.bn == 64;
+    if (p.ksize == 4) return n64 ? col_launch<16, false, 4, false, 64>(p, s) : col_launch<16, false, 4, false, 32>(p, s);
+    if (p.kc == 32) return n64 ? col_launch<32, false, 3, false, 64>(p, s) : col_launch<32, false, 3, false, 32>(p, s);
+    if (p.kc == 16) return n64 ? col_launch<16, false, 3, false, 64>(p, s) : col_launch<16, false, 3, false, 32>(p, s);
+    return n64 ? col_launch<8, false, 3, false, 64>(p, s) : col_launch<8, false, 3, false, 32>(p, s);
 }
 
 }  // namespace pvnet
 
 extern "C" {
-// test hook: epilogue warp sets of the fused-head column kernel (plans built afterwards); 0 = default
-int pvnet_conv_set_head_epilogue_sets(int sets)
-{
-    PV_CHECK_ARG(sets >= 0 && sets <= 2, "sets must be 0, 1 or 2");
-    pvnet::g_head_epi = sets;
-    return PVNET_OK;
-}
 // test hook: 0 auto, 1 force the per-tap kernel, 2 force the column kernel
 int pvnet_conv_set_mode(int mode)
 {

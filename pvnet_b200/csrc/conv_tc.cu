@@ -1,30 +1,28 @@
-// conv_tc.cu -- implicit-GEMM 2-D convolution on the 5th-gen tensor cores (sm_100a).
+// conv_tc.cu -- implicit-GEMM 2-D convolution on the Hopper tensor cores (wgmma, sm_90a).
 //
-// One CTA computes a 128-pixel x BN-channel output tile of an NHWC convolution
+// One CTA computes 128-pixel x BN-channel output tiles of an NHWC convolution
 // (lib/networks/resnet.py:28-35 `conv3x3`, the 1x1 downsample convs, and the decoder convs
 // of lib/networks/model_repository.py:22-58), with BatchNorm folded into weights/bias and
 // the activation / residual add fused into the epilogue:
 //
-//   M = 128 output pixels (a TH x TW patch of one image), one TMEM lane each
-//   N = BN output channels (<= 256), one TMEM fp32 column each
-//   K = taps x Cin, walked tap by tap in chunks of KC input channels
+//   M = 128 output pixels (a TH x TW = 8 x 16 patch of one image)
+//   N = BN output channels (32, 64 or 128)
+//   K = taps x Cin, walked tap by tap in chunks of 32 input channels
 //
-//   warp 0    TMA producer: per K-block one 4-D box {KC ch, TW, TH, 1 image} of the NHWC
-//             input, shifted by the tap's (dy,dx)*dilation -- out-of-bounds coordinates are
-//             zero-filled by TMA, which IS the conv padding -- plus one 2-D box {KC, BN} of
-//             the packed weights [Cout][tap][Cin]; 128B/32B-swizzled K-major tiles.
-//   warp 1    TMEM allocation; one elected lane issues tcgen05.mma.kind::tf32 (fp32
-//             accumulate in TMEM) and commits to the stage's "empty" mbarrier.
-//   warps 2-5 epilogue: tcgen05.ld 32 columns at a time -> +bias (+residual) -> ReLU /
-//             LeakyReLU(0.1) -> optional round-to-tf32 -> NHWC output at a channel offset of a
-//             (possibly wider) destination buffer, so torch.cat never happens.  The persistent
-//             kernel (k_conv_tap_p, the one the backbone runs) stages each warp's 32 pixels x 32
-//             channels in shared memory and stores them with one TMA box; k_conv_tc keeps
-//             direct 128-bit stores.
+//   warp 8       TMA producer: per K-block one 4-D box {32 ch, TW, TH, 1 image} of the NHWC input,
+//                shifted by the tap's (dy,dx)*dilation -- out-of-bounds coordinates are zero-filled
+//                by TMA, which IS the conv padding -- plus one 2-D box {32, BN} of the packed weights
+//                [Cout][tap][Cin]; 128-byte-swizzled K-major tiles in a ring of mbarrier-guarded stages.
+//   warps 0-7    two consumer warpgroups, 64 pixel rows each: wgmma.m64nBNk8 (tf32 in, fp32
+//                accumulate in registers) straight from the stage, then the epilogue: +bias (+residual)
+//                -> ReLU / LeakyReLU(0.1) -> optional round-to-tf32 -> NHWC output at a channel offset
+//                of a (possibly wider) destination buffer, so torch.cat never happens.
 //
-// k_conv_tap_p adds: CTAs persistent over (M tile, N tile) items with a continuous TMA ring
-// (4..8 stages, as many as fit), two TMEM accumulator stages (epilogue of item i overlaps the MMAs
-// of item i+1), and the tail split of the static schedule (see conv_plan).
+// CTAs are persistent over (M tile, N tile) items (static round-robin; the ring runs on across items,
+// so the producer fetches the next item's operands during the current epilogue), or one item per CTA.
+// MC (pvnet_conv_set_multicast(1)): clusters of two CTAs on adjacent M tiles of the same N tile; each CTA
+// loads its A box and HALF of the weight tile, multicast into both, so the weights cross L2 -> SM once per
+// pair; a stage is refilled only after the consumers of BOTH CTAs released it.
 //
 // Stride-2 convolutions read the input through four "parity plane" tensor maps (even/odd
 // rows x even/odd columns); each tap then is a stride-1 box in one plane.
@@ -49,344 +47,78 @@ struct ConvGeom {
     int round_out;  // round stored values to tf32 (they feed another tensor-core conv)
     signed char tap_map[9];
     short tap_ox[9], tap_oy[9];
-    // persistent kernel, tail split: items [0, n_full) are (M tile, BN-channel) tiles; each of the
-    // remaining (M tile, N tile) pairs is cut into tail_split items of tail_bn channels so that the
-    // last, partially filled round of the static schedule costs a fraction of a full round
-    int n_full, n_items, tail_bn, tail_split;
-    int stages;     // persistent kernel: depth of the TMA ring (4..8, as many as fit next to the staging buffers)
+    int n_items;    // M tiles x N tiles, N tile fastest
+    int stages;     // depth of the TMA ring
 };
-
-// item index -> (M tile, first output channel, channels) of the persistent schedule
-struct ConvItem {
-    int m_tile, n0, bn;
-};
-__device__ __forceinline__ ConvItem conv_item(const ConvGeom &g, int item, int n_tiles_n)
-{
-    ConvItem r;
-    int base = item, sub = 0;
-    r.bn = g.BN;
-    if (item >= g.n_full) {
-        const int j = item - g.n_full;
-        base = g.n_full + j / g.tail_split;
-        sub = j - (j / g.tail_split) * g.tail_split;
-        r.bn = g.tail_bn;
-    }
-    r.m_tile = base / n_tiles_n;                       // N tile fastest
-    r.n0 = (base - r.m_tile * n_tiles_n) * g.BN + sub * g.tail_bn;
-    return r;
-}
 
 struct AMaps {
     CUtensorMap m[4];
 };
 
-constexpr int CONV_THREADS = 192;
+constexpr int CONV_THREADS = 288;      // two consumer warpgroups + one producer warp
+constexpr int CONV_KC = 32;            // input channels per K-block: one 128-byte swizzled row per pixel
+constexpr int CONV_A_BYTES = 128 * CONV_KC * 4;
 
-template <int KC>
-struct ConvCfg {
-    static constexpr int SWIZZLE = KC * 4;              // bytes per K-major row: 128 or 32
-    static constexpr int A_BYTES = 128 * KC * 4;
-    static constexpr int STAGES = KC == 32 ? 4 : 8;
-    static constexpr int b_bytes(int bn) { return bn * KC * 4; }
-    static constexpr size_t smem_bytes(int bn)
-    {
-        return 1024 + (size_t)STAGES * (A_BYTES + b_bytes(bn)) + 256;
-    }
-};
-
-// MC = 1: launched as clusters of 2 CTAs (adjacent M tiles, same N tile).  Each CTA loads its own
-// A box and HALF of the {KC, BN} weight tile, multicast into both CTAs' shared memory: the weight
-// tile, 2/3 of the bytes of a K-block at BN=256, crosses L2->SM once per pair instead of twice.
-// (ncu/bench: the 60x80 layers were bound at ~49 B/clk/SM of L2->SM traffic, 245 cycles per MMA
-// against the 128-cycle floor measured in benchmarks/micro/mma_rate.cu.)
-template <int KC, int MC>
+template <int BN, bool MC>
 __global__ void __launch_bounds__(CONV_THREADS, 1)
-    k_conv_tc(const __grid_constant__ AMaps amaps, const __grid_constant__ CUtensorMap tmB, const ConvGeom g,
-              const float *__restrict__ bias, const float *__restrict__ res, float *__restrict__ out)
+    k_conv_tap(const __grid_constant__ AMaps amaps, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ ConvGeom g,
+               const float *__restrict__ bias, const float *__restrict__ res, float *__restrict__ out)
 {
-    using Cfg = ConvCfg<KC>;
-    constexpr int STAGES = MC == 2 ? 6 : Cfg::STAGES;
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    // MC == 2: this CTA holds only its half (BN/2 rows) of the weight tile
-    const int b_bytes = (MC == 2 ? g.BN / 2 : g.BN) * KC * 4;
-    const int stage_bytes = Cfg::A_BYTES + b_bytes;
-    uint64_t *full = reinterpret_cast<uint64_t *>(smem + (size_t)STAGES * stage_bytes);
-    uint64_t *empty = full + STAGES;
-    uint64_t *tmem_full = empty + STAGES;
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(tmem_full + 1);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int tiles_per_img = g.tiles_x * g.tiles_y;
-    const uint32_t crank = MC ? ptx::cluster_ctarank() : 0u;
-    // an odd tile count leaves the last cluster one tile short: its second CTA recomputes the last
-    // tile (identical values) so that it still takes part in the multicast protocol
-    // 1-D grid, N tile fastest: the CTAs (or CTA pairs) that share an A tile run back to back, so
-    // the activation tile is fetched from DRAM once and served from L2 for the other N tiles
-    // (with N as the slow grid dimension ncu showed ~3x the compulsory DRAM reads on layer4).
-    const int n_tiles_n = g.Cout / g.BN;
-    int m_tile, n_tile;
-    if (MC) {
-        const int q = (int)blockIdx.x >> 1;
-        n_tile = q % n_tiles_n;
-        m_tile = 2 * (q / n_tiles_n) + (int)crank;
-    } else {
-        n_tile = (int)blockIdx.x % n_tiles_n;
-        m_tile = (int)blockIdx.x / n_tiles_n;
-    }
-    const int tile_lin = min(m_tile, g.total_m_tiles - 1);
-    const int img = tile_lin / tiles_per_img;
-    const int trem = tile_lin - img * tiles_per_img;
-    const int tyi = trem / g.tiles_x, txi = trem - tyi * g.tiles_x;
-    const int y0 = tyi * g.TH, x0 = txi * g.TW;
-    const int n0 = n_tile * g.BN;
-    const int nkb = g.taps * g.cin_chunks;
-
-    uint32_t tmem_cols = 32;
-    while (tmem_cols < (uint32_t)g.BN) tmem_cols <<= 1;
-
-    if (warp == 0 && lane == 0) {
-        ptx::prefetch_tensormap(&tmB);
-        ptx::prefetch_tensormap(&amaps.m[0]);
-        for (int s = 0; s < STAGES; ++s) {
-            ptx::mbar_init(&full[s], 1);
-            ptx::mbar_init(&empty[s], MC == 1 ? 2 : 1);   // MC 1: both CTAs of the pair must have consumed the stage
-        }
-        ptx::mbar_init(tmem_full, 1);
-        ptx::fence_barrier_init();
-    }
-    if (warp == 1) {
-        if (MC == 2) {
-            ptx::tmem_alloc_2sm(tmem_slot, tmem_cols);
-            ptx::tmem_relinquish_2sm();
-        } else {
-            ptx::tmem_alloc(tmem_slot, tmem_cols);
-            ptx::tmem_relinquish();
-        }
-    }
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (MC) ptx::cluster_sync();                       // peer barriers are initialised before any remote arrive
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (warp == 0) {
-        if (lane == 0) {
-            int s = 0, tap = 0, cc = 0;
-            uint32_t ph = 0;
-            for (int kb = 0; kb < nkb; ++kb) {
-                ptx::mbar_wait(&empty[s], ph ^ 1u);
-                uint8_t *sa = smem + (size_t)s * stage_bytes;
-                if (MC == 2) {
-                    // both CTAs load their A rows and their half of B; all bytes are counted on the
-                    // leader's barrier, which alone feeds the 2-SM MMA
-                    if (crank == 0) ptx::mbar_arrive_expect_tx(&full[s], (uint32_t)(2 * stage_bytes));
-                    ptx::tma_load_4d_2sm(sa, &amaps.m[g.tap_map[tap]], &full[s], cc * KC, x0 + g.tap_ox[tap],
-                                         y0 + g.tap_oy[tap], img);
-                    ptx::tma_load_2d_2sm(sa + Cfg::A_BYTES, &tmB, &full[s], tap * g.cin_pad + cc * KC,
-                                         n0 + (int)crank * (g.BN / 2));
-                    goto advance;
-                }
-                ptx::mbar_arrive_expect_tx(&full[s], (uint32_t)stage_bytes);
-                ptx::tma_load_4d(sa, &amaps.m[g.tap_map[tap]], &full[s], cc * KC, x0 + g.tap_ox[tap],
-                                 y0 + g.tap_oy[tap], img);
-                if (MC) {
-                    const int half = b_bytes / 2;      // rows [crank*BN/2, +BN/2) of the weight tile
-                    ptx::tma_load_2d_mc(sa + Cfg::A_BYTES + crank * half, &tmB, &full[s], tap * g.cin_pad + cc * KC,
-                                        n0 + (int)crank * (g.BN / 2), (uint16_t)0x3);
-                } else {
-                    ptx::tma_load_2d(sa + Cfg::A_BYTES, &tmB, &full[s], tap * g.cin_pad + cc * KC, n0);
-                }
-            advance:
-                if (++cc == g.cin_chunks) {
-                    cc = 0;
-                    ++tap;
-                }
-                if (++s == STAGES) {
-                    s = 0;
-                    ph ^= 1u;
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // The whole warp runs the loop converged (warp-uniform values stay in uniform registers);
-        // one elected lane issues the MMAs and commits.
-        if (MC != 2 || crank == 0) {
-            const uint32_t idesc = ptx::make_idesc_tf32(MC == 2 ? 256 : 128, g.BN);
-            const uint64_t dbase = ptx::make_kmajor_desc(0, Cfg::SWIZZLE);
-            const uint32_t smem_u = ptx::smem_u32(smem);
-            int s = 0;
-            uint32_t ph = 0;
-            for (int kb = 0; kb < nkb; ++kb) {
-                ptx::mbar_wait(&full[s], ph);
-                ptx::tc_fence_after();
-                const uint32_t sa = smem_u + (uint32_t)s * (uint32_t)stage_bytes;
-                const uint64_t adesc = dbase + (uint64_t)(sa >> 4);
-                const uint64_t bdesc = dbase + (uint64_t)((sa + Cfg::A_BYTES) >> 4);
-                if (ptx::elect_one()) {
-#pragma unroll
-                    for (int k = 0; k < KC / 8; ++k) {   // 8 tf32 = 32 B per MMA along K: +2 in 16-byte units
-                        if (MC == 2)
-                            ptx::mma_tf32_ss_2sm(tmem_base, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc,
-                                                 (kb | k) != 0 ? 1u : 0u);
-                        else
-                            ptx::mma_tf32_ss(tmem_base, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc,
-                                             (kb | k) != 0 ? 1u : 0u);
-                    }
-                    if (MC == 2) ptx::mma_commit_2sm_mc(&empty[s], (uint16_t)0x3);
-                    else if (MC == 1) ptx::mma_commit_mc(&empty[s], (uint16_t)0x3);
-                    else ptx::mma_commit(&empty[s]);
-                }
-                __syncwarp();
-                if (++s == STAGES) {
-                    s = 0;
-                    ph ^= 1u;
-                }
-            }
-            if (ptx::elect_one()) {
-                if (MC == 2) ptx::mma_commit_2sm_mc(tmem_full, (uint16_t)0x3);
-                else ptx::mma_commit(tmem_full);
-            }
-            __syncwarp();
-        }
-    } else {
-        // TMEM lane quarter a warp may touch is (warp id % 4)
-        const int q = warp & 3;
-        const int m = q * 32 + lane;
-        const int ty = m / g.TW, tx = m - ty * g.TW;
-        const int y = y0 + ty, x = x0 + tx;
-        const bool valid = (y < g.Ho) && (x < g.Wo);
-        const size_t pix = ((size_t)img * g.Ho + y) * g.Wo + x;
-        float *optr = out + pix * g.out_cs + g.out_co + n0;
-        const float *rptr = res ? res + pix * g.res_cs + g.res_co + n0 : nullptr;
-        ptx::mbar_wait(tmem_full, 0);
-        ptx::tc_fence_after();
-        for (int c0 = 0; c0 < g.BN; c0 += 32) {
-            uint32_t r[32];
-            ptx::tmem_ld_32x32b_x32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c0, r);
-            ptx::tmem_ld_wait();
-            if (valid) {
-#pragma unroll
-                for (int j = 0; j < 32; j += 4) {
-                    const float4 bv = __ldg(reinterpret_cast<const float4 *>(bias + n0 + c0 + j));
-                    float4 v = make_float4(__uint_as_float(r[j]) + bv.x, __uint_as_float(r[j + 1]) + bv.y,
-                                           __uint_as_float(r[j + 2]) + bv.z, __uint_as_float(r[j + 3]) + bv.w);
-                    if (rptr) {
-                        const float4 rv = __ldg(reinterpret_cast<const float4 *>(rptr + c0 + j));
-                        v.x += rv.x;
-                        v.y += rv.y;
-                        v.z += rv.z;
-                        v.w += rv.w;
-                    }
-                    if (g.act == 1) {
-                        v.x = fmaxf(v.x, 0.f);
-                        v.y = fmaxf(v.y, 0.f);
-                        v.z = fmaxf(v.z, 0.f);
-                        v.w = fmaxf(v.w, 0.f);
-                    } else if (g.act == 2) {
-                        v.x = v.x > 0.f ? v.x : 0.1f * v.x;
-                        v.y = v.y > 0.f ? v.y : 0.1f * v.y;
-                        v.z = v.z > 0.f ? v.z : 0.1f * v.z;
-                        v.w = v.w > 0.f ? v.w : 0.1f * v.w;
-                    }
-                    if (g.round_out) {
-                        v.x = ptx::round_tf32(v.x);
-                        v.y = ptx::round_tf32(v.y);
-                        v.z = ptx::round_tf32(v.z);
-                        v.w = ptx::round_tf32(v.w);
-                    }
-                    *reinterpret_cast<float4 *>(optr + c0 + j) = v;
-                }
-            }
-        }
-    }
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (MC) ptx::cluster_sync();                       // no CTA exits while its peer may still write into it
-    if (warp == 1) {
-        ptx::tc_fence_after();
-        if (MC == 2) ptx::tmem_dealloc_2sm(tmem_base, tmem_cols);
-        else ptx::tmem_dealloc(tmem_base, tmem_cols);
-    }
-}
-
-// ------------------------------------------------------------------ persistent per-tap kernel
-// Same tile math as k_conv_tc<KC,0>, but each CTA walks a static round-robin list of
-// (M tile, N tile) items with a continuous TMA ring and TWO TMEM accumulator stages, so the
-// prologue (barrier init, TMEM allocation, first TMA round trip) is paid once per CTA and the
-// epilogue of item i overlaps the MMAs of item i+1.  For the short-K layers (layer2, 1x1
-// downsamples, conv8s/conv4s) the per-tile prologue + epilogue of the one-tile-per-CTA kernel
-// cost as much as the MMAs themselves.
-template <int KC>
-__global__ void __launch_bounds__(CONV_THREADS, 2)
-    k_conv_tap_p(const __grid_constant__ AMaps amaps, const __grid_constant__ CUtensorMap tmB,
-                 const __grid_constant__ CUtensorMap tmB2 /* {KC, tail_bn} boxes of the same weights */,
-                 const __grid_constant__ CUtensorMap tmO, const __grid_constant__ ConvGeom g,
-                 const float *__restrict__ bias, const float *__restrict__ res, float *__restrict__ out)
-{
-    using Cfg = ConvCfg<KC>;
+    constexpr int B_BYTES = BN * CONV_KC * 4;
+    constexpr int STAGE_BYTES = CONV_A_BYTES + B_BYTES;
     const int STAGES = g.stages;
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    const int b_bytes = g.BN * KC * 4;
-    const int stage_bytes = Cfg::A_BYTES + b_bytes;
-    uint8_t *sOut = smem + (size_t)STAGES * stage_bytes;   // TMA-store staging: 4 epilogue warps x 2 buffers x 4 KB
-    uint64_t *full = reinterpret_cast<uint64_t *>(sOut + 32768);
+    uint64_t *full = reinterpret_cast<uint64_t *>(smem + (size_t)STAGES * STAGE_BYTES);
     uint64_t *empty = full + STAGES;
-    uint64_t *tfull = empty + STAGES;      // [2]
-    uint64_t *tempty = tfull + 2;          // [2]
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(tempty + 2);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int tiles_per_img = g.tiles_x * g.tiles_y;
-    const int n_tiles_n = g.Cout / g.BN;
-    const int n_items = g.n_items;
+    const int n_tiles_n = g.Cout / BN;
     const int nkb = g.taps * g.cin_chunks;
-    uint32_t tmem_cols = 32;
-    while (tmem_cols < (uint32_t)(2 * g.BN)) tmem_cols <<= 1;
+    // MC: item = (M tile pair, N tile); CTA rank r of the pair takes M tile 2*pair + r (an odd tile count
+    // leaves the last pair one tile short: its second CTA recomputes the last tile, identical values)
+    const uint32_t crank = MC ? ptx::cluster_ctarank() : 0u;
+    const int unit = MC ? (int)blockIdx.x >> 1 : (int)blockIdx.x, nunits = MC ? (int)gridDim.x >> 1 : (int)gridDim.x;
+    auto item_tile = [&](int item, int &m_tile, int &n0) {
+        const int mi = item / n_tiles_n;
+        n0 = (item - mi * n_tiles_n) * BN;
+        m_tile = MC ? min(2 * mi + (int)crank, g.total_m_tiles - 1) : mi;
+    };
 
-    if (warp == 0 && lane == 0) {
-        ptx::prefetch_tensormap(&tmB);
-        ptx::prefetch_tensormap(&amaps.m[0]);
+    if (threadIdx.x == 0) {
         for (int s = 0; s < STAGES; ++s) {
             ptx::mbar_init(&full[s], 1);
-            ptx::mbar_init(&empty[s], 1);
-        }
-        for (int s = 0; s < 2; ++s) {
-            ptx::mbar_init(&tfull[s], 1);
-            ptx::mbar_init(&tempty[s], 4);
+            ptx::mbar_init(&empty[s], MC ? 16 : 8);    // one arrive per consumer warp (of both CTAs with MC)
         }
         ptx::fence_barrier_init();
     }
-    if (warp == 1) {
-        ptx::tmem_alloc(tmem_slot, tmem_cols);
-        ptx::tmem_relinquish();
-    }
-    ptx::tc_fence_before();
     __syncthreads();
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
+    if (MC) ptx::cluster_sync();                      // the peer's barriers exist before any remote arrive or multicast
 
-    if (warp == 0) {
+    if (warp == 8) {
         if (lane == 0) {
             int s = 0;
             uint32_t ph = 0;
-            for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-                const ConvItem ci = conv_item(g, item, n_tiles_n);
-                const int img = ci.m_tile / tiles_per_img;
-                const int trem = ci.m_tile - img * tiles_per_img;
+            for (int item = unit; item < g.n_items; item += nunits) {
+                int m_tile, n0;
+                item_tile(item, m_tile, n0);
+                const int img = m_tile / tiles_per_img;
+                const int trem = m_tile - img * tiles_per_img;
                 const int tyi = trem / g.tiles_x, txi = trem - tyi * g.tiles_x;
                 const int y0 = tyi * g.TH, x0 = txi * g.TW;
-                const CUtensorMap *bmap = ci.bn == g.BN ? &tmB : &tmB2;
-                const uint32_t tx_bytes = (uint32_t)(Cfg::A_BYTES + ci.bn * KC * 4);
                 for (int tap = 0; tap < g.taps; ++tap)
                     for (int cc = 0; cc < g.cin_chunks; ++cc) {
                         ptx::mbar_wait(&empty[s], ph ^ 1u);
-                        ptx::mbar_arrive_expect_tx(&full[s], tx_bytes);
-                        uint8_t *sa = smem + (size_t)s * stage_bytes;
-                        ptx::tma_load_4d(sa, &amaps.m[g.tap_map[tap]], &full[s], cc * KC, x0 + g.tap_ox[tap],
+                        ptx::mbar_arrive_expect_tx(&full[s], (uint32_t)STAGE_BYTES);
+                        uint8_t *sa = smem + (size_t)s * STAGE_BYTES;
+                        ptx::tma_load_4d(sa, &amaps.m[g.tap_map[tap]], &full[s], cc * CONV_KC, x0 + g.tap_ox[tap],
                                          y0 + g.tap_oy[tap], img);
-                        ptx::tma_load_2d(sa + Cfg::A_BYTES, bmap, &full[s], tap * g.cin_pad + cc * KC, ci.n0);
+                        if (MC)     // rows [crank*BN/2, +BN/2) of the weight tile, into both CTAs
+                            ptx::tma_load_2d_mc(sa + CONV_A_BYTES + crank * (B_BYTES / 2), &tmB, &full[s],
+                                                tap * g.cin_pad + cc * CONV_KC, n0 + (int)crank * (BN / 2), (uint16_t)0x3);
+                        else
+                            ptx::tma_load_2d(sa + CONV_A_BYTES, &tmB, &full[s], tap * g.cin_pad + cc * CONV_KC, n0);
                         if (++s == STAGES) {
                             s = 0;
                             ph ^= 1u;
@@ -394,112 +126,77 @@ __global__ void __launch_bounds__(CONV_THREADS, 2)
                     }
             }
         }
-    } else if (warp == 1) {
-        const uint64_t dbase = ptx::make_kmajor_desc(0, Cfg::SWIZZLE);
+    } else {
+        // consumer warpgroup wg: pixel rows [64 wg, 64 wg + 64) of the tile
+        const int wg = warp >> 2, wq = warp & 3;
+        const int g8 = lane >> 2, t4 = lane & 3;
         const uint32_t smem_u = ptx::smem_u32(smem);
+        auto release = [&](int st) {        // this warp is done reading stage st (in both CTAs' rings with MC)
+            ptx::mbar_arrive(&empty[st]);
+            if (MC) ptx::mbar_arrive_cluster(&empty[st], crank ^ 1u);
+        };
         int s = 0;
-        uint32_t ph = 0, it = 0;
-        for (int item = blockIdx.x; item < n_items; item += gridDim.x, ++it) {
-            const uint32_t as = it & 1u;
-            const uint32_t idesc = ptx::make_idesc_tf32(128, item < g.n_full ? g.BN : g.tail_bn);
-            ptx::mbar_wait(&tempty[as], ((it >> 1) & 1u) ^ 1u);
-            ptx::tc_fence_after();
-            const uint32_t tacc = tmem_base + as * (uint32_t)g.BN;
+        uint32_t ph = 0;
+        for (int item = unit; item < g.n_items; item += nunits) {
+            float acc[BN / 2];
+#pragma unroll
+            for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+            int prev = -1;
             for (int kb = 0; kb < nkb; ++kb) {
                 ptx::mbar_wait(&full[s], ph);
-                ptx::tc_fence_after();
-                const uint32_t sa = smem_u + (uint32_t)s * (uint32_t)stage_bytes;
-                const uint64_t adesc = dbase + (uint64_t)(sa >> 4);
-                const uint64_t bdesc = dbase + (uint64_t)((sa + Cfg::A_BYTES) >> 4);
-                if (ptx::elect_one()) {
+                const uint32_t sa = smem_u + (uint32_t)s * (uint32_t)STAGE_BYTES;
+                const uint64_t adesc = ptx::make_kmajor_desc(sa + (uint32_t)(wg * 64 * 128), 128);
+                const uint64_t bdesc = ptx::make_kmajor_desc(sa + (uint32_t)CONV_A_BYTES, 128);
+                ptx::wgmma_fence();
 #pragma unroll
-                    for (int k = 0; k < KC / 8; ++k)
-                        ptx::mma_tf32_ss(tacc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc,
-                                         (kb | k) != 0 ? 1u : 0u);
-                    ptx::mma_commit(&empty[s]);
-                }
-                __syncwarp();
+                for (int k = 0; k < CONV_KC / 8; ++k)   // 8 tf32 = 32 bytes along K: +2 in 16-byte units
+                    ptx::Wgmma<BN>::ss(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (kb | k) != 0 ? 1u : 0u);
+                ptx::wgmma_commit();
+                // the previous K-block's MMAs have finished reading their stage: hand it back
+                ptx::wgmma_wait<1>();
+                ptx::fence_regs(acc);
+                if (prev >= 0 && lane == 0) release(prev);
+                prev = s;
                 if (++s == STAGES) {
                     s = 0;
                     ph ^= 1u;
                 }
             }
-            if (ptx::elect_one()) ptx::mma_commit(&tfull[as]);
-            __syncwarp();
-        }
-    } else {
-        const int q = warp & 3;
-        const uint32_t stage_u = ptx::smem_u32(sOut) + (uint32_t)(q * 8192);
-        uint32_t it = 0, nstore = 0;
-        for (int item = blockIdx.x; item < n_items; item += gridDim.x, ++it) {
-            const uint32_t as = it & 1u;
-            const ConvItem ci = conv_item(g, item, n_tiles_n);
-            const int img = ci.m_tile / tiles_per_img;
-            const int trem = ci.m_tile - img * tiles_per_img;
+            ptx::wgmma_wait<0>();
+            ptx::fence_regs(acc);
+            if (lane == 0) release(prev);
+
+            int m_tile, n0;
+            item_tile(item, m_tile, n0);
+            const int img = m_tile / tiles_per_img;
+            const int trem = m_tile - img * tiles_per_img;
             const int tyi = trem / g.tiles_x, txi = trem - tyi * g.tiles_x;
-            const int n0 = ci.n0, bn = ci.bn;
-            // Residual: fetched COALESCED (load i of lane l = pixel 4i + l/8 of this warp, 16-byte
-            // chunk l%8: four full 128-byte lines per instruction) and handed to the pixel-owning lanes
-            // through this warp's rows of the staging tile; the first 32 channels are issued before
-            // waiting for the accumulator.
-            float4 rpre[8];
-            const float *rbase = nullptr;
-            if (res != nullptr) {
-                rbase = res + (((size_t)img * g.Ho + tyi * g.TH) * g.Wo + txi * g.TW) * g.res_cs + g.res_co + n0;
-                res_fetch8<16>(rpre, rbase, q, lane, tyi * g.TH, txi * g.TW, g.Ho, g.Wo, g.res_cs);
-            }
-            ptx::mbar_wait(&tfull[as], (it >> 1) & 1u);
-            ptx::tc_fence_after();
-            const uint32_t tacc = tmem_base + ((uint32_t)(q * 32) << 16) + as * (uint32_t)g.BN;
-            for (int c0 = 0; c0 < bn; c0 += 32) {
-                uint32_t r[32];
-                ptx::tmem_ld_32x32b_x32(tacc + (uint32_t)c0, r);
-                ptx::tmem_ld_wait();
-                if (c0 + 32 >= bn) {      // everything is in registers: give the TMEM stage back
-                    ptx::tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) ptx::mbar_arrive(&tempty[as]);
-                }
-                float v[32];
 #pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    const float4 bv = __ldg(reinterpret_cast<const float4 *>(bias + n0 + c0) + j);
-                    v[4 * j] = __uint_as_float(r[4 * j]) + bv.x;
-                    v[4 * j + 1] = __uint_as_float(r[4 * j + 1]) + bv.y;
-                    v[4 * j + 2] = __uint_as_float(r[4 * j + 2]) + bv.z;
-                    v[4 * j + 3] = __uint_as_float(r[4 * j + 3]) + bv.w;
+            for (int h = 0; h < 2; ++h) {
+                const int m = wg * 64 + wq * 16 + g8 + 8 * h;
+                const int y = tyi * g.TH + m / g.TW, x = txi * g.TW + m % g.TW;
+                if (y >= g.Ho || x >= g.Wo) continue;
+                const size_t pix = ((size_t)img * g.Ho + y) * g.Wo + x;
+                float *optr = out + pix * g.out_cs + g.out_co + n0;
+                const float *rptr = res ? res + pix * g.res_cs + g.res_co + n0 : nullptr;
+#pragma unroll
+                for (int j = 0; j < BN / 8; ++j) {
+                    const int c = 8 * j + 2 * t4;
+                    const float2 bv = __ldg(reinterpret_cast<const float2 *>(bias + n0 + c));
+                    float2 v = make_float2(acc[4 * j + 2 * h] + bv.x, acc[4 * j + 2 * h + 1] + bv.y);
+                    if (rptr) {
+                        const float2 rv = __ldg(reinterpret_cast<const float2 *>(rptr + c));
+                        v.x += rv.x;
+                        v.y += rv.y;
+                    }
+                    v.x = epi_act(v.x, g.act, g.round_out);
+                    v.y = epi_act(v.y, g.act, g.round_out);
+                    *reinterpret_cast<float2 *>(optr + c) = v;
                 }
-                // Stores go through shared memory and one TMA box per warp and 32 channels (a thread owns
-                // a pixel: direct 16-byte stores would hit 32 strided records per instruction); pixels
-                // outside the image are clipped by the TMA store.  Two buffers per warp: the store issued
-                // two chunks ago has left the one used now.
-                const uint32_t buf = stage_u + (nstore & 1u) * 4096u;
-                if (lane == 0) ptx::tma_store_wait_read1();
-                __syncwarp();
-                if (res != nullptr) {
-                    epi_add_residual(v, rpre, buf, lane);
-                    if (c0 + 32 < bn)
-                        res_fetch8<16>(rpre, rbase + c0 + 32, q, lane, tyi * g.TH, txi * g.TW, g.Ho, g.Wo, g.res_cs);
-                }
-                epi_activate(v, g.act, g.round_out);
-                epi_stage(v, buf, lane);
-                ptx::fence_proxy_async();
-                __syncwarp();
-                if (lane == 0) {
-                    ptx::tma_store_4d_u32(&tmO, buf, n0 + c0, txi * g.TW, tyi * g.TH + 2 * q, img);
-                    ptx::tma_store_commit();
-                }
-                ++nstore;
             }
         }
-        if (lane == 0) ptx::tma_store_wait_all();      // every issuing lane drains its own bulk groups
     }
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        ptx::tc_fence_after();
-        ptx::tmem_dealloc(tmem_base, tmem_cols);
-    }
+    if (MC) ptx::cluster_sync();                      // no CTA exits while its peer may still write into it
 }
 
 // ------------------------------------------------------------------ host side
@@ -556,21 +253,19 @@ int tma_encode(CUtensorMap *m, const void *base, int rank, const cuuint64_t *dim
 // long as the pointers and shapes stay the same).
 struct ConvPlan {
     AMaps amaps;
-    CUtensorMap tmB, tmB2, tmO;
+    CUtensorMap tmB;
     ConvGeom g;
-    int kc, mc, persist;
     dim3 grid;
     size_t smem;
+    int mc;
     const float *bias, *res;
     float *out;
 };
 
-// how 256-row weight tiles run: 0 single CTA (persistent kernel; default: measured 5.68 ms per
-// backbone step against 6.21 ms with mode 2); 1 CTA pairs, weight tile multicast into both;
-// 2 CTA pairs, one cta_group::2 MMA per k-step, each CTA holds half of the weight tile
+// 1: CTAs persistent over the items (grid = one CTA per SM); 0: one item per CTA (pvnet_conv_set_persistent)
+int g_conv_persist = 1;
+// 1: CTA pairs share each weight tile through TMA multicast (pvnet_conv_set_multicast; default 0)
 int g_conv_mc = 0;
-int g_conv_persist = 1;   // single-CTA tiles use the persistent kernel (pvnet_conv_set_persistent)
-int conv_kc(int) { return 32; }   // ragged last channel chunk: TMA zero-fills, weights are zero-padded
 
 int conv_plan(const ConvDesc &d, ConvPlan *p)
 {
@@ -587,12 +282,11 @@ int conv_plan(const ConvDesc &d, ConvPlan *p)
     PV_CHECK_ARG(((uintptr_t)d.in % 16 == 0) && ((uintptr_t)d.w % 16 == 0) && ((uintptr_t)d.out % 16 == 0) &&
                      ((uintptr_t)d.bias % 16 == 0),
                  "conv: pointers must be 16-byte aligned");
-    const int kc = conv_kc(d.Cin);
     PV_CHECK_ARG(d.Cin % 4 == 0, "conv: Cin %d must be a multiple of 4", d.Cin);
+    const int kc = CONV_KC;             // ragged last channel chunk: TMA zero-fills, weights are zero-padded
     ConvGeom &g = p->g;
     g.Ho = d.H / d.stride;
     g.Wo = d.W / d.stride;
-    // 128-pixel patch: wide for big maps (full 128-byte rows per warp), 8x16 otherwise
     g.TH = 8;
     g.TW = 16;
     g.tiles_x = (g.Wo + g.TW - 1) / g.TW;
@@ -602,18 +296,8 @@ int conv_plan(const ConvDesc &d, ConvPlan *p)
     g.cin_chunks = (d.Cin + kc - 1) / kc;
     g.cin_pad = g.cin_chunks * kc;
     g.Cout = d.Cout;
-    g.BN = d.Cout > 256 ? 256 : d.Cout;
-    // Small batches (the reference's own calling shape is batch 1: 38 M tiles at 60x80 for 148 SMs): narrower N
-    // tiles until every SM has an item -- MEASURED SLOWER and therefore off by default (batch 1, backbone + v3 as
-    // one CUDA graph: 0.80 ms with the wide tiles, 0.86 ms with N = 64/128 tiles): a 128x64 tile needs 24 KB of
-    // operands per 192 MMA cycles = 125 B/clk/SM, the L2->SM fill limit, on 152 SMs at once.
-    static const int env_small = [] {
-        const char *e = getenv("PVNET_CONV_SMALL_BATCH_SPLIT");     // tuning knob: 1 enables
-        return e ? atoi(e) : 0;
-    }();
-    if (env_small)
-        while (g.BN > 64 && (long long)g.total_m_tiles * (d.Cout / g.BN) < sm_count()) g.BN /= 2;
-    PV_CHECK_ARG(d.Cout % g.BN == 0, "conv: Cout %d not a multiple of the N tile %d", d.Cout, g.BN);
+    // N tile: 128 channels (64 fp32 accumulators per consumer thread) where Cout allows
+    g.BN = d.Cout % 128 == 0 ? 128 : (d.Cout % 64 == 0 ? 64 : 32);
     g.out_cs = d.out_cs;
     g.out_co = d.out_co;
     g.res_cs = d.res_cs;
@@ -636,7 +320,6 @@ int conv_plan(const ConvDesc &d, ConvPlan *p)
             g.tap_ox[t] = (short)((dx - px) / 2);
         }
     }
-    p->kc = kc;
     const int swz = kc * 4;
     // A: NHWC input (or its four parity planes for stride 2)
     const int nplanes = d.stride == 2 ? 4 : 1;
@@ -656,128 +339,61 @@ int conv_plan(const ConvDesc &d, ConvPlan *p)
     {
         cuuint64_t dims[2] = {(cuuint64_t)g.taps * g.cin_pad, (cuuint64_t)d.Cout};
         cuuint64_t strides[1] = {(cuuint64_t)g.taps * g.cin_pad * 4};
-        // pairs of CTAs multicast the weight tile when it is the 256-row one (g_conv_mc: test hook)
-        static const int env_mc = [] {
-            const char *e = getenv("PVNET_CONV_MC");       // tuning knob: overrides the default cluster mode
-            return e ? atoi(e) : -1;
-        }();
-        p->mc = g.BN == 256 ? (env_mc >= 0 ? env_mc : g_conv_mc) : 0;
-        cuuint32_t box[2] = {(cuuint32_t)kc, (cuuint32_t)(p->mc ? g.BN / 2 : g.BN)};
+        p->mc = g_conv_mc;
+        cuuint32_t box[2] = {(cuuint32_t)kc, (cuuint32_t)(p->mc ? g.BN / 2 : g.BN)};    // MC: each CTA loads half
         int rc = tma_encode(&p->tmB, d.w, 2, dims, strides, box, swz);
         if (rc) return rc;
     }
-    const int m_ctas = p->mc ? (g.total_m_tiles + 1) / 2 * 2 : g.total_m_tiles;
-    p->grid = dim3((unsigned)(m_ctas * (d.Cout / g.BN)));
-    p->smem = p->mc == 2 ? (size_t)(1024 + 6 * (ConvCfg<32>::A_BYTES + 128 * 32 * 4) + 256)
-                         : ConvCfg<32>::smem_bytes(g.BN);
-    // single-CTA tiles run on the persistent kernel: grid = resident CTAs
-    p->persist = (p->mc == 0 && g_conv_persist) ? 1 : 0;
-    p->tmO = p->tmB;
-    if (p->persist) {
-        // ring depth: 4 stages when two CTAs share the SM (BN <= 64), otherwise as many (<= 8) as fit
-        // next to the 32 KB of epilogue staging: BN=128 tiles need 128 B/clk/SM of L2->SM fill at full
-        // MMA rate, a deeper ring covers more of the L2 latency
-        const size_t stage_b = (size_t)ConvCfg<32>::A_BYTES + (size_t)g.BN * 32 * 4;
-        static const int env_stages = [] {
-            const char *e = getenv("PVNET_CONV_STAGES");        // tuning knob: 0 = auto
-            return e ? atoi(e) : 0;
-        }();
-        int st = 4;
-        if (g.BN > 64) {
-            st = (int)((227 * 1024 - 32768 - 2048) / stage_b);
-            if (st > 8) st = 8;
-            if (st < 4) st = 4;
-        }
-        if (env_stages >= 2 && env_stages <= 8 && 1024 + env_stages * stage_b + 256 + 32768 <= 227 * 1024) st = env_stages;
-        g.stages = st;
-        p->smem = 1024 + (size_t)st * stage_b + 256;
-        p->smem += 32768;                       // staging buffers of the TMA-store epilogue
-        cuuint64_t odims[4] = {(cuuint64_t)d.Cout, (cuuint64_t)g.Wo, (cuuint64_t)g.Ho, (cuuint64_t)d.b};
-        cuuint64_t ostr[3] = {(cuuint64_t)d.out_cs * 4, (cuuint64_t)g.Wo * d.out_cs * 4,
-                              (cuuint64_t)g.Ho * g.Wo * d.out_cs * 4};
-        cuuint32_t obox[4] = {32, (cuuint32_t)g.TW, (cuuint32_t)(32 / g.TW), 1};      // one epilogue warp: 32 pixels
-        int rc = tma_encode(&p->tmO, d.out + d.out_co, 4, odims, ostr, obox, 128);
-        if (rc) return rc;
-        int per_sm = (int)((227 * 1024) / p->smem);
-        if (per_sm > 2) per_sm = 2;
-        if (per_sm * 2 * g.BN > 512) per_sm = 512 / (2 * g.BN);      // TMEM: two accumulator stages per CTA
-        if (per_sm < 1) per_sm = 1;
-        const long long G = (long long)sm_count() * per_sm;
-        const long long items = (long long)g.total_m_tiles * (d.Cout / g.BN);
-        // Tail split.  The schedule is static round-robin, so `rem` leftover items would cost a whole
-        // extra round on `rem` CTAs while the others idle (600 items on 148 CTAs: 5 rounds for 4.05
-        // rounds of work).  Cut each leftover item into `split` channel slices: the last round then
-        // lasts floor(tail_bn)/floor(BN) of a full one (MMA issue floors in cycles per K=8 step,
-        // benchmarks/micro/mma_rate.cu: N=256 128, N=128 64, N=64 48, N=32 40).
-        const long long rem = items % G;
-        int split = 1;
-        static const int env_tail = [] {
-            const char *e = getenv("PVNET_CONV_TAIL_SPLIT");     // tuning knob: 0 disables the tail split
-            return e ? atoi(e) : 1;
-        }();
-        if (rem > 0 && env_tail) {
-            auto floor_cycles = [](int n) { return n >= 256 ? 128 : (n >= 128 ? 64 : (n >= 64 ? 48 : 40)); };
-            int best_cost = floor_cycles(g.BN);
-            for (int sp = 2; g.BN / sp >= 32 && rem * sp <= G; sp *= 2)
-                if (floor_cycles(g.BN / sp) < best_cost) {
-                    best_cost = floor_cycles(g.BN / sp);
-                    split = sp;
-                }
-        }
-        g.tail_split = split;
-        g.tail_bn = g.BN / split;
-        g.n_full = (int)(split > 1 ? items - rem : items);
-        g.n_items = (int)(g.n_full + (split > 1 ? rem * split : 0));
-        long long grid = G;
-        if (grid > g.n_items) grid = g.n_items;
-        p->grid = dim3((unsigned)grid);
-        p->tmB2 = p->tmB;
-        if (split > 1) {
-            cuuint64_t dims[2] = {(cuuint64_t)g.taps * g.cin_pad, (cuuint64_t)d.Cout};
-            cuuint64_t strides[1] = {(cuuint64_t)g.taps * g.cin_pad * 4};
-            cuuint32_t box[2] = {(cuuint32_t)kc, (cuuint32_t)g.tail_bn};
-            rc = tma_encode(&p->tmB2, d.w, 2, dims, strides, box, swz);
-            if (rc) return rc;
-        }
-    }
+    // ring: as many stages as fit (at most 8) in the 227 KB a block may use
+    const size_t stage_b = (size_t)CONV_A_BYTES + (size_t)g.BN * kc * 4;
+    int st = (int)((227 * 1024 - 1024 - 256) / stage_b);
+    if (st > 8) st = 8;
+    g.stages = st;
+    p->smem = 1024 + (size_t)st * stage_b + 256;
+    // items: (M tile, N tile), or with MC (M tile pair, N tile) run by a two-CTA cluster
+    const int m_units = p->mc ? (g.total_m_tiles + 1) / 2 : g.total_m_tiles;
+    g.n_items = m_units * (d.Cout / g.BN);
+    long long units = g_conv_persist ? (long long)sm_count() / (p->mc ? 2 : 1) : (long long)g.n_items;
+    if (units > g.n_items) units = g.n_items;
+    p->grid = dim3((unsigned)(units * (p->mc ? 2 : 1)));
     p->bias = d.bias;
     p->res = d.res;
     p->out = d.out;
     return PVNET_OK;
 }
 
+template <int BN, bool MC>
+int conv_launch_t(const ConvPlan &p, cudaStream_t s)
+{
+    const cudaError_t attr_err = ensure_max_smem((const void *)k_conv_tap<BN, MC>, 227 * 1024);
+    PV_CUDA(attr_err);
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = p.grid;
+    cfg.blockDim = dim3(CONV_THREADS);
+    cfg.dynamicSmemBytes = p.smem;
+    cfg.stream = s;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = MC ? 2 : 1;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = MC ? 1 : 0;
+    PV_CUDA(cudaLaunchKernelEx(&cfg, k_conv_tap<BN, MC>, p.amaps, p.tmB, p.g, p.bias, p.res, p.out));
+    PV_LAUNCHED("k_conv_tap");
+    return PVNET_OK;
+}
+
 int conv_launch(const ConvPlan &p, cudaStream_t s)
 {
-    const int max_smem = 227 * 1024;
-    const void *fn = p.mc == 2 ? (const void *)k_conv_tc<32, 2>
-                     : p.mc == 1 ? (const void *)k_conv_tc<32, 1>
-                     : p.persist ? (const void *)k_conv_tap_p<32> : (const void *)k_conv_tc<32, 0>;
-    const cudaError_t attr_err = ensure_max_smem(fn, max_smem);
-    PV_CUDA(attr_err);
     if (p.mc) {
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = p.grid;
-        cfg.blockDim = dim3(CONV_THREADS);
-        cfg.dynamicSmemBytes = p.smem;
-        cfg.stream = s;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = 2;
-        attr[0].val.clusterDim.y = 1;
-        attr[0].val.clusterDim.z = 1;
-        cfg.attrs = attr;
-        cfg.numAttrs = 1;
-        if (p.mc == 2)
-            PV_CUDA(cudaLaunchKernelEx(&cfg, k_conv_tc<32, 2>, p.amaps, p.tmB, p.g, p.bias, p.res, p.out));
-        else
-            PV_CUDA(cudaLaunchKernelEx(&cfg, k_conv_tc<32, 1>, p.amaps, p.tmB, p.g, p.bias, p.res, p.out));
-    } else if (p.persist) {
-        k_conv_tap_p<32><<<p.grid, CONV_THREADS, p.smem, s>>>(p.amaps, p.tmB, p.tmB2, p.tmO, p.g, p.bias, p.res, p.out);
-    } else {
-        k_conv_tc<32, 0><<<p.grid, CONV_THREADS, p.smem, s>>>(p.amaps, p.tmB, p.g, p.bias, p.res, p.out);
+        if (p.g.BN == 128) return conv_launch_t<128, true>(p, s);
+        if (p.g.BN == 64) return conv_launch_t<64, true>(p, s);
+        return conv_launch_t<32, true>(p, s);
     }
-    PV_LAUNCHED("k_conv_tc");
-    return PVNET_OK;
+    if (p.g.BN == 128) return conv_launch_t<128, false>(p, s);
+    if (p.g.BN == 64) return conv_launch_t<64, false>(p, s);
+    return conv_launch_t<32, false>(p, s);
 }
 
 size_t conv_plan_size() { return sizeof(ConvPlan); }
@@ -788,15 +404,16 @@ int conv_launch_at(const void *storage, cudaStream_t s) { return conv_launch(*st
 
 extern "C" {
 
-int pvnet_conv_set_persistent(int on)
+int pvnet_conv_set_multicast(int on)
 {
-    pvnet::g_conv_persist = on ? 1 : 0;
+    PV_CHECK_ARG(on == 0 || on == 1, "multicast mode must be 0 or 1");
+    pvnet::g_conv_mc = on;
     return PVNET_OK;
 }
 
-int pvnet_conv_set_multicast(int on)
+int pvnet_conv_set_persistent(int on)
 {
-    pvnet::g_conv_mc = on < 0 ? 0 : (on > 2 ? 2 : on);
+    pvnet::g_conv_persist = on ? 1 : 0;
     return PVNET_OK;
 }
 

@@ -32,7 +32,6 @@ struct ConvDesc {
     // half-resolution tensor up_src [b,H/2,W/2,Cin], interpolated inside the kernel straight into the
     // operand stages (model_repository.py:75: the upsampled tensor is never written)
     const float *up_src = nullptr;
-    int up_mode = 1;   // 1: interpolated by the epilogue warps (two CTAs per SM); 2: by eight dedicated warps (one CTA per SM)
 };
 
 // Optional fused 1x1 head (convraw.3 + argmax) for the column kernel's epilogue.
@@ -80,81 +79,13 @@ __device__ __forceinline__ float lerp3(float w0, float a, float w1, float b, flo
 {
     return __fmaf_rn(w2, c, __fmaf_rn(w1, b, __fmul_rn(w0, a)));
 }
-// Coalesced residual fetch shared by the conv epilogues (128-pixel tiles TW pixels wide, one pixel
-// per thread, epilogue warp q owns tile rows q*32/TW ...).  Load i of lane l reads the 16-byte chunk
-// (l % 8) of warp-pixel 4*i + l/8, i.e. four full 128-byte lines per instruction instead of 32
-// strided sectors.  `base` points at (tile origin, first channel of the 32-channel group);
-// out-of-image pixels read nothing.
-template <int TW>
-__device__ __forceinline__ void res_fetch8(float4 (&dst)[8], const float *base, int q, int lane, int y0, int x0,
-                                           int Ho, int Wo, int res_cs)
+// Epilogue element shared by the conv kernels: activation, then optional rounding to tf32 (the value
+// feeds another tensor-core conv).
+__device__ __forceinline__ float epi_act(float v, int act, int round_out)
 {
-    static_assert(TW == 8 || TW == 16, "tile width");
-    constexpr int ROWS = 32 / TW;                       // tile rows per warp
-    const int yy = y0 + ROWS * q, xx = x0 + (lane >> 3);
-    const float *p = base + ((size_t)(ROWS * q) * Wo + (lane >> 3)) * res_cs + (lane & 7) * 4;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-        const int dy = (4 * i) / TW, dx = (4 * i) % TW;
-        dst[i] = (yy + dy < Ho && xx + dx < Wo)
-                     ? __ldg(reinterpret_cast<const float4 *>(p + ((size_t)dy * Wo + dx) * res_cs))
-                     : make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-}
-// Epilogue tail shared by the conv kernels: v[32] (one pixel, 32 channels, bias already added)
-// -> (+ residual) -> activation -> optional tf32 rounding -> this warp's 32 rows of a 128-byte-
-// swizzled staging buffer -> ONE TMA box per warp (32 channels x 32 pixels).  Each epilogue warp owns
-// two 4 KB buffers and its own bulk-store groups, so no CTA-wide barrier is needed: lane 0 waits
-// until the store issued two chunks ago has finished reading its buffer, the warp writes, fences the
-// async proxy and lane 0 issues the next store.  `buf` is the shared-space address of the buffer to
-// use now; row r of it holds pixel r of the warp, 16-byte chunk j at position j ^ (r & 7).
-template <int ACT, bool ROUND>
-__device__ __forceinline__ void epi_activate(float (&v)[32])
-{
-#pragma unroll
-    for (int j = 0; j < 32; ++j) {
-        if (ACT == 1) v[j] = fmaxf(v[j], 0.f);
-        if (ACT == 2) v[j] = fmaxf(v[j], 0.1f * v[j]);      // LeakyReLU(0.1): max(x, 0.1x)
-        if (ROUND) v[j] = ptx::round_tf32(v[j]);
-    }
-}
-__device__ __forceinline__ void epi_activate(float (&v)[32], int act, int round_out)
-{
-    // one warp-uniform branch per chunk instead of per-element predicates
-    if (round_out) {
-        if (act == 1) epi_activate<1, true>(v);
-        else if (act == 2) epi_activate<2, true>(v);
-        else epi_activate<0, true>(v);
-    } else {
-        if (act == 1) epi_activate<1, false>(v);
-        else if (act == 2) epi_activate<2, false>(v);
-    }
-}
-// residual: rpre (coalesced fetch layout, see res_fetch8) -> rows of `buf` -> added to the owning lane's v
-__device__ __forceinline__ void epi_add_residual(float (&v)[32], const float4 (&rpre)[8], uint32_t buf, int lane)
-{
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-        const int row = i * 4 + (lane >> 3);
-        ptx::sts128(buf + (uint32_t)(row * 128 + (((lane & 7) ^ (row & 7)) << 4)), rpre[i]);
-    }
-    __syncwarp();
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-        const float4 rv = ptx::lds128(buf + (uint32_t)(lane * 128 + ((j ^ (lane & 7)) << 4)));
-        v[4 * j] += rv.x;
-        v[4 * j + 1] += rv.y;
-        v[4 * j + 2] += rv.z;
-        v[4 * j + 3] += rv.w;
-    }
-    __syncwarp();
-}
-__device__ __forceinline__ void epi_stage(const float (&v)[32], uint32_t buf, int lane)
-{
-#pragma unroll
-    for (int j = 0; j < 8; ++j)
-        ptx::sts128(buf + (uint32_t)(lane * 128 + ((j ^ (lane & 7)) << 4)),
-               make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]));
+    if (act == 1) v = fmaxf(v, 0.f);
+    else if (act == 2) v = fmaxf(v, 0.1f * v);       // LeakyReLU(0.1): max(x, 0.1x)
+    return round_out ? ptx::round_tf32(v) : v;
 }
 #endif
 

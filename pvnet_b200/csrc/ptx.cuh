@@ -1,5 +1,5 @@
-// ptx.cuh -- thin inline-PTX wrappers for the sm_100a features the conv path uses:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld), fences.
+// ptx.cuh -- thin inline-PTX wrappers for the sm_90a features the conv path uses:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma (warpgroup MMA, tf32 in / fp32 accumulate), fences.
 #pragma once
 #include <cstdint>
 #include <cuda.h>
@@ -127,44 +127,6 @@ __device__ __forceinline__ void named_bar_sync(int id, int nthreads)
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
-// multicast variant: the box lands at the same shared-memory offset of every CTA in cta_mask and
-// completes tx bytes on the mbarrier at the same offset in each of them
-__device__ __forceinline__ void tma_load_2d_mc(void *smem_dst, const CUtensorMap *m, uint64_t *bar, int c0, int c1,
-                                               uint16_t cta_mask)
-{
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
-        " [%0], [%1, {%4, %5}], [%2], %3;"
-        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "h"(cta_mask), "r"(c0),
-        "r"(c1)
-        : "memory");
-}
-
-// cta_group::2 variants: issued by BOTH CTAs of a pair, each into its own shared memory; the
-// transaction bytes are counted on the LEADER CTA's mbarrier (peer bit 24 of the shared::cluster
-// address cleared), because only the leader issues the 2-SM MMA.
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;
-__device__ __forceinline__ void tma_load_4d_2sm(void *smem_dst, const CUtensorMap *m, uint64_t *leader_bar, int c0,
-                                                int c1, int c2, int c3)
-{
-    asm volatile(
-        "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-        " [%0], [%1, {%3, %4, %5, %6}], [%2];"
-        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(leader_bar) & kPeerBitMask),
-        "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-        : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_2sm(void *smem_dst, const CUtensorMap *m, uint64_t *leader_bar, int c0,
-                                                int c1)
-{
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-        " [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(leader_bar) & kPeerBitMask),
-        "r"(c0), "r"(c1)
-        : "memory");
-}
-
 // ---------------------------------------------------------------- clusters
 __device__ __forceinline__ uint32_t cluster_ctarank()
 {
@@ -176,140 +138,112 @@ __device__ __forceinline__ void cluster_sync()
 {
     asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
+// arrive on the mbarrier at the same shared-memory offset in CTA `rank` of the cluster
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t *bar, uint32_t rank)
+{
+    asm volatile(
+        "{\n\t.reg .b32 ra;\n\tmapa.shared::cluster.u32 ra, %0, %1;\n\t"
+        "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}" ::"r"(smem_u32(bar)), "r"(rank)
+        : "memory");
+}
+// TMA load multicast: the box lands at the same shared-memory offset of every CTA in cta_mask and
+// completes its bytes on the mbarrier at the same offset in each of them
+__device__ __forceinline__ void tma_load_2d_mc(void *smem_dst, const CUtensorMap *m, uint64_t *bar, int c0, int c1,
+                                               uint16_t cta_mask)
+{
+    asm volatile(
+        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+        " [%0], [%1, {%4, %5}], [%2], %3;"
+        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "h"(cta_mask), "r"(c0),
+        "r"(c1)
+        : "memory");
+}
 
-// ---------------------------------------------------------------- tcgen05
-__device__ __forceinline__ void tmem_alloc(uint32_t *smem_result, uint32_t ncols)
+// ---------------------------------------------------------------- wgmma
+// The four warps of a warpgroup issue one MMA together: D[64 x N] (fp32, registers) (+)= A[64 x 8] * B[N x 8]^T,
+// tf32 operands, both K-major.  A comes from a shared-memory descriptor or from registers (thread layout of
+// mma.m16n8k8 per warp: a0 (row g, k t), a1 (row g+8, k t), a2 (row g, k t+4), a3 (row g+8, k t+4), g = lane/4,
+// t = lane%4, warp w of the group owning rows 16w..16w+15).  D: for each 8-column block j, d[4j] (row g, col
+// 8j+2t), d[4j+1] (row g, col 8j+2t+1), d[4j+2] (row g+8, col 8j+2t), d[4j+3] (row g+8, col 8j+2t+1).
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads/writes across an MMA that is still in flight
+template <int R>
+__device__ __forceinline__ void fence_regs(float (&d)[R])
 {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-                 "r"(ncols)
-                 : "memory");
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_relinquish()
-{
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols)
-{
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before()
-{
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after()
-{
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]^T, tf32 inputs, fp32 accumulate, one CTA
-__device__ __forceinline__ void mma_tf32_ss(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                            uint32_t accumulate)
-{
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// mbarrier arrives once every tcgen05.mma issued so far by this thread has completed
-__device__ __forceinline__ void mma_commit(uint64_t *bar)
-{
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-// same, arriving on the barrier at this offset in every CTA of cta_mask
-__device__ __forceinline__ void mma_commit_mc(uint64_t *bar, uint16_t cta_mask)
-{
-    asm volatile(
-        "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-        ::"r"(smem_u32(bar)), "h"(cta_mask)
-        : "memory");
-}
-// ---- cta_group::2: one MMA spans a CTA pair (M = 2 x 128 rows, each CTA holds half of A's rows,
-// half of B's rows, and its own 128 lanes of D)
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t *smem_result, uint32_t ncols)
-{
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-                 "r"(ncols)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_2sm()
-{
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t ncols)
-{
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void mma_tf32_ss_2sm(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                                uint32_t accumulate)
-{
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void mma_commit_2sm_mc(uint64_t *bar, uint16_t cta_mask)
-{
-    asm volatile(
-        "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-        ::"r"(smem_u32(bar)), "h"(cta_mask)
-        : "memory");
-}
-// A operand from TMEM (128 lanes x 8 fp32 columns per k-step), B from shared memory
-__device__ __forceinline__ void mma_tf32_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc,
-                                            uint32_t accumulate)
-{
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// registers -> TMEM, 32 lanes x 32 columns (the mirror of tmem_ld_32x32b_x32)
-__device__ __forceinline__ void tmem_st_32x32b_x32(uint32_t taddr, const uint32_t (&r)[32])
-{
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-        "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-        "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-        "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]),
-        "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]),
-        "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait()
-{
-    asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
-// 32 lanes x 32 consecutive fp32 columns: thread i of the warp gets lane (base_lane+i)
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32])
-{
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait()
-{
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
+
+template <int N>
+struct Wgmma;
+template <>
+struct Wgmma<32> {
+    // D[64 x 32] (+)= A[smem desc] * B[smem desc]^T
+    __device__ __forceinline__ static void ss(float (&d)[16], uint64_t adesc, uint64_t bdesc, uint32_t accumulate)
+    {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1;\n\t}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+            : "l"(adesc), "l"(bdesc), "r"(accumulate));
+    }
+    // D[64 x 32] (+)= A[registers] * B[smem desc]^T
+    __device__ __forceinline__ static void rs(float (&d)[16], const uint32_t (&a)[4], uint64_t bdesc, uint32_t accumulate)
+    {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1;\n\t}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
+    }
+};
+
+template <>
+struct Wgmma<64> {
+    // D[64 x 64] (+)= A[smem desc] * B[smem desc]^T
+    __device__ __forceinline__ static void ss(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accumulate)
+    {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+            : "l"(adesc), "l"(bdesc), "r"(accumulate));
+    }
+    // D[64 x 64] (+)= A[registers] * B[smem desc]^T
+    __device__ __forceinline__ static void rs(float (&d)[32], const uint32_t (&a)[4], uint64_t bdesc, uint32_t accumulate)
+    {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1;\n\t}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
+    }
+};
+
+template <>
+struct Wgmma<128> {
+    // D[64 x 128] (+)= A[smem desc] * B[smem desc]^T
+    __device__ __forceinline__ static void ss(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate)
+    {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+            : "l"(adesc), "l"(bdesc), "r"(accumulate));
+    }
+    // D[64 x 128] (+)= A[registers] * B[smem desc]^T
+    __device__ __forceinline__ static void rs(float (&d)[64], const uint32_t (&a)[4], uint64_t bdesc, uint32_t accumulate)
+    {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1;\n\t}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
+    }
+};
 
 // fp32 -> tf32, round to nearest (ties away), result in an fp32 container
 __device__ __forceinline__ float round_tf32(float x)
@@ -319,20 +253,23 @@ __device__ __forceinline__ float round_tf32(float x)
     return __uint_as_float(r);
 }
 
+
 // ---------------------------------------------------------------- descriptors
-// K-major shared-memory operand descriptor (cute::UMMA::SmemDescriptor bit layout):
-//   [0,14) start>>4, [16,30) LBO>>4, [32,46) SBO>>4, [46,48) version=1, [61,64) swizzle mode
-// swizzle_bytes in {128, 64, 32}: rows are swizzle_bytes wide, 8-row atoms, SBO = 8*swizzle_bytes.
+// K-major shared-memory operand descriptor of wgmma: [0,14) start>>4, [16,30) LBO>>4 (unused by the swizzled
+// K-major layouts), [32,46) SBO>>4 = distance of 8-row groups, [62,64) layout: 1 = 128-byte, 2 = 64-byte,
+// 3 = 32-byte swizzle.  Rows are swizzle_bytes wide (what TMA wrote with the same swizzle), so SBO = 8 rows.
+// Tiles start on a swizzle-repeat boundary (base offset 0); stepping along K inside a row adds to the start.
 __device__ __forceinline__ uint64_t make_kmajor_desc(uint32_t smem_addr, uint32_t swizzle_bytes)
 {
-    const uint64_t layout = swizzle_bytes == 128 ? 2ull : (swizzle_bytes == 64 ? 4ull : 6ull);
+    const uint64_t layout = swizzle_bytes == 128 ? 1ull : (swizzle_bytes == 64 ? 2ull : 3ull);
     const uint64_t sbo = (8ull * swizzle_bytes) >> 4;
-    return (uint64_t)((smem_addr & 0x3ffff) >> 4) | (1ull << 16) | (sbo << 32) | (1ull << 46) | (layout << 61);
+    return (uint64_t)((smem_addr & 0x3ffff) >> 4) | (1ull << 16) | (sbo << 32) | (layout << 62);
 }
-// tf32 x tf32 -> f32, both operands K-major, M x N tile (cute::UMMA::InstrDescriptor)
-__host__ __device__ constexpr uint32_t make_idesc_tf32(int m, int n)
+// byte offset -> swizzled byte offset inside a tile of swizzle_bytes-wide rows (the pattern TMA writes:
+// 16-byte chunk bits [4, 4+log2(swizzle_bytes/16)) XOR the same number of bits from bit 7 up)
+__device__ __forceinline__ uint32_t swizzle_off(uint32_t off, uint32_t swizzle_bytes)
 {
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
+    return off ^ ((off >> 3) & (swizzle_bytes - 16u));
 }
 
 }  // namespace ptx

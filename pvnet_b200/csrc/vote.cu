@@ -1,4 +1,4 @@
-// vote.cu -- PVNet RANSAC voting layer for B200 (sm_100a).
+// vote.cu -- PVNet RANSAC voting layer for H100 (sm_90a).
 //
 // What the reference does per image (lib/ransac_voting_gpu_layer/ransac_voting_gpu.py:514-598):
 // torch.nonzero / masked_select compaction, generate_hypothesis kernel, a u8
@@ -30,7 +30,7 @@
 // |theta| < theta_T (cos theta_T = thresh), i.e.
 //     m = |d| sin(theta_T - |theta|) = sin(theta_T) (d.u) - cos(theta_T) |d.v| > 0,
 // u = n/|n|, v = (-u_y, u_x): two linear functionals of the hypothesis per pixel.  k_vote3
-// evaluates them in segment-centred coordinates (4 FMA as 2 FFMA2), -m (1 FADD), counts its sign bit and tracks
+// evaluates them in segment-centred coordinates (4 FMA), -m (1 FADD), counts its sign bit and tracks
 // min |m| against a per-hypothesis guard band B (DESIGN.md section 3 bounds both the reference's rounding,
 // <= (7 + 1/T) ulp on the cosine, and ours): m > B counts, |m| <= B (or NaN) is re-decided by
 // exact_inlier(), the reference's own instruction sequence.  Tests outside the band cannot
@@ -61,7 +61,7 @@ struct Strides {
 };
 
 // ------------------------------------------------------------------ exact sequences
-// src/ransac_voting_kernel.cu:107-125 as nvcc compiles it for sm_100a (SASS checked):
+// src/ransac_voting_kernel.cu:107-125 as nvcc compiles it (SASS checked):
 // intrinsics pin every rounding so this compiler cannot contract differently.
 __device__ __forceinline__ bool exact_inlier(float nx, float ny, float cx, float cy, float hx, float hy,
                                              float thresh)
@@ -77,7 +77,7 @@ __device__ __forceinline__ bool exact_inlier(float nx, float ny, float cx, float
     return ang > thresh;
 }
 
-// src/ransac_voting_kernel.cu:28-48 (SASS-derived contraction, DESIGN.md "FP sequence")
+// src/ransac_voting_kernel.cu:28-48 (contraction read off the SASS of the sm_90a build, DESIGN.md "FP sequence")
 __device__ __forceinline__ float2 exact_hypothesis(float d0x, float d0y, float cx0, float cy0, float d1x,
                                                    float d1y, float cx1, float cy1)
 {
@@ -90,7 +90,7 @@ __device__ __forceinline__ float2 exact_hypothesis(float d0x, float d0y, float c
     const float s1 = __fmaf_rn(d1y, cx1, -__fmul_rn(d1x, cy1));
     const float s0 = __fmaf_rn(d0y, cx0, -__fmul_rn(d0x, cy0));
     const float y = __fdiv_rn(__fmaf_rn(d1y, s0, -__fmul_rn(d0y, s1)), det_y);
-    const float x = __fdiv_rn(__fmaf_rn(d0x, s1, -__fmul_rn(d1x, s0)), det_x);
+    const float x = __fdiv_rn(__fmaf_rn(-d1x, s0, __fmul_rn(d0x, s1)), det_x);
     return make_float2(x, y);
 }
 
@@ -550,29 +550,17 @@ __global__ void __launch_bounds__(VT_THREADS, HPL > 4 ? 2 : 4)
 // B = beta (|hx'| + |hy'| + r1) + b0 per hypothesis and segment (|d| <= |h'|_1 + r1): beta carries the
 // reference's rounding band (7 + 1/T) ulp T / sin(theta_T) and ours, see DESIGN.md section 3.
 //
-// Instruction mix (profiles/r02_micro_vote_mix.txt: every step below is a measured row):
-//   * two hypotheses ride in one FFMA2 (fma.rn.f32x2): half the issue slots of 4 FFMA; the pixel operands are
-//     stored pre-duplicated so a pair comes straight out of LDS.128;
+// Instruction mix:
+//   * two hypotheses are kept as a pair (f32x2) so a pair of pixel operands comes straight out of one LDS.128
+//     (the pixel operands are stored pre-duplicated); sm_90a evaluates the pair as two lane-wise FFMA;
 //   * the FAST decision is the sign bit of  e = |perp| - num = -m  (one FADD), added to an integer count by ONE
 //     ALU-pipe instruction (LEA.HI cnt, e, cnt, RZ, 1  =  cnt + (e >> 31)); a NaN e is the canonical positive NaN:
-//     not counted.  (Before: cnt += fma.sat(m, 2^64, -B 2^64), two more FMA-pipe cycles per test -- the FMA pipe is
-//     the busy one: 7 -> 5 cycles per test, config-4 layer 3.72 -> 3.46 ms.)
-//   * the guard band is NOT tested per test (one FSETP.OR per test made a serial predicate chain and a branch per
-//     pixel group: 8.7 vs 8.0 cycles per 32 tests in the microbenchmark at our 4 warps per sub-partition, and
-//     4.57 vs 3.96 ms on the config-4 layer): every hypothesis keeps  mab = min over the sub-chunk of |e|  -- one
-//     FMNMX3.NAN with |.| operand modifiers per TWO tests, ALU pipe -- compared with B once per 64 pixels.  A
-//     hypothesis with !(mab > B) is re-walked by the whole warp (2 pixels per lane, the same fma chains bit for bit)
-//     and exactly its in-band tests get exact_inlier() on the raw values; one RED adds  exact - fast.
-//     Outside the band sign(m) IS the reference's decision (that is what B bounds), inside it is corrected: the
-//     counts are the reference's.
-// Per test: 2 FFMA2 + FADD + LEA.HI + 1/2 FMNMX3 = 4.5 issue slots (5.0 with LDS and loop: 160 instructions per
-// 4 pixels x 8 hypotheses), 5 FMA-pipe cycles, no branch inside a sub-chunk.
-// Measured and rejected on the way (config-4 layer, ms, planted / random field; with the fma.sat count unless
-// noted): staging the cone EDGES so that m = min(m+, m-) is an FMNMX (4.24 / 4.06); two 2-input FMNMX instead of the
-// FMNMX3 (4.18 / 4.09); packed FADD2 count adds (3.69 / 3.63 at best, within 1 % of 3.72 / 3.66); HPL = 4 with 3 CTAs
-// per SM (4.24 / 4.17; with the sign-bit count 3.95 / 3.89 against 3.46 / 3.40); queueing the in-band tests so that one
-// exact_inlier() pass serves 32 of them (3.46 / 3.42: no gain, other warps already hide that path); source-level
-// software pipelining of the ALU ops against the next pair's FFMA2 (microbenchmark rows 18, 19: ptxas re-clusters).
+//     not counted;
+//   * the guard band is NOT tested per test: every hypothesis keeps  mab = min over the sub-chunk of |e|  (NaN-
+//     propagating min with |.| operands), compared with B once per 64 pixels.  A hypothesis with !(mab > B) is
+//     re-walked by the whole warp (2 pixels per lane, the same fma chains bit for bit) and exactly its in-band tests
+//     get exact_inlier() on the raw values; one RED adds  exact - fast.  Outside the band sign(m) IS the reference's
+//     decision (that is what B bounds), inside it is corrected: the counts are the reference's.
 typedef unsigned long long f32x2;
 __device__ __forceinline__ f32x2 pk2(float a, float b)
 {
@@ -584,11 +572,14 @@ __device__ __forceinline__ void upk2(f32x2 v, float &a, float &b)
 {
     asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v));
 }
+// two lane-wise fma.rn (sm_90a has no packed fp32 FMA; the results are the same bits)
 __device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c)
 {
-    f32x2 r;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-    return r;
+    float a0, a1, b0, b1, c0, c1;
+    upk2(a, a0, a1);
+    upk2(b, b0, b1);
+    upk2(c, c0, c1);
+    return pk2(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
 }
 __device__ __forceinline__ void lds_2x64(uint32_t addr, f32x2 &a, f32x2 &b)
 {
@@ -599,7 +590,7 @@ constexpr int VT_SUB = 64;        // pixels per staged sub-chunk (2 per lane)
 __device__ __forceinline__ float min3_nan_abs(float a, float b, float c)     // min(a, |b|, |c|), NaN if any is
 {
     float r;
-    asm("min.NaN.f32 %0, %1, %2, %3;" : "=f"(r) : "f"(a), "f"(fabsf(b)), "f"(fabsf(c)));
+    asm("{\n\t.reg .f32 t;\n\tmin.NaN.f32 t, %1, %2;\n\tmin.NaN.f32 %0, t, %3;\n\t}" : "=f"(r) : "f"(a), "f"(fabsf(b)), "f"(fabsf(c)));
     return r;
 }
 
@@ -1263,7 +1254,7 @@ __global__ void __launch_bounds__(256)
 // 1:1 stand-ins for generate_hypothesis_vanishing_point / voting_for_hypothesis_vanishing_point
 // (src/ransac_voting_kernel.cu:170-230, :263-305): homogeneous intersections [hn,vn,3] of the two pixels'
 // lines and the |cos| test against them.  Rounding sequence read off the SASS nvcc 12.9 emits for the
-// reference file (sm_100a, default -fmad): every fma below is one the compiler contracted, every
+// reference file (default -fmad): every fma below is one the compiler contracted, every
 // __fmul_rn a product it kept separate because the value is used twice.
 __device__ __forceinline__ void exact_vp_hypothesis(float dx0, float dy0, float cx0, float cy0, float dx1, float dy1,
                                                     float cx1, float cy1, float &ox, float &oy, float &oz)

@@ -1,6 +1,6 @@
 """`Resnet18_8s` with the reference's constructor, forward signature and state-dict keys
 (zju3dv/pvnet lib/networks/model_repository.py:7-80), backed in eval mode by the native
-sm_100a backbone (tcgen05 implicit-GEMM convs behind include/pvnet_b200.h).
+sm_90a backbone (wgmma implicit-GEMM convs behind include/pvnet_b200.h).
 
     net = Resnet18_8s(ver_dim=18, seg_dim=2)
     net.load_state_dict(ckpt['net'])          # reference checkpoints load unchanged
@@ -9,9 +9,9 @@ sm_100a backbone (tcgen05 implicit-GEMM convs behind include/pvnet_b200.h).
 
 * eval mode on CUDA -> `pvnet_backbone_forward`: BatchNorm folded into TF32 conv weights
   (the reference's cuDNN path also runs TF32 on this hardware: torch's
-  `cudnn.allow_tf32` default), fp32 accumulation.  Every convolution runs on tcgen05 with TF32
+  `cudnn.allow_tf32` default), fp32 accumulation.  Every convolution runs on wgmma with TF32
   operands: the 7x7/2 stem as a 4x4 conv over the 2x2 space-to-depth image, and convraw.3 (1x1 +
-  bias) as a TS-mode MMA inside convraw.0's epilogue, fused with torch.argmax over the
+  bias) as a register-A wgmma inside convraw.0's epilogue, fused with torch.argmax over the
   segmentation logits (head weights are rounded to TF32; the fp32 `k_head`/`k_stem` kernels remain as
   the `pvnet_conv_set_mode(1)` test path).  There is no PyTorch fallback in this mode: if the library
   is missing it raises.
@@ -157,9 +157,8 @@ class Resnet18_8s(nn.Module):
 
     def set_fused_upsample(self, on=None):
         """A/B switch of the 1/2 -> 1 upsampling inside convraw.0's loader (pvnet_backbone_set_fused_upsample):
-        None = library default, False / 0 = separate k_upsample2x launch, True / 1 = fused on the epilogue warps,
-        2 = fused on dedicated interpolation warps."""
-        self._nat.fuse_up = -1 if on is None else (2 if on == 2 else int(bool(on)))
+        None = library default, False / 0 = separate k_upsample2x launch, True / nonzero = fused."""
+        self._nat.fuse_up = -1 if on is None else int(bool(on))
         return self
 
     def _sync_options(self, dev):

@@ -1,4 +1,4 @@
-"""Host side of the B200 voting layer: the reference's Python API over libpvnet_b200.so.
+"""Host side of the H100 voting layer: the reference's Python API over libpvnet_b200.so.
 
 Same names, argument meaning and defaults as zju3dv/pvnet's
 ``lib/ransac_voting_gpu_layer/ransac_voting_gpu.py`` for the functions on the
@@ -19,7 +19,7 @@ inference hot path:
 so ``tools/demo.py`` / ``tools/train_linemod.py --test_model`` keep working when
 ``lib/ransac_voting_gpu_layer/ransac_voting_gpu.py`` is this module (the shim under
 ``lib/`` re-exports it).  Tensors in, tensors out; the work happens in hand-written
-sm_100a kernels behind the C ABI of ``include/pvnet_b200.h``.  There is no CPU or
+sm_90a kernels behind the C ABI of ``include/pvnet_b200.h``.  There is no CPU or
 PyTorch fallback: without the library or a CUDA device these functions raise.
 
 Randomness (``rng=``):

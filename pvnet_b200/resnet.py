@@ -9,7 +9,7 @@ maps the reference returns (:220).  Module/parameter names match the reference s
 checkpoints load with ``load_state_dict`` (SURVEY.md §8b "Weights").
 
 This PyTorch graph is what train mode (BatchNorm batch statistics, autograd) runs;
-eval-mode inference goes through the native sm_100a path in
+eval-mode inference goes through the native sm_90a path in
 ``pvnet_b200.model_repository.Resnet18_8s``.
 """
 from __future__ import annotations

@@ -1,8 +1,8 @@
-"""Regenerates tests/golden/*.npz.  Run in the authoring container, where
-/root/reference exists:   python tests/golden/make_golden.py
+"""Regenerates tests/golden/*.npz.  Run with PVNET_REFERENCE naming a checkout of
+the reference project:   PVNET_REFERENCE=<path> python tests/golden/make_golden.py
 
 demo_cat.npz -- the reference's only usable known-answer fixture (SURVEY.md §4,
-App. E).  From /root/reference/data/demo (cat_mask.png, cat_points_3d.txt,
+App. E).  From <reference>/data/demo (cat_mask.png, cat_points_3d.txt,
 cat_pose.npy) and the LINEMOD intrinsics of lib/utils/base_utils.py:240-243 it
 derives, exactly as tools/demo.py:58-71,74-88 (`compute_vertex`, `read_data`) do:
   fg_yx      [2289,2] int16   foreground pixel coordinates (row-major order)
@@ -20,6 +20,9 @@ import sys
 
 import numpy as np
 
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
+from tests.helpers import reference_root  # noqa: E402
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
@@ -27,7 +30,7 @@ sys.path.insert(0, ROOT)
 
 def make_demo():
     import cv2
-    demo = "/root/reference/data/demo"
+    demo = os.path.join(reference_root(), "data", "demo")
     mask = cv2.imread(os.path.join(demo, "cat_mask.png"))[..., 0]
     mask = (mask != 0)
     pts3d = np.loadtxt(os.path.join(demo, "cat_points_3d.txt"))

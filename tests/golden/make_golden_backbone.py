@@ -1,7 +1,7 @@
-"""Regenerates tests/golden/resnet18_8s_ref.npz.  Run in the authoring container:
-    python tests/golden/make_golden_backbone.py
+"""Regenerates tests/golden/resnet18_8s_ref_{k9,k17}.npz from a checkout of the reference project:
+    PVNET_REFERENCE=<path of the zju3dv/pvnet tree> python tests/golden/make_golden_backbone.py
 
-Imports the REFERENCE network classes from /root/reference/lib/networks/{resnet,
+Imports the REFERENCE network classes from <reference>/lib/networks/{resnet,
 model_repository}.py (by file path, with `lib.utils.config` stubbed and the ImageNet
 download at resnet.py:231 switched off), loads the deterministic weights of
 tests/helpers.seeded_state_dict, runs Resnet18_8s(18,2).eval() on a seeded input on the
@@ -17,9 +17,12 @@ import types
 import numpy as np
 import torch
 
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
+from tests.helpers import reference_root  # noqa: E402
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
-REF = "/root/reference/lib/networks"
+REF = os.path.join(reference_root(), "lib", "networks")
 
 
 def load_reference_classes():
@@ -54,20 +57,20 @@ def load_reference_classes():
 def main():
     cls = load_reference_classes()
     sys.path.insert(0, ROOT)
-    from tests.helpers import seeded_state_dict
+    from tests.helpers import BACKBONE_CASES, seeded_state_dict
     out = {}
-    for tag, (ver, seg, h, w) in {"k9": (18, 2, 64, 96), "k17": (34, 2, 48, 64)}.items():
+    for tag, (ver, seg) in {"k9": (18, 2), "k17": (34, 2)}.items():
+        h, w = BACKBONE_CASES[tag]
         net = cls(ver, seg)
         net.load_state_dict(seeded_state_dict(net, seed=1))
         net.eval()
         x = torch.from_numpy(np.random.default_rng(7).standard_normal((2, 3, h, w), dtype=np.float32))
         with torch.no_grad():
             s, v = net(x)
-        out[tag + "_x"] = x.numpy()
-        out[tag + "_seg"] = s.numpy().copy()
-        out[tag + "_ver"] = v.numpy().copy()
-    np.savez_compressed(os.path.join(HERE, "resnet18_8s_ref.npz"), **out)
-    print({k: v.shape for k, v in out.items()})
+        # the input is not stored (tests.helpers.backbone_golden regenerates it): each file stays under 1 MB
+        out[tag] = {"seg": s.numpy().copy(), "ver": v.numpy().copy()}
+        np.savez_compressed(os.path.join(HERE, f"resnet18_8s_ref_{tag}.npz"), **out[tag])
+    print({t: {k: v.shape for k, v in d.items()} for t, d in out.items()})
 
 
 if __name__ == "__main__":

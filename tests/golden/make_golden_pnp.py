@@ -1,4 +1,4 @@
-"""Generates tests/golden/pnp_cases.npz (run in the authoring container: needs /root/reference, cv2, scipy).
+"""Generates tests/golden/pnp_cases.npz (needs PVNET_REFERENCE = a checkout of the reference project, cv2, scipy).
 
 Cases:
   demo        the reference's own fixture: data/demo/cat_points_3d.txt (+ centre) projected with
@@ -16,11 +16,14 @@ import sys
 
 import numpy as np
 
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
+from tests.helpers import reference_root  # noqa: E402
+
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
 from oracle import pnp_oracle as pn  # noqa: E402
 
-REF = "/root/reference/data/demo"
+REF = os.path.join(reference_root(), "data", "demo")
 
 
 def main():

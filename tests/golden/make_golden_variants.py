@@ -1,8 +1,8 @@
 """Regenerates tests/golden/ref_variants.npz by running the REFERENCE'S OWN Python functions.
 
-Run in the authoring container (needs /root/reference):  python tests/golden/make_golden_variants.py
+Needs PVNET_REFERENCE = a checkout of the reference project:  python tests/golden/make_golden_variants.py
 
-lib/ransac_voting_gpu_layer/ransac_voting_gpu.py is imported unmodified from /root/reference
+lib/ransac_voting_gpu_layer/ransac_voting_gpu.py is imported unmodified from the reference project
 with its compiled extension `ransac_voting` replaced by a stub whose two functions call the
 oracle's C kernels (oracle/pvnet_oracle.c -- pinned bit-exactly against the reference's CUDA
 kernels by tests/test_gpu_reference_layer.py) on CPU tensors.  The stub also records every
@@ -27,6 +27,9 @@ import types
 
 import numpy as np
 import torch
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
+from tests.helpers import reference_root  # noqa: E402
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
@@ -56,14 +59,14 @@ def import_reference():
     stub.voting_for_hypothesis = voting_for_hypothesis
     for name in ("lib", "lib.ransac_voting_gpu_layer"):
         m = types.ModuleType(name)
-        m.__path__ = [os.path.join("/root/reference", *name.split("."))]
+        m.__path__ = [os.path.join(reference_root(), *name.split("."))]
         sys.modules[name] = m
     sys.modules["lib.ransac_voting_gpu_layer.ransac_voting"] = stub
     sys.modules["lib.ransac_voting_gpu_layer"].ransac_voting = stub
     import importlib.util
     spec = importlib.util.spec_from_file_location(
         "lib.ransac_voting_gpu_layer.ransac_voting_gpu",
-        "/root/reference/lib/ransac_voting_gpu_layer/ransac_voting_gpu.py")
+        os.path.join(reference_root(), "lib", "ransac_voting_gpu_layer", "ransac_voting_gpu.py"))
     mod = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(mod)
     return mod, recorded

@@ -1,5 +1,7 @@
 """Shared test helpers (CPU side)."""
+import hashlib
 import os
+import re
 
 import numpy as np
 
@@ -89,3 +91,84 @@ def variant_inputs(seed, n_fg=900, classes=1):
     vertex = np.stack([np.cos(ang), np.sin(ang)], -1).astype(np.float32)
     vertex[mask == 0] = 0
     return mask[None], vertex[None], kps
+
+
+BACKBONE_CASES = {"k9": (64, 96), "k17": (48, 64)}       # tag -> input height, width (batch 2)
+
+
+def backbone_golden():
+    """Outputs of the reference network classes (tests/golden/resnet18_8s_ref_<tag>.npz, made by
+    tests/golden/make_golden_backbone.py) with their inputs, which are regenerated from the same seed:
+    {tag_x, tag_seg, tag_ver} for tag in BACKBONE_CASES."""
+    out = {}
+    for tag, (h, w) in BACKBONE_CASES.items():
+        z = np.load(os.path.join(GOLDEN, f"resnet18_8s_ref_{tag}.npz"))
+        out[tag + "_x"] = np.random.default_rng(7).standard_normal((2, 3, h, w), dtype=np.float32)
+        out[tag + "_seg"], out[tag + "_ver"] = z["seg"], z["ver"]
+    return out
+
+
+def reference_root():
+    """The reference project's checkout named by PVNET_REFERENCE (the golden generators need it)."""
+    root = os.environ.get("PVNET_REFERENCE")
+    if not root or not os.path.isdir(os.path.join(root, "lib")):
+        raise SystemExit("set PVNET_REFERENCE to a checkout of the reference project (zju3dv/pvnet); got %r" % root)
+    return root
+
+
+# ------------------------------------------------------------------ stored outputs of the reference's CUDA kernels
+RECORD_REF = os.environ.get("PVNET_RECORD_REF_GOLDEN") == "1"     # set by tests/golden/make_golden_ref.py
+_DIGEST_ABOVE = 4096                                               # bytes: larger exact arrays are stored as sha256
+
+
+def _np(a):
+    if hasattr(a, "detach"):
+        return a.detach().cpu().numpy()
+    return np.asarray(a)
+
+
+def _pack(a):
+    """What a golden file holds for one exact array: the array, or a digest of dtype, shape and bytes."""
+    a = np.ascontiguousarray(_np(a))
+    if a.nbytes <= _DIGEST_ABOVE:
+        return a
+    return np.array(hashlib.sha256(f"{a.dtype.str}{a.shape}".encode() + a.tobytes()).hexdigest())
+
+
+def same_as_stored(got, stored):
+    """Bit-exact equality of `got` with a stored array or digest."""
+    got = _pack(got)
+    if got.dtype.kind == "U" or stored.dtype.kind == "U":
+        return str(got) == str(stored)
+    return got.dtype == stored.dtype and got.shape == stored.shape and got.tobytes() == stored.tobytes()
+
+
+def reference_kernels():
+    """oracle.ref_cuda: the reference's own kernels; only needed while recording."""
+    from oracle import ref_cuda
+    assert ref_cuda.available(), "recording needs oracle/_ref/libpvnet_refcuda.so (build() with PVNET_REFERENCE set)"
+    return ref_cuda
+
+
+class RefGolden:
+    """Outputs of the reference's kernels under a key, in tests/golden/<name>: computed by `fn` while recording
+    (PVNET_RECORD_REF_GOLDEN=1, needs oracle/_ref), read from the file otherwise.  Names in `exact` are packed
+    (_pack: compare with same_as_stored), the rest are stored whole."""
+
+    def __init__(self, name):
+        self.path = os.path.join(GOLDEN, name)
+        self.data = None
+
+    def get(self, key, fn, exact=()):
+        if self.data is None:
+            self.data = {} if RECORD_REF else dict(np.load(self.path))
+        key = re.sub(r"\W+", "_", key)
+        if RECORD_REF:
+            for name, v in fn().items():
+                self.data[f"{key}/{name}"] = _pack(v) if name in exact else np.asarray(_np(v))
+        pre = key + "/"
+        return {k[len(pre):]: v for k, v in self.data.items() if k.startswith(pre)}
+
+    def save(self):
+        if RECORD_REF and self.data:
+            np.savez_compressed(self.path, **self.data)

@@ -1,14 +1,14 @@
 """CPU: the reference's import lines resolve against the shims under lib/, and the public
 signatures (parameter names and defaults) equal the reference's.  The expected signatures are
-transcribed from lib/ransac_voting_gpu_layer/ransac_voting_gpu.py; when /root/reference is present
-(authoring container) they are re-derived from its source with `ast` and compared as well."""
-import ast
+transcribed from lib/ransac_voting_gpu_layer/ransac_voting_gpu.py and compared with
+tests/golden/ref_signatures.json, the signatures derived from the reference's source with `ast`."""
 import inspect
+import json
 import os
 
 import pytest
 
-REF = "/root/reference/lib/ransac_voting_gpu_layer/ransac_voting_gpu.py"
+from tests.helpers import GOLDEN
 
 EXPECTED = {
     "ransac_voting_layer": "mask, vertex, class_num, round_hyp_num, inlier_thresh=0.999, confidence=0.99, max_iter=20, min_num=5, max_num=30000",
@@ -50,15 +50,6 @@ def test_signature_equals_reference(name):
     assert _positional_signature(getattr(shim, name)) == EXPECTED[name]
 
 
-@pytest.mark.skipif(not os.path.exists(REF), reason="reference tree not present (GPU box)")
 def test_expected_signatures_match_reference_source():
-    tree = ast.parse(open(REF).read())
-    found = {}
-    for node in tree.body:
-        if isinstance(node, ast.FunctionDef) and node.name in EXPECTED:
-            a = node.args
-            names = [x.arg for x in a.args]
-            defaults = [None] * (len(names) - len(a.defaults)) + [ast.literal_eval(d) for d in a.defaults]
-            found[node.name] = ", ".join(n if d is None and i < len(names) - len(a.defaults) else f"{n}={d!r}"
-                                         for i, (n, d) in enumerate(zip(names, defaults)))
-    assert found == EXPECTED
+    with open(os.path.join(GOLDEN, "ref_signatures.json")) as f:
+        assert json.load(f) == EXPECTED

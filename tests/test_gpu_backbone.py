@@ -1,4 +1,4 @@
-"""GPU: the native Resnet18_8s (tcgen05 convs) against (a) the golden outputs produced by the
+"""GPU: the native Resnet18_8s (wgmma convs) against (a) the golden outputs produced by the
 REFERENCE classes on the CPU in true fp32, (b) our torch graph on the GPU with TF32 off.
 
 Tolerance.  The native path computes every conv with TF32 inputs (10-bit mantissa) and fp32
@@ -7,14 +7,13 @@ accumulation -- what the reference's own cuDNN path does on this GPU under torch
 error cuDNN-TF32 itself shows on the same input in the same test (floor 3e-3 of the range, in case cuDNN
 picks fp32 kernels for the small test shapes): a dropped K-block or tap in any layer, or a wrong BN fold,
 moves the output by far more.  Argmax flips against the fp32 graph are bounded too."""
-import os
 
 import numpy as np
 import pytest
 import torch
 
 from pvnet_b200.model_repository import Resnet18_8s
-from tests.helpers import GOLDEN, seeded_state_dict
+from tests.helpers import backbone_golden, seeded_state_dict
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -52,7 +51,7 @@ def _cudnn_tf32_error(net, x, ref):
 @pytest.mark.parametrize("tag,ver", [("k9", 18), ("k17", 34)])
 def test_native_vs_reference_golden(tag, ver, mode):
     from pvnet_b200 import conv as pc
-    z = np.load(os.path.join(GOLDEN, "resnet18_8s_ref.npz"))
+    z = backbone_golden()
     pc.set_mode(mode)
     try:
         net = _net(ver)
@@ -156,7 +155,7 @@ def test_odd_sizes_multiple_of_8():
 
 @pytest.mark.parametrize("shape", [(2, 480, 640), (1, 72, 104), (3, 16, 16), (1, 256, 264)], ids=str)
 @pytest.mark.parametrize("pixel_major", [False, True], ids=["nchw", "pixel-major"])
-@pytest.mark.parametrize("mode", [1, 2], ids=["epilogue warps", "dedicated warps"])
+@pytest.mark.parametrize("mode", [1, 2], ids=["epilogue warps", "dedicated warps"])     # any nonzero mode: the fused form
 def test_fused_upsample_equals_separate_launch(shape, pixel_major, mode):
     """convraw.0 interpolating its upsampled input itself (pvnet_backbone_set_fused_upsample) against the separate
     k_upsample2x launch it replaces: the same ATen arithmetic on the same conv2s.0 output, so the two forwards agree to the last bit
@@ -179,25 +178,6 @@ def test_fused_upsample_equals_separate_launch(shape, pixel_major, mode):
     print(f"\n[fused upsample] {shape} pixel_major={pixel_major}: max abs diff {d:.3e}, launches {launches0} -> {launches1}")
     assert torch.equal(fused, sep), f"fused and separate upsampling differ by {d:.3e}"
     assert torch.equal(mfused, msep)
-
-
-@pytest.mark.parametrize("fused", [False, True], ids=["separate upsampling", "fused upsampling"])
-def test_two_epilogue_sets_equal_one(fused):
-    """The fused-head kernel with two epilogue warp sets alternating tiles (tuning knob, 96 registers per thread)
-    computes exactly what the default single set does."""
-    from pvnet_b200 import conv as pc
-    x = torch.from_numpy(np.random.default_rng(6).standard_normal((2, 3, 240, 328), dtype=np.float32)).to(DEV)
-    outs = []
-    for sets in (1, 2):
-        pc.set_head_epilogue_sets(sets)
-        try:
-            net = _net(18, seed=12).set_fused_upsample(1 if fused else 0)     # a fresh handle: plans are built under the hook
-            with torch.no_grad():
-                outs.append(net.forward_native(x, with_mask=True, mask_dtype=torch.uint8))
-            torch.cuda.synchronize()
-        finally:
-            pc.set_head_epilogue_sets(0)
-    assert torch.equal(outs[0][0], outs[1][0]) and torch.equal(outs[0][1], outs[1][1])
 
 
 def _launches(fn):

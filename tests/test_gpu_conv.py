@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 convolution primitive against torch (fp64 reference computed from
+"""GPU: the wgmma convolution primitive against torch (fp64 reference computed from
 TF32-truncated operands: isolates indexing / layout / descriptor errors from TF32 rounding)."""
 import numpy as np
 import pytest
@@ -78,14 +78,12 @@ def test_conv_vs_torch(cfg, persistent):
 
 
 def test_conv_persistent_many_items_per_cta():
-    """More (M tile, N tile) items than resident CTAs: TMEM ping-pong and the continuous ring."""
+    """More (M tile, N tile) items than resident CTAs: every CTA loops, the TMA ring runs on across items."""
     pc.set_mode(pc.MODE_PER_TAP)
-    pc.set_multicast(0)
     try:
         _run_case(4, 120, 160, 64, 128, 3, 1, 1, 1, True, seed=11)     # 600 items, 1 CTA/SM
-        _run_case(2, 60, 80, 128, 512, 1, 1, 1, 0, False, seed=12)     # two N tiles per M tile, BN=256 (TMEM 512)
+        _run_case(2, 60, 80, 128, 512, 1, 1, 1, 0, False, seed=12)     # four N tiles per M tile
     finally:
-        pc.set_multicast(0)
         pc.set_mode(pc.MODE_AUTO)
 
 
@@ -95,7 +93,7 @@ def test_conv_persistent_many_items_per_cta():
     (2, 24, 40, 64, 64, 3, 1, 1, 1, True),      # layer1 BasicBlock conv2: residual + ReLU, partial tiles, N=64
     (1, 40, 48, 40, 32, 3, 1, 1, 2, False),     # convraw.0: Cin=40 -> 8-channel chunks, LeakyReLU
     (1, 48, 80, 128, 32, 3, 1, 1, 2, False),    # conv2s.0 shape (weights 147 KB resident)
-    (3, 64, 96, 64, 64, 3, 1, 1, 1, False),     # many tiles per CTA: exercises the persistent loop / TMEM ping-pong
+    (3, 64, 96, 64, 64, 3, 1, 1, 1, False),     # many tiles per CTA: exercises the persistent loop
     (1, 32, 40, 192, 64, 3, 1, 1, 2, False),    # conv4s.0 shape: 442 KB of weights -> tiles stream with the A boxes
     (2, 20, 44, 64, 64, 3, 1, 1, 1, True),      # width and height not multiples of the 16 x 8 tile, residual
 ])
@@ -118,7 +116,7 @@ def test_conv_column_kernel_rejects_dilation():
 
 
 def test_conv_column_kernel_large_persistent():
-    """More tiles than resident CTAs (148 SMs x 2): every CTA loops several times."""
+    """More tiles than resident CTAs (one per SM): every CTA loops several times."""
     pc.set_mode(pc.MODE_COLUMN)
     try:
         _run_case(2, 240, 320, 40, 32, 3, 1, 1, 2, False, seed=3)
@@ -138,35 +136,49 @@ def test_conv_round_out_is_tf32():
     assert ((out.view(torch.int32) & 0x1FFF) == 0).all()
 
 
-def test_conv_column_kernel_4x4_s2d_stem_shape():
-    """ksize 4 = taps at offsets {-2,-1,0,1} (the space-to-depth form of the 7x7/2 stem),
-    Cin=16 -> 64-byte swizzled rows, weights [64][4][4][16] resident."""
-    g = torch.Generator().manual_seed(4)
+def _run_4x4_case(cout, seed):
+    """ksize 4 = taps at offsets {-2,-1,0,1} (the space-to-depth form of the 7x7/2 stem), Cin=16 -> 64-byte
+    swizzled rows, weights [cout][4][4][16] resident."""
+    g = torch.Generator().manual_seed(seed)
     b, H, W = 2, 40, 56
     x = torch.randn(b, 16, H, W, generator=g)
-    w = torch.randn(64, 16, 4, 4, generator=g) / 16.0
-    bias = torch.randn(64, generator=g)
+    w = torch.randn(cout, 16, 4, 4, generator=g) / 16.0
+    bias = torch.randn(cout, generator=g)
     ref = F.relu(F.conv2d(F.pad(_trunc_tf32(x), (2, 1, 2, 1)).double(), pc.round_tf32(w).double(), bias.double()))
     xin = x.permute(0, 2, 3, 1).contiguous().to(DEV)
-    out = torch.empty(b, H, W, 64, device=DEV)
-    pc.conv2d_nhwc(xin, 0, 16, pc.pack_weight(w.to(DEV)), bias.to(DEV), out, 0, 64, 4, 1, 1, pc.ACT_RELU)
+    out = torch.full((b, H, W, cout + 32), -3.0, device=DEV)        # 32 channels beyond cout must stay untouched
+    pc.conv2d_nhwc(xin, 0, 16, pc.pack_weight(w.to(DEV)), bias.to(DEV), out, 0, cout, 4, 1, 1, pc.ACT_RELU)
     torch.cuda.synchronize()
-    err = (out.permute(0, 3, 1, 2).double().cpu() - ref).abs().max().item()
+    err = (out[..., :cout].permute(0, 3, 1, 2).double().cpu() - ref).abs().max().item()
     assert err <= 2e-5 * max(ref.abs().max().item(), 1.0) + 1e-5, err
+    assert (out[..., cout:] == -3.0).all()
 
 
-@pytest.mark.parametrize("mc", [2, 1, 0], ids=["cta_group2", "multicast", "single-cta"])
+def test_conv_column_kernel_4x4_s2d_stem_shape():
+    """The stem's shape: 64 output channels."""
+    _run_4x4_case(64, 4)
+
+
+def test_conv_column_kernel_4x4_cout32():
+    """A 4x4 layer with 32 output channels runs on its own instantiation (N = 32)."""
+    _run_4x4_case(32, 5)
+
+
+@pytest.mark.parametrize("mc", [1, 0], ids=["multicast", "single-cta"])
 @pytest.mark.parametrize("cfg", [
     (1, 24, 40, 128, 256, 3, 1, 2, 1, False),   # 9 M tiles: odd -> the last cluster's 2nd CTA duplicates a tile
-    (2, 24, 40, 64, 512, 3, 1, 4, 1, True),     # two N tiles, residual
+    (2, 24, 40, 64, 512, 3, 1, 4, 1, True),     # four N tiles, residual
     (2, 60, 80, 256, 256, 1, 1, 1, 0, False),   # 1x1, 80 M tiles
 ])
 def test_conv_cluster_multicast(cfg, mc):
-    """256-row weight tiles: 2-CTA clusters with TMA multicast vs the plain launch."""
+    """Wide layers: 2-CTA clusters sharing each weight tile through TMA multicast vs the plain launch."""
     pc.set_mode(pc.MODE_PER_TAP)
     pc.set_multicast(mc)
     try:
         _run_case(*cfg)
+        pc.set_persistent(False)      # one (M tile pair, N tile) per cluster
+        _run_case(*cfg)
     finally:
+        pc.set_persistent(True)
         pc.set_multicast(0)
         pc.set_mode(pc.MODE_AUTO)

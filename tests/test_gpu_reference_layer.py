@@ -1,20 +1,27 @@
-"""GPU box only: the reference's OWN CUDA kernels (oracle/_ref, compiled verbatim from
-/root/reference by oracle/Makefile in the authoring container) against the oracle and
-against the product.  This is what pins the oracle (SURVEY.md §8c) and what measures
-"within 1e-4 of the reference CUDA layer"."""
+"""GPU: the product and the oracle against the outputs of the reference's OWN CUDA kernels
+(ransac_voting_kernel.cu compiled verbatim by oracle/Makefile into oracle/_ref, run through the
+reference layer's own torch orchestration in oracle/ref_cuda.py).  Those outputs are stored in
+tests/golden/ref_layer.npz (tests/golden/make_golden_ref.py records them on a GPU where
+oracle/_ref is built), so every run compares against them without the reference.  This is what pins
+the oracle (SURVEY.md §8c) and what measures "within 1e-4 of the reference CUDA layer"."""
 import numpy as np
 import pytest
 import torch
 
 from oracle import pvnet_oracle as po
-from oracle import ref_cuda
 from pvnet_b200 import ransac_voting_gpu as rv
 from pvnet_b200 import synthetic as syn
-from tests.helpers import cfg1_inputs, demo_fixture
+from tests.helpers import RefGolden, cfg1_inputs, demo_fixture, reference_kernels, same_as_stored
 
-pytestmark = [pytest.mark.gpu,
-              pytest.mark.skipif(not ref_cuda.available(), reason="oracle/_ref/libpvnet_refcuda.so not built")]
+pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
+_gold = RefGolden("ref_layer.npz")
+
+
+@pytest.fixture(scope="module", autouse=True)
+def _write_golden():
+    yield
+    _gold.save()
 
 
 def _dev_inputs(mask_np, field_np):
@@ -29,13 +36,18 @@ def test_reference_kernels_pin_the_oracle(kind):
     mask, field, idxs = cfg1_inputs(kind)
     coords, direct = po.compact(mask.astype(np.uint8), syn.as_reference_view(field[None])[0])
     d, c, i = (torch.from_numpy(a).to(DEV) for a in (direct, coords, idxs))
-    hyp = ref_cuda.generate_hypothesis(d, c, i)
+
+    def reference():
+        rc = reference_kernels()
+        hyp = rc.generate_hypothesis(d, c, i)
+        inl = torch.zeros([128, 9, 10000], dtype=torch.uint8, device=DEV)
+        rc.voting_for_hypothesis(d, c, hyp, inl, 0.99)
+        return {"hyp": hyp, "counts": inl.sum(2).to(torch.int32), "inl8": inl[:8]}
+    ref = _gold.get(f"pin_{kind}", reference, exact=("hyp", "counts", "inl8"))
     ohyp = po.generate_hypothesis_kernel(direct, coords, idxs)
-    assert np.array_equal(hyp.cpu().numpy().view(np.uint32), ohyp.view(np.uint32))
-    inl = torch.zeros([128, 9, 10000], dtype=torch.uint8, device=DEV)
-    ref_cuda.voting_for_hypothesis(d, c, hyp, inl, 0.99)
-    assert np.array_equal(inl.sum(2).cpu().numpy().astype(np.int32), po.vote_counts(direct, coords, ohyp, 0.99))
-    assert np.array_equal(inl[:8].cpu().numpy(), po.voting_for_hypothesis_kernel(direct, coords, ohyp[:8], 0.99))
+    assert same_as_stored(ohyp, ref["hyp"])
+    assert same_as_stored(po.vote_counts(direct, coords, ohyp, 0.99).astype(np.int32), ref["counts"])
+    assert same_as_stored(po.voting_for_hypothesis_kernel(direct, coords, ohyp[:8], 0.99).astype(np.uint8), ref["inl8"])
 
 
 def test_reference_kernels_pin_the_oracle_on_edge_values():
@@ -48,16 +60,23 @@ def test_reference_kernels_pin_the_oracle_on_edge_values():
     coords = np.stack([rng.integers(0, 640, tn), rng.integers(0, 480, tn)], 1).astype(np.float32)
     idxs = rng.integers(0, tn, (hn, vn, 2), dtype=np.int32)
     d, c, i = (torch.from_numpy(a).to(DEV) for a in (direct, coords, idxs))
-    hyp = ref_cuda.generate_hypothesis(d, c, i)
     ohyp = po.generate_hypothesis_kernel(direct, coords, idxs)
-    assert np.array_equal(hyp.cpu().numpy().view(np.uint32), ohyp.view(np.uint32))
     # also hypotheses ON pixels (norm2 == 0) and far away
     extra = np.concatenate([coords[:32, None, :].repeat(vn, 1), np.full((8, vn, 2), 3e7, np.float32)]).astype(np.float32)
-    for thresh in (0.99, 0.5, -0.25):
-        for hp in (ohyp, extra):
+    cases = [(thresh, j, hp) for thresh in (0.99, 0.5, -0.25) for j, hp in enumerate((ohyp, extra))]
+
+    def reference():
+        rc = reference_kernels()
+        out = {"hyp": rc.generate_hypothesis(d, c, i)}
+        for thresh, j, hp in cases:
             inl = torch.zeros([hp.shape[0], vn, tn], dtype=torch.uint8, device=DEV)
-            ref_cuda.voting_for_hypothesis(d, c, torch.from_numpy(hp).to(DEV), inl, thresh)
-            assert np.array_equal(inl.cpu().numpy(), po.voting_for_hypothesis_kernel(direct, coords, hp, thresh))
+            rc.voting_for_hypothesis(d, c, torch.from_numpy(hp).to(DEV), inl, thresh)
+            out[f"inl_{thresh}_{j}"] = inl
+        return out
+    ref = _gold.get("edge", reference, exact=["hyp"] + [f"inl_{t}_{j}" for t, j, _ in cases])
+    assert same_as_stored(ohyp, ref["hyp"])
+    for thresh, j, hp in cases:
+        assert same_as_stored(po.voting_for_hypothesis_kernel(direct, coords, hp, thresh).astype(np.uint8), ref[f"inl_{thresh}_{j}"])
 
 
 def _product_vs_reference_layer(mask_np, field_np, hn, thresh, max_num=30000, label=""):
@@ -67,23 +86,33 @@ def _product_vs_reference_layer(mask_np, field_np, hn, thresh, max_num=30000, la
     within 1e-4 of the reference layer once the reference's fp32 refit rounding is taken
     out (fp64 run).  Returns the gaps."""
     mask, vertex = _dev_inputs(mask_np, field_np)
-    rec = []
-    torch.manual_seed(0)
-    ref_kp = ref_cuda.layer_v3(mask, vertex, hn, inlier_thresh=thresh, max_num=max_num, record=rec)
-    torch.manual_seed(0)
-    ref_kp64 = ref_cuda.layer_v3(mask, vertex, hn, inlier_thresh=thresh, max_num=max_num,
-                                 refit_dtype=torch.float64)
+
+    def reference():
+        rc = reference_kernels()
+        rec = []
+        torch.manual_seed(0)
+        out = {"kp": rc.layer_v3(mask, vertex, hn, inlier_thresh=thresh, max_num=max_num, record=rec)}
+        torch.manual_seed(0)
+        out["kp64"] = rc.layer_v3(mask, vertex, hn, inlier_thresh=thresh, max_num=max_num, refit_dtype=torch.float64)
+        for bi, r in enumerate(rec):
+            out[f"rec{bi}"] = np.array(r is not None)
+            if r is not None:
+                out.update({f"idxs{bi}": r["idxs"], f"tn{bi}": np.array(r["tn"]), f"counts{bi}": r["counts"],
+                            f"hyp{bi}": r["hyp"]})
+        return out
+    ref = _gold.get(label, reference, exact=[f"{n}{bi}" for n in ("idxs", "counts", "hyp") for bi in range(mask.shape[0])])
     torch.manual_seed(0)
     kp, dbg = rv.ransac_voting_layer_v3(mask, vertex, hn, inlier_thresh=thresh, max_num=max_num, return_debug=True)
-    for bi, r in enumerate(rec):
-        if r is None:
+    for bi in range(mask.shape[0]):
+        if not ref.get(f"rec{bi}", False):
             continue
         # fixed-seed parity: same samples drawn, same counts, same winner
-        assert torch.equal(dbg["idxs"][bi], r["idxs"]), "RNG stream differs from the reference's"
-        assert int(dbg["tn"][bi]) == r["tn"]
-        assert torch.equal(dbg["counts"][bi].long(), r["counts"]), "inlier counts differ from the reference layer"
-        assert torch.equal(dbg["hyp"][bi], r["hyp"])
-    kp, ref_kp, ref_kp64 = kp.cpu().numpy(), ref_kp.cpu().numpy(), ref_kp64.cpu().numpy()
+        assert same_as_stored(dbg["idxs"][bi], ref[f"idxs{bi}"]), "RNG stream differs from the reference's"
+        assert int(dbg["tn"][bi]) == int(ref[f"tn{bi}"])
+        assert same_as_stored(dbg["counts"][bi].long(), ref[f"counts{bi}"]), "inlier counts differ from the reference layer"
+        assert same_as_stored(dbg["hyp"][bi], ref[f"hyp{bi}"])
+    ref_kp, ref_kp64 = ref["kp"], ref["kp64"]
+    kp = kp.cpu().numpy()
     gap32 = np.abs(kp - ref_kp).max()
     gap64 = np.abs(kp - ref_kp64).max()
     noise = np.abs(ref_kp - ref_kp64).max()
@@ -137,36 +166,51 @@ def test_covariance_fixed_seed_parity():
     mask, vertex = _dev_inputs(masks, fields)
     torch.manual_seed(1)
     mean = rv.ransac_voting_layer_v3(mask, vertex, 256, inlier_thresh=0.99)
-    rec = []
-    torch.manual_seed(2)
-    _, ref_cov = ref_cuda.layer_cov_with_mean(mask, vertex, mean, round_hyp_num=128, min_hyp_num=512,
-                                              inlier_thresh=0.99, record=rec)
+    ref = _ref_cov("cov_parity", mask, vertex, mean, dict(round_hyp_num=128, min_hyp_num=512, inlier_thresh=0.99), 2)
     torch.manual_seed(2)
     _, cov, dbg = rv.estimate_voting_distribution_with_mean(mask, vertex, mean, round_hyp_num=128, min_hyp_num=512,
                                                             inlier_thresh=0.99, return_debug=True)
-    for bi, r in enumerate(rec):
-        assert torch.equal(dbg["idxs"][bi], r["idxs"])
-        assert torch.equal(dbg["counts"][bi].long(), r["counts"])
+    for bi in range(mask.shape[0]):
+        if f"idxs{bi}" not in ref:
+            continue
+        assert same_as_stored(dbg["idxs"][bi], ref[f"idxs{bi}"])
+        assert same_as_stored(dbg["counts"][bi].long(), ref[f"counts{bi}"])
+    ref_cov = torch.from_numpy(ref["cov"]).to(DEV)
     gap = (cov - ref_cov).abs()
     print(f"\n[reference-layer gap] covariance: max abs {gap.max().item():.3e}, "
           f"max rel {(gap / ref_cov.abs().clamp_min(1e-6)).max().item():.3e}, |cov| max {ref_cov.abs().max().item():.3e}")
     assert torch.allclose(cov, ref_cov, atol=1e-4, rtol=1e-4)
 
 
+def _ref_cov(key, mask, vertex, mean, kw, seed):
+    """reference layer estimate_voting_distribution_with_mean under torch.manual_seed(seed): covariances and,
+    per image, the recorded samples and counts"""
+    def reference():
+        rec = []
+        torch.manual_seed(seed)
+        _, cov = reference_kernels().layer_cov_with_mean(mask, vertex, mean, record=rec, **kw)
+        out = {"cov": cov}
+        for bi, r in enumerate(rec):
+            out.update({f"idxs{bi}": r["idxs"], f"counts{bi}": r["counts"]})
+        return out
+    return _gold.get(key, reference, exact=[f"{n}{bi}" for n in ("idxs", "counts") for bi in range(mask.shape[0])])
+
+
 def _cov_vs_reference_layer(masks, fields, hn, min_hyp, thresh, max_num, seed):
     mask, vertex = _dev_inputs(masks, fields)
     torch.manual_seed(seed)
     mean = rv.ransac_voting_layer_v3(mask, vertex, hn, inlier_thresh=thresh, max_num=max_num)
-    rec = []
-    torch.manual_seed(seed + 1)
-    _, ref_cov = ref_cuda.layer_cov_with_mean(mask, vertex, mean, round_hyp_num=hn, min_hyp_num=min_hyp,
-                                              inlier_thresh=thresh, max_num=max_num, record=rec)
+    ref = _ref_cov(f"cov_{seed}", mask, vertex, mean,
+                   dict(round_hyp_num=hn, min_hyp_num=min_hyp, inlier_thresh=thresh, max_num=max_num), seed + 1)
     torch.manual_seed(seed + 1)
     _, cov, dbg = rv.estimate_voting_distribution_with_mean(mask, vertex, mean, round_hyp_num=hn, min_hyp_num=min_hyp,
                                                             inlier_thresh=thresh, max_num=max_num, return_debug=True)
-    for bi, r in enumerate(rec):
-        assert torch.equal(dbg["idxs"][bi], r["idxs"]), "RNG stream differs from the reference's"
-        assert torch.equal(dbg["counts"][bi].long(), r["counts"]), "inlier counts differ from the reference layer"
+    for bi in range(mask.shape[0]):
+        if f"idxs{bi}" not in ref:
+            continue
+        assert same_as_stored(dbg["idxs"][bi], ref[f"idxs{bi}"]), "RNG stream differs from the reference's"
+        assert same_as_stored(dbg["counts"][bi].long(), ref[f"counts{bi}"]), "inlier counts differ from the reference layer"
+    ref_cov = torch.from_numpy(ref["cov"]).to(DEV)
     assert torch.allclose(cov, ref_cov, atol=1e-4, rtol=1e-4), (cov - ref_cov).abs().max().item()
 
 

@@ -13,7 +13,7 @@ from lib.ransac_voting_gpu_layer.ransac_voting_gpu import (estimate_voting_distr
                                                            ransac_voting_layer_v4)
 from oracle import pvnet_oracle as po
 from pvnet_b200 import synthetic as syn
-from tests.helpers import variant_inputs
+from tests.helpers import RefGolden, reference_kernels, same_as_stored, variant_inputs
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -137,8 +137,16 @@ def _vp_inputs(seed, tn=3000, vn=4, hn=96):
     return direct, coords, idxs
 
 
+_gold = RefGolden("ref_vp.npz")
+
+
+@pytest.fixture(scope="module", autouse=True)
+def _write_golden():
+    yield
+    _gold.save()
+
+
 def test_vanishing_point_pair_bit_exact_vs_oracle_and_reference_kernels():
-    from oracle import ref_cuda
     from pvnet_b200 import ransac_voting as ext
     direct, coords, idxs = _vp_inputs(21)
     d, c, i = (torch.from_numpy(a).to(DEV) for a in (direct, coords, idxs))
@@ -153,14 +161,25 @@ def test_vanishing_point_pair_bit_exact_vs_oracle_and_reference_kernels():
         assert np.array_equal(inl.cpu().numpy(), oinl)
         assert np.array_equal(cnt.cpu().numpy(), oinl.sum(2))
         assert oinl.sum() > 1000
-    if ref_cuda.available() and hasattr(ref_cuda.lib(), "pvref_generate_hypothesis_vp"):
-        rhyp = ref_cuda.generate_hypothesis_vanishing_point(d, c, i)     # the reference's own kernels pin both
-        assert torch.equal(rhyp.view(torch.int32), hyp.view(torch.int32))
-        rinl = torch.zeros([96, 4, 3000], dtype=torch.uint8, device=DEV)
-        ref_cuda.voting_for_hypothesis_vanishing_point(d, c, rhyp, rinl, 0.99)
+
+    # the reference's own kernels (stored outputs, tests/golden/ref_vp.npz) pin the oracle and the product
+    def reference():
+        rc = reference_kernels()
+        rhyp = rc.generate_hypothesis_vanishing_point(d, c, i)
+        out = {"hyp": rhyp}
+        for thresh in (0.99, 0.5):
+            rinl = torch.zeros([96, 4, 3000], dtype=torch.uint8, device=DEV)
+            rc.voting_for_hypothesis_vanishing_point(d, c, rhyp, rinl, thresh)
+            out[f"inl_{thresh}"] = rinl
+        return out
+    ref = _gold.get("vp21", reference, exact=("hyp", "inl_0.99", "inl_0.5"))
+    assert same_as_stored(hyp, ref["hyp"]) and same_as_stored(ohyp, ref["hyp"])
+    for thresh in (0.99, 0.5):
         inl = torch.zeros([96, 4, 3000], dtype=torch.uint8, device=DEV)
-        ext.voting_for_hypothesis_vanishing_point(d, c, hyp, inl, 0.99)
-        assert torch.equal(rinl, inl)
+        ext.voting_for_hypothesis_vanishing_point(d, c, hyp, inl, thresh)
+        assert same_as_stored(inl, ref[f"inl_{thresh}"])
+        assert same_as_stored(po.voting_for_hypothesis_vanishing_point_kernel(direct, coords, ohyp, thresh).astype(np.uint8),
+                              ref[f"inl_{thresh}"])
 
 
 def test_v2_against_reference_fixture(gold):
