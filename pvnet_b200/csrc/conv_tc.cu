@@ -6,7 +6,7 @@
 // the activation / residual add fused into the epilogue:
 //
 //   M = 128 output pixels (a TH x TW = 8 x 16 patch of one image)
-//   N = BN output channels (32, 64 or 128)
+//   N = BN output channels (32, 64, 128 or 256: conv_plan picks the one its model says finishes first)
 //   K = taps x Cin, walked tap by tap in chunks of 32 input channels
 //
 //   warp 8       TMA producer: per K-block one 4-D box {32 ch, TW, TH, 1 image} of the NHWC input,
@@ -171,27 +171,53 @@ __global__ void __launch_bounds__(CONV_THREADS, 1)
             const int img = m_tile / tiles_per_img;
             const int trem = m_tile - img * tiles_per_img;
             const int tyi = trem / g.tiles_x, txi = trem - tyi * g.tiles_x;
+            // this thread's two pixel rows (g8 and g8 + 8 of its warp's 16)
+            bool ok[2];
+            float *optr[2];
+            const float *rptr[2];
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const int m = wg * 64 + wq * 16 + g8 + 8 * h;
                 const int y = tyi * g.TH + m / g.TW, x = txi * g.TW + m % g.TW;
-                if (y >= g.Ho || x >= g.Wo) continue;
-                const size_t pix = ((size_t)img * g.Ho + y) * g.Wo + x;
-                float *optr = out + pix * g.out_cs + g.out_co + n0;
-                const float *rptr = res ? res + pix * g.res_cs + g.res_co + n0 : nullptr;
+                ok[h] = y < g.Ho && x < g.Wo;
+                const size_t pix = ok[h] ? ((size_t)img * g.Ho + y) * g.Wo + x : 0;
+                optr[h] = out + pix * g.out_cs + g.out_co + n0;
+                rptr[h] = res ? res + pix * g.res_cs + g.res_co + n0 : nullptr;
+            }
+            // groups of JC 8-channel blocks: every bias and residual load of a group is issued before its
+            // arithmetic, so the epilogue waits for one load latency per group rather than one per block.
+            // With 288 threads the 64K registers split over four sub-partitions allow 168 per thread; BN = 256
+            // holds 128 accumulators, so its groups are 2 blocks to stay clear of spills.
+            constexpr int JC = BN == 256 ? 2 : (BN / 8 < 8 ? BN / 8 : 8);
 #pragma unroll
-                for (int j = 0; j < BN / 8; ++j) {
-                    const int c = 8 * j + 2 * t4;
-                    const float2 bv = __ldg(reinterpret_cast<const float2 *>(bias + n0 + c));
-                    float2 v = make_float2(acc[4 * j + 2 * h] + bv.x, acc[4 * j + 2 * h + 1] + bv.y);
-                    if (rptr) {
-                        const float2 rv = __ldg(reinterpret_cast<const float2 *>(rptr + c));
-                        v.x += rv.x;
-                        v.y += rv.y;
+            for (int j0 = 0; j0 < BN / 8; j0 += JC) {
+                float2 bv[JC], rv[2][JC];
+#pragma unroll
+                for (int jj = 0; jj < JC; ++jj)
+                    bv[jj] = __ldg(reinterpret_cast<const float2 *>(bias + n0 + 8 * (j0 + jj) + 2 * t4));
+                if (res) {
+#pragma unroll
+                    for (int h = 0; h < 2; ++h)
+#pragma unroll
+                        for (int jj = 0; jj < JC; ++jj)
+                            rv[h][jj] = ok[h] ? __ldg(reinterpret_cast<const float2 *>(rptr[h] + 8 * (j0 + jj) + 2 * t4))
+                                              : make_float2(0.f, 0.f);
+                }
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    if (!ok[h]) continue;
+#pragma unroll
+                    for (int jj = 0; jj < JC; ++jj) {
+                        const int j = j0 + jj;
+                        float2 v = make_float2(acc[4 * j + 2 * h] + bv[jj].x, acc[4 * j + 2 * h + 1] + bv[jj].y);
+                        if (res) {
+                            v.x += rv[h][jj].x;
+                            v.y += rv[h][jj].y;
+                        }
+                        v.x = epi_act(v.x, g.act, g.round_out);
+                        v.y = epi_act(v.y, g.act, g.round_out);
+                        *reinterpret_cast<float2 *>(optr[h] + 8 * j + 2 * t4) = v;
                     }
-                    v.x = epi_act(v.x, g.act, g.round_out);
-                    v.y = epi_act(v.y, g.act, g.round_out);
-                    *reinterpret_cast<float2 *>(optr + c) = v;
                 }
             }
         }
@@ -296,8 +322,24 @@ int conv_plan(const ConvDesc &d, ConvPlan *p)
     g.cin_chunks = (d.Cin + kc - 1) / kc;
     g.cin_pad = g.cin_chunks * kc;
     g.Cout = d.Cout;
-    // N tile: 128 channels (64 fp32 accumulators per consumer thread) where Cout allows
-    g.BN = d.Cout % 128 == 0 ? 128 : (d.Cout % 64 == 0 ? 64 : 32);
+    // N tile: the divisor of Cout among 256/128/64/32 that the model says finishes first. The kernel is bound
+    // by operand delivery into shared memory -- every K-block brings a 16 KB A box and a BN x 128 B weight
+    // tile, whatever BN is -- and the persistent CTAs (one per SM) take the items round-robin, so a layer
+    // costs about rounds x per-item bytes, rounds = ceil(items / SMs). Ties go to the wider tile. Every BN
+    // sums each output element over the same K sequence, so the choice does not change the results.
+    {
+        const long long sms = sm_count() > 0 ? sm_count() : 1;
+        long long best = -1;
+        for (int bn = 256; bn >= 32; bn >>= 1) {
+            if (d.Cout % bn) continue;
+            const long long items = (long long)g.total_m_tiles * (d.Cout / bn);
+            const long long cost = (items + sms - 1) / sms * (CONV_A_BYTES + bn * kc * 4);
+            if (best < 0 || cost < best) {
+                best = cost;
+                g.BN = bn;
+            }
+        }
+    }
     g.out_cs = d.out_cs;
     g.out_co = d.out_co;
     g.res_cs = d.res_cs;
@@ -387,10 +429,12 @@ int conv_launch_t(const ConvPlan &p, cudaStream_t s)
 int conv_launch(const ConvPlan &p, cudaStream_t s)
 {
     if (p.mc) {
+        if (p.g.BN == 256) return conv_launch_t<256, true>(p, s);
         if (p.g.BN == 128) return conv_launch_t<128, true>(p, s);
         if (p.g.BN == 64) return conv_launch_t<64, true>(p, s);
         return conv_launch_t<32, true>(p, s);
     }
+    if (p.g.BN == 256) return conv_launch_t<256, false>(p, s);
     if (p.g.BN == 128) return conv_launch_t<128, false>(p, s);
     if (p.g.BN == 64) return conv_launch_t<64, false>(p, s);
     return conv_launch_t<32, false>(p, s);
