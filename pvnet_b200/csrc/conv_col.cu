@@ -9,9 +9,10 @@
 //     CTA is persistent over output tiles (grid = one CTA per SM, static round-robin);
 //   * "halo box": for each channel chunk ONE TMA box of (TH+KH-1) x (TW+KH-1) pixels is loaded and
 //     all KH x KW taps read from it: A traffic is (TH+2)(TW+2)/(TH*TW) = 1.41x the tile instead of 9x.
-//     A tap's operand rows start anywhere in the box, so the consumer warpgroups gather the A
-//     fragments into registers (undoing the box's swizzle) and issue register-A wgmma; the weights
-//     are shared-memory descriptor operands;
+//     A tap's operand is the box shifted by the tap offset: a descriptor starting at that pixel, with
+//     8-row groups one box row apart, addresses it in place (the swizzle follows the absolute address).
+//     Both operands are shared-memory descriptors, and one chunk's MMAs stay in flight while the
+//     previous chunk's stage is released;
 //   * optional fused head (convraw.3 1x1 + bias + argmax) in the epilogue: the activated 128 x 32 tile
 //     is already in the register layout of a wgmma A operand, so the head is one more MMA, and the
 //     reference's NCHW output is written directly -- the [b,H,W,32] intermediate never exists;
@@ -118,13 +119,13 @@ __device__ __forceinline__ void up_fill_rows(const float *base, unsigned rstride
                     wc = __shfl_sync(0xffffffffu, wc_l, i);
         const int e = (i >> 1) - S0;
         // Rounding to tf32 (nearest, ties away -- cvt.rna.tf32, what k_upsample2x stores): add half an ulp of
-        // the 10-bit mantissa; the 13 low bits that remain are cleared when the MMA operand is gathered (see
-        // k_conv_col), so the MMA sees exactly the values the separate launch feeds it.
+        // the 10-bit mantissa and clear the 13 low bits, so the MMA reads exactly the values the separate
+        // launch stores.
         float4 o;
-        o.x = __uint_as_float(__float_as_uint(lerp3(wa, t[e].x, wb, t[e + 1].x, wc, t[e + 2].x)) + 0x1000u);
-        o.y = __uint_as_float(__float_as_uint(lerp3(wa, t[e].y, wb, t[e + 1].y, wc, t[e + 2].y)) + 0x1000u);
-        o.z = __uint_as_float(__float_as_uint(lerp3(wa, t[e].z, wb, t[e + 1].z, wc, t[e + 2].z)) + 0x1000u);
-        o.w = __uint_as_float(__float_as_uint(lerp3(wa, t[e].w, wb, t[e + 1].w, wc, t[e + 2].w)) + 0x1000u);
+        o.x = __uint_as_float((__float_as_uint(lerp3(wa, t[e].x, wb, t[e + 1].x, wc, t[e + 2].x)) + 0x1000u) & 0xFFFFE000u);
+        o.y = __uint_as_float((__float_as_uint(lerp3(wa, t[e].y, wb, t[e + 1].y, wc, t[e + 2].y)) + 0x1000u) & 0xFFFFE000u);
+        o.z = __uint_as_float((__float_as_uint(lerp3(wa, t[e].z, wb, t[e + 1].z, wc, t[e + 2].z)) + 0x1000u) & 0xFFFFE000u);
+        o.w = __uint_as_float((__float_as_uint(lerp3(wa, t[e].w, wb, t[e + 1].w, wc, t[e + 2].w)) + 0x1000u) & 0xFFFFE000u);
         const int rr = i * PITCH + c;
         if (act) ptx::sts128(sbase + (uint32_t)(i * PITCH * 32) + (uint32_t)((hf ^ ((rr >> 2) & 1)) << 4), o);
     }
@@ -279,11 +280,12 @@ __global__ void __launch_bounds__(COL_THREADS, 1)
         return;
     }
 
-    // consumer warpgroup wg: tile rows [8 wg, 8 wg + 8); this thread's A rows are tile pixels
-    // (8 wg + 2 wq, g8) and (8 wg + 2 wq + 1, g8), i.e. box rows rr0 and rr0 + PITCH at tap (0, 0)
+    // consumer warpgroup wg: tile rows [8 wg, 8 wg + 8).  At tap (kh, kw) its 64 A rows are 8 core-matrix groups
+    // of 8 consecutive box pixels, group i at box row 8 wg + i + kh from column kw: a K-major operand whose groups
+    // are PITCH box pixels apart, addressed by a descriptor that starts at that pixel (see make_kmajor_desc).
+    // Thread (wq, lane) holds the accumulator rows of tile pixels (8 wg + 2 wq, g8) and (8 wg + 2 wq + 1, g8).
     const int wg = warp >> 2, wq = warp & 3;
     const int g8 = lane >> 2, t4 = lane & 3;
-    const uint32_t rr0 = (uint32_t)((8 * wg + 2 * wq) * PITCH + g8);
     const uint32_t sA_u = ptx::smem_u32(sA), sB_u = ptx::smem_u32(sB);
     if (g.resident) ptx::mbar_wait(wfull, 0);
     int s = 0;
@@ -292,69 +294,74 @@ __global__ void __launch_bounds__(COL_THREADS, 1)
         float acc[BN / 2];
 #pragma unroll
         for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+        int prev = -1;
         for (int cc = 0; cc < g.cin_chunks; ++cc) {
             ptx::mbar_wait(&full[s], ph);
             const uint32_t a0 = sA_u + (uint32_t)s * (uint32_t)stage_bytes;
             const uint32_t b0 = g.resident ? sB_u + (uint32_t)(cc * KH * KH * B_TILE) : a0 + (uint32_t)A_BYTES;
-            // taps in groups of TG (a whole tap row for the narrow chunks, one tap for 32-channel chunks: register
-            // budget): gather the group's A fragments (tf32: the low 13 bits cleared), then TG * KC/8 MMAs
-            constexpr int TG = KC == 32 ? 1 : KH;
+            const uint64_t ad0 = ptx::make_kmajor_desc(a0 + (uint32_t)(8 * wg * PITCH * ROWB), ROWB, PITCH * ROWB);
+            const uint64_t bd0 = ptx::make_kmajor_desc(b0, ROWB);
+            // the chunk's taps, then 8-channel K steps, into one accumulator; descriptor start addresses count
+            // 16-byte units
+            ptx::wgmma_fence();
 #pragma unroll
-            for (int t0 = 0; t0 < KH * KH; t0 += TG) {
-                uint32_t a[TG][KC / 8][4];
+            for (int t = 0; t < KH * KH; ++t) {
+                const uint64_t ad = ad0 + (uint64_t)(((t / KH) * PITCH + t % KH) * ROWB / 16);
+                const uint64_t bd = bd0 + (uint64_t)(t * B_TILE / 16);
 #pragma unroll
-                for (int u = 0; u < TG; ++u)
-#pragma unroll
-                    for (int ks = 0; ks < KC / 8; ++ks)
-#pragma unroll
-                        for (int f = 0; f < 4; ++f) {
-                            const int kh = (t0 + u) / KH, kw = (t0 + u) % KH;
-                            const uint32_t rr = rr0 + (uint32_t)((kh + (f & 1)) * PITCH + kw);
-                            const uint32_t off = rr * ROWB + (uint32_t)((8 * ks + t4 + 4 * (f >> 1)) * 4);
-                            uint32_t v;
-                            asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(a0 + ptx::swizzle_off(off, ROWB)));
-                            a[u][ks][f] = v & 0xFFFFE000u;
-                        }
-                ptx::wgmma_fence();
-#pragma unroll
-                for (int u = 0; u < TG; ++u) {
-                    const uint64_t bd = ptx::make_kmajor_desc(b0 + (uint32_t)((t0 + u) * B_TILE), ROWB);
-#pragma unroll
-                    for (int ks = 0; ks < KC / 8; ++ks)
-                        ptx::Wgmma<BN>::rs(acc, a[u][ks], bd + (uint64_t)(2 * ks), (cc | (t0 + u) | ks) != 0 ? 1u : 0u);
-                }
-                ptx::wgmma_commit();
-                ptx::wgmma_wait<0>();
-                ptx::fence_regs(acc);
+                for (int ks = 0; ks < KC / 8; ++ks)
+                    ptx::Wgmma<BN>::ss(acc, ad + (uint64_t)(2 * ks), bd + (uint64_t)(2 * ks), (cc | t | ks) != 0 ? 1u : 0u);
             }
-            __syncwarp();
-            if (lane == 0) ptx::mbar_arrive(&empty[s]);
+            ptx::wgmma_commit();
+            // the previous chunk's MMAs have finished reading their stage: hand it back
+            ptx::wgmma_wait<1>();
+            ptx::fence_regs(acc);
+            if (prev >= 0 && lane == 0) ptx::mbar_arrive(&empty[prev]);
+            prev = s;
             if (++s == g.stages) {
                 s = 0;
                 ph ^= 1u;
             }
         }
+        ptx::wgmma_wait<0>();
+        ptx::fence_regs(acc);
+        if (lane == 0) ptx::mbar_arrive(&empty[prev]);
 
         const int img = tile / tiles_per_img;
         const int trem = tile - img * tiles_per_img;
         const int tyi = trem / g.tiles_x, txi = trem - tyi * g.tiles_x;
         const int ty = 8 * wg + 2 * wq;
         if constexpr (!HEAD) {
+            bool ok[2];
+            size_t pix[2];
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const int y = tyi * COL_TH + ty + h, x = txi * COL_TW + g8;
-                if (y >= g.Ho || x >= g.Wo) continue;
-                const size_t pix = ((size_t)img * g.Ho + y) * g.Wo + x;
-                float *optr = out + pix * g.out_cs + g.out_co;
-                const float *rptr = res ? res + pix * g.res_cs + g.res_co : nullptr;
+                ok[h] = y < g.Ho && x < g.Wo;
+                pix[h] = ok[h] ? ((size_t)img * g.Ho + y) * g.Wo + x : 0;
+            }
+            // every residual load of the thread's two pixels is issued before any arithmetic: the epilogue waits
+            // for one load latency rather than one per 8-channel block
+            float2 rv[2][BN / 8];
+            if (res) {
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+#pragma unroll
+                    for (int j = 0; j < BN / 8; ++j)
+                        rv[h][j] = ok[h] ? __ldg(reinterpret_cast<const float2 *>(res + pix[h] * g.res_cs + g.res_co + 8 * j + 2 * t4))
+                                         : make_float2(0.f, 0.f);
+            }
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                if (!ok[h]) continue;
+                float *optr = out + pix[h] * g.out_cs + g.out_co;
 #pragma unroll
                 for (int j = 0; j < BN / 8; ++j) {
                     const int c = 8 * j + 2 * t4;
                     float2 v = make_float2(acc[4 * j + 2 * h] + s_bias[c], acc[4 * j + 2 * h + 1] + s_bias[c + 1]);
-                    if (rptr) {
-                        const float2 rv = __ldg(reinterpret_cast<const float2 *>(rptr + c));
-                        v.x += rv.x;
-                        v.y += rv.y;
+                    if (res) {
+                        v.x += rv[h][j].x;
+                        v.y += rv[h][j].y;
                     }
                     v.x = epi_act(v.x, g.act, g.round_out);
                     v.y = epi_act(v.y, g.act, g.round_out);
