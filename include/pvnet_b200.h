@@ -24,6 +24,8 @@
  *   lib/ransac_voting_gpu_layer/src/ransac_voting.cpp:61-99       the vanishing-point kernel pair
  *   tools/train_linemod.py:119-130                                UncertaintyEvalWrapper.forward (v3 + with_mean)
  *   lib/utils/extend_utils/extend_utils.py:63-114                 uncertainty_pnp (+ evaluation_utils.py:165-201)
+ *   lib/utils/extend_utils/src/nearest_neighborhood.cu:123-163    findNearestPointIdxLauncher
+ *   lib/utils/evaluation_utils.py:75-141                          the pose metrics (ADD(-S), 2D projection, 5 cm 5 deg)
  *   lib/networks/model_repository.py:64-80                        Resnet18_8s.forward
  * INTEGRATION.md shows the ctypes binding the reference's Python wrapper uses.
  */
@@ -243,6 +245,38 @@ PVNET_API int pvnet_covariance_to_weights(const float *cov, int n, float *weight
 PVNET_API int pvnet_uncertainty_pnp(const float *points_2d, const float *cov, const float *weights_2d,
                                     const float *points_3d, const double camera_matrix[9], int b, int pn,
                                     double *out_pose, int32_t *out_info, pvnet_stream_t stream);
+
+/* ------------------------------------------------------------------ pose evaluation
+ * The metrics tools/train_linemod.py:177-229 (`val()`) reports, computed per image on the host there
+ * (lib/utils/evaluation_utils.py:75-141).
+ *
+ * pvnet_find_nearest_point_idx: replaces findNearestPointIdxLauncher
+ *   (lib/utils/extend_utils/src/nearest_neighborhood.cu:123-163, called by extend_utils.py:39-60).  For every
+ *   query point the index of the nearest reference point of the same image: ref_pts f32 [b,pn1,dim], que_pts f32
+ *   [b,pn2,dim], idxs int32 [b,pn2]; dim 2 or 3.  Bit-identical to the reference kernel: the same FP32 rounding
+ *   sequence (DESIGN.md §2), a NaN distance never wins, ties keep the lowest index, and a query with no finite
+ *   distance below FLT_MAX gets 0.  (The reference's exclude_self has no caller and is not provided.)
+ *
+ * pvnet_pose_metrics: evaluation_utils.py:75-141 for a batch of images of one object.
+ *   pose_pred, pose_gt f64 [b,3,4] (R | t); model f32 [n,3] (the mesh vertices, get_ply_model);
+ *   the camera is EITHER camera_matrix, a HOST array of 9 doubles (row-major K, one for all images), OR
+ *   camera_dev, a device f64 [b,3,3] (per-image K, intri_type 'use_intrinsic'); pass NULL for the other.
+ *   out f64 [b,4] = (add, proj, trans_cm, angle_deg):
+ *     add       mean over vertices of |(R_p X + t_p) - (R_g X + t_g)|                      (:97-98,115)
+ *               symmetric != 0: ADD-S, the distance from every gt-transformed vertex to the nearest
+ *               pred-transformed vertex, searched as above on the fp32 roundings          (:125-128, :54-62)
+ *     proj      mean pixel distance of the two projections (R X + t) K^T -> [:2] / z      (:76-78)
+ *               sym_proj != 0: the nearest-point form of projection_2d_sym                (:83-86)
+ *     trans_cm  100 |t_p - t_g|;  angle_deg = deg(acos((min(tr(R_p R_g^T), 3) - 1) / 2))    (:136-140)
+ *   The fp64 operation order of the transform and the projection is fixed (eval.cu); the result is
+ *   run-to-run deterministic.  Workspace: pvnet_pose_metrics_workspace_bytes(b, n). */
+PVNET_API int pvnet_find_nearest_point_idx(const float *ref_pts, const float *que_pts, int32_t *idxs,
+                                           int b, int pn1, int pn2, int dim, pvnet_stream_t stream);
+PVNET_API int pvnet_pose_metrics_workspace_bytes(int b, int n, size_t *bytes);
+PVNET_API int pvnet_pose_metrics(const double *pose_pred, const double *pose_gt, const float *model, int n,
+                                 const double camera_matrix[9], const double *camera_dev, int b,
+                                 int symmetric, int sym_proj, double *out,
+                                 void *workspace, size_t workspace_bytes, pvnet_stream_t stream);
 
 /* The vanishing-point pair of the reference extension (ransac_voting.cpp:61-99 ->
  * ransac_voting_kernel.cu:170-260, :263-351; used by ransac_voting_vanish_point_layer,
