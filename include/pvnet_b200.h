@@ -26,6 +26,8 @@
  *   lib/utils/extend_utils/extend_utils.py:63-114                 uncertainty_pnp (+ evaluation_utils.py:165-201)
  *   lib/utils/extend_utils/src/nearest_neighborhood.cu:123-163    findNearestPointIdxLauncher
  *   lib/utils/evaluation_utils.py:75-141                          the pose metrics (ADD(-S), 2D projection, 5 cm 5 deg)
+ *   lib/utils/net_utils.py:54-80,329-348                          smooth_l1_loss, compute_precision_recall
+ *   tools/train_linemod.py:83-91                                  NetWrapper's cross-entropy (nn.CrossEntropyLoss)
  *   lib/networks/model_repository.py:64-80                        Resnet18_8s.forward
  * INTEGRATION.md shows the ctypes binding the reference's Python wrapper uses.
  */
@@ -277,6 +279,38 @@ PVNET_API int pvnet_pose_metrics(const double *pose_pred, const double *pose_gt,
                                  const double camera_matrix[9], const double *camera_dev, int b,
                                  int symmetric, int sym_proj, double *out,
                                  void *workspace, size_t workspace_bytes, pvnet_stream_t stream);
+
+/* ------------------------------------------------------------------ validation losses
+ * The per-image figures the reference's NetWrapper.forward (tools/train_linemod.py:79-91, tools/demo.py:31-43)
+ * computes from the full-resolution outputs and val() prints, in one pass over them (losses.cu, DESIGN.md §10):
+ *   loss_seg     f32 [b]  nn.CrossEntropyLoss(reduce=False) then the mean over pixels  (train_linemod.py:83,87-88):
+ *                         -log_softmax(seg)[t] in fp32 as torch computes it; t = -100 (ignore_index) adds 0 and still
+ *                         counts; any other t outside [0,C) makes the image's value NaN (torch: a device-side assert)
+ *   loss_vertex  normalize != 0: f32 [b] = sum(in) / (ver_dim * sum(w) + 1e-3) per image   (net_utils.py:73-74);
+ *                normalize == 0: f32 [b,ver_dim,h,w] contiguous, the elementwise `in_loss` (net_utils.py:64-71),
+ *                bit-identical to torch's chain of fp32 ops, with c1 = 1/sigma^2, c2 = sigma^2/2, c3 = 0.5/sigma^2
+ *                derived in double from `sigma` and rounded to float.  (The reference's reduce=True computes a mean
+ *                and discards it, :76-77; the value stays per image.)
+ *   precision, recall  f32 [b]  compute_precision_recall (net_utils.py:329-348): argmax over the C channels (first
+ *                maximum, a NaN wins), exact int64 counts tp, fp, fn, then (tp+1)/(tp+fp+1) and (tp+1)/(tp+fn+1) in
+ *                fp32: bit-identical to torch's fp32 sums while those stay below 2^24; above that the counts are
+ *                exact and rounded once, where torch's fp32 sums depend on its summation order.
+ * A NULL output skips its part.  Inputs are read in place with ELEMENT strides (the stride along w must be 1):
+ *   seg_pred f32 [b,C,h,w] (seg_strides[4]) and mask [b,h,w] (mask_strides[3], elements of mask_elem_size bytes:
+ *   8 int64, 4 int32, 1 uint8 / bool) for loss_seg / precision / recall;
+ *   vertex_pred, vertex f32 [b,ver_dim,h,w] and vertex_weights f32 [b,1,h,w] (strides[4] each) for loss_vertex.
+ * seg_pred and vertex_pred may be channel slices of one [b,C+ver_dim,h,w] tensor (Resnet18_8s.forward,
+ * model_repository.py:77-78).  Sums are fp64 / int64 in a fixed order: run-to-run identical, graph capturable.
+ * Workspace: pvnet_seg_vertex_losses_workspace_bytes(b, h, w). */
+PVNET_API int pvnet_seg_vertex_losses_workspace_bytes(int b, int h, int w, size_t *bytes);
+PVNET_API int pvnet_seg_vertex_losses(const float *seg_pred, const int64_t seg_strides[4],
+                                      const void *mask, int mask_elem_size, const int64_t mask_strides[3],
+                                      const float *vertex_pred, const int64_t pred_strides[4],
+                                      const float *vertex, const int64_t vertex_strides[4],
+                                      const float *vertex_weights, const int64_t weight_strides[4],
+                                      int b, int h, int w, int C, int ver_dim, double sigma, int normalize,
+                                      float *loss_seg, float *loss_vertex, float *precision, float *recall,
+                                      void *workspace, size_t workspace_bytes, pvnet_stream_t stream);
 
 /* The vanishing-point pair of the reference extension (ransac_voting.cpp:61-99 ->
  * ransac_voting_kernel.cu:170-260, :263-351; used by ransac_voting_vanish_point_layer,

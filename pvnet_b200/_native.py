@@ -57,6 +57,11 @@ SIGNATURES = {
     "pvnet_pose_metrics_workspace_bytes": (c_int, [c_int, c_int, ctypes.POINTER(c_size_t)]),
     "pvnet_pose_metrics": (c_int, [c_void_p, c_void_p, c_void_p, c_int, ctypes.POINTER(ctypes.c_double), c_void_p,
                                    c_int, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "pvnet_seg_vertex_losses_workspace_bytes": (c_int, [c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
+    "pvnet_seg_vertex_losses": (c_int, [c_void_p, c_int64_p, c_void_p, c_int, c_int64_p, c_void_p, c_int64_p,
+                                        c_void_p, c_int64_p, c_void_p, c_int64_p, c_int, c_int, c_int, c_int, c_int,
+                                        ctypes.c_double, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                                        c_void_p, c_size_t, c_void_p]),
     "pvnet_generate_hypothesis": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "pvnet_voting_for_hypothesis": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float,
                                             c_void_p]),
