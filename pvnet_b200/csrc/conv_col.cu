@@ -14,8 +14,9 @@
 //     Both operands are shared-memory descriptors, and one chunk's MMAs stay in flight while the
 //     previous chunk's stage is released;
 //   * optional fused head (convraw.3 1x1 + bias + argmax) in the epilogue: the activated 128 x 32 tile
-//     is already in the register layout of a wgmma A operand, so the head is one more MMA, and the
-//     reference's NCHW output is written directly -- the [b,H,W,32] intermediate never exists;
+//     is already in the register layout of a wgmma A operand, so the head is one more MMA; its output is staged
+//     in shared memory and stored by the producer warpgroup's otherwise idle warps while the next tile's MMAs
+//     run -- the [b,H,W,32] intermediate never exists;
 //   * optional fused bilinear x2 upsampling of convraw.0's first input (the producer warps interpolate
 //     it into the operand stages instead of TMA loading it).
 #include "conv_tc.cuh"
@@ -34,6 +35,19 @@ namespace {
 constexpr int COL_TH = 16, COL_TW = 8;
 constexpr int COL_THREADS = 384;       // consumer warpgroups 0 and 1 (64 tile pixels each), producer warpgroup 2
 constexpr int HEAD_MAX = 64;
+
+// Fused head: one tile's output (128 pixels x head_cout fp32, then 128 argmax bytes) is staged in shared memory,
+// double-buffered, and copied to global memory by warps that issue no MMAs.  Pixel-major staging keeps a pixel's
+// channels at a pitch of 8 mod 16 floats, so the consumers' float2 writes (lane = pixel g8, channel pair t4) hit
+// four disjoint 8-bank windows per half-warp; NCHW staging is [cout][16][8] with a channel pitch of 4 mod 16
+// floats, so the scalar writes of channels 2t4 and 2t4+1 spread the four t4 lanes 8 banks apart.
+__host__ __device__ constexpr int head_pitch(int hc) { return hc <= 8 ? 8 : (hc <= 24 ? 24 : 40); }
+constexpr int HEAD_CPITCH = COL_TH * COL_TW + 4;
+__host__ __device__ constexpr int head_stage_floats(int hc)
+{
+    return COL_TH * COL_TW * head_pitch(hc) > hc * HEAD_CPITCH ? COL_TH * COL_TW * head_pitch(hc) : hc * HEAD_CPITCH;
+}
+__host__ __device__ constexpr int head_stage_bytes(int hc) { return (head_stage_floats(hc) * 4 + COL_TH * COL_TW + 127) & ~127; }
 
 struct ColGeom {
     int Ho, Wo, tiles_x, tiles_y, total_tiles;
@@ -170,36 +184,104 @@ __device__ __forceinline__ void up_fill_chunk(const ColUp &u, const ColGeom &g, 
     up_fill_rows<0, ROWS>(base, rstride, olo, ohi, R0, u.h, act, vx, w1x_, u.zero, wa_l, wb_l, wc_l, sbase, c, hf);
 }
 
+// Copies one staged head tile (see head_pitch) to head_out and mask; thread `tid` of `nthr`.  The tile is 32*hc
+// units of four floats: pixel-major, 2*hc of them cover one tile row's contiguous run of 8*hc floats; NCHW, two
+// cover one channel's 8 pixels of a tile row.  A unit is one 16-byte store when the layout keeps it aligned and
+// inside one pixel (pixel-major) or inside the image (NCHW), otherwise four scalar stores.  sv and sm are the
+// shared-memory addresses of the staged values and argmax bytes.
+__device__ __forceinline__ void head_store_tile(const ColGeom &g, uint32_t sv, uint32_t sm, float *head_out, void *mask,
+                                                int img, int y0, int x0, int tid, int nthr)
+{
+    const int hc = g.head_cout, pp = head_pitch(hc);
+    const int nx = min(COL_TW, g.Wo - x0), ny = min(COL_TH, g.Ho - y0);
+    const size_t npix = (size_t)g.Ho * g.Wo;
+    const bool vec = (reinterpret_cast<uintptr_t>(head_out) & 15) == 0 && (g.head_nhwc ? hc % 4 == 0 : g.Wo % 4 == 0);
+    for (int u = tid; u < 32 * hc; u += nthr) {
+        if (g.head_nhwc) {
+            const int r = u / (2 * hc), e0 = 4 * (u - r * 2 * hc);
+            if (r >= ny) continue;
+            float *dst = head_out + (((size_t)img * g.Ho + y0 + r) * g.Wo + x0) * hc + e0;
+            if (vec) {
+                const int col = e0 / hc;
+                if (col < nx)
+                    *reinterpret_cast<float4 *>(dst) = ptx::lds128(sv + 4u * (uint32_t)((r * COL_TW + col) * pp + e0 - col * hc));
+            } else {
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    const int col = (e0 + i) / hc;
+                    if (col < nx) dst[i] = ptx::lds32(sv + 4u * (uint32_t)((r * COL_TW + col) * pp + e0 + i - col * hc));
+                }
+            }
+        } else {
+            const int co = u >> 5, r = (u >> 1) & 15, xo = 4 * (u & 1);
+            if (r >= ny) continue;
+            float *dst = head_out + ((size_t)img * hc + co) * npix + (size_t)(y0 + r) * g.Wo + x0 + xo;
+            const uint32_t src = sv + 4u * (uint32_t)(co * HEAD_CPITCH + r * COL_TW + xo);
+            if (vec) {
+                if (xo < nx) *reinterpret_cast<float4 *>(dst) = ptx::lds128(src);
+            } else {
+#pragma unroll
+                for (int i = 0; i < 4; ++i)
+                    if (xo + i < nx) dst[i] = ptx::lds32(src + 4u * i);
+            }
+        }
+    }
+    if (!mask) return;
+    for (int p = tid; p < COL_TH * COL_TW; p += nthr) {
+        const int r = p / COL_TW, c = p % COL_TW;
+        if (r >= ny || c >= nx) continue;
+        const size_t pix = ((size_t)img * g.Ho + y0 + r) * g.Wo + x0 + c;
+        const uint32_t v = ptx::lds8(sm + (uint32_t)p);
+        if (g.mask_esz == 8) reinterpret_cast<long long *>(mask)[pix] = v;
+        else reinterpret_cast<unsigned char *>(mask)[pix] = (unsigned char)v;
+    }
+}
+
 
 
 // BN = Cout (32 or 64); KC channels per chunk (rows of KC*4 bytes, swizzled by the same amount).
-template <int KC, bool HEAD, int KH, bool UP, int BN>
+// WIDE (convraw.0 with a 32-channel first source): the four 8-channel chunks of the first source are loaded as one
+// 128-byte-swizzled box, with their weights as 128-byte-swizzled [32][32] tiles, and the MMAs still run chunk by
+// chunk, tap by tap, so every output sums the same products in the same order as with 8-channel boxes.  The
+// 32-byte-swizzled operands of 8-channel chunks ran the same MMAs at about half the rate (DESIGN.md section 6).
+template <int KC, bool HEAD, int KH, bool UP, int BN, bool WIDE = false>
 __global__ void __launch_bounds__(COL_THREADS, 1)
     k_conv_col(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
-               const __grid_constant__ CUtensorMap tmB, const __grid_constant__ ColGeom g,
+               const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmBw, const __grid_constant__ ColGeom g,
                const float *__restrict__ bias, const float *__restrict__ res, float *__restrict__ out,
                const float *__restrict__ head_w, const float *__restrict__ head_b, float *__restrict__ head_out,
                void *__restrict__ mask, const ColUp up)
 {
     static_assert(!UP || (HEAD && KC == 8 && KH == 3), "fused upsampling: convraw.0 form only");
     static_assert(!HEAD || BN == 32, "fused head: 32 input channels");
+    static_assert(!WIDE || (HEAD && !UP && KC == 8 && KH == 3), "wide first source: convraw.0 form only");
     constexpr int ROWB = KC * 4;                       // bytes per K-major row
     constexpr int B_TILE = BN * ROWB;                  // one [BN][KC] weight tile (a multiple of 1024 bytes)
     constexpr int PITCH = COL_TW + KH - 1;             // box pitch in pixels (= shared-memory rows)
     constexpr int A_BOX = (COL_TH + KH - 1) * PITCH * ROWB;
     constexpr int A_BYTES = (A_BOX + 1023) & ~1023;    // stages stay 1024-byte aligned
+    // WIDE: the first source's 32 channels arrive as one box of 128-byte rows (WIDE_BOX), the second source's 8 as
+    // a box of 32-byte rows; a stage is sized for the wide box
+    constexpr int WIDE_BOX = (COL_TH + KH - 1) * PITCH * 128;
+    constexpr int WIDE_BYTES = (WIDE_BOX + 1023) & ~1023;
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     const int n_btiles = KH * KH * g.cin_chunks;
-    const int stage_bytes = A_BYTES + (g.resident ? 0 : KH * KH * B_TILE);
+    const int n_loads = WIDE ? 2 : g.cin_chunks;         // operand boxes per tile (one ring stage each)
+    const int stage_bytes = WIDE ? WIDE_BYTES : A_BYTES + (g.resident ? 0 : KH * KH * B_TILE);
     uint8_t *sB = smem;
     uint8_t *sA = smem + (g.resident ? (size_t)n_btiles * B_TILE : 0);
     uint8_t *sH = sA + (size_t)g.stages * stage_bytes;            // HEAD: head weights, 32 x 32, 128-byte swizzle
-    uint64_t *wfull = reinterpret_cast<uint64_t *>(sH + (HEAD ? 4096 : 0));
+    uint8_t *sHS = sH + (HEAD ? 4096 : 0);                        // HEAD: two head output staging buffers
+    const int hs_bytes = HEAD ? head_stage_bytes(g.head_cout) : 0;
+    uint64_t *wfull = reinterpret_cast<uint64_t *>(sHS + 2 * hs_bytes);
     uint64_t *full = wfull + 1;
     uint64_t *empty = full + g.stages;
-    float *s_bias = reinterpret_cast<float *>(empty + g.stages);  // [BN]
+    uint64_t *hstaged = empty + g.stages;                         // HEAD: [2] staging buffer written by the consumers
+    uint64_t *hfree = hstaged + 2;                                // HEAD: [2] staging buffer copied out by the store warps
+    float *s_bias = reinterpret_cast<float *>(empty + g.stages + (HEAD ? 4 : 0));  // [BN]
     float *s_head = s_bias + 64;                                  // [32]
+    constexpr int STORE_THREADS = 96;                             // HEAD && !UP: producer warps 9-11 store the head output
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (threadIdx.x == 0) {
@@ -208,6 +290,11 @@ __global__ void __launch_bounds__(COL_THREADS, 1)
             ptx::mbar_init(&full[s], 1);
             ptx::mbar_init(&empty[s], 8);              // one arrive per consumer warp
         }
+        if (HEAD && !UP)
+            for (int b = 0; b < 2; ++b) {
+                ptx::mbar_init(&hstaged[b], 256);      // every consumer thread, after its own shared-memory writes
+                ptx::mbar_init(&hfree[b], STORE_THREADS);
+            }
         ptx::fence_barrier_init();
     }
     for (int i = threadIdx.x; i < BN; i += blockDim.x) s_bias[i] = bias[i];
@@ -231,11 +318,31 @@ __global__ void __launch_bounds__(COL_THREADS, 1)
         // producer warpgroup: warp 8 lane 0 issues the TMA loads; with UP, warp 8 + q also interpolates chunk q
         const int pw = warp - 8;
         if (pw == 0 && lane == 0 && g.resident) {
-            // all weights, once: tile t = cc*KH*KH + kh*KH + kw <- packed [Cout][kh][kw][cin]
+            // all weights, once: tile t = cc*KH*KH + kh*KH + kw <- packed [Cout][kh][kw][cin]; WIDE: the first
+            // source's chunks as KH*KH [BN][32] tiles of 128-byte rows, in the same bytes
             ptx::mbar_arrive_expect_tx(wfull, (uint32_t)(n_btiles * B_TILE));
-            for (int cc = 0; cc < g.cin_chunks; ++cc)
+            for (int cc = WIDE ? g.split_chunk : 0; cc < g.cin_chunks; ++cc)
                 for (int t = 0; t < KH * KH; ++t)
                     ptx::tma_load_2d(sB + (size_t)(cc * KH * KH + t) * B_TILE, &tmB, wfull, t * g.cin_pad + cc * KC, 0);
+            if (WIDE)
+                for (int t = 0; t < KH * KH; ++t) ptx::tma_load_2d(sB + (size_t)t * BN * 128, &tmBw, wfull, t * g.cin_pad, 0);
+        }
+        if (HEAD && !UP && pw != 0) {
+            // store warps: the CTA's tiles in the consumers' order, buffer it & 1, the ring's parity discipline
+            const int tid = threadIdx.x - 9 * 32;
+            int it = 0;
+            for (int tile = blockIdx.x; tile < g.total_tiles; tile += gridDim.x, ++it) {
+                const int b = it & 1;
+                const int img = tile / tiles_per_img;
+                const int trem = tile - img * tiles_per_img;
+                const int tyi = trem / g.tiles_x, txi = trem - tyi * g.tiles_x;
+                const uint32_t buf = ptx::smem_u32(sHS) + (uint32_t)(b * hs_bytes);
+                ptx::mbar_wait(&hstaged[b], (uint32_t)(it >> 1) & 1u);
+                head_store_tile(g, buf, buf + 4u * (uint32_t)head_stage_floats(g.head_cout), head_out, mask, img, tyi * COL_TH,
+                                txi * COL_TW, tid, STORE_THREADS);
+                ptx::mbar_arrive(&hfree[b]);
+            }
+            return;
         }
         if (!UP && pw != 0) return;
         int s = 0;
@@ -246,9 +353,16 @@ __global__ void __launch_bounds__(COL_THREADS, 1)
             const int trem = tile - img * tiles_per_img;
             const int tyi = trem / g.tiles_x, txi = trem - tyi * g.tiles_x;
             const int y0 = tyi * COL_TH, x0 = txi * COL_TW;
-            for (int cc = 0; cc < g.cin_chunks; ++cc) {
+            for (int cc = 0; cc < n_loads; ++cc) {
                 uint8_t *st = sA + (size_t)s * stage_bytes;
-                if (UP && cc < g.split_chunk) {
+                if (WIDE) {
+                    if (pw == 0 && lane == 0) {
+                        ptx::mbar_wait(&empty[s], ph ^ 1u);
+                        ptx::mbar_arrive_expect_tx(&full[s], (uint32_t)(cc == 0 ? WIDE_BOX : A_BOX));
+                        ptx::tma_load_4d(st, cc == 0 ? &tmA : &tmA2, &full[s], 0, x0 - g.pad_l, y0 - g.pad_t, img);
+                    }
+                    __syncwarp();
+                } else if (UP && cc < g.split_chunk) {
                     if (pw == cc) {
                         ptx::mbar_wait(&empty[s], ph ^ 1u);
                         up_fill_chunk(up, g, img, y0, x0, cc, lane, ptx::smem_u32(st));
@@ -290,27 +404,42 @@ __global__ void __launch_bounds__(COL_THREADS, 1)
     if (g.resident) ptx::mbar_wait(wfull, 0);
     int s = 0;
     uint32_t ph = 0;
-    for (int tile = blockIdx.x; tile < g.total_tiles; tile += gridDim.x) {
+    int it = 0;
+    for (int tile = blockIdx.x; tile < g.total_tiles; tile += gridDim.x, ++it) {
         float acc[BN / 2];
 #pragma unroll
         for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
         int prev = -1;
-        for (int cc = 0; cc < g.cin_chunks; ++cc) {
+        for (int cc = 0; cc < n_loads; ++cc) {
             ptx::mbar_wait(&full[s], ph);
             const uint32_t a0 = sA_u + (uint32_t)s * (uint32_t)stage_bytes;
-            const uint32_t b0 = g.resident ? sB_u + (uint32_t)(cc * KH * KH * B_TILE) : a0 + (uint32_t)A_BYTES;
-            const uint64_t ad0 = ptx::make_kmajor_desc(a0 + (uint32_t)(8 * wg * PITCH * ROWB), ROWB, PITCH * ROWB);
-            const uint64_t bd0 = ptx::make_kmajor_desc(b0, ROWB);
-            // the chunk's taps, then 8-channel K steps, into one accumulator; descriptor start addresses count
-            // 16-byte units
             ptx::wgmma_fence();
+            if (WIDE && cc == 0) {
+                // the first source's four 8-channel chunks (32-byte K steps inside the 128-byte rows), each over
+                // all taps: the order of the 8-channel-box form
+                const uint64_t ad0 = ptx::make_kmajor_desc(a0 + (uint32_t)(8 * wg * PITCH * 128), 128, PITCH * 128);
+                const uint64_t bd0 = ptx::make_kmajor_desc(sB_u, 128);
 #pragma unroll
-            for (int t = 0; t < KH * KH; ++t) {
-                const uint64_t ad = ad0 + (uint64_t)(((t / KH) * PITCH + t % KH) * ROWB / 16);
-                const uint64_t bd = bd0 + (uint64_t)(t * B_TILE / 16);
+                for (int ks = 0; ks < 4; ++ks)
 #pragma unroll
-                for (int ks = 0; ks < KC / 8; ++ks)
-                    ptx::Wgmma<BN>::ss(acc, ad + (uint64_t)(2 * ks), bd + (uint64_t)(2 * ks), (cc | t | ks) != 0 ? 1u : 0u);
+                    for (int t = 0; t < KH * KH; ++t)
+                        ptx::Wgmma<BN>::ss(acc, ad0 + (uint64_t)(((t / KH) * PITCH + t % KH) * 128 / 16 + 2 * ks),
+                                           bd0 + (uint64_t)(t * (BN * 128) / 16 + 2 * ks), (t | ks) != 0 ? 1u : 0u);
+            } else {
+                const int c8 = WIDE ? g.split_chunk : cc;      // the chunk's index in 8-channel units
+                const uint32_t b0 = g.resident ? sB_u + (uint32_t)(c8 * KH * KH * B_TILE) : a0 + (uint32_t)A_BYTES;
+                const uint64_t ad0 = ptx::make_kmajor_desc(a0 + (uint32_t)(8 * wg * PITCH * ROWB), ROWB, PITCH * ROWB);
+                const uint64_t bd0 = ptx::make_kmajor_desc(b0, ROWB);
+                // the chunk's taps, then 8-channel K steps, into one accumulator; descriptor start addresses count
+                // 16-byte units
+#pragma unroll
+                for (int t = 0; t < KH * KH; ++t) {
+                    const uint64_t ad = ad0 + (uint64_t)(((t / KH) * PITCH + t % KH) * ROWB / 16);
+                    const uint64_t bd = bd0 + (uint64_t)(t * B_TILE / 16);
+#pragma unroll
+                    for (int ks = 0; ks < KC / 8; ++ks)
+                        ptx::Wgmma<BN>::ss(acc, ad + (uint64_t)(2 * ks), bd + (uint64_t)(2 * ks), (c8 | t | ks) != 0 ? 1u : 0u);
+                }
             }
             ptx::wgmma_commit();
             // the previous chunk's MMAs have finished reading their stage: hand it back
@@ -391,29 +520,38 @@ __global__ void __launch_bounds__(COL_THREADS, 1)
             ptx::wgmma_commit();
             ptx::wgmma_wait<0>();
             ptx::fence_regs(hacc);
+            // into staging buffer it & 1 (head_pitch), once the store side has copied out what it held two tiles ago
+            const int hc = g.head_cout, pp = head_pitch(hc);
+            const uint32_t sv = ptx::smem_u32(sHS) + (uint32_t)((it & 1) * hs_bytes);
+            const uint32_t sm = sv + 4u * (uint32_t)head_stage_floats(hc);
+            if (!UP) ptx::mbar_wait(&hfree[it & 1], ((uint32_t)(it >> 1) & 1u) ^ 1u);
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
-                const int y = tyi * COL_TH + ty + h, x = txi * COL_TW + g8;
-                const bool valid = y < g.Ho && x < g.Wo;
-                const size_t pix = ((size_t)img * g.Ho + y) * g.Wo + x;
-                const size_t npix = (size_t)g.Ho * g.Wo;
+                const uint32_t p = (uint32_t)((ty + h) * COL_TW + g8);
                 float best = -INFINITY;
                 int best_c = 0;
 #pragma unroll
-                for (int j = 0; j < 4; ++j)
+                for (int j = 0; j < 4; ++j) {
+                    const int co = 8 * j + 2 * t4;
+                    float val[2];
 #pragma unroll
                     for (int e = 0; e < 2; ++e) {
-                        const int co = 8 * j + 2 * t4 + e;
-                        const float val = hacc[4 * j + 2 * h + e] + s_head[co];
-                        if (co < g.head_seg && val > best) {
-                            best = val;
-                            best_c = co;
-                        }
-                        if (valid && co < g.head_cout) {
-                            if (g.head_nhwc) head_out[pix * (size_t)g.head_cout + co] = val;
-                            else head_out[((size_t)img * g.head_cout + co) * npix + (size_t)y * g.Wo + x] = val;
+                        val[e] = hacc[4 * j + 2 * h + e] + s_head[co + e];
+                        if (co + e < g.head_seg && val[e] > best) {
+                            best = val[e];
+                            best_c = co + e;
                         }
                     }
+                    // channel co + 1 == hc (odd hc) lands in the pixel's padding
+                    if (co < hc) {
+                        if (g.head_nhwc) {
+                            ptx::sts64(sv + 4u * (p * pp + co), make_float2(val[0], val[1]));
+                        } else {
+                            ptx::sts32(sv + 4u * (co * HEAD_CPITCH + p), val[0]);
+                            if (co + 1 < hc) ptx::sts32(sv + 4u * ((co + 1) * HEAD_CPITCH + p), val[1]);
+                        }
+                    }
+                }
                 // torch.argmax over the four lanes of the pixel: the largest value, the lowest channel among equals
 #pragma unroll
                 for (int o = 1; o < 4; o <<= 1) {
@@ -424,19 +562,24 @@ __global__ void __launch_bounds__(COL_THREADS, 1)
                         best_c = oc;
                     }
                 }
-                if (valid && mask && t4 == 0) {
-                    if (g.mask_esz == 8) reinterpret_cast<long long *>(mask)[pix] = best_c;
-                    else reinterpret_cast<unsigned char *>(mask)[pix] = (unsigned char)best_c;
-                }
+                if (t4 == 0) ptx::sts8(sm + p, (uint32_t)best_c);
+            }
+            if (!UP) {
+                ptx::mbar_arrive(&hstaged[it & 1]);
+            } else {
+                // the producer warps interpolate: the consumers copy the tile out themselves.  Buffer it & 1 is
+                // written again two tiles later, after every consumer has passed the next tile's barrier.
+                ptx::named_bar_sync(1, 256);
+                head_store_tile(g, sv, sm, head_out, mask, img, tyi * COL_TH, txi * COL_TW, threadIdx.x, 256);
             }
         }
     }
 }
 
 struct ColPlan {
-    CUtensorMap tmA, tmA2, tmB;
+    CUtensorMap tmA, tmA2, tmB, tmBw;
     ColGeom g;
-    int kc, ksize, head, up, bn;
+    int kc, ksize, head, up, bn, wide;
     ColUp cup;
     unsigned grid;
     size_t smem;
@@ -462,19 +605,20 @@ size_t col_smem(int kc, int ksize, int cin_chunks, int bn, int stages, bool head
            (size_t)(1 + 2 * stages) * 8 + (64 + 32) * 4;
 }
 
-template <int KC, bool HEAD, int KH, bool UP, int BN>
+template <int KC, bool HEAD, int KH, bool UP, int BN, bool WIDE = false>
 int col_launch(const ColPlan &p, cudaStream_t s)
 {
     // the instantiation must be the plan's: weight boxes, barrier byte counts and stores are sized by BN
-    if (p.bn != BN || p.kc != KC || p.ksize != KH || p.head != (HEAD ? 1 : 0) || p.up != (UP ? 1 : 0)) {
+    if (p.bn != BN || p.kc != KC || p.ksize != KH || p.head != (HEAD ? 1 : 0) || p.up != (UP ? 1 : 0) ||
+        p.wide != (WIDE ? 1 : 0)) {
         set_error("conv(col): no kernel instantiation for this plan (Cout %d, chunk %d, ksize %d)", p.bn, p.kc, p.ksize);
         return PVNET_E_STATE;
     }
-    auto fn = k_conv_col<KC, HEAD, KH, UP, BN>;
+    auto fn = k_conv_col<KC, HEAD, KH, UP, BN, WIDE>;
     const cudaError_t attr_err = ensure_max_smem((const void *)fn, (int)SMEM_LIMIT);
     PV_CUDA(attr_err);
     const HeadDesc &h = p.hd;
-    fn<<<p.grid, COL_THREADS, p.smem, s>>>(p.tmA, p.tmA2, p.tmB, p.g, p.bias, p.res, p.out, p.head ? h.w : nullptr,
+    fn<<<p.grid, COL_THREADS, p.smem, s>>>(p.tmA, p.tmA2, p.tmB, p.tmBw, p.g, p.bias, p.res, p.out, p.head ? h.w : nullptr,
                                            p.head ? h.bias : nullptr, p.head ? h.out_nchw : nullptr,
                                            p.head ? h.mask : nullptr, p.cup);
     PV_LAUNCHED("k_conv_col");
@@ -542,18 +686,28 @@ int conv_col_plan_at(const ConvDesc &d, const HeadDesc *head, void *storage)
     // Resident weights whenever at least 2 A stages (one channel chunk with all its taps each) still
     // fit next to them; otherwise the KH*KW weight tiles of a chunk travel with its A box.
     const bool hd = head != nullptr;
+    // the head's two output staging buffers and their four barriers
+    const size_t hs = hd ? 2 * (size_t)head_stage_bytes(head->cout) + 4 * 8 : 0;
+    // convraw.0's 32 + 8 channel form loads its first source as one box of 128-byte rows (WIDE in k_conv_col);
+    // its stages then hold that box instead of an 8-channel one
+    bool wide = hd && !d.up_src && d.in2 && d.Cin == 32 && d.Cin2 == 8 && kc == 8 && d.ksize == 3;
+    const size_t wx = col_smem(32, 3, 0, 0, 1, false, false) - col_smem(8, 3, 0, 0, 1, false, false);
     int stages = 8;
     bool resident = true;
-    while (stages > 2 && col_smem(kc, d.ksize, g.cin_chunks, d.Cout, stages, hd, true) > SMEM_LIMIT) --stages;
-    if (col_smem(kc, d.ksize, g.cin_chunks, d.Cout, stages, hd, true) > SMEM_LIMIT) {
+    while (stages > 2 && col_smem(kc, d.ksize, g.cin_chunks, d.Cout, stages, hd, true) + hs + (wide ? stages * wx : 0) > SMEM_LIMIT)
+        --stages;
+    if (col_smem(kc, d.ksize, g.cin_chunks, d.Cout, stages, hd, true) + hs + (wide ? stages * wx : 0) > SMEM_LIMIT) {
+        wide = false;
         resident = false;
         stages = 8;
-        while (stages > 2 && col_smem(kc, d.ksize, g.cin_chunks, d.Cout, stages, hd, false) > SMEM_LIMIT) --stages;
+        while (stages > 2 && col_smem(kc, d.ksize, g.cin_chunks, d.Cout, stages, hd, false) + hs > SMEM_LIMIT) --stages;
     }
     PV_CHECK_ARG(!d.up_src || resident, "conv(col): fused upsampling needs resident weights");
     g.stages = stages;
     g.resident = resident ? 1 : 0;
-    p->smem = col_smem(kc, d.ksize, g.cin_chunks, d.Cout, stages, hd, resident);
+    p->smem = col_smem(kc, d.ksize, g.cin_chunks, d.Cout, stages, hd, resident) + hs + (wide ? stages * wx : 0);
+    p->wide = wide ? 1 : 0;
+    PV_CHECK_ARG(p->smem <= SMEM_LIMIT, "conv(col): layer does not fit in shared memory");
     p->kc = kc;
     p->ksize = d.ksize;
     p->bn = d.Cout;
@@ -565,8 +719,9 @@ int conv_col_plan_at(const ConvDesc &d, const HeadDesc *head, void *storage)
         cuuint64_t dims[4] = {(cuuint64_t)d.Cin, (cuuint64_t)d.W, (cuuint64_t)d.H, (cuuint64_t)d.b};
         cuuint64_t strides[3] = {(cuuint64_t)d.in_cs * 4, (cuuint64_t)d.W * d.in_cs * 4,
                                  (cuuint64_t)d.H * d.W * d.in_cs * 4};
-        cuuint32_t box[4] = {(cuuint32_t)kc, (cuuint32_t)(COL_TW + d.ksize - 1), (cuuint32_t)(COL_TH + d.ksize - 1), 1};
-        int rc = tma_encode(&p->tmA, base, 4, dims, strides, box, kc * 4);
+        const int akc = wide ? 32 : kc;
+        cuuint32_t box[4] = {(cuuint32_t)akc, (cuuint32_t)(COL_TW + d.ksize - 1), (cuuint32_t)(COL_TH + d.ksize - 1), 1};
+        int rc = tma_encode(&p->tmA, base, 4, dims, strides, box, akc * 4);
         if (rc) return rc;
         p->tmA2 = p->tmA;
     }
@@ -586,6 +741,11 @@ int conv_col_plan_at(const ConvDesc &d, const HeadDesc *head, void *storage)
         cuuint32_t box[2] = {(cuuint32_t)kc, (cuuint32_t)d.Cout};
         int rc = tma_encode(&p->tmB, d.w, 2, dims, strides, box, kc * 4);
         if (rc) return rc;
+        p->tmBw = p->tmB;
+        if (wide) {
+            box[0] = 32;
+            if ((rc = tma_encode(&p->tmBw, d.w, 2, dims, strides, box, 128))) return rc;
+        }
     }
     PV_CHECK_ARG(!head || (uintptr_t)head->w % 16 == 0, "conv(col): head weights must be 16-byte aligned");
     long long grid = (long long)sm_count();
@@ -611,6 +771,7 @@ int conv_col_launch_at(const void *storage, cudaStream_t s)
 {
     const ColPlan &p = *static_cast<const ColPlan *>(storage);
     if (p.up) return col_launch<8, true, 3, true, 32>(p, s);
+    if (p.wide) return col_launch<8, true, 3, false, 32, true>(p, s);
     if (p.head) return p.kc == 32 ? col_launch<32, true, 3, false, 32>(p, s) : col_launch<8, true, 3, false, 32>(p, s);
     const bool n64 = p.bn == 64;
     if (p.ksize == 4) return n64 ? col_launch<16, false, 4, false, 64>(p, s) : col_launch<16, false, 4, false, 32>(p, s);

@@ -114,6 +114,24 @@ __device__ __forceinline__ float4 lds128(uint32_t addr)
     asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr) : "memory");
     return v;
 }
+__device__ __forceinline__ void sts64(uint32_t addr, float2 v)
+{
+    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(v.x), "f"(v.y) : "memory");
+}
+__device__ __forceinline__ void sts32(uint32_t addr, float v) { asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(v) : "memory"); }
+__device__ __forceinline__ float lds32(uint32_t addr)
+{
+    float v;
+    asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr) : "memory");
+    return v;
+}
+__device__ __forceinline__ void sts8(uint32_t addr, uint32_t v) { asm volatile("st.shared.u8 [%0], %1;" ::"r"(addr), "r"(v) : "memory"); }
+__device__ __forceinline__ uint32_t lds8(uint32_t addr)
+{
+    uint32_t v;
+    asm volatile("ld.shared.u8 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
+    return v;
+}
 __device__ __forceinline__ void tma_store_4d_u32(const CUtensorMap *m, uint32_t smem_src, int c0, int c1, int c2, int c3)
 {
     asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(
