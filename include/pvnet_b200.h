@@ -26,6 +26,8 @@
  *   lib/utils/extend_utils/extend_utils.py:63-114                 uncertainty_pnp (+ evaluation_utils.py:165-201)
  *   lib/utils/extend_utils/src/nearest_neighborhood.cu:123-163    findNearestPointIdxLauncher
  *   lib/utils/evaluation_utils.py:75-141                          the pose metrics (ADD(-S), 2D projection, 5 cm 5 deg)
+ *   lib/utils/extend_utils/src/farthest_point_sampling.cpp        farthest_point_sampling[_init_center]
+ *   lib/utils/extend_utils/src/mesh_rasterization.cpp             mesh_binary_rasterization
  *   lib/utils/net_utils.py:54-80,329-348                          smooth_l1_loss, compute_precision_recall
  *   tools/train_linemod.py:83-91                                  NetWrapper's cross-entropy (nn.CrossEntropyLoss)
  *   lib/networks/model_repository.py:64-80                        Resnet18_8s.forward
@@ -311,6 +313,28 @@ PVNET_API int pvnet_seg_vertex_losses(const float *seg_pred, const int64_t seg_s
                                       int b, int h, int w, int C, int ver_dim, double sigma, int normalize,
                                       float *loss_seg, float *loss_vertex, float *precision, float *recall,
                                       void *workspace, size_t workspace_bytes, pvnet_stream_t stream);
+
+/* ------------------------------------------------------------------ dataset tooling (extend.cu, DESIGN.md §11)
+ * pvnet_farthest_point_sampling: replaces farthest_point_sampling / farthest_point_sampling_init_center
+ *   (lib/utils/extend_utils/src/farthest_point_sampling.cpp:77-105,122-160,166-204, called by extend_utils.py:22-37).
+ *   pts f32 [b,pn,3]; idxs int32 [b,sn] receives each cloud's sample indices in selection order.
+ *   start int32 [b] (device) gives each cloud's first index, taken modulo pn as the reference takes rand() % pn;
+ *   start == NULL is the init_center mode: the first index is the point farthest from the bounding-box centre.
+ *   Bit-identical to the reference's binary: the same FP32 sequence, ties keep the lowest index, NaN distances
+ *   never win, and a round where no unselected point has min_dist > 0 yields index 0 (even if already selected).
+ *   sn == 0 does nothing.  Workspace: pvnet_farthest_point_sampling_workspace_bytes(b, pn) (0 for clouds that fit
+ *   on chip; workspace may then be NULL).
+ *
+ * pvnet_mesh_binary_rasterization: replaces mesh_binary_rasterization (src/mesh_rasterization.cpp:43-71, called by
+ *   extend_utils.py:7-20).  triangles f32 [b,tn,3,2] (x, y in pixels); mask uint8 [b,h,w] is overwritten with 0/1,
+ *   bit-identical to the reference.  Triangles whose box the reference cannot convert to int (a bound of 2^31 or
+ *   more in magnitude) are skipped: they cover no in-range pixel.  h, w >= 2; tn may be 0. */
+PVNET_API int pvnet_farthest_point_sampling_workspace_bytes(int b, int pn, size_t *bytes);
+PVNET_API int pvnet_farthest_point_sampling(const float *pts, const int32_t *start, int b, int pn, int sn,
+                                            int32_t *idxs, void *workspace, size_t workspace_bytes,
+                                            pvnet_stream_t stream);
+PVNET_API int pvnet_mesh_binary_rasterization(const float *triangles, int b, int tn, int h, int w, uint8_t *mask,
+                                              pvnet_stream_t stream);
 
 /* The vanishing-point pair of the reference extension (ransac_voting.cpp:61-99 ->
  * ransac_voting_kernel.cu:170-260, :263-351; used by ransac_voting_vanish_point_layer,

@@ -156,6 +156,25 @@ __device__ __forceinline__ void cluster_sync()
 {
     asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
+// the shared::cluster address of `p`'s shared-memory offset in CTA `rank` of the cluster (DSMEM)
+__device__ __forceinline__ uint32_t mapa(const void *p, uint32_t rank)
+{
+    uint32_t r;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_u32(p)), "r"(rank));
+    return r;
+}
+__device__ __forceinline__ float ld_cluster_f32(uint32_t addr)
+{
+    float v;
+    asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(v) : "r"(addr) : "memory");
+    return v;
+}
+__device__ __forceinline__ unsigned long long ld_cluster_u64(uint32_t addr)
+{
+    unsigned long long v;
+    asm volatile("ld.shared::cluster.u64 %0, [%1];" : "=l"(v) : "r"(addr) : "memory");
+    return v;
+}
 // arrive on the mbarrier at the same shared-memory offset in CTA `rank` of the cluster
 __device__ __forceinline__ void mbar_arrive_cluster(uint64_t *bar, uint32_t rank)
 {

@@ -1,4 +1,10 @@
-"""Device-side uncertainty-driven PnP: the reference's `uncertainty_pnp`
+"""The reference's lib/utils/extend_utils on the device.
+
+Farthest point sampling and binary mesh rasterisation (`farthest_point_sampling`, `mesh_binary_rasterization`,
+extend_utils.py:7-37) run over `pvnet_farthest_point_sampling` / `pvnet_mesh_binary_rasterization` (csrc/extend.cu)
+and return what the reference's compiled code returns, bit for bit (DESIGN.md §11).
+
+Device-side uncertainty-driven PnP: the reference's `uncertainty_pnp`
 (zju3dv/pvnet lib/utils/extend_utils/extend_utils.py:63-114) and the covariance -> weight step of
 `Evaluator.evaluate_uncertainty` (lib/utils/evaluation_utils.py:165-201), over the C ABI
 (`pvnet_uncertainty_pnp`, `pvnet_covariance_to_weights` in include/pvnet_b200.h).
@@ -82,3 +88,104 @@ def uncertainty_pnp(points_2d, weights_2d, points_3d, camera_matrix):
     w = torch.as_tensor(np.asarray(weights_2d, np.float32), device=dev)[None]
     assert p2.shape[1] == np.asarray(points_3d).shape[0] and p2.shape[1] >= 4          # extend_utils.py:72
     return uncertainty_pnp_batched(p2, np.asarray(points_3d, np.float32), camera_matrix, weights_2d=w)[0].cpu().numpy()
+
+
+def _default_device():
+    if not torch.cuda.is_available():
+        raise RuntimeError("pvnet_b200: this function needs a CUDA device (there is no CPU path)")
+    return torch.device("cuda", torch.cuda.current_device())
+
+
+def farthest_point_sampling(pts, sn, init_center=False, *, start=None, return_indices=False):
+    """The reference's farthest_point_sampling (extend_utils.py:22-37) over `pvnet_farthest_point_sampling`.
+
+    numpy pts [pn,3] -> float32 numpy [sn,3], the sampled points ``pts[idxs]``, as the reference returns.  A CUDA
+    tensor [pn,3] or [b,pn,3] (one cloud per batch entry) gives a float32 CUDA tensor [sn,3] / [b,sn,3] and does
+    not synchronise.  return_indices=True returns the int32 indices [sn] / [b,sn] instead of the points.
+
+    init_center=True starts from the point farthest from the bounding-box centre and is deterministic (the mode
+    lib/utils/data_utils.py uses for the keypoints).  Otherwise the reference starts at rand() % pn; here `start`
+    (an int, or one per cloud) is that first index, taken modulo pn, and when it is None it is drawn uniformly in
+    [0, pn) from torch's default generator (the CUDA one for CUDA input).
+    """
+    as_numpy = not isinstance(pts, torch.Tensor)
+    if as_numpy:
+        pts = np.asarray(pts)
+        pn = pts.shape[0]
+        assert pts.shape[1] == 3                                                      # extend_utils.py:24
+        dev = _default_device()
+        p = torch.as_tensor(np.ascontiguousarray(pts, np.float32), device=dev)[None]
+    else:
+        if not pts.is_cuda:
+            raise RuntimeError("pvnet_b200: `pts` must be a CUDA tensor (there is no CPU path)")
+        if pts.dim() not in (2, 3) or pts.shape[-1] != 3:
+            raise ValueError(f"pts must be [pn,3] or [b,pn,3], got {tuple(pts.shape)}")
+        dev = pts.device
+        p = (pts if pts.dim() == 3 else pts[None]).contiguous().float()
+    b, pn = int(p.shape[0]), int(p.shape[1])
+    if pn < 1:
+        raise ValueError("farthest_point_sampling needs at least one point")
+    sn = int(sn)
+    if sn < 0:
+        raise ValueError(f"negative sample count {sn}")
+    st = None
+    if not init_center:
+        if start is None:
+            st = torch.randint(0, pn, (b,), dtype=torch.int32, device=dev)
+        else:
+            st = torch.as_tensor(start, dtype=torch.int32).reshape(-1).to(dev)
+            if st.numel() == 1:
+                st = st.expand(b)
+            if st.numel() != b:
+                raise ValueError(f"start has {st.numel()} entries for {b} clouds")
+            st = st.contiguous()
+    idxs = torch.empty((b, sn), dtype=torch.int32, device=dev)
+    L = _native.lib()
+    with torch.cuda.device(dev):
+        need = ctypes.c_size_t()
+        _native.check(L.pvnet_farthest_point_sampling_workspace_bytes(b, pn, ctypes.byref(need)),
+                      "pvnet_farthest_point_sampling_workspace_bytes")
+        ws = torch.empty(need.value, dtype=torch.uint8, device=dev) if need.value else None
+        _native.check(L.pvnet_farthest_point_sampling(
+            p.data_ptr(), None if st is None else st.data_ptr(), b, pn, sn, idxs.data_ptr(),
+            None if ws is None else ws.data_ptr(), need.value, _stream(dev)), "pvnet_farthest_point_sampling")
+    single = as_numpy or pts.dim() == 2
+    if return_indices:
+        out = idxs[0] if single else idxs
+    else:
+        out = torch.gather(p, 1, idxs.long()[..., None].expand(b, sn, 3))
+        out = out[0] if single else out
+    return out.cpu().numpy() if as_numpy else out
+
+
+def mesh_binary_rasterization(triangles_2d, h, w):
+    """The reference's mesh_binary_rasterization (extend_utils.py:7-20) over `pvnet_mesh_binary_rasterization`.
+
+    numpy triangles [tn,3,2] (pixel x, y) -> uint8 numpy mask [h,w] of 0/1.  A CUDA tensor [tn,3,2] or [b,tn,3,2]
+    gives a uint8 CUDA tensor [h,w] / [b,h,w] without synchronising."""
+    as_numpy = not isinstance(triangles_2d, torch.Tensor)
+    if as_numpy:
+        t = np.asarray(triangles_2d)
+        assert t.shape[1] == 3                                                        # extend_utils.py:9-10
+        assert t.shape[2] == 2
+        dev = _default_device()
+        tri = torch.as_tensor(np.ascontiguousarray(t, np.float32), device=dev)[None]
+    else:
+        if not triangles_2d.is_cuda:
+            raise RuntimeError("pvnet_b200: `triangles_2d` must be a CUDA tensor (there is no CPU path)")
+        if triangles_2d.dim() not in (3, 4) or tuple(triangles_2d.shape[-2:]) != (3, 2):
+            raise ValueError(f"triangles_2d must be [tn,3,2] or [b,tn,3,2], got {tuple(triangles_2d.shape)}")
+        dev = triangles_2d.device
+        tri = (triangles_2d if triangles_2d.dim() == 4 else triangles_2d[None]).contiguous().float()
+    b, tn = int(tri.shape[0]), int(tri.shape[1])
+    h, w = int(h), int(w)
+    if h < 2 or w < 2:
+        raise ValueError(f"the mask must be at least 2x2, got {h}x{w}")
+    mask = torch.empty((b, h, w), dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        _native.check(_native.lib().pvnet_mesh_binary_rasterization(tri.data_ptr() if tn else None, b, tn, h, w,
+                                                                     mask.data_ptr(), _stream(dev)),
+                      "pvnet_mesh_binary_rasterization")
+    single = as_numpy or triangles_2d.dim() == 3
+    out = mask[0] if single else mask
+    return out.cpu().numpy() if as_numpy else out
