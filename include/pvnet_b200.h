@@ -314,6 +314,33 @@ PVNET_API int pvnet_seg_vertex_losses(const float *seg_pred, const int64_t seg_s
                                       float *loss_seg, float *loss_vertex, float *precision, float *recall,
                                       void *workspace, size_t workspace_bytes, pvnet_stream_t stream);
 
+/* Keypoint targets (losses.cu, DESIGN.md §12): the ground-truth vertex field of the reference's loader,
+ * compute_vertex_hcoords (lib/datasets/linemod_dataset.py:68-81; tools/demo.py:58-71 is the case hw = 1), built from
+ * the mask and the keypoints instead of read from memory.  hcoords is device memory [b,K,3] contiguous, float32
+ * (hcoords_f64 == 0) or float64; each (hx, hy, hw) is widened to fp64.  For a pixel (x, y) with mask == 1 (exactly 1:
+ * a value of 2 is background) and keypoint k, every op rounded on its own as numpy does:
+ *   vx = hx - x*hw, vy = hy - y*hw; unless use_motion: n = sqrt(vx*vx + vy*vy), n < 1e-3 -> n + 1e-3, v = v / n;
+ *   channel 2k = (float)vx, channel 2k+1 = (float)vy (round to nearest); every other pixel +0.0f.
+ * NaN and inf propagate as in numpy.  The field is bit-identical to the reference's for the hcoords passed in.
+ *
+ * pvnet_vertex_targets: writes the field to vertex_out f32 [b,2K,h,w] contiguous (the loader's [h,w,2K] after
+ *   permute(2,0,1)).  mask as for pvnet_seg_vertex_losses (element strides, unit stride along w).
+ * pvnet_seg_vertex_losses_keypoints: pvnet_seg_vertex_losses with the vertex targets computed as above in place of
+ *   `vertex` (ver_dim must be 2K); the mask is read for loss_vertex too.  Every output is bit-identical to
+ *   pvnet_seg_vertex_losses on the field pvnet_vertex_targets writes.  Same workspace query, same NULL-output rule,
+ *   same determinism; graph capturable. */
+PVNET_API int pvnet_vertex_targets(const void *mask, int mask_elem_size, const int64_t mask_strides[3],
+                                   const void *hcoords, int hcoords_f64, int b, int h, int w, int K, int use_motion,
+                                   float *vertex_out, pvnet_stream_t stream);
+PVNET_API int pvnet_seg_vertex_losses_keypoints(const float *seg_pred, const int64_t seg_strides[4],
+                                                const void *mask, int mask_elem_size, const int64_t mask_strides[3],
+                                                const float *vertex_pred, const int64_t pred_strides[4],
+                                                const void *hcoords, int hcoords_f64, int use_motion,
+                                                const float *vertex_weights, const int64_t weight_strides[4],
+                                                int b, int h, int w, int C, int ver_dim, double sigma, int normalize,
+                                                float *loss_seg, float *loss_vertex, float *precision, float *recall,
+                                                void *workspace, size_t workspace_bytes, pvnet_stream_t stream);
+
 /* ------------------------------------------------------------------ dataset tooling (extend.cu, DESIGN.md §11)
  * pvnet_farthest_point_sampling: replaces farthest_point_sampling / farthest_point_sampling_init_center
  *   (lib/utils/extend_utils/src/farthest_point_sampling.cpp:77-105,122-160,166-204, called by extend_utils.py:22-37).

@@ -62,6 +62,12 @@ SIGNATURES = {
                                         c_void_p, c_int64_p, c_void_p, c_int64_p, c_int, c_int, c_int, c_int, c_int,
                                         ctypes.c_double, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                                         c_void_p, c_size_t, c_void_p]),
+    "pvnet_vertex_targets": (c_int, [c_void_p, c_int, c_int64_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,
+                                     c_void_p, c_void_p]),
+    "pvnet_seg_vertex_losses_keypoints": (c_int, [c_void_p, c_int64_p, c_void_p, c_int, c_int64_p, c_void_p, c_int64_p,
+                                                  c_void_p, c_int, c_int, c_void_p, c_int64_p, c_int, c_int, c_int,
+                                                  c_int, c_int, ctypes.c_double, c_int, c_void_p, c_void_p, c_void_p,
+                                                  c_void_p, c_void_p, c_size_t, c_void_p]),
     "pvnet_farthest_point_sampling_workspace_bytes": (c_int, [c_int, c_int, ctypes.POINTER(c_size_t)]),
     "pvnet_farthest_point_sampling": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_size_t,
                                               c_void_p]),

@@ -7,6 +7,10 @@ reference's entry points import from that module.
     compute_precision_recall(scores, target, reduce=False)
     seg_vertex_losses(seg_pred, vertex_pred, mask, vertex, vertex_weights)
                                    -> (loss_seg, loss_vertex, precision, recall), all four in one launch pair
+    vertex_targets(mask, hcoords, use_motion=False)
+                                   the loader's ground-truth vertex field [b,2K,h,w] (compute_vertex_hcoords)
+    seg_vertex_losses_from_keypoints(seg_pred, vertex_pred, mask, hcoords, vertex_weights, use_motion=False)
+                                   seg_vertex_losses with that field computed in registers, never stored
     NetWrapper(net)                the reference's NetWrapper with the fused call in eval / no_grad
     AverageMeter, Recorder, load_model, save_model, adjust_learning_rate, set_learning_rate
 
@@ -63,6 +67,17 @@ def _check_vertex(vertex_pred, vertex_targets, vertex_weights):
         raise ValueError(f"vertex_weights must be [b,1,h,w] = {(b, 1, h, w)}, got {tuple(vertex_weights.shape)}")
 
 
+def _check_keypoints(mask, hcoords):
+    if mask.dim() != 3:
+        raise ValueError(f"mask must be [b,h,w], got {tuple(mask.shape)}")
+    if mask.dtype not in _MASK_DTYPES:
+        raise ValueError(f"mask dtype {mask.dtype} is not one of int64, int32, uint8, bool")
+    if hcoords.dim() != 3 or hcoords.shape[0] != mask.shape[0] or hcoords.shape[1] < 1 or hcoords.shape[2] != 3:
+        raise ValueError(f"hcoords must be [b,K,3] with b = {mask.shape[0]} and K >= 1, got {tuple(hcoords.shape)}")
+    if hcoords.dtype not in (torch.float32, torch.float64):
+        raise ValueError(f"hcoords must be float32 or float64, got {hcoords.dtype}")
+
+
 def _check_seg(scores, target):
     _check_float("seg_pred", scores)
     if scores.dim() != 4:
@@ -75,9 +90,10 @@ def _check_seg(scores, target):
 
 
 def _native_losses(seg=None, mask=None, pred=None, tgt=None, wgt=None, sigma=1.0, normalize=True,
-                   want=("seg", "ver", "precision", "recall")):
-    """One pvnet_seg_vertex_losses call; returns {part: tensor} for the parts in `want`."""
-    xs = [x for x in (seg, mask, pred, tgt, wgt) if x is not None]
+                   want=("seg", "ver", "precision", "recall"), hcoords=None, use_motion=False):
+    """One pvnet_seg_vertex_losses call (pvnet_seg_vertex_losses_keypoints when `hcoords` replaces `tgt`); returns
+    {part: tensor} for the parts in `want`."""
+    xs = [x for x in (seg, mask, pred, tgt, wgt, hcoords) if x is not None]
     if not all(x.is_cuda for x in xs):
         raise RuntimeError("pvnet_b200: the validation losses need CUDA tensors (there is no CPU path)")
     dev = xs[0].device
@@ -90,19 +106,29 @@ def _native_losses(seg=None, mask=None, pred=None, tgt=None, wgt=None, sigma=1.0
     C = vd = 0
     if seg is not None:
         seg, s_seg = _strides(seg, 4)
-        mask, s_mask = _strides(mask, 3)
         C = seg.shape[1]
-        args += [seg.data_ptr(), s_seg, mask.data_ptr(), mask.element_size(), s_mask]
+        args += [seg.data_ptr(), s_seg]
     else:
-        args += [None, None, None, 0, None]
+        args += [None, None]
+    if mask is not None:
+        mask, s_mask = _strides(mask, 3)
+        args += [mask.data_ptr(), mask.element_size(), s_mask]
+    else:
+        args += [None, 0, None]
     if pred is not None:
         pred, s_pred = _strides(pred, 4)
-        tgt, s_tgt = _strides(tgt, 4)
-        wgt, s_wgt = _strides(wgt, 4)
         vd = pred.shape[1]
-        args += [pred.data_ptr(), s_pred, tgt.data_ptr(), s_tgt, wgt.data_ptr(), s_wgt]
+        args += [pred.data_ptr(), s_pred]
+        if hcoords is None:
+            tgt, s_tgt = _strides(tgt, 4)
+            args += [tgt.data_ptr(), s_tgt]
+        else:
+            hcoords = hcoords.detach().contiguous()
+            args += [hcoords.data_ptr(), int(hcoords.dtype == torch.float64), int(bool(use_motion))]
+        wgt, s_wgt = _strides(wgt, 4)
+        args += [wgt.data_ptr(), s_wgt]
     else:
-        args += [None] * 6
+        args += [None] * (6 if hcoords is None else 7)
     out = {}
     for part in want:
         shape = [b, vd, h, w] if part == "ver" and not normalize else [b]
@@ -112,12 +138,13 @@ def _native_losses(seg=None, mask=None, pred=None, tgt=None, wgt=None, sigma=1.0
                   "pvnet_seg_vertex_losses_workspace_bytes")
     ws = torch.empty([nbytes.value], dtype=torch.uint8, device=dev)
     ptr = {k: v.data_ptr() for k, v in out.items()}
+    name = "pvnet_seg_vertex_losses" if hcoords is None else "pvnet_seg_vertex_losses_keypoints"
     with torch.cuda.device(dev):
-        _native.check(L.pvnet_seg_vertex_losses(*args, b, h, w, C, vd, float(sigma), int(bool(normalize)),
-                                                ptr.get("seg"), ptr.get("ver"), ptr.get("precision"),
-                                                ptr.get("recall"), ws.data_ptr(), nbytes.value,
-                                                ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
-                      "pvnet_seg_vertex_losses")
+        _native.check(getattr(L, name)(*args, b, h, w, C, vd, float(sigma), int(bool(normalize)),
+                                       ptr.get("seg"), ptr.get("ver"), ptr.get("precision"), ptr.get("recall"),
+                                       ws.data_ptr(), nbytes.value,
+                                       ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
+                      name)
     return out
 
 
@@ -197,6 +224,60 @@ def seg_vertex_losses(seg_pred, vertex_pred, mask, vertex, vertex_weights):
         return (_cross_entropy_torch(seg_pred, mask),
                 _smooth_l1_torch(vertex_pred, vertex, vertex_weights, 1.0, True), precision, recall)
     r = _native_losses(seg_pred, mask, vertex_pred, vertex, vertex_weights)
+    return r["seg"], r["ver"], r["precision"], r["recall"]
+
+
+def vertex_targets(mask, hcoords, use_motion=False):
+    """The loader's ground-truth vertex field on the device: compute_vertex_hcoords
+    (lib/datasets/linemod_dataset.py:68-81) for every image, as the loader collates it (`.permute(2,0,1)`).
+    mask [b,h,w] (int64, int32, uint8 or bool; foreground is mask == 1), hcoords [b,K,3] float32 or float64 with rows
+    (hx, hy, hw) -> float32 [b,2K,h,w].  Bit-identical to the reference's numpy for the hcoords passed in; the
+    loader's keypoints are float64, so pass those (not their float32 rounding) where exact equality with the loader
+    matters.  tools/demo.py's compute_vertex(mask, points_2d) is hcoords = [points_2d, 1]."""
+    _check_keypoints(mask, hcoords)
+    if not (mask.is_cuda and hcoords.is_cuda):
+        raise RuntimeError("pvnet_b200: vertex_targets needs CUDA tensors (there is no CPU path)")
+    if mask.device != hcoords.device:
+        raise ValueError("mask and hcoords must be on the same device")
+    dev = mask.device
+    b, h, w = mask.shape
+    K = hcoords.shape[1]
+    mask, s_mask = _strides(mask, 3)
+    hc = hcoords.detach().contiguous()
+    out = torch.empty([b, 2 * K, h, w], dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        _native.check(_native.lib().pvnet_vertex_targets(
+            mask.data_ptr(), mask.element_size(), s_mask, hc.data_ptr(), int(hc.dtype == torch.float64), b, h, w, K,
+            int(bool(use_motion)), out.data_ptr(), ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
+            "pvnet_vertex_targets")
+    return out
+
+
+def seg_vertex_losses_from_keypoints(seg_pred, vertex_pred, mask, hcoords, vertex_weights, use_motion=False):
+    """seg_vertex_losses with the vertex targets built from the keypoints instead of read from a [b,2K,h,w] tensor:
+    the same four float32 [b] figures, bit-identical to seg_vertex_losses(seg_pred, vertex_pred, mask,
+    vertex_targets(mask, hcoords, use_motion), vertex_weights), in one launch pair that never materialises the field.
+    hcoords [b,K,3] float32 or float64, with ver_dim == 2K.  In grad mode the field is materialised with
+    vertex_targets and the torch expressions evaluated on it."""
+    _check_seg(seg_pred, mask)
+    for name, x in (("vertex_pred", vertex_pred), ("vertex_weights", vertex_weights)):
+        _check_float(name, x)
+    if vertex_pred.dim() != 4:
+        raise ValueError(f"vertex_pred must be [b,ver_dim,h,w], got {tuple(vertex_pred.shape)}")
+    b, vd, h, w = vertex_pred.shape
+    if tuple(vertex_weights.shape) != (b, 1, h, w):
+        raise ValueError(f"vertex_weights must be [b,1,h,w] = {(b, 1, h, w)}, got {tuple(vertex_weights.shape)}")
+    if seg_pred.shape[0] != b or seg_pred.shape[2:] != vertex_pred.shape[2:]:
+        raise ValueError(f"seg_pred {tuple(seg_pred.shape)} and vertex_pred {tuple(vertex_pred.shape)} differ in b,h,w")
+    _check_keypoints(mask, hcoords)
+    if vd != 2 * hcoords.shape[1]:
+        raise ValueError(f"ver_dim {vd} is not 2 x the {hcoords.shape[1]} keypoints of hcoords")
+    if _use_torch(seg_pred, vertex_pred, vertex_weights):
+        vertex = vertex_targets(mask, hcoords, use_motion)
+        precision, recall = _precision_recall_torch(seg_pred, mask)
+        return (_cross_entropy_torch(seg_pred, mask),
+                _smooth_l1_torch(vertex_pred, vertex, vertex_weights, 1.0, True), precision, recall)
+    r = _native_losses(seg_pred, mask, vertex_pred, None, vertex_weights, hcoords=hcoords, use_motion=use_motion)
     return r["seg"], r["ver"], r["precision"], r["recall"]
 
 
