@@ -96,11 +96,14 @@ def p3p(P, f):
         if abs(v.imag) > 1e-6 * max(1.0, abs(v.real)):
             continue
         v = v.real
-        for _ in range(4):                                     # Newton polish on the quartic
-            pv = np.polyval(coef, v)
+        for _ in range(12):                                    # Newton polish on the quartic, to convergence (near a
+            pv = np.polyval(coef, v)                           # nearly double root it converges only linearly)
             dv = np.polyval(np.polyder(coef), v)
-            if dv != 0:
-                v -= pv / dv
+            if dv == 0:
+                break
+            v -= pv / dv
+            if abs(pv / dv) < 1e-15 * max(1.0, abs(v)):
+                break
         den = 2 * (cg - v * ca)
         if abs(den) < 1e-14 or v <= 0:
             continue

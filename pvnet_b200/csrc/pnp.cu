@@ -13,17 +13,25 @@
 // registers), so the loop has no divergence.  Rotation is kept as a matrix and updated on the manifold (R <- exp(dw) R), which has the
 // same minimiser as the reference's angle-axis parametrisation; damping follows Ceres'
 // Levenberg-Marquardt strategy (diagonal scaling, radius /= max(1/3, 1 - (2 rho - 1)^3) on success,
-// shrink by 2, 4, 8.. on failure) but iterates to |step| < 1e-9 (the next one is ~1e-11) instead of Ceres'
-// function_tolerance 1e-6, i.e. to the minimiser the reference approximates.
-// Initialisation: Grunert's P3P quartic (roots by Durand-Kerner + Newton polish) on the first three
-// of the four selected points, the fourth picks the solution -- OpenCV's SOLVEPNP_P3P contract.
+// shrink by 2, 4, 8.. on failure) but iterates until it has taken a step with max |delta| < 1e-9 instead of Ceres'
+// function_tolerance 1e-6, i.e. to the minimiser the reference approximates.  Where Gauss-Newton converges
+// quadratically the next step would be ~1e-11; on large-residual problems it converges only linearly and a last
+// step below 1e-9 can leave a few 1e-8.  It also stops when max |J^T r| < 1e-14 (an absolute threshold), and when
+// all 12 damping tries of one iteration fail to lower the cost (status 0 in both cases); a step below 1e-9 counts
+// as convergence however heavily it was damped.
+// Initialisation: Grunert's P3P quartic (roots by Durand-Kerner, fp32 then fp64, + fp64 Newton polish of the real
+// ones) on the first three of the four selected points, the fourth picks the solution -- OpenCV's SOLVEPNP_P3P
+// contract.
 #include "common.cuh"
 
 #include <cmath>
 
 namespace {
 
-constexpr int PNP_MAX_ITERS = 100;
+// Most images converge in 4-12 iterations.  A P3P start whose first, nearly undamped step overshoots in depth
+// (t_z 1.2 -> 3.2 on one 5-point image of the tests) then crawls back along a curved valley and needs ~240; the
+// cap leaves room for twice that.  An image that reaches it returns a non-converged pose with status bit 2.
+constexpr int PNP_MAX_ITERS = 500;
 
 __device__ __forceinline__ double warp_sum_all(double v)
 {
@@ -55,9 +63,50 @@ __device__ __forceinline__ void tri_frame(Vec3 p0, Vec3 p1, Vec3 p2, double (&F)
     F[6] = e1.z; F[7] = e2.z; F[8] = e3.z;
 }
 
-// all roots of c4 z^4 + .. + c0: Durand-Kerner in fp32 (it only has to separate the roots: P3P's quartics have
-// clustered roots whose last digits never settle, and one warp's serial fp64 divisions were a third of the
-// kernel's time), then the real ones are Newton-polished in fp64 on the real polynomial.
+// one Durand-Kerner sweep over the four roots (zr + i zi) of the monic z^4 + f3 z^3 + f2 z^2 + f1 z + f0; returns
+// the largest |correction| (|re| + |im|)
+template <typename T>
+__device__ __forceinline__ T durand_kerner_sweep(T (&zr)[4], T (&zi)[4], T f3, T f2, T f1, T f0)
+{
+    T move = T(0);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        // p(z) by Horner (monic)
+        T vr = zr[k] + f3, vi = zi[k];
+        T tr = vr * zr[k] - vi * zi[k] + f2, ti = vr * zi[k] + vi * zr[k];
+        vr = tr * zr[k] - ti * zi[k] + f1;
+        vi = tr * zi[k] + ti * zr[k];
+        tr = vr * zr[k] - vi * zi[k] + f0;
+        ti = vr * zi[k] + vi * zr[k];
+        T dr = T(1), di = T(0);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            if (j == k) continue;
+            const T er = zr[k] - zr[j], ei = zi[k] - zi[j];
+            const T xr = dr * er - di * ei, xi = dr * ei + di * er;
+            dr = xr;
+            di = xi;
+        }
+        const T den = dr * dr + di * di;
+        if (den > T(0)) {
+            const T inv = T(1) / den;
+            const T qr = (tr * dr + ti * di) * inv, qi = (ti * dr - tr * di) * inv;
+            zr[k] -= qr;
+            zi[k] -= qi;
+            move = fmax(move, fabs(qr) + fabs(qi));
+        }
+    }
+    return move;
+}
+
+// all roots of c4 z^4 + .. + c0 by Durand-Kerner: fp32 sweeps from a circle bring the four estimates near the roots
+// cheaply, then fp64 sweeps on all four at once separate them.  P3P's quartics have their roots clustered near
+// v = 1 with gaps ~1e-2, while rounding the coefficients to fp32 moves such a cluster by about as much: the fp32
+// estimates alone can sit on the wrong root, and polishing them one at a time (Newton) merges neighbours and loses
+// real roots.  The simultaneous fp64 iteration keeps the four apart; it stops when the largest correction is below
+// 1e-10 of the root bound (2-3 sweeps for most quartics, up to 64 for near-double roots, whose corrections stall at
+// the rounding floor).  The real roots (|im| <= 1e-6 max(1, |re|)) are then Newton-polished on the real polynomial
+// and kept where the quartic vanishes to 1e-9 of its terms' magnitude.
 __device__ int quartic_real_roots(const double (&c)[5], double (&out)[4])
 {
     if (!(fabs(c[4]) > 1e-300)) return 0;
@@ -78,44 +127,21 @@ __device__ int quartic_real_roots(const double (&c)[5], double (&out)[4])
             pi = ni;
         }
     }
-    for (int it = 0; it < 48; ++it) {
-        float move = 0.0f;
+    for (int it = 0; it < 48; ++it)
+        if (durand_kerner_sweep(zr, zi, f3, f2, f1, f0) < 2e-6f * rad) break;
+    double wr[4], wi[4];
 #pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            // p(z) by Horner (monic)
-            float vr = zr[k] + f3, vi = zi[k];
-            float tr = vr * zr[k] - vi * zi[k] + f2, ti = vr * zi[k] + vi * zr[k];
-            vr = tr * zr[k] - ti * zi[k] + f1;
-            vi = tr * zi[k] + ti * zr[k];
-            tr = vr * zr[k] - vi * zi[k] + f0;
-            ti = vr * zi[k] + vi * zr[k];
-            float dr = 1.0f, di = 0.0f;
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                if (j == k) continue;
-                const float er = zr[k] - zr[j], ei = zi[k] - zi[j];
-                const float xr = dr * er - di * ei, xi = dr * ei + di * er;
-                dr = xr;
-                di = xi;
-            }
-            const float den = dr * dr + di * di;
-            if (den > 0.0f) {
-                const float inv = 1.0f / den;
-                const float qr = (tr * dr + ti * di) * inv, qi = (ti * dr - tr * di) * inv;
-                zr[k] -= qr;
-                zi[k] -= qi;
-                move = fmaxf(move, fabsf(qr) + fabsf(qi));
-            }
-        }
-        if (move < 2e-6f * rad) break;
+    for (int k = 0; k < 4; ++k) {
+        wr[k] = zr[k];
+        wi[k] = zi[k];
     }
+    for (int it = 0; it < 64; ++it)
+        if (durand_kerner_sweep(wr, wi, a3, a2, a1, a0) < 1e-10 * (double)rad) break;
     int n = 0;
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-        // generous real-root filter (fp32 separation of near-double roots), then fp64 Newton; a complex pair that
-        // slipped through polishes to a point where the quartic is not ~0 and is dropped
-        if (!(fabsf(zi[k]) <= 2e-2f * fmaxf(1.0f, fabsf(zr[k])))) continue;
-        double v = (double)zr[k];
+        if (!(fabs(wi[k]) <= 1e-6 * fmax(1.0, fabs(wr[k])))) continue;
+        double v = wr[k];
         for (int it = 0; it < 12; ++it) {
             const double p = (((v + a3) * v + a2) * v + a1) * v + a0;
             const double d = ((4.0 * v + 3.0 * a3) * v + 2.0 * a2) * v + a1;
