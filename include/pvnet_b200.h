@@ -343,6 +343,48 @@ PVNET_API int pvnet_seg_vertex_losses_keypoints(const float *seg_pred, const int
                                                 float *loss_seg, float *loss_vertex, float *precision, float *recall,
                                                 void *workspace, size_t workspace_bytes, pvnet_stream_t stream);
 
+/* Gradients of the training losses (losses.cu, DESIGN.md §13): d loss_seg / d seg_pred and d loss_vertex /
+ * d vertex_pred for the normalised loss_vertex (normalize must be nonzero), each the sequence torch's CUDA autograd
+ * runs through the reference's expressions (nn.CrossEntropyLoss(reduction='none') + .view(b,-1).mean(1);
+ * net_utils.py:54-80 with torch.pow(diff, 2)), every op rounded on its own.  Per image, with N = h*w:
+ *   seg:    g = gs * (1.0f / (float)N) with gs = grad_loss_seg[b]; lp_c = (x_c - m) - logf(s) as in the forward;
+ *           S = 0 + sum_c gO_c in channel order with gO_t = -g at the target and 0 elsewhere;
+ *           grad_seg_c = fmaf(-expf(lp_c), S, gO_c).  t = -100 gives gO = 0 (0 in every channel unless the pixel's
+ *           log-softmax is NaN, as in torch); any other t outside [0,C) makes every element of the image NaN.
+ *   vertex: gi = gv / (ver_dim*sum(w) + 1e-3f) with gv = grad_loss_vertex[b] and the forward's denominator bit for
+ *           bit (recomputed in the forward's summation order); d = w*(p - t), s = |d| < 1/sigma^2,
+ *           grad_vertex = (((gi*s)*c2)*(2*d) + (gi*(1 - s))*sgn(d)) * w, c2 = sigma^2/2 rounded to float,
+ *           sgn(+-0) = sgn(NaN) = 0.
+ * Inputs as for pvnet_seg_vertex_losses / _keypoints.  grad_loss_seg, grad_loss_vertex: f32 [b] device, each
+ * nullable.  grad_seg f32 [b,C,h,w] and grad_vertex f32 [b,ver_dim,h,w] are written through element strides (unit
+ * stride along w), each nullable; they may be channel slices of one [b,C+ver_dim,h,w] tensor.  A NULL loss
+ * gradient means that loss contributes nothing: its output, when not NULL, is written as zeros, and the inputs only
+ * that part needs are not read.  Precision and recall have no gradient.  No allocation, no synchronisation,
+ * run-to-run identical, graph capturable.  Workspace: pvnet_seg_vertex_losses_workspace_bytes(b, h, w). */
+PVNET_API int pvnet_seg_vertex_losses_backward(const float *seg_pred, const int64_t seg_strides[4],
+                                               const void *mask, int mask_elem_size, const int64_t mask_strides[3],
+                                               const float *vertex_pred, const int64_t pred_strides[4],
+                                               const float *vertex, const int64_t vertex_strides[4],
+                                               const float *vertex_weights, const int64_t weight_strides[4],
+                                               int b, int h, int w, int C, int ver_dim, double sigma, int normalize,
+                                               const float *grad_loss_seg, const float *grad_loss_vertex,
+                                               float *grad_seg, const int64_t grad_seg_strides[4],
+                                               float *grad_vertex, const int64_t grad_vertex_strides[4],
+                                               void *workspace, size_t workspace_bytes, pvnet_stream_t stream);
+PVNET_API int pvnet_seg_vertex_losses_keypoints_backward(const float *seg_pred, const int64_t seg_strides[4],
+                                                         const void *mask, int mask_elem_size,
+                                                         const int64_t mask_strides[3],
+                                                         const float *vertex_pred, const int64_t pred_strides[4],
+                                                         const void *hcoords, int hcoords_f64, int use_motion,
+                                                         const float *vertex_weights, const int64_t weight_strides[4],
+                                                         int b, int h, int w, int C, int ver_dim, double sigma,
+                                                         int normalize, const float *grad_loss_seg,
+                                                         const float *grad_loss_vertex,
+                                                         float *grad_seg, const int64_t grad_seg_strides[4],
+                                                         float *grad_vertex, const int64_t grad_vertex_strides[4],
+                                                         void *workspace, size_t workspace_bytes,
+                                                         pvnet_stream_t stream);
+
 /* ------------------------------------------------------------------ dataset tooling (extend.cu, DESIGN.md §11)
  * pvnet_farthest_point_sampling: replaces farthest_point_sampling / farthest_point_sampling_init_center
  *   (lib/utils/extend_utils/src/farthest_point_sampling.cpp:77-105,122-160,166-204, called by extend_utils.py:22-37).

@@ -68,7 +68,16 @@ SIGNATURES = {
                                                   c_void_p, c_int, c_int, c_void_p, c_int64_p, c_int, c_int, c_int,
                                                   c_int, c_int, ctypes.c_double, c_int, c_void_p, c_void_p, c_void_p,
                                                   c_void_p, c_void_p, c_size_t, c_void_p]),
-    "pvnet_farthest_point_sampling_workspace_bytes": (c_int, [c_int, c_int, ctypes.POINTER(c_size_t)]),
+    "pvnet_seg_vertex_losses_backward": (c_int, [c_void_p, c_int64_p, c_void_p, c_int, c_int64_p, c_void_p, c_int64_p,
+                                                 c_void_p, c_int64_p, c_void_p, c_int64_p, c_int, c_int, c_int, c_int,
+                                                 c_int, ctypes.c_double, c_int, c_void_p, c_void_p, c_void_p,
+                                                 c_int64_p, c_void_p, c_int64_p, c_void_p, c_size_t, c_void_p]),
+    "pvnet_seg_vertex_losses_keypoints_backward": (c_int, [c_void_p, c_int64_p, c_void_p, c_int, c_int64_p, c_void_p,
+                                                           c_int64_p, c_void_p, c_int, c_int, c_void_p, c_int64_p,
+                                                           c_int, c_int, c_int, c_int, c_int, ctypes.c_double, c_int,
+                                                           c_void_p, c_void_p, c_void_p, c_int64_p, c_void_p,
+                                                           c_int64_p, c_void_p, c_size_t, c_void_p]),
+    "pvnet_farthest_point_sampling_workspace_bytes":(c_int, [c_int, c_int, ctypes.POINTER(c_size_t)]),
     "pvnet_farthest_point_sampling": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_size_t,
                                               c_void_p]),
     "pvnet_mesh_binary_rasterization": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),

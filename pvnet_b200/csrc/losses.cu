@@ -382,6 +382,210 @@ __global__ void __launch_bounds__(LS_THREADS) k_vertex_targets(VtArgs a, KpArgs 
     }
 }
 
+// ------------------------------------------------------------------ gradients (DESIGN.md §13)
+// The gradients of loss_seg and of the normalised loss_vertex with respect to seg_pred and vertex_pred, each the
+// sequence torch's CUDA autograd runs through the reference's expressions, every op rounded on its own:
+//   cross-entropy: g = gs * (1.0f / (float)(h*w))   (MeanBackward: ATen divides a CUDA tensor by a CPU scalar as a
+//     multiplication by its float reciprocal); per pixel lp_c = (x_c - m) - logf(s) as in the forward,
+//     S = 0 + gO_0 + ... + gO_{C-1} with gO_t = -g at the target and 0 elsewhere (NLLLoss2d backward), and
+//     grad_c = fmaf(-expf(lp_c), S, gO_c) (the log-softmax backward epilogue gO - exp(out)*S, which nvcc contracts);
+//     t = -100 gives gO = 0; any other t outside [0,C) makes every seg-gradient element of the image NaN.
+//   smooth-L1: gi = gv / den with den = ver_dim*(float)Σw + 1e-3f recomputed in the forward's fixed order
+//     (k_weight_sum_partial + k_grad_final), then per element with d = w*(p - t), s = |d| < c1:
+//     A = ((gi*s)*c2)*(2*d)  (MulBackward, MulBackward, PowBackward)   B = (gi*(1 - s))*sgn(d)  (AbsBackward)
+//     grad = (A + B)*w: autograd runs PowBackward0 before AbsBackward0, so A is in the buffer and B is added.
+//     sgn is torch's CUDA sign: (0 < d) - (d < 0), so 0 for +-0 and NaN.
+struct GradArgs {
+    float *gseg;                                   // [b,C,h,w] through strides, or NULL
+    long long gs_b, gs_c, gs_h;
+    float *gver;                                   // [b,vd,h,w] through strides, or NULL
+    long long gv_b, gv_c, gv_h;
+    const float *gls;                              // grad_loss_seg [b]; NULL: gseg is written as zeros
+    const float *gi;                               // gv / den per image (k_grad_final); NULL: gver written as zeros
+    int *bad;                                      // [b, chunks] per-CTA invalid-target flags
+    float inv_n;                                   // 1.0f / (float)(h*w)
+};
+
+__device__ __forceinline__ void store4(float *p, bool full, int n, const float (&v)[4])
+{
+    if (full)
+        *reinterpret_cast<float4 *>(p) = make_float4(v[0], v[1], v[2], v[3]);
+    else
+        for (int j = 0; j < n; ++j) p[j] = v[j];
+}
+
+// the smooth-L1 gradient of one vertex channel of a quad
+__device__ __forceinline__ void ver_grad(const LossArgs &a, float gi, const float (&wv)[4], const float (&pv)[4],
+                                         const float (&tv)[4], float (&o)[4])
+{
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        const float d = __fmul_rn(wv[j], __fsub_rn(pv[j], tv[j]));
+        const float s = fabsf(d) < a.c1 ? 1.f : 0.f;
+        const float sg = (float)((0.f < d) - (d < 0.f));
+        const float A = __fmul_rn(__fmul_rn(__fmul_rn(gi, s), a.c2), __fmul_rn(2.f, d));
+        const float B = __fmul_rn(__fmul_rn(gi, __fsub_rn(1.f, s)), sg);
+        o[j] = __fmul_rn(__fadd_rn(A, B), wv[j]);
+    }
+}
+
+// grid (chunks, b), the quad assignment of k_losses_partial; each thread writes its quads' gradients
+template <typename MT, bool KP>
+__global__ void __launch_bounds__(LS_THREADS, KP ? LS_KP_MIN_BLOCKS : 3)
+    k_losses_backward(LossArgs a, GradArgs g, KpArgs kp)
+{
+    const int img = blockIdx.y;
+    const float gs = g.gls ? __fmul_rn(__ldg(g.gls + img), g.inv_n) : 0.f;
+    const float gi = g.gi ? __ldg(g.gi + img) : 0.f;
+    const float zero[4] = {0.f, 0.f, 0.f, 0.f};
+    int bad = 0;
+    const int q_end = min(a.nquads, (int)(blockIdx.x + 1) * LS_QPB);
+    for (int q = blockIdx.x * LS_QPB + threadIdx.x; q < q_end; q += LS_THREADS) {
+        const int y = q / a.qw;
+        const int x0 = (q - y * a.qw) * 4;
+        const int n = min(4, a.w - x0);
+        const bool full = a.vec && n == 4;
+
+        if (g.gseg) {
+            float *o0 = g.gseg + img * g.gs_b + y * g.gs_h + x0;
+            if (!g.gls) {
+                for (int c = 0; c < a.C; ++c) store4(o0 + c * g.gs_c, full, n, zero);
+            } else {
+                const float *s0 = a.seg + img * a.seg_b + y * a.seg_h + x0;
+                long long t[4];
+                load_mask4(static_cast<const MT *>(a.mask) + img * a.m_b + y * a.m_h + x0, full, n, t);
+                float v[4], m[4], s[4] = {0.f, 0.f, 0.f, 0.f}, ls[4], S[4];
+                load4(s0, full, n, m);
+                for (int c = 1; c < a.C; ++c) {
+                    load4(s0 + c * a.seg_c, full, n, v);
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) m[j] = fmaxf(m[j], v[j]);
+                }
+                for (int c = 0; c < a.C; ++c) {
+                    load4(s0 + c * a.seg_c, full, n, v);
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) s[j] = __fadd_rn(s[j], expf(__fsub_rn(v[j], m[j])));
+                }
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    ls[j] = logf(s[j]);
+                    const bool valid = t[j] >= 0 && t[j] < a.C;
+                    if (j < n && !valid && t[j] != LS_IGNORE) bad = 1;
+                    S[j] = valid ? __fadd_rn(0.f, -gs) : 0.f;          // the zeros of the other channels add nothing
+                }
+                for (int c = 0; c < a.C; ++c) {
+                    load4(s0 + c * a.seg_c, full, n, v);
+                    float o[4];
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) {
+                        const float e = expf(__fsub_rn(__fsub_rn(v[j], m[j]), ls[j]));
+                        o[j] = __fmaf_rn(-e, S[j], t[j] == c ? -gs : 0.f);
+                    }
+                    store4(o0 + c * g.gs_c, full, n, o);
+                }
+            }
+        }
+
+        if (g.gver) {
+            float *o0 = g.gver + img * g.gv_b + y * g.gv_h + x0;
+            if (!g.gi) {
+                for (int c = 0; c < a.vd; ++c) store4(o0 + c * g.gv_c, full, n, zero);
+                continue;
+            }
+            float wv[4], o[4];
+            load4(a.wgt + img * a.w_b + y * a.w_h + x0, full, n, wv);
+            const float *p0 = a.pred + img * a.p_b + y * a.p_h + x0;
+            if constexpr (KP) {
+                bool fg[4];
+                fg_quad(static_cast<const MT *>(a.mask) + img * a.m_b + y * a.m_h + x0, full, n, fg);
+                for (int k = 0; k < kp.K; ++k) {
+                    float px[4], py[4], tx[4], ty[4];
+                    load4(p0 + 2 * k * a.p_c, full, n, px);
+                    load4(p0 + (2 * k + 1) * a.p_c, full, n, py);
+                    kp_quad(kp, img, k, x0, y, fg, tx, ty);
+                    ver_grad(a, gi, wv, px, tx, o);
+                    store4(o0 + 2 * k * g.gv_c, full, n, o);
+                    ver_grad(a, gi, wv, py, ty, o);
+                    store4(o0 + (2 * k + 1) * g.gv_c, full, n, o);
+                }
+            } else {
+                const float *t0 = a.tgt + img * a.t_b + y * a.t_h + x0;
+#pragma unroll 2
+                for (int c = 0; c < a.vd; ++c) {
+                    float pv[4], tv[4];
+                    load4(p0 + c * a.p_c, full, n, pv);
+                    load4(t0 + c * a.t_c, full, n, tv);
+                    ver_grad(a, gi, wv, pv, tv, o);
+                    store4(o0 + c * g.gv_c, full, n, o);
+                }
+            }
+        }
+    }
+    if (g.gseg && g.gls) {
+        bad = __syncthreads_or(bad);
+        if (threadIdx.x == 0) g.bad[(size_t)img * gridDim.x + blockIdx.x] = bad;
+    }
+}
+
+// grid (chunks, b): Σw of each CTA's quads, summed exactly as k_losses_partial sums `sw` (same thread order, shuffle
+// tree and warp order), so that k_grad_final's denominator is the forward's bit for bit
+__global__ void __launch_bounds__(LS_THREADS) k_weight_sum_partial(LossArgs a, double *__restrict__ partial)
+{
+    const int img = blockIdx.y;
+    double sw = 0.0;
+    const int q_end = min(a.nquads, (int)(blockIdx.x + 1) * LS_QPB);
+    for (int q = blockIdx.x * LS_QPB + threadIdx.x; q < q_end; q += LS_THREADS) {
+        const int y = q / a.qw;
+        const int x0 = (q - y * a.qw) * 4;
+        const int n = min(4, a.w - x0);
+        float wv[4];
+        load4(a.wgt + img * a.w_b + y * a.w_h + x0, a.vec && n == 4, n, wv);
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+            if (j < n) sw += (double)wv[j];
+    }
+    __shared__ double s_w[LS_THREADS / 32];
+    sw = warp_sum(sw);
+    if ((threadIdx.x & 31) == 0) s_w[threadIdx.x >> 5] = sw;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double r = s_w[0];
+        for (int i = 1; i < LS_THREADS / 32; ++i) r += s_w[i];
+        partial[(size_t)img * gridDim.x + blockIdx.x] = r;
+    }
+}
+
+// one thread per image: gi = gv / (ver_dim * Σw + 1e-3), k_losses_final's denominator
+__global__ void k_grad_final(const double *__restrict__ partial, int chunks, int b, int vd,
+                             const float *__restrict__ grad_loss_vertex, float *gi)
+{
+    const int img = blockIdx.x * blockDim.x + threadIdx.x;
+    if (img >= b) return;
+    double r = partial[(size_t)img * chunks];
+    for (int c = 1; c < chunks; ++c) r += partial[(size_t)img * chunks + c];
+    const float den = __fadd_rn(__fmul_rn((float)vd, __double2float_rn(r)), 1e-3f);
+    gi[img] = __fdiv_rn(grad_loss_vertex[img], den);
+}
+
+// grid (chunks, b): an image with an invalid target anywhere gets NaN in its whole seg gradient
+__global__ void __launch_bounds__(LS_THREADS) k_seg_grad_invalid(LossArgs a, GradArgs g)
+{
+    const int img = blockIdx.y;
+    int bad = 0;
+    for (int i = threadIdx.x; i < (int)gridDim.x; i += LS_THREADS) bad |= g.bad[(size_t)img * gridDim.x + i];
+    if (!__syncthreads_or(bad)) return;
+    const float qnan = __int_as_float(0x7fffffff);
+    const float nan4[4] = {qnan, qnan, qnan, qnan};
+    const int q_end = min(a.nquads, (int)(blockIdx.x + 1) * LS_QPB);
+    for (int q = blockIdx.x * LS_QPB + threadIdx.x; q < q_end; q += LS_THREADS) {
+        const int y = q / a.qw;
+        const int x0 = (q - y * a.qw) * 4;
+        const int n = min(4, a.w - x0);
+        for (int c = 0; c < a.C; ++c)
+            store4(g.gseg + img * g.gs_b + y * g.gs_h + x0 + c * g.gs_c, a.vec && n == 4, n, nan4);
+    }
+}
+
 int ls_chunks(int h, int w)
 {
     const long long nq = (long long)h * ((w + 3) / 4);
@@ -503,6 +707,145 @@ int seg_vertex_losses(const float *seg_pred, const int64_t seg_strides[4], const
     return PVNET_OK;
 }
 
+// pvnet_seg_vertex_losses_backward (kp == NULL) and pvnet_seg_vertex_losses_keypoints_backward (kp)
+int seg_vertex_losses_backward(const float *seg_pred, const int64_t seg_strides[4], const void *mask,
+                               int mask_elem_size, const int64_t mask_strides[3], const float *vertex_pred,
+                               const int64_t pred_strides[4], const float *vertex, const int64_t vertex_strides[4],
+                               const KpArgs *kp, const float *vertex_weights, const int64_t weight_strides[4], int b,
+                               int h, int w, int C, int ver_dim, double sigma, int normalize,
+                               const float *grad_loss_seg, const float *grad_loss_vertex, float *grad_seg,
+                               const int64_t grad_seg_strides[4], float *grad_vertex,
+                               const int64_t grad_vertex_strides[4], void *workspace, size_t workspace_bytes,
+                               pvnet_stream_t stream)
+{
+    PV_CHECK_ARG(b >= 1 && h >= 1 && w >= 1, "non-positive dimension (b=%d, h=%d, w=%d)", b, h, w);
+    PV_CHECK_ARG(b <= 65535, "batch %d above 65535", b);
+    PV_CHECK_ARG(grad_seg || grad_vertex, "no output requested (grad_seg, grad_vertex both null)");
+    const bool do_ce = grad_seg && grad_loss_seg, do_ver = grad_vertex && grad_loss_vertex;
+    const bool need_mask = do_ce || (do_ver && kp);
+    if (grad_seg) {
+        PV_CHECK_ARG(grad_seg_strides, "null pointer (grad_seg_strides)");
+        PV_CHECK_ARG(C >= 1, "non-positive dimension (C=%d)", C);
+        PV_CHECK_ARG(grad_seg_strides[3] == 1, "unit stride along w is not 1 (grad_seg %lld)",
+                     (long long)grad_seg_strides[3]);
+    }
+    if (grad_vertex) {
+        PV_CHECK_ARG(grad_vertex_strides, "null pointer (grad_vertex_strides)");
+        PV_CHECK_ARG(ver_dim >= 1, "non-positive dimension (ver_dim=%d)", ver_dim);
+        PV_CHECK_ARG(grad_vertex_strides[3] == 1, "unit stride along w is not 1 (grad_vertex %lld)",
+                     (long long)grad_vertex_strides[3]);
+    }
+    if (do_ce) {
+        PV_CHECK_ARG(seg_pred && seg_strides, "null pointer (seg_pred or its strides)");
+        PV_CHECK_ARG(seg_strides[3] == 1, "unit stride along w is not 1 (seg %lld)", (long long)seg_strides[3]);
+    }
+    if (need_mask) {
+        PV_CHECK_ARG(mask && mask_strides, "null pointer (mask or its strides)");
+        PV_CHECK_ARG(mask_elem_size == 1 || mask_elem_size == 4 || mask_elem_size == 8,
+                     "mask_elem_size %d is not 1, 4 or 8", mask_elem_size);
+        PV_CHECK_ARG(mask_strides[2] == 1, "unit stride along w is not 1 (mask %lld)", (long long)mask_strides[2]);
+    }
+    if (do_ver) {
+        PV_CHECK_ARG(vertex_pred && pred_strides && vertex_weights && weight_strides,
+                     "null pointer (vertex_pred / vertex_weights or their strides)");
+        PV_CHECK_ARG(pred_strides[3] == 1 && weight_strides[3] == 1,
+                     "unit stride along w is not 1 (vertex_pred %lld, vertex_weights %lld)",
+                     (long long)pred_strides[3], (long long)weight_strides[3]);
+        if (kp) {
+            PV_CHECK_ARG(kp->hc, "null pointer (hcoords)");
+            PV_CHECK_ARG(ver_dim == 2 * kp->K, "ver_dim %d is not 2 x the number of keypoints", ver_dim);
+        } else {
+            PV_CHECK_ARG(vertex && vertex_strides, "null pointer (vertex or its strides)");
+            PV_CHECK_ARG(vertex_strides[3] == 1, "unit stride along w is not 1 (vertex %lld)",
+                         (long long)vertex_strides[3]);
+        }
+        PV_CHECK_ARG(sigma == sigma && sigma != 0.0, "sigma %g is zero or NaN", sigma);
+        PV_CHECK_ARG(normalize, "the gradient is that of the normalised loss (normalize must be nonzero)");
+    }
+    PV_CHECK_ARG(workspace, "null pointer (workspace)");
+    size_t need = 0;
+    if (pvnet_seg_vertex_losses_workspace_bytes(b, h, w, &need) != PVNET_OK) return PVNET_E_INVALID;
+    PV_CHECK_ARG(workspace_bytes >= need, "workspace %zu bytes < %zu", workspace_bytes, need);
+
+    LossArgs a = {};
+    GradArgs g = {};
+    a.h = h, a.w = w, a.C = C, a.vd = ver_dim, a.qw = (w + 3) / 4, a.nquads = h * a.qw;
+    bool vec = true;
+    if (grad_seg) {
+        g.gseg = grad_seg, g.gs_b = grad_seg_strides[0], g.gs_c = grad_seg_strides[1], g.gs_h = grad_seg_strides[2];
+        vec = vec && aligned(grad_seg, 16) && strides_ok(grad_seg_strides, 3);
+    }
+    if (grad_vertex) {
+        g.gver = grad_vertex, g.gv_b = grad_vertex_strides[0], g.gv_c = grad_vertex_strides[1];
+        g.gv_h = grad_vertex_strides[2];
+        vec = vec && aligned(grad_vertex, 16) && strides_ok(grad_vertex_strides, 3);
+    }
+    if (do_ce) {
+        a.seg = seg_pred, a.seg_b = seg_strides[0], a.seg_c = seg_strides[1], a.seg_h = seg_strides[2];
+        vec = vec && aligned(seg_pred, 16) && strides_ok(seg_strides, 3);
+        g.gls = grad_loss_seg;
+        g.inv_n = 1.0f / (float)((long long)h * w);    // ATen: opmath_t(1.0) / the scalar as opmath_t
+    }
+    if (need_mask) {
+        a.mask = mask, a.m_b = mask_strides[0], a.m_h = mask_strides[1];
+        vec = vec && aligned(mask, 4 * mask_elem_size) && strides_ok(mask_strides, 2);
+    }
+    if (do_ver) {
+        const double s2 = sigma * sigma;
+        a.c1 = (float)(1.0 / s2), a.c2 = (float)(s2 / 2.0);
+        a.pred = vertex_pred, a.p_b = pred_strides[0], a.p_c = pred_strides[1], a.p_h = pred_strides[2];
+        if (!kp) {
+            a.tgt = vertex, a.t_b = vertex_strides[0], a.t_c = vertex_strides[1], a.t_h = vertex_strides[2];
+            vec = vec && aligned(vertex, 16) && strides_ok(vertex_strides, 3);
+        }
+        a.wgt = vertex_weights, a.w_b = weight_strides[0], a.w_h = weight_strides[2];
+        vec = vec && aligned(vertex_pred, 16) && aligned(vertex_weights, 16) && strides_ok(pred_strides, 3) &&
+              weight_strides[0] % 4 == 0 && weight_strides[2] % 4 == 0;
+    }
+    a.vec = vec;
+    // workspace: Σw partials (double [b, chunks]), gi (float [b]), invalid-target flags (int [b, chunks])
+    const int chunks = ls_chunks(h, w);
+    double *wsum = static_cast<double *>(workspace);
+    float *gi = reinterpret_cast<float *>(wsum + (size_t)b * chunks);
+    g.bad = reinterpret_cast<int *>(gi + b);
+    const dim3 grid(chunks, b);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (do_ver) {
+        LossArgs wa = a;
+        wa.vec = aligned(vertex_weights, 16) && weight_strides[0] % 4 == 0 && weight_strides[2] % 4 == 0;
+        k_weight_sum_partial<<<grid, LS_THREADS, 0, st>>>(wa, wsum);
+        PV_LAUNCHED("k_weight_sum_partial");
+        k_grad_final<<<(b + 127) / 128, 128, 0, st>>>(wsum, chunks, b, ver_dim, grad_loss_vertex, gi);
+        PV_LAUNCHED("k_grad_final");
+        g.gi = gi;
+    }
+    const int msz = need_mask ? mask_elem_size : 8;
+    if (kp && do_ver) {
+        if (msz == 8)
+            k_losses_backward<long long, true><<<grid, LS_THREADS, 0, st>>>(a, g, *kp);
+        else if (msz == 4)
+            k_losses_backward<int, true><<<grid, LS_THREADS, 0, st>>>(a, g, *kp);
+        else
+            k_losses_backward<unsigned char, true><<<grid, LS_THREADS, 0, st>>>(a, g, *kp);
+        PV_LAUNCHED(msz == 8 ? "k_losses_backward<int64, keypoints>"
+                    : msz == 4 ? "k_losses_backward<int32, keypoints>" : "k_losses_backward<uint8, keypoints>");
+    } else {
+        if (msz == 8)
+            k_losses_backward<long long, false><<<grid, LS_THREADS, 0, st>>>(a, g, KpArgs{});
+        else if (msz == 4)
+            k_losses_backward<int, false><<<grid, LS_THREADS, 0, st>>>(a, g, KpArgs{});
+        else
+            k_losses_backward<unsigned char, false><<<grid, LS_THREADS, 0, st>>>(a, g, KpArgs{});
+        PV_LAUNCHED(msz == 8 ? "k_losses_backward<int64>" : msz == 4 ? "k_losses_backward<int32>"
+                                                                      : "k_losses_backward<uint8>");
+    }
+    if (do_ce) {
+        k_seg_grad_invalid<<<grid, LS_THREADS, 0, st>>>(a, g);
+        PV_LAUNCHED("k_seg_grad_invalid");
+    }
+    return PVNET_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -541,6 +884,39 @@ int pvnet_seg_vertex_losses_keypoints(const float *seg_pred, const int64_t seg_s
     return seg_vertex_losses(seg_pred, seg_strides, mask, mask_elem_size, mask_strides, vertex_pred, pred_strides,
                              nullptr, nullptr, &kp, vertex_weights, weight_strides, b, h, w, C, ver_dim, sigma,
                              normalize, loss_seg, loss_vertex, precision, recall, workspace, workspace_bytes, stream);
+}
+
+int pvnet_seg_vertex_losses_backward(const float *seg_pred, const int64_t seg_strides[4], const void *mask,
+                                     int mask_elem_size, const int64_t mask_strides[3], const float *vertex_pred,
+                                     const int64_t pred_strides[4], const float *vertex,
+                                     const int64_t vertex_strides[4], const float *vertex_weights,
+                                     const int64_t weight_strides[4], int b, int h, int w, int C, int ver_dim,
+                                     double sigma, int normalize, const float *grad_loss_seg,
+                                     const float *grad_loss_vertex, float *grad_seg, const int64_t grad_seg_strides[4],
+                                     float *grad_vertex, const int64_t grad_vertex_strides[4], void *workspace,
+                                     size_t workspace_bytes, pvnet_stream_t stream)
+{
+    return seg_vertex_losses_backward(seg_pred, seg_strides, mask, mask_elem_size, mask_strides, vertex_pred,
+                                      pred_strides, vertex, vertex_strides, nullptr, vertex_weights, weight_strides, b,
+                                      h, w, C, ver_dim, sigma, normalize, grad_loss_seg, grad_loss_vertex, grad_seg,
+                                      grad_seg_strides, grad_vertex, grad_vertex_strides, workspace, workspace_bytes,
+                                      stream);
+}
+
+int pvnet_seg_vertex_losses_keypoints_backward(
+    const float *seg_pred, const int64_t seg_strides[4], const void *mask, int mask_elem_size,
+    const int64_t mask_strides[3], const float *vertex_pred, const int64_t pred_strides[4], const void *hcoords,
+    int hcoords_f64, int use_motion, const float *vertex_weights, const int64_t weight_strides[4], int b, int h, int w,
+    int C, int ver_dim, double sigma, int normalize, const float *grad_loss_seg, const float *grad_loss_vertex,
+    float *grad_seg, const int64_t grad_seg_strides[4], float *grad_vertex, const int64_t grad_vertex_strides[4],
+    void *workspace, size_t workspace_bytes, pvnet_stream_t stream)
+{
+    const KpArgs kp = {hcoords, ver_dim / 2, hcoords_f64 != 0, use_motion != 0};
+    return seg_vertex_losses_backward(seg_pred, seg_strides, mask, mask_elem_size, mask_strides, vertex_pred,
+                                      pred_strides, nullptr, nullptr, &kp, vertex_weights, weight_strides, b, h, w, C,
+                                      ver_dim, sigma, normalize, grad_loss_seg, grad_loss_vertex, grad_seg,
+                                      grad_seg_strides, grad_vertex, grad_vertex_strides, workspace, workspace_bytes,
+                                      stream);
 }
 
 int pvnet_vertex_targets(const void *mask, int mask_elem_size, const int64_t mask_strides[3], const void *hcoords,

@@ -11,13 +11,18 @@ reference's entry points import from that module.
                                    the loader's ground-truth vertex field [b,2K,h,w] (compute_vertex_hcoords)
     seg_vertex_losses_from_keypoints(seg_pred, vertex_pred, mask, hcoords, vertex_weights, use_motion=False)
                                    seg_vertex_losses with that field computed in registers, never stored
+    seg_vertex_training_losses(seg_pred, vertex_pred, mask, vertex, vertex_weights)
+    seg_vertex_training_losses_from_keypoints(seg_pred, vertex_pred, mask, hcoords, vertex_weights, use_motion=False)
+                                   the same two with loss_seg / loss_vertex differentiable through the device
+                                   backward (training)
     NetWrapper(net)                the reference's NetWrapper with the fused call in eval / no_grad
     AverageMeter, Recorder, load_model, save_model, adjust_learning_rate, set_learning_rate
 
 Inputs are read in place through their strides (seg_pred / vertex_pred may be channel slices of the network's one
 output tensor).  When grad is enabled and an input requires grad (training; tools/demo.py, which runs the network in
-train mode) the functions evaluate the same semantics as torch expressions so that backward() works, as
-Resnet18_8s runs its train mode in PyTorch.  Otherwise there is no CPU path: CPU tensors raise RuntimeError.
+train mode) the functions other than the two *_training_losses evaluate the same semantics as torch expressions so
+that backward() works, as Resnet18_8s runs its train mode in PyTorch.  Otherwise there is no CPU path: CPU tensors
+raise RuntimeError.
 Importing this module loads neither tensorboardX, easydict, torchvision nor matplotlib.
 """
 from __future__ import annotations
@@ -28,6 +33,8 @@ import re
 
 import torch
 from torch import nn
+from torch.autograd.function import once_differentiable
+from torch.autograd.graph import get_gradient_edge
 from torch.nn import functional as F
 
 from . import _native
@@ -78,6 +85,29 @@ def _check_keypoints(mask, hcoords):
         raise ValueError(f"hcoords must be float32 or float64, got {hcoords.dtype}")
 
 
+def _check_field_losses(seg_pred, vertex_pred, mask, vertex, vertex_weights):
+    _check_seg(seg_pred, mask)
+    _check_vertex(vertex_pred, vertex, vertex_weights)
+    if seg_pred.shape[0] != vertex_pred.shape[0] or seg_pred.shape[2:] != vertex_pred.shape[2:]:
+        raise ValueError(f"seg_pred {tuple(seg_pred.shape)} and vertex_pred {tuple(vertex_pred.shape)} differ in b,h,w")
+
+
+def _check_keypoint_losses(seg_pred, vertex_pred, mask, hcoords, vertex_weights):
+    _check_seg(seg_pred, mask)
+    for name, x in (("vertex_pred", vertex_pred), ("vertex_weights", vertex_weights)):
+        _check_float(name, x)
+    if vertex_pred.dim() != 4:
+        raise ValueError(f"vertex_pred must be [b,ver_dim,h,w], got {tuple(vertex_pred.shape)}")
+    b, vd, h, w = vertex_pred.shape
+    if tuple(vertex_weights.shape) != (b, 1, h, w):
+        raise ValueError(f"vertex_weights must be [b,1,h,w] = {(b, 1, h, w)}, got {tuple(vertex_weights.shape)}")
+    if seg_pred.shape[0] != b or seg_pred.shape[2:] != vertex_pred.shape[2:]:
+        raise ValueError(f"seg_pred {tuple(seg_pred.shape)} and vertex_pred {tuple(vertex_pred.shape)} differ in b,h,w")
+    _check_keypoints(mask, hcoords)
+    if vd != 2 * hcoords.shape[1]:
+        raise ValueError(f"ver_dim {vd} is not 2 x the {hcoords.shape[1]} keypoints of hcoords")
+
+
 def _check_seg(scores, target):
     _check_float("seg_pred", scores)
     if scores.dim() != 4:
@@ -89,10 +119,9 @@ def _check_seg(scores, target):
         raise ValueError(f"mask dtype {target.dtype} is not one of int64, int32, uint8, bool")
 
 
-def _native_losses(seg=None, mask=None, pred=None, tgt=None, wgt=None, sigma=1.0, normalize=True,
-                   want=("seg", "ver", "precision", "recall"), hcoords=None, use_motion=False):
-    """One pvnet_seg_vertex_losses call (pvnet_seg_vertex_losses_keypoints when `hcoords` replaces `tgt`); returns
-    {part: tensor} for the parts in `want`."""
+def _input_args(seg, mask, pred, tgt, wgt, hcoords, use_motion):
+    """The input arguments shared by the loss entry points and their backward, in C-ABI order, with the tensors they
+    point into (kept alive by the caller), (b, h, w, C, ver_dim) and the device."""
     xs = [x for x in (seg, mask, pred, tgt, wgt, hcoords) if x is not None]
     if not all(x.is_cuda for x in xs):
         raise RuntimeError("pvnet_b200: the validation losses need CUDA tensors (there is no CPU path)")
@@ -101,7 +130,6 @@ def _native_losses(seg=None, mask=None, pred=None, tgt=None, wgt=None, sigma=1.0
         raise ValueError("all inputs must be on the same device")
     ref = seg if seg is not None else pred
     b, _, h, w = ref.shape
-    L = _native.lib()
     args = []
     C = vd = 0
     if seg is not None:
@@ -129,6 +157,15 @@ def _native_losses(seg=None, mask=None, pred=None, tgt=None, wgt=None, sigma=1.0
         args += [wgt.data_ptr(), s_wgt]
     else:
         args += [None] * (6 if hcoords is None else 7)
+    return args, (seg, mask, pred, tgt, wgt, hcoords), (b, h, w, C, vd), dev
+
+
+def _native_losses(seg=None, mask=None, pred=None, tgt=None, wgt=None, sigma=1.0, normalize=True,
+                   want=("seg", "ver", "precision", "recall"), hcoords=None, use_motion=False):
+    """One pvnet_seg_vertex_losses call (pvnet_seg_vertex_losses_keypoints when `hcoords` replaces `tgt`); returns
+    {part: tensor} for the parts in `want`."""
+    args, keep, (b, h, w, C, vd), dev = _input_args(seg, mask, pred, tgt, wgt, hcoords, use_motion)
+    L = _native.lib()
     out = {}
     for part in want:
         shape = [b, vd, h, w] if part == "ver" and not normalize else [b]
@@ -146,6 +183,101 @@ def _native_losses(seg=None, mask=None, pred=None, tgt=None, wgt=None, sigma=1.0
                                        ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
                       name)
     return out
+
+
+def _native_losses_backward(seg, mask, pred, tgt, wgt, hcoords, use_motion, g_seg, g_ver, grad_seg, grad_ver):
+    """One pvnet_seg_vertex_losses_backward call (_keypoints_backward when `hcoords` replaces `tgt`) writing
+    grad_seg / grad_ver (either may be None) from the loss gradients g_seg / g_ver ([b] or None)."""
+    args, keep, (b, h, w, C, vd), dev = _input_args(seg, mask, pred, tgt, wgt, hcoords, use_motion)
+    L = _native.lib()
+    g_seg, g_ver = (None if g is None else g.detach().float().contiguous() for g in (g_seg, g_ver))
+    outs = []
+    for g in (grad_seg, grad_ver):
+        if g is None:
+            outs += [None, None]
+        else:
+            outs += [g.data_ptr(), (ctypes.c_int64 * 4)(*g.stride())]
+    nbytes = ctypes.c_size_t()
+    _native.check(L.pvnet_seg_vertex_losses_workspace_bytes(b, h, w, ctypes.byref(nbytes)),
+                  "pvnet_seg_vertex_losses_workspace_bytes")
+    ws = torch.empty([nbytes.value], dtype=torch.uint8, device=dev)
+    name = "pvnet_seg_vertex_losses_backward" if hcoords is None else "pvnet_seg_vertex_losses_keypoints_backward"
+    with torch.cuda.device(dev):
+        _native.check(getattr(L, name)(*args, b, h, w, C, vd, 1.0, 1,
+                                       None if g_seg is None else g_seg.data_ptr(),
+                                       None if g_ver is None else g_ver.data_ptr(), *outs, ws.data_ptr(),
+                                       nbytes.value, ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
+                      name)
+
+
+class _TrainingLosses(torch.autograd.Function):
+    """loss_seg, loss_vertex, precision, recall of one pvnet_seg_vertex_losses[_keypoints] call, with the backward
+    of the first two.  x is seg_pred, or (vertex_pred None) the [b,C+vd,h,w] tensor whose channel ranges [0,C) and
+    [C,C+vd) are seg_pred and vertex_pred: its gradient is then written once, as one tensor."""
+
+    @staticmethod
+    def forward(ctx, x, vertex_pred, mask, vertex, weights, hcoords, use_motion, C):
+        seg, pred = (x[:, :C], x[:, C:]) if vertex_pred is None else (x, vertex_pred)
+        r = _native_losses(seg, mask, pred, vertex, weights, hcoords=hcoords, use_motion=use_motion)
+        ctx.save_for_backward(x, vertex_pred, mask, vertex, weights, hcoords)
+        ctx.use_motion, ctx.C = use_motion, C
+        ctx.mark_non_differentiable(r["precision"], r["recall"])
+        ctx.set_materialize_grads(False)
+        return r["seg"], r["ver"], r["precision"], r["recall"]
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g_seg, g_ver, _g_precision, _g_recall):
+        x, vertex_pred, mask, vertex, weights, hcoords = ctx.saved_tensors
+        C = ctx.C
+        none = (None,) * 6
+        if g_seg is None and g_ver is None:
+            return (None, None) + none
+        if vertex_pred is None:
+            gx = torch.empty(x.shape, dtype=torch.float32, device=x.device)
+            _native_losses_backward(x[:, :C], mask, x[:, C:], vertex, weights, hcoords, ctx.use_motion, g_seg, g_ver,
+                                    gx[:, :C], gx[:, C:])
+            return (gx, None) + none
+        gs = None if g_seg is None else torch.empty(x.shape, dtype=torch.float32, device=x.device)
+        gv = None if g_ver is None else torch.empty(vertex_pred.shape, dtype=torch.float32, device=x.device)
+        _native_losses_backward(x, mask, vertex_pred, vertex, weights, hcoords, ctx.use_motion, g_seg, g_ver, gs, gv)
+        return (gs, gv) + none
+
+
+def _one_output(seg_pred, vertex_pred):
+    """The 4-D tensor whose channel ranges [0,C) and [C,C+vd) seg_pred and vertex_pred are, when gradients reach it
+    through those two views alone; otherwise None."""
+    base = seg_pred._base
+    if base is None or vertex_pred._base is not base or base.dim() != 4 or not base.requires_grad:
+        return None
+    b, C, h, w = seg_pred.shape
+    if tuple(base.shape) != (b, C + vertex_pred.shape[1], h, w) or base.dtype != torch.float32:
+        return None
+    if seg_pred.stride() != base.stride() or vertex_pred.stride() != base.stride():
+        return None
+    if (seg_pred.storage_offset() != base.storage_offset()
+            or vertex_pred.storage_offset() != base.storage_offset() + C * base.stride(1)):
+        return None
+    edge = get_gradient_edge(base)
+    for x in (seg_pred, vertex_pred):
+        nxt = x.grad_fn.next_functions if x.grad_fn is not None else ()
+        if len(nxt) != 1 or nxt[0][0] is not edge.node or nxt[0][1] != edge.output_nr:
+            return None
+    return base
+
+
+def _training_losses(seg_pred, vertex_pred, mask, vertex, vertex_weights, hcoords, use_motion):
+    xs = [x for x in (seg_pred, vertex_pred, mask, vertex, vertex_weights, hcoords) if x is not None]
+    if not all(x.is_cuda for x in xs):
+        raise RuntimeError("pvnet_b200: the training losses need CUDA tensors (there is no CPU path)")
+    for name, x in (("vertex", vertex), ("vertex_weights", vertex_weights), ("hcoords", hcoords)):
+        if x is not None and x.requires_grad:
+            raise ValueError(f"{name} requires grad: only seg_pred and vertex_pred get gradients")
+    C = seg_pred.shape[1]
+    base = _one_output(seg_pred, vertex_pred) if torch.is_grad_enabled() else None
+    if base is not None:
+        return _TrainingLosses.apply(base, None, mask, vertex, vertex_weights, hcoords, use_motion, C)
+    return _TrainingLosses.apply(seg_pred, vertex_pred, mask, vertex, vertex_weights, hcoords, use_motion, C)
 
 
 # ----------------------------------------------------------------------------- torch expressions (grad mode)
@@ -215,10 +347,7 @@ def seg_vertex_losses(seg_pred, vertex_pred, mask, vertex, vertex_weights):
     """The four per-image figures of NetWrapper.forward (train_linemod.py:87-90) in one pass:
     loss_seg (cross-entropy, mean over pixels), loss_vertex (smooth_l1_loss, normalize=True), precision, recall;
     each float32 [b]."""
-    _check_seg(seg_pred, mask)
-    _check_vertex(vertex_pred, vertex, vertex_weights)
-    if seg_pred.shape[0] != vertex_pred.shape[0] or seg_pred.shape[2:] != vertex_pred.shape[2:]:
-        raise ValueError(f"seg_pred {tuple(seg_pred.shape)} and vertex_pred {tuple(vertex_pred.shape)} differ in b,h,w")
+    _check_field_losses(seg_pred, vertex_pred, mask, vertex, vertex_weights)
     if _use_torch(seg_pred, vertex_pred, vertex, vertex_weights):
         precision, recall = _precision_recall_torch(seg_pred, mask)
         return (_cross_entropy_torch(seg_pred, mask),
@@ -259,19 +388,7 @@ def seg_vertex_losses_from_keypoints(seg_pred, vertex_pred, mask, hcoords, verte
     vertex_targets(mask, hcoords, use_motion), vertex_weights), in one launch pair that never materialises the field.
     hcoords [b,K,3] float32 or float64, with ver_dim == 2K.  In grad mode the field is materialised with
     vertex_targets and the torch expressions evaluated on it."""
-    _check_seg(seg_pred, mask)
-    for name, x in (("vertex_pred", vertex_pred), ("vertex_weights", vertex_weights)):
-        _check_float(name, x)
-    if vertex_pred.dim() != 4:
-        raise ValueError(f"vertex_pred must be [b,ver_dim,h,w], got {tuple(vertex_pred.shape)}")
-    b, vd, h, w = vertex_pred.shape
-    if tuple(vertex_weights.shape) != (b, 1, h, w):
-        raise ValueError(f"vertex_weights must be [b,1,h,w] = {(b, 1, h, w)}, got {tuple(vertex_weights.shape)}")
-    if seg_pred.shape[0] != b or seg_pred.shape[2:] != vertex_pred.shape[2:]:
-        raise ValueError(f"seg_pred {tuple(seg_pred.shape)} and vertex_pred {tuple(vertex_pred.shape)} differ in b,h,w")
-    _check_keypoints(mask, hcoords)
-    if vd != 2 * hcoords.shape[1]:
-        raise ValueError(f"ver_dim {vd} is not 2 x the {hcoords.shape[1]} keypoints of hcoords")
+    _check_keypoint_losses(seg_pred, vertex_pred, mask, hcoords, vertex_weights)
     if _use_torch(seg_pred, vertex_pred, vertex_weights):
         vertex = vertex_targets(mask, hcoords, use_motion)
         precision, recall = _precision_recall_torch(seg_pred, mask)
@@ -279,6 +396,25 @@ def seg_vertex_losses_from_keypoints(seg_pred, vertex_pred, mask, hcoords, verte
                 _smooth_l1_torch(vertex_pred, vertex, vertex_weights, 1.0, True), precision, recall)
     r = _native_losses(seg_pred, mask, vertex_pred, None, vertex_weights, hcoords=hcoords, use_motion=use_motion)
     return r["seg"], r["ver"], r["precision"], r["recall"]
+
+
+def seg_vertex_training_losses(seg_pred, vertex_pred, mask, vertex, vertex_weights):
+    """seg_vertex_losses for training: the same four float32 [b] figures from the same kernel (bit-identical to
+    seg_vertex_losses without grad), with loss_seg and loss_vertex differentiable with respect to seg_pred and
+    vertex_pred through the device backward (pvnet_seg_vertex_losses_backward, DESIGN.md §13); precision and recall
+    are not differentiable.  When seg_pred and vertex_pred are the channel slices [0,C) and [C,C+vd) of one output
+    tensor (Resnet18_8s.forward), the gradient is written once into a tensor of that output's shape.  CUDA tensors
+    only; vertex and vertex_weights must not require grad (ValueError)."""
+    _check_field_losses(seg_pred, vertex_pred, mask, vertex, vertex_weights)
+    return _training_losses(seg_pred, vertex_pred, mask, vertex, vertex_weights, None, False)
+
+
+def seg_vertex_training_losses_from_keypoints(seg_pred, vertex_pred, mask, hcoords, vertex_weights, use_motion=False):
+    """seg_vertex_training_losses with the vertex targets computed from the keypoints as
+    seg_vertex_losses_from_keypoints does, in the forward and in the backward: the [b,2K,h,w] field is never
+    stored.  hcoords must not require grad (ValueError)."""
+    _check_keypoint_losses(seg_pred, vertex_pred, mask, hcoords, vertex_weights)
+    return _training_losses(seg_pred, vertex_pred, mask, None, vertex_weights, hcoords, use_motion)
 
 
 class NetWrapper(nn.Module):
