@@ -447,6 +447,37 @@ PVNET_API int pvnet_conv2d_nhwc(const float *in, int in_cs, int in_co, int Cin,
                                 int b, int H, int W, int ksize, int stride, int dilation,
                                 int act, int round_out, pvnet_stream_t stream);
 
+/* Weight gradient of a stride-1 NHWC convolution on the Hopper tensor cores (wgmma, TF32 operands, fp32
+ * accumulate): the dW half of the backward that autograd runs through the convolutions of
+ * lib/networks/resnet.py:28-35,54-70 and model_repository.py:22-58 during training.
+ *
+ *   dw[co][ci][kh][kw] = sum_{n,y,x} dout[n,y,x,dout_co+co] * in[n, y+(kh-c)*dil, x+(kw-c)*dil, in_co+ci]
+ *                        c = (ksize-1)/2, out-of-image `in` reads are zero (padding dilation*(ksize-1)/2)
+ *
+ *   in        NHWC [b,H,W,in_cs], the forward's input, read at channels [in_co, in_co+Cin)
+ *   dout      NHWC [b,H,W,dout_cs], the gradient of the forward's output (same grid: stride 1), read at
+ *             [dout_co, dout_co+Cout).  A stride-2 layer's gradient is first spread onto the input's grid
+ *             with pvnet_zero_insert2x_nhwc; its dW is then this stride-1 form with the same padding.
+ *   dw        [Cout][Cin][ksize][ksize] fp32 contiguous (torch's Conv2d.weight layout), overwritten
+ *   ksize 1|3, dilation >= 1; Cin, Cout, strides and offsets multiples of 4 floats; in/dout 16-byte aligned.
+ * Both operands enter the MMA as TF32 (the low 13 mantissa bits are ignored).  The pixels are split over CTAs
+ * whose partial tiles go to `workspace` (pvnet_conv2d_nhwc_wgrad_workspace_bytes, which depends on the shape
+ * and on the current device) and are summed in a fixed order: the result is identical run to run.  Allocates
+ * nothing, launches two kernels on `stream`. */
+PVNET_API int pvnet_conv2d_nhwc_wgrad_workspace_bytes(int Cin, int Cout, int b, int H, int W, int ksize,
+                                                      size_t *bytes);
+PVNET_API int pvnet_conv2d_nhwc_wgrad(const float *in, int in_cs, int in_co, int Cin,
+                                      const float *dout, int dout_cs, int dout_co, int Cout, float *dw,
+                                      int b, int H, int W, int ksize, int dilation,
+                                      void *workspace, size_t workspace_bytes, pvnet_stream_t stream);
+/* Zero insertion for the stride-2 convolutions' backward (layer2.0.conv1, layer2.0.downsample.0):
+ *   out[n,y,x,out_co+c] = (y, x even) ? in[n,y/2,x/2,in_co+c] : 0      on the full H x W grid
+ * in NHWC [b,H/2,W/2,in_cs], out NHWC [b,H,W,out_cs]; H, W even; C, strides and offsets multiples of 4 floats.
+ * With it dX = pvnet_conv2d_nhwc(out, flipped transposed weights, stride 1, padding (k-1)/2) and
+ * dW = pvnet_conv2d_nhwc_wgrad(X, out). */
+PVNET_API int pvnet_zero_insert2x_nhwc(const float *in, int in_cs, int in_co, int C, float *out, int out_cs,
+                                       int out_co, int b, int H, int W, pvnet_stream_t stream);
+
 /* Test hook: which convolution kernel pvnet_conv2d_nhwc / the backbone use for layers both can
  * run.  0 = automatic (persistent weights-resident column kernel for 3x3 stride-1 layers with
  * Cout <= 64 whose weights fit in shared memory, per-tap kernel otherwise), 1 = per-tap kernel

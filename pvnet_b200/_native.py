@@ -92,6 +92,12 @@ SIGNATURES = {
     "pvnet_conv2d_nhwc": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int,
                                   c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
                                   c_int, c_int, c_void_p]),
+    "pvnet_conv2d_nhwc_wgrad_workspace_bytes": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int,
+                                                        ctypes.POINTER(c_size_t)]),
+    "pvnet_conv2d_nhwc_wgrad": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_int, c_void_p,
+                                        c_int, c_int, c_int, c_int, c_int, c_void_p, c_size_t, c_void_p]),
+    "pvnet_zero_insert2x_nhwc": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int,
+                                         c_void_p]),
     "pvnet_conv_set_mode": (c_int, [c_int]),
     "pvnet_conv_set_multicast": (c_int, [c_int]),
     "pvnet_conv_set_persistent": (c_int, [c_int]),

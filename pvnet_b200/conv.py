@@ -10,6 +10,7 @@ from __future__ import annotations
 import ctypes
 
 import torch
+from torch.autograd.function import once_differentiable
 
 from . import _native
 
@@ -102,3 +103,104 @@ def conv2d_nhwc(inp, in_co, cin, w_packed, bias, out, out_co, cout, ksize, strid
             _p(out), out.shape[3], out_co, cout, b, H, W, ksize, stride, dilation, act, int(round_out),
             ctypes.c_void_p(torch.cuda.current_stream(inp.device).cuda_stream)), "pvnet_conv2d_nhwc")
     return out
+
+
+# ----------------------------------------------------------------------------- training (autograd)
+def pack_dgrad_weight(w: torch.Tensor, n: int | None = None, tf32: bool = True) -> torch.Tensor:
+    """[Cout,Cin,k,k] -> the data-gradient operand [n][k*k][cin_padded(Cout)]: taps flipped (kh,kw) ->
+    (k-1-kh,k-1-kw), Cout and Cin swapped, rounded to TF32; n (default Cin) keeps the first n input channels.
+    pvnet_conv2d_nhwc(dY, this, bias 0, act none, same dilation and padding) is then conv2d_input of a stride-1
+    convolution (of a stride-2 one on the zero-inserted dY)."""
+    wt = w.detach().flip(2, 3).transpose(0, 1)
+    return pack_weight(wt if n is None else wt[:n], tf32=tf32)
+
+
+def conv2d_nhwc_wgrad(inp, in_co, cin, dout, dout_co, cout, ksize, dilation=1):
+    """pvnet_conv2d_nhwc_wgrad: inp [b,H,W,in_cs] and dout [b,H,W,dout_cs] contiguous NHWC fp32 on one device
+    -> dW [cout,cin,ksize,ksize] fp32 (workspace from the caching allocator, current stream)."""
+    b, H, W, in_cs = inp.shape
+    L = _native.lib()
+    dev = inp.device
+    with torch.cuda.device(dev):
+        n = ctypes.c_size_t()
+        _native.check(L.pvnet_conv2d_nhwc_wgrad_workspace_bytes(cin, cout, b, H, W, ksize, ctypes.byref(n)),
+                      "pvnet_conv2d_nhwc_wgrad_workspace_bytes")
+        ws = torch.empty(max(n.value, 16), dtype=torch.uint8, device=dev)
+        dw = torch.empty(cout, cin, ksize, ksize, dtype=torch.float32, device=dev)
+        _native.check(L.pvnet_conv2d_nhwc_wgrad(
+            _p(inp), in_cs, in_co, cin, _p(dout), dout.shape[3], dout_co, cout, _p(dw), b, H, W, ksize, dilation,
+            _p(ws), ws.numel(), ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "pvnet_conv2d_nhwc_wgrad")
+    return dw
+
+
+def zero_insert2x(inp, out=None):
+    """pvnet_zero_insert2x_nhwc: inp [b,h,w,C] contiguous NHWC -> [b,2h,2w,C] with inp at the even pixels, 0 elsewhere."""
+    b, h, w, C = inp.shape
+    if out is None:
+        out = torch.empty(b, 2 * h, 2 * w, C, dtype=torch.float32, device=inp.device)
+    with torch.cuda.device(inp.device):
+        _native.check(_native.lib().pvnet_zero_insert2x_nhwc(
+            _p(inp), C, 0, C, _p(out), out.shape[3], 0, b, 2 * h, 2 * w,
+            ctypes.c_void_p(torch.cuda.current_stream(inp.device).cuda_stream)), "pvnet_zero_insert2x_nhwc")
+    return out
+
+
+def _nhwc(t):
+    """[b,C,H,W] -> its [b,H,W,C] view, after making the storage channels_last."""
+    return t.contiguous(memory_format=torch.channels_last).permute(0, 2, 3, 1)
+
+
+class Conv2dNHWC(torch.autograd.Function):
+    """One bias-free convolution of a [b,C,H,W] channels_last tensor (physically NHWC) with a torch
+    [Cout,Cin,k,k] weight, Cin <= C (the weight is zero-extended over the input's extra channels).  padding =
+    dilation*(k-1)/2, the only padding Resnet18_8s uses.  Forward: pvnet_conv2d_nhwc.  Backward: the data gradient
+    as pvnet_conv2d_nhwc of dY with pack_dgrad_weight (only input channels [0, dgrad_channels) get one; the rest
+    are zero) and pvnet_conv2d_nhwc_wgrad; a stride-2 layer first zero-inserts dY.  Runs on the input's device and
+    its current stream."""
+
+    @staticmethod
+    def forward(ctx, x, weight, stride, dilation, dgrad_channels):
+        b, C, H, W = x.shape
+        cout, cin, k, _ = weight.shape
+        if not x.is_cuda or x.dtype != torch.float32 or weight.dtype != torch.float32:
+            raise ValueError("Conv2dNHWC needs float32 CUDA tensors")
+        if cin > C:
+            raise ValueError(f"weight has {cin} input channels, the input {C}")
+        xh = _nhwc(x)
+        out = torch.empty(b, cout, H // stride, W // stride, dtype=torch.float32, device=x.device,
+                          memory_format=torch.channels_last)
+        wp = pack_weight(weight.detach(), cin_pad=cin_padded(C))
+        bias = torch.zeros(cout, dtype=torch.float32, device=x.device)
+        conv2d_nhwc(xh, 0, C, wp, bias, out.permute(0, 2, 3, 1), 0, cout, k, stride, dilation)
+        ctx.save_for_backward(xh, weight)
+        ctx.stride, ctx.dilation, ctx.dgrad_channels = stride, dilation, dgrad_channels
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gy):
+        xh, weight = ctx.saved_tensors
+        b, H, W, C = xh.shape
+        cout, cin, k, _ = weight.shape
+        gyh = _nhwc(gy.float())
+        if ctx.stride == 2:
+            gyh = zero_insert2x(gyh)
+        dx = dw = None
+        if ctx.needs_input_grad[0]:
+            n = C if ctx.dgrad_channels is None else ctx.dgrad_channels
+            dx = torch.empty(b, C, H, W, dtype=torch.float32, device=xh.device, memory_format=torch.channels_last)
+            if n < C:
+                dx[:, n:].zero_()
+            bias = torch.zeros(n, dtype=torch.float32, device=xh.device)
+            conv2d_nhwc(gyh, 0, cout, pack_dgrad_weight(weight, n), bias, dx.permute(0, 2, 3, 1), 0, n, k, 1,
+                        ctx.dilation)
+        if ctx.needs_input_grad[1]:
+            dw = conv2d_nhwc_wgrad(xh, 0, C, gyh, 0, cout, k, ctx.dilation)
+            if cin < C:
+                dw = dw[:, :cin].contiguous()
+        return dx, dw, None, None, None
+
+
+def conv2d_train(x, weight, stride=1, dilation=1, dgrad_channels=None):
+    """Conv2dNHWC.apply: the native convolution under autograd (see Conv2dNHWC)."""
+    return Conv2dNHWC.apply(x, weight, stride, dilation, dgrad_channels)

@@ -20,8 +20,9 @@ sm_90a backbone (wgmma implicit-GEMM convs behind include/pvnet_b200.h).
   native handles and packed weights (keyed by the source module's weight versions), so weights are
   packed once per device, never per forward, and a handle is destroyed exactly once.
 * train mode (BatchNorm batch statistics, autograd; also what tools/demo.py runs because it
-  never calls .eval(), SURVEY App. C.6) -> the plain PyTorch graph below, as SURVEY.md §7
-  prescribes; training is out of scope for the native path.
+  never calls .eval(), SURVEY App. C.6) -> `forward` runs the plain PyTorch graph below, as SURVEY.md §7
+  prescribes.  `forward_train` is the same graph with its 24 trunk/decoder convolutions (forward, data and
+  weight gradients) on the native kernels (DESIGN.md §14).
 """
 from __future__ import annotations
 
@@ -311,6 +312,65 @@ class Resnet18_8s(nn.Module):
             ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
             self._nat.workspaces[key] = ws
         return ws
+
+    # ------------------------------------------------------------------ training path
+    @staticmethod
+    def _conv_bn_act(seq, x, dgrad_channels=None):
+        """nn.Sequential(Conv2d, BatchNorm2d, activation) with the convolution on the native kernels."""
+        conv = seq[0]
+        y = pc.conv2d_train(x, conv.weight, conv.stride[0], conv.dilation[0], dgrad_channels)
+        return seq[2](seq[1](y))
+
+    @staticmethod
+    def _block_train(blk, x):
+        """resnet.BasicBlock.forward with its two (three) convolutions on the native kernels."""
+        y = blk.relu(blk.bn1(pc.conv2d_train(x, blk.conv1.weight, blk.conv1.stride[0], blk.conv1.dilation[0])))
+        y = blk.bn2(pc.conv2d_train(y, blk.conv2.weight, 1, blk.conv2.dilation[0]))
+        if blk.downsample is None:
+            skip = x
+        else:
+            ds = blk.downsample
+            skip = ds[1](pc.conv2d_train(x, ds[0].weight, ds[0].stride[0], 1))
+        return blk.relu(y + skip)
+
+    def forward_train(self, x):
+        """The train-mode forward (`_forward_torch`) with the 24 convolutions of slots 1..24 on the native tensor-core
+        kernels under autograd (pvnet_b200.conv.Conv2dNHWC: pvnet_conv2d_nhwc forward, its data gradient and
+        pvnet_conv2d_nhwc_wgrad backward).  Activations are channels_last, so the BatchNorm, ReLU/LeakyReLU, max-pool,
+        cat and upsampling modules -- called as themselves, following their own `training` flag and updating their
+        running statistics as nn.BatchNorm2d does -- run on the NHWC storage without layout copies.  The stem and
+        the head convraw.3 stay torch convolutions.  convraw.0 reads cat[fm, image, 5 zero channels] like the eval
+        path; the image gets no gradient, so it must not require one (ValueError).
+
+        Returns (seg_pred, ver_pred), the channel slices of one contiguous NCHW tensor: the training losses then
+        write a single gradient for it, and read it on their vectorised path (a channels_last head would leave
+        them strided).  NetWrapper's change: `seg_pred, vertex_pred = self.net.forward_train(image)`."""
+        if x.requires_grad:
+            raise ValueError("forward_train: the input image must not require grad (it gets no gradient)")
+        if not x.is_cuda:
+            raise RuntimeError("pvnet_b200: forward_train runs only on CUDA (no CPU fallback)")
+        cl = torch.channels_last
+        x = x.float().contiguous(memory_format=cl)
+        t = self.resnet18_8s
+        x2s = t.relu(t.bn1(t.conv1(x)))
+        x4s = t.maxpool(x2s)
+        for blk in t.layer1:
+            x4s = self._block_train(blk, x4s)
+        x8s = x4s
+        for blk in t.layer2:
+            x8s = self._block_train(blk, x8s)
+        x32s = x8s
+        for blk in (*t.layer3, *t.layer4):
+            x32s = self._block_train(blk, x32s)
+        xfc = self._conv_bn_act(t.fc, x32s)
+        fm = self.up8sto4s(self._conv_bn_act(self.conv8s, torch.cat([xfc, x8s], 1)))
+        fm = self.up4sto2s(self._conv_bn_act(self.conv4s, torch.cat([fm, x4s], 1)))
+        fm = self.up2storaw(self._conv_bn_act(self.conv2s, torch.cat([fm, x2s], 1)))
+        b, _, h, w = x.shape
+        pad = torch.zeros(b, 5, h, w, dtype=torch.float32, device=x.device).contiguous(memory_format=cl)
+        y = self._conv_bn_act(self.convraw, torch.cat([fm, x, pad], 1), dgrad_channels=fm.shape[1])
+        out = self.convraw[3](y).contiguous()
+        return out[:, :self.seg_dim], out[:, self.seg_dim:]
 
     def forward(self, x, feature_alignment=False):
         if self.training or not x.is_cuda:
