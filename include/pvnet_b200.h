@@ -478,6 +478,25 @@ PVNET_API int pvnet_conv2d_nhwc_wgrad(const float *in, int in_cs, int in_co, int
 PVNET_API int pvnet_zero_insert2x_nhwc(const float *in, int in_cs, int in_co, int C, float *out, int out_cs,
                                        int out_co, int b, int H, int W, pvnet_stream_t stream);
 
+/* Bilinear x2 upsampling with align_corners=True (nn.UpsamplingBilinear2d(scale_factor=2),
+ * lib/networks/model_repository.py:35,43,51) for training, forward and backward.
+ *
+ * pvnet_upsample2x_nhwc: in NHWC [b,h,w,C] dense -> out NHWC [b,2h,2w,out_cs] at channels [out_co, out_co+C), the
+ *   other channels untouched.  Exact fp32 (not rounded to TF32 like the eval path's upsampling): bit for bit what
+ *   torch's CUDA F.interpolate(scale_factor=2, mode="bilinear", align_corners=True) returns for a channels_last input
+ *   (shown for C >= 16; the decoder's C is 32 to 128).
+ * pvnet_upsample2x_backward_nhwc: dout NHWC [b,2h,2w,dout_cs], read at channels [dout_co, dout_co+C) -> din NHWC
+ *   [b,h,w,C] dense, overwritten with dX = U^T dout.  Each element is the sum of exactly the terms torch's CUDA
+ *   backward adds to it with atomics -- (hl * wl) * g, two rounded fp32 products -- taken in a fixed order (output
+ *   pixels ascending, then torch's term order within one output pixel): no atomics, identical run to run, and a
+ *   result torch's own backward can return.
+ * Both: C, strides and offsets multiples of 4 floats; pointers 16-byte aligned; b*4*h*w*cs and b*h*w*C below 2^32
+ * elements.  Allocate nothing, launch one kernel on `stream`; bad arguments return PVNET_E_INVALID. */
+PVNET_API int pvnet_upsample2x_nhwc(const float *in, int C, float *out, int out_cs, int out_co, int b, int h, int w,
+                                    pvnet_stream_t stream);
+PVNET_API int pvnet_upsample2x_backward_nhwc(const float *dout, int dout_cs, int dout_co, int C, float *din, int b,
+                                             int h, int w, pvnet_stream_t stream);
+
 /* Test hook: which convolution kernel pvnet_conv2d_nhwc / the backbone use for layers both can
  * run.  0 = automatic (persistent weights-resident column kernel for 3x3 stride-1 layers with
  * Cout <= 64 whose weights fit in shared memory, per-tap kernel otherwise), 1 = per-tap kernel

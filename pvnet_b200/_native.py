@@ -98,6 +98,8 @@ SIGNATURES = {
                                         c_int, c_int, c_int, c_int, c_int, c_void_p, c_size_t, c_void_p]),
     "pvnet_zero_insert2x_nhwc": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                          c_void_p]),
+    "pvnet_upsample2x_nhwc": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "pvnet_upsample2x_backward_nhwc": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_int, c_void_p]),
     "pvnet_conv_set_mode": (c_int, [c_int]),
     "pvnet_conv_set_multicast": (c_int, [c_int]),
     "pvnet_conv_set_persistent": (c_int, [c_int]),

@@ -204,3 +204,67 @@ class Conv2dNHWC(torch.autograd.Function):
 def conv2d_train(x, weight, stride=1, dilation=1, dgrad_channels=None):
     """Conv2dNHWC.apply: the native convolution under autograd (see Conv2dNHWC)."""
     return Conv2dNHWC.apply(x, weight, stride, dilation, dgrad_channels)
+
+
+class Upsample2xCatNHWC(torch.autograd.Function):
+    """torch.cat([F.interpolate(low, scale_factor=2, mode="bilinear", align_corners=True), *rest], 1) as one
+    channels_last tensor, for [b,C,h,w] `low` and [b,Ci,2h,2w] `rest` (C and C + sum Ci multiples of 4).  Forward:
+    pvnet_upsample2x_nhwc writes the upsampled channels straight into the concatenated buffer (bit for bit torch's
+    CUDA forward), and the `rest` tensors are copied behind them.  Backward: `low` gets pvnet_upsample2x_backward_nhwc
+    of the gradient's first C channels, read in place (the terms of torch's backward in a fixed order, without
+    atomics, so identical run to run); each rest[i] gets its channel slice of the gradient, as cat's backward gives
+    it.  Runs on the input's device and its current stream."""
+
+    @staticmethod
+    def forward(ctx, low, *rest):
+        b, C, h, w = low.shape
+        if not low.is_cuda or low.dtype != torch.float32 or any(r.dtype != torch.float32 for r in rest):
+            raise ValueError("Upsample2xCatNHWC needs float32 CUDA tensors")
+        if any(r.shape[0] != b or r.shape[2:] != (2 * h, 2 * w) for r in rest):
+            raise ValueError(f"every concatenated tensor must be [{b}, C, {2 * h}, {2 * w}]")
+        widths = [C] + [r.shape[1] for r in rest]
+        if C % 4 or sum(widths) % 4:
+            raise ValueError(f"C and the concatenated width must be multiples of 4, got {widths}")
+        dev = low.device
+        out = torch.empty(b, sum(widths), 2 * h, 2 * w, dtype=torch.float32, device=dev,
+                          memory_format=torch.channels_last)
+        lh = _nhwc(low)
+        with torch.cuda.device(dev):
+            _native.check(_native.lib().pvnet_upsample2x_nhwc(
+                _p(lh), C, _p(out), out.shape[1], 0, b, h, w,
+                ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "pvnet_upsample2x_nhwc")
+        co = C
+        for r in rest:
+            out[:, co:co + r.shape[1]].copy_(r)
+            co += r.shape[1]
+        ctx.widths = widths
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gy):
+        widths = ctx.widths
+        b, _, H, W = gy.shape
+        C, h, w = widths[0], H // 2, W // 2
+        grads = [None] * len(widths)
+        if ctx.needs_input_grad[0]:
+            gyh = _nhwc(gy.float())
+            dev = gyh.device
+            dlow = torch.empty(b, C, h, w, dtype=torch.float32, device=dev, memory_format=torch.channels_last)
+            with torch.cuda.device(dev):
+                _native.check(_native.lib().pvnet_upsample2x_backward_nhwc(
+                    _p(gyh), gyh.shape[3], 0, C, _p(dlow), b, h, w,
+                    ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "pvnet_upsample2x_backward_nhwc")
+            grads[0] = dlow
+        co = C
+        for k, c in enumerate(widths[1:], 1):
+            if ctx.needs_input_grad[k]:
+                grads[k] = gy[:, co:co + c]
+            co += c
+        return tuple(grads)
+
+
+def upsample2x_cat(low, *rest):
+    """Upsample2xCatNHWC.apply: cat([F.interpolate(low, x2, bilinear, align_corners=True), *rest], 1) on the native
+    kernels under autograd (see Upsample2xCatNHWC)."""
+    return Upsample2xCatNHWC.apply(low, *rest)

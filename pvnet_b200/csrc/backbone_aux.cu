@@ -286,10 +286,77 @@ __device__ __forceinline__ float4 round_tf32_4(const float4 &v)
                        __uint_as_float((__float_as_uint(v.z) + 0x1000u) & 0xffffe000u),
                        __uint_as_float((__float_as_uint(v.w) + 0x1000u) & 0xffffe000u));
 }
+// ATen's index expressions for output index o of one axis (area_pixel_compute_source_index with align_corners, then
+// upsample_bilinear2d's clamp): output o reads input i0 with weight l0 and i1 = i0 + (i0 < in-1) with weight l1.
+// Written with _rn intrinsics so that no contraction can fuse `scale*o - i0` (torch's kernel rounds src first).
+struct UpSrc {
+    int i0, i1;
+    float l0, l1;
+};
+__device__ __forceinline__ UpSrc up_src(float scale, int o, int in)
+{
+    const float src = __fmul_rn(scale, (float)o);
+    const int i0 = (int)src;
+    const float l1 = __fsub_rn(src, (float)i0);
+    return {i0, i0 + (i0 < in - 1 ? 1 : 0), __fsub_rn(1.f, l1), l1};
+}
+
+// The training forward: torch's CUDA F.interpolate on a channels_last tensor (upsample_bilinear2d_nhwc_out_frame)
+// bit for bit.  Its SASS (sm_90, torch 2.11) contracts h0*(w0*v00 + w1*v01) + h1*(w0*v10 + w1*v11) as
+//   a = fma(w1, v01, w0*v00)     b = fma(w0, v10, w1*v11)     out = fma(h0, a, h1*b)
+// -- not lerp2's sequence for b and out -- so each output is computed from its own four loads, unrounded.
+__device__ __forceinline__ void upsample2x_exact_block(const float *__restrict__ in, float *__restrict__ out, int n,
+                                                       int j, int k, int h, int w, int C, int out_cs, int out_co,
+                                                       float sy, float sx)
+{
+    const int c4 = C >> 2;
+    const unsigned Wo = 2u * w;
+#pragma unroll
+    for (int oy = 0; oy < 2; ++oy) {
+        const UpSrc ry = up_src(sy, 2 * j + oy, h);
+        const unsigned r0 = ((unsigned)n * h + ry.i0) * (unsigned)w, r1 = ((unsigned)n * h + ry.i1) * (unsigned)w;
+#pragma unroll
+        for (int ox = 0; ox < 2; ++ox) {
+            const UpSrc rx = up_src(sx, 2 * k + ox, w);
+            const unsigned o00 = (r0 + rx.i0) * (unsigned)C, o01 = (r0 + rx.i1) * (unsigned)C;
+            const unsigned o10 = (r1 + rx.i0) * (unsigned)C, o11 = (r1 + rx.i1) * (unsigned)C;
+            const unsigned oo = (((unsigned)n * 2u * h + 2u * j + oy) * Wo + 2u * k + ox) * (unsigned)out_cs +
+                                (unsigned)out_co;
+            for (int cg = threadIdx.x; cg < c4; cg += 8) {
+                const float *ip = in + cg * 4;
+                const float4 v00 = __ldg(reinterpret_cast<const float4 *>(ip + o00));
+                const float4 v01 = __ldg(reinterpret_cast<const float4 *>(ip + o01));
+                const float4 v10 = __ldg(reinterpret_cast<const float4 *>(ip + o10));
+                const float4 v11 = __ldg(reinterpret_cast<const float4 *>(ip + o11));
+                float4 r;
+#define PV_UP_EXACT(f)                                                                                     \
+    r.f = __fmaf_rn(ry.l0, __fmaf_rn(rx.l1, v01.f, __fmul_rn(rx.l0, v00.f)),                               \
+                    __fmul_rn(ry.l1, __fmaf_rn(rx.l0, v10.f, __fmul_rn(rx.l1, v11.f))))
+                PV_UP_EXACT(x);
+                PV_UP_EXACT(y);
+                PV_UP_EXACT(z);
+                PV_UP_EXACT(w);
+#undef PV_UP_EXACT
+                *reinterpret_cast<float4 *>(out + oo + cg * 4) = r;
+            }
+        }
+    }
+}
+
+// TF32 = true: the eval path's kernel (values rounded to tf32 for the next tensor-core conv); false: the training
+// forward, exact fp32 in torch's rounding sequence (upsample2x_exact_block).
+template <bool TF32>
 __global__ void __launch_bounds__(256)
     k_upsample2x(const float *__restrict__ in, float *__restrict__ out, int h, int w, int C, int out_cs, int out_co,
                  float sy, float sx)
 {
+    if constexpr (!TF32) {
+        const int k = blockIdx.x * blockDim.y + threadIdx.y;
+        if (k >= w) return;
+        const int n = blockIdx.y / h, j = blockIdx.y - n * h;
+        upsample2x_exact_block(in, out, n, j, k, h, w, C, out_cs, out_co, sy, sx);
+        return;
+    }
     // One thread = the 2x2 output block (2j..2j+1, 2k..2k+1) of 4-channel groups cg, cg+8, ...  With
     // align_corners=True and scale 2 the source rows of output rows 2j, 2j+1 all lie in
     // {j-1, j, j+1} (same for columns), so the block needs a 3x3 neighbourhood: 9 loads for 4
@@ -400,10 +467,162 @@ int launch_upsample2x(const float *in, float *out, int b, int h, int w, int C, i
                  "upsample: tensor too large for 32-bit element offsets");
     const float sy = (float)(h - 1) / (float)(2 * h - 1), sx = (float)(w - 1) / (float)(2 * w - 1);
     dim3 grid((unsigned)((w + 31) / 32), (unsigned)(b * h));
-    k_upsample2x<<<grid, dim3(8, 32), 0, s>>>(in, out, h, w, C, out_cs, out_co, sy, sx);
+    k_upsample2x<true><<<grid, dim3(8, 32), 0, s>>>(in, out, h, w, C, out_cs, out_co, sy, sx);
     PV_LAUNCHED("k_upsample2x");
     return PVNET_OK;
 }
+
+// ------------------------------------------------------------------ bilinear x2 backward
+// dX = U^T dY for the training forward above, as a gather: input pixel (i, j) sums exactly the terms ATen's CUDA
+// backward (upsample_bilinear2d_backward_nhwc_out_frame) adds to it with atomics -- term = (hl * wl) * g, two
+// rounded products -- in a fixed order: output pixels ascending (row-major), and within one output pixel ATen's term
+// order (l0 l0, l0 l1, l1 l0, l1 l1).  No atomics: run-to-run identical, and a sum torch's own backward can return.
+// Window rule (oracle/upsample_oracle.py, tests/test_upsample_grad_cpu.py): input index i along an axis is fed by
+// the outputs o = 2i-2 ... 2i+3 whose up_src lands on i (slot 0 if i0 == i, slot 1 if i1 == i; both at the last
+// index, where i0p = 0).  Away from the borders that is always o = 2i-1, 2i through slot 1 and 2i+1, 2i+2 through
+// slot 0 (the interior pattern): a thread whose row and column are both interior takes 16 unconditional terms with
+// the products hl*wl computed once; every other thread walks the 6 x 6 candidates.
+// One thread = one input pixel, 4-channel groups cg, cg+8, ...  blockDim = (8 channel groups, 32 pixels of a row),
+// grid.y = image * h + i.  dY rows 2i-1 ... 2i+2 are shared with the neighbouring rows' blocks through L1/L2, so dY
+// comes from HBM about once.
+__device__ __forceinline__ bool up_interior(float scale, int i, int in)
+{
+    if (i < 1 || i > in - 2) return false;
+    bool ok = true;
+#pragma unroll
+    for (int r = 0; r < 6; ++r) {
+        const UpSrc u = up_src(scale, 2 * i - 2 + r, in);
+        const bool s0 = u.i0 == i, s1 = u.i1 == i;
+        ok = ok && (r == 1 || r == 2 ? (s1 && !s0) : r == 3 || r == 4 ? (s0 && !s1) : (!s0 && !s1));
+    }
+    return ok;
+}
+
+__global__ void __launch_bounds__(256)
+    k_upsample2x_backward(const float *__restrict__ dout, int dout_cs, int dout_co, float *__restrict__ din, int h,
+                          int w, int C, float sy, float sx)
+{
+    const int c4 = C >> 2;
+    const int j = blockIdx.x * blockDim.y + threadIdx.y;
+    if (j >= w) return;
+    const int n = blockIdx.y / h, i = blockIdx.y - n * h;
+    const unsigned Wo = 2u * w;
+    const unsigned img = (unsigned)n * 2u * h;
+    const unsigned dx_off = ((unsigned)blockIdx.y * (unsigned)w + (unsigned)j) * (unsigned)C;
+    const float *gp = dout + dout_co;
+
+    if (up_interior(sy, i, h) && up_interior(sx, j, w)) {
+        float wy[4], wx[4];
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+            const UpSrc uy = up_src(sy, 2 * i - 1 + r, h), ux = up_src(sx, 2 * j - 1 + r, w);
+            wy[r] = r < 2 ? uy.l1 : uy.l0;
+            wx[r] = r < 2 ? ux.l1 : ux.l0;
+        }
+        float p[4][4];
+#pragma unroll
+        for (int r = 0; r < 4; ++r)
+#pragma unroll
+            for (int c = 0; c < 4; ++c) p[r][c] = __fmul_rn(wy[r], wx[c]);
+        const unsigned g00 = ((img + 2u * i - 1u) * Wo + 2u * j - 1u) * (unsigned)dout_cs;
+        const unsigned grow = Wo * (unsigned)dout_cs;
+        for (int cg = threadIdx.x; cg < c4; cg += 8) {
+            float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+            for (int r = 0; r < 4; ++r)
+#pragma unroll
+                for (int c = 0; c < 4; ++c) {
+                    const float4 g = __ldg(reinterpret_cast<const float4 *>(
+                        gp + g00 + (unsigned)r * grow + (unsigned)c * (unsigned)dout_cs + cg * 4));
+                    acc.x = __fadd_rn(acc.x, __fmul_rn(p[r][c], g.x));
+                    acc.y = __fadd_rn(acc.y, __fmul_rn(p[r][c], g.y));
+                    acc.z = __fadd_rn(acc.z, __fmul_rn(p[r][c], g.z));
+                    acc.w = __fadd_rn(acc.w, __fmul_rn(p[r][c], g.w));
+                }
+            *reinterpret_cast<float4 *>(din + dx_off + cg * 4) = acc;
+        }
+        return;
+    }
+    // borders: every candidate (oy, ox), the terms that land on (i, j) in ATen's order
+    for (int cg = threadIdx.x; cg < c4; cg += 8) {
+        float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll 1
+        for (int r = 0; r < 6; ++r) {
+            const int oy = 2 * i - 2 + r;
+            if (oy < 0 || oy >= 2 * h) continue;
+            const UpSrc uy = up_src(sy, oy, h);
+            const bool y0 = uy.i0 == i, y1 = uy.i1 == i;
+            if (!y0 && !y1) continue;
+#pragma unroll 1
+            for (int c = 0; c < 6; ++c) {
+                const int ox = 2 * j - 2 + c;
+                if (ox < 0 || ox >= (int)Wo) continue;
+                const UpSrc ux = up_src(sx, ox, w);
+                const bool x0 = ux.i0 == j, x1 = ux.i1 == j;
+                if (!x0 && !x1) continue;
+                const float4 g = __ldg(reinterpret_cast<const float4 *>(
+                    gp + ((img + (unsigned)oy) * Wo + (unsigned)ox) * (unsigned)dout_cs + cg * 4));
+#pragma unroll
+                for (int t = 0; t < 4; ++t) {
+                    const bool hit = (t < 2 ? y0 : y1) && ((t & 1) ? x1 : x0);
+                    if (!hit) continue;
+                    const float q = __fmul_rn(t < 2 ? uy.l0 : uy.l1, (t & 1) ? ux.l1 : ux.l0);
+                    acc.x = __fadd_rn(acc.x, __fmul_rn(q, g.x));
+                    acc.y = __fadd_rn(acc.y, __fmul_rn(q, g.y));
+                    acc.z = __fadd_rn(acc.z, __fmul_rn(q, g.z));
+                    acc.w = __fadd_rn(acc.w, __fmul_rn(q, g.w));
+                }
+            }
+        }
+        *reinterpret_cast<float4 *>(din + dx_off + cg * 4) = acc;
+    }
+}
+
+static int check_upsample_args(const char *what, const float *dense, int C, const float *sliced, int cs, int co,
+                               int b, int h, int w)
+{
+    PV_CHECK_ARG(dense && sliced, "%s: null pointer", what);
+    PV_CHECK_ARG(b > 0 && h > 0 && w > 0, "%s: b, h, w must be positive", what);
+    PV_CHECK_ARG(C > 0 && C % 4 == 0 && cs % 4 == 0 && co % 4 == 0 && co >= 0,
+                 "%s: channels, stride and offset must be multiples of 4 floats", what);
+    PV_CHECK_ARG(co + C <= cs, "%s: channel slice exceeds its buffer", what);
+    PV_CHECK_ARG((uintptr_t)dense % 16 == 0 && (uintptr_t)sliced % 16 == 0, "%s: pointers must be 16-byte aligned",
+                 what);
+    PV_CHECK_ARG((long long)b * 4 * h * w * cs < (1LL << 32) && (long long)b * h * w * C < (1LL << 32),
+                 "%s: tensor too large for 32-bit element offsets", what);
+    return PVNET_OK;
+}
+
+}  // namespace pvnet
+
+extern "C" {
+
+int pvnet_upsample2x_nhwc(const float *in, int C, float *out, int out_cs, int out_co, int b, int h, int w,
+                          pvnet_stream_t stream)
+{
+    if (int rc = pvnet::check_upsample_args("upsample2x", in, C, out, out_cs, out_co, b, h, w)) return rc;
+    const float sy = (float)(h - 1) / (float)(2 * h - 1), sx = (float)(w - 1) / (float)(2 * w - 1);
+    dim3 grid((unsigned)((w + 31) / 32), (unsigned)(b * h));
+    pvnet::k_upsample2x<false><<<grid, dim3(8, 32), 0, (cudaStream_t)stream>>>(in, out, h, w, C, out_cs, out_co, sy, sx);
+    PV_LAUNCHED("k_upsample2x_exact");
+    return PVNET_OK;
+}
+
+int pvnet_upsample2x_backward_nhwc(const float *dout, int dout_cs, int dout_co, int C, float *din, int b, int h, int w,
+                                   pvnet_stream_t stream)
+{
+    if (int rc = pvnet::check_upsample_args("upsample2x backward", din, C, dout, dout_cs, dout_co, b, h, w)) return rc;
+    const float sy = (float)(h - 1) / (float)(2 * h - 1), sx = (float)(w - 1) / (float)(2 * w - 1);
+    dim3 grid((unsigned)((w + 31) / 32), (unsigned)(b * h));
+    pvnet::k_upsample2x_backward<<<grid, dim3(8, 32), 0, (cudaStream_t)stream>>>(dout, dout_cs, dout_co, din, h, w, C,
+                                                                                 sy, sx);
+    PV_LAUNCHED("k_upsample2x_backward");
+    return PVNET_OK;
+}
+
+}  // extern "C"
+
+namespace pvnet {
 
 // ------------------------------------------------------------------ head
 // convraw.3: 1x1 conv raw_dim(=32) -> seg_dim+ver_dim with bias (model_repository.py:57), in

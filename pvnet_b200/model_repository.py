@@ -336,11 +336,13 @@ class Resnet18_8s(nn.Module):
     def forward_train(self, x):
         """The train-mode forward (`_forward_torch`) with the 24 convolutions of slots 1..24 on the native tensor-core
         kernels under autograd (pvnet_b200.conv.Conv2dNHWC: pvnet_conv2d_nhwc forward, its data gradient and
-        pvnet_conv2d_nhwc_wgrad backward).  Activations are channels_last, so the BatchNorm, ReLU/LeakyReLU, max-pool,
-        cat and upsampling modules -- called as themselves, following their own `training` flag and updating their
-        running statistics as nn.BatchNorm2d does -- run on the NHWC storage without layout copies.  The stem and
-        the head convraw.3 stay torch convolutions.  convraw.0 reads cat[fm, image, 5 zero channels] like the eval
-        path; the image gets no gradient, so it must not require one (ValueError).
+        pvnet_conv2d_nhwc_wgrad backward).  The three upsample-and-concatenate steps of the decoder are
+        pvnet_b200.conv.upsample2x_cat (bit for bit torch's forward; a fixed-order backward without atomics), so the
+        step runs under torch.use_deterministic_algorithms(True).  Activations are channels_last, so the BatchNorm,
+        ReLU/LeakyReLU, max-pool and cat modules -- called as themselves, following their own `training` flag and
+        updating their running statistics as nn.BatchNorm2d does -- run on the NHWC storage without layout copies.
+        The stem and the head convraw.3 stay torch convolutions.  convraw.0 reads cat[fm, image, 5 zero channels] like
+        the eval path; the image gets no gradient, so it must not require one (ValueError).
 
         Returns (seg_pred, ver_pred), the channel slices of one contiguous NCHW tensor: the training losses then
         write a single gradient for it, and read it on their vectorised path (a channels_last head would leave
@@ -363,12 +365,12 @@ class Resnet18_8s(nn.Module):
         for blk in (*t.layer3, *t.layer4):
             x32s = self._block_train(blk, x32s)
         xfc = self._conv_bn_act(t.fc, x32s)
-        fm = self.up8sto4s(self._conv_bn_act(self.conv8s, torch.cat([xfc, x8s], 1)))
-        fm = self.up4sto2s(self._conv_bn_act(self.conv4s, torch.cat([fm, x4s], 1)))
-        fm = self.up2storaw(self._conv_bn_act(self.conv2s, torch.cat([fm, x2s], 1)))
+        fm = self._conv_bn_act(self.conv8s, torch.cat([xfc, x8s], 1))
+        fm = self._conv_bn_act(self.conv4s, pc.upsample2x_cat(fm, x4s))
+        fm = self._conv_bn_act(self.conv2s, pc.upsample2x_cat(fm, x2s))
         b, _, h, w = x.shape
         pad = torch.zeros(b, 5, h, w, dtype=torch.float32, device=x.device).contiguous(memory_format=cl)
-        y = self._conv_bn_act(self.convraw, torch.cat([fm, x, pad], 1), dgrad_channels=fm.shape[1])
+        y = self._conv_bn_act(self.convraw, pc.upsample2x_cat(fm, x, pad), dgrad_channels=fm.shape[1])
         out = self.convraw[3](y).contiguous()
         return out[:, :self.seg_dim], out[:, self.seg_dim:]
 
