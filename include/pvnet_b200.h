@@ -497,6 +497,49 @@ PVNET_API int pvnet_upsample2x_nhwc(const float *in, int C, float *out, int out_
 PVNET_API int pvnet_upsample2x_backward_nhwc(const float *dout, int dout_cs, int dout_co, int C, float *din, int b,
                                              int h, int w, pvnet_stream_t stream);
 
+/* Train-mode BatchNorm2d fused with its activation and the residual add of a BasicBlock (lib/networks/resnet.py
+ * BasicBlock.forward, model_repository.py's Conv2d -> BatchNorm2d -> ReLU / LeakyReLU(0.1) sequences), forward and
+ * backward, on dense NHWC fp32 tensors of npix = b*H*W pixels and C channels (C a multiple of 4, up to 1024;
+ * pointers 16-byte aligned; element offsets are 64-bit).
+ *
+ *   form 0  y = act(bn(x))               act 0 none, 1 ReLU, 2 LeakyReLU(0.1)
+ *   form 1  y = relu(bn(x) + z)          identity block tail: z is the skip
+ *   form 2  y = relu(bn(x) + bn_z(z))    downsample block tail: z is the downsample convolution's output
+ *
+ * bn(v) = fma(v, scale, shift) rounded to fp32, then the add, then the activation (the module graph's rounding).
+ * With batch_stats, mean and biased variance are fp64 over a fixed partition of the pixels (256-pixel partials
+ * merged in a fixed order: identical run to run, whatever the device); scale = fp32(gamma*invstd) and
+ * shift = fp32(beta - mean*scale), invstd = 1/sqrt(var + eps); running_mean/running_var (when non-NULL) become
+ * (1-f)*r + f*stat in fp32, with the unbiased variance var*N/(N-1).  Without batch_stats (a module in eval mode)
+ * the running statistics normalise and are left alone.
+ *
+ * The backward recomputes each element's pre-activation value from the same bits, g = dy*act'(pre) (ReLU: 0 where
+ * pre <= 0; LeakyReLU: dy*0.1f where pre <= 0), and writes dx = A*g + B*x + Cc with per-channel fp32 coefficients
+ * rounded once from fp64 sums of g and g*(x - mean) (B = Cc = 0 without batch_stats); dweight = invstd*sum g*(x-mean),
+ * dbias = sum g (NULL: not written).  Form 1 writes dz = g, form 2 dz = bn_z's data gradient (and dweight_z, dbias_z).
+ * The backward reads the `saved` and `coef` the forward wrote.  Allocate nothing; launch on `stream`. */
+typedef struct pvnet_batchnorm {
+    const float *weight;   /* [C] gamma, or NULL for 1 */
+    const float *bias;     /* [C] beta, or NULL for 0 */
+    float *running_mean;   /* [C] or NULL */
+    float *running_var;    /* [C] or NULL */
+    int batch_stats;       /* 1: normalise with the batch's statistics; 0: with running_mean/running_var */
+    double factor;         /* running-stat factor f: momentum, or 1/num_batches_tracked when momentum is None */
+    double eps;
+    double *saved;         /* [3][C] fp64, written by the forward: mean, biased variance, invstd */
+    float *coef;           /* [2][C] fp32, written by the forward: scale, shift */
+} pvnet_batchnorm_t;
+/* Workspace of one forward or backward call of `form` (fp64 partial sums and the backward's coefficients). */
+PVNET_API int pvnet_batchnorm_workspace_bytes(int form, int C, long long npix, size_t *bytes);
+PVNET_API int pvnet_batchnorm_act_forward(int form, int act, const float *x, const float *z, long long npix, int C,
+                                          const pvnet_batchnorm_t *bn, const pvnet_batchnorm_t *bn_z, float *y,
+                                          void *workspace, size_t workspace_bytes, pvnet_stream_t stream);
+PVNET_API int pvnet_batchnorm_act_backward(int form, int act, const float *dy, const float *x, const float *z,
+                                           long long npix, int C, const pvnet_batchnorm_t *bn,
+                                           const pvnet_batchnorm_t *bn_z, float *dx, float *dz, float *dweight,
+                                           float *dbias, float *dweight_z, float *dbias_z, void *workspace,
+                                           size_t workspace_bytes, pvnet_stream_t stream);
+
 /* Test hook: which convolution kernel pvnet_conv2d_nhwc / the backbone use for layers both can
  * run.  0 = automatic (persistent weights-resident column kernel for 3x3 stride-1 layers with
  * Cout <= 64 whose weights fit in shared memory, per-tap kernel otherwise), 1 = per-tap kernel

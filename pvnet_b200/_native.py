@@ -21,6 +21,16 @@ c_float = ctypes.c_float
 c_size_t = ctypes.c_size_t
 c_int64_p = ctypes.POINTER(ctypes.c_int64)
 
+
+class BatchNormParams(ctypes.Structure):
+    """pvnet_batchnorm_t: one BatchNorm2d's device pointers and mode (include/pvnet_b200.h)."""
+    _fields_ = [("weight", c_void_p), ("bias", c_void_p), ("running_mean", c_void_p), ("running_var", c_void_p),
+                ("batch_stats", c_int), ("factor", ctypes.c_double), ("eps", ctypes.c_double),
+                ("saved", c_void_p), ("coef", c_void_p)]
+
+
+c_bn_p = ctypes.POINTER(BatchNormParams)
+
 # name -> (restype, argtypes); must list every symbol include/pvnet_b200.h declares
 SIGNATURES = {
     "pvnet_last_error": (ctypes.c_char_p, []),
@@ -100,6 +110,12 @@ SIGNATURES = {
                                          c_void_p]),
     "pvnet_upsample2x_nhwc": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "pvnet_upsample2x_backward_nhwc": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "pvnet_batchnorm_workspace_bytes": (c_int, [c_int, c_int, ctypes.c_longlong, ctypes.POINTER(c_size_t)]),
+    "pvnet_batchnorm_act_forward": (c_int, [c_int, c_int, c_void_p, c_void_p, ctypes.c_longlong, c_int, c_bn_p, c_bn_p,
+                                            c_void_p, c_void_p, c_size_t, c_void_p]),
+    "pvnet_batchnorm_act_backward": (c_int, [c_int, c_int, c_void_p, c_void_p, c_void_p, ctypes.c_longlong, c_int,
+                                             c_bn_p, c_bn_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                             c_void_p, c_size_t, c_void_p]),
     "pvnet_conv_set_mode": (c_int, [c_int]),
     "pvnet_conv_set_multicast": (c_int, [c_int]),
     "pvnet_conv_set_persistent": (c_int, [c_int]),

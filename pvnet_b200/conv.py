@@ -268,3 +268,190 @@ def upsample2x_cat(low, *rest):
     """Upsample2xCatNHWC.apply: cat([F.interpolate(low, x2, bilinear, align_corners=True), *rest], 1) on the native
     kernels under autograd (see Upsample2xCatNHWC)."""
     return Upsample2xCatNHWC.apply(low, *rest)
+
+
+# ----------------------------------------------------------------------------- train-mode BatchNorm (autograd)
+FORM_ACT, FORM_ADD_RELU, FORM_ADD_BN_RELU = 0, 1, 2
+
+
+def act_of(module) -> int:
+    """The activation code of an nn.ReLU / nn.LeakyReLU(0.1) / nn.Identity module (anything else: ValueError)."""
+    if isinstance(module, torch.nn.ReLU):
+        return ACT_RELU
+    if isinstance(module, torch.nn.LeakyReLU) and module.negative_slope == 0.1:
+        return ACT_LEAKY
+    if isinstance(module, torch.nn.Identity):
+        return ACT_NONE
+    raise ValueError(f"no native activation for {module!r} (ReLU, LeakyReLU(0.1) or Identity)")
+
+
+class BatchNormState:
+    """One nn.BatchNorm2d call as the native kernels take it, decided the way nn.BatchNorm2d.forward decides: batch
+    statistics when the module is training (or has no running statistics), an update of running_mean/running_var
+    when it also tracks them, the factor `momentum` or 1/num_batches_tracked (momentum=None), and
+    num_batches_tracked.add_(1) exactly when the module would do it (at construction, i.e. once per forward call).
+    It also owns the fp64 statistics [3][C] (mean, biased variance, invstd) and fp32 scale/shift [2][C] that the
+    forward writes and the backward reads."""
+
+    def __init__(self, bn, device):
+        if not isinstance(bn, torch.nn.modules.batchnorm._BatchNorm):
+            raise ValueError(f"expected a BatchNorm module, got {type(bn).__name__}")
+        factor = 0.0 if bn.momentum is None else float(bn.momentum)
+        if bn.training and bn.track_running_stats and bn.num_batches_tracked is not None:
+            bn.num_batches_tracked.add_(1)
+            if bn.momentum is None:
+                factor = 1.0 / float(bn.num_batches_tracked)      # a host read, as in nn.BatchNorm2d
+        self.batch_stats = bn.training or (bn.running_mean is None and bn.running_var is None)
+        use_buffers = not bn.training or bn.track_running_stats
+        self.running_mean = bn.running_mean if use_buffers else None
+        self.running_var = bn.running_var if use_buffers else None
+        self.factor, self.eps = factor, float(bn.eps)
+        C = bn.num_features
+        for t in (bn.weight, bn.bias, self.running_mean, self.running_var):
+            if t is not None and (t.dtype != torch.float32 or t.device != torch.device(device) or not t.is_contiguous()
+                                  or t.numel() != C):
+                raise ValueError("BatchNorm parameters and buffers must be contiguous float32 [C] on the input's device")
+        self.saved = torch.empty(3, C, dtype=torch.float64, device=device)
+        self.coef = torch.empty(2, C, dtype=torch.float32, device=device)
+
+    def params(self, weight=None, bias=None):
+        return _native.BatchNormParams(
+            None if weight is None else weight.data_ptr(), None if bias is None else bias.data_ptr(),
+            None if self.running_mean is None else self.running_mean.data_ptr(),
+            None if self.running_var is None else self.running_var.data_ptr(),
+            int(self.batch_stats), self.factor, self.eps, self.saved.data_ptr(), self.coef.data_ptr())
+
+
+def _bn_check(t, C, shape=None):
+    if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.float32 or t.dim() != 4:
+        raise ValueError("the native BatchNorm needs float32 CUDA [b,C,H,W] tensors")
+    if t.shape[1] != C or (shape is not None and t.shape != shape):
+        raise ValueError(f"expected {C} channels{'' if shape is None else ' and shape ' + str(tuple(shape))}, "
+                         f"got {tuple(t.shape)}")
+
+
+def _bn_operand(t, C, shape=None):
+    _bn_check(t, C, shape)
+    return _nhwc(t)
+
+
+def _bn_workspace(form, C, npix, dev):
+    n = ctypes.c_size_t()
+    _native.check(_native.lib().pvnet_batchnorm_workspace_bytes(form, C, npix, ctypes.byref(n)),
+                  "pvnet_batchnorm_workspace_bytes")
+    return torch.empty(max(n.value, 16), dtype=torch.uint8, device=dev)
+
+
+def batchnorm_forward(form, act, xh, zh, st, weight, bias, st_z=None, weight_z=None, bias_z=None):
+    """pvnet_batchnorm_act_forward on NHWC views xh (and zh) -> y [b,C,H,W] channels_last; st / st_z are the
+    BatchNormStates (their running statistics are updated in place, their saved/coef written)."""
+    b, H, W, C = xh.shape
+    dev = xh.device
+    with torch.cuda.device(dev):
+        ws = _bn_workspace(form, C, b * H * W, dev)
+        y = torch.empty(b, C, H, W, dtype=torch.float32, device=dev, memory_format=torch.channels_last)
+        p = st.params(weight, bias)
+        pz = None if st_z is None else ctypes.byref(st_z.params(weight_z, bias_z))
+        _native.check(_native.lib().pvnet_batchnorm_act_forward(
+            form, act, _p(xh), _p(zh), b * H * W, C, ctypes.byref(p), pz, _p(y), _p(ws), ws.numel(),
+            ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "pvnet_batchnorm_act_forward")
+    return y
+
+
+def batchnorm_backward(form, act, gyh, xh, zh, st, weight, st_z=None, weight_z=None, param_grads=(True, True)):
+    """pvnet_batchnorm_act_backward -> (dx, dz, dweight, dbias, dweight_z, dbias_z): dx, dz [b,C,H,W] channels_last
+    (dz None for form 0), the parameter gradients [C] (None where the BatchNorm has no affine parameters or
+    param_grads says they are not wanted)."""
+    b, H, W, C = xh.shape
+    dev = xh.device
+    new = lambda: torch.empty(b, C, H, W, dtype=torch.float32, device=dev, memory_format=torch.channels_last)  # noqa
+    vec = lambda w, want: None if w is None or not want else torch.empty(C, dtype=torch.float32, device=dev)  # noqa
+    with torch.cuda.device(dev):
+        ws = _bn_workspace(form, C, b * H * W, dev)
+        dx = new()
+        dz = None if form == FORM_ACT else new()
+        dw, db = vec(weight, param_grads[0]), vec(weight, param_grads[1])
+        dwz = dbz = None
+        if form == FORM_ADD_BN_RELU:
+            dwz, dbz = vec(weight_z, param_grads[0]), vec(weight_z, param_grads[1])
+        p = st.params(weight)
+        pz = None if st_z is None else ctypes.byref(st_z.params(weight_z))
+        _native.check(_native.lib().pvnet_batchnorm_act_backward(
+            form, act, _p(gyh), _p(xh), _p(zh), b * H * W, C, ctypes.byref(p), pz, _p(dx), _p(dz), _p(dw), _p(db),
+            _p(dwz), _p(dbz), _p(ws), ws.numel(), ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
+            "pvnet_batchnorm_act_backward")
+    return dx, dz, dw, db, dwz, dbz
+
+
+class BatchNormActNHWC(torch.autograd.Function):
+    """act(BatchNorm2d(x)) for a [b,C,H,W] float32 CUDA tensor (C a multiple of 4; made channels_last if it is not),
+    with act none, ReLU or LeakyReLU(0.1): the `conv -> BatchNorm2d -> act` tail of Resnet18_8s's layers.  Forward:
+    pvnet_batchnorm_act_forward (fp64 batch statistics over a fixed partition, the running-stat update, then one
+    pass y = act(fma(x, scale, shift))).  Backward: pvnet_batchnorm_act_backward (the mask recomputed from x, fp64
+    per-channel sums in a fixed order, dx = a*g + b*x + c), identical run to run.  `weight` and `bias` are the module's
+    own parameters (they get gradients), `state` a BatchNormState built from the module for this call.  Saves x only
+    (plus the [C] statistics).  Runs on the input's device and its current stream."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, state, act):
+        xh = _bn_operand(x, state.coef.shape[1])
+        y = batchnorm_forward(FORM_ACT, act, xh, None, state, weight, bias)
+        ctx.save_for_backward(xh, weight)
+        ctx.state, ctx.act = state, act
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gy):
+        xh, weight = ctx.saved_tensors
+        dx, _, dw, db, _, _ = batchnorm_backward(FORM_ACT, ctx.act, _nhwc(gy.float()), xh, None, ctx.state, weight,
+                                                 param_grads=ctx.needs_input_grad[1:3])
+        return dx, dw, db, None, None
+
+
+class BatchNormAddReluNHWC(torch.autograd.Function):
+    """relu(bn(a) + skip) -- a BasicBlock's tail -- or, with a second BatchNorm, relu(bn(a) + bn_z(z)) -- the tail of
+    a block with a downsample, both BatchNorms applied in one pass.  Forward pvnet_batchnorm_act_forward, backward
+    pvnet_batchnorm_act_backward (form 1 or 2, see BatchNormActNHWC); the skip gets g = dy*relu'(pre) itself, z the
+    data gradient of bn_z.  Saves a and the skip / z, tensors the block's convolutions keep anyway."""
+
+    @staticmethod
+    def forward(ctx, a, weight, bias, state, z, weight_z, bias_z, state_z):
+        C = state.coef.shape[1]
+        ah = _bn_operand(a, C)
+        zh = _bn_operand(z, C, a.shape)
+        form = FORM_ADD_RELU if state_z is None else FORM_ADD_BN_RELU
+        y = batchnorm_forward(form, ACT_RELU, ah, zh, state, weight, bias, state_z, weight_z, bias_z)
+        ctx.save_for_backward(ah, zh, weight, weight_z)
+        ctx.state, ctx.state_z, ctx.form = state, state_z, form
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gy):
+        ah, zh, weight, weight_z = ctx.saved_tensors
+        n = ctx.needs_input_grad
+        dx, dz, dw, db, dwz, dbz = batchnorm_backward(
+            ctx.form, ACT_RELU, _nhwc(gy.float()), ah, zh, ctx.state, weight, ctx.state_z, weight_z,
+            param_grads=(n[1] or n[5], n[2] or n[6]))
+        return dx, dw if n[1] else None, db if n[2] else None, None, dz, dwz if n[5] else None, \
+            dbz if n[6] else None, None
+
+
+def bn_act(bn, x, act=ACT_NONE):
+    """act(bn(x)) on the native kernels under autograd, following the module's training flag, momentum, eps and
+    track_running_stats (see BatchNormActNHWC, BatchNormState)."""
+    _bn_check(x, bn.num_features)                 # before the state counts a batch
+    return BatchNormActNHWC.apply(x, bn.weight, bn.bias, BatchNormState(bn, x.device), act)
+
+
+def bn_add_relu(bn, a, skip, bn_skip=None):
+    """relu(bn(a) + skip), or relu(bn(a) + bn_skip(skip)) when bn_skip is given, on the native kernels under
+    autograd (see BatchNormAddReluNHWC)."""
+    _bn_check(a, bn.num_features)
+    _bn_check(skip, bn.num_features, a.shape)
+    state = BatchNormState(bn, a.device)
+    if bn_skip is None:
+        return BatchNormAddReluNHWC.apply(a, bn.weight, bn.bias, state, skip, None, None, None)
+    return BatchNormAddReluNHWC.apply(a, bn.weight, bn.bias, state, skip, bn_skip.weight, bn_skip.bias,
+                                      BatchNormState(bn_skip, a.device))

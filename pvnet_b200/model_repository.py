@@ -22,7 +22,8 @@ sm_90a backbone (wgmma implicit-GEMM convs behind include/pvnet_b200.h).
 * train mode (BatchNorm batch statistics, autograd; also what tools/demo.py runs because it
   never calls .eval(), SURVEY App. C.6) -> `forward` runs the plain PyTorch graph below, as SURVEY.md §7
   prescribes.  `forward_train` is the same graph with its 24 trunk/decoder convolutions (forward, data and
-  weight gradients) on the native kernels (DESIGN.md §14).
+  weight gradients, DESIGN.md §14) and its 25 BatchNorm layers with their activations and residual adds
+  (DESIGN.md §16) on the native kernels.
 """
 from __future__ import annotations
 
@@ -316,22 +317,23 @@ class Resnet18_8s(nn.Module):
     # ------------------------------------------------------------------ training path
     @staticmethod
     def _conv_bn_act(seq, x, dgrad_channels=None):
-        """nn.Sequential(Conv2d, BatchNorm2d, activation) with the convolution on the native kernels."""
+        """nn.Sequential(Conv2d, BatchNorm2d, activation) with the convolution and the BatchNorm + activation on the
+        native kernels."""
         conv = seq[0]
         y = pc.conv2d_train(x, conv.weight, conv.stride[0], conv.dilation[0], dgrad_channels)
-        return seq[2](seq[1](y))
+        return pc.bn_act(seq[1], y, pc.act_of(seq[2]))
 
     @staticmethod
     def _block_train(blk, x):
-        """resnet.BasicBlock.forward with its two (three) convolutions on the native kernels."""
-        y = blk.relu(blk.bn1(pc.conv2d_train(x, blk.conv1.weight, blk.conv1.stride[0], blk.conv1.dilation[0])))
-        y = blk.bn2(pc.conv2d_train(y, blk.conv2.weight, 1, blk.conv2.dilation[0]))
+        """resnet.BasicBlock.forward with its two (three) convolutions, its BatchNorms, ReLUs and residual add on the
+        native kernels: bn2, the downsample's BatchNorm, the add and the ReLU are one pass."""
+        relu = pc.act_of(blk.relu)
+        y = pc.bn_act(blk.bn1, pc.conv2d_train(x, blk.conv1.weight, blk.conv1.stride[0], blk.conv1.dilation[0]), relu)
+        y = pc.conv2d_train(y, blk.conv2.weight, 1, blk.conv2.dilation[0])
         if blk.downsample is None:
-            skip = x
-        else:
-            ds = blk.downsample
-            skip = ds[1](pc.conv2d_train(x, ds[0].weight, ds[0].stride[0], 1))
-        return blk.relu(y + skip)
+            return pc.bn_add_relu(blk.bn2, y, x)
+        ds = blk.downsample
+        return pc.bn_add_relu(blk.bn2, y, pc.conv2d_train(x, ds[0].weight, ds[0].stride[0], 1), ds[1])
 
     def forward_train(self, x):
         """The train-mode forward (`_forward_torch`) with the 24 convolutions of slots 1..24 on the native tensor-core
@@ -354,7 +356,7 @@ class Resnet18_8s(nn.Module):
         cl = torch.channels_last
         x = x.float().contiguous(memory_format=cl)
         t = self.resnet18_8s
-        x2s = t.relu(t.bn1(t.conv1(x)))
+        x2s = pc.bn_act(t.bn1, t.conv1(x), pc.act_of(t.relu))
         x4s = t.maxpool(x2s)
         for blk in t.layer1:
             x4s = self._block_train(blk, x4s)
