@@ -540,6 +540,48 @@ PVNET_API int pvnet_batchnorm_act_backward(int form, int act, const float *dy, c
                                            float *dbias, float *dweight_z, float *dbias_z, void *workspace,
                                            size_t workspace_bytes, pvnet_stream_t stream);
 
+/* The stem, max-pool and head of Resnet18_8s's training step (lib/networks/resnet.py:201-204,
+ * model_repository.py:57), forward and backward.  Each launches on `stream` and allocates nothing; bad arguments
+ * return PVNET_E_INVALID with a message.
+ *
+ * pvnet_stem_s2d_nhwc: conv1 (3 -> 64, 7x7, stride 2, pad 3) of image_nchw f32 [b,3,H,W] (H, W even; 8-byte
+ *   aligned) as the eval path computes it: s2d [b,H/2,W/2,16] is written with the 2x2 space-to-depth image
+ *   (channel (py*2+px)*3+c, 4 zero channels, rounded to TF32) and out NHWC [b,H/2,W/2,64] = the 4x4 stride-1 tensor-core
+ *   convolution of s2d with w_s2d (packed [64][4][4][16] as backbone slot 26, TF32) plus bias [64], fp32, no
+ *   activation.  s2d is what pvnet_stem_s2d_wgrad reads.
+ * pvnet_stem_s2d_wgrad: dw [64][3][7][7] (torch's layout, overwritten) = the weight gradient of that convolution for
+ *   dout NHWC [b,H/2,W/2,64] dense: the 4x4 weight gradient on s2d (TF32 operands, dout truncated by the tensor
+ *   cores, fp32 accumulation, pixel splits added in a fixed order: identical run to run), folded back onto the
+ *   147 weights of the 7x7 kernel.  The workspace size depends on the current device's SM count.
+ * pvnet_maxpool3x3s2_nhwc: nn.MaxPool2d(3, stride 2, padding 1) of in NHWC [b,H,W,C] dense (C a multiple of 4, H and
+ *   W even) -> out NHWC [b,H/2,W/2,C] and code uint8 [b,H/2,W/2,C], the argmax's window position dy*3+dx (dy, dx in
+ *   0..2 from the window origin (2oy-1, 2ox-1)).  torch's rule: the window scanned row-major from -inf, an element
+ *   wins when v > max or v is NaN; with no winner the first in-image element is the argmax.
+ * pvnet_maxpool3x3s2_backward_nhwc: din NHWC [b,H,W,C] (every element written) = each input's sum of the dout of
+ *   the windows whose code points at it, outputs ascending from 0.0f (ATen's order), no atomics.
+ * pvnet_head1x1_nchw: out NCHW [b,Cout,H,W] contiguous = bias[o] + sum_c w[o][c]*y[c], one fp32 fmaf chain per
+ *   output (c ascending from bias[o]), for y NHWC [b,H,W,Cin] dense (Cin a multiple of 32) and w [Cout][Cin].
+ * pvnet_head1x1_backward: for dout NCHW [b,Cout,H,W] contiguous: dy NHWC [b,H,W,Cin] = sum_o w[o][c]*dout[o] (an fmaf
+ *   chain, o ascending from 0); dw [Cout][Cin] = sum_p dout[p][o]*y[p][c] and db [Cout] = sum_p dout[p][o] in fp64
+ *   over a fixed partition of the pixels, merged in a fixed order and rounded once to fp32.  Any of dy, dw, db may
+ *   be NULL (not computed); the workspace is needed only for dw / db.
+ * All offsets are 64-bit; pointers 16-byte aligned unless stated. */
+PVNET_API int pvnet_stem_s2d_nhwc(const float *image_nchw, const float *w_s2d, const float *bias, float *s2d,
+                                  float *out, int b, int H, int W, pvnet_stream_t stream);
+PVNET_API int pvnet_stem_s2d_wgrad_workspace_bytes(int b, int H, int W, size_t *bytes);
+PVNET_API int pvnet_stem_s2d_wgrad(const float *s2d, const float *dout, float *dw, int b, int H, int W,
+                                   void *workspace, size_t workspace_bytes, pvnet_stream_t stream);
+PVNET_API int pvnet_maxpool3x3s2_nhwc(const float *in, float *out, uint8_t *code, int b, int H, int W, int C,
+                                      pvnet_stream_t stream);
+PVNET_API int pvnet_maxpool3x3s2_backward_nhwc(const float *dout, const uint8_t *code, float *din, int b, int H, int W,
+                                               int C, pvnet_stream_t stream);
+PVNET_API int pvnet_head1x1_nchw(const float *y, const float *w, const float *bias, float *out, int b, int H, int W,
+                                 int Cin, int Cout, pvnet_stream_t stream);
+PVNET_API int pvnet_head1x1_backward_workspace_bytes(int b, int H, int W, int Cin, int Cout, size_t *bytes);
+PVNET_API int pvnet_head1x1_backward(const float *dout, const float *y, const float *w, float *dy, float *dw,
+                                     float *db, int b, int H, int W, int Cin, int Cout, void *workspace,
+                                     size_t workspace_bytes, pvnet_stream_t stream);
+
 /* Test hook: which convolution kernel pvnet_conv2d_nhwc / the backbone use for layers both can
  * run.  0 = automatic (persistent weights-resident column kernel for 3x3 stride-1 layers with
  * Cout <= 64 whose weights fit in shared memory, per-tap kernel otherwise), 1 = per-tap kernel

@@ -116,6 +116,16 @@ SIGNATURES = {
     "pvnet_batchnorm_act_backward": (c_int, [c_int, c_int, c_void_p, c_void_p, c_void_p, ctypes.c_longlong, c_int,
                                              c_bn_p, c_bn_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                              c_void_p, c_size_t, c_void_p]),
+    "pvnet_stem_s2d_nhwc": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "pvnet_stem_s2d_wgrad_workspace_bytes": (c_int, [c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
+    "pvnet_stem_s2d_wgrad": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_size_t, c_void_p]),
+    "pvnet_maxpool3x3s2_nhwc": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "pvnet_maxpool3x3s2_backward_nhwc": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "pvnet_head1x1_nchw": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
+                                   c_void_p]),
+    "pvnet_head1x1_backward_workspace_bytes": (c_int, [c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
+    "pvnet_head1x1_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
+                                       c_int, c_int, c_int, c_void_p, c_size_t, c_void_p]),
     "pvnet_conv_set_mode": (c_int, [c_int]),
     "pvnet_conv_set_multicast": (c_int, [c_int]),
     "pvnet_conv_set_persistent": (c_int, [c_int]),

@@ -455,3 +455,213 @@ def bn_add_relu(bn, a, skip, bn_skip=None):
         return BatchNormAddReluNHWC.apply(a, bn.weight, bn.bias, state, skip, None, None, None)
     return BatchNormAddReluNHWC.apply(a, bn.weight, bn.bias, state, skip, bn_skip.weight, bn_skip.bias,
                                       BatchNormState(bn_skip, a.device))
+
+
+# ----------------------------------------------------------------------------- stem, max-pool and head (autograd)
+def _stream(dev):
+    return ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+
+
+def stem_s2d_index(device=None) -> torch.Tensor:
+    """[256] int64 on `device` (default CPU): for entry (ty, tx, ch) of pack_stem_s2d's [4][4][16] layout, the index
+    into conv1's weight flattened per output channel as [3][7][7] (c*49 + kh*7 + kw, kh = 2ty+py-1, kw = 2tx+px-1,
+    ch = (py*2+px)*3+c), or 147 where the entry is a zero (kh or kw outside 0..6, or ch >= 12).  147 entries are a
+    bijection onto the weights; it maps the packed weights one way and folds the s2d weight gradient back the other.
+    Built with device arithmetic, so no host-to-device copy (and no stream synchronisation) is involved: the training
+    stem can run inside a CUDA-graph capture."""
+    i = torch.arange(256, dtype=torch.int64, device=device)
+    ty, tx, ch = i // 64, (i // 16) % 4, i % 16
+    par, c = ch // 3, ch % 3
+    kh, kw = 2 * ty + par // 2 - 1, 2 * tx + par % 2 - 1
+    ok = (ch < 12) & (kh >= 0) & (kh <= 6) & (kw >= 0) & (kw <= 6)
+    return torch.where(ok, c * 49 + kh * 7 + kw, torch.full_like(i, 147))
+
+
+_STEM_INDEX = {}                 # (device type, index) -> stem_s2d_index on that device
+
+
+def _stem_index_on(device) -> torch.Tensor:
+    """stem_s2d_index(device), built once per device.  Inside a CUDA-graph capture an index not yet cached is built
+    for that call only (its memory would belong to the graph's pool)."""
+    key = (device.type, device.index)
+    idx = _STEM_INDEX.get(key)
+    if idx is None:
+        idx = stem_s2d_index(device)
+        if not (device.type == "cuda" and torch.cuda.is_current_stream_capturing()):
+            _STEM_INDEX[key] = idx
+    return idx
+
+
+def pack_stem_s2d_train(w: torch.Tensor) -> torch.Tensor:
+    """pack_stem_s2d as one gather on w's device (the values are identical): [64,3,7,7] -> [64][4][4][16],
+    TF32-rounded."""
+    cout = w.shape[0]
+    flat = torch.cat([w.reshape(cout, 147), w.new_zeros(cout, 1)], 1)
+    return round_tf32(torch.index_select(flat, 1, _stem_index_on(w.device)).reshape(cout, 4, 4, 16))
+
+
+def _check_float_cuda(what, *ts):
+    for t in ts:
+        if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.float32:
+            raise ValueError(f"{what} needs float32 CUDA tensors")
+
+
+class StemS2dNHWC(torch.autograd.Function):
+    """conv1 of Resnet18_8s (weight [64,3,7,7], stride 2, padding 3, no bias) of a [b,3,H,W] float32 CUDA image (H, W
+    even) that needs no gradient.  Forward: pvnet_stem_s2d_nhwc, the eval path's tensor-core form -- the 2x2
+    space-to-depth image S, TF32-rounded, and the 4x4 stride-1 convolution with the weights packed by
+    pack_stem_s2d_train -- into a channels_last [b,64,H/2,W/2].  Backward: the weight gradient only
+    (pvnet_stem_s2d_wgrad: the 4x4 gradient on S, all 16 taps per CTA, folded back to [64,3,7,7]).  Saves S only.
+    Runs on the input's device and its current stream."""
+
+    @staticmethod
+    def forward(ctx, x, weight):
+        _check_float_cuda("StemS2dNHWC", x, weight)
+        if x.requires_grad:
+            raise ValueError("StemS2dNHWC: the image gets no gradient, so it must not require one")
+        if x.dim() != 4 or x.shape[1] != 3 or x.shape[2] % 2 or x.shape[3] % 2 or tuple(weight.shape) != (64, 3, 7, 7):
+            raise ValueError(f"StemS2dNHWC needs x [b,3,H,W] with H, W even and weight [64,3,7,7], got "
+                             f"{tuple(x.shape)} and {tuple(weight.shape)}")
+        b, _, H, W = x.shape
+        dev = x.device
+        xc = x.contiguous()
+        s2d = torch.empty(b, H // 2, W // 2, 16, dtype=torch.float32, device=dev)
+        out = torch.empty(b, 64, H // 2, W // 2, dtype=torch.float32, device=dev, memory_format=torch.channels_last)
+        w4 = pack_stem_s2d_train(weight.detach())
+        bias = torch.zeros(64, dtype=torch.float32, device=dev)
+        with torch.cuda.device(dev):
+            _native.check(_native.lib().pvnet_stem_s2d_nhwc(_p(xc), _p(w4), _p(bias), _p(s2d), _p(out), b, H, W,
+                                                            _stream(dev)), "pvnet_stem_s2d_nhwc")
+        ctx.save_for_backward(s2d)
+        ctx.hw = (H, W)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gy):
+        s2d, = ctx.saved_tensors
+        if not ctx.needs_input_grad[1]:
+            return None, None
+        b = s2d.shape[0]
+        H, W = ctx.hw
+        dev = s2d.device
+        gyh = _nhwc(gy.float())
+        L = _native.lib()
+        with torch.cuda.device(dev):
+            n = ctypes.c_size_t()
+            _native.check(L.pvnet_stem_s2d_wgrad_workspace_bytes(b, H, W, ctypes.byref(n)),
+                          "pvnet_stem_s2d_wgrad_workspace_bytes")
+            ws = torch.empty(max(n.value, 16), dtype=torch.uint8, device=dev)
+            dw = torch.empty(64, 3, 7, 7, dtype=torch.float32, device=dev)
+            _native.check(L.pvnet_stem_s2d_wgrad(_p(s2d), _p(gyh), _p(dw), b, H, W, _p(ws), ws.numel(), _stream(dev)),
+                          "pvnet_stem_s2d_wgrad")
+        return None, dw
+
+
+def stem_train(x, weight):
+    """StemS2dNHWC.apply: conv1 (7x7/2, pad 3, no bias) on the native kernels under autograd."""
+    return StemS2dNHWC.apply(x, weight)
+
+
+class MaxPool3x3s2NHWC(torch.autograd.Function):
+    """nn.MaxPool2d(3, stride=2, padding=1) of a [b,C,H,W] float32 CUDA tensor (C a multiple of 4, H and W even; made
+    channels_last if it is not) -> channels_last [b,C,H/2,W/2].  Forward: pvnet_maxpool3x3s2_nhwc, torch's argmax rule
+    (NaN wins, ties to the first in row-major order), with a uint8 window code per output instead of int64 indices.
+    Backward: pvnet_maxpool3x3s2_backward_nhwc, a gather in ATen's order without atomics.  Saves the codes only."""
+
+    @staticmethod
+    def forward(ctx, x):
+        _check_float_cuda("MaxPool3x3s2NHWC", x)
+        if x.dim() != 4 or x.shape[1] % 4 or x.shape[2] % 2 or x.shape[3] % 2:
+            raise ValueError(f"MaxPool3x3s2NHWC needs [b,C,H,W] with C a multiple of 4 and H, W even, got "
+                             f"{tuple(x.shape)}")
+        b, C, H, W = x.shape
+        dev = x.device
+        xh = _nhwc(x)
+        out = torch.empty(b, C, H // 2, W // 2, dtype=torch.float32, device=dev, memory_format=torch.channels_last)
+        code = torch.empty(b, H // 2, W // 2, C, dtype=torch.uint8, device=dev)
+        with torch.cuda.device(dev):
+            _native.check(_native.lib().pvnet_maxpool3x3s2_nhwc(_p(xh), _p(out), _p(code), b, H, W, C, _stream(dev)),
+                          "pvnet_maxpool3x3s2_nhwc")
+        ctx.save_for_backward(code)
+        ctx.hw = (H, W)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gy):
+        code, = ctx.saved_tensors
+        b, _, _, C = code.shape
+        H, W = ctx.hw
+        dev = code.device
+        gyh = _nhwc(gy.float())
+        dx = torch.empty(b, C, H, W, dtype=torch.float32, device=dev, memory_format=torch.channels_last)
+        with torch.cuda.device(dev):
+            _native.check(_native.lib().pvnet_maxpool3x3s2_backward_nhwc(_p(gyh), _p(code), _p(dx), b, H, W, C,
+                                                                         _stream(dev)),
+                          "pvnet_maxpool3x3s2_backward_nhwc")
+        return dx
+
+
+def maxpool_train(x):
+    """MaxPool3x3s2NHWC.apply: nn.MaxPool2d(3, 2, 1) on the native kernels under autograd."""
+    return MaxPool3x3s2NHWC.apply(x)
+
+
+class Head1x1NCHW(torch.autograd.Function):
+    """The 1x1 convolution with bias convraw.3 of a [b,Cin,H,W] float32 CUDA tensor (Cin a multiple of 32; made
+    channels_last if it is not) -> a contiguous NCHW [b,Cout,H,W].  Forward: pvnet_head1x1_nchw, exact fp32 (one fmaf
+    chain per output from the bias).  Backward: pvnet_head1x1_backward, the input gradient as fmaf chains and the
+    weight and bias gradients as fp64 sums in a fixed order, rounded once (identical run to run); the parameter
+    gradients are skipped when the parameters need none.  Saves the input and the weight."""
+
+    @staticmethod
+    def forward(ctx, y, weight, bias):
+        _check_float_cuda("Head1x1NCHW", y, weight, bias)
+        cout, cin = weight.shape[:2]
+        if y.dim() != 4 or y.shape[1] != cin or tuple(weight.shape[2:]) != (1, 1) or tuple(bias.shape) != (cout,):
+            raise ValueError(f"Head1x1NCHW needs y [b,{cin},H,W], weight [Cout,Cin,1,1] and bias [Cout], got "
+                             f"{tuple(y.shape)}, {tuple(weight.shape)}, {tuple(bias.shape)}")
+        b, _, H, W = y.shape
+        dev = y.device
+        yh = _nhwc(y)
+        w2 = weight.detach().reshape(cout, cin).contiguous()
+        out = torch.empty(b, cout, H, W, dtype=torch.float32, device=dev)
+        with torch.cuda.device(dev):
+            _native.check(_native.lib().pvnet_head1x1_nchw(_p(yh), _p(w2), _p(bias.detach().contiguous()), _p(out), b,
+                                                           H, W, cin, cout, _stream(dev)), "pvnet_head1x1_nchw")
+        ctx.save_for_backward(yh, weight)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gout):
+        yh, weight = ctx.saved_tensors
+        b, H, W, cin = yh.shape
+        cout = weight.shape[0]
+        dev = yh.device
+        need_y, need_w, need_b = ctx.needs_input_grad
+        g = gout.float().contiguous()
+        w2 = weight.detach().reshape(cout, cin).contiguous()
+        dy = torch.empty(b, cin, H, W, dtype=torch.float32, device=dev,
+                         memory_format=torch.channels_last) if need_y else None
+        dw = torch.empty(cout, cin, dtype=torch.float32, device=dev) if need_w else None
+        db = torch.empty(cout, dtype=torch.float32, device=dev) if need_b else None
+        L = _native.lib()
+        with torch.cuda.device(dev):
+            ws = None
+            if need_w or need_b:
+                n = ctypes.c_size_t()
+                _native.check(L.pvnet_head1x1_backward_workspace_bytes(b, H, W, cin, cout, ctypes.byref(n)),
+                              "pvnet_head1x1_backward_workspace_bytes")
+                ws = torch.empty(max(n.value, 16), dtype=torch.uint8, device=dev)
+            _native.check(L.pvnet_head1x1_backward(_p(g), _p(yh), _p(w2), _p(dy), _p(dw), _p(db), b, H, W, cin, cout,
+                                                   _p(ws), 0 if ws is None else ws.numel(), _stream(dev)),
+                          "pvnet_head1x1_backward")
+        return dy, None if dw is None else dw.view(cout, cin, 1, 1), db
+
+
+def head_train(y, weight, bias):
+    """Head1x1NCHW.apply: convraw.3 (1x1 with bias) on the native kernels under autograd, as a contiguous NCHW
+    tensor."""
+    return Head1x1NCHW.apply(y, weight, bias)

@@ -5,6 +5,7 @@
 // All of them are HBM-bound streaming kernels except the stem (FP32 FMA bound).
 #include "conv_tc.cuh"
 #include "ptx.cuh"
+#include <algorithm>
 
 namespace pvnet {
 
@@ -122,10 +123,11 @@ int launch_pack_image(const float *in, float *out, int b, int H, int W, int out_
 // lib/datasets/linemod_dataset.py:191-195): (float(v) / 255 - mean[c]) / std[c], three correctly
 // rounded ops -- bit-identical to feeding the float path with the torch-normalised tensor, at a
 // quarter of the input bytes.
+// IMG = false (the training stem, pvnet_stem_s2d_nhwc): only S is written; `out` is not touched.
 struct Norm3 {
     float mean[3], std[3];
 };
-template <bool U8>
+template <bool U8, bool IMG = true>
 __global__ void __launch_bounds__(128)
     k_s2d_pack(const void *__restrict__ in_v, Norm3 nrm, float *__restrict__ s2d, float *__restrict__ out, int H, int W,
                int out_cs, int out_co)
@@ -180,13 +182,15 @@ __global__ void __launch_bounds__(128)
 #pragma unroll
         for (int j = 0; j < 4; ++j)
             sS[t * 4 + (j ^ ((t >> 1) & 3))] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
+        if constexpr (IMG) {
 #pragma unroll
-        for (int py = 0; py < 2; ++py)
+            for (int py = 0; py < 2; ++py)
 #pragma unroll
-            for (int px = 0; px < 2; ++px) {
-                const int b = (py * 2 + px) * 3;
-                sI[py][2 * t + px] = make_float4(v[b], v[b + 1], v[b + 2], 0.f);
-            }
+                for (int px = 0; px < 2; ++px) {
+                    const int b = (py * 2 + px) * 3;
+                    sI[py][2 * t + px] = make_float4(v[b], v[b + 1], v[b + 2], 0.f);
+                }
+        }
     }
     __syncthreads();
     const int npx = min(128, W2 - xb);                    // half-resolution pixels this block holds
@@ -196,6 +200,7 @@ __global__ void __launch_bounds__(128)
         const int L = t + 128 * r, px = L >> 2, j = L & 3;
         if (px < npx) so[L] = sS[px * 4 + (j ^ ((px >> 1) & 3))];
     }
+    if constexpr (!IMG) return;
     // image slice: lane pairs write the 32 bytes (3 channels + 5 zeros) of one full-resolution pixel
 #pragma unroll
     for (int py = 0; py < 2; ++py) {
@@ -264,6 +269,90 @@ int launch_maxpool(const float *in, float *out, int b, int H, int W, int C, int 
     k_maxpool<<<grid, 256, 0, s>>>(in, out, H, W, C, in_cs, in_co);
     PV_LAUNCHED("k_maxpool");
     return PVNET_OK;
+}
+
+// ------------------------------------------------------------------ max-pool 3x3/2 pad 1, training
+// Forward with argmax: torch's rule -- the window scanned row-major from -inf, an element wins when `v > max ||
+// isnan(v)`, and with no winner (all -inf) the first in-image element is the argmax.  The argmax is stored as a
+// uint8 window code (dy*3 + dx, dy/dx = 0..2 from the window origin (2oy-1, 2ox-1)).  One thread = one output pixel's
+// 4-channel group.  in NHWC [b,H,W,C] dense -> out NHWC [b,H/2,W/2,C], code [b,H/2,W/2,C]; 64-bit offsets.
+__global__ void __launch_bounds__(256)
+    k_maxpool_train(const float *__restrict__ in, float *__restrict__ out, uchar4 *__restrict__ code, int H, int W,
+                    int C, long long total)
+{
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= total) return;
+    const int c4 = C >> 2, Ho = H >> 1, Wo = W >> 1;
+    const long long pix = i / c4;
+    const int cg = (int)(i - pix * c4);
+    const int ox = (int)(pix % Wo);
+    const long long t = pix / Wo;
+    const int oy = (int)(t % Ho);
+    const long long n = t / Ho;
+    float m[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
+    int k[4] = {-1, -1, -1, -1};
+    int first = -1;
+#pragma unroll
+    for (int dy = 0; dy < 3; ++dy) {
+        const int iy = 2 * oy - 1 + dy;
+        if (iy < 0 || iy >= H) continue;
+#pragma unroll
+        for (int dx = 0; dx < 3; ++dx) {
+            const int ix = 2 * ox - 1 + dx;
+            if (ix < 0 || ix >= W) continue;
+            const float4 q = __ldg(reinterpret_cast<const float4 *>(in + ((n * H + iy) * W + ix) * C) + cg);
+            const float v[4] = {q.x, q.y, q.z, q.w};
+            const int cd = dy * 3 + dx;
+            if (first < 0) first = cd;
+#pragma unroll
+            for (int e = 0; e < 4; ++e)
+                if (v[e] > m[e] || isnan(v[e])) {
+                    m[e] = v[e];
+                    k[e] = cd;
+                }
+        }
+    }
+#pragma unroll
+    for (int e = 0; e < 4; ++e)
+        if (k[e] < 0) k[e] = first;
+    reinterpret_cast<float4 *>(out)[i] = make_float4(m[0], m[1], m[2], m[3]);
+    code[i] = make_uchar4((unsigned char)k[0], (unsigned char)k[1], (unsigned char)k[2], (unsigned char)k[3]);
+}
+
+// Backward as a gather: input pixel (iy, ix) adds the dY of the windows whose code points at it, in ATen's order --
+// outputs (oy, ox) ascending over ATen's window bounds, from 0.0f, one rounded fp32 add each.  No atomics.
+// dout NHWC [b,H/2,W/2,C] dense, code as the forward wrote it -> din NHWC [b,H,W,C] dense, every element written.
+__global__ void __launch_bounds__(256)
+    k_maxpool_train_backward(const float *__restrict__ dout, const uchar4 *__restrict__ code, float *__restrict__ din,
+                             int H, int W, int C, long long total)
+{
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= total) return;
+    const int c4 = C >> 2, Ho = H >> 1, Wo = W >> 1;
+    const long long pix = i / c4;
+    const int cg = (int)(i - pix * c4);
+    const int ix = (int)(pix % W);
+    const long long t = pix / W;
+    const int iy = (int)(t % H);
+    const long long n = t / H;
+    // ATen's p_start / p_end for kernel 3, stride 2, pad 1, dilation 1
+    const int oy0 = iy + 1 < 3 ? 0 : (iy + 1 - 3) / 2 + 1, oy1 = min((iy + 1) / 2 + 1, Ho);
+    const int ox0 = ix + 1 < 3 ? 0 : (ix + 1 - 3) / 2 + 1, ox1 = min((ix + 1) / 2 + 1, Wo);
+    float acc[4] = {0.f, 0.f, 0.f, 0.f};
+    for (int oy = oy0; oy < oy1; ++oy)
+        for (int ox = ox0; ox < ox1; ++ox) {
+            const int want = (iy - (2 * oy - 1)) * 3 + (ix - (2 * ox - 1));
+            const long long o = ((n * Ho + oy) * Wo + ox) * c4 + cg;
+            const uchar4 kq = __ldg(code + o);
+            const unsigned char kk[4] = {kq.x, kq.y, kq.z, kq.w};
+            if (kk[0] != want && kk[1] != want && kk[2] != want && kk[3] != want) continue;
+            const float4 gq = __ldg(reinterpret_cast<const float4 *>(dout) + o);
+            const float g[4] = {gq.x, gq.y, gq.z, gq.w};
+#pragma unroll
+            for (int e = 0; e < 4; ++e)
+                if (kk[e] == want) acc[e] = __fadd_rn(acc[e], g[e]);
+        }
+    reinterpret_cast<float4 *>(din)[i] = make_float4(acc[0], acc[1], acc[2], acc[3]);
 }
 
 // ------------------------------------------------------------------ bilinear x2, align_corners=True
@@ -618,6 +707,64 @@ int pvnet_upsample2x_backward_nhwc(const float *dout, int dout_cs, int dout_co, 
                                                                                  sy, sx);
     PV_LAUNCHED("k_upsample2x_backward");
     return PVNET_OK;
+}
+
+static int check_maxpool_args(const char *what, const void *a, const void *b, const void *c, int bn, int H, int W,
+                              int C)
+{
+    PV_CHECK_ARG(a && b && c, "%s: null pointer", what);
+    PV_CHECK_ARG(bn > 0 && H > 0 && W > 0 && H % 2 == 0 && W % 2 == 0, "%s: b, H, W must be positive, H and W even",
+                 what);
+    PV_CHECK_ARG(C > 0 && C % 4 == 0, "%s: C must be a positive multiple of 4", what);
+    PV_CHECK_ARG((uintptr_t)a % 16 == 0 && (uintptr_t)b % 16 == 0 && (uintptr_t)c % 16 == 0,
+                 "%s: pointers must be 16-byte aligned", what);
+    return PVNET_OK;
+}
+
+int pvnet_maxpool3x3s2_nhwc(const float *in, float *out, uint8_t *code, int b, int H, int W, int C,
+                            pvnet_stream_t stream)
+{
+    if (int rc = check_maxpool_args("maxpool", in, out, code, b, H, W, C)) return rc;
+    const long long total = (long long)b * (H / 2) * (W / 2) * (C / 4);
+    pvnet::k_maxpool_train<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+        in, out, reinterpret_cast<uchar4 *>(code), H, W, C, total);
+    PV_LAUNCHED("k_maxpool_train");
+    return PVNET_OK;
+}
+
+int pvnet_maxpool3x3s2_backward_nhwc(const float *dout, const uint8_t *code, float *din, int b, int H, int W, int C,
+                                     pvnet_stream_t stream)
+{
+    if (int rc = check_maxpool_args("maxpool backward", dout, code, din, b, H, W, C)) return rc;
+    const long long total = (long long)b * H * W * (C / 4);
+    pvnet::k_maxpool_train_backward<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+        dout, reinterpret_cast<const uchar4 *>(code), din, H, W, C, total);
+    PV_LAUNCHED("k_maxpool_train_backward");
+    return PVNET_OK;
+}
+
+int pvnet_stem_s2d_nhwc(const float *image_nchw, const float *w_s2d, const float *bias, float *s2d, float *out, int b,
+                        int H, int W, pvnet_stream_t stream)
+{
+    PV_CHECK_ARG(image_nchw && w_s2d && bias && s2d && out, "stem: null pointer");
+    PV_CHECK_ARG(b > 0 && H > 0 && W > 0 && H % 2 == 0 && W % 2 == 0, "stem: b, H, W must be positive, H and W even");
+    PV_CHECK_ARG((uintptr_t)image_nchw % 8 == 0 && (uintptr_t)s2d % 16 == 0 && (uintptr_t)out % 16 == 0 &&
+                     (uintptr_t)w_s2d % 16 == 0,
+                 "stem: image must be 8-byte, s2d / out / weights 16-byte aligned");
+    // k_s2d_pack's grid.y is image * H/2 + row, at most 65535: launch it over chunks of whole images
+    PV_CHECK_ARG(H / 2 <= 65535, "stem: H/2 = %d rows exceed the 65535-row launch limit", H / 2);
+    const int per = 65535 / (H / 2);
+    for (int n0 = 0; n0 < b; n0 += per) {
+        const int nb = std::min(per, b - n0);
+        const dim3 grid((unsigned)((W / 2 + 127) / 128), (unsigned)(nb * (H / 2)));
+        pvnet::k_s2d_pack<false, false><<<grid, 128, 0, (cudaStream_t)stream>>>(
+            image_nchw + (size_t)n0 * 3 * H * W, pvnet::Norm3{}, s2d + (size_t)n0 * (H / 2) * (W / 2) * 16, nullptr, H,
+            W, 0, 0);
+        PV_LAUNCHED("k_s2d_pack");
+    }
+    // the 7x7/2 convolution as the 4x4 stride-1 convolution on S (taps at offsets -2..1): the eval path's instantiation
+    return pvnet_conv2d_nhwc(s2d, 16, 0, 16, w_s2d, bias, nullptr, 0, 0, out, 64, 0, 64, b, H / 2, W / 2, 4, 1, 1, 0,
+                             0, stream);
 }
 
 }  // extern "C"

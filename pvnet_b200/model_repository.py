@@ -21,9 +21,9 @@ sm_90a backbone (wgmma implicit-GEMM convs behind include/pvnet_b200.h).
   packed once per device, never per forward, and a handle is destroyed exactly once.
 * train mode (BatchNorm batch statistics, autograd; also what tools/demo.py runs because it
   never calls .eval(), SURVEY App. C.6) -> `forward` runs the plain PyTorch graph below, as SURVEY.md §7
-  prescribes.  `forward_train` is the same graph with its 24 trunk/decoder convolutions (forward, data and
-  weight gradients, DESIGN.md §14) and its 25 BatchNorm layers with their activations and residual adds
-  (DESIGN.md §16) on the native kernels.
+  prescribes.  `forward_train` is the same graph with every layer on the native kernels: its 24 trunk/decoder
+  convolutions (forward, data and weight gradients, DESIGN.md §14), the upsampling (§15), its 25 BatchNorm layers
+  with their activations and residual adds (§16), and the stem, max-pool and head (§17).
 """
 from __future__ import annotations
 
@@ -335,29 +335,55 @@ class Resnet18_8s(nn.Module):
         ds = blk.downsample
         return pc.bn_add_relu(blk.bn2, y, pc.conv2d_train(x, ds[0].weight, ds[0].stride[0], 1), ds[1])
 
-    def forward_train(self, x):
-        """The train-mode forward (`_forward_torch`) with the 24 convolutions of slots 1..24 on the native tensor-core
-        kernels under autograd (pvnet_b200.conv.Conv2dNHWC: pvnet_conv2d_nhwc forward, its data gradient and
-        pvnet_conv2d_nhwc_wgrad backward).  The three upsample-and-concatenate steps of the decoder are
-        pvnet_b200.conv.upsample2x_cat (bit for bit torch's forward; a fixed-order backward without atomics), so the
-        step runs under torch.use_deterministic_algorithms(True).  Activations are channels_last, so the BatchNorm,
-        ReLU/LeakyReLU, max-pool and cat modules -- called as themselves, following their own `training` flag and
-        updating their running statistics as nn.BatchNorm2d does -- run on the NHWC storage without layout copies.
-        The stem and the head convraw.3 stay torch convolutions.  convraw.0 reads cat[fm, image, 5 zero channels] like
-        the eval path; the image gets no gradient, so it must not require one (ValueError).
+    def _check_train_modules(self):
+        """ValueError unless conv1, the max-pool and convraw.3 still have the shapes forward_train's kernels
+        implement."""
+        t = self.resnet18_8s
+        c1, mp, hd = t.conv1, t.maxpool, self.convraw[3]
+        pair = lambda v: tuple(v) if isinstance(v, (tuple, list)) else (v, v)  # noqa: E731
+        if not (isinstance(c1, nn.Conv2d) and tuple(c1.weight.shape) == (64, 3, 7, 7) and c1.stride == (2, 2)
+                and c1.padding == (3, 3) and c1.dilation == (1, 1) and c1.groups == 1 and c1.bias is None
+                and c1.padding_mode == "zeros"):
+            raise ValueError("forward_train: conv1 must be a [64,3,7,7] convolution, stride 2, padding 3, no bias")
+        if not (isinstance(mp, nn.MaxPool2d) and pair(mp.kernel_size) == (3, 3) and pair(mp.stride) == (2, 2)
+                and pair(mp.padding) == (1, 1) and pair(mp.dilation) == (1, 1) and not mp.ceil_mode
+                and not mp.return_indices):
+            raise ValueError("forward_train: the max-pool must be 3x3, stride 2, padding 1, dilation 1, no ceil_mode")
+        if not (isinstance(hd, nn.Conv2d) and hd.kernel_size == (1, 1) and hd.stride == (1, 1) and hd.padding == (0, 0)
+                and hd.dilation == (1, 1) and hd.groups == 1 and hd.bias is not None):
+            raise ValueError("forward_train: convraw[3] must be a 1x1 convolution with bias")
 
-        Returns (seg_pred, ver_pred), the channel slices of one contiguous NCHW tensor: the training losses then
-        write a single gradient for it, and read it on their vectorised path (a channels_last head would leave
-        them strided).  NetWrapper's change: `seg_pred, vertex_pred = self.net.forward_train(image)`."""
+    def forward_train(self, x):
+        """The train-mode forward (`_forward_torch`) with every layer on the native kernels under autograd:
+        * the stem conv1 as pvnet_b200.conv.stem_train (the eval path's space-to-depth tensor-core forward, a wgmma
+          weight gradient; the image gets no gradient, so it must not require one: ValueError);
+        * the 24 convolutions of slots 1..24 as pvnet_b200.conv.Conv2dNHWC (pvnet_conv2d_nhwc forward, its data
+          gradient and pvnet_conv2d_nhwc_wgrad backward);
+        * the 25 BatchNorm layers with their ReLU/LeakyReLU and residual adds as pvnet_b200.conv.bn_act / bn_add_relu,
+          following each module's own `training` flag, momentum and running statistics;
+        * the max-pool as pvnet_b200.conv.maxpool_train (torch's argmax rule, a gather backward);
+        * the three upsample-and-concatenate steps of the decoder as pvnet_b200.conv.upsample2x_cat (bit for bit
+          torch's forward; a fixed-order backward without atomics);
+        * the head convraw.3 as pvnet_b200.conv.head_train (exact fp32 forward, fixed-order fp64 parameter gradients).
+        No step uses cuDNN, and the step runs under torch.use_deterministic_algorithms(True).  Activations are
+        channels_last.  convraw.0 reads cat[fm, image, 5 zero channels] like the eval path.  Raises ValueError when
+        conv1, the max-pool or convraw.3 no longer have the shapes these kernels implement.
+
+        Returns (seg_pred, ver_pred), the channel slices of one contiguous NCHW tensor that the head writes directly:
+        the training losses then write a single gradient for it, and read it on their vectorised path.  NetWrapper's
+        change: `seg_pred, vertex_pred = self.net.forward_train(image)`."""
         if x.requires_grad:
             raise ValueError("forward_train: the input image must not require grad (it gets no gradient)")
         if not x.is_cuda:
             raise RuntimeError("pvnet_b200: forward_train runs only on CUDA (no CPU fallback)")
+        self._check_train_modules()
         cl = torch.channels_last
-        x = x.float().contiguous(memory_format=cl)
+        x = x.float()
+        x_nchw = x.contiguous()                       # the stem's space-to-depth pack reads NCHW
+        x = x.contiguous(memory_format=cl)            # convraw.0's concatenated input
         t = self.resnet18_8s
-        x2s = pc.bn_act(t.bn1, t.conv1(x), pc.act_of(t.relu))
-        x4s = t.maxpool(x2s)
+        x2s = pc.bn_act(t.bn1, pc.stem_train(x_nchw, t.conv1.weight), pc.act_of(t.relu))
+        x4s = pc.maxpool_train(x2s)
         for blk in t.layer1:
             x4s = self._block_train(blk, x4s)
         x8s = x4s
@@ -373,7 +399,8 @@ class Resnet18_8s(nn.Module):
         b, _, h, w = x.shape
         pad = torch.zeros(b, 5, h, w, dtype=torch.float32, device=x.device).contiguous(memory_format=cl)
         y = self._conv_bn_act(self.convraw, pc.upsample2x_cat(fm, x, pad), dgrad_channels=fm.shape[1])
-        out = self.convraw[3](y).contiguous()
+        head = self.convraw[3]
+        out = pc.head_train(y, head.weight, head.bias)
         return out[:, :self.seg_dim], out[:, self.seg_dim:]
 
     def forward(self, x, feature_alignment=False):
