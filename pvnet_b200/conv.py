@@ -438,11 +438,26 @@ class BatchNormAddReluNHWC(torch.autograd.Function):
             dbz if n[6] else None, None
 
 
+class BatchSizeError(ValueError, RuntimeError):
+    """Batch statistics over a single value per channel.  A ValueError, as nn.BatchNorm2d raises it; also a
+    RuntimeError, the class the C ABI's argument check has always reported it with."""
+
+
+def _bn_batch_check(state, x):
+    """nn.BatchNorm2d's _verify_batch_size, at the same point: after the module counted the batch, before any
+    statistic or running buffer is touched."""
+    if state.batch_stats and x.shape[0] * x.shape[2] * x.shape[3] == 1:
+        raise BatchSizeError(f"expected more than one value per channel when training, got input size "
+                             f"{tuple(x.shape)}")
+
+
 def bn_act(bn, x, act=ACT_NONE):
     """act(bn(x)) on the native kernels under autograd, following the module's training flag, momentum, eps and
     track_running_stats (see BatchNormActNHWC, BatchNormState)."""
     _bn_check(x, bn.num_features)                 # before the state counts a batch
-    return BatchNormActNHWC.apply(x, bn.weight, bn.bias, BatchNormState(bn, x.device), act)
+    state = BatchNormState(bn, x.device)
+    _bn_batch_check(state, x)
+    return BatchNormActNHWC.apply(x, bn.weight, bn.bias, state, act)
 
 
 def bn_add_relu(bn, a, skip, bn_skip=None):
@@ -451,6 +466,7 @@ def bn_add_relu(bn, a, skip, bn_skip=None):
     _bn_check(a, bn.num_features)
     _bn_check(skip, bn.num_features, a.shape)
     state = BatchNormState(bn, a.device)
+    _bn_batch_check(state, a)                     # bn raises before bn_skip runs, as in BasicBlock.forward
     if bn_skip is None:
         return BatchNormAddReluNHWC.apply(a, bn.weight, bn.bias, state, skip, None, None, None)
     return BatchNormAddReluNHWC.apply(a, bn.weight, bn.bias, state, skip, bn_skip.weight, bn_skip.bias,

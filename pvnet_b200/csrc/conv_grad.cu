@@ -27,6 +27,11 @@
 namespace pvnet {
 
 constexpr int WG_KP = 32;     // pixels per K-block: one 128-byte row of the K-major X tile
+// K-blocks one wgmma accumulator sums, in the one-warpgroup variants, before the CTA adds it into its partial tile and
+// restarts it from 0: the tensor cores' fp32 accumulation loses more than IEEE addition over long chains (DESIGN.md
+// §14, "Numerics")
+constexpr int WG_FLUSH_KB = 32;
+static_assert((WG_FLUSH_KB & (WG_FLUSH_KB - 1)) == 0, "WG_FLUSH_KB must be a power of 2");
 
 struct WgradGeom {
     const float *x, *dy;
@@ -46,6 +51,9 @@ __global__ void __launch_bounds__(NWG * 128, 2) k_conv_wgrad(const __grid_consta
 {
     constexpr int NT = NWG * 128;
     constexpr int BM = 64 * NWG;
+    // The two-warpgroup variants run at their 128-register limit (two CTAs of 256 threads per SM), where the flush
+    // spills; their layers have Cout >= 128, so more tiles and shorter chains per split.
+    constexpr bool FLUSH = NWG == 1;
     constexpr int LDA = BM + 8;                  // floats per pixel row of the dY tile: 8 t + g hits 32 banks
     constexpr int XI = WG_KP * BN / 4 / NT;      // float4 loads of X per thread and K-block
     constexpr int DI = WG_KP * BM / 4 / NT;      // float4 loads of dY per thread and K-block
@@ -113,6 +121,29 @@ __global__ void __launch_bounds__(NWG * 128, 2) k_conv_wgrad(const __grid_consta
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
 
+    // acc -> part[split][co][tap][ci]: stored by the first flush, added (fp32) by the later ones.  Each thread reads
+    // back only what it wrote itself.
+    auto flush = [&](bool first) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int co = co0 + mrow + 8 * h;
+            if (co >= g.Cout) continue;
+            float *dst = g.part + (((long long)split * g.Cout + co) * g.taps + tap) * g.Cin;
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j) {
+                const int ci = ci0 + 8 * j + 2 * t4;
+                if (ci < g.Cin) {
+                    float2 v = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+                    if (!first) {
+                        const float2 o = *reinterpret_cast<const float2 *>(dst + ci);
+                        v = make_float2(o.x + v.x, o.y + v.y);
+                    }
+                    *reinterpret_cast<float2 *>(dst + ci) = v;
+                }
+            }
+        }
+    };
+
     load(kb0);
     for (int kb = kb0; kb < kb1; ++kb) {
         __syncthreads();                               // every warpgroup's MMAs on the previous tiles have completed
@@ -129,6 +160,13 @@ __global__ void __launch_bounds__(NWG * 128, 2) k_conv_wgrad(const __grid_consta
             ptx::sts128(sa + (uint32_t)(((d_p + 8 * j) * LDA + 4 * d_q) * 4), dr[j]);
         ptx::fence_proxy_async();                      // generic-proxy stores -> visible to wgmma's operand reads
         __syncthreads();
+        if constexpr (FLUSH) {
+            if (kb > kb0 && ((kb - kb0) & (WG_FLUSH_KB - 1)) == 0) {   // K-blocks [kb - WG_FLUSH_KB, kb) are in acc
+                flush(kb - kb0 == WG_FLUSH_KB);        // here the loader's registers are free
+#pragma unroll
+                for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+            }
+        }
         if (kb + 1 < kb1) load(kb + 1);                // in flight during this K-block's MMAs
         uint32_t a[WG_KP / 8][4];
 #pragma unroll
@@ -148,20 +186,7 @@ __global__ void __launch_bounds__(NWG * 128, 2) k_conv_wgrad(const __grid_consta
         ptx::wgmma_wait<0>();                          // the A registers and the tiles are reused next K-block
         ptx::fence_regs(acc);
     }
-
-    // partial tile -> part[split][co][tap][ci]
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-        const int co = co0 + mrow + 8 * h;
-        if (co >= g.Cout) continue;
-        float *dst = g.part + (((long long)split * g.Cout + co) * g.taps + tap) * g.Cin;
-#pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-            const int ci = ci0 + 8 * j + 2 * t4;
-            if (ci < g.Cin)
-                *reinterpret_cast<float2 *>(dst + ci) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
-        }
-    }
+    flush(!FLUSH || kb1 - kb0 <= WG_FLUSH_KB);
 }
 
 // dW[co][ci][tap] (torch's [Cout][Cin][kh][kw]) = sum over splits, in split order.  Threads walk the partials in
