@@ -303,6 +303,10 @@ PVNET_API int pvnet_pose_metrics(const double *pose_pred, const double *pose_gt,
  *   seg_pred f32 [b,C,h,w] (seg_strides[4]) and mask [b,h,w] (mask_strides[3], elements of mask_elem_size bytes:
  *   8 int64, 4 int32, 1 uint8 / bool) for loss_seg / precision / recall;
  *   vertex_pred, vertex f32 [b,ver_dim,h,w] and vertex_weights f32 [b,1,h,w] (strides[4] each) for loss_vertex.
+ *   vertex_weights and weight_strides both NULL: each pixel's weight is its mask value converted to float, the
+ *   loader's vertex_weights = mask.unsqueeze(0).float() (linemod_dataset.py:227), read where the weights would be
+ *   read, so every output equals the call with that tensor; the mask is then needed for loss_vertex.  A NULL
+ *   vertex_weights with non-NULL strides is refused.  The same rule holds for the _keypoints and _backward forms.
  * seg_pred and vertex_pred may be channel slices of one [b,C+ver_dim,h,w] tensor (Resnet18_8s.forward,
  * model_repository.py:77-78).  Sums are fp64 / int64 in a fixed order: run-to-run identical, graph capturable.
  * Workspace: pvnet_seg_vertex_losses_workspace_bytes(b, h, w). */
@@ -549,6 +553,13 @@ PVNET_API int pvnet_batchnorm_act_backward(int form, int act, const float *dy, c
  *   (channel (py*2+px)*3+c, 4 zero channels, rounded to TF32) and out NHWC [b,H/2,W/2,64] = the 4x4 stride-1 tensor-core
  *   convolution of s2d with w_s2d (packed [64][4][4][16] as backbone slot 26, TF32) plus bias [64], fp32, no
  *   activation.  s2d is what pvnet_stem_s2d_wgrad reads.
+ * pvnet_stem_s2d_u8_nhwc: pvnet_stem_s2d_nhwc of the raw image image_u8 uint8 [b,H,W,3] contiguous (H, W even;
+ *   2-byte aligned), normalised on the device as torchvision's ToTensor + Normalize on the CPU compute it:
+ *   v = (float(u) / 255 - mean3[c]) / std3[c], three correctly rounded fp32 ops (mean3 / std3: 3 host floats each,
+ *   finite, std nonzero).  s2d and out are the float form's for the image v.  In the same pass the caller's
+ *   channels_last buffer img NHWC [b,H,W,img_cs] gets v unrounded in channels [img_co, img_co+3) and zeros in
+ *   [img_co+3, img_co+8) (img_co, img_cs multiples of 4, img_co+8 <= img_cs): convraw.0's image and pad channels;
+ *   its other channels are not touched.
  * pvnet_stem_s2d_wgrad: dw [64][3][7][7] (torch's layout, overwritten) = the weight gradient of that convolution for
  *   dout NHWC [b,H/2,W/2,64] dense: the 4x4 weight gradient on s2d (TF32 operands, dout truncated by the tensor
  *   cores, fp32 accumulation, pixel splits added in a fixed order: identical run to run), folded back onto the
@@ -568,6 +579,9 @@ PVNET_API int pvnet_batchnorm_act_backward(int form, int act, const float *dy, c
  * All offsets are 64-bit; pointers 16-byte aligned unless stated. */
 PVNET_API int pvnet_stem_s2d_nhwc(const float *image_nchw, const float *w_s2d, const float *bias, float *s2d,
                                   float *out, int b, int H, int W, pvnet_stream_t stream);
+PVNET_API int pvnet_stem_s2d_u8_nhwc(const uint8_t *image_u8, const float *mean3, const float *std3,
+                                     const float *w_s2d, const float *bias, float *s2d, float *out, float *img,
+                                     int img_cs, int img_co, int b, int H, int W, pvnet_stream_t stream);
 PVNET_API int pvnet_stem_s2d_wgrad_workspace_bytes(int b, int H, int W, size_t *bytes);
 PVNET_API int pvnet_stem_s2d_wgrad(const float *s2d, const float *dout, float *dw, int b, int H, int W,
                                    void *workspace, size_t workspace_bytes, pvnet_stream_t stream);

@@ -270,6 +270,54 @@ def upsample2x_cat(low, *rest):
     return Upsample2xCatNHWC.apply(low, *rest)
 
 
+class Upsample2xIntoNHWC(torch.autograd.Function):
+    """Upsample2xCatNHWC with the concatenated buffer given: F.interpolate(low, scale_factor=2, mode="bilinear",
+    align_corners=True) of a [b,C,h,w] `low` written in place into channels [0, C) of `buf`, a channels_last
+    [b,Cb,2h,2w] float32 tensor that needs no gradient, whose other channels the caller has filled (the uint8
+    training path: the stem's pack writes convraw.0's image and pad channels).  Returns `buf` (marked dirty).
+    Forward pvnet_upsample2x_nhwc, backward pvnet_upsample2x_backward_nhwc of the gradient's first C channels, as
+    Upsample2xCatNHWC; no copy of the other channels is made in either direction."""
+
+    @staticmethod
+    def forward(ctx, low, buf):
+        _check_float_cuda("Upsample2xIntoNHWC", low, buf)
+        b, C, h, w = low.shape
+        if buf.dim() != 4 or buf.shape[0] != b or tuple(buf.shape[2:]) != (2 * h, 2 * w) or buf.shape[1] < C or \
+                not buf.is_contiguous(memory_format=torch.channels_last):
+            raise ValueError(f"buf must be a channels_last [{b}, >= {C}, {2 * h}, {2 * w}] tensor, got "
+                             f"{tuple(buf.shape)}")
+        if buf.requires_grad:
+            raise ValueError("Upsample2xIntoNHWC: buf gets no gradient, so it must not require one")
+        dev = low.device
+        lh = _nhwc(low)
+        with torch.cuda.device(dev):
+            _native.check(_native.lib().pvnet_upsample2x_nhwc(_p(lh), C, _p(buf), buf.shape[1], 0, b, h, w,
+                                                              _stream(dev)), "pvnet_upsample2x_nhwc")
+        ctx.mark_dirty(buf)
+        ctx.C = C
+        return buf
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gy):
+        if not ctx.needs_input_grad[0]:
+            return None, None
+        b, _, H, W = gy.shape
+        C, h, w = ctx.C, H // 2, W // 2
+        gyh = _nhwc(gy.float())
+        dev = gyh.device
+        dlow = torch.empty(b, C, h, w, dtype=torch.float32, device=dev, memory_format=torch.channels_last)
+        with torch.cuda.device(dev):
+            _native.check(_native.lib().pvnet_upsample2x_backward_nhwc(_p(gyh), gyh.shape[3], 0, C, _p(dlow), b, h, w,
+                                                                       _stream(dev)), "pvnet_upsample2x_backward_nhwc")
+        return dlow, None
+
+
+def upsample2x_into(low, buf):
+    """Upsample2xIntoNHWC.apply: the upsampled `low` written into the first channels of `buf` under autograd."""
+    return Upsample2xIntoNHWC.apply(low, buf)
+
+
 # ----------------------------------------------------------------------------- train-mode BatchNorm (autograd)
 FORM_ACT, FORM_ADD_RELU, FORM_ADD_BN_RELU = 0, 1, 2
 
@@ -555,28 +603,95 @@ class StemS2dNHWC(torch.autograd.Function):
     @staticmethod
     @once_differentiable
     def backward(ctx, gy):
-        s2d, = ctx.saved_tensors
         if not ctx.needs_input_grad[1]:
             return None, None
-        b = s2d.shape[0]
-        H, W = ctx.hw
-        dev = s2d.device
-        gyh = _nhwc(gy.float())
-        L = _native.lib()
-        with torch.cuda.device(dev):
-            n = ctypes.c_size_t()
-            _native.check(L.pvnet_stem_s2d_wgrad_workspace_bytes(b, H, W, ctypes.byref(n)),
-                          "pvnet_stem_s2d_wgrad_workspace_bytes")
-            ws = torch.empty(max(n.value, 16), dtype=torch.uint8, device=dev)
-            dw = torch.empty(64, 3, 7, 7, dtype=torch.float32, device=dev)
-            _native.check(L.pvnet_stem_s2d_wgrad(_p(s2d), _p(gyh), _p(dw), b, H, W, _p(ws), ws.numel(), _stream(dev)),
-                          "pvnet_stem_s2d_wgrad")
-        return None, dw
+        return None, _stem_wgrad(ctx, gy)
+
+
+def _stem_wgrad(ctx, gy):
+    """pvnet_stem_s2d_wgrad of the S the forward saved: dW [64,3,7,7]."""
+    s2d, = ctx.saved_tensors
+    b = s2d.shape[0]
+    H, W = ctx.hw
+    dev = s2d.device
+    gyh = _nhwc(gy.float())
+    L = _native.lib()
+    with torch.cuda.device(dev):
+        n = ctypes.c_size_t()
+        _native.check(L.pvnet_stem_s2d_wgrad_workspace_bytes(b, H, W, ctypes.byref(n)),
+                      "pvnet_stem_s2d_wgrad_workspace_bytes")
+        ws = torch.empty(max(n.value, 16), dtype=torch.uint8, device=dev)
+        dw = torch.empty(64, 3, 7, 7, dtype=torch.float32, device=dev)
+        _native.check(L.pvnet_stem_s2d_wgrad(_p(s2d), _p(gyh), _p(dw), b, H, W, _p(ws), ws.numel(), _stream(dev)),
+                      "pvnet_stem_s2d_wgrad")
+    return dw
 
 
 def stem_train(x, weight):
     """StemS2dNHWC.apply: conv1 (7x7/2, pad 3, no bias) on the native kernels under autograd."""
     return StemS2dNHWC.apply(x, weight)
+
+
+def norm3(mean, std):
+    """ToTensor + Normalize constants (sequences of numbers or CPU tensors; a CUDA tensor would cost a synchronising
+    read) as the two ctypes float[3] pvnet_stem_s2d_u8_nhwc takes; ValueError unless each has exactly three values."""
+    vals = []
+    for name, v in (("mean", mean), ("std", std)):
+        v = [float(t) for t in (v.flatten().tolist() if isinstance(v, torch.Tensor) else v)]
+        if len(v) != 3:
+            raise ValueError(f"{name} must have 3 values (one per colour channel), got {len(v)}")
+        vals.append((ctypes.c_float * 3)(*v))
+    return vals
+
+
+class StemS2dU8NHWC(torch.autograd.Function):
+    """StemS2dNHWC of a raw uint8 [b,H,W,3] image (contiguous, H, W even), normalised on the device as torchvision's
+    ToTensor + Normalize compute it on the CPU ((u/255 - mean)/std, three correctly rounded fp32 ops):
+    pvnet_stem_s2d_u8_nhwc.  In the same pass it writes the normalised image, unrounded, into channels [co, co+3) of
+    `img` (a [b,C,H,W] channels_last float32 buffer; the 5 channels behind it get zeros, the others are not touched):
+    convraw.0's concatenated input.  `img` gets no gradient and must not require one.  The output, S and the weight
+    gradient are StemS2dNHWC's for the normalised image."""
+
+    @staticmethod
+    def forward(ctx, x, weight, mean, std, img, co):
+        _check_float_cuda("StemS2dU8NHWC", weight, img)
+        if not x.is_cuda or x.dtype != torch.uint8:
+            raise ValueError(f"StemS2dU8NHWC needs a uint8 CUDA image, got {x.dtype} on {x.device}")
+        if x.dim() != 4 or x.shape[3] != 3 or x.shape[1] % 2 or x.shape[2] % 2 or tuple(weight.shape) != (64, 3, 7, 7):
+            raise ValueError(f"StemS2dU8NHWC needs x [b,H,W,3] with H, W even and weight [64,3,7,7], got "
+                             f"{tuple(x.shape)} and {tuple(weight.shape)}")
+        b, H, W, _ = x.shape
+        if img.dim() != 4 or img.shape[0] != b or tuple(img.shape[2:]) != (H, W) or \
+                not img.is_contiguous(memory_format=torch.channels_last):
+            raise ValueError(f"img must be a channels_last [{b},C,{H},{W}] buffer, got {tuple(img.shape)}")
+        if img.requires_grad:
+            raise ValueError("StemS2dU8NHWC: img gets no gradient, so it must not require one")
+        mean3, std3 = norm3(mean, std)
+        dev = x.device
+        xc = x.contiguous()
+        s2d = torch.empty(b, H // 2, W // 2, 16, dtype=torch.float32, device=dev)
+        out = torch.empty(b, 64, H // 2, W // 2, dtype=torch.float32, device=dev, memory_format=torch.channels_last)
+        w4 = pack_stem_s2d_train(weight.detach())
+        bias = torch.zeros(64, dtype=torch.float32, device=dev)
+        with torch.cuda.device(dev):
+            _native.check(_native.lib().pvnet_stem_s2d_u8_nhwc(
+                _p(xc), mean3, std3, _p(w4), _p(bias), _p(s2d), _p(out), _p(img), img.shape[1], co, b, H, W,
+                _stream(dev)), "pvnet_stem_s2d_u8_nhwc")
+        ctx.save_for_backward(s2d)
+        ctx.hw = (H, W)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gy):
+        dw = _stem_wgrad(ctx, gy) if ctx.needs_input_grad[1] else None
+        return None, dw, None, None, None, None
+
+
+def stem_train_u8(x, weight, mean, std, img, co):
+    """StemS2dU8NHWC.apply: conv1 of a raw uint8 image, normalised on the device, which also fills convraw.0's image
+    channels of `img` (see StemS2dU8NHWC)."""
+    return StemS2dU8NHWC.apply(x, weight, mean, std, img, co)
 
 
 class MaxPool3x3s2NHWC(torch.autograd.Function):

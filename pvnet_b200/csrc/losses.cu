@@ -151,6 +151,21 @@ __device__ __forceinline__ void fg_quad(const MT *p, bool full, int n, bool (&fg
     for (int j = 0; j < 4; ++j) fg[j] = j < n && t[j] == 1;       // np.argwhere(mask == 1)
 }
 
+// the vertex weights of a quad: read from a.wgt, or (MW: the caller passed no weights) the pixel's mask value
+// converted to float -- the reference's vertex_weights = mask.unsqueeze(0).float() (linemod_dataset.py:227)
+template <typename MT, bool MW>
+__device__ __forceinline__ void weights4(const LossArgs &a, int img, int y, int x0, bool full, int n, float (&wv)[4])
+{
+    if constexpr (MW) {
+        long long t[4];
+        load_mask4(static_cast<const MT *>(a.mask) + img * a.m_b + y * a.m_h + x0, full, n, t);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) wv[j] = (float)t[j];
+    } else {
+        load4(a.wgt + img * a.w_b + y * a.w_h + x0, full, n, wv);
+    }
+}
+
 template <typename T>
 __device__ __forceinline__ T warp_sum(T v)
 {
@@ -191,8 +206,9 @@ __device__ __forceinline__ void ver_channel(const LossArgs &a, int c, float *e0,
 constexpr int LS_KP_MIN_BLOCKS = 2;
 
 // grid (chunks, b), MT = the mask element type (int64, int32, uint8 / bool); KP: the vertex targets are computed
-// from the keypoints `kp` (foreground = mask == 1) instead of read from a.tgt
-template <typename MT, bool KP>
+// from the keypoints `kp` (foreground = mask == 1) instead of read from a.tgt; MW: the vertex weights are the mask
+// values (weights4) instead of read from a.wgt
+template <typename MT, bool KP, bool MW = false>
 __global__ void __launch_bounds__(LS_THREADS, KP ? LS_KP_MIN_BLOCKS : 3)
     k_losses_partial(LossArgs a, LossPartial *__restrict__ partial, KpArgs kp)
 {
@@ -255,7 +271,7 @@ __global__ void __launch_bounds__(LS_THREADS, KP ? LS_KP_MIN_BLOCKS : 3)
 
         if (a.do_ver) {
             float wv[4];
-            load4(a.wgt + img * a.w_b + y * a.w_h + x0, full, n, wv);
+            weights4<MT, MW>(a, img, y, x0, full, n, wv);
 #pragma unroll
             for (int j = 0; j < 4; ++j)
                 if (j < n) sw += (double)wv[j];
@@ -429,8 +445,8 @@ __device__ __forceinline__ void ver_grad(const LossArgs &a, float gi, const floa
     }
 }
 
-// grid (chunks, b), the quad assignment of k_losses_partial; each thread writes its quads' gradients
-template <typename MT, bool KP>
+// grid (chunks, b), the quad assignment of k_losses_partial; each thread writes its quads' gradients (MW as there)
+template <typename MT, bool KP, bool MW = false>
 __global__ void __launch_bounds__(LS_THREADS, KP ? LS_KP_MIN_BLOCKS : 3)
     k_losses_backward(LossArgs a, GradArgs g, KpArgs kp)
 {
@@ -493,7 +509,7 @@ __global__ void __launch_bounds__(LS_THREADS, KP ? LS_KP_MIN_BLOCKS : 3)
                 continue;
             }
             float wv[4], o[4];
-            load4(a.wgt + img * a.w_b + y * a.w_h + x0, full, n, wv);
+            weights4<MT, MW>(a, img, y, x0, full, n, wv);
             const float *p0 = a.pred + img * a.p_b + y * a.p_h + x0;
             if constexpr (KP) {
                 bool fg[4];
@@ -528,7 +544,9 @@ __global__ void __launch_bounds__(LS_THREADS, KP ? LS_KP_MIN_BLOCKS : 3)
 }
 
 // grid (chunks, b): Σw of each CTA's quads, summed exactly as k_losses_partial sums `sw` (same thread order, shuffle
-// tree and warp order), so that k_grad_final's denominator is the forward's bit for bit
+// tree and warp order), so that k_grad_final's denominator is the forward's bit for bit (MW: the weights are the mask
+// values of element type MT, weights4)
+template <typename MT, bool MW>
 __global__ void __launch_bounds__(LS_THREADS) k_weight_sum_partial(LossArgs a, double *__restrict__ partial)
 {
     const int img = blockIdx.y;
@@ -539,7 +557,7 @@ __global__ void __launch_bounds__(LS_THREADS) k_weight_sum_partial(LossArgs a, d
         const int x0 = (q - y * a.qw) * 4;
         const int n = min(4, a.w - x0);
         float wv[4];
-        load4(a.wgt + img * a.w_b + y * a.w_h + x0, a.vec && n == 4, n, wv);
+        weights4<MT, MW>(a, img, y, x0, a.vec && n == 4, n, wv);
 #pragma unroll
         for (int j = 0; j < 4; ++j)
             if (j < n) sw += (double)wv[j];
@@ -601,15 +619,26 @@ bool strides_ok(const int64_t *s, int k)
     return true;
 }
 
-template <bool KP>
+template <bool KP, bool MW = false>
 void launch_partial(int msz, dim3 grid, cudaStream_t st, const LossArgs &a, LossPartial *partial, const KpArgs &kp)
 {
     if (msz == 8)
-        k_losses_partial<long long, KP><<<grid, LS_THREADS, 0, st>>>(a, partial, kp);
+        k_losses_partial<long long, KP, MW><<<grid, LS_THREADS, 0, st>>>(a, partial, kp);
     else if (msz == 4)
-        k_losses_partial<int, KP><<<grid, LS_THREADS, 0, st>>>(a, partial, kp);
+        k_losses_partial<int, KP, MW><<<grid, LS_THREADS, 0, st>>>(a, partial, kp);
     else
-        k_losses_partial<unsigned char, KP><<<grid, LS_THREADS, 0, st>>>(a, partial, kp);
+        k_losses_partial<unsigned char, KP, MW><<<grid, LS_THREADS, 0, st>>>(a, partial, kp);
+}
+
+template <bool KP, bool MW>
+void launch_backward(int msz, dim3 grid, cudaStream_t st, const LossArgs &a, const GradArgs &g, const KpArgs &kp)
+{
+    if (msz == 8)
+        k_losses_backward<long long, KP, MW><<<grid, LS_THREADS, 0, st>>>(a, g, kp);
+    else if (msz == 4)
+        k_losses_backward<int, KP, MW><<<grid, LS_THREADS, 0, st>>>(a, g, kp);
+    else
+        k_losses_backward<unsigned char, KP, MW><<<grid, LS_THREADS, 0, st>>>(a, g, kp);
 }
 
 // pvnet_seg_vertex_losses (kp == NULL: targets read from vertex) and pvnet_seg_vertex_losses_keypoints (kp: targets
@@ -625,7 +654,9 @@ int seg_vertex_losses(const float *seg_pred, const int64_t seg_strides[4], const
     PV_CHECK_ARG(b <= 65535, "batch %d above 65535", b);
     const bool do_ce = loss_seg != nullptr, do_pr = precision != nullptr || recall != nullptr;
     const bool do_ver = loss_vertex != nullptr;
-    const bool need_mask = do_ce || do_pr || (do_ver && kp);
+    // no weights and no weight strides: the weights are the mask values (a NULL pointer with strides stays an error)
+    const bool mw = do_ver && !vertex_weights && !weight_strides;
+    const bool need_mask = do_ce || do_pr || (do_ver && (kp || mw));
     PV_CHECK_ARG(do_ce || do_pr || do_ver, "no output requested (loss_seg, loss_vertex, precision, recall all null)");
     if (do_ce || do_pr) {
         PV_CHECK_ARG(seg_pred && seg_strides, "null pointer (seg_pred or its strides)");
@@ -639,12 +670,12 @@ int seg_vertex_losses(const float *seg_pred, const int64_t seg_strides[4], const
         PV_CHECK_ARG(mask_strides[2] == 1, "unit stride along w is not 1 (mask %lld)", (long long)mask_strides[2]);
     }
     if (do_ver) {
-        PV_CHECK_ARG(vertex_pred && pred_strides && vertex_weights && weight_strides,
+        PV_CHECK_ARG(vertex_pred && pred_strides && (mw || (vertex_weights && weight_strides)),
                      "null pointer (vertex_pred / vertex_weights or their strides)");
         PV_CHECK_ARG(ver_dim >= 1, "non-positive dimension (ver_dim=%d)", ver_dim);
-        PV_CHECK_ARG(pred_strides[3] == 1 && weight_strides[3] == 1,
+        PV_CHECK_ARG(pred_strides[3] == 1 && (mw || weight_strides[3] == 1),
                      "unit stride along w is not 1 (vertex_pred %lld, vertex_weights %lld)",
-                     (long long)pred_strides[3], (long long)weight_strides[3]);
+                     (long long)pred_strides[3], mw ? 1LL : (long long)weight_strides[3]);
         if (kp) {
             PV_CHECK_ARG(kp->hc, "null pointer (hcoords)");
             PV_CHECK_ARG(ver_dim == 2 * kp->K, "ver_dim %d is not 2 x the number of keypoints", ver_dim);
@@ -681,10 +712,12 @@ int seg_vertex_losses(const float *seg_pred, const int64_t seg_strides[4], const
             a.tgt = vertex, a.t_b = vertex_strides[0], a.t_c = vertex_strides[1], a.t_h = vertex_strides[2];
             vec = vec && aligned(vertex, 16) && strides_ok(vertex_strides, 3);
         }
-        a.wgt = vertex_weights, a.w_b = weight_strides[0], a.w_h = weight_strides[2];
+        if (!mw) {
+            a.wgt = vertex_weights, a.w_b = weight_strides[0], a.w_h = weight_strides[2];
+            vec = vec && aligned(vertex_weights, 16) && weight_strides[0] % 4 == 0 && weight_strides[2] % 4 == 0;
+        }
         a.elem = normalize ? nullptr : loss_vertex;
-        vec = vec && aligned(vertex_pred, 16) && aligned(vertex_weights, 16) && strides_ok(pred_strides, 3) &&
-              weight_strides[0] % 4 == 0 && weight_strides[2] % 4 == 0 &&
+        vec = vec && aligned(vertex_pred, 16) && strides_ok(pred_strides, 3) &&
               (normalize || (aligned(loss_vertex, 16) && w % 4 == 0));
     }
     a.vec = vec;
@@ -694,11 +727,17 @@ int seg_vertex_losses(const float *seg_pred, const int64_t seg_strides[4], const
     cudaStream_t st = (cudaStream_t)stream;
     const int msz = need_mask ? mask_elem_size : 8;
     if (kp && do_ver) {
-        launch_partial<true>(msz, grid, st, a, partial, *kp);
+        if (mw)
+            launch_partial<true, true>(msz, grid, st, a, partial, *kp);
+        else
+            launch_partial<true>(msz, grid, st, a, partial, *kp);
         PV_LAUNCHED(msz == 8 ? "k_losses_partial<int64, keypoints>"
                     : msz == 4 ? "k_losses_partial<int32, keypoints>" : "k_losses_partial<uint8, keypoints>");
     } else {
-        launch_partial<false>(msz, grid, st, a, partial, KpArgs{});
+        if (mw)
+            launch_partial<false, true>(msz, grid, st, a, partial, KpArgs{});
+        else
+            launch_partial<false>(msz, grid, st, a, partial, KpArgs{});
         PV_LAUNCHED(msz == 8 ? "k_losses_partial<int64>" : msz == 4 ? "k_losses_partial<int32>" : "k_losses_partial<uint8>");
     }
     k_losses_final<<<(b + 127) / 128, 128, 0, st>>>(partial, chunks, b, (double)h * w, ver_dim, loss_seg,
@@ -722,7 +761,8 @@ int seg_vertex_losses_backward(const float *seg_pred, const int64_t seg_strides[
     PV_CHECK_ARG(b <= 65535, "batch %d above 65535", b);
     PV_CHECK_ARG(grad_seg || grad_vertex, "no output requested (grad_seg, grad_vertex both null)");
     const bool do_ce = grad_seg && grad_loss_seg, do_ver = grad_vertex && grad_loss_vertex;
-    const bool need_mask = do_ce || (do_ver && kp);
+    const bool mw = do_ver && !vertex_weights && !weight_strides;     // weights = mask values, as in the forward
+    const bool need_mask = do_ce || (do_ver && (kp || mw));
     if (grad_seg) {
         PV_CHECK_ARG(grad_seg_strides, "null pointer (grad_seg_strides)");
         PV_CHECK_ARG(C >= 1, "non-positive dimension (C=%d)", C);
@@ -746,11 +786,11 @@ int seg_vertex_losses_backward(const float *seg_pred, const int64_t seg_strides[
         PV_CHECK_ARG(mask_strides[2] == 1, "unit stride along w is not 1 (mask %lld)", (long long)mask_strides[2]);
     }
     if (do_ver) {
-        PV_CHECK_ARG(vertex_pred && pred_strides && vertex_weights && weight_strides,
+        PV_CHECK_ARG(vertex_pred && pred_strides && (mw || (vertex_weights && weight_strides)),
                      "null pointer (vertex_pred / vertex_weights or their strides)");
-        PV_CHECK_ARG(pred_strides[3] == 1 && weight_strides[3] == 1,
+        PV_CHECK_ARG(pred_strides[3] == 1 && (mw || weight_strides[3] == 1),
                      "unit stride along w is not 1 (vertex_pred %lld, vertex_weights %lld)",
-                     (long long)pred_strides[3], (long long)weight_strides[3]);
+                     (long long)pred_strides[3], mw ? 1LL : (long long)weight_strides[3]);
         if (kp) {
             PV_CHECK_ARG(kp->hc, "null pointer (hcoords)");
             PV_CHECK_ARG(ver_dim == 2 * kp->K, "ver_dim %d is not 2 x the number of keypoints", ver_dim);
@@ -798,9 +838,11 @@ int seg_vertex_losses_backward(const float *seg_pred, const int64_t seg_strides[
             a.tgt = vertex, a.t_b = vertex_strides[0], a.t_c = vertex_strides[1], a.t_h = vertex_strides[2];
             vec = vec && aligned(vertex, 16) && strides_ok(vertex_strides, 3);
         }
-        a.wgt = vertex_weights, a.w_b = weight_strides[0], a.w_h = weight_strides[2];
-        vec = vec && aligned(vertex_pred, 16) && aligned(vertex_weights, 16) && strides_ok(pred_strides, 3) &&
-              weight_strides[0] % 4 == 0 && weight_strides[2] % 4 == 0;
+        if (!mw) {
+            a.wgt = vertex_weights, a.w_b = weight_strides[0], a.w_h = weight_strides[2];
+            vec = vec && aligned(vertex_weights, 16) && weight_strides[0] % 4 == 0 && weight_strides[2] % 4 == 0;
+        }
+        vec = vec && aligned(vertex_pred, 16) && strides_ok(pred_strides, 3);
     }
     a.vec = vec;
     // workspace: Σw partials (double [b, chunks]), gi (float [b]), invalid-target flags (int [b, chunks])
@@ -810,32 +852,39 @@ int seg_vertex_losses_backward(const float *seg_pred, const int64_t seg_strides[
     g.bad = reinterpret_cast<int *>(gi + b);
     const dim3 grid(chunks, b);
     cudaStream_t st = (cudaStream_t)stream;
+    const int msz = need_mask ? mask_elem_size : 8;
     if (do_ver) {
         LossArgs wa = a;
-        wa.vec = aligned(vertex_weights, 16) && weight_strides[0] % 4 == 0 && weight_strides[2] % 4 == 0;
-        k_weight_sum_partial<<<grid, LS_THREADS, 0, st>>>(wa, wsum);
+        if (mw) {
+            // the mask's own vectorisation rule; the sums do not depend on it
+            wa.vec = aligned(mask, 4 * mask_elem_size) && strides_ok(mask_strides, 2);
+            if (msz == 8)
+                k_weight_sum_partial<long long, true><<<grid, LS_THREADS, 0, st>>>(wa, wsum);
+            else if (msz == 4)
+                k_weight_sum_partial<int, true><<<grid, LS_THREADS, 0, st>>>(wa, wsum);
+            else
+                k_weight_sum_partial<unsigned char, true><<<grid, LS_THREADS, 0, st>>>(wa, wsum);
+        } else {
+            wa.vec = aligned(vertex_weights, 16) && weight_strides[0] % 4 == 0 && weight_strides[2] % 4 == 0;
+            k_weight_sum_partial<float, false><<<grid, LS_THREADS, 0, st>>>(wa, wsum);
+        }
         PV_LAUNCHED("k_weight_sum_partial");
         k_grad_final<<<(b + 127) / 128, 128, 0, st>>>(wsum, chunks, b, ver_dim, grad_loss_vertex, gi);
         PV_LAUNCHED("k_grad_final");
         g.gi = gi;
     }
-    const int msz = need_mask ? mask_elem_size : 8;
     if (kp && do_ver) {
-        if (msz == 8)
-            k_losses_backward<long long, true><<<grid, LS_THREADS, 0, st>>>(a, g, *kp);
-        else if (msz == 4)
-            k_losses_backward<int, true><<<grid, LS_THREADS, 0, st>>>(a, g, *kp);
+        if (mw)
+            launch_backward<true, true>(msz, grid, st, a, g, *kp);
         else
-            k_losses_backward<unsigned char, true><<<grid, LS_THREADS, 0, st>>>(a, g, *kp);
+            launch_backward<true, false>(msz, grid, st, a, g, *kp);
         PV_LAUNCHED(msz == 8 ? "k_losses_backward<int64, keypoints>"
                     : msz == 4 ? "k_losses_backward<int32, keypoints>" : "k_losses_backward<uint8, keypoints>");
     } else {
-        if (msz == 8)
-            k_losses_backward<long long, false><<<grid, LS_THREADS, 0, st>>>(a, g, KpArgs{});
-        else if (msz == 4)
-            k_losses_backward<int, false><<<grid, LS_THREADS, 0, st>>>(a, g, KpArgs{});
+        if (mw)
+            launch_backward<false, true>(msz, grid, st, a, g, KpArgs{});
         else
-            k_losses_backward<unsigned char, false><<<grid, LS_THREADS, 0, st>>>(a, g, KpArgs{});
+            launch_backward<false, false>(msz, grid, st, a, g, KpArgs{});
         PV_LAUNCHED(msz == 8 ? "k_losses_backward<int64>" : msz == 4 ? "k_losses_backward<int32>"
                                                                       : "k_losses_backward<uint8>");
     }

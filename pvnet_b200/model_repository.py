@@ -353,7 +353,7 @@ class Resnet18_8s(nn.Module):
                 and hd.dilation == (1, 1) and hd.groups == 1 and hd.bias is not None):
             raise ValueError("forward_train: convraw[3] must be a 1x1 convolution with bias")
 
-    def forward_train(self, x):
+    def forward_train(self, x, mean=None, std=None):
         """The train-mode forward (`_forward_torch`) with every layer on the native kernels under autograd:
         * the stem conv1 as pvnet_b200.conv.stem_train (the eval path's space-to-depth tensor-core forward, a wgmma
           weight gradient; the image gets no gradient, so it must not require one: ValueError);
@@ -371,18 +371,43 @@ class Resnet18_8s(nn.Module):
 
         Returns (seg_pred, ver_pred), the channel slices of one contiguous NCHW tensor that the head writes directly:
         the training losses then write a single gradient for it, and read it on their vectorised path.  NetWrapper's
-        change: `seg_pred, vertex_pred = self.net.forward_train(image)`."""
+        change: `seg_pred, vertex_pred = self.net.forward_train(image)`.
+
+        x may also be the loader's raw uint8 [b,H,W,3] image (before ToTensor), with mean= and std= the Normalize
+        constants (3 numbers each), as forward_native takes it: the stem's pack (pvnet_b200.conv.stem_train_u8)
+        normalises it on the device exactly as ToTensor + Normalize do on the CPU and writes the normalised image into
+        convraw.0's input buffer, allocated once per step, into which upsample2x_into then writes the upsampled
+        decoder features: no float image and no concatenation copy.  Every output, gradient and running statistic is
+        that of the float path on the normalised image.  ValueError for a uint8 input without mean and std, for mean
+        or std with a float input, and for a uint8 input that is not [b,H,W,3]."""
         if x.requires_grad:
             raise ValueError("forward_train: the input image must not require grad (it gets no gradient)")
+        raw_u8 = x.dtype == torch.uint8
+        if raw_u8:
+            if mean is None or std is None:
+                raise ValueError("forward_train: a uint8 image needs mean= and std= (the Normalize constants)")
+            if x.dim() != 4 or x.shape[3] != 3:
+                raise ValueError(f"forward_train: a uint8 image must be [b,H,W,3], got {tuple(x.shape)}")
+        elif mean is not None or std is not None:
+            raise ValueError("forward_train: mean= and std= apply to a uint8 image; a float image is already "
+                             "normalised")
         if not x.is_cuda:
             raise RuntimeError("pvnet_b200: forward_train runs only on CUDA (no CPU fallback)")
         self._check_train_modules()
         cl = torch.channels_last
-        x = x.float()
-        x_nchw = x.contiguous()                       # the stem's space-to-depth pack reads NCHW
-        x = x.contiguous(memory_format=cl)            # convraw.0's concatenated input
         t = self.resnet18_8s
-        x2s = pc.bn_act(t.bn1, pc.stem_train(x_nchw, t.conv1.weight), pc.act_of(t.relu))
+        if raw_u8:
+            b, h, w, _ = x.shape
+            s2dim = self.conv2s[0].out_channels
+            # convraw.0's input cat[fm, image, 5 zeros]: the stem's pack fills channels [s2dim, s2dim+8) now, the
+            # decoder's upsampling channels [0, s2dim) at the end
+            raw_in = torch.empty(b, s2dim + 8, h, w, dtype=torch.float32, device=x.device, memory_format=cl)
+            x2s = pc.bn_act(t.bn1, pc.stem_train_u8(x, t.conv1.weight, mean, std, raw_in, s2dim), pc.act_of(t.relu))
+        else:
+            x = x.float()
+            x_nchw = x.contiguous()                   # the stem's space-to-depth pack reads NCHW
+            x = x.contiguous(memory_format=cl)        # convraw.0's concatenated input
+            x2s = pc.bn_act(t.bn1, pc.stem_train(x_nchw, t.conv1.weight), pc.act_of(t.relu))
         x4s = pc.maxpool_train(x2s)
         for blk in t.layer1:
             x4s = self._block_train(blk, x4s)
@@ -396,9 +421,12 @@ class Resnet18_8s(nn.Module):
         fm = self._conv_bn_act(self.conv8s, torch.cat([xfc, x8s], 1))
         fm = self._conv_bn_act(self.conv4s, pc.upsample2x_cat(fm, x4s))
         fm = self._conv_bn_act(self.conv2s, pc.upsample2x_cat(fm, x2s))
-        b, _, h, w = x.shape
-        pad = torch.zeros(b, 5, h, w, dtype=torch.float32, device=x.device).contiguous(memory_format=cl)
-        y = self._conv_bn_act(self.convraw, pc.upsample2x_cat(fm, x, pad), dgrad_channels=fm.shape[1])
+        if raw_u8:
+            y = self._conv_bn_act(self.convraw, pc.upsample2x_into(fm, raw_in), dgrad_channels=fm.shape[1])
+        else:
+            b, _, h, w = x.shape
+            pad = torch.zeros(b, 5, h, w, dtype=torch.float32, device=x.device).contiguous(memory_format=cl)
+            y = self._conv_bn_act(self.convraw, pc.upsample2x_cat(fm, x, pad), dgrad_channels=fm.shape[1])
         head = self.convraw[3]
         out = pc.head_train(y, head.weight, head.bias)
         return out[:, :self.seg_dim], out[:, self.seg_dim:]

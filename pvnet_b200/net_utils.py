@@ -5,8 +5,10 @@ reference's entry points import from that module.
 
     smooth_l1_loss(vertex_pred, vertex_targets, vertex_weights, sigma=1.0, normalize=True, reduce=True)
     compute_precision_recall(scores, target, reduce=False)
-    seg_vertex_losses(seg_pred, vertex_pred, mask, vertex, vertex_weights)
-                                   -> (loss_seg, loss_vertex, precision, recall), all four in one launch pair
+    seg_vertex_losses(seg_pred, vertex_pred, mask, vertex, vertex_weights=None)
+                                   -> (loss_seg, loss_vertex, precision, recall), all four in one launch pair;
+                                   vertex_weights=None: the weights are the mask's values (mask_weights), read by
+                                   the kernels from the mask (here and in the three functions below)
     vertex_targets(mask, hcoords, use_motion=False)
                                    the loader's ground-truth vertex field [b,2K,h,w] (compute_vertex_hcoords)
     seg_vertex_losses_from_keypoints(seg_pred, vertex_pred, mask, hcoords, vertex_weights, use_motion=False)
@@ -63,15 +65,32 @@ def _check_float(name, x):
 
 
 def _check_vertex(vertex_pred, vertex_targets, vertex_weights):
+    """vertex_weights None passes: the callers that allow it take the weights from the mask."""
     for name, x in (("vertex_pred", vertex_pred), ("vertex_targets", vertex_targets),
                     ("vertex_weights", vertex_weights)):
-        _check_float(name, x)
+        if x is not None or name != "vertex_weights":
+            _check_float(name, x)
     if vertex_pred.dim() != 4 or vertex_targets.shape != vertex_pred.shape:
         raise ValueError(f"vertex_pred {tuple(vertex_pred.shape)} and vertex_targets {tuple(vertex_targets.shape)} "
                          "must both be [b,ver_dim,h,w]")
+    _check_weights(vertex_pred, vertex_weights)
+
+
+def _check_weights(vertex_pred, vertex_weights):
+    """vertex_weights float32 [b,1,h,w] for vertex_pred [b,vd,h,w], or None (the weights are the mask's values)."""
+    if vertex_weights is None:
+        return
+    _check_float("vertex_weights", vertex_weights)
     b, _, h, w = vertex_pred.shape
     if tuple(vertex_weights.shape) != (b, 1, h, w):
         raise ValueError(f"vertex_weights must be [b,1,h,w] = {(b, 1, h, w)}, got {tuple(vertex_weights.shape)}")
+
+
+def mask_weights(mask):
+    """The vertex weights the loader derives from the mask: vertex_weights = mask.unsqueeze(0).float() per image
+    (linemod_dataset.py:227), i.e. mask.unsqueeze(1).float() for a batch.  What the loss functions use when they are
+    given vertex_weights=None (the kernels convert each mask value where they would read the weight)."""
+    return mask.unsqueeze(1).float()
 
 
 def _check_keypoints(mask, hcoords):
@@ -94,13 +113,11 @@ def _check_field_losses(seg_pred, vertex_pred, mask, vertex, vertex_weights):
 
 def _check_keypoint_losses(seg_pred, vertex_pred, mask, hcoords, vertex_weights):
     _check_seg(seg_pred, mask)
-    for name, x in (("vertex_pred", vertex_pred), ("vertex_weights", vertex_weights)):
-        _check_float(name, x)
+    _check_float("vertex_pred", vertex_pred)
     if vertex_pred.dim() != 4:
         raise ValueError(f"vertex_pred must be [b,ver_dim,h,w], got {tuple(vertex_pred.shape)}")
     b, vd, h, w = vertex_pred.shape
-    if tuple(vertex_weights.shape) != (b, 1, h, w):
-        raise ValueError(f"vertex_weights must be [b,1,h,w] = {(b, 1, h, w)}, got {tuple(vertex_weights.shape)}")
+    _check_weights(vertex_pred, vertex_weights)
     if seg_pred.shape[0] != b or seg_pred.shape[2:] != vertex_pred.shape[2:]:
         raise ValueError(f"seg_pred {tuple(seg_pred.shape)} and vertex_pred {tuple(vertex_pred.shape)} differ in b,h,w")
     _check_keypoints(mask, hcoords)
@@ -153,8 +170,11 @@ def _input_args(seg, mask, pred, tgt, wgt, hcoords, use_motion):
         else:
             hcoords = hcoords.detach().contiguous()
             args += [hcoords.data_ptr(), int(hcoords.dtype == torch.float64), int(bool(use_motion))]
-        wgt, s_wgt = _strides(wgt, 4)
-        args += [wgt.data_ptr(), s_wgt]
+        if wgt is None:                         # both NULL: the kernels take the weights from the mask
+            args += [None, None]
+        else:
+            wgt, s_wgt = _strides(wgt, 4)
+            args += [wgt.data_ptr(), s_wgt]
     else:
         args += [None] * (6 if hcoords is None else 7)
     return args, (seg, mask, pred, tgt, wgt, hcoords), (b, h, w, C, vd), dev
@@ -321,7 +341,9 @@ def smooth_l1_loss(vertex_pred, vertex_targets, vertex_weights, sigma=1.0, norma
     """net_utils.py:54-80.  vertex_pred, vertex_targets [b,ver_dim,h,w], vertex_weights [b,1,h,w], float32.
     normalize: per-image sum(in) / (ver_dim * sum(w) + 1e-3) -> [b]; otherwise the elementwise loss [b,ver_dim,h,w],
     bit-identical to torch's fp32 ops.  `reduce` is accepted and, as in the reference (whose mean is discarded),
-    leaves the result per image."""
+    leaves the result per image.  There is no mask to take the weights from, so vertex_weights is required."""
+    if vertex_weights is None:
+        raise ValueError("smooth_l1_loss needs vertex_weights (it has no mask to take them from)")
     _check_vertex(vertex_pred, vertex_targets, vertex_weights)
     if _use_torch(vertex_pred, vertex_targets, vertex_weights):
         return _smooth_l1_torch(vertex_pred, vertex_targets, vertex_weights, sigma, normalize)
@@ -343,15 +365,17 @@ def compute_precision_recall(scores, target, reduce=False):
     return precision, recall
 
 
-def seg_vertex_losses(seg_pred, vertex_pred, mask, vertex, vertex_weights):
+def seg_vertex_losses(seg_pred, vertex_pred, mask, vertex, vertex_weights=None):
     """The four per-image figures of NetWrapper.forward (train_linemod.py:87-90) in one pass:
     loss_seg (cross-entropy, mean over pixels), loss_vertex (smooth_l1_loss, normalize=True), precision, recall;
-    each float32 [b]."""
+    each float32 [b].  vertex_weights=None: the weights are the mask's values, mask_weights(mask) (the loader's
+    vertex_weights), converted in the kernel where it would read them: the outputs equal the call with that tensor."""
     _check_field_losses(seg_pred, vertex_pred, mask, vertex, vertex_weights)
     if _use_torch(seg_pred, vertex_pred, vertex, vertex_weights):
+        weights = mask_weights(mask) if vertex_weights is None else vertex_weights
         precision, recall = _precision_recall_torch(seg_pred, mask)
         return (_cross_entropy_torch(seg_pred, mask),
-                _smooth_l1_torch(vertex_pred, vertex, vertex_weights, 1.0, True), precision, recall)
+                _smooth_l1_torch(vertex_pred, vertex, weights, 1.0, True), precision, recall)
     r = _native_losses(seg_pred, mask, vertex_pred, vertex, vertex_weights)
     return r["seg"], r["ver"], r["precision"], r["recall"]
 
@@ -382,37 +406,41 @@ def vertex_targets(mask, hcoords, use_motion=False):
     return out
 
 
-def seg_vertex_losses_from_keypoints(seg_pred, vertex_pred, mask, hcoords, vertex_weights, use_motion=False):
+def seg_vertex_losses_from_keypoints(seg_pred, vertex_pred, mask, hcoords, vertex_weights=None, use_motion=False):
     """seg_vertex_losses with the vertex targets built from the keypoints instead of read from a [b,2K,h,w] tensor:
     the same four float32 [b] figures, bit-identical to seg_vertex_losses(seg_pred, vertex_pred, mask,
     vertex_targets(mask, hcoords, use_motion), vertex_weights), in one launch pair that never materialises the field.
-    hcoords [b,K,3] float32 or float64, with ver_dim == 2K.  In grad mode the field is materialised with
-    vertex_targets and the torch expressions evaluated on it."""
+    hcoords [b,K,3] float32 or float64, with ver_dim == 2K.  vertex_weights=None takes the weights from the mask, as
+    seg_vertex_losses does.  In grad mode the field is materialised with vertex_targets and the torch expressions
+    evaluated on it."""
     _check_keypoint_losses(seg_pred, vertex_pred, mask, hcoords, vertex_weights)
     if _use_torch(seg_pred, vertex_pred, vertex_weights):
         vertex = vertex_targets(mask, hcoords, use_motion)
+        weights = mask_weights(mask) if vertex_weights is None else vertex_weights
         precision, recall = _precision_recall_torch(seg_pred, mask)
         return (_cross_entropy_torch(seg_pred, mask),
-                _smooth_l1_torch(vertex_pred, vertex, vertex_weights, 1.0, True), precision, recall)
+                _smooth_l1_torch(vertex_pred, vertex, weights, 1.0, True), precision, recall)
     r = _native_losses(seg_pred, mask, vertex_pred, None, vertex_weights, hcoords=hcoords, use_motion=use_motion)
     return r["seg"], r["ver"], r["precision"], r["recall"]
 
 
-def seg_vertex_training_losses(seg_pred, vertex_pred, mask, vertex, vertex_weights):
+def seg_vertex_training_losses(seg_pred, vertex_pred, mask, vertex, vertex_weights=None):
     """seg_vertex_losses for training: the same four float32 [b] figures from the same kernel (bit-identical to
     seg_vertex_losses without grad), with loss_seg and loss_vertex differentiable with respect to seg_pred and
     vertex_pred through the device backward (pvnet_seg_vertex_losses_backward, DESIGN.md §13); precision and recall
     are not differentiable.  When seg_pred and vertex_pred are the channel slices [0,C) and [C,C+vd) of one output
     tensor (Resnet18_8s.forward), the gradient is written once into a tensor of that output's shape.  CUDA tensors
-    only; vertex and vertex_weights must not require grad (ValueError)."""
+    only; vertex and vertex_weights must not require grad (ValueError).  vertex_weights=None takes the weights from
+    the mask in the forward and the backward (seg_vertex_losses): the loader need not send them."""
     _check_field_losses(seg_pred, vertex_pred, mask, vertex, vertex_weights)
     return _training_losses(seg_pred, vertex_pred, mask, vertex, vertex_weights, None, False)
 
 
-def seg_vertex_training_losses_from_keypoints(seg_pred, vertex_pred, mask, hcoords, vertex_weights, use_motion=False):
+def seg_vertex_training_losses_from_keypoints(seg_pred, vertex_pred, mask, hcoords, vertex_weights=None,
+                                              use_motion=False):
     """seg_vertex_training_losses with the vertex targets computed from the keypoints as
     seg_vertex_losses_from_keypoints does, in the forward and in the backward: the [b,2K,h,w] field is never
-    stored.  hcoords must not require grad (ValueError)."""
+    stored.  hcoords must not require grad (ValueError).  vertex_weights=None takes the weights from the mask."""
     _check_keypoint_losses(seg_pred, vertex_pred, mask, hcoords, vertex_weights)
     return _training_losses(seg_pred, vertex_pred, mask, None, vertex_weights, hcoords, use_motion)
 
