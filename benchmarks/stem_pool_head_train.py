@@ -2,7 +2,9 @@
 
 Part one, per piece at batch 16 and 32, 480 x 640, on the same operands (channels_last for torch, as the torch graph
 runs them): the native forward and backward against
-  stem     cuDNN conv1 forward (F.conv2d, TF32) and its weight gradient (aten.convolution_backward, weight only);
+  stem     cuDNN conv1 forward (F.conv2d, TF32) plus the copy of the image and its 5 zero channels into convraw.0's
+           input, which the native stem writes in the same pass, and its weight gradient (aten.convolution_backward,
+           weight only);
   max-pool F.max_pool2d (3, 2, 1) and its autograd backward;
   head     convraw.3 as F.conv2d(y, w, b).contiguous() and its autograd backward (input, weight and bias gradients).
 CUDA events, WARM warm-up calls, REPS timed calls with the native and torch forms alternated, the median.  Shares
@@ -44,7 +46,11 @@ HBM, TF32 = 3.35e12, 495e12
 CL = torch.channels_last
 
 
-def torch_stem(x, w):
+def torch_stem(x, w, img, co, mean=None, std=None):
+    """pc.stem_train of a float image in torch: cuDNN's conv1, and the image and 5 zero channels written into
+    channels [co, co+8) of convraw.0's input img."""
+    img[:, co:co + 3].copy_(x)
+    img[:, co + 3:co + 8].zero_()
     return F.conv2d(x.contiguous(memory_format=CL), w, stride=2, padding=3)
 
 
@@ -64,15 +70,16 @@ def piece_rows(b, dev):
     xc = x.contiguous(memory_format=CL)
     w = (0.1 * torch.randn(64, 3, 7, 7, device=dev, generator=g)).requires_grad_()
     dy = torch.randn(b, 64, H // 2, W // 2, device=dev, generator=g).contiguous(memory_format=CL)
-    st = {"y": pc.stem_train(x, w)}
+    img = torch.empty(b, 8, H, W, device=dev, memory_format=CL)
+    st = {"y": pc.stem_train(x, w, img, 0)}
 
     def stem_fwd():
         with torch.no_grad():
-            pc.stem_train(x, w)
+            pc.stem_train(x, w, img, 0)
 
     def cudnn_fwd():
         with torch.no_grad():
-            F.conv2d(xc, w, stride=2, padding=3)
+            torch_stem(xc, w, img, 0)
 
     def stem_wgrad():
         torch.autograd.grad(st["y"], w, dy, retain_graph=True)
@@ -92,7 +99,7 @@ def piece_rows(b, dev):
         row[f"native_{part}_TFLOPs"] = flops / (row[f"native_{part}_ms"] * 1e-3) / 1e12
         row[f"native_{part}_fraction_of_tf32_peak"] = row[f"native_{part}_TFLOPs"] * 1e12 / TF32
     rows.append(row)
-    del st, x, xc, dy
+    del st, x, xc, dy, img
     torch.cuda.empty_cache()
 
     # max-pool

@@ -548,18 +548,19 @@ PVNET_API int pvnet_batchnorm_act_backward(int form, int act, const float *dy, c
  * model_repository.py:57), forward and backward.  Each launches on `stream` and allocates nothing; bad arguments
  * return PVNET_E_INVALID with a message.
  *
- * pvnet_stem_s2d_nhwc: conv1 (3 -> 64, 7x7, stride 2, pad 3) of image_nchw f32 [b,3,H,W] (H, W even; 8-byte
- *   aligned) as the eval path computes it: s2d [b,H/2,W/2,16] is written with the 2x2 space-to-depth image
- *   (channel (py*2+px)*3+c, 4 zero channels, rounded to TF32) and out NHWC [b,H/2,W/2,64] = the 4x4 stride-1 tensor-core
- *   convolution of s2d with w_s2d (packed [64][4][4][16] as backbone slot 26, TF32) plus bias [64], fp32, no
- *   activation.  s2d is what pvnet_stem_s2d_wgrad reads.
- * pvnet_stem_s2d_u8_nhwc: pvnet_stem_s2d_nhwc of the raw image image_u8 uint8 [b,H,W,3] contiguous (H, W even;
- *   2-byte aligned), normalised on the device as torchvision's ToTensor + Normalize on the CPU compute it:
- *   v = (float(u) / 255 - mean3[c]) / std3[c], three correctly rounded fp32 ops (mean3 / std3: 3 host floats each,
- *   finite, std nonzero).  s2d and out are the float form's for the image v.  In the same pass the caller's
- *   channels_last buffer img NHWC [b,H,W,img_cs] gets v unrounded in channels [img_co, img_co+3) and zeros in
- *   [img_co+3, img_co+8) (img_co, img_cs multiples of 4, img_co+8 <= img_cs): convraw.0's image and pad channels;
- *   its other channels are not touched.
+ * pvnet_stem_s2d_nhwc: conv1 (3 -> 64, 7x7, stride 2, pad 3) of a training batch as the eval path computes it, the
+ *   image in either form pvnet_backbone_forward / pvnet_backbone_forward_u8 take:
+ *   - image_is_u8 = 0: image f32 NCHW [b,3,H,W] (8-byte aligned); mean3 and std3 must be NULL.
+ *   - image_is_u8 = 1: image uint8 [b,H,W,3] contiguous (2-byte aligned), normalised on the device as torchvision's
+ *     ToTensor + Normalize on the CPU compute it: v = (float(u) / 255 - mean3[c]) / std3[c], three correctly rounded
+ *     fp32 ops (mean3 / std3: 3 host floats each, finite, std nonzero).  Every output below is the float form's for
+ *     the image v.
+ *   H, W even.  s2d [b,H/2,W/2,16] is written with the 2x2 space-to-depth image (channel (py*2+px)*3+c, 4 zero
+ *   channels, rounded to TF32) and out NHWC [b,H/2,W/2,64] = the 4x4 stride-1 tensor-core convolution of s2d with
+ *   w_s2d (packed [64][4][4][16] as backbone slot 26, TF32) plus bias [64], fp32, no activation.  s2d is what
+ *   pvnet_stem_s2d_wgrad reads.  In the same pass the caller's channels_last buffer img NHWC [b,H,W,img_cs] gets the
+ *   fp32 image unrounded in channels [img_co, img_co+3) and zeros in [img_co+3, img_co+8) (img_co, img_cs multiples
+ *   of 4, img_co+8 <= img_cs): convraw.0's image and pad channels; its other channels are not touched.
  * pvnet_stem_s2d_wgrad: dw [64][3][7][7] (torch's layout, overwritten) = the weight gradient of that convolution for
  *   dout NHWC [b,H/2,W/2,64] dense: the 4x4 weight gradient on s2d (TF32 operands, dout truncated by the tensor
  *   cores, fp32 accumulation, pixel splits added in a fixed order: identical run to run), folded back onto the
@@ -577,11 +578,9 @@ PVNET_API int pvnet_batchnorm_act_backward(int form, int act, const float *dy, c
  *   over a fixed partition of the pixels, merged in a fixed order and rounded once to fp32.  Any of dy, dw, db may
  *   be NULL (not computed); the workspace is needed only for dw / db.
  * All offsets are 64-bit; pointers 16-byte aligned unless stated. */
-PVNET_API int pvnet_stem_s2d_nhwc(const float *image_nchw, const float *w_s2d, const float *bias, float *s2d,
-                                  float *out, int b, int H, int W, pvnet_stream_t stream);
-PVNET_API int pvnet_stem_s2d_u8_nhwc(const uint8_t *image_u8, const float *mean3, const float *std3,
-                                     const float *w_s2d, const float *bias, float *s2d, float *out, float *img,
-                                     int img_cs, int img_co, int b, int H, int W, pvnet_stream_t stream);
+PVNET_API int pvnet_stem_s2d_nhwc(const void *image, int image_is_u8, const float *mean3, const float *std3,
+                                  const float *w_s2d, const float *bias, float *s2d, float *out, float *img, int img_cs,
+                                  int img_co, int b, int H, int W, pvnet_stream_t stream);
 PVNET_API int pvnet_stem_s2d_wgrad_workspace_bytes(int b, int H, int W, size_t *bytes);
 PVNET_API int pvnet_stem_s2d_wgrad(const float *s2d, const float *dout, float *dw, int b, int H, int W,
                                    void *workspace, size_t workspace_bytes, pvnet_stream_t stream);

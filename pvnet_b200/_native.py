@@ -116,9 +116,9 @@ SIGNATURES = {
     "pvnet_batchnorm_act_backward": (c_int, [c_int, c_int, c_void_p, c_void_p, c_void_p, ctypes.c_longlong, c_int,
                                              c_bn_p, c_bn_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                              c_void_p, c_size_t, c_void_p]),
-    "pvnet_stem_s2d_nhwc": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
-    "pvnet_stem_s2d_u8_nhwc": (c_int, [c_void_p, ctypes.POINTER(c_float), ctypes.POINTER(c_float), c_void_p, c_void_p,
-                                       c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "pvnet_stem_s2d_nhwc": (c_int, [c_void_p, c_int, ctypes.POINTER(c_float), ctypes.POINTER(c_float), c_void_p,
+                                    c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
+                                    c_void_p]),
     "pvnet_stem_s2d_wgrad_workspace_bytes": (c_int, [c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
     "pvnet_stem_s2d_wgrad": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_size_t, c_void_p]),
     "pvnet_maxpool3x3s2_nhwc": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),

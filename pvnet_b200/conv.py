@@ -92,6 +92,18 @@ def _p(t):
     return None if t is None else ctypes.c_void_p(t.data_ptr())
 
 
+def _stream(dev):
+    return ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+
+
+def _workspace(dev, query_fn_name, *args):
+    """A uint8 workspace on `dev` (from the caching allocator, at least 16 bytes) of the size the C ABI's
+    `query_fn_name(*args, size_t *bytes)` reports."""
+    n = ctypes.c_size_t()
+    _native.check(getattr(_native.lib(), query_fn_name)(*args, ctypes.byref(n)), query_fn_name)
+    return torch.empty(max(n.value, 16), dtype=torch.uint8, device=dev)
+
+
 def conv2d_nhwc(inp, in_co, cin, w_packed, bias, out, out_co, cout, ksize, stride=1, dilation=1, act=ACT_NONE,
                 res=None, res_co=0, round_out=False):
     """inp [b,H,W,in_cs] / out [b,Ho,Wo,out_cs] / res [b,Ho,Wo,res_cs]: contiguous NHWC fp32
@@ -101,7 +113,7 @@ def conv2d_nhwc(inp, in_co, cin, w_packed, bias, out, out_co, cout, ksize, strid
         _native.check(_native.lib().pvnet_conv2d_nhwc(
             _p(inp), in_cs, in_co, cin, _p(w_packed), _p(bias), _p(res), 0 if res is None else res.shape[3], res_co,
             _p(out), out.shape[3], out_co, cout, b, H, W, ksize, stride, dilation, act, int(round_out),
-            ctypes.c_void_p(torch.cuda.current_stream(inp.device).cuda_stream)), "pvnet_conv2d_nhwc")
+            _stream(inp.device)), "pvnet_conv2d_nhwc")
     return out
 
 
@@ -119,17 +131,13 @@ def conv2d_nhwc_wgrad(inp, in_co, cin, dout, dout_co, cout, ksize, dilation=1):
     """pvnet_conv2d_nhwc_wgrad: inp [b,H,W,in_cs] and dout [b,H,W,dout_cs] contiguous NHWC fp32 on one device
     -> dW [cout,cin,ksize,ksize] fp32 (workspace from the caching allocator, current stream)."""
     b, H, W, in_cs = inp.shape
-    L = _native.lib()
     dev = inp.device
     with torch.cuda.device(dev):
-        n = ctypes.c_size_t()
-        _native.check(L.pvnet_conv2d_nhwc_wgrad_workspace_bytes(cin, cout, b, H, W, ksize, ctypes.byref(n)),
-                      "pvnet_conv2d_nhwc_wgrad_workspace_bytes")
-        ws = torch.empty(max(n.value, 16), dtype=torch.uint8, device=dev)
+        ws = _workspace(dev, "pvnet_conv2d_nhwc_wgrad_workspace_bytes", cin, cout, b, H, W, ksize)
         dw = torch.empty(cout, cin, ksize, ksize, dtype=torch.float32, device=dev)
-        _native.check(L.pvnet_conv2d_nhwc_wgrad(
+        _native.check(_native.lib().pvnet_conv2d_nhwc_wgrad(
             _p(inp), in_cs, in_co, cin, _p(dout), dout.shape[3], dout_co, cout, _p(dw), b, H, W, ksize, dilation,
-            _p(ws), ws.numel(), ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "pvnet_conv2d_nhwc_wgrad")
+            _p(ws), ws.numel(), _stream(dev)), "pvnet_conv2d_nhwc_wgrad")
     return dw
 
 
@@ -140,8 +148,8 @@ def zero_insert2x(inp, out=None):
         out = torch.empty(b, 2 * h, 2 * w, C, dtype=torch.float32, device=inp.device)
     with torch.cuda.device(inp.device):
         _native.check(_native.lib().pvnet_zero_insert2x_nhwc(
-            _p(inp), C, 0, C, _p(out), out.shape[3], 0, b, 2 * h, 2 * w,
-            ctypes.c_void_p(torch.cuda.current_stream(inp.device).cuda_stream)), "pvnet_zero_insert2x_nhwc")
+            _p(inp), C, 0, C, _p(out), out.shape[3], 0, b, 2 * h, 2 * w, _stream(inp.device)),
+            "pvnet_zero_insert2x_nhwc")
     return out
 
 
@@ -213,32 +221,46 @@ class Upsample2xCatNHWC(torch.autograd.Function):
     CUDA forward), and the `rest` tensors are copied behind them.  Backward: `low` gets pvnet_upsample2x_backward_nhwc
     of the gradient's first C channels, read in place (the terms of torch's backward in a fixed order, without
     atomics, so identical run to run); each rest[i] gets its channel slice of the gradient, as cat's backward gives
-    it.  Runs on the input's device and its current stream."""
+    it.  Runs on the input's device and its current stream.
+
+    With `buf` given (and no `rest`) the concatenated buffer is the caller's: a channels_last [b,Cb,2h,2w] float32
+    tensor that needs no gradient, whose channels behind the first C the caller has filled (forward_train: the stem
+    writes convraw.0's image and pad channels).  The upsampled channels are written into it in place, and it is
+    returned, marked dirty; its other channels are not copied in either direction."""
 
     @staticmethod
-    def forward(ctx, low, *rest):
+    def forward(ctx, low, buf, *rest):
         b, C, h, w = low.shape
-        if not low.is_cuda or low.dtype != torch.float32 or any(r.dtype != torch.float32 for r in rest):
-            raise ValueError("Upsample2xCatNHWC needs float32 CUDA tensors")
-        if any(r.shape[0] != b or r.shape[2:] != (2 * h, 2 * w) for r in rest):
-            raise ValueError(f"every concatenated tensor must be [{b}, C, {2 * h}, {2 * w}]")
         widths = [C] + [r.shape[1] for r in rest]
-        if C % 4 or sum(widths) % 4:
-            raise ValueError(f"C and the concatenated width must be multiples of 4, got {widths}")
+        if buf is None:
+            if not low.is_cuda or low.dtype != torch.float32 or any(r.dtype != torch.float32 for r in rest):
+                raise ValueError("Upsample2xCatNHWC needs float32 CUDA tensors")
+            if any(r.shape[0] != b or r.shape[2:] != (2 * h, 2 * w) for r in rest):
+                raise ValueError(f"every concatenated tensor must be [{b}, C, {2 * h}, {2 * w}]")
+            if C % 4 or sum(widths) % 4:
+                raise ValueError(f"C and the concatenated width must be multiples of 4, got {widths}")
+            buf = torch.empty(b, sum(widths), 2 * h, 2 * w, dtype=torch.float32, device=low.device,
+                              memory_format=torch.channels_last)
+        else:
+            _check_float_cuda("Upsample2xCatNHWC", low, buf)
+            if buf.dim() != 4 or buf.shape[0] != b or tuple(buf.shape[2:]) != (2 * h, 2 * w) or buf.shape[1] < C or \
+                    not buf.is_contiguous(memory_format=torch.channels_last):
+                raise ValueError(f"buf must be a channels_last [{b}, >= {C}, {2 * h}, {2 * w}] tensor, got "
+                                 f"{tuple(buf.shape)}")
+            if buf.requires_grad:
+                raise ValueError("Upsample2xCatNHWC: buf gets no gradient, so it must not require one")
+            ctx.mark_dirty(buf)
         dev = low.device
-        out = torch.empty(b, sum(widths), 2 * h, 2 * w, dtype=torch.float32, device=dev,
-                          memory_format=torch.channels_last)
         lh = _nhwc(low)
         with torch.cuda.device(dev):
             _native.check(_native.lib().pvnet_upsample2x_nhwc(
-                _p(lh), C, _p(out), out.shape[1], 0, b, h, w,
-                ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "pvnet_upsample2x_nhwc")
+                _p(lh), C, _p(buf), buf.shape[1], 0, b, h, w, _stream(dev)), "pvnet_upsample2x_nhwc")
         co = C
         for r in rest:
-            out[:, co:co + r.shape[1]].copy_(r)
+            buf[:, co:co + r.shape[1]].copy_(r)
             co += r.shape[1]
         ctx.widths = widths
-        return out
+        return buf
 
     @staticmethod
     @once_differentiable
@@ -246,18 +268,17 @@ class Upsample2xCatNHWC(torch.autograd.Function):
         widths = ctx.widths
         b, _, H, W = gy.shape
         C, h, w = widths[0], H // 2, W // 2
-        grads = [None] * len(widths)
+        grads = [None] * (len(widths) + 1)          # low, buf, *rest
         if ctx.needs_input_grad[0]:
             gyh = _nhwc(gy.float())
             dev = gyh.device
             dlow = torch.empty(b, C, h, w, dtype=torch.float32, device=dev, memory_format=torch.channels_last)
             with torch.cuda.device(dev):
                 _native.check(_native.lib().pvnet_upsample2x_backward_nhwc(
-                    _p(gyh), gyh.shape[3], 0, C, _p(dlow), b, h, w,
-                    ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "pvnet_upsample2x_backward_nhwc")
+                    _p(gyh), gyh.shape[3], 0, C, _p(dlow), b, h, w, _stream(dev)), "pvnet_upsample2x_backward_nhwc")
             grads[0] = dlow
         co = C
-        for k, c in enumerate(widths[1:], 1):
+        for k, c in enumerate(widths[1:], 2):
             if ctx.needs_input_grad[k]:
                 grads[k] = gy[:, co:co + c]
             co += c
@@ -267,55 +288,13 @@ class Upsample2xCatNHWC(torch.autograd.Function):
 def upsample2x_cat(low, *rest):
     """Upsample2xCatNHWC.apply: cat([F.interpolate(low, x2, bilinear, align_corners=True), *rest], 1) on the native
     kernels under autograd (see Upsample2xCatNHWC)."""
-    return Upsample2xCatNHWC.apply(low, *rest)
-
-
-class Upsample2xIntoNHWC(torch.autograd.Function):
-    """Upsample2xCatNHWC with the concatenated buffer given: F.interpolate(low, scale_factor=2, mode="bilinear",
-    align_corners=True) of a [b,C,h,w] `low` written in place into channels [0, C) of `buf`, a channels_last
-    [b,Cb,2h,2w] float32 tensor that needs no gradient, whose other channels the caller has filled (the uint8
-    training path: the stem's pack writes convraw.0's image and pad channels).  Returns `buf` (marked dirty).
-    Forward pvnet_upsample2x_nhwc, backward pvnet_upsample2x_backward_nhwc of the gradient's first C channels, as
-    Upsample2xCatNHWC; no copy of the other channels is made in either direction."""
-
-    @staticmethod
-    def forward(ctx, low, buf):
-        _check_float_cuda("Upsample2xIntoNHWC", low, buf)
-        b, C, h, w = low.shape
-        if buf.dim() != 4 or buf.shape[0] != b or tuple(buf.shape[2:]) != (2 * h, 2 * w) or buf.shape[1] < C or \
-                not buf.is_contiguous(memory_format=torch.channels_last):
-            raise ValueError(f"buf must be a channels_last [{b}, >= {C}, {2 * h}, {2 * w}] tensor, got "
-                             f"{tuple(buf.shape)}")
-        if buf.requires_grad:
-            raise ValueError("Upsample2xIntoNHWC: buf gets no gradient, so it must not require one")
-        dev = low.device
-        lh = _nhwc(low)
-        with torch.cuda.device(dev):
-            _native.check(_native.lib().pvnet_upsample2x_nhwc(_p(lh), C, _p(buf), buf.shape[1], 0, b, h, w,
-                                                              _stream(dev)), "pvnet_upsample2x_nhwc")
-        ctx.mark_dirty(buf)
-        ctx.C = C
-        return buf
-
-    @staticmethod
-    @once_differentiable
-    def backward(ctx, gy):
-        if not ctx.needs_input_grad[0]:
-            return None, None
-        b, _, H, W = gy.shape
-        C, h, w = ctx.C, H // 2, W // 2
-        gyh = _nhwc(gy.float())
-        dev = gyh.device
-        dlow = torch.empty(b, C, h, w, dtype=torch.float32, device=dev, memory_format=torch.channels_last)
-        with torch.cuda.device(dev):
-            _native.check(_native.lib().pvnet_upsample2x_backward_nhwc(_p(gyh), gyh.shape[3], 0, C, _p(dlow), b, h, w,
-                                                                       _stream(dev)), "pvnet_upsample2x_backward_nhwc")
-        return dlow, None
+    return Upsample2xCatNHWC.apply(low, None, *rest)
 
 
 def upsample2x_into(low, buf):
-    """Upsample2xIntoNHWC.apply: the upsampled `low` written into the first channels of `buf` under autograd."""
-    return Upsample2xIntoNHWC.apply(low, buf)
+    """Upsample2xCatNHWC.apply with the caller's buffer: the upsampled `low` written into the first channels of `buf`
+    under autograd, `buf` returned."""
+    return Upsample2xCatNHWC.apply(low, buf)
 
 
 # ----------------------------------------------------------------------------- train-mode BatchNorm (autograd)
@@ -383,26 +362,19 @@ def _bn_operand(t, C, shape=None):
     return _nhwc(t)
 
 
-def _bn_workspace(form, C, npix, dev):
-    n = ctypes.c_size_t()
-    _native.check(_native.lib().pvnet_batchnorm_workspace_bytes(form, C, npix, ctypes.byref(n)),
-                  "pvnet_batchnorm_workspace_bytes")
-    return torch.empty(max(n.value, 16), dtype=torch.uint8, device=dev)
-
-
 def batchnorm_forward(form, act, xh, zh, st, weight, bias, st_z=None, weight_z=None, bias_z=None):
     """pvnet_batchnorm_act_forward on NHWC views xh (and zh) -> y [b,C,H,W] channels_last; st / st_z are the
     BatchNormStates (their running statistics are updated in place, their saved/coef written)."""
     b, H, W, C = xh.shape
     dev = xh.device
     with torch.cuda.device(dev):
-        ws = _bn_workspace(form, C, b * H * W, dev)
+        ws = _workspace(dev, "pvnet_batchnorm_workspace_bytes", form, C, b * H * W)
         y = torch.empty(b, C, H, W, dtype=torch.float32, device=dev, memory_format=torch.channels_last)
         p = st.params(weight, bias)
         pz = None if st_z is None else ctypes.byref(st_z.params(weight_z, bias_z))
         _native.check(_native.lib().pvnet_batchnorm_act_forward(
-            form, act, _p(xh), _p(zh), b * H * W, C, ctypes.byref(p), pz, _p(y), _p(ws), ws.numel(),
-            ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "pvnet_batchnorm_act_forward")
+            form, act, _p(xh), _p(zh), b * H * W, C, ctypes.byref(p), pz, _p(y), _p(ws), ws.numel(), _stream(dev)),
+            "pvnet_batchnorm_act_forward")
     return y
 
 
@@ -415,7 +387,7 @@ def batchnorm_backward(form, act, gyh, xh, zh, st, weight, st_z=None, weight_z=N
     new = lambda: torch.empty(b, C, H, W, dtype=torch.float32, device=dev, memory_format=torch.channels_last)  # noqa
     vec = lambda w, want: None if w is None or not want else torch.empty(C, dtype=torch.float32, device=dev)  # noqa
     with torch.cuda.device(dev):
-        ws = _bn_workspace(form, C, b * H * W, dev)
+        ws = _workspace(dev, "pvnet_batchnorm_workspace_bytes", form, C, b * H * W)
         dx = new()
         dz = None if form == FORM_ACT else new()
         dw, db = vec(weight, param_grads[0]), vec(weight, param_grads[1])
@@ -426,8 +398,7 @@ def batchnorm_backward(form, act, gyh, xh, zh, st, weight, st_z=None, weight_z=N
         pz = None if st_z is None else ctypes.byref(st_z.params(weight_z))
         _native.check(_native.lib().pvnet_batchnorm_act_backward(
             form, act, _p(gyh), _p(xh), _p(zh), b * H * W, C, ctypes.byref(p), pz, _p(dx), _p(dz), _p(dw), _p(db),
-            _p(dwz), _p(dbz), _p(ws), ws.numel(), ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
-            "pvnet_batchnorm_act_backward")
+            _p(dwz), _p(dbz), _p(ws), ws.numel(), _stream(dev)), "pvnet_batchnorm_act_backward")
     return dx, dz, dw, db, dwz, dbz
 
 
@@ -522,10 +493,6 @@ def bn_add_relu(bn, a, skip, bn_skip=None):
 
 
 # ----------------------------------------------------------------------------- stem, max-pool and head (autograd)
-def _stream(dev):
-    return ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-
-
 def stem_s2d_index(device=None) -> torch.Tensor:
     """[256] int64 on `device` (default CPU): for entry (ty, tx, ch) of pack_stem_s2d's [4][4][16] layout, the index
     into conv1's weight flattened per output channel as [3][7][7] (c*49 + kh*7 + kw, kh = 2ty+py-1, kw = 2tx+px-1,
@@ -570,71 +537,10 @@ def _check_float_cuda(what, *ts):
             raise ValueError(f"{what} needs float32 CUDA tensors")
 
 
-class StemS2dNHWC(torch.autograd.Function):
-    """conv1 of Resnet18_8s (weight [64,3,7,7], stride 2, padding 3, no bias) of a [b,3,H,W] float32 CUDA image (H, W
-    even) that needs no gradient.  Forward: pvnet_stem_s2d_nhwc, the eval path's tensor-core form -- the 2x2
-    space-to-depth image S, TF32-rounded, and the 4x4 stride-1 convolution with the weights packed by
-    pack_stem_s2d_train -- into a channels_last [b,64,H/2,W/2].  Backward: the weight gradient only
-    (pvnet_stem_s2d_wgrad: the 4x4 gradient on S, all 16 taps per CTA, folded back to [64,3,7,7]).  Saves S only.
-    Runs on the input's device and its current stream."""
-
-    @staticmethod
-    def forward(ctx, x, weight):
-        _check_float_cuda("StemS2dNHWC", x, weight)
-        if x.requires_grad:
-            raise ValueError("StemS2dNHWC: the image gets no gradient, so it must not require one")
-        if x.dim() != 4 or x.shape[1] != 3 or x.shape[2] % 2 or x.shape[3] % 2 or tuple(weight.shape) != (64, 3, 7, 7):
-            raise ValueError(f"StemS2dNHWC needs x [b,3,H,W] with H, W even and weight [64,3,7,7], got "
-                             f"{tuple(x.shape)} and {tuple(weight.shape)}")
-        b, _, H, W = x.shape
-        dev = x.device
-        xc = x.contiguous()
-        s2d = torch.empty(b, H // 2, W // 2, 16, dtype=torch.float32, device=dev)
-        out = torch.empty(b, 64, H // 2, W // 2, dtype=torch.float32, device=dev, memory_format=torch.channels_last)
-        w4 = pack_stem_s2d_train(weight.detach())
-        bias = torch.zeros(64, dtype=torch.float32, device=dev)
-        with torch.cuda.device(dev):
-            _native.check(_native.lib().pvnet_stem_s2d_nhwc(_p(xc), _p(w4), _p(bias), _p(s2d), _p(out), b, H, W,
-                                                            _stream(dev)), "pvnet_stem_s2d_nhwc")
-        ctx.save_for_backward(s2d)
-        ctx.hw = (H, W)
-        return out
-
-    @staticmethod
-    @once_differentiable
-    def backward(ctx, gy):
-        if not ctx.needs_input_grad[1]:
-            return None, None
-        return None, _stem_wgrad(ctx, gy)
-
-
-def _stem_wgrad(ctx, gy):
-    """pvnet_stem_s2d_wgrad of the S the forward saved: dW [64,3,7,7]."""
-    s2d, = ctx.saved_tensors
-    b = s2d.shape[0]
-    H, W = ctx.hw
-    dev = s2d.device
-    gyh = _nhwc(gy.float())
-    L = _native.lib()
-    with torch.cuda.device(dev):
-        n = ctypes.c_size_t()
-        _native.check(L.pvnet_stem_s2d_wgrad_workspace_bytes(b, H, W, ctypes.byref(n)),
-                      "pvnet_stem_s2d_wgrad_workspace_bytes")
-        ws = torch.empty(max(n.value, 16), dtype=torch.uint8, device=dev)
-        dw = torch.empty(64, 3, 7, 7, dtype=torch.float32, device=dev)
-        _native.check(L.pvnet_stem_s2d_wgrad(_p(s2d), _p(gyh), _p(dw), b, H, W, _p(ws), ws.numel(), _stream(dev)),
-                      "pvnet_stem_s2d_wgrad")
-    return dw
-
-
-def stem_train(x, weight):
-    """StemS2dNHWC.apply: conv1 (7x7/2, pad 3, no bias) on the native kernels under autograd."""
-    return StemS2dNHWC.apply(x, weight)
-
-
 def norm3(mean, std):
     """ToTensor + Normalize constants (sequences of numbers or CPU tensors; a CUDA tensor would cost a synchronising
-    read) as the two ctypes float[3] pvnet_stem_s2d_u8_nhwc takes; ValueError unless each has exactly three values."""
+    read) as the two ctypes float[3] pvnet_stem_s2d_nhwc takes for a uint8 image; ValueError unless each has exactly
+    three values."""
     vals = []
     for name, v in (("mean", mean), ("std", std)):
         v = [float(t) for t in (v.flatten().tolist() if isinstance(v, torch.Tensor) else v)]
@@ -644,29 +550,56 @@ def norm3(mean, std):
     return vals
 
 
-class StemS2dU8NHWC(torch.autograd.Function):
-    """StemS2dNHWC of a raw uint8 [b,H,W,3] image (contiguous, H, W even), normalised on the device as torchvision's
-    ToTensor + Normalize compute it on the CPU ((u/255 - mean)/std, three correctly rounded fp32 ops):
-    pvnet_stem_s2d_u8_nhwc.  In the same pass it writes the normalised image, unrounded, into channels [co, co+3) of
-    `img` (a [b,C,H,W] channels_last float32 buffer; the 5 channels behind it get zeros, the others are not touched):
-    convraw.0's concatenated input.  `img` gets no gradient and must not require one.  The output, S and the weight
-    gradient are StemS2dNHWC's for the normalised image."""
+class StemS2dNHWC(torch.autograd.Function):
+    """conv1 of Resnet18_8s (weight [64,3,7,7], stride 2, padding 3, no bias) of an image that needs no gradient, in
+    either of two forms (H, W even):
+    * a [b,3,H,W] float32 CUDA image, with mean and std None;
+    * a raw uint8 [b,H,W,3] CUDA image with the Normalize constants mean and std (3 values each), normalised on the
+      device as torchvision's ToTensor + Normalize compute it on the CPU ((u/255 - mean)/std, three correctly rounded
+      fp32 ops).  Every result is the float form's for the normalised image.
+    Forward: pvnet_stem_s2d_nhwc, the eval path's tensor-core form -- the 2x2 space-to-depth image S, TF32-rounded,
+    and the 4x4 stride-1 convolution with the weights packed by pack_stem_s2d_train -- into a channels_last
+    [b,64,H/2,W/2].  In the same pass it writes the fp32 image, unrounded, into channels [co, co+3) of `img` (a
+    [b,C,H,W] channels_last float32 buffer that gets no gradient; the 5 channels behind it get zeros, the others are
+    not touched): convraw.0's concatenated input.  With img None (a caller that wants conv1 alone) those channels go
+    to a scratch buffer.  Backward: the weight gradient only (pvnet_stem_s2d_wgrad: the 4x4
+    gradient on S, all 16 taps per CTA, folded back to [64,3,7,7]).  Saves S only.  Runs on the input's device and
+    its current stream."""
 
     @staticmethod
-    def forward(ctx, x, weight, mean, std, img, co):
-        _check_float_cuda("StemS2dU8NHWC", weight, img)
-        if not x.is_cuda or x.dtype != torch.uint8:
-            raise ValueError(f"StemS2dU8NHWC needs a uint8 CUDA image, got {x.dtype} on {x.device}")
-        if x.dim() != 4 or x.shape[3] != 3 or x.shape[1] % 2 or x.shape[2] % 2 or tuple(weight.shape) != (64, 3, 7, 7):
-            raise ValueError(f"StemS2dU8NHWC needs x [b,H,W,3] with H, W even and weight [64,3,7,7], got "
-                             f"{tuple(x.shape)} and {tuple(weight.shape)}")
-        b, H, W, _ = x.shape
+    def forward(ctx, x, weight, img, co, mean, std):
+        _check_float_cuda("StemS2dNHWC", weight, *([] if img is None else [img]))
+        is_u8 = x.dtype == torch.uint8
+        if is_u8:
+            if not x.is_cuda:
+                raise ValueError(f"StemS2dNHWC needs a uint8 CUDA image, got one on {x.device}")
+            if mean is None or std is None:
+                raise ValueError("StemS2dNHWC: a uint8 image needs mean and std (the Normalize constants)")
+            if x.dim() != 4 or x.shape[3] != 3 or x.shape[1] % 2 or x.shape[2] % 2:
+                raise ValueError(f"StemS2dNHWC needs a uint8 x [b,H,W,3] with H, W even, got {tuple(x.shape)}")
+            b, H, W, _ = x.shape
+            mean3, std3 = norm3(mean, std)
+        else:
+            _check_float_cuda("StemS2dNHWC", x)
+            if x.requires_grad:
+                raise ValueError("StemS2dNHWC: the image gets no gradient, so it must not require one")
+            if mean is not None or std is not None:
+                raise ValueError("StemS2dNHWC: mean and std apply to a uint8 image; a float image is already "
+                                 "normalised")
+            if x.dim() != 4 or x.shape[1] != 3 or x.shape[2] % 2 or x.shape[3] % 2:
+                raise ValueError(f"StemS2dNHWC needs a float x [b,3,H,W] with H, W even, got {tuple(x.shape)}")
+            b, _, H, W = x.shape
+            mean3 = std3 = None
+        if tuple(weight.shape) != (64, 3, 7, 7):
+            raise ValueError(f"StemS2dNHWC needs weight [64,3,7,7], got {tuple(weight.shape)}")
+        if img is None:
+            img, co = torch.empty(b, 8, H, W, dtype=torch.float32, device=x.device,
+                                  memory_format=torch.channels_last), 0
         if img.dim() != 4 or img.shape[0] != b or tuple(img.shape[2:]) != (H, W) or \
                 not img.is_contiguous(memory_format=torch.channels_last):
             raise ValueError(f"img must be a channels_last [{b},C,{H},{W}] buffer, got {tuple(img.shape)}")
         if img.requires_grad:
-            raise ValueError("StemS2dU8NHWC: img gets no gradient, so it must not require one")
-        mean3, std3 = norm3(mean, std)
+            raise ValueError("StemS2dNHWC: img gets no gradient, so it must not require one")
         dev = x.device
         xc = x.contiguous()
         s2d = torch.empty(b, H // 2, W // 2, 16, dtype=torch.float32, device=dev)
@@ -674,9 +607,9 @@ class StemS2dU8NHWC(torch.autograd.Function):
         w4 = pack_stem_s2d_train(weight.detach())
         bias = torch.zeros(64, dtype=torch.float32, device=dev)
         with torch.cuda.device(dev):
-            _native.check(_native.lib().pvnet_stem_s2d_u8_nhwc(
-                _p(xc), mean3, std3, _p(w4), _p(bias), _p(s2d), _p(out), _p(img), img.shape[1], co, b, H, W,
-                _stream(dev)), "pvnet_stem_s2d_u8_nhwc")
+            _native.check(_native.lib().pvnet_stem_s2d_nhwc(
+                _p(xc), int(is_u8), mean3, std3, _p(w4), _p(bias), _p(s2d), _p(out), _p(img), img.shape[1], co, b, H,
+                W, _stream(dev)), "pvnet_stem_s2d_nhwc")
         ctx.save_for_backward(s2d)
         ctx.hw = (H, W)
         return out
@@ -684,14 +617,26 @@ class StemS2dU8NHWC(torch.autograd.Function):
     @staticmethod
     @once_differentiable
     def backward(ctx, gy):
-        dw = _stem_wgrad(ctx, gy) if ctx.needs_input_grad[1] else None
+        if not ctx.needs_input_grad[1]:
+            return None, None, None, None, None, None
+        s2d, = ctx.saved_tensors
+        b = s2d.shape[0]
+        H, W = ctx.hw
+        dev = s2d.device
+        gyh = _nhwc(gy.float())
+        with torch.cuda.device(dev):
+            ws = _workspace(dev, "pvnet_stem_s2d_wgrad_workspace_bytes", b, H, W)
+            dw = torch.empty(64, 3, 7, 7, dtype=torch.float32, device=dev)
+            _native.check(_native.lib().pvnet_stem_s2d_wgrad(_p(s2d), _p(gyh), _p(dw), b, H, W, _p(ws), ws.numel(),
+                                                             _stream(dev)), "pvnet_stem_s2d_wgrad")
         return None, dw, None, None, None, None
 
 
-def stem_train_u8(x, weight, mean, std, img, co):
-    """StemS2dU8NHWC.apply: conv1 of a raw uint8 image, normalised on the device, which also fills convraw.0's image
-    channels of `img` (see StemS2dU8NHWC)."""
-    return StemS2dU8NHWC.apply(x, weight, mean, std, img, co)
+def stem_train(x, weight, img=None, co=0, mean=None, std=None):
+    """StemS2dNHWC.apply: conv1 (7x7/2, pad 3, no bias) on the native kernels under autograd, of a float image or of a
+    raw uint8 image normalised on the device; it also fills convraw.0's image and pad channels [co, co+8) of `img`
+    when one is given (see StemS2dNHWC)."""
+    return StemS2dNHWC.apply(x, weight, img, co, mean, std)
 
 
 class MaxPool3x3s2NHWC(torch.autograd.Function):
@@ -778,17 +723,12 @@ class Head1x1NCHW(torch.autograd.Function):
                          memory_format=torch.channels_last) if need_y else None
         dw = torch.empty(cout, cin, dtype=torch.float32, device=dev) if need_w else None
         db = torch.empty(cout, dtype=torch.float32, device=dev) if need_b else None
-        L = _native.lib()
         with torch.cuda.device(dev):
-            ws = None
-            if need_w or need_b:
-                n = ctypes.c_size_t()
-                _native.check(L.pvnet_head1x1_backward_workspace_bytes(b, H, W, cin, cout, ctypes.byref(n)),
-                              "pvnet_head1x1_backward_workspace_bytes")
-                ws = torch.empty(max(n.value, 16), dtype=torch.uint8, device=dev)
-            _native.check(L.pvnet_head1x1_backward(_p(g), _p(yh), _p(w2), _p(dy), _p(dw), _p(db), b, H, W, cin, cout,
-                                                   _p(ws), 0 if ws is None else ws.numel(), _stream(dev)),
-                          "pvnet_head1x1_backward")
+            ws = _workspace(dev, "pvnet_head1x1_backward_workspace_bytes", b, H, W, cin, cout) if need_w or need_b \
+                else None
+            _native.check(_native.lib().pvnet_head1x1_backward(
+                _p(g), _p(yh), _p(w2), _p(dy), _p(dw), _p(db), b, H, W, cin, cout, _p(ws),
+                0 if ws is None else ws.numel(), _stream(dev)), "pvnet_head1x1_backward")
         return dy, None if dw is None else dw.view(cout, cin, 1, 1), db
 
 

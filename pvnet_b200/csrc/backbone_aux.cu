@@ -124,18 +124,16 @@ int launch_pack_image(const float *in, float *out, int b, int H, int W, int out_
 // lib/datasets/linemod_dataset.py:191-195): (float(v) / 255 - mean[c]) / std[c], three correctly
 // rounded ops -- bit-identical to feeding the float path with the torch-normalised tensor, at a
 // quarter of the input bytes.
-// IMG = false (the training stem, pvnet_stem_s2d_nhwc): only S is written; `out` is not touched.
-// RAW = true (U8 only; the uint8 training stem, pvnet_stem_s2d_u8_nhwc): the image slice gets the normalised values
-// unrounded, the fp32 image the float training path concatenates into convraw.0's input; S stays TF32-rounded.
+// RAW = true (the training stem, pvnet_stem_s2d_nhwc): the image slice gets the fp32 image values unrounded (the
+// normalised values for a uint8 input), the image convraw.0 reads in training; S stays TF32-rounded.
 struct Norm3 {
     float mean[3], std[3];
 };
-template <bool U8, bool IMG = true, bool RAW = false>
+template <bool U8, bool RAW = false>
 __global__ void __launch_bounds__(128)
     k_s2d_pack(const void *__restrict__ in_v, Norm3 nrm, float *__restrict__ s2d, float *__restrict__ out, int H, int W,
                int out_cs, int out_co)
 {
-    static_assert(!RAW || (U8 && IMG), "RAW writes the image slice of a uint8 input");
     const float *in = static_cast<const float *>(in_v);
     // grid.y = image * H/2 + half-resolution row; a block covers 128 half-resolution columns.
     // Loads are coalesced float2 reads of the six (channel, row) lines; both outputs are staged in
@@ -150,7 +148,7 @@ __global__ void __launch_bounds__(128)
     const size_t plane = (size_t)H * W;
     if (x2 < W2) {
         float v[16];
-        float raw[12];                    // RAW: the unrounded normalised values, in v's order
+        float raw[12];                    // RAW: the unrounded values, in v's order
         if (U8) {
             // two rows x (2 pixels x 3 bytes): three 16-bit loads per row, coalesced across the warp
             const unsigned short *src8 = reinterpret_cast<const unsigned short *>(
@@ -182,24 +180,26 @@ __global__ void __launch_bounds__(128)
                     const float2 q = __ldg(reinterpret_cast<const float2 *>(src + c * plane + py * W));
                     v[(py * 2 + 0) * 3 + c] = ptx::round_tf32(q.x);
                     v[(py * 2 + 1) * 3 + c] = ptx::round_tf32(q.y);
+                    if constexpr (RAW) {
+                        raw[(py * 2 + 0) * 3 + c] = q.x;
+                        raw[(py * 2 + 1) * 3 + c] = q.y;
+                    }
                 }
         }
         v[12] = v[13] = v[14] = v[15] = 0.f;
 #pragma unroll
         for (int j = 0; j < 4; ++j)
             sS[t * 4 + (j ^ ((t >> 1) & 3))] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-        if constexpr (IMG) {
 #pragma unroll
-            for (int py = 0; py < 2; ++py)
+        for (int py = 0; py < 2; ++py)
 #pragma unroll
-                for (int px = 0; px < 2; ++px) {
-                    const int b = (py * 2 + px) * 3;
-                    if constexpr (RAW)
-                        sI[py][2 * t + px] = make_float4(raw[b], raw[b + 1], raw[b + 2], 0.f);
-                    else
-                        sI[py][2 * t + px] = make_float4(v[b], v[b + 1], v[b + 2], 0.f);
-                }
-        }
+            for (int px = 0; px < 2; ++px) {
+                const int b = (py * 2 + px) * 3;
+                if constexpr (RAW)
+                    sI[py][2 * t + px] = make_float4(raw[b], raw[b + 1], raw[b + 2], 0.f);
+                else
+                    sI[py][2 * t + px] = make_float4(v[b], v[b + 1], v[b + 2], 0.f);
+            }
     }
     __syncthreads();
     const int npx = min(128, W2 - xb);                    // half-resolution pixels this block holds
@@ -209,7 +209,6 @@ __global__ void __launch_bounds__(128)
         const int L = t + 128 * r, px = L >> 2, j = L & 3;
         if (px < npx) so[L] = sS[px * 4 + (j ^ ((px >> 1) & 3))];
     }
-    if constexpr (!IMG) return;
     // image slice: lane pairs write the 32 bytes (3 channels + 5 zeros) of one full-resolution pixel
 #pragma unroll
     for (int py = 0; py < 2; ++py) {
@@ -752,62 +751,46 @@ int pvnet_maxpool3x3s2_backward_nhwc(const float *dout, const uint8_t *code, flo
     return PVNET_OK;
 }
 
-int pvnet_stem_s2d_nhwc(const float *image_nchw, const float *w_s2d, const float *bias, float *s2d, float *out, int b,
-                        int H, int W, pvnet_stream_t stream)
+int pvnet_stem_s2d_nhwc(const void *image, int image_is_u8, const float *mean3, const float *std3, const float *w_s2d,
+                        const float *bias, float *s2d, float *out, float *img, int img_cs, int img_co, int b, int H,
+                        int W, pvnet_stream_t stream)
 {
-    PV_CHECK_ARG(image_nchw && w_s2d && bias && s2d && out, "stem: null pointer");
-    PV_CHECK_ARG(b > 0 && H > 0 && W > 0 && H % 2 == 0 && W % 2 == 0, "stem: b, H, W must be positive, H and W even");
-    PV_CHECK_ARG((uintptr_t)image_nchw % 8 == 0 && (uintptr_t)s2d % 16 == 0 && (uintptr_t)out % 16 == 0 &&
-                     (uintptr_t)w_s2d % 16 == 0,
-                 "stem: image must be 8-byte, s2d / out / weights 16-byte aligned");
-    // k_s2d_pack's grid.y is image * H/2 + row, at most 65535: launch it over chunks of whole images
+    PV_CHECK_ARG(image && w_s2d && bias && s2d && out && img, "stem: null pointer");
+    PV_CHECK_ARG(image_is_u8 ? mean3 && std3 : !mean3 && !std3,
+                 "stem: mean and std must be given for a uint8 image and NULL for a float image");
+    PV_CHECK_ARG(b > 0 && H > 0 && W > 0, "stem: b, H, W must be positive");
+    PV_CHECK_ARG(H % 2 == 0 && W % 2 == 0, "stem: H and W must be even, got %d x %d", H, W);
+    PV_CHECK_ARG((uintptr_t)image % (image_is_u8 ? 2 : 8) == 0 && (uintptr_t)s2d % 16 == 0 &&
+                     (uintptr_t)out % 16 == 0 && (uintptr_t)img % 16 == 0 && (uintptr_t)w_s2d % 16 == 0,
+                 "stem: image must be 2-byte (uint8) or 8-byte (float), s2d / out / img / weights 16-byte aligned");
+    PV_CHECK_ARG(img_co >= 0 && img_co % 4 == 0 && img_cs % 4 == 0 && img_co + 8 <= img_cs,
+                 "stem: image slice [%d, %d+8) must lie in a channel stride %d, offset and stride multiples of 4",
+                 img_co, img_co, img_cs);
+    pvnet::Norm3 nrm{};                    // read by the uint8 form only
+    for (int c = 0; image_is_u8 && c < 3; ++c) {
+        PV_CHECK_ARG(std::isfinite(mean3[c]) && std::isfinite(std3[c]) && std3[c] != 0.f,
+                     "stem: mean and std must be finite and std nonzero (channel %d: %g, %g)", c, mean3[c], std3[c]);
+        nrm.mean[c] = mean3[c];
+        nrm.std[c] = std3[c];
+    }
+    // k_s2d_pack's grid.y is image * H/2 + row, at most 65535: launch it over chunks of whole images.  Either image
+    // holds 3*H*W elements per image.
     PV_CHECK_ARG(H / 2 <= 65535, "stem: H/2 = %d rows exceed the 65535-row launch limit", H / 2);
     const int per = 65535 / (H / 2);
     for (int n0 = 0; n0 < b; n0 += per) {
         const int nb = std::min(per, b - n0);
         const dim3 grid((unsigned)((W / 2 + 127) / 128), (unsigned)(nb * (H / 2)));
-        pvnet::k_s2d_pack<false, false><<<grid, 128, 0, (cudaStream_t)stream>>>(
-            image_nchw + (size_t)n0 * 3 * H * W, pvnet::Norm3{}, s2d + (size_t)n0 * (H / 2) * (W / 2) * 16, nullptr, H,
-            W, 0, 0);
+        const size_t in0 = (size_t)n0 * 3 * H * W;
+        float *s2d0 = s2d + (size_t)n0 * (H / 2) * (W / 2) * 16, *img0 = img + (size_t)n0 * H * W * img_cs;
+        if (image_is_u8)
+            pvnet::k_s2d_pack<true, true><<<grid, 128, 0, (cudaStream_t)stream>>>(
+                static_cast<const uint8_t *>(image) + in0, nrm, s2d0, img0, H, W, img_cs, img_co);
+        else
+            pvnet::k_s2d_pack<false, true><<<grid, 128, 0, (cudaStream_t)stream>>>(
+                static_cast<const float *>(image) + in0, nrm, s2d0, img0, H, W, img_cs, img_co);
         PV_LAUNCHED("k_s2d_pack");
     }
     // the 7x7/2 convolution as the 4x4 stride-1 convolution on S (taps at offsets -2..1): the eval path's instantiation
-    return pvnet_conv2d_nhwc(s2d, 16, 0, 16, w_s2d, bias, nullptr, 0, 0, out, 64, 0, 64, b, H / 2, W / 2, 4, 1, 1, 0,
-                             0, stream);
-}
-
-int pvnet_stem_s2d_u8_nhwc(const uint8_t *image_u8, const float *mean3, const float *std3, const float *w_s2d,
-                           const float *bias, float *s2d, float *out, float *img, int img_cs, int img_co, int b, int H,
-                           int W, pvnet_stream_t stream)
-{
-    PV_CHECK_ARG(image_u8 && mean3 && std3 && w_s2d && bias && s2d && out && img, "stem u8: null pointer");
-    PV_CHECK_ARG(b > 0 && H > 0 && W > 0, "stem u8: b, H, W must be positive");
-    PV_CHECK_ARG(H % 2 == 0 && W % 2 == 0, "stem u8: H and W must be even, got %d x %d", H, W);
-    PV_CHECK_ARG((uintptr_t)image_u8 % 2 == 0 && (uintptr_t)s2d % 16 == 0 && (uintptr_t)out % 16 == 0 &&
-                     (uintptr_t)img % 16 == 0 && (uintptr_t)w_s2d % 16 == 0,
-                 "stem u8: image must be 2-byte, s2d / out / img / weights 16-byte aligned");
-    PV_CHECK_ARG(img_co >= 0 && img_co % 4 == 0 && img_cs % 4 == 0 && img_co + 8 <= img_cs,
-                 "stem u8: image slice [%d, %d+8) must lie in a channel stride %d, offset and stride multiples of 4",
-                 img_co, img_co, img_cs);
-    pvnet::Norm3 nrm{};
-    for (int c = 0; c < 3; ++c) {
-        PV_CHECK_ARG(std::isfinite(mean3[c]) && std::isfinite(std3[c]) && std3[c] != 0.f,
-                     "stem u8: mean and std must be finite and std nonzero (channel %d: %g, %g)", c, mean3[c],
-                     std3[c]);
-        nrm.mean[c] = mean3[c];
-        nrm.std[c] = std3[c];
-    }
-    PV_CHECK_ARG(H / 2 <= 65535, "stem u8: H/2 = %d rows exceed the 65535-row launch limit", H / 2);
-    // as pvnet_stem_s2d_nhwc: chunks of whole images keep grid.y = image * H/2 + row within 65535
-    const int per = 65535 / (H / 2);
-    for (int n0 = 0; n0 < b; n0 += per) {
-        const int nb = std::min(per, b - n0);
-        const dim3 grid((unsigned)((W / 2 + 127) / 128), (unsigned)(nb * (H / 2)));
-        pvnet::k_s2d_pack<true, true, true><<<grid, 128, 0, (cudaStream_t)stream>>>(
-            image_u8 + (size_t)n0 * H * W * 3, nrm, s2d + (size_t)n0 * (H / 2) * (W / 2) * 16,
-            img + (size_t)n0 * H * W * img_cs, H, W, img_cs, img_co);
-        PV_LAUNCHED("k_s2d_pack<u8, raw image>");
-    }
     return pvnet_conv2d_nhwc(s2d, 16, 0, 16, w_s2d, bias, nullptr, 0, 0, out, 64, 0, 64, b, H / 2, W / 2, 4, 1, 1, 0,
                              0, stream);
 }

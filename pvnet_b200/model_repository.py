@@ -356,14 +356,16 @@ class Resnet18_8s(nn.Module):
     def forward_train(self, x, mean=None, std=None):
         """The train-mode forward (`_forward_torch`) with every layer on the native kernels under autograd:
         * the stem conv1 as pvnet_b200.conv.stem_train (the eval path's space-to-depth tensor-core forward, a wgmma
-          weight gradient; the image gets no gradient, so it must not require one: ValueError);
+          weight gradient; the image gets no gradient, so it must not require one: ValueError), which also writes the
+          image and 5 zero channels into convraw.0's input buffer, allocated once per step;
         * the 24 convolutions of slots 1..24 as pvnet_b200.conv.Conv2dNHWC (pvnet_conv2d_nhwc forward, its data
           gradient and pvnet_conv2d_nhwc_wgrad backward);
         * the 25 BatchNorm layers with their ReLU/LeakyReLU and residual adds as pvnet_b200.conv.bn_act / bn_add_relu,
           following each module's own `training` flag, momentum and running statistics;
         * the max-pool as pvnet_b200.conv.maxpool_train (torch's argmax rule, a gather backward);
         * the three upsample-and-concatenate steps of the decoder as pvnet_b200.conv.upsample2x_cat (bit for bit
-          torch's forward; a fixed-order backward without atomics);
+          torch's forward; a fixed-order backward without atomics), the last one as upsample2x_into, which writes the
+          upsampled features into convraw.0's input buffer in place: no image copy and no concatenation copy;
         * the head convraw.3 as pvnet_b200.conv.head_train (exact fp32 forward, fixed-order fp64 parameter gradients).
         No step uses cuDNN, and the step runs under torch.use_deterministic_algorithms(True).  Activations are
         channels_last.  convraw.0 reads cat[fm, image, 5 zero channels] like the eval path.  Raises ValueError when
@@ -374,12 +376,10 @@ class Resnet18_8s(nn.Module):
         change: `seg_pred, vertex_pred = self.net.forward_train(image)`.
 
         x may also be the loader's raw uint8 [b,H,W,3] image (before ToTensor), with mean= and std= the Normalize
-        constants (3 numbers each), as forward_native takes it: the stem's pack (pvnet_b200.conv.stem_train_u8)
-        normalises it on the device exactly as ToTensor + Normalize do on the CPU and writes the normalised image into
-        convraw.0's input buffer, allocated once per step, into which upsample2x_into then writes the upsampled
-        decoder features: no float image and no concatenation copy.  Every output, gradient and running statistic is
-        that of the float path on the normalised image.  ValueError for a uint8 input without mean and std, for mean
-        or std with a float input, and for a uint8 input that is not [b,H,W,3]."""
+        constants (3 numbers each), as forward_native takes it: the stem's pack normalises it on the device exactly as
+        ToTensor + Normalize do on the CPU, so no float image exists.  Every output, gradient and running statistic
+        is that of the float path on the normalised image.  ValueError for a uint8 input without mean and std, for
+        mean or std with a float input, and for a uint8 input that is not [b,H,W,3]."""
         if x.requires_grad:
             raise ValueError("forward_train: the input image must not require grad (it gets no gradient)")
         raw_u8 = x.dtype == torch.uint8
@@ -394,20 +394,18 @@ class Resnet18_8s(nn.Module):
         if not x.is_cuda:
             raise RuntimeError("pvnet_b200: forward_train runs only on CUDA (no CPU fallback)")
         self._check_train_modules()
-        cl = torch.channels_last
         t = self.resnet18_8s
         if raw_u8:
             b, h, w, _ = x.shape
-            s2dim = self.conv2s[0].out_channels
-            # convraw.0's input cat[fm, image, 5 zeros]: the stem's pack fills channels [s2dim, s2dim+8) now, the
-            # decoder's upsampling channels [0, s2dim) at the end
-            raw_in = torch.empty(b, s2dim + 8, h, w, dtype=torch.float32, device=x.device, memory_format=cl)
-            x2s = pc.bn_act(t.bn1, pc.stem_train_u8(x, t.conv1.weight, mean, std, raw_in, s2dim), pc.act_of(t.relu))
         else:
             x = x.float()
-            x_nchw = x.contiguous()                   # the stem's space-to-depth pack reads NCHW
-            x = x.contiguous(memory_format=cl)        # convraw.0's concatenated input
-            x2s = pc.bn_act(t.bn1, pc.stem_train(x_nchw, t.conv1.weight), pc.act_of(t.relu))
+            b, h, w = x.shape[0], x.shape[-2], x.shape[-1]      # [b,3,H,W], checked by the stem
+        s2dim = self.conv2s[0].out_channels
+        # convraw.0's input cat[fm, image, 5 zeros]: the stem fills channels [s2dim, s2dim+8) now, the decoder's
+        # upsampling channels [0, s2dim) at the end
+        raw_in = torch.empty(b, s2dim + 8, h, w, dtype=torch.float32, device=x.device,
+                             memory_format=torch.channels_last)
+        x2s = pc.bn_act(t.bn1, pc.stem_train(x, t.conv1.weight, raw_in, s2dim, mean, std), pc.act_of(t.relu))
         x4s = pc.maxpool_train(x2s)
         for blk in t.layer1:
             x4s = self._block_train(blk, x4s)
@@ -421,12 +419,7 @@ class Resnet18_8s(nn.Module):
         fm = self._conv_bn_act(self.conv8s, torch.cat([xfc, x8s], 1))
         fm = self._conv_bn_act(self.conv4s, pc.upsample2x_cat(fm, x4s))
         fm = self._conv_bn_act(self.conv2s, pc.upsample2x_cat(fm, x2s))
-        if raw_u8:
-            y = self._conv_bn_act(self.convraw, pc.upsample2x_into(fm, raw_in), dgrad_channels=fm.shape[1])
-        else:
-            b, _, h, w = x.shape
-            pad = torch.zeros(b, 5, h, w, dtype=torch.float32, device=x.device).contiguous(memory_format=cl)
-            y = self._conv_bn_act(self.convraw, pc.upsample2x_cat(fm, x, pad), dgrad_channels=fm.shape[1])
+        y = self._conv_bn_act(self.convraw, pc.upsample2x_into(fm, raw_in), dgrad_channels=fm.shape[1])
         head = self.convraw[3]
         out = pc.head_train(y, head.weight, head.bias)
         return out[:, :self.seg_dim], out[:, self.seg_dim:]

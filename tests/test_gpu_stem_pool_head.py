@@ -70,13 +70,15 @@ def test_stem_weight_gradient_run_to_run_and_frozen():
     assert net.resnet18_8s.bn1.weight.grad is not None
 
 
-def test_stem_bad_arguments_return_a_status():
+def test_stem_and_wgrad_bad_arguments_return_a_status():
     L = _native.lib()
     n = ctypes.c_size_t()
     assert L.pvnet_stem_s2d_wgrad_workspace_bytes(2, 7, 8, ctypes.byref(n)) == -1
     assert b"even" in L.pvnet_last_error()
-    assert L.pvnet_stem_s2d_nhwc(None, None, None, None, None, 1, 8, 8, None) == -1
-    assert b"null" in L.pvnet_last_error()
+    mean3 = (ctypes.c_float * 3)(0.5, 0.5, 0.5)
+    for is_u8, m in ((0, None), (1, mean3)):            # a float image, a uint8 image
+        assert L.pvnet_stem_s2d_nhwc(None, is_u8, m, m, None, None, None, None, None, 8, 0, 1, 8, 8, None) == -1
+        assert b"null" in L.pvnet_last_error()
 
 
 # ----------------------------------------------------------------------------- max-pool

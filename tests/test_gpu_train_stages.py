@@ -418,7 +418,7 @@ def _run_case(case, monkeypatch):
 
 
 @pytest.mark.parametrize("case", CASES, ids=[c[0] for c in CASES])
-def test_step_layer_by_layer(case, monkeypatch):
+def test_step_native_calls_layer_by_layer(case, monkeypatch):
     _run_case(case, monkeypatch)
 
 

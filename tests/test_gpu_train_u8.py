@@ -1,5 +1,6 @@
-"""The compact training input on the H100 (DESIGN.md §18): the uint8 stem pack (pvnet_stem_s2d_u8_nhwc) against
-torch's normalisation, a forward_train(uint8, mean, std) step against the float path bit for bit, the losses with
+"""The compact training input on the H100 (DESIGN.md §18): the stem pack (pvnet_stem_s2d_nhwc) of a uint8 image against
+torch's normalisation and of a float image against the image itself, a forward_train(uint8, mean, std) step against the
+float path bit for bit, the losses with
 vertex_weights=None against the loader's mask.unsqueeze(1).float(), CUDA-graph replay, no synchronisation,
 deterministic mode, and the C ABI's refusals."""
 import copy
@@ -40,49 +41,78 @@ def _normalised(u8):
     return x.sub(mean).div(std).contiguous()
 
 
-def _stem_u8(u8, w4, img, co):
-    b, H, W, _ = u8.shape
+def _stem(x, w4, img, co):
+    """pvnet_stem_s2d_nhwc of a uint8 [b,H,W,3] image (ImageNet constants) or a float [b,3,H,W] one -> (S, out);
+    img [b,H,W,cs] gets the image and pad channels at co."""
+    is_u8 = x.dtype == torch.uint8
+    b, H, W = (x.shape[0], *x.shape[1:3]) if is_u8 else (x.shape[0], *x.shape[2:])
     s2d = torch.full((b, H // 2, W // 2, 16), float("nan"), device=DEV)
     out = torch.empty(b, H // 2, W // 2, 64, device=DEV)
-    mean3, std3 = pc.norm3(IMAGENET_MEAN, IMAGENET_STD)
-    _native.check(_native.lib().pvnet_stem_s2d_u8_nhwc(
-        u8.data_ptr(), mean3, std3, w4.data_ptr(), torch.zeros(64, device=DEV).data_ptr(), s2d.data_ptr(),
+    mean3, std3 = pc.norm3(IMAGENET_MEAN, IMAGENET_STD) if is_u8 else (None, None)
+    _native.check(_native.lib().pvnet_stem_s2d_nhwc(
+        x.data_ptr(), int(is_u8), mean3, std3, w4.data_ptr(), torch.zeros(64, device=DEV).data_ptr(), s2d.data_ptr(),
         out.data_ptr(), img.data_ptr(), img.shape[3], co, b, H, W,
-        ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)), "pvnet_stem_s2d_u8_nhwc")
+        ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)), "pvnet_stem_s2d_nhwc")
     return s2d, out
 
 
+def _s2d(x):
+    """The space-to-depth image of a float [b,3,H,W] image, TF32-rounded: what the pack writes as S."""
+    b, _, H, W = x.shape
+    xr = pc.round_tf32(x)
+    want = torch.zeros(b, H // 2, W // 2, 16, device=DEV)
+    for py in range(2):
+        for px in range(2):
+            ch = (py * 2 + px) * 3
+            want[..., ch:ch + 3] = xr[:, :, py::2, px::2].permute(0, 2, 3, 1)
+    return want
+
+
 @pytest.mark.parametrize("b,H,W", SHAPES)
-def test_pack_equals_torch_normalisation(b, H, W):
+def test_uint8_pack_equals_torch_normalisation(b, H, W):
     u8 = _u8(b, H, W, H + W + b)
     w = 0.1 * torch.randn(64, 3, 7, 7, device=DEV, generator=torch.Generator(device=DEV).manual_seed(1))
     w4 = pc.pack_stem_s2d_train(w)
     img = torch.full((b, H, W, 40), float("nan"), device=DEV)
-    s2d, out = _stem_u8(u8, w4, img, 32)
+    s2d, out = _stem(u8, w4, img, 32)
     x = _normalised(u8)
-    xr = pc.round_tf32(x)
-    want_s = torch.zeros(b, H // 2, W // 2, 16, device=DEV)
-    for py in range(2):
-        for px in range(2):
-            ch = (py * 2 + px) * 3
-            want_s[..., ch:ch + 3] = xr[:, :, py::2, px::2].permute(0, 2, 3, 1)
-    assert torch.equal(s2d, want_s)
+    assert torch.equal(s2d, _s2d(x))
     assert torch.equal(img[..., 32:35], x.permute(0, 2, 3, 1))               # unrounded, as the float path's cat
     pad = img[..., 35:40]
     assert torch.equal(pad, torch.zeros_like(pad)) and not torch.signbit(pad).any()
     assert torch.isnan(img[..., :32]).all()                                     # the decoder's channels untouched
-    # the convolution: the float path's stem on the normalised image
-    s2d_f = torch.empty_like(s2d)
-    out_f = torch.empty_like(out)
-    _native.check(_native.lib().pvnet_stem_s2d_nhwc(
-        x.data_ptr(), w4.data_ptr(), torch.zeros(64, device=DEV).data_ptr(), s2d_f.data_ptr(), out_f.data_ptr(), b,
-        H, W, ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)), "pvnet_stem_s2d_nhwc")
+    # the float stem on the normalised image: the same S, convolution and image slice (bits, NaNs included)
+    img_f = torch.full_like(img, float("nan"))
+    s2d_f, out_f = _stem(x, w4, img_f, 32)
     assert torch.equal(s2d_f, s2d) and torch.equal(out_f, out)
+    assert torch.equal(img_f.view(torch.int32), img.view(torch.int32))
     if b * H * W <= 3 * 72 * 104:                                               # the numpy restatement, and the CPU
         S, buf = pack_u8(u8.cpu().numpy(), IMAGENET_MEAN, IMAGENET_STD, np.full((b, H, W, 40), np.nan, np.float32),
                          32)
         assert S.tobytes() == s2d.cpu().numpy().tobytes()
         assert buf[..., 32:].tobytes() == img[..., 32:].cpu().numpy().tobytes()
+
+
+@pytest.mark.parametrize("b,H,W", SHAPES)
+def test_float_pack_writes_the_image_unrounded(b, H, W):
+    # the float stem's image slice is the image itself, bit for bit (a negative zero and values that S rounds
+    # included), then 5 zeros with no sign bit; every other channel is left as it was
+    g = torch.Generator(device=DEV).manual_seed(H + W + b + 1)
+    x = torch.randn(b, 3, H, W, device=DEV, generator=g)
+    x.view(-1)[:3] = torch.tensor([-0.0, 1.0 + 2.0 ** -20, -(1.0 + 2.0 ** -11)], device=DEV)
+    w4 = pc.pack_stem_s2d_train(0.1 * torch.randn(64, 3, 7, 7, device=DEV, generator=g))
+    img = torch.full((b, H, W, 48), float("nan"), device=DEV)
+    s2d, out = _stem(x, w4, img, 36)
+    assert torch.equal(s2d, _s2d(x))
+    bits = lambda t: t.contiguous().view(torch.int32)  # noqa: E731
+    assert torch.equal(bits(img[..., 36:39]), bits(x.permute(0, 2, 3, 1)))
+    pad = img[..., 39:44]
+    assert torch.equal(pad, torch.zeros_like(pad)) and not torch.signbit(pad).any()
+    assert torch.isnan(img[..., :36]).all() and torch.isnan(img[..., 44:]).all()
+    # the convolution is the one the eval path runs on S
+    want = torch.empty_like(out)
+    pc.conv2d_nhwc(s2d, 0, 16, w4, torch.zeros(64, device=DEV), want, 0, 64, 4)
+    assert torch.equal(out, want)
 
 
 def _batch(b, H, W, seed):
@@ -226,10 +256,8 @@ def test_uint8_step_does_not_synchronise_and_is_deterministic():
     _assert_same_state(net, twin)
 
 
-def test_forward_train_uint8_graph_has_no_float_image_or_cat():
-    net = Resnet18_8s(ver_dim=18, seg_dim=2).to(DEV).train()
-    seg, _ = net.forward_train(_u8(1, 64, 96, 0), mean=IMAGENET_MEAN, std=IMAGENET_STD)
-    names, seen, stack = [], set(), [seg.grad_fn]
+def _node_names(t):
+    names, seen, stack = [], set(), [t.grad_fn]
     while stack:
         n = stack.pop()
         if n is None or n in seen:
@@ -237,12 +265,21 @@ def test_forward_train_uint8_graph_has_no_float_image_or_cat():
         seen.add(n)
         names.append(type(n).__name__)
         stack += [f for f, _ in n.next_functions]
-    assert names.count("StemS2dU8NHWCBackward") == 1 and "StemS2dNHWCBackward" not in names
-    assert names.count("Upsample2xIntoNHWCBackward") == 1 and names.count("Upsample2xCatNHWCBackward") == 2
+    return names
+
+
+def test_forward_train_uint8_graph_is_the_float_graph():
+    # both inputs run one stem Function and one upsampling Function: no float image, no image copy and no cat for
+    # convraw.0's input on either path
+    net = Resnet18_8s(ver_dim=18, seg_dim=2).to(DEV).train()
+    u8 = _u8(1, 64, 96, 0)
+    names = _node_names(net.forward_train(u8, mean=IMAGENET_MEAN, std=IMAGENET_STD)[0])
+    assert names.count("StemS2dNHWCBackward") == 1 and names.count("Upsample2xCatNHWCBackward") == 3
     assert names.count("CatBackward0") == 1                                     # conv8s's cat[xfc, x8s] only
+    assert sorted(names) == sorted(_node_names(net.forward_train(_normalised(u8))[0]))
 
 
-def test_bad_arguments_return_invalid():
+def test_bad_arguments_return_invalid_for_both_image_forms():
     L = _native.lib()
     u8 = torch.zeros(2 * 8 * 8 * 3 + 2, dtype=torch.uint8, device=DEV)
     f = torch.zeros(1 << 16, device=DEV)
@@ -250,13 +287,17 @@ def test_bad_arguments_return_invalid():
     _, zero3 = pc.norm3(IMAGENET_MEAN, [0.2, 0.0, 0.2])
     p = f.data_ptr()
 
-    def call(img=u8.data_ptr(), m=mean3, s=std3, w4=p, out=p, buf=p, cs=40, co=32, b=2, H=8, W=8):
-        return L.pvnet_stem_s2d_u8_nhwc(img, m, s, w4, p, p, out, buf, cs, co, b, H, W, None)
+    def call(img=u8.data_ptr(), is_u8=1, m=mean3, s=std3, w4=p, out=p, buf=p, cs=40, co=32, b=2, H=8, W=8):
+        return L.pvnet_stem_s2d_nhwc(img, is_u8, m, s, w4, p, p, out, buf, cs, co, b, H, W, None)
+    flt = dict(img=p, is_u8=0, m=None, s=None)
     cases = [
         (dict(img=None), b"null"), (dict(buf=None), b"null"), (dict(b=0), b"positive"),
         (dict(W=7), b"even"), (dict(H=9), b"even"), (dict(img=u8.data_ptr() + 1), b"aligned"),
         (dict(out=p + 4), b"aligned"), (dict(co=30), b"multiples of 4"), (dict(co=36), b"channel stride"),
-        (dict(cs=38, co=28), b"multiples of 4"), (dict(s=zero3), b"std"),
+        (dict(cs=38, co=28), b"multiples of 4"), (dict(s=zero3), b"std"), (dict(m=None), b"mean"),
+        # a float image: mean and std NULL, 8-byte aligned, and the same checks of the image slice
+        (dict(flt, s=std3), b"NULL"), (dict(flt, img=p + 4), b"aligned"), (dict(flt, buf=None), b"null"),
+        (dict(flt, co=36), b"channel stride"), (dict(flt, H=6, W=5), b"even"),
     ]
     for kw, text in cases:
         assert call(**kw) == -1, kw

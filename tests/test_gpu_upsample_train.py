@@ -110,6 +110,26 @@ def test_bad_arguments_return_a_status():
         _native.check(L.pvnet_upsample2x_nhwc(p(x), 6, p(out), 8, 0, 1, 4, 4, _stream()), "pvnet_upsample2x_nhwc")
 
 
+def test_upsample2x_into_values_gradients_and_node():
+    # the caller's buffer: the upsampled channels written in place, the others left as they were; `low` gets the same
+    # gradient as from upsample2x_cat
+    g = torch.Generator(device=DEV).manual_seed(4)
+    cl = torch.channels_last
+    low = torch.randn(2, 32, 30, 40, device=DEV, generator=g).contiguous(memory_format=cl).requires_grad_()
+    buf = torch.randn(2, 40, 60, 80, device=DEV, generator=g).contiguous(memory_format=cl)
+    rest = buf[:, 32:].clone()
+    out = pc.upsample2x_into(low, buf)
+    assert out is buf and type(out.grad_fn).__name__ == "Upsample2xCatNHWCBackward"
+    assert torch.equal(out, torch.cat([_torch_up(low), rest], 1))
+    gy = torch.randn(out.shape, device=DEV, generator=g).contiguous(memory_format=cl)
+    out.backward(gy)
+    assert torch.equal(low.grad, _backward(gy.permute(0, 2, 3, 1).contiguous(), 0, 32).permute(0, 3, 1, 2))
+    with pytest.raises(ValueError, match="must not require"):
+        pc.upsample2x_into(low, torch.zeros_like(buf).requires_grad_())
+    with pytest.raises(ValueError, match="channels_last"):
+        pc.upsample2x_into(low, torch.zeros(2, 40, 60, 80, device=DEV))
+
+
 def test_upsample2x_cat_values_gradients_and_node():
     g = torch.Generator(device=DEV).manual_seed(3)
     cl = torch.channels_last
@@ -161,6 +181,7 @@ def test_forward_train_outputs_and_statistics_unchanged(monkeypatch):
     x = torch.randn(2, 3, 128, 160, device=DEV, generator=torch.Generator(device=DEV).manual_seed(1))
     out_n = net.forward_train(x)
     monkeypatch.setattr(pc, "upsample2x_cat", lambda low, *rest: torch.cat([_torch_up(low), *rest], 1))
+    monkeypatch.setattr(pc, "upsample2x_into", lambda low, buf: torch.cat([_torch_up(low), buf[:, low.shape[1]:]], 1))
     out_t = ref.forward_train(x)
     assert torch.equal(out_n[0], out_t[0]) and torch.equal(out_n[1], out_t[1])
     bn, bt = dict(net.named_buffers()), dict(ref.named_buffers())

@@ -143,7 +143,7 @@ def test_forward_train_argument_checks():
         net.forward_train(torch.zeros(1, 3, 64, 64))
 
 
-def test_stem_and_upsample_argument_checks():
+def test_norm3_stem_and_upsample_argument_checks():
     w = torch.zeros(64, 3, 7, 7)
     buf = torch.zeros(1, 40, 8, 8).contiguous(memory_format=torch.channels_last)
     with pytest.raises(ValueError, match="3 values"):
@@ -153,6 +153,6 @@ def test_stem_and_upsample_argument_checks():
     m, s = pc.norm3(torch.tensor(IMAGENET_MEAN), IMAGENET_STD)
     assert list(m) == [float(F32(v)) for v in IMAGENET_MEAN] and list(s) == [float(F32(v)) for v in IMAGENET_STD]
     with pytest.raises(ValueError, match="CUDA"):
-        pc.stem_train_u8(torch.zeros(1, 8, 8, 3, dtype=torch.uint8), w, IMAGENET_MEAN, IMAGENET_STD, buf, 32)
+        pc.stem_train(torch.zeros(1, 8, 8, 3, dtype=torch.uint8), w, buf, 32, IMAGENET_MEAN, IMAGENET_STD)
     with pytest.raises(ValueError, match="CUDA"):
         pc.upsample2x_into(torch.zeros(1, 32, 4, 4), buf)

@@ -126,7 +126,7 @@ class Capture:
         self.param_name = {id(p): n for n, p in net.named_parameters()}
         self.module_name = {id(m): n for n, m in net.named_modules()}
         self.orig = {k: getattr(pc, k) for k in ("stem_train", "bn_act", "bn_add_relu", "conv2d_train",
-                                                  "maxpool_train", "upsample2x_cat", "head_train")}
+                                                  "maxpool_train", "upsample2x_cat", "upsample2x_into", "head_train")}
 
     def install(self, monkeypatch):
         for k in self.orig:
@@ -160,9 +160,9 @@ class Capture:
     def _snapshot(bn):
         return tuple(t.detach().clone() for t in (bn.running_mean, bn.running_var, bn.num_batches_tracked))
 
-    def stem_train(self, x, weight):
+    def stem_train(self, x, weight, img, co, mean=None, std=None):
         rec, (xv,) = self._begin("stem", self._weight_owner(weight), x)
-        return self._end(rec, self.orig["stem_train"](xv, weight))
+        return self._end(rec, self.orig["stem_train"](xv, weight, img, co, mean, std))
 
     def conv2d_train(self, x, weight, stride=1, dilation=1, dgrad_channels=None):
         rec, (xv,) = self._begin("conv", self._weight_owner(weight), x)
@@ -188,6 +188,14 @@ class Capture:
     def upsample2x_cat(self, low, *rest):
         rec, passed = self._begin("upsample_cat", None, low, *rest)
         return self._end(rec, self.orig["upsample2x_cat"](*passed))
+
+    def upsample2x_into(self, low, buf):
+        """Recorded as the upsample_cat it stands for: the `rest` inputs are the buffer's channels behind low's (the
+        image and zero channels the stem wrote), copied before the call, and the output is the whole buffer."""
+        C = low.shape[1]
+        rec, (lv,) = self._begin("upsample_cat", None, low)
+        rec.inputs += [buf[:, C:C + 3].clone(), buf[:, C + 3:].clone()]
+        return self._end(rec, self.orig["upsample2x_into"](lv, buf))
 
     def head_train(self, y, weight, bias):
         rec, (yv,) = self._begin("head", self._weight_owner(weight), y)

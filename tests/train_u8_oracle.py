@@ -2,9 +2,9 @@
 
   normalise: torchvision's ToTensor + Normalize as the loader runs them on the CPU, (float(u) / 255 - mean) / std,
     three correctly rounded fp32 operations (numpy rounds each float32 operation once);
-  pack_u8: what pvnet_stem_s2d_u8_nhwc's pack writes -- S, the 2x2 space-to-depth image (channel (py*2+px)*3+c,
-    TF32-rounded, 4 zero channels), and, in a caller's channels_last buffer, the normalised image unrounded at
-    channels [co, co+3) and zeros at [co+3, co+8), every other channel left as it was;
+  pack_u8: what pvnet_stem_s2d_nhwc's pack writes for a uint8 image -- S, the 2x2 space-to-depth image (channel
+    (py*2+px)*3+c, TF32-rounded, 4 zero channels), and, in a caller's channels_last buffer, the normalised image
+    unrounded at channels [co, co+3) and zeros at [co+3, co+8), every other channel left as it was;
   mask_weights: the loader's vertex_weights, mask.unsqueeze(0).float() per image (linemod_dataset.py:227).
 """
 from __future__ import annotations
