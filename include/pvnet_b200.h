@@ -67,6 +67,8 @@ enum {
 };
 
 PVNET_API const char *pvnet_last_error(void);
+/* ABI version.  2: backbone slot 0 holds the stem in its space-to-depth packing (was [7*7][3][64]) and the
+ * backbone has 26 conv slots. */
 PVNET_API int pvnet_version(void);
 
 /* ------------------------------------------------------------------ voting layer */
@@ -557,7 +559,7 @@ PVNET_API int pvnet_batchnorm_act_backward(int form, int act, const float *dy, c
  *     the image v.
  *   H, W even.  s2d [b,H/2,W/2,16] is written with the 2x2 space-to-depth image (channel (py*2+px)*3+c, 4 zero
  *   channels, rounded to TF32) and out NHWC [b,H/2,W/2,64] = the 4x4 stride-1 tensor-core convolution of s2d with
- *   w_s2d (packed [64][4][4][16] as backbone slot 26, TF32) plus bias [64], fp32, no activation.  s2d is what
+ *   w_s2d (packed [64][4][4][16] as backbone slot 0, TF32) plus bias [64], fp32, no activation.  s2d is what
  *   pvnet_stem_s2d_wgrad reads.  In the same pass the caller's channels_last buffer img NHWC [b,H,W,img_cs] gets the
  *   fp32 image unrounded in channels [img_co, img_co+3) and zeros in [img_co+3, img_co+8) (img_co, img_cs multiples
  *   of 4, img_co+8 <= img_cs): convraw.0's image and pad channels; its other channels are not touched.
@@ -595,10 +597,10 @@ PVNET_API int pvnet_head1x1_backward(const float *dout, const float *y, const fl
                                      float *db, int b, int H, int W, int Cin, int Cout, void *workspace,
                                      size_t workspace_bytes, pvnet_stream_t stream);
 
-/* Test hook: which convolution kernel pvnet_conv2d_nhwc / the backbone use for layers both can
- * run.  0 = automatic (persistent weights-resident column kernel for 3x3 stride-1 layers with
- * Cout <= 64 whose weights fit in shared memory, per-tap kernel otherwise), 1 = per-tap kernel
- * only, 2 = column kernel (error if the layer is not eligible). */
+/* Test hook: which convolution kernel pvnet_conv2d_nhwc uses for layers both can run (the backbone
+ * always plans automatically).  0 = automatic (persistent weights-resident column kernel for 3x3
+ * stride-1 layers with Cout <= 64 whose weights fit in shared memory, per-tap kernel otherwise),
+ * 1 = per-tap kernel only, 2 = column kernel (error if the layer is not eligible). */
 PVNET_API int pvnet_conv_set_mode(int mode);
 /* Test hook: 1 = the per-tap kernel runs as clusters of two CTAs on adjacent M tiles that share each
  * weight tile through TMA multicast; 0 (default) = single CTAs. */
@@ -612,7 +614,9 @@ PVNET_API int pvnet_conv_set_persistent(int on);
  * The handle is a host-side table of per-convolution weight pointers plus cached tensor
  * maps; it owns no device memory.  Weights are DEVICE pointers owned by the caller and
  * must stay valid while the handle is used:
- *   slot 0               stem conv1+bn1, packed [7*7][3][64] (tap, cin, cout), bias [64]
+ *   slot 0               stem conv1+bn1, the 7x7 stride-2 conv written as a 4x4 stride-1 conv over
+ *                        the 2x2 space-to-depth image, packed [64][4][4][16] (tap (ty,tx), channel
+ *                        (py*2+px)*3+c holds w[c][2ty+py-1][2tx+px-1]; rest 0), bias [64]
  *   slots 1..24          the 3x3 / 1x1 convs in execution order (layer1.0.conv1, layer1.0.conv2,
  *                        layer1.1.conv1, layer1.1.conv2, layer2.0.conv1, layer2.0.downsample,
  *                        layer2.0.conv2, layer2.1.conv1, layer2.1.conv2, layer3.* and layer4.* in the
@@ -620,9 +624,6 @@ PVNET_API int pvnet_conv_set_persistent(int on);
  *                        [Cout][kh*kw][cin_pad] with its BatchNorm folded in, bias [Cout].  convraw.0 reads
  *                        s2dim+8 buffer channels (s2dim upsampled, 3 image, 5 zeros); cin_pad rounds up to 32.
  *   slot 25              convraw.3 (1x1, with bias): [seg_dim+ver_dim][32], bias [seg_dim+ver_dim]
- *   slot 26              the stem once more for the tensor-core path: the 7x7 stride-2 conv written as
- *                        a 4x4 stride-1 conv over the 2x2 space-to-depth image, packed [64][4][4][16]
- *                        (tap (ty,tx), channel (py*2+px)*3+c holds w[c][2ty+py-1][2tx+px-1]; rest 0)
  * pvnet_backbone_forward:
  *   image_nchw  f32 [b,3,h,w] (h,w multiples of 8)
  *   out_nchw    f32 [b,seg_dim+ver_dim,h,w]: seg logits are channels [0,seg_dim), the vertex
@@ -642,12 +643,6 @@ PVNET_API int pvnet_backbone_set_conv(pvnet_backbone_t *m, int slot, const float
  * vertex layout [b,h,w,K,2] the voting layer's gather reads without sector waste (the contiguous
  * form of the permuted view of tools/demo.py:48-50). */
 PVNET_API int pvnet_backbone_set_output_layout(pvnet_backbone_t *m, int pixel_major);
-/* The last decoder upsampling, F.interpolate(x2s_up, scale_factor=2, mode='bilinear', align_corners=True)
- * (model_repository.py:75), can run inside convraw.0's operand loader: the full-resolution
- * [b,h,w,s2dim] tensor is then never written, the output is bit-identical.  on != 0 selects the fused
- * form (the producer warps of convraw.0 interpolate into its operand stages), 0 the separate upsampling
- * launch, -1 = default (environment variable PVNET_FUSE_UP, else the separate launch). */
-PVNET_API int pvnet_backbone_set_fused_upsample(pvnet_backbone_t *m, int on);
 PVNET_API int pvnet_backbone_workspace_bytes(const pvnet_backbone_t *m, int b, int h, int w, size_t *bytes);
 PVNET_API int pvnet_backbone_forward(pvnet_backbone_t *m, const float *image_nchw, int b, int h, int w,
                                      float *out_nchw, void *mask_out, int mask_elem_size,

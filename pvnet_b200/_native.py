@@ -136,7 +136,6 @@ SIGNATURES = {
     "pvnet_backbone_num_convs": (c_int, []),
     "pvnet_backbone_set_conv": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
     "pvnet_backbone_set_output_layout": (c_int, [c_void_p, c_int]),
-    "pvnet_backbone_set_fused_upsample": (c_int, [c_void_p, c_int]),
     "pvnet_backbone_workspace_bytes": (c_int, [c_void_p, c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
     "pvnet_backbone_forward": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int,
                                        c_void_p, c_size_t, c_void_p]),

@@ -19,7 +19,7 @@ MODE_AUTO, MODE_PER_TAP, MODE_COLUMN = 0, 1, 2
 
 
 def set_mode(mode: int):
-    """Test hook (pvnet_conv_set_mode): which kernel runs layers both kernels support."""
+    """Test hook (pvnet_conv_set_mode): which kernel pvnet_conv2d_nhwc runs for layers both kernels support."""
     _native.check(_native.lib().pvnet_conv_set_mode(int(mode)), "pvnet_conv_set_mode")
 
 

@@ -1,23 +1,24 @@
 // backbone.cu -- Resnet18_8s.forward (lib/networks/model_repository.py:64-80 over
 // lib/networks/resnet.py:200-220) as one launch sequence on the caller's stream:
-// 25 wgmma convolutions (conv_tc.cu, conv_col.cu) + stem / max-pool / 3 upsamplings / image packing /
-// head (backbone_aux.cu).  Eval mode only: BatchNorm is folded into the packed weights by
-// the host layer (pvnet_b200/model_repository.py).  Activations are NHWC fp32 (TF32-rounded
-// where they feed a tensor-core conv); every torch.cat of the decoder is replaced by
+// 25 wgmma convolutions (conv_tc.cu, conv_col.cu; the stem as a 4x4 conv on the space-to-depth image) +
+// image packing / max-pool / 3 upsamplings / head (backbone_aux.cu).  Eval mode only: BatchNorm is folded
+// into the packed weights by the host layer (pvnet_b200/model_repository.py).  Activations are NHWC fp32
+// (TF32-rounded where they feed a tensor-core conv); every torch.cat of the decoder is replaced by
 // producers writing into channel slices of one buffer:
 //
 //   C8 [b,H/8,W/8, fc+128]   xfc -> [0,fc)        x8s (layer2) -> [fc,fc+128)
 //   C4 [b,H/4,W/4, s8+64]    up(conv8s) -> [0,s8) x4s (layer1) -> [s8,s8+64)
 //   C2 [b,H/2,W/2, s4+64]    up(conv4s) -> [0,s4) x2s (stem)   -> [s4,s4+64)
-//   C1 [b,H,  W,   s2+8]     up(conv2s) -> [0,s2) image        -> [s2,s2+3), zeros to +8
+//   C1 [b,H,  W,   s2]       up(conv2s), followed by [b,H,W,8]: image (3 channels, zeros to 8); convraw.0
+//                            reads the two dense parts as its two sources (ConvDesc::in2)
 #include "conv_tc.cuh"
 
-#include <cstdlib>
 #include <vector>
 
 using namespace pvnet;
 
-// conv slots, in execution order.  Slot 0 (stem) and the last (head) are not tensor-core convs.
+// conv slots, in execution order.  Slot 0 is the stem as a 4x4 conv on the space-to-depth image; the last (head)
+// runs in convraw.0's epilogue or as k_head.
 enum {
     CV_STEM = 0,
     CV_L1_0_C1, CV_L1_0_C2, CV_L1_1_C1, CV_L1_1_C2,
@@ -25,7 +26,6 @@ enum {
     CV_L3_0_C1, CV_L3_0_DS, CV_L3_0_C2, CV_L3_1_C1, CV_L3_1_C2,
     CV_L4_0_C1, CV_L4_0_DS, CV_L4_0_C2, CV_L4_1_C1, CV_L4_1_C2,
     CV_FC, CV_CONV8S, CV_CONV4S, CV_CONV2S, CV_CONVRAW0, CV_HEAD,
-    CV_STEM_TC,   // the stem again, packed [64][4][4][16] for the space-to-depth tensor-core form
     CV_COUNT
 };
 
@@ -39,23 +39,8 @@ struct pvnet_backbone {
     std::vector<unsigned char> plans;   // CV_COUNT slots of plan_stride() bytes
     bool use_col[CV_COUNT] = {};         // slot runs on the persistent column kernel (conv_col.cu)
     bool head_fused = false;             // convraw.3 + argmax run inside convraw.0's epilogue
-    bool stem_tc = false;                // stem runs as a 4x4 conv on the space-to-depth image
-    bool raw_split = false;              // convraw.0 reads the upsampled features and the image slice from two dense buffers
     int out_nhwc = 0;                    // output layout: 0 = [b,C,H,W] (reference), 1 = pixel-major [b,H,W,C]
-    int fuse_up = -1;                    // 1/2 -> 1 upsampling inside convraw.0's loader: -1 = default (PVNET_FUSE_UP, off)
-    bool up2_fused = false;              // the current plan has no separate 1/2 -> 1 upsampling launch
 };
-
-// default of the fused 1/2 -> 1 upsampling (tuning knob PVNET_FUSE_UP, read once): OFF.  Both forms compute the
-// same bits; the separate k_upsample2x launch is the default.
-static int env_fuse_up()
-{
-    static const int v = [] {
-        const char *e = getenv("PVNET_FUSE_UP");
-        return e ? atoi(e) : 0;
-    }();
-    return v;
-}
 
 // where the image comes from: float32 NCHW (already normalised) or raw uint8 HWC + mean/std
 struct ImageSrc {
@@ -145,7 +130,7 @@ int build_plans(pvnet_backbone *m, const Buffers &B, int b, int h, int w)
     m->head_fused = false;
     auto plan = [&](int slot, const ConvDesc &d) {
         void *st = m->plans.data() + ps * slot;
-        const bool col = g_conv_mode != 1 && conv_col_eligible(d);
+        const bool col = conv_col_eligible(d);
         m->use_col[slot] = col;
         if (!col) return conv_plan_at(d, st);
         if (slot == CV_CONVRAW0 && m->raw == 32 && m->seg_dim + m->ver_dim <= 32) {
@@ -158,15 +143,10 @@ int build_plans(pvnet_backbone *m, const Buffers &B, int b, int h, int w)
         return conv_col_plan_at(d, nullptr, st);
     };
     const int h2 = h / 2, w2 = w / 2, h4 = h / 4, w4 = w / 4, h8 = h / 8, w8 = w / 8;
-    const int c4s = m->s8 + 64, c8s = m->fc + 128, c2s = m->s4 + 64, c1s = m->s2 + 8;
+    const int c4s = m->s8 + 64, c8s = m->fc + 128, c2s = m->s4 + 64;
     int rc = 0;
     // stem (resnet.py:201-203) as a 4x4 stride-1 conv on the 2x2 space-to-depth image
-    m->stem_tc = g_conv_mode != 1;
-    if (m->stem_tc) {
-        ConvDesc d = cd(m, CV_STEM_TC, B.S2D, 16, 0, 16, B.C2, c2s, m->s4, 64, b, h2, w2, 4, 1, 1, 1);
-        m->use_col[CV_STEM_TC] = true;
-        if ((rc = conv_col_plan_at(d, nullptr, m->plans.data() + ps * CV_STEM_TC))) return rc;
-    }
+    if ((rc = plan(CV_STEM, cd(m, CV_STEM, B.S2D, 16, 0, 16, B.C2, c2s, m->s4, 64, b, h2, w2, 4, 1, 1, 1)))) return rc;
     // layer1 (resnet.py:206): two BasicBlocks at 1/4 resolution
     if ((rc = plan(CV_L1_0_C1, cd(m, CV_L1_0_C1, B.P, 64, 0, 64, B.A1, 64, 0, 64, b, h4, w4, 3, 1, 1, 1)))) return rc;
     if ((rc = plan(CV_L1_0_C2, cd(m, CV_L1_0_C2, B.A1, 64, 0, 64, B.B1, 64, 0, 64, b, h4, w4, 3, 1, 1, 1, B.P, 64, 0)))) return rc;
@@ -196,34 +176,14 @@ int build_plans(pvnet_backbone *m, const Buffers &B, int b, int h, int w)
     if ((rc = plan(CV_CONV8S, cd(m, CV_CONV8S, B.C8, c8s, 0, c8s, B.U8, m->s8, 0, m->s8, b, h8, w8, 3, 1, 1, 2)))) return rc;
     if ((rc = plan(CV_CONV4S, cd(m, CV_CONV4S, B.C4, c4s, 0, c4s, B.U4, m->s4, 0, m->s4, b, h4, w4, 3, 1, 1, 2)))) return rc;
     if ((rc = plan(CV_CONV2S, cd(m, CV_CONV2S, B.C2, c2s, 0, c2s, B.U2, m->s2, 0, m->s2, b, h2, w2, 3, 1, 1, 2)))) return rc;
-    // convraw.0 reads cat(upsampled features [s2], image [3 -> 8]).  With the column kernel the two
-    // parts live in two dense buffers (the first p1*s2 and the next p1*8 floats of C1) read through two
-    // tensor maps: a 32-byte image slice inside every 160-byte record made both producers write at
-    // ~2 TB/s.  The per-tap kernel (test mode) keeps the single interleaved buffer.
-    ConvDesc draw = cd(m, CV_CONVRAW0, B.C1, c1s, 0, c1s, B.R0, m->raw, 0, m->raw, b, h, w, 3, 1, 1, 2, nullptr, 0, 0,
+    // convraw.0 reads cat(upsampled features [s2], image [3 -> 8]) from two dense buffers (the first p1*s2 and the
+    // next p1*8 floats of C1) through two tensor maps: a 32-byte image slice inside every 160-byte record made both
+    // producers write at ~2 TB/s.
+    ConvDesc draw = cd(m, CV_CONVRAW0, B.C1, m->s2, 0, m->s2, B.R0, m->raw, 0, m->raw, b, h, w, 3, 1, 1, 2, nullptr, 0, 0,
                        /*round_out=*/0);
-    m->raw_split = false;
-    m->up2_fused = false;
-    if (g_conv_mode != 1 && m->s2 % 8 == 0) {
-        ConvDesc ds = draw;
-        ds.in_cs = m->s2;
-        ds.Cin = m->s2;
-        ds.in2 = B.C1 + (size_t)b * h * w * m->s2;
-        ds.in2_cs = 8;
-        ds.in2_co = 0;
-        ds.Cin2 = 8;
-        if (conv_col_eligible(ds)) {
-            draw = ds;
-            m->raw_split = true;
-            // F.interpolate(x2s_up, scale 2) (model_repository.py:75) inside convraw.0's operand loader: conv2s.0's
-            // half-resolution output U2 is the source, the full-resolution tensor is never written
-            const int want = m->fuse_up < 0 ? env_fuse_up() : m->fuse_up;
-            if (want != 0 && m->s2 == 32 && m->raw == 32 && m->seg_dim + m->ver_dim <= 32) {
-                draw.up_src = B.U2;
-                m->up2_fused = true;
-            }
-        }
-    }
+    draw.in2 = B.C1 + (size_t)b * h * w * m->s2;
+    draw.in2_cs = 8;
+    draw.Cin2 = 8;
     if ((rc = plan(CV_CONVRAW0, draw))) return rc;
     return PVNET_OK;
 }
@@ -266,14 +226,6 @@ int pvnet_backbone_set_output_layout(pvnet_backbone_t *m, int pixel_major)
     return PVNET_OK;
 }
 
-int pvnet_backbone_set_fused_upsample(pvnet_backbone_t *m, int on)
-{
-    PV_CHECK_ARG(m, "null handle");
-    m->fuse_up = on < 0 ? -1 : (on ? 1 : 0);
-    m->p_ws = nullptr;   // replan
-    return PVNET_OK;
-}
-
 int pvnet_backbone_set_conv(pvnet_backbone_t *m, int slot, const float *w_packed, const float *bias)
 {
     PV_CHECK_ARG(m, "null handle");
@@ -295,7 +247,7 @@ int pvnet_backbone_workspace_bytes(const pvnet_backbone_t *m, int b, int h, int 
 
 // The forward pass as an ordered list of stages (one kernel launch each).
 namespace {
-enum StageKind { ST_STEM, ST_PACK, ST_POOL, ST_CONV, ST_UP8, ST_UP4, ST_UP2, ST_HEAD };
+enum StageKind { ST_PACK, ST_POOL, ST_CONV, ST_UP8, ST_UP4, ST_UP2, ST_HEAD };
 struct Stage {
     StageKind kind;
     int slot;
@@ -303,7 +255,7 @@ struct Stage {
 };
 const Stage kStages[] = {
     {ST_PACK, -1, "image: space-to-depth + NHWC slice packing"},
-    {ST_STEM, CV_STEM, "stem conv1+bn1+relu"},
+    {ST_CONV, CV_STEM, "stem conv1+bn1+relu"},
     {ST_POOL, -1, "maxpool 3x3/2"},
     {ST_CONV, CV_L1_0_C1, "layer1.0.conv1"}, {ST_CONV, CV_L1_0_C2, "layer1.0.conv2"},
     {ST_CONV, CV_L1_1_C1, "layer1.1.conv1"}, {ST_CONV, CV_L1_1_C2, "layer1.1.conv2"},
@@ -355,23 +307,12 @@ int prepare(pvnet_backbone *m, const ImageSrc &img, int b, int h, int w, float *
 int run_stage(pvnet_backbone *m, const Stage &st, const Buffers &B, const ImageSrc &img, int b, int h, int w,
               float *out_nchw, void *mask_out, int mask_elem_size, cudaStream_t s)
 {
-    const float *image_nchw = static_cast<const float *>(img.ptr);
-    if (img.is_u8 && !(m->stem_tc)) {
-        set_error("uint8 image input needs the default convolution mode (tensor-core stem)");
-        return PVNET_E_INVALID;
-    }
     const int h2 = h / 2, w2 = w / 2, h4 = h / 4, w4 = w / 4, h8 = h / 8, w8 = w / 8;
-    const int c4s = m->s8 + 64, c2s = m->s4 + 64, c1s = m->s2 + 8;
+    const int c4s = m->s8 + 64, c2s = m->s4 + 64;
     switch (st.kind) {
-    case ST_STEM:
-        if (m->stem_tc) return conv_col_launch_at(m->plans.data() + plan_stride() * CV_STEM_TC, s);
-        return launch_stem(image_nchw, m->w[CV_STEM], m->bias[CV_STEM], B.C2, b, h, w, c2s, m->s4, s);
     case ST_PACK:
-        if (m->stem_tc && m->raw_split)
-            return launch_s2d_pack(img.ptr, img.is_u8, img.mean, img.std, B.S2D, B.C1 + (size_t)b * h * w * m->s2, b, h, w, 8,
-                                   0, s);
-        if (m->stem_tc) return launch_s2d_pack(img.ptr, img.is_u8, img.mean, img.std, B.S2D, B.C1, b, h, w, c1s, m->s2, s);
-        return launch_pack_image(image_nchw, B.C1, b, h, w, c1s, m->s2, s);
+        return launch_s2d_pack(img.ptr, img.is_u8, img.mean, img.std, B.S2D, B.C1 + (size_t)b * h * w * m->s2, b, h, w, 8, 0,
+                               s);
     case ST_POOL: return launch_maxpool(B.C2, B.P, b, h2, w2, 64, c2s, m->s4, s);
     case ST_CONV: {
         unsigned char *pl = m->plans.data() + plan_stride() * st.slot;
@@ -381,9 +322,7 @@ int run_stage(pvnet_backbone *m, const Stage &st, const Buffers &B, const ImageS
     }
     case ST_UP8: return launch_upsample2x(B.U8, B.C4, b, h8, w8, m->s8, c4s, 0, s);
     case ST_UP4: return launch_upsample2x(B.U4, B.C2, b, h4, w4, m->s4, c2s, 0, s);
-    case ST_UP2:
-        if (m->up2_fused) return PVNET_OK;     // interpolated inside convraw.0
-        return launch_upsample2x(B.U2, B.C1, b, h2, w2, m->s2, m->raw_split ? m->s2 : c1s, 0, s);
+    case ST_UP2: return launch_upsample2x(B.U2, B.C1, b, h2, w2, m->s2, m->s2, 0, s);
     case ST_HEAD:
         if (m->head_fused) return PVNET_OK;    // already written by convraw.0's epilogue
         return launch_head(B.R0, m->w[CV_HEAD], m->bias[CV_HEAD], out_nchw, mask_out, mask_elem_size, m->seg_dim,

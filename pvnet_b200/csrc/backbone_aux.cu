@@ -1,118 +1,14 @@
 // backbone_aux.cu -- the non-GEMM kernels of Resnet18_8s (lib/networks/resnet.py:200-220,
-// lib/networks/model_repository.py:64-80): stem conv 7x7/2 (Cin=3), max-pool 3x3/2,
-// bilinear x2 upsampling (align_corners=True), NCHW image -> NHWC slice packing, and the
+// lib/networks/model_repository.py:64-80): the image's space-to-depth + NHWC slice packing for the
+// tensor-core stem and convraw.0, max-pool 3x3/2, bilinear x2 upsampling (align_corners=True), and the
 // final 1x1 conv + per-pixel argmax head that writes the reference's NCHW outputs.
-// All of them are HBM-bound streaming kernels except the stem (FP32 FMA bound).
+// All of them are HBM-bound streaming kernels.
 #include "conv_tc.cuh"
 #include "ptx.cuh"
 #include <algorithm>
 #include <cmath>
 
 namespace pvnet {
-
-// ------------------------------------------------------------------ stem
-// conv1 (3->64, 7x7, stride 2, pad 3) + folded bn1 + ReLU (resnet.py:201-203).
-// in: NCHW [b,3,H,W]; out: NHWC [b,H/2,W/2,out_cs] at out_co (64 channels), tf32-rounded.
-// CTA: 8 x 32 output pixels x 64 channels.  Shared memory: the 21 x 69 x 3 input patch and
-// all 64*147 weights ([tap][ci][co] so a thread reads 4 consecutive co as one LDS.128
-// broadcast).  Thread = one output pixel, 64 accumulators.
-constexpr int STEM_TY = 8, STEM_TX = 32;
-constexpr int STEM_PH = STEM_TY * 2 + 5, STEM_PW = STEM_TX * 2 + 5;   // 21 x 69
-constexpr int STEM_PWP = STEM_PW + 1;
-
-__global__ void __launch_bounds__(256)
-    k_stem(const float *__restrict__ in, const float *__restrict__ w /*[49][3][64]*/,
-           const float *__restrict__ bias /*[64]*/, float *__restrict__ out, int H, int W, int out_cs, int out_co)
-{
-    extern __shared__ float sm[];
-    float *sw = sm;                               // 147*64
-    float *sp = sm + 147 * 64;                    // [3][21][70]
-    const int Ho = H / 2, Wo = W / 2;
-    const int n = blockIdx.z;
-    const int oy0 = blockIdx.y * STEM_TY, ox0 = blockIdx.x * STEM_TX;
-    for (int i = threadIdx.x; i < 147 * 64; i += 256) sw[i] = w[i];
-    const int iy0 = oy0 * 2 - 3, ix0 = ox0 * 2 - 3;
-    for (int i = threadIdx.x; i < 3 * STEM_PH * STEM_PW; i += 256) {
-        const int c = i / (STEM_PH * STEM_PW);
-        const int r = i - c * (STEM_PH * STEM_PW);
-        const int py = r / STEM_PW, px = r - py * STEM_PW;
-        const int iy = iy0 + py, ix = ix0 + px;
-        float v = 0.f;
-        if (iy >= 0 && iy < H && ix >= 0 && ix < W) v = in[(((size_t)n * 3 + c) * H + iy) * W + ix];
-        sp[(c * STEM_PH + py) * STEM_PWP + px] = v;
-    }
-    __syncthreads();
-    const int ty = threadIdx.x / STEM_TX, tx = threadIdx.x % STEM_TX;
-    float acc[64];
-#pragma unroll
-    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
-    for (int kh = 0; kh < 7; ++kh) {
-        for (int kw = 0; kw < 7; ++kw) {
-#pragma unroll
-            for (int c = 0; c < 3; ++c) {
-                const float v = sp[(c * STEM_PH + ty * 2 + kh) * STEM_PWP + tx * 2 + kw];
-                const float4 *wv = reinterpret_cast<const float4 *>(sw + ((kh * 7 + kw) * 3 + c) * 64);
-#pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                    const float4 ww = wv[j];
-                    acc[4 * j + 0] = fmaf(v, ww.x, acc[4 * j + 0]);
-                    acc[4 * j + 1] = fmaf(v, ww.y, acc[4 * j + 1]);
-                    acc[4 * j + 2] = fmaf(v, ww.z, acc[4 * j + 2]);
-                    acc[4 * j + 3] = fmaf(v, ww.w, acc[4 * j + 3]);
-                }
-            }
-        }
-    }
-    const int oy = oy0 + ty, ox = ox0 + tx;
-    if (oy < Ho && ox < Wo) {
-        float *o = out + (((size_t)n * Ho + oy) * Wo + ox) * out_cs + out_co;
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-            float4 v;
-            v.x = ptx::round_tf32(fmaxf(acc[4 * j + 0] + bias[4 * j + 0], 0.f));
-            v.y = ptx::round_tf32(fmaxf(acc[4 * j + 1] + bias[4 * j + 1], 0.f));
-            v.z = ptx::round_tf32(fmaxf(acc[4 * j + 2] + bias[4 * j + 2], 0.f));
-            v.w = ptx::round_tf32(fmaxf(acc[4 * j + 3] + bias[4 * j + 3], 0.f));
-            reinterpret_cast<float4 *>(o)[j] = v;
-        }
-    }
-}
-
-int launch_stem(const float *in, const float *w, const float *bias, float *out, int b, int H, int W, int out_cs,
-                int out_co, cudaStream_t s)
-{
-    const size_t smem = (147 * 64 + 3 * STEM_PH * STEM_PWP) * sizeof(float);
-    PV_CUDA(ensure_max_smem((const void *)k_stem, (int)smem));
-    dim3 grid((W / 2 + STEM_TX - 1) / STEM_TX, (H / 2 + STEM_TY - 1) / STEM_TY, b);
-    k_stem<<<grid, 256, smem, s>>>(in, w, bias, out, H, W, out_cs, out_co);
-    PV_LAUNCHED("k_stem");
-    return PVNET_OK;
-}
-
-// ------------------------------------------------------------------ image packing
-// NCHW [b,3,H,W] -> NHWC slice [.., co..co+8): 3 image channels (tf32-rounded) + 5 zeros
-__global__ void k_pack_image(const float *__restrict__ in, float *__restrict__ out, int npix_per_img, long long total,
-                             int out_cs, int out_co)
-{
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= total) return;
-    const long long n = i / npix_per_img;
-    const long long p = i - n * npix_per_img;
-    const float *src = in + n * 3 * (long long)npix_per_img + p;
-    float4 a = make_float4(ptx::round_tf32(src[0]), ptx::round_tf32(src[npix_per_img]),
-                           ptx::round_tf32(src[2 * (long long)npix_per_img]), 0.f);
-    float4 *o = reinterpret_cast<float4 *>(out + i * out_cs + out_co);
-    o[0] = a;
-    o[1] = make_float4(0.f, 0.f, 0.f, 0.f);
-}
-
-int launch_pack_image(const float *in, float *out, int b, int H, int W, int out_cs, int out_co, cudaStream_t s)
-{
-    const long long total = (long long)b * H * W;
-    k_pack_image<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(in, out, H * W, total, out_cs, out_co);
-    PV_LAUNCHED("k_pack_image");
-    return PVNET_OK;
-}
 
 // ------------------------------------------------------------------ space-to-depth + image packing
 // One pass over the NCHW image that writes (a) S [b,H/2,W/2,16]: the 2x2 space-to-depth image,
@@ -501,8 +397,8 @@ __global__ void __launch_bounds__(256)
     // All blocks but those of the first row / column (and a last one whose scale*index rounds down) have the same
     // pattern: output 2j reads source rows (j-1, j), output 2j+1 rows (j, j+1), same for columns -- two-term sums (8 instead of 12
     // floating-point instructions per float4; the kernel is issue-bound).  lerp3 with its zero weight rounds
-    // identically (fmul of the first product, fma of the second; adding 0*x changes nothing), so both paths and the
-    // column kernel's fused loader agree to the last bit.
+    // identically (fmul of the first product, fma of the second; adding 0*x changes nothing), so both paths
+    // agree to the last bit.
     const bool interior = !pat[0][0] && pat[1][0] && !pat[0][1] && pat[1][1];
     if (interior) {
         const float a0 = wx[0][0], a1 = wx[0][1], b0 = wx[1][1], b1 = wx[1][2];      // column weights of outputs 2k, 2k+1

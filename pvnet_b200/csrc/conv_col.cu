@@ -16,9 +16,12 @@
 //   * optional fused head (convraw.3 1x1 + bias + argmax) in the epilogue: the activated 128 x 32 tile
 //     is already in the register layout of a wgmma A operand, so the head is one more MMA; its output is staged
 //     in shared memory and stored by the producer warpgroup's otherwise idle warps while the next tile's MMAs
-//     run -- the [b,H,W,32] intermediate never exists;
-//   * optional fused bilinear x2 upsampling of convraw.0's first input (the producer warps interpolate
-//     it into the operand stages instead of TMA loading it).
+//     run -- the [b,H,W,32] intermediate never exists.
+//
+// k_conv_col<KC, HEAD, KH, BN, WIDE> is instantiated per layer form: KC channels per chunk (8, 16 or 32), KH x KH
+// taps (3, or 4 for the stem), BN = Cout (32 or 64), HEAD the fused head (convraw.0 only, BN 32), WIDE convraw.0's
+// two-source input with its 32-channel first source loaded as one 128-byte-swizzled box.  conv_col_launch_at picks
+// the instantiation a plan was made for.
 #include "conv_tc.cuh"
 #include "ptx.cuh"
 
@@ -62,127 +65,6 @@ struct ColGeom {
     int head_cout, head_seg, mask_esz;
     int head_nhwc;          // fused head writes pixel-major [b,H,W,cout] instead of the reference's NCHW
 };
-
-// fused bilinear x2 upsampling of the first split_chunk channel chunks (UP variant of the kernel)
-struct ColUp {
-    const float *src;       // half-resolution source [b,h,w,cs], dense
-    int h, w, cs;
-    float sy, sx;           // ATen's align_corners scale (in-1)/(out-1)
-    unsigned zero;          // always 0; opaque to the compiler (see up_fill_rows)
-};
-
-// Fused upsampling (UP variant of the kernel): producer warp q interpolates channel chunk q (8 channels)
-// of one tile's halo box -- (COL_TH+2) x (COL_TW+2) full-resolution pixels, zero outside the image like
-// the TMA box it replaces -- straight into the operand stage, in the 32-byte-swizzled layout TMA would
-// have written (16-byte half `hf` of box row rr sits at rr*32 + ((hf ^ (rr>>2 & 1)) << 4): address bit 4
-// XOR bit 7).  Arithmetic is k_upsample2x's (backbone_aux.cu), i.e. ATen's upsample_bilinear2d with
-// align_corners: src = scale*dst, out = h0*(w0*v00 + w1*v01) + h1*(w0*v10 + w1*v11), rounded to tf32.
-// Lane = (box column, half): it walks its column top to bottom, keeping the horizontally interpolated
-// source rows in registers (10 rows x 2 loads for 18 outputs instead of 4 loads per output).  With
-// scale 2 the source row pair of output row y0-1+i is (E, E+1), E = y0/2 - 1 + i/2, except in the
-// last image row when scale*y rounds below E (then it is (E-1, E)): a three-row window with one zero
-// weight covers both, as in k_upsample2x.
-__device__ __forceinline__ float4 ldg_nc_v4_volatile(const float *p)
-{
-    float4 v;
-    asm volatile("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p));
-    return v;
-}
-// Box rows [I0, I1) of one lane's column: loads the window slots these rows need (slot 0 never: it only ever
-// carries the zero weight, see above), interpolates horizontally, then vertically row by row.
-template <int I0, int I1>
-__device__ __forceinline__ void up_fill_rows(const float *base, unsigned rstride, unsigned olo, unsigned ohi, int R0, int uh,
-                                             bool act, bool vx, float w1x_, unsigned zero, float wa_l, float wb_l, float wc_l,
-                                             uint32_t sbase, int c, int hf)
-{
-    constexpr int PITCH = COL_TW + 2;
-    constexpr int S0 = I0 >> 1, S1 = ((I1 - 1) >> 1) + 2;      // window slots of these rows
-    constexpr int L0 = S0 < 1 ? 1 : S0, NL = S1 - L0 + 1;      // slots actually loaded
-    // All source loads are issued before anything consumes them (volatile asm keeps them together) ...
-    float4 a[NL], b[NL];
-#pragma unroll
-    for (int j = L0; j <= S1; ++j) {
-        a[j - L0] = b[j - L0] = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (act) {
-            const unsigned ro = (unsigned)min(max(R0 + j, 0), uh - 1) * rstride;
-            a[j - L0] = ldg_nc_v4_volatile(base + (ro + olo));
-            b[j - L0] = ldg_nc_v4_volatile(base + (ro + ohi));
-        }
-    }
-    // ... and nothing may consume them before the last one has landed: ptxas otherwise starts on the first
-    // output rows as soon as their three source rows are there and parks the remaining loads behind those
-    // stores (3-4 exposed L2 round trips per tile instead of one).  The interpolation weight is made to
-    // depend on every load through an AND with a kernel parameter that is always zero.
-    unsigned dep = 0;
-#pragma unroll
-    for (int j = 0; j < NL; ++j) dep |= __float_as_uint(a[j].x) | __float_as_uint(b[j].x);
-    float w1x = __uint_as_float(__float_as_uint(w1x_) | (dep & zero)), w0x = 1.f - w1x_;
-    if (!vx) w0x = w1x = 0.f;
-    float4 t[S1 - S0 + 1];
-    if (S0 == 0) t[0] = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-    for (int j = L0; j <= S1; ++j) {
-        t[j - S0].x = __fmaf_rn(w1x, b[j - L0].x, __fmul_rn(w0x, a[j - L0].x));   // lerp3 with a zero third weight
-        t[j - S0].y = __fmaf_rn(w1x, b[j - L0].y, __fmul_rn(w0x, a[j - L0].y));
-        t[j - S0].z = __fmaf_rn(w1x, b[j - L0].z, __fmul_rn(w0x, a[j - L0].z));
-        t[j - S0].w = __fmaf_rn(w1x, b[j - L0].w, __fmul_rn(w0x, a[j - L0].w));
-    }
-#pragma unroll
-    for (int i = I0; i < I1; ++i) {
-        const float wa = __shfl_sync(0xffffffffu, wa_l, i), wb = __shfl_sync(0xffffffffu, wb_l, i),
-                    wc = __shfl_sync(0xffffffffu, wc_l, i);
-        const int e = (i >> 1) - S0;
-        // Rounding to tf32 (nearest, ties away -- cvt.rna.tf32, what k_upsample2x stores): add half an ulp of
-        // the 10-bit mantissa and clear the 13 low bits, so the MMA reads exactly the values the separate
-        // launch stores.
-        float4 o;
-        o.x = __uint_as_float((__float_as_uint(lerp3(wa, t[e].x, wb, t[e + 1].x, wc, t[e + 2].x)) + 0x1000u) & 0xFFFFE000u);
-        o.y = __uint_as_float((__float_as_uint(lerp3(wa, t[e].y, wb, t[e + 1].y, wc, t[e + 2].y)) + 0x1000u) & 0xFFFFE000u);
-        o.z = __uint_as_float((__float_as_uint(lerp3(wa, t[e].z, wb, t[e + 1].z, wc, t[e + 2].z)) + 0x1000u) & 0xFFFFE000u);
-        o.w = __uint_as_float((__float_as_uint(lerp3(wa, t[e].w, wb, t[e + 1].w, wc, t[e + 2].w)) + 0x1000u) & 0xFFFFE000u);
-        const int rr = i * PITCH + c;
-        if (act) ptx::sts128(sbase + (uint32_t)(i * PITCH * 32) + (uint32_t)((hf ^ ((rr >> 2) & 1)) << 4), o);
-    }
-}
-
-// The whole column at once (20 loads in flight).
-__device__ __forceinline__ void up_fill_chunk(const ColUp &u, const ColGeom &g, int img, int y0, int x0, int q, int lane,
-                                              uint32_t stage_addr)
-{
-    constexpr int PITCH = COL_TW + 2, ROWS = COL_TH + 2;
-    const bool act = lane < 2 * PITCH;                 // lanes 20..31 only take part in the shuffles
-    const int c = act ? lane >> 1 : 0, hf = lane & 1;
-    const int x = x0 - 1 + c;
-    const bool vx = act && x >= 0 && x < g.Wo;
-    const int xc = min(max(x, 0), g.Wo - 1);
-    const float fx = u.sx * (float)xc;
-    const int xlo = (int)fx;
-    const int xhi = min(xlo + 1, u.w - 1);
-    const float w1x_ = fx - (float)xlo;
-    const int R0 = (y0 >> 1) - 2;
-    // Vertical weights: lane r works out box row r's window weights once; the row loop fetches them with
-    // three shuffles (the weights are the same for the whole warp: ~20 instructions per row otherwise).
-    // Rows outside the image get zero weights -- the conv's zero padding -- and columns outside get zero
-    // horizontal weights, so no output needs a select.
-    float wa_l = 0.f, wb_l = 0.f, wc_l = 0.f;
-    {
-        const int y = y0 - 1 + lane;
-        if (lane < ROWS && y >= 0 && y < g.Ho) {
-            const float fy = u.sy * (float)y;
-            const int ylo = (int)fy;
-            const float h1 = fy - (float)ylo, h0 = 1.f - h1;
-            const bool low = ylo < R0 + 1 + (lane >> 1);   // source pair is rows (E-1, E) rather than (E, E+1)
-            wa_l = low ? h0 : 0.f;
-            wb_l = low ? h1 : h0;
-            wc_l = low ? 0.f : h1;
-        }
-    }
-    const float *base = u.src + (size_t)img * u.h * u.w * u.cs + q * 8 + hf * 4;
-    const unsigned rstride = (unsigned)u.w * (unsigned)u.cs;      // 32-bit element offsets inside one image
-    const unsigned olo = (unsigned)xlo * (unsigned)u.cs, ohi = (unsigned)xhi * (unsigned)u.cs;
-    const uint32_t sbase = stage_addr + (uint32_t)(c * 32);   // box row rr = i*PITCH + c sits at rr*32 + ((hf ^ bit 2 of rr) << 4)
-    up_fill_rows<0, ROWS>(base, rstride, olo, ohi, R0, u.h, act, vx, w1x_, u.zero, wa_l, wb_l, wc_l, sbase, c, hf);
-}
 
 // Copies one staged head tile (see head_pitch) to head_out and mask; thread `tid` of `nthr`.  The tile is 32*hc
 // units of four floats: pixel-major, 2*hc of them cover one tile row's contiguous run of 8*hc floats; NCHW, two
@@ -237,24 +119,21 @@ __device__ __forceinline__ void head_store_tile(const ColGeom &g, uint32_t sv, u
     }
 }
 
-
-
 // BN = Cout (32 or 64); KC channels per chunk (rows of KC*4 bytes, swizzled by the same amount).
 // WIDE (convraw.0 with a 32-channel first source): the four 8-channel chunks of the first source are loaded as one
 // 128-byte-swizzled box, with their weights as 128-byte-swizzled [32][32] tiles, and the MMAs still run chunk by
 // chunk, tap by tap, so every output sums the same products in the same order as with 8-channel boxes.  The
 // 32-byte-swizzled operands of 8-channel chunks ran the same MMAs at about half the rate (DESIGN.md section 6).
-template <int KC, bool HEAD, int KH, bool UP, int BN, bool WIDE = false>
+template <int KC, bool HEAD, int KH, int BN, bool WIDE = false>
 __global__ void __launch_bounds__(COL_THREADS, 1)
     k_conv_col(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
                const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmBw, const __grid_constant__ ColGeom g,
                const float *__restrict__ bias, const float *__restrict__ res, float *__restrict__ out,
                const float *__restrict__ head_w, const float *__restrict__ head_b, float *__restrict__ head_out,
-               void *__restrict__ mask, const ColUp up)
+               void *__restrict__ mask)
 {
-    static_assert(!UP || (HEAD && KC == 8 && KH == 3), "fused upsampling: convraw.0 form only");
     static_assert(!HEAD || BN == 32, "fused head: 32 input channels");
-    static_assert(!WIDE || (HEAD && !UP && KC == 8 && KH == 3), "wide first source: convraw.0 form only");
+    static_assert(!WIDE || (HEAD && KC == 8 && KH == 3), "wide first source: convraw.0 form only");
     constexpr int ROWB = KC * 4;                       // bytes per K-major row
     constexpr int B_TILE = BN * ROWB;                  // one [BN][KC] weight tile (a multiple of 1024 bytes)
     constexpr int PITCH = COL_TW + KH - 1;             // box pitch in pixels (= shared-memory rows)
@@ -281,7 +160,7 @@ __global__ void __launch_bounds__(COL_THREADS, 1)
     uint64_t *hfree = hstaged + 2;                                // HEAD: [2] staging buffer copied out by the store warps
     float *s_bias = reinterpret_cast<float *>(empty + g.stages + (HEAD ? 4 : 0));  // [BN]
     float *s_head = s_bias + 64;                                  // [32]
-    constexpr int STORE_THREADS = 96;                             // HEAD && !UP: producer warps 9-11 store the head output
+    constexpr int STORE_THREADS = 96;                             // HEAD: producer warps 9-11 store the head output
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (threadIdx.x == 0) {
@@ -290,7 +169,7 @@ __global__ void __launch_bounds__(COL_THREADS, 1)
             ptx::mbar_init(&full[s], 1);
             ptx::mbar_init(&empty[s], 8);              // one arrive per consumer warp
         }
-        if (HEAD && !UP)
+        if (HEAD)
             for (int b = 0; b < 2; ++b) {
                 ptx::mbar_init(&hstaged[b], 256);      // every consumer thread, after its own shared-memory writes
                 ptx::mbar_init(&hfree[b], STORE_THREADS);
@@ -315,7 +194,7 @@ __global__ void __launch_bounds__(COL_THREADS, 1)
     const int tiles_per_img = g.tiles_x * g.tiles_y;
 
     if (warp >= 8) {
-        // producer warpgroup: warp 8 lane 0 issues the TMA loads; with UP, warp 8 + q also interpolates chunk q
+        // producer warpgroup: warp 8 lane 0 issues the TMA loads; with HEAD, warps 9-11 store the head output
         const int pw = warp - 8;
         if (pw == 0 && lane == 0 && g.resident) {
             // all weights, once: tile t = cc*KH*KH + kh*KH + kw <- packed [Cout][kh][kw][cin]; WIDE: the first
@@ -327,7 +206,7 @@ __global__ void __launch_bounds__(COL_THREADS, 1)
             if (WIDE)
                 for (int t = 0; t < KH * KH; ++t) ptx::tma_load_2d(sB + (size_t)t * BN * 128, &tmBw, wfull, t * g.cin_pad, 0);
         }
-        if (HEAD && !UP && pw != 0) {
+        if (HEAD && pw != 0) {
             // store warps: the CTA's tiles in the consumers' order, buffer it & 1, the ring's parity discipline
             const int tid = threadIdx.x - 9 * 32;
             int it = 0;
@@ -344,7 +223,7 @@ __global__ void __launch_bounds__(COL_THREADS, 1)
             }
             return;
         }
-        if (!UP && pw != 0) return;
+        if (pw != 0) return;
         int s = 0;
         uint32_t ph = 0;
         const uint32_t tx_bytes = (uint32_t)(A_BOX + (g.resident ? 0 : KH * KH * B_TILE));
@@ -362,15 +241,6 @@ __global__ void __launch_bounds__(COL_THREADS, 1)
                         ptx::tma_load_4d(st, cc == 0 ? &tmA : &tmA2, &full[s], 0, x0 - g.pad_l, y0 - g.pad_t, img);
                     }
                     __syncwarp();
-                } else if (UP && cc < g.split_chunk) {
-                    if (pw == cc) {
-                        ptx::mbar_wait(&empty[s], ph ^ 1u);
-                        up_fill_chunk(up, g, img, y0, x0, cc, lane, ptx::smem_u32(st));
-                        // generic-proxy stores into a stage that a later round refills by TMA (async proxy)
-                        ptx::fence_proxy_async();
-                        __syncwarp();
-                        if (lane == 0) ptx::mbar_arrive(&full[s]);
-                    }
                 } else if (pw == 0) {
                     if (lane == 0) {
                         ptx::mbar_wait(&empty[s], ph ^ 1u);
@@ -524,7 +394,7 @@ __global__ void __launch_bounds__(COL_THREADS, 1)
             const int hc = g.head_cout, pp = head_pitch(hc);
             const uint32_t sv = ptx::smem_u32(sHS) + (uint32_t)((it & 1) * hs_bytes);
             const uint32_t sm = sv + 4u * (uint32_t)head_stage_floats(hc);
-            if (!UP) ptx::mbar_wait(&hfree[it & 1], ((uint32_t)(it >> 1) & 1u) ^ 1u);
+            ptx::mbar_wait(&hfree[it & 1], ((uint32_t)(it >> 1) & 1u) ^ 1u);
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const uint32_t p = (uint32_t)((ty + h) * COL_TW + g8);
@@ -564,14 +434,7 @@ __global__ void __launch_bounds__(COL_THREADS, 1)
                 }
                 if (t4 == 0) ptx::sts8(sm + p, (uint32_t)best_c);
             }
-            if (!UP) {
-                ptx::mbar_arrive(&hstaged[it & 1]);
-            } else {
-                // the producer warps interpolate: the consumers copy the tile out themselves.  Buffer it & 1 is
-                // written again two tiles later, after every consumer has passed the next tile's barrier.
-                ptx::named_bar_sync(1, 256);
-                head_store_tile(g, sv, sm, head_out, mask, img, tyi * COL_TH, txi * COL_TW, threadIdx.x, 256);
-            }
+            ptx::mbar_arrive(&hstaged[it & 1]);
         }
     }
 }
@@ -579,8 +442,7 @@ __global__ void __launch_bounds__(COL_THREADS, 1)
 struct ColPlan {
     CUtensorMap tmA, tmA2, tmB, tmBw;
     ColGeom g;
-    int kc, ksize, head, up, bn, wide;
-    ColUp cup;
+    int kc, ksize, head, bn, wide;
     unsigned grid;
     size_t smem;
     const float *bias, *res;
@@ -605,22 +467,21 @@ size_t col_smem(int kc, int ksize, int cin_chunks, int bn, int stages, bool head
            (size_t)(1 + 2 * stages) * 8 + (64 + 32) * 4;
 }
 
-template <int KC, bool HEAD, int KH, bool UP, int BN, bool WIDE = false>
+template <int KC, bool HEAD, int KH, int BN, bool WIDE = false>
 int col_launch(const ColPlan &p, cudaStream_t s)
 {
     // the instantiation must be the plan's: weight boxes, barrier byte counts and stores are sized by BN
-    if (p.bn != BN || p.kc != KC || p.ksize != KH || p.head != (HEAD ? 1 : 0) || p.up != (UP ? 1 : 0) ||
-        p.wide != (WIDE ? 1 : 0)) {
+    if (p.bn != BN || p.kc != KC || p.ksize != KH || p.head != (HEAD ? 1 : 0) || p.wide != (WIDE ? 1 : 0)) {
         set_error("conv(col): no kernel instantiation for this plan (Cout %d, chunk %d, ksize %d)", p.bn, p.kc, p.ksize);
         return PVNET_E_STATE;
     }
-    auto fn = k_conv_col<KC, HEAD, KH, UP, BN, WIDE>;
+    auto fn = k_conv_col<KC, HEAD, KH, BN, WIDE>;
     const cudaError_t attr_err = ensure_max_smem((const void *)fn, (int)SMEM_LIMIT);
     PV_CUDA(attr_err);
     const HeadDesc &h = p.hd;
     fn<<<p.grid, COL_THREADS, p.smem, s>>>(p.tmA, p.tmA2, p.tmB, p.tmBw, p.g, p.bias, p.res, p.out, p.head ? h.w : nullptr,
                                            p.head ? h.bias : nullptr, p.head ? h.out_nchw : nullptr,
-                                           p.head ? h.mask : nullptr, p.cup);
+                                           p.head ? h.mask : nullptr);
     PV_LAUNCHED("k_conv_col");
     return PVNET_OK;
 }
@@ -645,10 +506,7 @@ int conv_col_plan_at(const ConvDesc &d, const HeadDesc *head, void *storage)
 {
     ColPlan *p = new (storage) ColPlan();
     PV_CHECK_ARG(conv_col_eligible(d), "conv(col): layer not eligible for the column kernel");
-    PV_CHECK_ARG((d.in || d.up_src) && d.w && d.bias && (d.out || head), "conv(col): null pointer");
-    PV_CHECK_ARG(!d.up_src || (head && d.in2 && col_kc(d.Cin + d.Cin2) == 8 && d.Cin == 32 && d.Cin2 == 8 && d.ksize == 3 &&
-                               d.H % 2 == 0 && d.W % 2 == 0 && (uintptr_t)d.up_src % 16 == 0),
-                 "conv(col): fused upsampling needs the convraw.0 form (32 upsampled + 8 direct channels, fused head)");
+    PV_CHECK_ARG(d.in && d.w && d.bias && (d.out || head), "conv(col): null pointer");
     PV_CHECK_ARG(d.in_cs % 4 == 0 && d.in_co % 4 == 0 && d.out_cs % 4 == 0 && d.out_co % 4 == 0,
                  "conv(col): channel strides/offsets must be multiples of 4 floats");
     PV_CHECK_ARG(!d.res || (d.res_cs % 4 == 0 && d.res_co % 4 == 0), "conv(col): residual stride/offset alignment");
@@ -676,13 +534,6 @@ int conv_col_plan_at(const ConvDesc &d, const HeadDesc *head, void *storage)
     g.head_seg = head ? head->seg_dim : 0;
     g.mask_esz = head ? head->mask_esz : 0;
     g.head_nhwc = 0;
-    p->cup.src = d.up_src;
-    p->cup.h = d.H / 2;
-    p->cup.w = d.W / 2;
-    p->cup.cs = d.Cin;
-    p->cup.sy = (float)(p->cup.h - 1) / (float)(2 * p->cup.h - 1);   // launch_upsample2x's scales
-    p->cup.sx = (float)(p->cup.w - 1) / (float)(2 * p->cup.w - 1);
-    p->cup.zero = 0;
     // Resident weights whenever at least 2 A stages (one channel chunk with all its taps each) still
     // fit next to them; otherwise the KH*KW weight tiles of a chunk travel with its A box.
     const bool hd = head != nullptr;
@@ -690,7 +541,7 @@ int conv_col_plan_at(const ConvDesc &d, const HeadDesc *head, void *storage)
     const size_t hs = hd ? 2 * (size_t)head_stage_bytes(head->cout) + 4 * 8 : 0;
     // convraw.0's 32 + 8 channel form loads its first source as one box of 128-byte rows (WIDE in k_conv_col);
     // its stages then hold that box instead of an 8-channel one
-    bool wide = hd && !d.up_src && d.in2 && d.Cin == 32 && d.Cin2 == 8 && kc == 8 && d.ksize == 3;
+    bool wide = hd && d.in2 && d.Cin == 32 && d.Cin2 == 8 && kc == 8 && d.ksize == 3;
     const size_t wx = col_smem(32, 3, 0, 0, 1, false, false) - col_smem(8, 3, 0, 0, 1, false, false);
     int stages = 8;
     bool resident = true;
@@ -702,7 +553,6 @@ int conv_col_plan_at(const ConvDesc &d, const HeadDesc *head, void *storage)
         stages = 8;
         while (stages > 2 && col_smem(kc, d.ksize, g.cin_chunks, d.Cout, stages, hd, false) + hs > SMEM_LIMIT) --stages;
     }
-    PV_CHECK_ARG(!d.up_src || resident, "conv(col): fused upsampling needs resident weights");
     g.stages = stages;
     g.resident = resident ? 1 : 0;
     p->smem = col_smem(kc, d.ksize, g.cin_chunks, d.Cout, stages, hd, resident) + hs + (wide ? stages * wx : 0);
@@ -712,9 +562,8 @@ int conv_col_plan_at(const ConvDesc &d, const HeadDesc *head, void *storage)
     p->ksize = d.ksize;
     p->bn = d.Cout;
     p->head = hd ? 1 : 0;
-    p->up = d.up_src ? 1 : 0;
     if (head) p->hd = *head;
-    if (!d.up_src) {
+    {
         const float *base = d.in + d.in_co;
         cuuint64_t dims[4] = {(cuuint64_t)d.Cin, (cuuint64_t)d.W, (cuuint64_t)d.H, (cuuint64_t)d.b};
         cuuint64_t strides[3] = {(cuuint64_t)d.in_cs * 4, (cuuint64_t)d.W * d.in_cs * 4,
@@ -733,7 +582,6 @@ int conv_col_plan_at(const ConvDesc &d, const HeadDesc *head, void *storage)
         cuuint32_t box[4] = {(cuuint32_t)kc, (cuuint32_t)(COL_TW + d.ksize - 1), (cuuint32_t)(COL_TH + d.ksize - 1), 1};
         int rc = tma_encode(&p->tmA2, d.in2 + d.in2_co, 4, dims, strides, box, kc * 4);
         if (rc) return rc;
-        if (d.up_src) p->tmA = p->tmA2;     // the first source is interpolated in the kernel, not read by TMA
     }
     {
         cuuint64_t dims[2] = {(cuuint64_t)d.ksize * d.ksize * g.cin_pad, (cuuint64_t)d.Cout};
@@ -770,14 +618,13 @@ void conv_col_set_head_ptrs(void *storage, float *out_nchw, void *mask, int mask
 int conv_col_launch_at(const void *storage, cudaStream_t s)
 {
     const ColPlan &p = *static_cast<const ColPlan *>(storage);
-    if (p.up) return col_launch<8, true, 3, true, 32>(p, s);
-    if (p.wide) return col_launch<8, true, 3, false, 32, true>(p, s);
-    if (p.head) return p.kc == 32 ? col_launch<32, true, 3, false, 32>(p, s) : col_launch<8, true, 3, false, 32>(p, s);
+    if (p.wide) return col_launch<8, true, 3, 32, true>(p, s);
+    if (p.head) return p.kc == 32 ? col_launch<32, true, 3, 32>(p, s) : col_launch<8, true, 3, 32>(p, s);
     const bool n64 = p.bn == 64;
-    if (p.ksize == 4) return n64 ? col_launch<16, false, 4, false, 64>(p, s) : col_launch<16, false, 4, false, 32>(p, s);
-    if (p.kc == 32) return n64 ? col_launch<32, false, 3, false, 64>(p, s) : col_launch<32, false, 3, false, 32>(p, s);
-    if (p.kc == 16) return n64 ? col_launch<16, false, 3, false, 64>(p, s) : col_launch<16, false, 3, false, 32>(p, s);
-    return n64 ? col_launch<8, false, 3, false, 64>(p, s) : col_launch<8, false, 3, false, 32>(p, s);
+    if (p.ksize == 4) return n64 ? col_launch<16, false, 4, 64>(p, s) : col_launch<16, false, 4, 32>(p, s);
+    if (p.kc == 32) return n64 ? col_launch<32, false, 3, 64>(p, s) : col_launch<32, false, 3, 32>(p, s);
+    if (p.kc == 16) return n64 ? col_launch<16, false, 3, 64>(p, s) : col_launch<16, false, 3, 32>(p, s);
+    return n64 ? col_launch<8, false, 3, 64>(p, s) : col_launch<8, false, 3, 32>(p, s);
 }
 
 }  // namespace pvnet

@@ -27,11 +27,6 @@ struct ConvDesc {
     // concatenated input write dense records of their own
     const float *in2 = nullptr;
     int in2_cs = 0, in2_co = 0, Cin2 = 0;
-    // optional fused upsampling (column kernel with the fused head only): channels [0, Cin) are NOT read
-    // from `in` but are F.interpolate(up_src, scale 2, bilinear, align_corners=True) of the dense
-    // half-resolution tensor up_src [b,H/2,W/2,Cin], interpolated inside the kernel straight into the
-    // operand stages (model_repository.py:75: the upsampled tensor is never written)
-    const float *up_src = nullptr;
 };
 
 // Optional fused 1x1 head (convraw.3 + argmax) for the column kernel's epilogue.
@@ -47,7 +42,7 @@ struct HeadDesc {
 int tma_encode(CUtensorMap *m, const void *base, int rank, const cuuint64_t *dims, const cuuint64_t *strides_bytes,
                const cuuint32_t *box, int swizzle_bytes);
 
-// conv mode override for tests: 0 auto, 1 force per-tap kernel, 2 force column kernel
+// conv mode override for tests (pvnet_conv2d_nhwc only): 0 auto, 1 force per-tap kernel, 2 force column kernel
 extern int g_conv_mode;
 bool conv_col_eligible(const ConvDesc &d);
 size_t conv_col_plan_size();
@@ -60,9 +55,6 @@ size_t conv_plan_size();
 int conv_plan_at(const ConvDesc &d, void *plan_storage);
 int conv_launch_at(const void *plan_storage, cudaStream_t s);
 
-int launch_stem(const float *in, const float *w, const float *bias, float *out, int b, int H, int W, int out_cs,
-                int out_co, cudaStream_t s);
-int launch_pack_image(const float *in, float *out, int b, int H, int W, int out_cs, int out_co, cudaStream_t s);
 int launch_s2d_pack(const void *in, int in_is_u8, const float *mean3, const float *std3, float *s2d, float *out, int b,
                     int H, int W, int out_cs, int out_co, cudaStream_t s);
 int launch_maxpool(const float *in, float *out, int b, int H, int W, int C, int in_cs, int in_co, cudaStream_t s);
@@ -72,9 +64,9 @@ int launch_head(const float *in, const float *w, const float *bias, float *out, 
                 int seg_dim, int Cout, int b, int H, int W, int nhwc, cudaStream_t s);
 
 #ifdef __CUDACC__
-// Three-slot interpolation sum with a FIXED rounding sequence (one weight of the window is zero): both
-// upsampling implementations -- k_upsample2x and the column kernel's fused loader -- go through it, so they
-// agree to the last bit whatever contraction the compiler would have picked for `a*b + c*d + e*f`.
+// Three-slot interpolation sum with a FIXED rounding sequence (one weight of the window is zero): k_upsample2x
+// goes through it, so its result does not depend on the contraction the compiler would have picked for
+// `a*b + c*d + e*f`.
 __device__ __forceinline__ float lerp3(float w0, float a, float w1, float b, float w2, float c)
 {
     return __fmaf_rn(w2, c, __fmaf_rn(w1, b, __fmul_rn(w0, a)));

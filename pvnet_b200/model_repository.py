@@ -12,8 +12,8 @@ sm_90a backbone (wgmma implicit-GEMM convs behind include/pvnet_b200.h).
   `cudnn.allow_tf32` default), fp32 accumulation.  Every convolution runs on wgmma with TF32
   operands: the 7x7/2 stem as a 4x4 conv over the 2x2 space-to-depth image, and convraw.3 (1x1 +
   bias) as a register-A wgmma inside convraw.0's epilogue, fused with torch.argmax over the
-  segmentation logits (head weights are rounded to TF32; the fp32 `k_head`/`k_stem` kernels remain as
-  the `pvnet_conv_set_mode(1)` test path).  There is no PyTorch fallback in this mode: if the library
+  segmentation logits (head weights are rounded to TF32).  When seg_dim + ver_dim > 32 the head runs
+  as the separate fp32 `k_head` kernel.  There is no PyTorch fallback in this mode: if the library
   is missing it raises.
 * `nn.DataParallel(net, device_ids=[...])` (the reference's own multi-GPU wrapper,
   tools/train_linemod.py:258, tools/demo.py:160) works: replicas share ONE per-device cache of
@@ -65,7 +65,6 @@ class _NativeEntry:
     def __init__(self, handle, keep, key):
         self.handle, self.keep, self.key = handle, keep, key
         self.packs = 1
-        self.fuse_up = -1            # what pvnet_backbone_set_fused_upsample was last told (-1: library default)
         self._fin = weakref.finalize(self, _NativeEntry._destroy, handle.value)
 
     @staticmethod
@@ -84,7 +83,6 @@ class _NativeState:
         self.entries = {}          # device index -> _NativeEntry
         self.workspaces = {}       # (device index, stream) -> uint8 tensor
         self.pack_count = 0        # how many times weights were folded + packed (tests assert on it)
-        self.fuse_up = -1          # -1 library default (separate launch), 0 separate upsampling launch, 1 fused
 
 
 class Resnet18_8s(nn.Module):
@@ -157,20 +155,6 @@ class Resnet18_8s(nn.Module):
     def native_pack_count(self):
         return self._nat.pack_count
 
-    def set_fused_upsample(self, on=None):
-        """A/B switch of the 1/2 -> 1 upsampling inside convraw.0's loader (pvnet_backbone_set_fused_upsample):
-        None = library default, False / 0 = separate k_upsample2x launch, True / nonzero = fused."""
-        self._nat.fuse_up = -1 if on is None else int(bool(on))
-        return self
-
-    def _sync_options(self, dev):
-        dev = torch.device(dev)
-        ent = self._nat.entries[dev.index if dev.index is not None else torch.cuda.current_device()]
-        if ent.fuse_up != self._nat.fuse_up:
-            _native.check(_native.lib().pvnet_backbone_set_fused_upsample(ent.handle, self._nat.fuse_up),
-                          "pvnet_backbone_set_fused_upsample")
-            ent.fuse_up = self._nat.fuse_up
-
     def _prepare_native(self, device):
         """Fold BatchNorm (eval statistics) into the conv weights, pack them K-major, round
         to TF32, hand the pointers to the C handle.  Redone when any parameter changes; cached per
@@ -212,8 +196,8 @@ class Resnet18_8s(nn.Module):
                 else:
                     w, b = pc.fold_bn(conv.weight, conv_bias=conv.bias)
                 w, b = w.to(device), b.to(device).contiguous()
-                if slot == 0:                         # stem: fp32 [tap][cin][cout]
-                    packed = w.permute(2, 3, 1, 0).reshape(49, 3, 64).contiguous()
+                if slot == 0:                         # stem: a 4x4 conv over the 2x2 space-to-depth image
+                    packed = pc.pack_stem_s2d(w)
                 elif conv_name == "convraw.3":        # head: fp32 [cout][32]
                     packed = pc.round_tf32(w.reshape(w.shape[0], w.shape[1]))   # fused path feeds it to a tf32 MMA
                 elif conv_name == "convraw.0":        # cat[fm(s2dim), image(3)] -> s2dim+8 input channels
@@ -223,15 +207,6 @@ class Resnet18_8s(nn.Module):
                 keep += [packed, b]
                 _native.check(L.pvnet_backbone_set_conv(handle, slot, packed.data_ptr(), b.data_ptr()),
                               f"pvnet_backbone_set_conv({conv_name})")
-            # slot 26: the stem as a 4x4 conv over the 2x2 space-to-depth image (tensor-core path)
-            bn = mods["resnet18_8s.bn1"]
-            w, b = pc.fold_bn(mods["resnet18_8s.conv1"].weight, bn.weight, bn.bias, bn.running_mean, bn.running_var,
-                              bn.eps)
-            w4 = pc.pack_stem_s2d(w.to(device))
-            b = b.to(device).contiguous()
-            keep += [w4, b]
-            _native.check(L.pvnet_backbone_set_conv(handle, len(_SLOTS), w4.data_ptr(), b.data_ptr()),
-                          "pvnet_backbone_set_conv(stem s2d)")
         return _NativeEntry(handle, keep, key)
 
     def forward_native(self, x, with_mask=False, mask_dtype=torch.int64, mean=None, std=None, pixel_major=False):
@@ -257,7 +232,6 @@ class Resnet18_8s(nn.Module):
         dev = x.device
         with torch.cuda.device(dev):
             handle = self._prepare_native(dev)
-            self._sync_options(dev)
             L = _native.lib()
             n = ctypes.c_size_t()
             _native.check(L.pvnet_backbone_workspace_bytes(handle, b, h, w, ctypes.byref(n)),
@@ -289,7 +263,6 @@ class Resnet18_8s(nn.Module):
         dev = x.device
         with torch.cuda.device(dev):
             handle = self._prepare_native(dev)
-            self._sync_options(dev)
             L = _native.lib()
             n = ctypes.c_size_t()
             _native.check(L.pvnet_backbone_workspace_bytes(handle, b, h, w, ctypes.byref(n)), "pvnet_backbone_workspace_bytes")

@@ -62,27 +62,23 @@ class Stage(NamedTuple):
     round_out: bool = True      # output rounded to TF32 (it feeds a tensor-core conv)
 
 
-def stages(dims, seg_dim, ver_dim, b, h, w, auto=True):
-    """The stage table for one configuration.  auto=True is the default convolution mode (tensor-core stem over
-    the space-to-depth image, convraw.0 reading two dense buffers, the head fused into convraw.0 when
-    seg_dim + ver_dim <= 32); auto=False is the per-tap test mode (k_pack_image, k_stem, the interleaved
-    convraw.0 input and k_head)."""
+def stages(dims, seg_dim, ver_dim, b, h, w):
+    """The stage table for one configuration: the tensor-core stem over the space-to-depth image, convraw.0 reading
+    two dense buffers, the head fused into convraw.0 when seg_dim + ver_dim <= 32."""
     fc, s8, s4, s2, raw = dims
     p1 = b * h * w
     g1, g2, g4, g8 = (b, h, w), (b, h // 2, w // 2), (b, h // 4, w // 4), (b, h // 8, w // 8)
-    c1s, c2s, c4s, c8s = s2 + 8, s4 + 64, s8 + 64, fc + 128
+    c2s, c4s, c8s = s4 + 64, s8 + 64, fc + 128
     ctot = seg_dim + ver_dim
-    fused = auto and raw == 32 and ctot <= 32
+    fused = raw == 32 and ctot <= 32
 
     def full(buf, grid, c):
         return Region(buf, 0, grid, c, 0, c)
 
     x = Region("x", 0, g1, 3, 0, 3)
     s2d = full("S2D", g2, 16)
-    if auto:        # two dense buffers: the upsampled features, then the 8-channel image slice
-        up1, img = Region("C1", 0, g1, s2, 0, s2), Region("C1", p1 * s2, g1, 8, 0, 8)
-    else:           # one interleaved [b, h, w, s2 + 8] buffer
-        up1, img = Region("C1", 0, g1, c1s, 0, s2), Region("C1", 0, g1, c1s, s2, 8)
+    # two dense buffers: the upsampled features, then the 8-channel image slice
+    up1, img = Region("C1", 0, g1, s2, 0, s2), Region("C1", p1 * s2, g1, 8, 0, 8)
     x2s, up2 = Region("C2", 0, g2, c2s, s4, 64), Region("C2", 0, g2, c2s, 0, s4)
     x4s, up4 = Region("C4", 0, g4, c4s, s8, 64), Region("C4", 0, g4, c4s, 0, s8)
     x8s, xfc = Region("C8", 0, g8, c8s, fc, 128), Region("C8", 0, g8, c8s, 0, fc)
@@ -105,8 +101,8 @@ def stages(dims, seg_dim, ver_dim, b, h, w, auto=True):
         return Stage(name, "conv", inputs, outp, f"{conv}.0", f"{conv}.1", "leaky", None, round_out)
 
     return [
-        Stage("image: space-to-depth + NHWC slice packing", "pack", (x,), (s2d, img) if auto else (img,)),
-        Stage("stem conv1+bn1+relu", "stem", (s2d,) if auto else (x,), (x2s,), T + "conv1", T + "bn1", "relu"),
+        Stage("image: space-to-depth + NHWC slice packing", "pack", (x,), (s2d, img)),
+        Stage("stem conv1+bn1+relu", "stem", (s2d,), (x2s,), T + "conv1", T + "bn1", "relu"),
         Stage("maxpool 3x3/2", "pool", (x2s,), (P,)),
         block("layer1.0.conv1", "layer1.0", "conv1", P, A1),
         block("layer1.0.conv2", "layer1.0", "conv2", A1, B1, res=P),

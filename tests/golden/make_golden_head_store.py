@@ -59,7 +59,6 @@ def cases():
 def main():
     path = sys.argv[1] if len(sys.argv) > 1 else os.path.join(HERE, "head_store.json")
     net = make_net()
-    net.set_fused_upsample(False)
     rows = []
     for shape, pixel_major, mask_dtype in cases():
         out_sha, mask_sha = digests(net, make_input(shape), pixel_major, mask_dtype)

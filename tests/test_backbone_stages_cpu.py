@@ -33,26 +33,24 @@ def test_layout_matches_library(dims, shape):
     assert list(at) == list(bs.BUFFERS) and sorted(at.values()) == list(at.values())
 
 
-@pytest.mark.parametrize("auto", [True, False], ids=["auto", "per-tap"])
 @pytest.mark.parametrize("seg,ver", [(2, 18), (2, 34), (3, 18)])
-def test_stage_table_matches_library(seg, ver, auto):
+def test_stage_table_matches_library(seg, ver):
     L = _native.lib()
-    table = bs.stages(bs.DEFAULT_DIMS, seg, ver, 2, 64, 96, auto=auto)
+    table = bs.stages(bs.DEFAULT_DIMS, seg, ver, 2, 64, 96)
     assert len(table) == L.pvnet_backbone_num_stages()
     assert [s.name for s in table] == [L.pvnet_backbone_stage_name(i).decode() for i in range(len(table))]
     # exactly one stage, the head when convraw.0 carries it, launches nothing
     idle = [s.name for s in table if not s.writes]
-    assert idle == ([table[-1].name] if auto and seg + ver <= 32 else [])
+    assert idle == ([table[-1].name] if seg + ver <= 32 else [])
 
 
 def test_stage_regions_lie_inside_their_buffers():
     for dims in WIDTHS:
-        for auto in (True, False):
-            b, h, w = 2, 72, 104
-            sizes = bs.buffer_floats(dims, b, h, w)
-            for st in bs.stages(dims, 2, 18, b, h, w, auto=auto):
-                for r in st.reads + st.writes + ((st.res,) if st.res else ()):
-                    if r.buf in sizes:
-                        n, hh, ww = r.grid
-                        assert r.off + n * hh * ww * r.cs <= sizes[r.buf], (st.name, r)
-                        assert 0 <= r.co and r.co + r.cc <= r.cs, (st.name, r)
+        b, h, w = 2, 72, 104
+        sizes = bs.buffer_floats(dims, b, h, w)
+        for st in bs.stages(dims, 2, 18, b, h, w):
+            for r in st.reads + st.writes + ((st.res,) if st.res else ()):
+                if r.buf in sizes:
+                    n, hh, ww = r.grid
+                    assert r.off + n * hh * ww * r.cs <= sizes[r.buf], (st.name, r)
+                    assert 0 <= r.co and r.co + r.cc <= r.cs, (st.name, r)

@@ -47,20 +47,14 @@ def _cudnn_tf32_error(net, x, ref):
     return (t - ref).abs().max().item()
 
 
-@pytest.mark.parametrize("mode", [0, 1], ids=["auto(column+fused head)", "per-tap only"])
 @pytest.mark.parametrize("tag,ver", [("k9", 18), ("k17", 34)])
-def test_native_vs_reference_golden(tag, ver, mode):
-    from pvnet_b200 import conv as pc
+def test_native_vs_reference_golden(tag, ver):
     z = backbone_golden()
-    pc.set_mode(mode)
-    try:
-        net = _net(ver)
-        x = torch.from_numpy(z[tag + "_x"]).to(DEV)
-        with torch.no_grad():
-            seg, v = net(x)
-        torch.cuda.synchronize()
-    finally:
-        pc.set_mode(0)
+    net = _net(ver)
+    x = torch.from_numpy(z[tag + "_x"]).to(DEV)
+    with torch.no_grad():
+        seg, v = net(x)
+    torch.cuda.synchronize()
     gold = torch.from_numpy(np.concatenate([z[tag + "_seg"], z[tag + "_ver"]], 1)).to(DEV)
     e_cudnn = _cudnn_tf32_error(net, x, gold)
     for name, got, ref in (("seg", seg, z[tag + "_seg"]), ("ver", v, z[tag + "_ver"])):
@@ -151,37 +145,3 @@ def test_odd_sizes_multiple_of_8():
                 ref = torch.cat(net._forward_torch(x), 1)
             out = net.forward_native(x)
         assert (out - ref).abs().max().item() <= max(3 * _cudnn_tf32_error(net, x, ref), 3e-3 * ref.abs().max().item())
-
-
-@pytest.mark.parametrize("shape", [(2, 480, 640), (1, 72, 104), (3, 16, 16), (1, 256, 264)], ids=str)
-@pytest.mark.parametrize("pixel_major", [False, True], ids=["nchw", "pixel-major"])
-@pytest.mark.parametrize("mode", [1, 2], ids=["epilogue warps", "dedicated warps"])     # any nonzero mode: the fused form
-def test_fused_upsample_equals_separate_launch(shape, pixel_major, mode):
-    """convraw.0 interpolating its upsampled input itself (pvnet_backbone_set_fused_upsample) against the separate
-    k_upsample2x launch it replaces: the same ATen arithmetic on the same conv2s.0 output, so the two forwards agree to the last bit
-    (partial tiles, image borders and the last-row rounding case of the align_corners scale included)."""
-    b, h, w = shape
-    net = _net(18, seed=11)
-    x = torch.from_numpy(np.random.default_rng(5).standard_normal((b, 3, h, w), dtype=np.float32)).to(DEV)
-    with torch.no_grad():
-        net.set_fused_upsample(False)
-        launches0 = _launches(lambda: net.forward_native(x, with_mask=True, mask_dtype=torch.uint8, pixel_major=pixel_major))
-        sep, msep = net.forward_native(x, with_mask=True, mask_dtype=torch.uint8, pixel_major=pixel_major)
-        sep, msep = sep.clone(), msep.clone()
-        net.set_fused_upsample(mode)
-        launches1 = _launches(lambda: net.forward_native(x, with_mask=True, mask_dtype=torch.uint8, pixel_major=pixel_major))
-        fused, mfused = net.forward_native(x, with_mask=True, mask_dtype=torch.uint8, pixel_major=pixel_major)
-        net.set_fused_upsample(None)
-    torch.cuda.synchronize()
-    assert launches1 == launches0 - 1, "the fused form has one launch less (no 1/2 -> 1 k_upsample2x)"
-    d = (fused - sep).abs().max().item()
-    print(f"\n[fused upsample] {shape} pixel_major={pixel_major}: max abs diff {d:.3e}, launches {launches0} -> {launches1}")
-    assert torch.equal(fused, sep), f"fused and separate upsampling differ by {d:.3e}"
-    assert torch.equal(mfused, msep)
-
-
-def _launches(fn):
-    from pvnet_b200 import _native
-    _native.launch_count_reset()
-    fn()
-    return _native.launch_count()

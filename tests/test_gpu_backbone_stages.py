@@ -34,7 +34,6 @@ import torch
 import torch.nn.functional as F
 
 from pvnet_b200 import _native
-from pvnet_b200 import conv as pc
 from pvnet_b200.model_repository import Resnet18_8s
 from tests import backbone_stages as bs
 from tests.helpers import seeded_state_dict
@@ -51,20 +50,18 @@ WIDE_S2 = (256, 128, 64, 256, 32)        # convraw.0 in = 256 + 8: 33 eight-chan
                                          # with each A stage (resident = 0 in conv_col_plan_at; checked with a
                                          # printf there while writing this test)
 CASES = [
-    # id, ver_dim, seg_dim, decoder widths, (b, h, w), default (auto) convolution mode
-    ("k9-2x64x96", 18, 2, bs.DEFAULT_DIMS, (2, 64, 96), True),
-    ("k9-1x72x104", 18, 2, bs.DEFAULT_DIMS, (1, 72, 104), True),     # 1/8 grid 9 x 13: odd stride-2 parity planes
-    ("k9-3x16x16", 18, 2, bs.DEFAULT_DIMS, (3, 16, 16), True),
-    ("k9-1x256x264", 18, 2, bs.DEFAULT_DIMS, (1, 256, 264), True),
-    ("k9-16x480x640", 18, 2, bs.DEFAULT_DIMS, (16, 480, 640), True),  # bench.py --config 2
-    ("k17-4x480x640", 34, 2, bs.DEFAULT_DIMS, (4, 480, 640), True),   # bench.py --config 5: unfused k_head
-    ("k17-2x48x64", 34, 2, bs.DEFAULT_DIMS, (2, 48, 64), True),
-    ("pertap-k9-2x64x96", 18, 2, bs.DEFAULT_DIMS, (2, 64, 96), False),
-    ("pertap-k9-1x72x104", 18, 2, bs.DEFAULT_DIMS, (1, 72, 104), False),
-    ("pertap-k17-2x64x96", 34, 2, bs.DEFAULT_DIMS, (2, 64, 96), False),
-    ("pertap-k17-1x72x104", 34, 2, bs.DEFAULT_DIMS, (1, 72, 104), False),
-    ("narrow-seg3-1x72x104", 18, 3, NARROW, (1, 72, 104), True),      # head width 21: odd, channel 21 in the padding
-    ("s2dim256-1x72x104", 18, 2, WIDE_S2, (1, 72, 104), True),
+    # id, ver_dim, seg_dim, decoder widths, (b, h, w)
+    ("k9-2x64x96", 18, 2, bs.DEFAULT_DIMS, (2, 64, 96)),
+    ("k9-1x72x104", 18, 2, bs.DEFAULT_DIMS, (1, 72, 104)),     # 1/8 grid 9 x 13: odd stride-2 parity planes
+    ("k9-3x16x16", 18, 2, bs.DEFAULT_DIMS, (3, 16, 16)),
+    ("k9-1x256x264", 18, 2, bs.DEFAULT_DIMS, (1, 256, 264)),
+    ("k9-16x480x640", 18, 2, bs.DEFAULT_DIMS, (16, 480, 640)),  # bench.py --config 2
+    ("k17-4x480x640", 34, 2, bs.DEFAULT_DIMS, (4, 480, 640)),   # bench.py --config 5: unfused k_head
+    ("k17-2x48x64", 34, 2, bs.DEFAULT_DIMS, (2, 48, 64)),
+    ("k17-2x64x96", 34, 2, bs.DEFAULT_DIMS, (2, 64, 96)),
+    ("k17-1x72x104", 34, 2, bs.DEFAULT_DIMS, (1, 72, 104)),
+    ("narrow-seg3-1x72x104", 18, 3, NARROW, (1, 72, 104)),      # head width 21: odd, channel 21 in the padding
+    ("s2dim256-1x72x104", 18, 2, WIDE_S2, (1, 72, 104)),
 ]
 OUTPUT_FORMS = [(False, torch.int64), (True, torch.uint8), (False, torch.uint8), (True, torch.int64)]
 
@@ -149,13 +146,12 @@ class _Guarded:
 
 
 class _StageRun:
-    def __init__(self, net, x, dims, seg, ver, auto):
+    def __init__(self, net, x, dims, seg, ver):
         self.net, self.x, self.dims, self.seg, self.ver = net, x, dims, seg, ver
         self.ctot = seg + ver
         self.b, _, self.h, self.w = x.shape
         self.mods = dict(net.named_modules())
-        self.table = bs.stages(dims, seg, ver, self.b, self.h, self.w, auto=auto)
-        self.auto = auto
+        self.table = bs.stages(dims, seg, ver, self.b, self.h, self.w)
         self.L = _native.lib()
         self.handle = net._prepare_native(DEV)
         n = ctypes.c_size_t()
@@ -229,7 +225,7 @@ class _StageRun:
             left = int((t == (255 if t.dtype == torch.uint8 else -1)).sum())
             assert left == 0, f"{st.name}: {left} elements of {r.buf} [{r.co}, {r.co + r.cc}) never written"
         # (c) TF32 invariant
-        if st.kind == "conv" or (st.kind == "stem" and self.auto):
+        if st.kind in ("conv", "stem"):
             for r in st.reads:
                 assert not (self.region(r) & 0x1FFF).any(), f"{st.name}: tensor-core input {r.buf} is not TF32-valued"
         for r in ws_writes:
@@ -256,11 +252,11 @@ class _StageRun:
     def _conv_input(self, st, n):
         return torch.cat([self.f32(r, n) for r in st.reads], 3)
 
-    def _conv_ref(self, st, inp, n, trunc=True):
+    def _conv_ref(self, st, inp, n):
         conv = self.mods[st.conv]
         w, b = _fold(self.mods, st.conv, st.bn)
         inp = inp[..., :conv.in_channels]
-        y = F.conv2d(_nchw(_trunc(inp) if trunc else inp).double(), (_r(w) if trunc else w).double(), None,
+        y = F.conv2d(_nchw(_trunc(inp)).double(), _r(w).double(), None,
                      conv.stride, conv.padding, conv.dilation)
         y = _nhwc(y) + b.double()
         if st.res is not None:
@@ -275,14 +271,13 @@ class _StageRun:
         rx = _nhwc(_r(self.x[n:n + 1]))
         h2, w2 = self.h // 2, self.w // 2
         img = F.pad(rx, (0, 5))
-        if self.auto:
-            s2d = rx.reshape(1, h2, 2, w2, 2, 3).permute(0, 1, 3, 2, 4, 5).reshape(1, h2, w2, 12)
-            _bits_equal(f"{st.name}: space-to-depth image", self.region(st.writes[0])[n:n + 1], F.pad(s2d, (0, 4)))
+        s2d = rx.reshape(1, h2, 2, w2, 2, 3).permute(0, 1, 3, 2, 4, 5).reshape(1, h2, w2, 12)
+        _bits_equal(f"{st.name}: space-to-depth image", self.region(st.writes[0])[n:n + 1], F.pad(s2d, (0, 4)))
         return _bits_equal(f"{st.name}: image slice", self.region(st.writes[-1])[n:n + 1], img)
 
     def _check_stem(self, st, n):
         x = _nhwc(self.x[n:n + 1])
-        ref = self._conv_ref(st, _r(x) if self.auto else x, n, trunc=self.auto)
+        ref = self._conv_ref(st, _r(x), n)
         return _within(st.name, self.f32(st.writes[0], n), ref, _conv_bound(ref, True))
 
     def _check_pool(self, st, n):
@@ -339,13 +334,11 @@ def _net(ver, seg, dims, seed):
 
 @pytest.mark.parametrize("case", CASES, ids=[c[0] for c in CASES])
 def test_every_stage_against_its_own_layer(case):
-    name, ver, seg, dims, (b, h, w), auto = case
+    name, ver, seg, dims, (b, h, w) = case
     x = torch.from_numpy(np.random.default_rng(h * w + b).standard_normal((b, 3, h, w), dtype=np.float32)).to(DEV)
-    if not auto:
-        pc.set_mode(pc.MODE_PER_TAP)
     try:
         with torch.no_grad():
-            run = _StageRun(_net(ver, seg, dims, seed=21), x, dims, seg, ver, auto)   # a fresh handle per mode
+            run = _StageRun(_net(ver, seg, dims, seed=21), x, dims, seg, ver)
             run.set_outputs(*OUTPUT_FORMS[0])
             checked = 0
             for i, st in enumerate(run.table):
@@ -357,10 +350,8 @@ def test_every_stage_against_its_own_layer(case):
                 else:
                     checked += run.run(i)
     finally:
-        if not auto:
-            pc.set_mode(pc.MODE_AUTO)
         torch.cuda.synchronize()
-    idle = 1 if auto and seg + ver <= 32 else 0        # the head, when convraw.0 carries it
+    idle = 1 if seg + ver <= 32 else 0        # the head, when convraw.0 carries it
     assert checked == run.L.pvnet_backbone_num_stages() - idle
     print(f"\n[stages {name}] worst |err|/bound per stage: " +
           ", ".join(f"{k}: {v:.2g}" for k, v in run.worst.items()))

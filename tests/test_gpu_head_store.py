@@ -1,8 +1,7 @@
 """GPU: convraw.0's fused head stages each tile's output in shared memory and warps that issue no MMAs copy it out.
 Only where the bytes are stored from changed, so every output and mask must be byte-identical to the digests
 recorded before that change (tests/golden/make_golden_head_store.py), in both layouts, with both mask dtypes and at
-shapes with partial tiles; and the fused-upsampling form, whose consumers copy the staged tile out themselves, must
-write the same bytes."""
+shapes with partial tiles."""
 import json
 import os
 
@@ -22,15 +21,10 @@ def net():
     return mg.make_net()
 
 
-@pytest.mark.parametrize("fused_upsample", [False, True], ids=["separate upsample", "fused upsample"])
 @pytest.mark.parametrize("shape,pixel_major,mask_dtype", list(mg.cases()),
                          ids=lambda v: str(v) if not isinstance(v, bool) else ("pixel-major" if v else "nchw"))
-def test_head_store_bytes_unchanged(net, shape, pixel_major, mask_dtype, fused_upsample):
-    net.set_fused_upsample(fused_upsample)
-    try:
-        got = mg.digests(net, mg.make_input(shape), pixel_major, mask_dtype)
-    finally:
-        net.set_fused_upsample(None)
+def test_head_store_bytes_unchanged(net, shape, pixel_major, mask_dtype):
+    got = mg.digests(net, mg.make_input(shape), pixel_major, mask_dtype)
     out_sha, mask_sha = GOLDEN[(tuple(shape), pixel_major, mask_dtype)]
     assert got[0] == out_sha, "head output bytes differ from the recorded digest"
     assert got[1] == mask_sha, "mask bytes differ from the recorded digest"
