@@ -31,6 +31,7 @@
  *   lib/utils/net_utils.py:54-80,329-348                          smooth_l1_loss, compute_precision_recall
  *   tools/train_linemod.py:83-91                                  NetWrapper's cross-entropy (nn.CrossEntropyLoss)
  *   lib/networks/model_repository.py:64-80                        Resnet18_8s.forward
+ *   tools/train_linemod.py:260                                    optim.Adam's step
  * INTEGRATION.md shows the ctypes binding the reference's Python wrapper uses.
  */
 #ifndef PVNET_B200_H_
@@ -596,6 +597,44 @@ PVNET_API int pvnet_head1x1_backward_workspace_bytes(int b, int H, int W, int Ci
 PVNET_API int pvnet_head1x1_backward(const float *dout, const float *y, const float *w, float *dy, float *dw,
                                      float *db, int b, int H, int W, int Cin, int Cout, void *workspace,
                                      size_t workspace_bytes, pvnet_stream_t stream);
+
+/* The optimizer step of tools/train_linemod.py:260 (optim.Adam(net.parameters(), lr=...)): one Adam step over a table
+ * of fp32 tensors, in place, one pass (each element reads p, g, m, v once and writes p, m, v once).
+ *
+ * One table entry, all DEVICE pointers to `numel` dense fp32 elements in one common order, 4-byte aligned (16-byte
+ * aligned entries use float4 accesses, the others scalar ones, with the same bits):
+ *   param       the parameter, updated in place
+ *   grad        its gradient, read only
+ *   exp_avg     the first-moment state m, updated in place
+ *   exp_avg_sq  the second-moment state v, updated in place
+ *   numel       element count; an entry with numel == 0 is skipped and its pointers are not looked at */
+typedef struct pvnet_adam_tensor {
+    void *param;
+    const void *grad;
+    void *exp_avg;
+    void *exp_avg_sq;
+    int64_t numel;
+} pvnet_adam_tensor_t;
+/* pvnet_adam_step:
+ *   tensors       HOST array of n_tensors entries (n_tensors == 0 is a no-op); read before the call returns.  The table
+ *                 travels to the device in the kernel's parameter space, pvnet_adam_chunk_tensors() non-empty entries
+ *                 per launch: no copy, no allocation, no synchronisation, launches on `stream` only.
+ *   lr, beta1, beta2, eps, weight_decay   torch.optim.Adam's hyper-parameters as doubles: lr, eps and weight_decay
+ *                 finite and >= 0, the betas in [0, 1).  weight_decay is the L2 form (added to the gradient).
+ *   step          the step count these tensors reach with this call (1 on the first step), >= 1; one value for the
+ *                 whole table -- tensors at different counts go into different calls.
+ * What is computed is torch.optim.Adam(foreach=False)'s sequence with amsgrad, maximize, capturable and differentiable
+ * off, per element in fp32, every operation rounded to nearest, the scalars prepared on the host in double and
+ * converted to fp32 once (DESIGN.md §19 states it operation by operation; oracle/adam_oracle.py restates it):
+ *   g += p*weight_decay (one FMA; skipped when weight_decay == 0);  m = fma(w1, g - m, m), w1 = float(1 - beta1)
+ *   (for w1 >= 0.5: m = fma(-(g - m), 1 - w1, g));  v = fma(float(1 - beta2), g*g, v*float(beta2));
+ *   denom = sqrt(v) * float(1.0 / sqrt(1 - beta2^step)) + float(eps);
+ *   p = fma(float(-lr / (1 - beta1^step)), m / denom, p).
+ * Bad arguments return PVNET_E_INVALID with a message before anything is launched. */
+PVNET_API int pvnet_adam_step(const pvnet_adam_tensor_t *tensors, int n_tensors, double lr, double beta1, double beta2,
+                              double eps, double weight_decay, int64_t step, pvnet_stream_t stream);
+/* Table entries one launch of pvnet_adam_step carries: a table of n non-empty entries takes ceil(n / this) launches. */
+PVNET_API int pvnet_adam_chunk_tensors(void);
 
 /* Test hook: which convolution kernel pvnet_conv2d_nhwc uses for layers both can run (the backbone
  * always plans automatically).  0 = automatic (persistent weights-resident column kernel for 3x3

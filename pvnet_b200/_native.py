@@ -31,6 +31,12 @@ class BatchNormParams(ctypes.Structure):
 
 c_bn_p = ctypes.POINTER(BatchNormParams)
 
+
+class AdamTensor(ctypes.Structure):
+    """pvnet_adam_tensor_t: one entry of pvnet_adam_step's host table (include/pvnet_b200.h)."""
+    _fields_ = [("param", c_void_p), ("grad", c_void_p), ("exp_avg", c_void_p), ("exp_avg_sq", c_void_p),
+                ("numel", ctypes.c_int64)]
+
 # name -> (restype, argtypes); must list every symbol include/pvnet_b200.h declares
 SIGNATURES = {
     "pvnet_last_error": (ctypes.c_char_p, []),
@@ -128,6 +134,9 @@ SIGNATURES = {
     "pvnet_head1x1_backward_workspace_bytes": (c_int, [c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
     "pvnet_head1x1_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
                                        c_int, c_int, c_int, c_void_p, c_size_t, c_void_p]),
+    "pvnet_adam_step": (c_int, [ctypes.POINTER(AdamTensor), c_int, ctypes.c_double, ctypes.c_double, ctypes.c_double,
+                                ctypes.c_double, ctypes.c_double, ctypes.c_int64, c_void_p]),
+    "pvnet_adam_chunk_tensors": (c_int, []),
     "pvnet_conv_set_mode": (c_int, [c_int]),
     "pvnet_conv_set_multicast": (c_int, [c_int]),
     "pvnet_conv_set_persistent": (c_int, [c_int]),
