@@ -1,6 +1,6 @@
 """Is the vote kernel power-capped when it runs back to back?  The config-4 voting layer (16 images x ~20000 px,
 K=9, 256 + 4096 hypotheses) repeated N times without pauses, nvidia-smi clocks and power sampled beside it;
-then the same calls with a 20 ms idle gap after each.  One JSON line per mode.  PVNET_VOTE_IMPL etc. select the kernel."""
+then the same calls with a 20 ms idle gap after each.  One JSON line per mode."""
 import json
 import os
 import subprocess
@@ -75,8 +75,7 @@ def main():
         w1 = time.time()
         ms = np.array([a.elapsed_time(c) for a, c in evs])
         clk, pw = smi.window(w0 + 0.3 * (w1 - w0), w1)
-        print(json.dumps(dict(mode=mode, field=field_kind, impl=os.environ.get("PVNET_VOTE_IMPL", "default"), form=os.environ.get("PVNET_VOTE_FORM", "default"),
-                              group=os.environ.get("PVNET_VOTE_GROUP", "default"),
+        print(json.dumps(dict(mode=mode, field=field_kind,
                               ms_first5=round(float(np.median(ms[:5])), 4), ms_last_half=round(float(np.median(ms[reps // 2:])), 4),
                               gtests_per_s_last_half=round(tests / float(np.median(ms[reps // 2:])) / 1e6, 1),
                               sm_mhz=clk, power_w=pw, wall_s=round(w1 - w0, 2))), flush=True)

@@ -35,12 +35,11 @@
 // <= (7 + 1/T) ulp on the cosine, and ours): m > B counts, |m| <= B (or NaN) is re-decided by
 // exact_inlier(), the reference's own instruction sequence.  Tests outside the band cannot
 // change sign under either rounding, so the counts are identical to the reference's, at
-// 4.5 issue slots per test (13.6 in round 1's num*|num| - T^2 d^2 form, kept as k_vote for A/B).
+// 4.5 issue slots per test.
 #include "common.cuh"
 
 #include <cfloat>
 #include <cmath>
-#include <cstdlib>
 
 namespace {
 
@@ -54,7 +53,6 @@ constexpr int VT_TILE = 512;      // pixels per staged tile (k_gather's bounding
 constexpr int VT_MAX_B = 1024;    // images per call (prefix table in shared memory)
 constexpr int RF_CHUNKS = 8;      // CTAs per (image, keypoint) in the refit pass
 constexpr int RF_THREADS = 256;
-constexpr float GUARD_EPS = 6e-6f;
 
 struct Strides {
     long long s[5];
@@ -380,161 +378,7 @@ __global__ void __launch_bounds__(256)
     hyp[((size_t)b * vn + vi) * HT + h_off + hi] = out;
 }
 
-// fast-path helpers of the vote kernels
-constexpr int VT_GROUP = 4;       // pixels per guard-band check
-__device__ __forceinline__ uint32_t ptx_smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ float4 lds_f4(uint32_t addr)
-{
-    float4 v;
-    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
-    return v;
-}
-// cnt += (a > b): one FSETP + one predicated IADD (the C form compiled to add + predicated move + move)
-__device__ __forceinline__ void count_if_gt(int &cnt, float a, float b)
-{
-    asm("{\n\t.reg .pred p;\n\tsetp.gt.f32 p, %1, %2;\n\t@p add.s32 %0, %0, 1;\n\t}" : "+r"(cnt) : "f"(a), "f"(b));
-}
-
 // ------------------------------------------------------------------ the vote
-// Persistent CTAs walk items (pixel tile, keypoint, hypothesis group).  Warps are
-// split wh (hypothesis groups of 128) x wp (pixel interleave); each lane owns
-// VT_HPL hypotheses; pixels come from shared memory as one broadcast LDS.128.
-template <int HPL, int TILE>
-__global__ void __launch_bounds__(VT_THREADS, HPL > 4 ? 2 : 4)
-    k_vote(const float *__restrict__ vertex, Strides st, const unsigned *__restrict__ pix,
-           const int *__restrict__ tn_arr, int npx, int nb, int vn, int hn, int HT, int h0, int wh,
-           const float2 *__restrict__ hyp, int *__restrict__ counts, float thresh, float t2, float band)
-{
-    __shared__ float4 tile[TILE];
-    __shared__ int red[VT_WARPS * 32 * HPL];
-    __shared__ int tile_prefix[VT_MAX_B + 1];
-
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    if (tid == 0) {
-        int acc = 0;
-        for (int i = 0; i < nb; ++i) {
-            tile_prefix[i] = acc;
-            acc += (tn_arr[i] + TILE - 1) / TILE;
-        }
-        tile_prefix[nb] = acc;
-    }
-    __syncthreads();
-    const int total_tiles = tile_prefix[nb];
-    const int HC = wh * 32 * HPL;               // hypotheses per item
-    const int hcn = (hn + HC - 1) / HC;
-    const long long n_items = (long long)total_tiles * vn * hcn;
-    const int wp_count = VT_WARPS / wh;
-    const int my_wh = warp % wh, my_wp = warp / wh;
-
-    for (long long it = blockIdx.x; it < n_items; it += gridDim.x) {
-        const int hc = (int)(it % hcn);
-        const long long r = it / hcn;
-        const int k = (int)(r % vn);
-        const int g = (int)(r / vn);
-        int lo = 0, hi = nb;                         // b with tile_prefix[b] <= g < tile_prefix[b+1]
-        while (hi - lo > 1) {
-            const int mid = (lo + hi) >> 1;
-            if (tile_prefix[mid] <= g) lo = mid; else hi = mid;
-        }
-        const int b = lo;
-        const int tn = tn_arr[b];
-        const int t0 = (g - tile_prefix[b]) * TILE;
-        const int len = min(TILE, tn - t0);
-        const long long vbase = (long long)b * st.s[0] + (long long)k * st.s[3];
-
-        // ---- stage: gather this tile's pixels and unit directions
-        for (int i = tid; i < len; i += VT_THREADS) {
-            const unsigned p = __ldg(pix + (size_t)b * npx + t0 + i);
-            const int x = p & 0xffff, y = p >> 16;
-            const long long off = vbase + y * st.s[1] + x * st.s[2];
-            const float nx = __ldg(vertex + off), ny = __ldg(vertex + off + st.s[4]);
-            const float n2 = fmaf(nx, nx, ny * ny);
-            const float rinv = rsqrtf(n2);
-            float ux = nx * rinv, uy = ny * rinv;
-            if (!(n2 > 1e-11f && n2 < 1e30f)) ux = uy = __int_as_float(0x7fc00000);  // -> exact path
-            tile[i] = make_float4((float)x, (float)y, ux, uy);
-        }
-        for (int i = tid; i < HC; i += VT_THREADS) red[i] = 0;
-        __syncthreads();
-
-        // ---- this lane's hypotheses
-        const int hbase = hc * HC + my_wh * (32 * HPL);
-        float hx[HPL], hy[HPL];
-        int cnt[HPL];
-#pragma unroll
-        for (int j = 0; j < HPL; ++j) {
-            const int h = hbase + j * 32 + lane;
-            float2 hp = make_float2(3.0e8f, 3.0e8f);   // padding hypothesis, count discarded
-            if (h < hn) hp = __ldg(hyp + ((size_t)b * vn + k) * HT + h0 + h);
-            hx[j] = hp.x;
-            hy[j] = hp.y;
-            cnt[j] = 0;
-        }
-
-        // ---- sweep the tile, VT_GROUP pixels at a time.  The fast path only counts and ORs one
-        // "some test fell inside the guard band" flag per lane; when any lane of the warp raises it
-        // (rare), the group is re-walked and exactly those tests are re-decided with the reference's
-        // own instruction sequence (they were NOT counted by the fast path: |e| <= bd excludes e > bd).
-        const uint32_t tile_u = ptx_smem_u32(tile);
-        auto sweep = [&](int i0, int n) {           // pixels i0, i0 + wp_count, ... (n of them, n <= VT_GROUP)
-            bool unc = false;
-#pragma unroll
-            for (int u = 0; u < VT_GROUP; ++u) {
-                if (u < n) {
-                    const float4 p = lds_f4(tile_u + (uint32_t)(i0 + u * wp_count) * 16u);
-#pragma unroll
-                    for (int j = 0; j < HPL; ++j) {
-                        const float dx = hx[j] - p.x, dy = hy[j] - p.y;
-                        const float d2 = fmaf(dx, dx, dy * dy);
-                        const float num = fmaf(dx, p.z, dy * p.w);
-                        const float s = num * fabsf(num);
-                        const float e = fmaf(-t2, d2, s);
-                        const float bd = fmaf(band, d2, 4e-12f);
-                        count_if_gt(cnt[j], e, bd);
-                        unc |= !(fabsf(e) > bd);
-                    }
-                }
-            }
-            if (__any_sync(0xffffffffu, unc)) {
-                if (unc) {
-                    for (int u = 0; u < n; ++u) {
-                        const float4 p = tile[i0 + u * wp_count];
-                        const long long off = vbase + (long long)p.y * st.s[1] + (long long)p.x * st.s[2];
-                        const float nx = __ldg(vertex + off), ny = __ldg(vertex + off + st.s[4]);
-#pragma unroll
-                        for (int j = 0; j < HPL; ++j) {
-                            const float dx = hx[j] - p.x, dy = hy[j] - p.y;
-                            const float d2 = fmaf(dx, dx, dy * dy);
-                            const float num = fmaf(dx, p.z, dy * p.w);
-                            const float s = num * fabsf(num);
-                            const float e = fmaf(-t2, d2, s);
-                            const float bd = fmaf(band, d2, 4e-12f);
-                            if (!(fabsf(e) > bd))
-                                cnt[j] += exact_inlier(nx, ny, p.x, p.y, hx[j], hy[j], thresh) ? 1 : 0;
-                        }
-                    }
-                }
-            }
-        };
-        int i = my_wp;
-        for (; i + (VT_GROUP - 1) * wp_count < len; i += VT_GROUP * wp_count) sweep(i, VT_GROUP);
-        if (i < len) sweep(i, (len - i + wp_count - 1) / wp_count);
-
-        // ---- combine the pixel-interleaved warps, then one atomic per hypothesis
-#pragma unroll
-        for (int j = 0; j < HPL; ++j)
-            if (cnt[j]) atomicAdd(&red[my_wh * (32 * HPL) + j * 32 + lane], cnt[j]);
-        __syncthreads();
-        for (int i = tid; i < HC; i += VT_THREADS) {
-            const int h = hc * HC + i;
-            const int v = red[i];
-            if (h < hn && v) atomicAdd(counts + ((size_t)b * vn + k) * HT + h0 + h, v);
-        }
-        __syncthreads();
-    }
-}
-
-// ------------------------------------------------------------------ the vote (round 2)
 // k_vote3: persistent kernel of AUTONOMOUS WARPS.  A warp pulls (image, keypoint, group of 32*HPL hypotheses,
 // pixel segment) items from a ticket counter, keeps its hypotheses and counts in registers for the whole segment,
 // stages 64 pixels at a time from the COMPACT lists (coalesced 4-/8-byte streams) into its private 3 KB of shared
@@ -585,6 +429,7 @@ __device__ __forceinline__ void lds_2x64(uint32_t addr, f32x2 &a, f32x2 &b)
 {
     asm volatile("ld.shared.v2.b64 {%0, %1}, [%2];" : "=l"(a), "=l"(b) : "r"(addr));
 }
+__device__ __forceinline__ uint32_t ptx_smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 constexpr int VT_SUB = 64;        // pixels per staged sub-chunk (2 per lane)
 
 __device__ __forceinline__ float min3_nan_abs(float a, float b, float c)     // min(a, |b|, |c|), NaN if any is
@@ -594,12 +439,13 @@ __device__ __forceinline__ float min3_nan_abs(float a, float b, float c)     // 
     return r;
 }
 
-template <int HPL, int G>
+template <int HPL>
 __global__ void __launch_bounds__(VT_THREADS, HPL > 4 ? 2 : 3)
     k_vote3(const unsigned *__restrict__ pix, const float2 *__restrict__ direct, const int *__restrict__ tn_arr, int npx,
             int cap, int nb, int vn, int hn, int HT, int h0, const float2 *__restrict__ hyp, int *__restrict__ counts,
             unsigned *__restrict__ ticket, float thresh, float sn, float cs, float beta, float b0, int items_per_warp)
 {
+    constexpr int G = 4;                      // pixels per unrolled step of the sweep
     static_assert(G % 2 == 0 && VT_SUB % G == 0, "pixels are swept in pairs");
     // per warp, per pixel 48 bytes: {sx,sx,sy,sy} {ns,ns,cx,cx} {cy,cy,nc,nc}
     __shared__ float4 rec_all[VT_WARPS * 3 * VT_SUB];
@@ -1471,60 +1317,20 @@ VoteConsts vote_consts(float thresh)
     return c;
 }
 
-// score columns [h0, h0 + hn) of the hypothesis tables (counts must be zero there)
-int launch_vote(const float *vertex, const Strides &st, int b, int h, int w, int vn, int hn, int HT, int h0, float thresh,
-                const VoteWs &ws, cudaStream_t s)
+// score columns [h0, h0 + hn) of the hypothesis tables (counts must be zero there).  Above 128 hypotheses per
+// keypoint a lane keeps 8 of them (106 registers, 2 resident CTAs per SM), otherwise 4 (80 registers, 3 CTAs per
+// SM), so that 128 or fewer hypotheses do not leave half of each lane's slots as padding.  The segment length
+// aims at 16 work items per resident warp (config-4 layer: 3.96 / 3.81 / 3.73 / 3.73 ms at 6 / 10 / 16 / 24).
+int launch_vote(int b, int h, int w, int vn, int hn, int HT, int h0, float thresh, const VoteWs &ws, cudaStream_t s)
 {
-    const int npx = h * w;
-    static const int impl = [] {
-        const char *e = getenv("PVNET_VOTE_IMPL");     // tuning knob: 0 = round-1 kernel (k_vote, A/B), 3 = k_vote3 (default)
-        return e ? atoi(e) : 3;
-    }();
-    static const int hpl_env = [] {
-        const char *e = getenv("PVNET_VOTE_HPL");      // tuning knob: hypotheses per lane of k_vote3 (4 or 8)
-        return e ? atoi(e) : 8;
-    }();
-    const int HPL = (impl != 0 && hpl_env == 8 && hn > 128) ? 8 : 4;
-    static const int ctas_per_sm = [] {
-        const char *e = getenv("PVNET_VOTE_CTAS");     // tuning knob: resident vote CTAs per SM
-        return e ? atoi(e) : 0;
-    }();
-    if (impl == 0) {
-        int wh = 1;                                    // hypothesis warps per CTA: 128 hypotheses per warp
-        while (wh < VT_WARPS && wh * 32 * 4 < hn) wh <<= 1;
-        const int HC = wh * 32 * 4;
-        const long long max_items = (long long)b * ((npx + VT_TILE - 1) / VT_TILE) * vn * ((hn + HC - 1) / HC);
-        long long grid = (long long)pvnet::sm_count() * (ctas_per_sm > 0 ? ctas_per_sm : 4);
-        if (grid > max_items) grid = max_items;
-        if (grid < 1) grid = 1;
-        // thresh <= 0 (or NaN) has no squared form: NaN makes every test take the exact path
-        const float t2 = (thresh > 0.f && thresh < 1e18f) ? thresh * thresh : nanf("");
-        const float band = GUARD_EPS * (thresh > 0.f ? thresh * thresh : 1.f);
-        k_vote<4, VT_TILE><<<(unsigned)grid, VT_THREADS, 0, s>>>(vertex, st, ws.pix, ws.tn, npx, b, vn, hn, HT, h0, wh,
-                                                                 ws.hyp, ws.counts, thresh, t2, band);
-        PV_LAUNCHED("k_vote");
-        return PVNET_OK;
-    }
+    const bool hpl8 = hn > 128;
     const VoteConsts vc = vote_consts(thresh);
-    const int per_sm = ctas_per_sm > 0 ? ctas_per_sm : (HPL > 4 ? 2 : 3);
-    const unsigned grid = (unsigned)(pvnet::sm_count() * per_sm);
+    const unsigned grid = (unsigned)(pvnet::sm_count() * (hpl8 ? 2 : 3));
+    const int items_per_warp = 16;
     PV_CUDA(cudaMemsetAsync(ws.ticket, 0, sizeof(unsigned), s));
-    static const int grp = [] {
-        const char *e = getenv("PVNET_VOTE_GROUP");    // tuning knob: pixels per unrolled step of the sweep (4 or 8)
-        return e ? atoi(e) : 4;
-    }();
-    static const int items_pw = [] {
-        const char *e = getenv("PVNET_VOTE_ITEMS");    // tuning knob: work items per resident warp the segment length aims at
-        return e ? atoi(e) : 16;                       // (config-4 layer: 3.96 / 3.81 / 3.73 / 3.73 ms at 6 / 10 / 16 / 24)
-    }();
-#define VOTE3(H_, G_)                                                                                                  \
-    k_vote3<H_, G_><<<grid, VT_THREADS, 0, s>>>(ws.pix, ws.direct, ws.tn, npx, ws.cap, b, vn, hn, HT, h0, ws.hyp, ws.counts, \
-                                                ws.ticket, thresh, vc.sn, vc.cs, vc.beta, vc.b0, items_pw)
-    if (HPL == 8 && grp == 8) VOTE3(8, 8);
-    else if (HPL == 8) VOTE3(8, 4);
-    else if (grp == 8) VOTE3(4, 8);
-    else VOTE3(4, 4);
-#undef VOTE3
+    (hpl8 ? k_vote3<8> : k_vote3<4>)<<<grid, VT_THREADS, 0, s>>>(ws.pix, ws.direct, ws.tn, h * w, ws.cap, b, vn, hn, HT,
+                                                                 h0, ws.hyp, ws.counts, ws.ticket, thresh, vc.sn, vc.cs,
+                                                                 vc.beta, vc.b0, items_per_warp);
     PV_LAUNCHED("k_vote3");
     return PVNET_OK;
 }
@@ -1625,20 +1431,14 @@ int pvnet_ransac_voting_v3(const void *mask, int mask_elem_size, const float *ve
                            size_t workspace_bytes, pvnet_stream_t stream)
 {
     PV_CHECK_ARG(idxs, "null idxs (use pvnet_ransac_voting_pipeline for device-side sampling)");
-    int rc = check_common(mask, mask_elem_size, vertex, (const long long *)vertex_strides, b, h, w, vn, hn);
+    // checked here as well so that an out-of-range hn is reported as such, not as "too many hypotheses"
+    const int rc = check_common(mask, mask_elem_size, vertex, (const long long *)vertex_strides, b, h, w, vn, hn);
     if (rc) return rc;
-    PV_CHECK_ARG(out_pts, "null out_pts");
-    const Strides st = to_strides(vertex_strides);
-    VoteWs ws = carve(workspace, b, h, w, vn, hn);
-    if ((rc = ws_check(ws, workspace, workspace_bytes))) return rc;
-    cudaStream_t s = (cudaStream_t)stream;
-    const Samples sm{idxs, selection, nullptr};
-    if ((rc = launch_pixels(mask, mask_elem_size, PVNET_MASK_NONZERO_BYTE, vertex, st, sm, b, h, w, vn, min_num, max_num, ws, s))) return rc;
-    PV_CUDA(cudaMemsetAsync(ws.counts, 0, sizeof(int) * (size_t)b * vn * hn, s));
-    if ((rc = launch_gen_hyp(sm, RNG_IDXS_V3, b, h, w, vn, hn, hn, 0, ws, s))) return rc;
-    if ((rc = launch_vote(vertex, st, b, h, w, vn, hn, hn, 0, inlier_thresh, ws, s))) return rc;
-    if ((rc = launch_refit(b, h, w, vn, hn, hn, inlier_thresh, ws, out_pts, s))) return rc;
-    return launch_export(ws, b, vn, hn, hn, 0, out_hyp, out_counts, out_tn, s);
+    // the pipeline without covariance and without a device RNG is exactly v3's launch sequence
+    return pvnet_ransac_voting_pipeline(mask, mask_elem_size, PVNET_MASK_NONZERO_BYTE, vertex, vertex_strides, idxs,
+                                        nullptr, selection, nullptr, b, h, w, vn, hn, inlier_thresh, 0, 0, 0, 0.f,
+                                        min_num, max_num, out_pts, nullptr, out_counts, out_hyp, nullptr, nullptr,
+                                        out_tn, workspace, workspace_bytes, stream);
 }
 
 int pvnet_refit_at_points(const void *mask, int mask_elem_size, const float *vertex, const int64_t vertex_strides[5],
@@ -1748,7 +1548,7 @@ int pvnet_vote_cov_with_mean(const void *mask, int mask_elem_size, const float *
     if ((rc = launch_pixels(mask, mask_elem_size, PVNET_MASK_EQUALS_ONE, vertex, st, sm, b, h, w, vn, min_num, max_num, ws, s))) return rc;
     PV_CUDA(cudaMemsetAsync(ws.counts, 0, sizeof(int) * (size_t)b * vn * hnt, s));
     if ((rc = launch_gen_hyp(sm, RNG_IDXS_COV, b, h, w, vn, hnt, hnt, 0, ws, s))) return rc;
-    if ((rc = launch_vote(vertex, st, b, h, w, vn, hnt, hnt, 0, inlier_thresh, ws, s))) return rc;
+    if ((rc = launch_vote(b, h, w, vn, hnt, hnt, 0, inlier_thresh, ws, s))) return rc;
     k_cov<<<b * vn, 256, 0, s>>>(ws.hyp, ws.counts, ws.tn, mean, vn, hnt, hnt, 0, min_hyp_num, out_cov);
     PV_LAUNCHED("k_cov");
     return launch_export(ws, b, vn, hnt, hnt, 0, out_hyp, out_counts, out_tn, s);
@@ -1791,10 +1591,10 @@ int pvnet_ransac_voting_pipeline(const void *mask, int mask_elem_size, int mask_
         if ((rc = launch_gen_hyp(smc, RNG_IDXS_COV, b, h, w, vn, hnt, HT, hn, ws, s))) return rc;
     }
     if (with_cov && cov_inlier_thresh == inlier_thresh) {
-        if ((rc = launch_vote(vertex, st, b, h, w, vn, HT, HT, 0, inlier_thresh, ws, s))) return rc;
+        if ((rc = launch_vote(b, h, w, vn, HT, HT, 0, inlier_thresh, ws, s))) return rc;
     } else {
-        if ((rc = launch_vote(vertex, st, b, h, w, vn, hn, HT, 0, inlier_thresh, ws, s))) return rc;
-        if (with_cov && (rc = launch_vote(vertex, st, b, h, w, vn, hnt, HT, hn, cov_inlier_thresh, ws, s))) return rc;
+        if ((rc = launch_vote(b, h, w, vn, hn, HT, 0, inlier_thresh, ws, s))) return rc;
+        if (with_cov && (rc = launch_vote(b, h, w, vn, hnt, HT, hn, cov_inlier_thresh, ws, s))) return rc;
     }
     if ((rc = launch_refit(b, h, w, vn, hn, HT, inlier_thresh, ws, out_pts, s))) return rc;
     if (with_cov) {

@@ -202,6 +202,19 @@ def _check_injected(idxs, selection, b, h, w, vn, hn_total, device):
     return idxs, selection
 
 
+def _samples(m, mode, rng, idxs, selection, b, h, w, vn, hn, rounds, min_num, max_num):
+    """The samples of a layer scoring `rounds * hn` hypotheses per keypoint: the caller's idxs / selection,
+    the reference's RNG calls replayed on mask `m` (read with `mode`), or one batched draw.  Returns
+    (idxs, selection, fg): fg is the per-image foreground count list when rng="reference" drew, else None."""
+    if idxs is not None:
+        return (*_check_injected(idxs, selection, b, h, w, vn, hn * rounds, m.device), None)
+    if rng == "reference":
+        return _draw_reference(m, mode, b, h, w, vn, hn, rounds, min_num, max_num)
+    if rng == "batched":
+        return (*_draw_batched(b, h, w, vn, hn * rounds, max_num, m.device), None)
+    raise ValueError(f"unknown rng mode {rng!r}")
+
+
 def ransac_voting_layer_v3(mask, vertex, round_hyp_num, inlier_thresh=0.999, confidence=0.99, max_iter=20,
                            min_num=5, max_num=30000, *, idxs=None, selection=None, rng="reference",
                            return_debug=False):
@@ -227,17 +240,11 @@ def ransac_voting_layer_v3(mask, vertex, round_hyp_num, inlier_thresh=0.999, con
     m, esz = _prep_mask(mask, _MASK_NONZERO_BYTE)
     v, strides = _prep_vertex(vertex)
     with torch.cuda.device(dev):
-        if idxs is not None:
-            idxs, selection = _check_injected(idxs, selection, b, h, w, vn, hn, dev)
-        elif rng == "reference":
-            idxs, selection, _ = _draw_reference(m, _MASK_NONZERO_BYTE, b, h, w, vn, hn, 1, min_num, max_num)
-        elif rng == "batched":
-            idxs, selection = _draw_batched(b, h, w, vn, hn, max_num, dev)
-        elif rng == "device":
+        if idxs is None and rng == "device":
             return ransac_voting_pipeline(mask, vertex, hn, inlier_thresh, with_covariance=False, min_num=min_num,
                                           max_num=max_num, rng="device", return_debug=return_debug)
-        else:
-            raise ValueError(f"unknown rng mode {rng!r}")
+        idxs, selection, _ = _samples(m, _MASK_NONZERO_BYTE, rng, idxs, selection, b, h, w, vn, hn, 1, min_num,
+                                      max_num)
         out = torch.empty([b, vn, 2], dtype=torch.float32, device=dev)
         counts = hyp = tn = None
         if return_debug:
@@ -333,14 +340,8 @@ def ransac_voting_layer_v5(mask, vertex, round_hyp_num, inlier_thresh=0.999, con
     m, esz = _prep_mask(mask, _MASK_NONZERO_BYTE)
     v, strides = _prep_vertex(vertex)
     with torch.cuda.device(dev):
-        if idxs is not None:
-            idxs, selection = _check_injected(idxs, selection, b, h, w, vn, hn, dev)
-        elif rng == "reference":
-            idxs, selection, _ = _draw_reference(m, _MASK_NONZERO_BYTE, b, h, w, vn, hn, 1, min_num, max_num)
-        elif rng == "batched":
-            idxs, selection = _draw_batched(b, h, w, vn, hn, max_num, dev)
-        else:
-            raise ValueError(f"unknown rng mode {rng!r}")
+        idxs, selection, _ = _samples(m, _MASK_NONZERO_BYTE, rng, idxs, selection, b, h, w, vn, hn, 1, min_num,
+                                      max_num)
         out = torch.empty([b, vn, 2], dtype=torch.float32, device=dev)
         conf = torch.empty([b, vn], dtype=torch.float32, device=dev)
         ws, ws_bytes = _workspace(b, h, w, vn, hn, dev)
@@ -375,19 +376,14 @@ def estimate_voting_distribution_with_mean(mask, vertex, mean, round_hyp_num=256
     if tuple(mean_c.shape) != (b, vn, 2):
         raise ValueError(f"mean must be [b,vn,2], got {tuple(mean_c.shape)}")
     with torch.cuda.device(dev):
-        if idxs is not None:
-            idxs, selection = _check_injected(idxs, selection, b, h, w, vn, hnt, dev)
-        elif rng == "reference":
-            idxs, selection, fg = _draw_reference(m, _MASK_EQUALS_ONE, b, h, w, vn, hn, rounds, min_num, max_num)
+        idxs, selection, fg = _samples(m, _MASK_EQUALS_ONE, rng, idxs, selection, b, h, w, vn, hn, rounds, min_num,
+                                       max_num)
+        if fg is not None:
             skipped = [f < min_num for f in fg]
             if any(skipped) and not all(skipped) and int(min_hyp_num) != hnt:
                 # the reference's torch.cat at :389 fails on this mix (SURVEY App. C.4)
                 raise RuntimeError("Sizes of tensors must match except in dimension 0 "
                                    f"(skipped images carry {min_hyp_num} rows, others {hnt})")
-        elif rng == "batched":
-            idxs, selection = _draw_batched(b, h, w, vn, hnt, max_num, dev)
-        else:
-            raise ValueError(f"unknown rng mode {rng!r}")
         cov = torch.empty([b, vn, 2, 2], dtype=torch.float32, device=dev)
         counts = hyp = tn = None
         if return_debug:
@@ -449,14 +445,8 @@ def ransac_voting_layer_v4(mask, vertex, round_hyp_num, inlier_thresh=0.99, conf
     m, esz = _prep_mask(mask, _MASK_NONZERO_BYTE)
     v, strides = _prep_vertex(vertex)
     with torch.cuda.device(dev):
-        if idxs is not None:
-            idxs, selection = _check_injected(idxs, selection, b, h, w, vn, hn, dev)
-        elif rng == "reference":
-            idxs, selection, _ = _draw_reference(m, _MASK_NONZERO_BYTE, b, h, w, vn, hn, 1, min_num, max_num)
-        elif rng == "batched":
-            idxs, selection = _draw_batched(b, h, w, vn, hn, max_num, dev)
-        else:
-            raise ValueError(f"unknown rng mode {rng!r}")
+        idxs, selection, _ = _samples(m, _MASK_NONZERO_BYTE, rng, idxs, selection, b, h, w, vn, hn, 1, min_num,
+                                      max_num)
         out = torch.empty([b, vn, 2], dtype=torch.float32, device=dev)
         var = torch.empty([b, vn], dtype=torch.float32, device=dev)
         ws, ws_bytes = _workspace(b, h, w, vn, hn, dev)
@@ -671,14 +661,8 @@ def estimate_voting_distribution(mask, vertex, round_hyp_num=256, min_hyp_num=40
     dev = mask.device
     m = _class_mask(mask, 1)
     with torch.cuda.device(dev):
-        if idxs is not None:
-            idxs, selection = _check_injected(idxs, selection, b, h, w, vn, hn * rounds, dev)
-        elif rng == "reference":
-            idxs, selection, _ = _draw_reference(m, _MASK_NONZERO_BYTE, b, h, w, vn, hn, rounds, min_num, max_num)
-        elif rng == "batched":
-            idxs, selection = _draw_batched(b, h, w, vn, hn * rounds, max_num, dev)
-        else:
-            raise ValueError(f"unknown rng mode {rng!r}")
+        idxs, selection, _ = _samples(m, _MASK_NONZERO_BYTE, rng, idxs, selection, b, h, w, vn, hn, rounds, min_num,
+                                      max_num)
         _, dbg = ransac_voting_layer_v3(m, vertex, hn * rounds, inlier_thresh, min_num=min_num, max_num=max_num,
                                         idxs=idxs, selection=selection, return_debug=True)
         tn = dbg["tn"].float()[:, None, None]
