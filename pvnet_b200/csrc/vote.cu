@@ -196,7 +196,8 @@ __global__ void __launch_bounds__(CH_THREADS) k_chunk_count(const T *__restrict_
 
 // pass 2: kept pixels per chunk.  Equals the foreground count unless the image has
 // more than max_num foreground pixels, in which case pixel i survives iff
-// selection[i] < p (ransac_voting_gpu.py:537-540).  Images below min_num keep nothing.
+// selection[i] < p (ransac_voting_gpu.py:537-540).  Images below min_num keep nothing,
+// even when they are also above max_num: the reference skips them first (:531-534).
 template <typename T>
 __global__ void __launch_bounds__(CH_THREADS)
     k_chunk_kept(const T *__restrict__ mask, int mode, const float *__restrict__ selection,
@@ -210,7 +211,7 @@ __global__ void __launch_bounds__(CH_THREADS)
     block_sum3(tot, z0, z1, scratch);
     const bool skip = tot < min_num;
     const bool have_sel = selection != nullptr || rng_state != nullptr;
-    const bool sub = tot > max_num;
+    const bool sub = tot > max_num && !skip;
     if (!sub || !have_sel) {
         if (threadIdx.x == 0) {
             chunk_kept[b * nchunk + c] = skip ? 0 : chunk_fg[b * nchunk + c];
