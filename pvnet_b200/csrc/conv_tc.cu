@@ -13,10 +13,15 @@
 //                shifted by the tap's (dy,dx)*dilation -- out-of-bounds coordinates are zero-filled
 //                by TMA, which IS the conv padding -- plus one 2-D box {32, BN} of the packed weights
 //                [Cout][tap][Cin]; 128-byte-swizzled K-major tiles in a ring of mbarrier-guarded stages.
+//                With a residual it also loads the residual's {32 ch, TW, TH, 1} boxes into the epilogue's
+//                staging buffers, as the consumers hand them back.
 //   warps 0-7    two consumer warpgroups, 64 pixel rows each: wgmma.m64nBNk8 (tf32 in, fp32
 //                accumulate in registers) straight from the stage, then the epilogue: +bias (+residual)
-//                -> ReLU / LeakyReLU(0.1) -> optional round-to-tf32 -> NHWC output at a channel offset
-//                of a (possibly wider) destination buffer, so torch.cat never happens.
+//                -> ReLU / LeakyReLU(0.1) -> optional round-to-tf32, written 32 channels at a time into
+//                one of two swizzled [128 pixels][32 channels] staging buffers and stored from there by
+//                TMA into the channel slice of a (possibly wider) NHWC destination buffer, so torch.cat
+//                never happens. TMA clips partial tiles. The consumers do not wait for a store to reach
+//                memory: the last slabs of a tile drain under the next tile's MMAs.
 //
 // CTAs are persistent over (M tile, N tile) items (static round-robin; the ring runs on across items,
 // so the producer fetches the next item's operands during the current epilogue), or one item per CTA.
@@ -58,19 +63,29 @@ struct AMaps {
 constexpr int CONV_THREADS = 288;      // two consumer warpgroups + one producer warp
 constexpr int CONV_KC = 32;            // input channels per K-block: one 128-byte swizzled row per pixel
 constexpr int CONV_A_BYTES = 128 * CONV_KC * 4;
+constexpr int CONV_SLAB = 32;          // output channels per epilogue slab: one 128-byte swizzled row per pixel
+constexpr int CONV_SLAB_BYTES = 128 * CONV_SLAB * 4;
+constexpr int CONV_EPI_BAR = 1;        // named barrier of the 256 consumer threads
 
 template <int BN, bool MC>
 __global__ void __launch_bounds__(CONV_THREADS, 1)
-    k_conv_tap(const __grid_constant__ AMaps amaps, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ ConvGeom g,
-               const float *__restrict__ bias, const float *__restrict__ res, float *__restrict__ out)
+    k_conv_tap(const __grid_constant__ AMaps amaps, const __grid_constant__ CUtensorMap tmB,
+               const __grid_constant__ CUtensorMap tmOut, const __grid_constant__ CUtensorMap tmRes,
+               const __grid_constant__ ConvGeom g, const float *__restrict__ bias, const int has_res)
 {
     constexpr int B_BYTES = BN * CONV_KC * 4;
     constexpr int STAGE_BYTES = CONV_A_BYTES + B_BYTES;
+    constexpr int SLABS = BN / CONV_SLAB;
     const int STAGES = g.stages;
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint64_t *full = reinterpret_cast<uint64_t *>(smem + (size_t)STAGES * STAGE_BYTES);
+    // two slab staging buffers behind the ring (a stage is a multiple of 1024 bytes, so they are 1024-byte aligned,
+    // what the 128-byte swizzle needs), then the barriers
+    uint8_t *slab = smem + (size_t)STAGES * STAGE_BYTES;
+    uint64_t *full = reinterpret_cast<uint64_t *>(slab + 2 * CONV_SLAB_BYTES);
     uint64_t *empty = full + STAGES;
+    uint64_t *res_full = empty + STAGES;   // [2] the residual slab has landed in staging buffer i
+    uint64_t *res_free = res_full + 2;     // [2] the last store out of staging buffer i has finished reading it
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int tiles_per_img = g.tiles_x * g.tiles_y;
@@ -91,6 +106,10 @@ __global__ void __launch_bounds__(CONV_THREADS, 1)
             ptx::mbar_init(&full[s], 1);
             ptx::mbar_init(&empty[s], MC ? 16 : 8);    // one arrive per consumer warp (of both CTAs with MC)
         }
+        for (int i = 0; i < 2; ++i) {
+            ptx::mbar_init(&res_full[i], 1);
+            ptx::mbar_init(&res_free[i], 1);
+        }
         ptx::fence_barrier_init();
     }
     __syncthreads();
@@ -98,6 +117,30 @@ __global__ void __launch_bounds__(CONV_THREADS, 1)
 
     if (warp == 8) {
         if (lane == 0) {
+            // Residual slabs ride into the staging buffers on the same thread, between operand loads: slab q of
+            // this CTA's slab sequence goes to buffer q & 1 once the consumers handed that buffer back (res_free),
+            // never blocking the ring. The buffers are free when an item's epilogue ends, so an item's first two
+            // residual slabs are fetched under its K loop and the later ones as its slabs are stored.
+            int r_item = has_res ? unit : g.n_items, r_slab = 0;
+            uint32_t rq = 0;
+            auto poll_res = [&]() {
+                if (r_item >= g.n_items) return;
+                const uint32_t b = rq & 1u;
+                if (!ptx::mbar_test_wait(&res_free[b], ((rq >> 1) & 1u) ^ 1u)) return;
+                int m_tile, n0;
+                item_tile(r_item, m_tile, n0);
+                const int img = m_tile / tiles_per_img;
+                const int trem = m_tile - img * tiles_per_img;
+                const int tyi = trem / g.tiles_x, txi = trem - tyi * g.tiles_x;
+                ptx::mbar_arrive_expect_tx(&res_full[b], (uint32_t)CONV_SLAB_BYTES);
+                ptx::tma_load_4d(slab + b * CONV_SLAB_BYTES, &tmRes, &res_full[b], n0 + r_slab * CONV_SLAB, txi * g.TW,
+                                 tyi * g.TH, img);
+                ++rq;
+                if (++r_slab == SLABS) {
+                    r_slab = 0;
+                    r_item += nunits;
+                }
+            };
             int s = 0;
             uint32_t ph = 0;
             for (int item = unit; item < g.n_items; item += nunits) {
@@ -109,7 +152,10 @@ __global__ void __launch_bounds__(CONV_THREADS, 1)
                 const int y0 = tyi * g.TH, x0 = txi * g.TW;
                 for (int tap = 0; tap < g.taps; ++tap)
                     for (int cc = 0; cc < g.cin_chunks; ++cc) {
-                        ptx::mbar_wait(&empty[s], ph ^ 1u);
+                        poll_res();
+                        // with residual slabs pending, look at the ring without being parked in try_wait
+                        while (!(has_res ? ptx::mbar_test_wait(&empty[s], ph ^ 1u) : ptx::mbar_try_wait(&empty[s], ph ^ 1u)))
+                            poll_res();
                         ptx::mbar_arrive_expect_tx(&full[s], (uint32_t)STAGE_BYTES);
                         uint8_t *sa = smem + (size_t)s * STAGE_BYTES;
                         ptx::tma_load_4d(sa, &amaps.m[g.tap_map[tap]], &full[s], cc * CONV_KC, x0 + g.tap_ox[tap],
@@ -125,6 +171,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 1)
                         }
                     }
             }
+            while (r_item < g.n_items) poll_res();
         }
     } else {
         // consumer warpgroup wg: pixel rows [64 wg, 64 wg + 64) of the tile
@@ -136,7 +183,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 1)
             if (MC) ptx::mbar_arrive_cluster(&empty[st], crank ^ 1u);
         };
         int s = 0;
-        uint32_t ph = 0;
+        uint32_t ph = 0, sq = 0;            // sq: slabs this CTA has stored so far
         for (int item = unit; item < g.n_items; item += nunits) {
             float acc[BN / 2];
 #pragma unroll
@@ -166,61 +213,75 @@ __global__ void __launch_bounds__(CONV_THREADS, 1)
             ptx::fence_regs(acc);
             if (lane == 0) release(prev);
 
+            // Epilogue, one 32-channel slab at a time through two staging buffers [128 pixels][32 channels], laid
+            // out as TMA lays out the A tile (pixel m = row, 128-byte swizzle: 16-byte chunk c of row m sits at chunk
+            // c ^ (m & 7)). A thread owns pixels m = 64 wg + 16 wq + g8 (+ 8) and, per 8-channel block jj of the slab,
+            // channels 8 jj + 2 t4 (+ 1): the 8 bytes at chunk (2 jj + (t4 >> 1)) ^ g8, offset 8 (t4 & 1). Of one
+            // warp's st.shared.v2 the eight rows g8 turn a row's two chunks into all eight chunks of the 128-byte
+            // bank line, each hit by exactly two rows -- the two wavefronts that 256 bytes need anyway; unswizzled,
+            // the eight rows would pile onto the same two chunks. Thread 0 then stores the slab with one TMA box
+            // {32, TW, TH, 1}; TMA clips what lies outside the tensor (partial tiles), and the consumers go on
+            // without waiting for the store to reach memory.
+            //
+            // Buffer q & 1 is rewritten for slab q only after the store of slab q - 2 has finished reading it: thread 0
+            // learns that from cp.async.bulk.wait_group.read and publishes it -- with a residual by arriving on
+            // res_free, on which the producer waits before it loads the residual slab there (res_full then releases
+            // the consumers); without one by the named barrier ahead of the writes. A residual slab is always loaded
+            // before the same slab is stored and no other slab touches those addresses, so each address sees its
+            // read before its write, as with the direct epilogue, when `res` and `out` are the same slice. Pixels
+            // outside the tensor read zeros and are clipped on the store.
             int m_tile, n0;
             item_tile(item, m_tile, n0);
             const int img = m_tile / tiles_per_img;
             const int trem = m_tile - img * tiles_per_img;
             const int tyi = trem / g.tiles_x, txi = trem - tyi * g.tiles_x;
-            // this thread's two pixel rows (g8 and g8 + 8 of its warp's 16)
-            bool ok[2];
-            float *optr[2];
-            const float *rptr[2];
+            const uint32_t row_off = (uint32_t)((wg * 64 + wq * 16 + g8) * 128 + (t4 & 1) * 8);
+            const uint32_t swz = (uint32_t)(((t4 >> 1) ^ g8) << 4);
+            const uint32_t slab_u = ptx::smem_u32(slab);
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int m = wg * 64 + wq * 16 + g8 + 8 * h;
-                const int y = tyi * g.TH + m / g.TW, x = txi * g.TW + m % g.TW;
-                ok[h] = y < g.Ho && x < g.Wo;
-                const size_t pix = ok[h] ? ((size_t)img * g.Ho + y) * g.Wo + x : 0;
-                optr[h] = out + pix * g.out_cs + g.out_co + n0;
-                rptr[h] = res ? res + pix * g.res_cs + g.res_co + n0 : nullptr;
-            }
-            // groups of JC 8-channel blocks: every bias and residual load of a group is issued before its
-            // arithmetic, so the epilogue waits for one load latency per group rather than one per block.
-            // With 288 threads the 64K registers split over four sub-partitions allow 168 per thread; BN = 256
-            // holds 128 accumulators, so its groups are 2 blocks to stay clear of spills.
-            constexpr int JC = BN == 256 ? 2 : (BN / 8 < 8 ? BN / 8 : 8);
+            for (int j = 0; j < SLABS; ++j, ++sq) {
+                const uint32_t b = sq & 1u;
+                const uint32_t base = slab_u + b * (uint32_t)CONV_SLAB_BYTES + row_off;
+                float2 bv[4];
 #pragma unroll
-            for (int j0 = 0; j0 < BN / 8; j0 += JC) {
-                float2 bv[JC], rv[2][JC];
+                for (int jj = 0; jj < 4; ++jj)
+                    bv[jj] = __ldg(reinterpret_cast<const float2 *>(bias + n0 + CONV_SLAB * j + 8 * jj + 2 * t4));
+                if (has_res) ptx::mbar_wait(&res_full[b], (sq >> 1) & 1u);
+                else ptx::named_bar_sync(CONV_EPI_BAR, 256);
 #pragma unroll
-                for (int jj = 0; jj < JC; ++jj)
-                    bv[jj] = __ldg(reinterpret_cast<const float2 *>(bias + n0 + 8 * (j0 + jj) + 2 * t4));
-                if (res) {
+                for (int jj = 0; jj < 4; ++jj)
 #pragma unroll
-                    for (int h = 0; h < 2; ++h)
-#pragma unroll
-                        for (int jj = 0; jj < JC; ++jj)
-                            rv[h][jj] = ok[h] ? __ldg(reinterpret_cast<const float2 *>(rptr[h] + 8 * (j0 + jj) + 2 * t4))
-                                              : make_float2(0.f, 0.f);
-                }
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    if (!ok[h]) continue;
-#pragma unroll
-                    for (int jj = 0; jj < JC; ++jj) {
-                        const int j = j0 + jj;
-                        float2 v = make_float2(acc[4 * j + 2 * h] + bv[jj].x, acc[4 * j + 2 * h + 1] + bv[jj].y);
-                        if (res) {
-                            v.x += rv[h][jj].x;
-                            v.y += rv[h][jj].y;
+                    for (int h = 0; h < 2; ++h) {
+                        const uint32_t addr = base + (uint32_t)(h * 8 * 128) + (swz ^ (uint32_t)(32 * jj));
+                        const int a = 4 * (4 * j + jj) + 2 * h;
+                        float2 v = make_float2(acc[a] + bv[jj].x, acc[a + 1] + bv[jj].y);
+                        if (has_res) {
+                            const float2 r = ptx::lds64(addr);
+                            v.x += r.x;
+                            v.y += r.y;
                         }
                         v.x = epi_act(v.x, g.act, g.round_out);
                         v.y = epi_act(v.y, g.act, g.round_out);
-                        *reinterpret_cast<float2 *>(optr[h] + 8 * j + 2 * t4) = v;
+                        ptx::sts64(addr, v);
+                    }
+                ptx::fence_proxy_async();
+                ptx::named_bar_sync(CONV_EPI_BAR, 256);
+                if (threadIdx.x == 0) {
+                    ptx::tma_store_4d(&tmOut, slab + b * CONV_SLAB_BYTES, n0 + CONV_SLAB * j, txi * g.TW, tyi * g.TH, img);
+                    ptx::tma_store_commit();
+                    // all but this store have finished reading (the item's last slab: this one too, so that both
+                    // buffers are free for the next item's first slabs while its K loop runs)
+                    if (j == SLABS - 1) ptx::tma_store_wait_read();
+                    else ptx::tma_store_wait_read1();
+                    if (has_res) {
+                        if (j > 0) ptx::mbar_arrive(&res_free[b ^ 1u]);
+                        if (j == SLABS - 1) ptx::mbar_arrive(&res_free[b]);
                     }
                 }
+                __syncwarp();       // warp 0 is whole again for the aligned barriers and MMAs that follow
             }
         }
+        if (threadIdx.x == 0) ptx::tma_store_wait_all();   // the stores have reached memory before the kernel ends
     }
     if (MC) ptx::cluster_sync();                      // no CTA exits while its peer may still write into it
 }
@@ -280,12 +341,13 @@ int tma_encode(CUtensorMap *m, const void *base, int rank, const cuuint64_t *dim
 struct ConvPlan {
     AMaps amaps;
     CUtensorMap tmB;
+    CUtensorMap tmOut, tmRes;   // destination and residual channel slices, boxes {32, TW, TH, 1}
     ConvGeom g;
     dim3 grid;
     size_t smem;
     int mc;
-    const float *bias, *res;
-    float *out;
+    const float *bias;
+    int has_res;
 };
 
 // 1: CTAs persistent over the items (grid = one CTA per SM); 0: one item per CTA (pvnet_conv_set_persistent)
@@ -386,12 +448,32 @@ int conv_plan(const ConvDesc &d, ConvPlan *p)
         int rc = tma_encode(&p->tmB, d.w, 2, dims, strides, box, swz);
         if (rc) return rc;
     }
-    // ring: as many stages as fit (at most 8) in the 227 KB a block may use
+    // destination and residual: the channel slice [co, co + Cout) of an NHWC buffer, stored / loaded one
+    // {32 channels, TW, TH, 1 image} box per slab. The argument checks above (16-byte aligned pointers, strides and
+    // offsets multiples of 4 floats) are what these maps need.
+    {
+        cuuint64_t dims[4] = {(cuuint64_t)d.Cout, (cuuint64_t)g.Wo, (cuuint64_t)g.Ho, (cuuint64_t)d.b};
+        cuuint32_t box[4] = {(cuuint32_t)CONV_SLAB, (cuuint32_t)g.TW, (cuuint32_t)g.TH, 1};
+        cuuint64_t ostr[3] = {(cuuint64_t)d.out_cs * 4, (cuuint64_t)g.Wo * d.out_cs * 4,
+                              (cuuint64_t)g.Ho * g.Wo * d.out_cs * 4};
+        int rc = tma_encode(&p->tmOut, d.out + d.out_co, 4, dims, ostr, box, CONV_SLAB * 4);
+        if (rc) return rc;
+        p->tmRes = p->tmOut;
+        if (d.res) {
+            PV_CHECK_ARG((uintptr_t)d.res % 16 == 0, "conv: pointers must be 16-byte aligned");
+            cuuint64_t rstr[3] = {(cuuint64_t)d.res_cs * 4, (cuuint64_t)g.Wo * d.res_cs * 4,
+                                  (cuuint64_t)g.Ho * g.Wo * d.res_cs * 4};
+            rc = tma_encode(&p->tmRes, d.res + d.res_co, 4, dims, rstr, box, CONV_SLAB * 4);
+            if (rc) return rc;
+        }
+    }
+    // ring: as many stages as fit (at most 8) in the 227 KB a block may use, beside the epilogue's two 16 KB slab
+    // buffers: 4 stages at BN 256 and 8 at BN 64 and 32, as without the buffers; BN 128 has 6 where 7 would fit
     const size_t stage_b = (size_t)CONV_A_BYTES + (size_t)g.BN * kc * 4;
-    int st = (int)((227 * 1024 - 1024 - 256) / stage_b);
+    int st = (int)((227 * 1024 - 1024 - 256 - 2 * CONV_SLAB_BYTES) / stage_b);
     if (st > 8) st = 8;
     g.stages = st;
-    p->smem = 1024 + (size_t)st * stage_b + 256;
+    p->smem = 1024 + (size_t)st * stage_b + 2 * CONV_SLAB_BYTES + 256;
     // items: (M tile, N tile), or with MC (M tile pair, N tile) run by a two-CTA cluster
     const int m_units = p->mc ? (g.total_m_tiles + 1) / 2 : g.total_m_tiles;
     g.n_items = m_units * (d.Cout / g.BN);
@@ -399,8 +481,7 @@ int conv_plan(const ConvDesc &d, ConvPlan *p)
     if (units > g.n_items) units = g.n_items;
     p->grid = dim3((unsigned)(units * (p->mc ? 2 : 1)));
     p->bias = d.bias;
-    p->res = d.res;
-    p->out = d.out;
+    p->has_res = d.res != nullptr;
     return PVNET_OK;
 }
 
@@ -421,7 +502,7 @@ int conv_launch_t(const ConvPlan &p, cudaStream_t s)
     attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr;
     cfg.numAttrs = MC ? 1 : 0;
-    PV_CUDA(cudaLaunchKernelEx(&cfg, k_conv_tap<BN, MC>, p.amaps, p.tmB, p.g, p.bias, p.res, p.out));
+    PV_CUDA(cudaLaunchKernelEx(&cfg, k_conv_tap<BN, MC>, p.amaps, p.tmB, p.tmOut, p.tmRes, p.g, p.bias, p.has_res));
     PV_LAUNCHED("k_conv_tap");
     return PVNET_OK;
 }

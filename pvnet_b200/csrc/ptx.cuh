@@ -61,6 +61,22 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t *bar, uint32_t parity)
         : "memory");
     return ok != 0;
 }
+// one look at the phase, never suspending the thread (try_wait may park it for a while): for a thread that polls
+// a barrier between other duties
+__device__ __forceinline__ bool mbar_test_wait(uint64_t *bar, uint32_t parity)
+{
+    uint32_t ok;
+    asm volatile(
+        "{\n\t"
+        ".reg .pred P1;\n\t"
+        "mbarrier.test_wait.parity.shared::cta.b64 P1, [%1], %2;\n\t"
+        "selp.b32 %0, 1, 0, P1;\n\t"
+        "}\n"
+        : "=r"(ok)
+        : "r"(smem_u32(bar)), "r"(parity)
+        : "memory");
+    return ok != 0;
+}
 __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity)
 {
     while (!mbar_try_wait(bar, parity)) {
@@ -117,6 +133,12 @@ __device__ __forceinline__ float4 lds128(uint32_t addr)
 __device__ __forceinline__ void sts64(uint32_t addr, float2 v)
 {
     asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(v.x), "f"(v.y) : "memory");
+}
+__device__ __forceinline__ float2 lds64(uint32_t addr)
+{
+    float2 v;
+    asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr) : "memory");
+    return v;
 }
 __device__ __forceinline__ void sts32(uint32_t addr, float v) { asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(v) : "memory"); }
 __device__ __forceinline__ float lds32(uint32_t addr)
