@@ -69,7 +69,10 @@ enum {
 
 PVNET_API const char *pvnet_last_error(void);
 /* ABI version.  2: backbone slot 0 holds the stem in its space-to-depth packing (was [7*7][3][64]) and the
- * backbone has 26 conv slots. */
+ * backbone has 26 conv slots.  3: pvnet_backbone_create_trunk builds a backbone from a trunk description
+ * (BasicBlock or Bottleneck, blocks per stage; Resnet34_8s, Resnet50_8s), whose conv-slot count and stage list are
+ * per handle (pvnet_backbone_handle_num_convs / _num_stages / _stage_name); raw_dim may be 64 there; the
+ * train-mode BatchNorm's block-tail forms (1, 2) take up to 2048 channels. */
 PVNET_API int pvnet_version(void);
 
 /* ------------------------------------------------------------------ voting layer */
@@ -506,7 +509,8 @@ PVNET_API int pvnet_upsample2x_backward_nhwc(const float *dout, int dout_cs, int
 
 /* Train-mode BatchNorm2d fused with its activation and the residual add of a BasicBlock (lib/networks/resnet.py
  * BasicBlock.forward, model_repository.py's Conv2d -> BatchNorm2d -> ReLU / LeakyReLU(0.1) sequences), forward and
- * backward, on dense NHWC fp32 tensors of npix = b*H*W pixels and C channels (C a multiple of 4, up to 1024;
+ * backward, on dense NHWC fp32 tensors of npix = b*H*W pixels and C channels (C a multiple of 4, up to 1024 for
+ * form 0 and up to 2048 for forms 1 and 2, the Bottleneck tails of Resnet50_8s's layer4;
  * pointers 16-byte aligned; element offsets are 64-bit).
  *
  *   form 0  y = act(bn(x))               act 0 none, 1 ReLU, 2 LeakyReLU(0.1)
@@ -648,7 +652,8 @@ PVNET_API int pvnet_conv_set_multicast(int on);
  * output tiles, continuous TMA ring); 0 = one tile per CTA. */
 PVNET_API int pvnet_conv_set_persistent(int on);
 
-/* Resnet18_8s.forward (lib/networks/model_repository.py:64-80), eval mode, whole batch.
+/* Resnet18_8s.forward (lib/networks/model_repository.py:64-80), eval mode, whole batch (Resnet34_8s / Resnet50_8s:
+ * pvnet_backbone_create_trunk below; the same calls with the handle's own slots and stages).
  *
  * The handle is a host-side table of per-convolution weight pointers plus cached tensor
  * maps; it owns no device memory.  Weights are DEVICE pointers owned by the caller and
@@ -673,8 +678,21 @@ PVNET_API int pvnet_conv_set_persistent(int on);
 typedef struct pvnet_backbone pvnet_backbone_t;
 PVNET_API int pvnet_backbone_create(int ver_dim, int seg_dim, int fcdim, int s8dim, int s4dim, int s2dim,
                                     int raw_dim, pvnet_backbone_t **out);
-PVNET_API void pvnet_backbone_destroy(pvnet_backbone_t *m);
+/* The Resnet18_8s plan's conv-slot count (26); a handle's own: pvnet_backbone_handle_num_convs. */
 PVNET_API int pvnet_backbone_num_convs(void);
+
+/* A backbone over any trunk of lib/networks/resnet.py's ResNet(block, blocks, output_stride=8) under the
+ * Resnet*_8s decoder (model_repository.py): block_kind PVNET_BLOCK_BASIC (resnet18 / resnet34) or
+ * PVNET_BLOCK_BOTTLENECK (resnet50, expansion 4), blocks[4] the blocks per stage (each in [1,64]), raw_dim 32 or
+ * 64, the other widths as pvnet_backbone_create takes them.  The conv slots follow the same pattern: slot 0 the
+ * stem; then per block conv1, (conv2,) the downsample (first block of a stage that has one), and the conv whose
+ * epilogue adds the skip (BasicBlock conv2, Bottleneck conv3); then fc.0, conv8s.0, conv4s.0, conv2s.0, convraw.0
+ * and convraw.3 as [seg_dim+ver_dim][raw_dim].  The 2-2-2-2 BasicBlock trunk gives pvnet_backbone_create's plan. */
+enum { PVNET_BLOCK_BASIC = 0, PVNET_BLOCK_BOTTLENECK = 1 };
+PVNET_API int pvnet_backbone_create_trunk(int block_kind, const int *blocks, int ver_dim, int seg_dim, int fcdim,
+                                          int s8dim, int s4dim, int s2dim, int raw_dim, pvnet_backbone_t **out);
+PVNET_API int pvnet_backbone_handle_num_convs(const pvnet_backbone_t *m);   /* -1 for a null handle */
+PVNET_API void pvnet_backbone_destroy(pvnet_backbone_t *m);
 PVNET_API int pvnet_backbone_set_conv(pvnet_backbone_t *m, int slot, const float *w_packed, const float *bias);
 /* Output layout of the following forward calls on this handle: 0 (default) = out [b,C,h,w], the
  * reference's NCHW tensor whose channel slices are seg_pred / ver_pred (model_repository.py:77-78);
@@ -709,9 +727,13 @@ PVNET_API int pvnet_jpeg_decode_batch(pvnet_jpeg_decoder_t *d, const uint8_t *co
                                       int b, int h, int w, uint8_t *out_hwc, pvnet_stream_t stream);
 
 /* The forward pass is an ordered list of single-kernel stages; these run/describe one of
- * them with the same arguments (per-layer timing in bench.py, layer-wise parity tests). */
+ * them with the same arguments (per-layer timing in bench.py, layer-wise parity tests).
+ * pvnet_backbone_num_stages / _stage_name describe the Resnet18_8s plan, the _handle_ forms the handle's own
+ * (its stage indices are what pvnet_backbone_run_stage takes; the name is valid while the handle lives). */
 PVNET_API int pvnet_backbone_num_stages(void);
 PVNET_API const char *pvnet_backbone_stage_name(int stage);
+PVNET_API int pvnet_backbone_handle_num_stages(const pvnet_backbone_t *m);  /* -1 for a null handle */
+PVNET_API const char *pvnet_backbone_handle_stage_name(const pvnet_backbone_t *m, int stage);
 PVNET_API int pvnet_backbone_run_stage(pvnet_backbone_t *m, int stage, const float *image_nchw, int b, int h, int w,
                                        float *out_nchw, void *mask_out, int mask_elem_size,
                                        void *workspace, size_t workspace_bytes, pvnet_stream_t stream);

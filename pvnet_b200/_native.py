@@ -141,8 +141,11 @@ SIGNATURES = {
     "pvnet_conv_set_multicast": (c_int, [c_int]),
     "pvnet_conv_set_persistent": (c_int, [c_int]),
     "pvnet_backbone_create": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_void_p)]),
+    "pvnet_backbone_create_trunk": (c_int, [c_int, ctypes.POINTER(c_int), c_int, c_int, c_int, c_int, c_int, c_int,
+                                            c_int, ctypes.POINTER(c_void_p)]),
     "pvnet_backbone_destroy": (None, [c_void_p]),
     "pvnet_backbone_num_convs": (c_int, []),
+    "pvnet_backbone_handle_num_convs": (c_int, [c_void_p]),
     "pvnet_backbone_set_conv": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
     "pvnet_backbone_set_output_layout": (c_int, [c_void_p, c_int]),
     "pvnet_backbone_workspace_bytes": (c_int, [c_void_p, c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
@@ -157,6 +160,8 @@ SIGNATURES = {
                                         c_int, c_void_p, c_void_p]),
     "pvnet_backbone_num_stages": (c_int, []),
     "pvnet_backbone_stage_name": (ctypes.c_char_p, [c_int]),
+    "pvnet_backbone_handle_num_stages": (c_int, [c_void_p]),
+    "pvnet_backbone_handle_stage_name": (ctypes.c_char_p, [c_void_p, c_int]),
     "pvnet_backbone_run_stage": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int,
                                          c_void_p, c_size_t, c_void_p]),
 }

@@ -696,28 +696,29 @@ int pvnet_stem_s2d_nhwc(const void *image, int image_is_u8, const float *mean3, 
 namespace pvnet {
 
 // ------------------------------------------------------------------ head
-// convraw.3: 1x1 conv raw_dim(=32) -> seg_dim+ver_dim with bias (model_repository.py:57), in
+// convraw.3: 1x1 conv raw_dim (CIN = 32 or 64) -> seg_dim+ver_dim with bias (model_repository.py:57), in
 // exact fp32, fused with torch.argmax(seg_pred,1) (tools/demo.py:52; first maximum wins).
-// in NHWC [b,H,W,32] -> out NCHW [b,Cout,H,W]; mask int64 [b,H,W] (or u8) optional.
+// in NHWC [b,H,W,CIN] -> out NCHW [b,Cout,H,W]; mask int64 [b,H,W] (or u8) optional.
 constexpr int HEAD_MAX_COUT = 64;
+template <int CIN>
 __global__ void __launch_bounds__(256)
-    k_head(const float *__restrict__ in, const float *__restrict__ w /*[Cout][32]*/, const float *__restrict__ bias,
+    k_head(const float *__restrict__ in, const float *__restrict__ w /*[Cout][CIN]*/, const float *__restrict__ bias,
            float *__restrict__ out, void *__restrict__ mask, int mask_esz, int seg_dim, int Cout, int npix,
            long long total, int nhwc)
 {
-    __shared__ float sw[HEAD_MAX_COUT * 32];
+    __shared__ float sw[HEAD_MAX_COUT * CIN];
     __shared__ float sb[HEAD_MAX_COUT];
-    for (int i = threadIdx.x; i < Cout * 32; i += 256) sw[i] = w[i];
+    for (int i = threadIdx.x; i < Cout * CIN; i += 256) sw[i] = w[i];
     for (int i = threadIdx.x; i < Cout; i += 256) sb[i] = bias[i];
     __syncthreads();
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= total) return;
     const long long n = i / npix;
     const long long p = i - n * npix;
-    float v[32];
-    const float4 *src = reinterpret_cast<const float4 *>(in + i * 32);
+    float v[CIN];
+    const float4 *src = reinterpret_cast<const float4 *>(in + i * CIN);
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
+    for (int j = 0; j < CIN / 4; ++j) {
         const float4 t = __ldg(src + j);
         v[4 * j] = t.x;
         v[4 * j + 1] = t.y;
@@ -730,9 +731,9 @@ __global__ void __launch_bounds__(256)
     const long long ostride = nhwc ? 1 : npix;
     for (int co = 0; co < Cout; ++co) {
         float acc = sb[co];
-        const float *wr = sw + co * 32;
+        const float *wr = sw + co * CIN;
 #pragma unroll
-        for (int j = 0; j < 32; ++j) acc = fmaf(v[j], wr[j], acc);
+        for (int j = 0; j < CIN; ++j) acc = fmaf(v[j], wr[j], acc);
         o[(long long)co * ostride] = acc;
         if (co < seg_dim && acc > best) {
             best = acc;
@@ -747,14 +748,18 @@ __global__ void __launch_bounds__(256)
     }
 }
 
-int launch_head(const float *in, const float *w, const float *bias, float *out, void *mask, int mask_esz, int seg_dim,
-                int Cout, int b, int H, int W, int nhwc, cudaStream_t s)
+int launch_head(const float *in, int cin, const float *w, const float *bias, float *out, void *mask, int mask_esz,
+                int seg_dim, int Cout, int b, int H, int W, int nhwc, cudaStream_t s)
 {
     PV_CHECK_ARG(Cout >= 1 && Cout <= HEAD_MAX_COUT, "head: %d output channels unsupported (max %d)", Cout,
                  HEAD_MAX_COUT);
+    PV_CHECK_ARG(cin == 32 || cin == 64, "head: %d input channels unsupported (32 or 64)", cin);
     const long long total = (long long)b * H * W;
-    k_head<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(in, w, bias, out, mask, mask_esz, seg_dim, Cout, H * W,
-                                                          total, nhwc);
+    const unsigned grid = (unsigned)((total + 255) / 256);
+    if (cin == 32)
+        k_head<32><<<grid, 256, 0, s>>>(in, w, bias, out, mask, mask_esz, seg_dim, Cout, H * W, total, nhwc);
+    else
+        k_head<64><<<grid, 256, 0, s>>>(in, w, bias, out, mask, mask_esz, seg_dim, Cout, H * W, total, nhwc);
     PV_LAUNCHED("k_head");
     return PVNET_OK;
 }

@@ -20,7 +20,13 @@ namespace {
 constexpr int BN_CHUNK = 256;     // pixels per partial sum
 constexpr int BN_LANES = 256;     // threads merging one channel's partials (the tree below assumes a power of two)
 constexpr int BN_THREADS = 256;   // reduce-pass block size target (channel quads x partial slots)
-constexpr int BN_MAX_C = 1024;    // C/4 channel quads must fit one BN_THREADS block
+// Channel limits per form.  act(bn(x)) keeps its contract of up to 1024 channels.  The block tails take 2048:
+// Resnet50_8s's layer4 ends every Bottleneck in bn3 + skip (form 1) or bn3 + the downsample's BatchNorm (form 2) at
+// 2048 channels, while no BatchNorm outside a block tail of the three networks is wider than 512.
+constexpr int BN_MAX_C = 1024;
+constexpr int BN_MAX_C_TAIL = 2048;
+
+int max_channels(int form) { return form == 0 ? BN_MAX_C : BN_MAX_C_TAIL; }
 
 enum { ACT_NONE = 0, ACT_RELU = 1, ACT_LEAKY = 2 };
 
@@ -73,12 +79,18 @@ __device__ __forceinline__ int block_x()
 
 __device__ __forceinline__ float f4(const float4 &v, int i) { return i == 0 ? v.x : i == 1 ? v.y : i == 2 ? v.z : v.w; }
 
+// The reduce passes: a block holds R partials of Qb channel quads (thread t: quad blockIdx.y * Qb + t % Qb, partial
+// blockIdx.x * R + t / Qb).  Up to 1024 channels one block row covers all Q quads (Qb = Q, gridDim.y = 1); wider layers
+// spread their quads over gridDim.y rows of BN_THREADS.  Which thread sums a partial changes nothing in its order.
+__device__ __forceinline__ int quad_of(int Qb) { return blockIdx.y * Qb + threadIdx.x % Qb; }
+
 // ------------------------------------------------------------------ statistics: fp64 shifted sums per partial
 // part[k][c][j], k = 0: sum (x - K_c), k = 1: sum (x - K_c)^2, K_c = x[pixel 0][c]
-__global__ void __launch_bounds__(BN_THREADS) k_bn_stats_partial(const float *__restrict__ x, long long npix, int Q, int R,
-                                                           long long P, double *__restrict__ part)
+__global__ void __launch_bounds__(BN_THREADS) k_bn_stats_partial(const float *__restrict__ x, long long npix, int Q, int Qb,
+                                                                 int R, long long P, double *__restrict__ part)
 {
-    const int q = threadIdx.x % Q, r = threadIdx.x / Q;
+    const int q = quad_of(Qb), r = threadIdx.x / Qb;
+    if (q >= Q) return;
     const long long j = (long long)blockIdx.x * R + r;
     if (j >= P) return;
     const float4 *x4 = reinterpret_cast<const float4 *>(x);
@@ -192,10 +204,12 @@ __global__ void __launch_bounds__(256) k_bn_apply(const float4 *__restrict__ x, 
 // statistics' partition
 template <int FORM, int ACT>
 __global__ void __launch_bounds__(BN_THREADS) k_bn_backward_reduce(const float *__restrict__ dy, const float *__restrict__ x,
-                                                             const float *__restrict__ z, long long npix, int Q, int R,
-                                                             long long P, BnDev bn, BnDev bz, double *__restrict__ part)
+                                                             const float *__restrict__ z, long long npix, int Q, int Qb,
+                                                             int R, long long P, BnDev bn, BnDev bz,
+                                                             double *__restrict__ part)
 {
-    const int q = threadIdx.x % Q, r = threadIdx.x / Q;
+    const int q = quad_of(Qb), r = threadIdx.x / Qb;
+    if (q >= Q) return;
     const long long j = (long long)blockIdx.x * R + r;
     if (j >= P) return;
     const int C = 4 * Q;
@@ -321,18 +335,19 @@ __global__ void __launch_bounds__(256) k_bn_backward_apply(const float4 *__restr
 
 // ------------------------------------------------------------------ host side
 struct Partition {
-    int Q, R;
+    int Q, Qb, R;
     long long P;
-    unsigned blocks;
+    dim3 grid;
 };
 
 Partition partition(int C, long long npix)
 {
     Partition p;
     p.Q = C / 4;
-    p.R = BN_THREADS / p.Q;
+    p.Qb = p.Q < BN_THREADS ? p.Q : BN_THREADS;
+    p.R = BN_THREADS / p.Qb;
     p.P = (npix + BN_CHUNK - 1) / BN_CHUNK;
-    p.blocks = (unsigned)((p.P + p.R - 1) / p.R);
+    p.grid = dim3((unsigned)((p.P + p.R - 1) / p.R), (unsigned)((p.Q + p.Qb - 1) / p.Qb));
     return p;
 }
 
@@ -352,8 +367,8 @@ int check_common(const char *what, int form, int act, const float *x, const floa
     PV_CHECK_ARG(form >= 0 && form <= 2, "%s: form must be 0, 1 or 2, got %d", what, form);
     PV_CHECK_ARG(act >= 0 && act <= 2, "%s: act must be 0 (none), 1 (ReLU) or 2 (LeakyReLU), got %d", what, act);
     PV_CHECK_ARG(form == 0 || act == ACT_RELU, "%s: the block tails (forms 1, 2) end in ReLU", what);
-    PV_CHECK_ARG(C > 0 && C % 4 == 0 && C <= BN_MAX_C, "%s: C must be a positive multiple of 4 up to %d, got %d", what,
-                 BN_MAX_C, C);
+    PV_CHECK_ARG(C > 0 && C % 4 == 0 && C <= max_channels(form),
+                 "%s: C must be a positive multiple of 4 up to %d (form %d), got %d", what, max_channels(form), form, C);
     PV_CHECK_ARG(npix > 0, "%s: the pixel count must be positive", what);
     // element offsets are 64-bit throughout; the grid of the reduce passes is what bounds the size
     PV_CHECK_ARG((npix + BN_CHUNK - 1) / BN_CHUNK < (1LL << 31) && npix <= (1LL << 62) / C,
@@ -413,8 +428,8 @@ void launch_backward(const float *dy, const float *x, const float *z, long long 
                      float *dz, cudaStream_t st, bool reduce)
 {
     if (reduce) {
-        k_bn_backward_reduce<FORM, ACT><<<pt.blocks, pt.Q * pt.R, 0, st>>>(dy, x, z, npix, pt.Q, pt.R, pt.P, bn, bz,
-                                                                            part);
+        k_bn_backward_reduce<FORM, ACT><<<pt.grid, pt.Qb * pt.R, 0, st>>>(dy, x, z, npix, pt.Q, pt.Qb, pt.R, pt.P, bn,
+                                                                           bz, part);
         return;
     }
     const long long nvec = npix * pt.Q;
@@ -442,9 +457,10 @@ extern "C" {
 int pvnet_batchnorm_workspace_bytes(int form, int C, long long npix, size_t *bytes)
 {
     PV_CHECK_ARG(bytes, "batchnorm workspace: null output");
-    PV_CHECK_ARG(form >= 0 && form <= 2 && C > 0 && C % 4 == 0 && C <= pvnet::BN_MAX_C && npix > 0,
-                 "batchnorm workspace: form must be 0, 1 or 2, C a positive multiple of 4 up to %d and the pixel "
-                 "count positive (form %d, C %d, %lld pixels)", pvnet::BN_MAX_C, form, C, npix);
+    PV_CHECK_ARG(form >= 0 && form <= 2 && C > 0 && C % 4 == 0 && C <= pvnet::max_channels(form) && npix > 0,
+                 "batchnorm workspace: form must be 0, 1 or 2, C a positive multiple of 4 up to %d (form 0) or %d "
+                 "(forms 1, 2) and the pixel count positive (form %d, C %d, %lld pixels)", pvnet::BN_MAX_C,
+                 pvnet::BN_MAX_C_TAIL, form, C, npix);
     *bytes = pvnet::workspace_bytes(form, C, npix);
     return PVNET_OK;
 }
@@ -466,7 +482,7 @@ int pvnet_batchnorm_act_forward(int form, int act, const float *x, const float *
     for (int k = 0; k < (form == 2 ? 2 : 1); ++k) {
         double *pk = part + (size_t)k * 2 * C * pt.P;
         if (ds[k]->batch_stats) {
-            k_bn_stats_partial<<<pt.blocks, pt.Q * pt.R, 0, st>>>(xs[k], npix, pt.Q, pt.R, pt.P, pk);
+            k_bn_stats_partial<<<pt.grid, pt.Qb * pt.R, 0, st>>>(xs[k], npix, pt.Q, pt.Qb, pt.R, pt.P, pk);
             PV_LAUNCHED("k_bn_stats_partial");
         }
         k_bn_finalize<<<C, BN_LANES, 0, st>>>(xs[k], pk, pt.P, npix, C, *ds[k]);

@@ -54,7 +54,7 @@ cudaError_t ensure_max_smem(const void *func, int bytes)
 extern "C" {
 
 const char *pvnet_last_error(void) { return pvnet::g_err; }
-int pvnet_version(void) { return 2; }
+int pvnet_version(void) { return 3; }
 long long pvnet_launch_count(void) { return pvnet::launch_counter(); }
 void pvnet_launch_count_reset(void) { pvnet::launch_counter() = 0; }
 

@@ -60,7 +60,8 @@ int launch_s2d_pack(const void *in, int in_is_u8, const float *mean3, const floa
 int launch_maxpool(const float *in, float *out, int b, int H, int W, int C, int in_cs, int in_co, cudaStream_t s);
 int launch_upsample2x(const float *in, float *out, int b, int h, int w, int C, int out_cs, int out_co,
                       cudaStream_t s);
-int launch_head(const float *in, const float *w, const float *bias, float *out, void *mask, int mask_esz,
+// in NHWC [b,H,W,cin], cin 32 or 64 (raw_dim)
+int launch_head(const float *in, int cin, const float *w, const float *bias, float *out, void *mask, int mask_esz,
                 int seg_dim, int Cout, int b, int H, int W, int nhwc, cudaStream_t s);
 
 #ifdef __CUDACC__

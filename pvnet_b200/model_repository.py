@@ -1,6 +1,9 @@
-"""`Resnet18_8s` with the reference's constructor, forward signature and state-dict keys
-(zju3dv/pvnet lib/networks/model_repository.py:7-80), backed in eval mode by the native
-sm_90a backbone (wgmma implicit-GEMM convs behind include/pvnet_b200.h).
+"""`Resnet18_8s`, `Resnet34_8s` and `Resnet50_8s` with the reference's constructors, forward signature and
+state-dict keys (zju3dv/pvnet lib/networks/model_repository.py:7-156,226-300), backed in eval mode by the native
+sm_90a backbone (wgmma implicit-GEMM convs behind include/pvnet_b200.h).  Resnet34_8s keeps its trunk under the
+attribute `resnet50_8s`, as the reference does (model_repository.py:246), so its checkpoints load unchanged.
+The notes below are written for Resnet18_8s; the two deeper networks share every mechanism (`_Resnet8s`), with
+raw_dim 64, so their head always runs as the separate fp32 `k_head`.
 
     net = Resnet18_8s(ver_dim=18, seg_dim=2)
     net.load_state_dict(ckpt['net'])          # reference checkpoints load unchanged
@@ -36,7 +39,7 @@ from torch import nn
 
 from . import _native
 from . import conv as pc
-from .resnet import resnet18
+from .resnet import Bottleneck, resnet18, resnet34, resnet50
 
 # execution-order conv slots of include/pvnet_b200.h (pvnet_backbone_set_conv)
 _SLOTS = [
@@ -85,20 +88,46 @@ class _NativeState:
         self.pack_count = 0        # how many times weights were folded + packed (tests assert on it)
 
 
-class Resnet18_8s(nn.Module):
-    def __init__(self, ver_dim, seg_dim, fcdim=256, s8dim=128, s4dim=64, s2dim=32, raw_dim=32):
+def _trunk_slots(trunk, prefix):
+    """(conv, BatchNorm) module names of a trunk in the native plan's order: the stem; per block conv1, (conv2,) the
+    downsample, and the conv whose epilogue adds the skip (pvnet_backbone_create_trunk); then fc.0."""
+    slots = [(prefix + "conv1", prefix + "bn1")]
+    for li in range(1, 5):
+        for bi, blk in enumerate(getattr(trunk, f"layer{li}")):
+            p = f"{prefix}layer{li}.{bi}."
+            names = ["1", "2", "3"] if isinstance(blk, Bottleneck) else ["1", "2"]
+            slots += [(f"{p}conv{n}", f"{p}bn{n}") for n in names[:-1]]
+            if blk.downsample is not None:
+                slots.append((p + "downsample.0", p + "downsample.1"))
+            slots.append((f"{p}conv{names[-1]}", f"{p}bn{names[-1]}"))
+    return slots + [(prefix + "fc.0", prefix + "fc.1")]
+
+
+_DECODER_SLOTS = [("conv8s.0", "conv8s.1"), ("conv4s.0", "conv4s.1"), ("conv2s.0", "conv2s.1"),
+                  ("convraw.0", "convraw.1"), ("convraw.3", None)]
+
+
+class _Resnet8s(nn.Module):
+    """The Resnet*_8s graph (a dilated trunk under model_repository.py's decoder) and everything that runs it on the
+    native kernels: the per-device cache of packed weights, the eval forward and `forward_train`.  Subclasses name
+    the trunk attribute (`_trunk_attr`) and the trunk; `x4c` / `x8c` are layer1 / layer2's output channels."""
+
+    _trunk_attr = None
+
+    def __init__(self, trunk, ver_dim, seg_dim, fcdim, s8dim, s4dim, s2dim, raw_dim):
         super().__init__()
-        trunk = resnet18(output_stride=8)
+        e = 4 if isinstance(trunk.layer1[0], Bottleneck) else 1
+        x4c, x8c = 64 * e, 128 * e
         self.ver_dim = ver_dim
         self.seg_dim = seg_dim
         self._dims = (fcdim, s8dim, s4dim, s2dim, raw_dim)
         trunk.fc = nn.Sequential(nn.Conv2d(trunk.inplanes, fcdim, 3, 1, 1, bias=False), nn.BatchNorm2d(fcdim),
                                  nn.ReLU(True))
-        self.resnet18_8s = trunk
-        self.conv8s = nn.Sequential(nn.Conv2d(128 + fcdim, s8dim, 3, 1, 1, bias=False), nn.BatchNorm2d(s8dim),
+        setattr(self, self._trunk_attr, trunk)
+        self.conv8s = nn.Sequential(nn.Conv2d(x8c + fcdim, s8dim, 3, 1, 1, bias=False), nn.BatchNorm2d(s8dim),
                                     nn.LeakyReLU(0.1, True))
         self.up8sto4s = nn.UpsamplingBilinear2d(scale_factor=2)
-        self.conv4s = nn.Sequential(nn.Conv2d(64 + s8dim, s4dim, 3, 1, 1, bias=False), nn.BatchNorm2d(s4dim),
+        self.conv4s = nn.Sequential(nn.Conv2d(x4c + s8dim, s4dim, 3, 1, 1, bias=False), nn.BatchNorm2d(s4dim),
                                     nn.LeakyReLU(0.1, True))
         self.up4sto2s = nn.UpsamplingBilinear2d(scale_factor=2)
         self.conv2s = nn.Sequential(nn.Conv2d(64 + s4dim, s2dim, 3, 1, 1, bias=False), nn.BatchNorm2d(s2dim),
@@ -111,8 +140,23 @@ class Resnet18_8s(nn.Module):
         self._frozen = False
 
     # ------------------------------------------------------------------ PyTorch graph
+    def _trunk(self):
+        return getattr(self, self._trunk_attr)
+
+    def _slots(self):
+        """Execution-order (conv, BatchNorm) module names of the native conv slots."""
+        return _trunk_slots(self._trunk(), self._trunk_attr + ".") + _DECODER_SLOTS
+
+    def _create_handle(self, handle):
+        """pvnet_backbone_create_trunk for this trunk."""
+        t = self._trunk()
+        kind = 1 if isinstance(t.layer1[0], Bottleneck) else 0
+        blocks = (ctypes.c_int * 4)(*(len(getattr(t, f"layer{i}")) for i in range(1, 5)))
+        _native.check(_native.lib().pvnet_backbone_create_trunk(kind, blocks, self.ver_dim, self.seg_dim, *self._dims,
+                                                                ctypes.byref(handle)), "pvnet_backbone_create_trunk")
+
     def _forward_torch(self, x):
-        x2s, x4s, x8s, _x16s, _x32s, xfc = self.resnet18_8s(x)
+        x2s, x4s, x8s, _x16s, _x32s, xfc = self._trunk()(x)
         fm = self.up8sto4s(self.conv8s(torch.cat([xfc, x8s], 1)))
         fm = self.up4sto2s(self.conv4s(torch.cat([fm, x4s], 1)))
         fm = self.up2storaw(self.conv2s(torch.cat([fm, x2s], 1)))
@@ -184,11 +228,10 @@ class Resnet18_8s(nn.Module):
         mods = dict(self.named_modules())
         fcdim, s8dim, s4dim, s2dim, raw_dim = self._dims
         handle = ctypes.c_void_p()
-        _native.check(L.pvnet_backbone_create(self.ver_dim, self.seg_dim, fcdim, s8dim, s4dim, s2dim, raw_dim,
-                                              ctypes.byref(handle)), "pvnet_backbone_create")
+        self._create_handle(handle)
         keep = []
         with torch.no_grad():
-            for slot, (conv_name, bn_name) in enumerate(_SLOTS):
+            for slot, (conv_name, bn_name) in enumerate(self._slots()):
                 conv = mods[conv_name]
                 if bn_name is not None:
                     bn = mods[bn_name]
@@ -198,8 +241,10 @@ class Resnet18_8s(nn.Module):
                 w, b = w.to(device), b.to(device).contiguous()
                 if slot == 0:                         # stem: a 4x4 conv over the 2x2 space-to-depth image
                     packed = pc.pack_stem_s2d(w)
-                elif conv_name == "convraw.3":        # head: fp32 [cout][32]
+                elif conv_name == "convraw.3" and raw_dim == 32:   # head: fp32 [cout][32]
                     packed = pc.round_tf32(w.reshape(w.shape[0], w.shape[1]))   # fused path feeds it to a tf32 MMA
+                elif conv_name == "convraw.3":        # head: fp32 [cout][64], exact in k_head
+                    packed = w.reshape(w.shape[0], w.shape[1]).contiguous()
                 elif conv_name == "convraw.0":        # cat[fm(s2dim), image(3)] -> s2dim+8 input channels
                     packed = pc.pack_weight(w, cin_pad=pc.cin_padded(s2dim + 8))
                 else:
@@ -298,20 +343,27 @@ class Resnet18_8s(nn.Module):
 
     @staticmethod
     def _block_train(blk, x):
-        """resnet.BasicBlock.forward with its two (three) convolutions, its BatchNorms, ReLUs and residual add on the
-        native kernels: bn2, the downsample's BatchNorm, the add and the ReLU are one pass."""
+        """resnet.BasicBlock.forward (resnet.Bottleneck.forward) with its two (three) convolutions and the downsample,
+        its BatchNorms, ReLUs and residual add on the native kernels: the last BatchNorm (bn2, bn3), the downsample's
+        BatchNorm, the add and the ReLU are one pass."""
         relu = pc.act_of(blk.relu)
         y = pc.bn_act(blk.bn1, pc.conv2d_train(x, blk.conv1.weight, blk.conv1.stride[0], blk.conv1.dilation[0]), relu)
-        y = pc.conv2d_train(y, blk.conv2.weight, 1, blk.conv2.dilation[0])
+        if isinstance(blk, Bottleneck):
+            y = pc.bn_act(blk.bn2, pc.conv2d_train(y, blk.conv2.weight, blk.conv2.stride[0], blk.conv2.dilation[0]),
+                          relu)
+            last, bn_last = blk.conv3, blk.bn3
+        else:
+            last, bn_last = blk.conv2, blk.bn2
+        y = pc.conv2d_train(y, last.weight, 1, last.dilation[0])
         if blk.downsample is None:
-            return pc.bn_add_relu(blk.bn2, y, x)
+            return pc.bn_add_relu(bn_last, y, x)
         ds = blk.downsample
-        return pc.bn_add_relu(blk.bn2, y, pc.conv2d_train(x, ds[0].weight, ds[0].stride[0], 1), ds[1])
+        return pc.bn_add_relu(bn_last, y, pc.conv2d_train(x, ds[0].weight, ds[0].stride[0], 1), ds[1])
 
     def _check_train_modules(self):
         """ValueError unless conv1, the max-pool and convraw.3 still have the shapes forward_train's kernels
         implement."""
-        t = self.resnet18_8s
+        t = self._trunk()
         c1, mp, hd = t.conv1, t.maxpool, self.convraw[3]
         pair = lambda v: tuple(v) if isinstance(v, (tuple, list)) else (v, v)  # noqa: E731
         if not (isinstance(c1, nn.Conv2d) and tuple(c1.weight.shape) == (64, 3, 7, 7) and c1.stride == (2, 2)
@@ -367,7 +419,7 @@ class Resnet18_8s(nn.Module):
         if not x.is_cuda:
             raise RuntimeError("pvnet_b200: forward_train runs only on CUDA (no CPU fallback)")
         self._check_train_modules()
-        t = self.resnet18_8s
+        t = self._trunk()
         if raw_u8:
             b, h, w, _ = x.shape
         else:
@@ -400,7 +452,38 @@ class Resnet18_8s(nn.Module):
     def forward(self, x, feature_alignment=False):
         if self.training or not x.is_cuda:
             if not self.training and not x.is_cuda:
-                raise RuntimeError("pvnet_b200: eval-mode Resnet18_8s runs only on CUDA (no CPU fallback)")
+                raise RuntimeError(f"pvnet_b200: eval-mode {type(self).__name__} runs only on CUDA (no CPU fallback)")
             return self._forward_torch(x)
         out = self.forward_native(x)
         return out[:, :self.seg_dim, :, :], out[:, self.seg_dim:, :, :]
+
+
+class Resnet18_8s(_Resnet8s):
+    _trunk_attr = "resnet18_8s"
+
+    def __init__(self, ver_dim, seg_dim, fcdim=256, s8dim=128, s4dim=64, s2dim=32, raw_dim=32):
+        super().__init__(resnet18(output_stride=8), ver_dim, seg_dim, fcdim, s8dim, s4dim, s2dim, raw_dim)
+
+    def _slots(self):
+        return _SLOTS
+
+    def _create_handle(self, handle):
+        fcdim, s8dim, s4dim, s2dim, raw_dim = self._dims
+        _native.check(_native.lib().pvnet_backbone_create(self.ver_dim, self.seg_dim, fcdim, s8dim, s4dim, s2dim,
+                                                          raw_dim, ctypes.byref(handle)), "pvnet_backbone_create")
+
+
+class Resnet34_8s(_Resnet8s):
+    """The reference's Resnet34_8s (model_repository.py:226-300): 3-4-6-3 BasicBlocks, stored as `resnet50_8s`."""
+    _trunk_attr = "resnet50_8s"
+
+    def __init__(self, ver_dim, seg_dim, fcdim=384, s8dim=256, s4dim=128, s2dim=64, raw_dim=64):
+        super().__init__(resnet34(output_stride=8), ver_dim, seg_dim, fcdim, s8dim, s4dim, s2dim, raw_dim)
+
+
+class Resnet50_8s(_Resnet8s):
+    """The reference's Resnet50_8s (model_repository.py:82-156): 3-4-6-3 Bottlenecks."""
+    _trunk_attr = "resnet50_8s"
+
+    def __init__(self, ver_dim, seg_dim, fcdim=384, s8dim=256, s4dim=128, s2dim=64, raw_dim=64):
+        super().__init__(resnet50(output_stride=8), ver_dim, seg_dim, fcdim, s8dim, s4dim, s2dim, raw_dim)
