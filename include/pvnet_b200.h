@@ -645,12 +645,6 @@ PVNET_API int pvnet_adam_chunk_tensors(void);
  * stride-1 layers with Cout <= 64 whose weights fit in shared memory, per-tap kernel otherwise),
  * 1 = per-tap kernel only, 2 = column kernel (error if the layer is not eligible). */
 PVNET_API int pvnet_conv_set_mode(int mode);
-/* Test hook: 1 = the per-tap kernel runs as clusters of two CTAs on adjacent M tiles that share each
- * weight tile through TMA multicast; 0 (default) = single CTAs. */
-PVNET_API int pvnet_conv_set_multicast(int on);
-/* Test hook: 1 (default) runs the per-tap kernel persistent (one CTA per SM looping over the
- * output tiles, continuous TMA ring); 0 = one tile per CTA. */
-PVNET_API int pvnet_conv_set_persistent(int on);
 
 /* Resnet18_8s.forward (lib/networks/model_repository.py:64-80), eval mode, whole batch (Resnet34_8s / Resnet50_8s:
  * pvnet_backbone_create_trunk below; the same calls with the handle's own slots and stages).

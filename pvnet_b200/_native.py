@@ -138,8 +138,6 @@ SIGNATURES = {
                                 ctypes.c_double, ctypes.c_double, ctypes.c_int64, c_void_p]),
     "pvnet_adam_chunk_tensors": (c_int, []),
     "pvnet_conv_set_mode": (c_int, [c_int]),
-    "pvnet_conv_set_multicast": (c_int, [c_int]),
-    "pvnet_conv_set_persistent": (c_int, [c_int]),
     "pvnet_backbone_create": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_void_p)]),
     "pvnet_backbone_create_trunk": (c_int, [c_int, ctypes.POINTER(c_int), c_int, c_int, c_int, c_int, c_int, c_int,
                                             c_int, ctypes.POINTER(c_void_p)]),

@@ -23,16 +23,6 @@ def set_mode(mode: int):
     _native.check(_native.lib().pvnet_conv_set_mode(int(mode)), "pvnet_conv_set_mode")
 
 
-def set_multicast(mode: int):
-    """Test hook (pvnet_conv_set_multicast): 0 single CTAs (default), 1 two-CTA clusters with weight multicast."""
-    _native.check(_native.lib().pvnet_conv_set_multicast(int(mode)), "pvnet_conv_set_multicast")
-
-
-def set_persistent(on: bool):
-    """Test hook (pvnet_conv_set_persistent): persistent variant of the per-tap kernel."""
-    _native.check(_native.lib().pvnet_conv_set_persistent(int(bool(on))), "pvnet_conv_set_persistent")
-
-
 def round_tf32(t: torch.Tensor) -> torch.Tensor:
     """Round fp32 to the nearest TF32 value (10 explicit mantissa bits), kept in fp32."""
     i = t.contiguous().view(torch.int32)

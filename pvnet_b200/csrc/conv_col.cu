@@ -18,10 +18,10 @@
 //     in shared memory and stored by the producer warpgroup's otherwise idle warps while the next tile's MMAs
 //     run -- the [b,H,W,32] intermediate never exists.
 //
-// k_conv_col<KC, HEAD, KH, BN, WIDE> is instantiated per layer form: KC channels per chunk (8, 16 or 32), KH x KH
-// taps (3, or 4 for the stem), BN = Cout (32 or 64), HEAD the fused head (convraw.0 only, BN 32), WIDE convraw.0's
-// two-source input with its 32-channel first source loaded as one 128-byte-swizzled box.  conv_col_launch_at picks
-// the instantiation a plan was made for.
+// k_conv_col<KC, HEAD, KH, BN, WIDE> is instantiated per layer form, eight in all: 3x3 taps with 32- or 8-channel
+// chunks and BN = Cout 32 or 64; the stem's 4x4 taps with 16-channel chunks, BN 32 or 64; and convraw.0's fused
+// head (HEAD, 8-channel chunks, BN 32), with or without WIDE, its two-source input with the 32-channel first source
+// loaded as one 128-byte-swizzled box.  conv_col_launch_at picks the instantiation a plan was made for.
 #include "conv_tc.cuh"
 #include "ptx.cuh"
 
@@ -133,6 +133,8 @@ __global__ void __launch_bounds__(COL_THREADS, 1)
                void *__restrict__ mask)
 {
     static_assert(!HEAD || BN == 32, "fused head: 32 input channels");
+    static_assert(!HEAD || KC == 8, "fused head: convraw.0's 8-channel chunks");
+    static_assert((KC == 16) == (KH == 4), "16-channel chunks are the 4x4 stem's, and only its");
     static_assert(!WIDE || (HEAD && KC == 8 && KH == 3), "wide first source: convraw.0 form only");
     constexpr int ROWB = KC * 4;                       // bytes per K-major row
     constexpr int B_TILE = BN * ROWB;                  // one [BN][KC] weight tile (a multiple of 1024 bytes)
@@ -510,7 +512,7 @@ int conv_col_plan_at(const ConvDesc &d, const HeadDesc *head, void *storage)
     PV_CHECK_ARG(d.in_cs % 4 == 0 && d.in_co % 4 == 0 && d.out_cs % 4 == 0 && d.out_co % 4 == 0,
                  "conv(col): channel strides/offsets must be multiples of 4 floats");
     PV_CHECK_ARG(!d.res || (d.res_cs % 4 == 0 && d.res_co % 4 == 0), "conv(col): residual stride/offset alignment");
-    PV_CHECK_ARG(!head || (d.Cout == 32 && col_kc(d.Cin + d.Cin2) != 16 && head->cout >= 1 && head->cout <= 32 && head->w && head->bias &&
+    PV_CHECK_ARG(!head || (d.Cout == 32 && col_kc(d.Cin + d.Cin2) == 8 && head->cout >= 1 && head->cout <= 32 && head->w && head->bias &&
                            head->out_nchw && (!head->mask || head->mask_esz == 1 || head->mask_esz == 8)),
                  "conv(col): bad fused-head description");
     const int kc = col_kc(d.Cin + d.Cin2);
@@ -619,11 +621,10 @@ int conv_col_launch_at(const void *storage, cudaStream_t s)
 {
     const ColPlan &p = *static_cast<const ColPlan *>(storage);
     if (p.wide) return col_launch<8, true, 3, 32, true>(p, s);
-    if (p.head) return p.kc == 32 ? col_launch<32, true, 3, 32>(p, s) : col_launch<8, true, 3, 32>(p, s);
+    if (p.head) return col_launch<8, true, 3, 32>(p, s);
     const bool n64 = p.bn == 64;
     if (p.ksize == 4) return n64 ? col_launch<16, false, 4, 64>(p, s) : col_launch<16, false, 4, 32>(p, s);
     if (p.kc == 32) return n64 ? col_launch<32, false, 3, 64>(p, s) : col_launch<32, false, 3, 32>(p, s);
-    if (p.kc == 16) return n64 ? col_launch<16, false, 3, 64>(p, s) : col_launch<16, false, 3, 32>(p, s);
     return n64 ? col_launch<8, false, 3, 64>(p, s) : col_launch<8, false, 3, 32>(p, s);
 }
 

@@ -24,10 +24,7 @@
 //                memory: the last slabs of a tile drain under the next tile's MMAs.
 //
 // CTAs are persistent over (M tile, N tile) items (static round-robin; the ring runs on across items,
-// so the producer fetches the next item's operands during the current epilogue), or one item per CTA.
-// MC (pvnet_conv_set_multicast(1)): clusters of two CTAs on adjacent M tiles of the same N tile; each CTA
-// loads its A box and HALF of the weight tile, multicast into both, so the weights cross L2 -> SM once per
-// pair; a stage is refilled only after the consumers of BOTH CTAs released it.
+// so the producer fetches the next item's operands during the current epilogue).
 //
 // Stride-2 convolutions read the input through four "parity plane" tensor maps (even/odd
 // rows x even/odd columns); each tap then is a stride-1 box in one plane.
@@ -67,7 +64,7 @@ constexpr int CONV_SLAB = 32;          // output channels per epilogue slab: one
 constexpr int CONV_SLAB_BYTES = 128 * CONV_SLAB * 4;
 constexpr int CONV_EPI_BAR = 1;        // named barrier of the 256 consumer threads
 
-template <int BN, bool MC>
+template <int BN>
 __global__ void __launch_bounds__(CONV_THREADS, 1)
     k_conv_tap(const __grid_constant__ AMaps amaps, const __grid_constant__ CUtensorMap tmB,
                const __grid_constant__ CUtensorMap tmOut, const __grid_constant__ CUtensorMap tmRes,
@@ -91,20 +88,16 @@ __global__ void __launch_bounds__(CONV_THREADS, 1)
     const int tiles_per_img = g.tiles_x * g.tiles_y;
     const int n_tiles_n = g.Cout / BN;
     const int nkb = g.taps * g.cin_chunks;
-    // MC: item = (M tile pair, N tile); CTA rank r of the pair takes M tile 2*pair + r (an odd tile count
-    // leaves the last pair one tile short: its second CTA recomputes the last tile, identical values)
-    const uint32_t crank = MC ? ptx::cluster_ctarank() : 0u;
-    const int unit = MC ? (int)blockIdx.x >> 1 : (int)blockIdx.x, nunits = MC ? (int)gridDim.x >> 1 : (int)gridDim.x;
+    const int unit = (int)blockIdx.x, nunits = (int)gridDim.x;
     auto item_tile = [&](int item, int &m_tile, int &n0) {
-        const int mi = item / n_tiles_n;
-        n0 = (item - mi * n_tiles_n) * BN;
-        m_tile = MC ? min(2 * mi + (int)crank, g.total_m_tiles - 1) : mi;
+        m_tile = item / n_tiles_n;
+        n0 = (item - m_tile * n_tiles_n) * BN;
     };
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < STAGES; ++s) {
             ptx::mbar_init(&full[s], 1);
-            ptx::mbar_init(&empty[s], MC ? 16 : 8);    // one arrive per consumer warp (of both CTAs with MC)
+            ptx::mbar_init(&empty[s], 8);    // one arrive per consumer warp
         }
         for (int i = 0; i < 2; ++i) {
             ptx::mbar_init(&res_full[i], 1);
@@ -113,7 +106,6 @@ __global__ void __launch_bounds__(CONV_THREADS, 1)
         ptx::fence_barrier_init();
     }
     __syncthreads();
-    if (MC) ptx::cluster_sync();                      // the peer's barriers exist before any remote arrive or multicast
 
     if (warp == 8) {
         if (lane == 0) {
@@ -160,11 +152,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 1)
                         uint8_t *sa = smem + (size_t)s * STAGE_BYTES;
                         ptx::tma_load_4d(sa, &amaps.m[g.tap_map[tap]], &full[s], cc * CONV_KC, x0 + g.tap_ox[tap],
                                          y0 + g.tap_oy[tap], img);
-                        if (MC)     // rows [crank*BN/2, +BN/2) of the weight tile, into both CTAs
-                            ptx::tma_load_2d_mc(sa + CONV_A_BYTES + crank * (B_BYTES / 2), &tmB, &full[s],
-                                                tap * g.cin_pad + cc * CONV_KC, n0 + (int)crank * (BN / 2), (uint16_t)0x3);
-                        else
-                            ptx::tma_load_2d(sa + CONV_A_BYTES, &tmB, &full[s], tap * g.cin_pad + cc * CONV_KC, n0);
+                        ptx::tma_load_2d(sa + CONV_A_BYTES, &tmB, &full[s], tap * g.cin_pad + cc * CONV_KC, n0);
                         if (++s == STAGES) {
                             s = 0;
                             ph ^= 1u;
@@ -178,10 +166,6 @@ __global__ void __launch_bounds__(CONV_THREADS, 1)
         const int wg = warp >> 2, wq = warp & 3;
         const int g8 = lane >> 2, t4 = lane & 3;
         const uint32_t smem_u = ptx::smem_u32(smem);
-        auto release = [&](int st) {        // this warp is done reading stage st (in both CTAs' rings with MC)
-            ptx::mbar_arrive(&empty[st]);
-            if (MC) ptx::mbar_arrive_cluster(&empty[st], crank ^ 1u);
-        };
         int s = 0;
         uint32_t ph = 0, sq = 0;            // sq: slabs this CTA has stored so far
         for (int item = unit; item < g.n_items; item += nunits) {
@@ -202,7 +186,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 1)
                 // the previous K-block's MMAs have finished reading their stage: hand it back
                 ptx::wgmma_wait<1>();
                 ptx::fence_regs(acc);
-                if (prev >= 0 && lane == 0) release(prev);
+                if (prev >= 0 && lane == 0) ptx::mbar_arrive(&empty[prev]);
                 prev = s;
                 if (++s == STAGES) {
                     s = 0;
@@ -211,7 +195,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 1)
             }
             ptx::wgmma_wait<0>();
             ptx::fence_regs(acc);
-            if (lane == 0) release(prev);
+            if (lane == 0) ptx::mbar_arrive(&empty[prev]);
 
             // Epilogue, one 32-channel slab at a time through two staging buffers [128 pixels][32 channels], laid
             // out as TMA lays out the A tile (pixel m = row, 128-byte swizzle: 16-byte chunk c of row m sits at chunk
@@ -283,7 +267,6 @@ __global__ void __launch_bounds__(CONV_THREADS, 1)
         }
         if (threadIdx.x == 0) ptx::tma_store_wait_all();   // the stores have reached memory before the kernel ends
     }
-    if (MC) ptx::cluster_sync();                      // no CTA exits while its peer may still write into it
 }
 
 // ------------------------------------------------------------------ host side
@@ -345,15 +328,9 @@ struct ConvPlan {
     ConvGeom g;
     dim3 grid;
     size_t smem;
-    int mc;
     const float *bias;
     int has_res;
 };
-
-// 1: CTAs persistent over the items (grid = one CTA per SM); 0: one item per CTA (pvnet_conv_set_persistent)
-int g_conv_persist = 1;
-// 1: CTA pairs share each weight tile through TMA multicast (pvnet_conv_set_multicast; default 0)
-int g_conv_mc = 0;
 
 int conv_plan(const ConvDesc &d, ConvPlan *p)
 {
@@ -443,8 +420,7 @@ int conv_plan(const ConvDesc &d, ConvPlan *p)
     {
         cuuint64_t dims[2] = {(cuuint64_t)g.taps * g.cin_pad, (cuuint64_t)d.Cout};
         cuuint64_t strides[1] = {(cuuint64_t)g.taps * g.cin_pad * 4};
-        p->mc = g_conv_mc;
-        cuuint32_t box[2] = {(cuuint32_t)kc, (cuuint32_t)(p->mc ? g.BN / 2 : g.BN)};    // MC: each CTA loads half
+        cuuint32_t box[2] = {(cuuint32_t)kc, (cuuint32_t)g.BN};
         int rc = tma_encode(&p->tmB, d.w, 2, dims, strides, box, swz);
         if (rc) return rc;
     }
@@ -474,51 +450,32 @@ int conv_plan(const ConvDesc &d, ConvPlan *p)
     if (st > 8) st = 8;
     g.stages = st;
     p->smem = 1024 + (size_t)st * stage_b + 2 * CONV_SLAB_BYTES + 256;
-    // items: (M tile, N tile), or with MC (M tile pair, N tile) run by a two-CTA cluster
-    const int m_units = p->mc ? (g.total_m_tiles + 1) / 2 : g.total_m_tiles;
-    g.n_items = m_units * (d.Cout / g.BN);
-    long long units = g_conv_persist ? (long long)sm_count() / (p->mc ? 2 : 1) : (long long)g.n_items;
-    if (units > g.n_items) units = g.n_items;
-    p->grid = dim3((unsigned)(units * (p->mc ? 2 : 1)));
+    // items: (M tile, N tile); one persistent CTA per SM, or one per item when there are fewer
+    g.n_items = g.total_m_tiles * (d.Cout / g.BN);
+    long long grid = (long long)sm_count();
+    if (grid > g.n_items) grid = g.n_items;
+    p->grid = dim3((unsigned)grid);
     p->bias = d.bias;
     p->has_res = d.res != nullptr;
     return PVNET_OK;
 }
 
-template <int BN, bool MC>
+template <int BN>
 int conv_launch_t(const ConvPlan &p, cudaStream_t s)
 {
-    const cudaError_t attr_err = ensure_max_smem((const void *)k_conv_tap<BN, MC>, 227 * 1024);
+    const cudaError_t attr_err = ensure_max_smem((const void *)k_conv_tap<BN>, 227 * 1024);
     PV_CUDA(attr_err);
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = p.grid;
-    cfg.blockDim = dim3(CONV_THREADS);
-    cfg.dynamicSmemBytes = p.smem;
-    cfg.stream = s;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = MC ? 2 : 1;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = MC ? 1 : 0;
-    PV_CUDA(cudaLaunchKernelEx(&cfg, k_conv_tap<BN, MC>, p.amaps, p.tmB, p.tmOut, p.tmRes, p.g, p.bias, p.has_res));
+    k_conv_tap<BN><<<p.grid, CONV_THREADS, p.smem, s>>>(p.amaps, p.tmB, p.tmOut, p.tmRes, p.g, p.bias, p.has_res);
     PV_LAUNCHED("k_conv_tap");
     return PVNET_OK;
 }
 
 int conv_launch(const ConvPlan &p, cudaStream_t s)
 {
-    if (p.mc) {
-        if (p.g.BN == 256) return conv_launch_t<256, true>(p, s);
-        if (p.g.BN == 128) return conv_launch_t<128, true>(p, s);
-        if (p.g.BN == 64) return conv_launch_t<64, true>(p, s);
-        return conv_launch_t<32, true>(p, s);
-    }
-    if (p.g.BN == 256) return conv_launch_t<256, false>(p, s);
-    if (p.g.BN == 128) return conv_launch_t<128, false>(p, s);
-    if (p.g.BN == 64) return conv_launch_t<64, false>(p, s);
-    return conv_launch_t<32, false>(p, s);
+    if (p.g.BN == 256) return conv_launch_t<256>(p, s);
+    if (p.g.BN == 128) return conv_launch_t<128>(p, s);
+    if (p.g.BN == 64) return conv_launch_t<64>(p, s);
+    return conv_launch_t<32>(p, s);
 }
 
 size_t conv_plan_size() { return sizeof(ConvPlan); }
@@ -528,19 +485,6 @@ int conv_launch_at(const void *storage, cudaStream_t s) { return conv_launch(*st
 }  // namespace pvnet
 
 extern "C" {
-
-int pvnet_conv_set_multicast(int on)
-{
-    PV_CHECK_ARG(on == 0 || on == 1, "multicast mode must be 0 or 1");
-    pvnet::g_conv_mc = on;
-    return PVNET_OK;
-}
-
-int pvnet_conv_set_persistent(int on)
-{
-    pvnet::g_conv_persist = on ? 1 : 0;
-    return PVNET_OK;
-}
 
 int pvnet_conv2d_nhwc(const float *in, int in_cs, int in_co, int Cin, const float *w_packed, const float *bias,
                       const float *res, int res_cs, int res_co, float *out, int out_cs, int out_co, int Cout, int b,

@@ -197,26 +197,6 @@ __device__ __forceinline__ unsigned long long ld_cluster_u64(uint32_t addr)
     asm volatile("ld.shared::cluster.u64 %0, [%1];" : "=l"(v) : "r"(addr) : "memory");
     return v;
 }
-// arrive on the mbarrier at the same shared-memory offset in CTA `rank` of the cluster
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t *bar, uint32_t rank)
-{
-    asm volatile(
-        "{\n\t.reg .b32 ra;\n\tmapa.shared::cluster.u32 ra, %0, %1;\n\t"
-        "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}" ::"r"(smem_u32(bar)), "r"(rank)
-        : "memory");
-}
-// TMA load multicast: the box lands at the same shared-memory offset of every CTA in cta_mask and
-// completes its bytes on the mbarrier at the same offset in each of them
-__device__ __forceinline__ void tma_load_2d_mc(void *smem_dst, const CUtensorMap *m, uint64_t *bar, int c0, int c1,
-                                               uint16_t cta_mask)
-{
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
-        " [%0], [%1, {%4, %5}], [%2], %3;"
-        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "h"(cta_mask), "r"(c0),
-        "r"(c1)
-        : "memory");
-}
 
 // ---------------------------------------------------------------- wgmma
 // The four warps of a warpgroup issue one MMA together: D[64 x N] (fp32, registers) (+)= A[64 x 8] * B[N x 8]^T,

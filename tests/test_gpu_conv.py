@@ -60,20 +60,19 @@ def _run_case(b, H, W, cin, cout, k, stride, dil, act, with_res, in_extra=0, out
     (2, 24, 40, 64, 64, 3, 1, 1, 1, True),      # partial tiles, residual + ReLU (BasicBlock)
     (1, 24, 40, 128, 256, 3, 1, 2, 1, False),   # dilation 2 (layer3)
     (1, 24, 40, 64, 512, 3, 1, 4, 1, True),     # dilation 4, two N tiles (layer4)
+    (2, 24, 40, 64, 512, 3, 1, 4, 1, True),     # four N tiles, residual
     (2, 24, 40, 128, 256, 1, 1, 1, 0, False),   # 1x1 downsample, no stride
+    (2, 60, 80, 256, 256, 1, 1, 1, 0, False),   # 1x1, 80 M tiles
     (2, 48, 80, 64, 128, 3, 2, 1, 1, False),    # stride-2 3x3 through parity planes (layer2.0.conv1)
     (2, 48, 80, 64, 128, 1, 2, 1, 0, False),    # stride-2 1x1 downsample
     (1, 40, 48, 40, 32, 3, 1, 1, 2, False),     # Cin=40 -> 8-channel K-blocks (convraw.0), LeakyReLU
     (1, 60, 80, 384, 128, 3, 1, 1, 2, False),   # conv8s shape
 ])
-@pytest.mark.parametrize("persistent", [True, False], ids=["persistent", "tile-per-cta"])
-def test_conv_vs_torch(cfg, persistent):
+def test_conv_vs_torch(cfg):
     pc.set_mode(pc.MODE_PER_TAP)
-    pc.set_persistent(persistent)
     try:
         _run_case(*cfg)
     finally:
-        pc.set_persistent(True)
         pc.set_mode(pc.MODE_AUTO)
 
 
@@ -162,23 +161,3 @@ def test_conv_column_kernel_4x4_s2d_stem_shape():
 def test_conv_column_kernel_4x4_cout32():
     """A 4x4 layer with 32 output channels runs on its own instantiation (N = 32)."""
     _run_4x4_case(32, 5)
-
-
-@pytest.mark.parametrize("mc", [1, 0], ids=["multicast", "single-cta"])
-@pytest.mark.parametrize("cfg", [
-    (1, 24, 40, 128, 256, 3, 1, 2, 1, False),   # 9 M tiles: odd -> the last cluster's 2nd CTA duplicates a tile
-    (2, 24, 40, 64, 512, 3, 1, 4, 1, True),     # four N tiles, residual
-    (2, 60, 80, 256, 256, 1, 1, 1, 0, False),   # 1x1, 80 M tiles
-])
-def test_conv_cluster_multicast(cfg, mc):
-    """Wide layers: 2-CTA clusters sharing each weight tile through TMA multicast vs the plain launch."""
-    pc.set_mode(pc.MODE_PER_TAP)
-    pc.set_multicast(mc)
-    try:
-        _run_case(*cfg)
-        pc.set_persistent(False)      # one (M tile pair, N tile) per cluster
-        _run_case(*cfg)
-    finally:
-        pc.set_persistent(True)
-        pc.set_multicast(0)
-        pc.set_mode(pc.MODE_AUTO)
