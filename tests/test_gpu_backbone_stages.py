@@ -1,8 +1,10 @@
-"""GPU: the native Resnet18_8s forward one launch at a time, each stage against an fp64 restatement of its own layer.
+"""GPU: the native Resnet18_8s, Resnet34_8s and Resnet50_8s forwards one launch at a time, each stage against an fp64
+restatement of its own layer.
 
-The end-to-end tests (test_gpu_backbone.py) bound the whole network by the error cuDNN-TF32 makes over 26 layers;
-a fault that moves one layer by 0.1 % hides in that.  Here every stage of `pvnet_backbone_run_stage` runs on a
-workspace the test owns (layout and stage table: tests/backbone_stages.py), and for each one:
+The end-to-end tests (test_gpu_backbone.py, test_gpu_deep_backbones.py) bound the whole network by the error
+cuDNN-TF32 makes over 26, 36 or 53 layers; a fault that moves one layer by 0.1 % hides in that.  Here every stage of
+`pvnet_backbone_run_stage` runs on a workspace the test owns (layout and stage table: tests/backbone_stages.py), and
+for each one:
 
 (a) exactly its output region changes: the rest of the workspace and the guard bands around `out` and the mask keep
     their bytes;
@@ -17,13 +19,17 @@ the module's 7x7/2 convolution (not the 4x4 space-to-depth form the library pack
 concatenation order come from the module.  r(.) is rounding to TF32 (nearest, ties away from zero).
 
 Bounds, per element:
-  conv / stem        |got - ref| <= 2^-11 |ref| + 2e-5 max(max|ref|, 1) + 1e-5
-                     (output rounding to TF32; fp32 accumulation over up to 4608 exact TF32 products); the 2^-11
-                     term is dropped where the output is not rounded (convraw.0 -> R0)
+  conv / stem        |got - ref| <= 2^-11 |ref| + acc, acc = 1e-5 R (tests/helpers.py conv_acc_bound)
+                     (output rounding to TF32; fp32 accumulation of K exact TF32 products).  R is the same conv on
+                     absolute values plus |bias| and |residual|, so the term grows with K: Resnet50_8s's fc.0 sums
+                     K = 18 432 products, where the largest (|err| - 2^-11 |ref|) / R measured on an H100 was 1.7e-6
+                     (2.8e-6 for the same shape in test_gpu_conv.py).  Where K <= 4608 (all of Resnet18_8s) acc is
+                     also held to 2e-5 max(max|ref|, 1) + 1e-5.  The 2^-11 term is dropped where the output is not
+                     rounded (convraw.0 -> R0)
   upsample x2        2^-11 |ref| + 2^-20 max|src|      (output rounding; fp32 interpolation weights and sums)
-  fused head         sum_k |W_ck| (2^-10 |a_k| + eps_conv) + 1e-6   (a = convraw.0's activation, which may land on
+  fused head         sum_k |W_ck| (2^-10 |a_k| + acc_k) + 1e-6   (a = convraw.0's activation, which may land on
                      either TF32 neighbour before the head MMA)
-  k_head (fp32)      2^-18 sum_k |W_ck R0_k| + 2^-23 |b_c|   (32 fp32 FMAs)
+  k_head (fp32)      2^-18 sum_k |W_ck R0_k| + 2^-23 |b_c|   (32 or 64 fp32 FMAs: 64 2^-24 is the worst case of 64)
   pack, max-pool     bit-exact;  mask: torch.argmax of the stage's own logits (first maximum wins), exact.
 """
 import ctypes
@@ -34,9 +40,9 @@ import torch
 import torch.nn.functional as F
 
 from pvnet_b200 import _native
-from pvnet_b200.model_repository import Resnet18_8s
+from pvnet_b200.model_repository import Resnet18_8s, Resnet34_8s, Resnet50_8s
 from tests import backbone_stages as bs
-from tests.helpers import seeded_state_dict
+from tests.helpers import conv_acc_bound, seeded_state_dict
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -49,19 +55,29 @@ WIDE_S2 = (256, 128, 64, 256, 32)        # convraw.0 in = 256 + 8: 33 eight-chan
                                          # weights (297 KB) exceed shared memory, so the fused head streams them
                                          # with each A stage (resident = 0 in conv_col_plan_at; checked with a
                                          # printf there while writing this test)
+NETS = {Resnet18_8s: bs.RESNET18, Resnet34_8s: bs.RESNET34, Resnet50_8s: bs.RESNET50}
 CASES = [
-    # id, ver_dim, seg_dim, decoder widths, (b, h, w)
-    ("k9-2x64x96", 18, 2, bs.DEFAULT_DIMS, (2, 64, 96)),
-    ("k9-1x72x104", 18, 2, bs.DEFAULT_DIMS, (1, 72, 104)),     # 1/8 grid 9 x 13: odd stride-2 parity planes
-    ("k9-3x16x16", 18, 2, bs.DEFAULT_DIMS, (3, 16, 16)),
-    ("k9-1x256x264", 18, 2, bs.DEFAULT_DIMS, (1, 256, 264)),
-    ("k9-16x480x640", 18, 2, bs.DEFAULT_DIMS, (16, 480, 640)),  # bench.py --config 2
-    ("k17-4x480x640", 34, 2, bs.DEFAULT_DIMS, (4, 480, 640)),   # bench.py --config 5: unfused k_head
-    ("k17-2x48x64", 34, 2, bs.DEFAULT_DIMS, (2, 48, 64)),
-    ("k17-2x64x96", 34, 2, bs.DEFAULT_DIMS, (2, 64, 96)),
-    ("k17-1x72x104", 34, 2, bs.DEFAULT_DIMS, (1, 72, 104)),
-    ("narrow-seg3-1x72x104", 18, 3, NARROW, (1, 72, 104)),      # head width 21: odd, channel 21 in the padding
-    ("s2dim256-1x72x104", 18, 2, WIDE_S2, (1, 72, 104)),
+    # id, network, ver_dim, seg_dim, decoder widths, (b, h, w)
+    ("k9-2x64x96", Resnet18_8s, 18, 2, bs.DEFAULT_DIMS, (2, 64, 96)),
+    ("k9-1x72x104", Resnet18_8s, 18, 2, bs.DEFAULT_DIMS, (1, 72, 104)),  # 1/8 grid 9 x 13: odd stride-2 parity planes
+    ("k9-3x16x16", Resnet18_8s, 18, 2, bs.DEFAULT_DIMS, (3, 16, 16)),
+    ("k9-1x256x264", Resnet18_8s, 18, 2, bs.DEFAULT_DIMS, (1, 256, 264)),
+    ("k9-16x480x640", Resnet18_8s, 18, 2, bs.DEFAULT_DIMS, (16, 480, 640)),  # bench.py --config 2
+    ("k17-4x480x640", Resnet18_8s, 34, 2, bs.DEFAULT_DIMS, (4, 480, 640)),   # bench.py --config 5: unfused k_head
+    ("k17-2x48x64", Resnet18_8s, 34, 2, bs.DEFAULT_DIMS, (2, 48, 64)),
+    ("k17-2x64x96", Resnet18_8s, 34, 2, bs.DEFAULT_DIMS, (2, 64, 96)),
+    ("k17-1x72x104", Resnet18_8s, 34, 2, bs.DEFAULT_DIMS, (1, 72, 104)),
+    # head width 21: odd, channel 21 in the padding
+    ("narrow-seg3-1x72x104", Resnet18_8s, 18, 3, NARROW, (1, 72, 104)),
+    ("s2dim256-1x72x104", Resnet18_8s, 18, 2, WIDE_S2, (1, 72, 104)),
+    # the deep networks (raw_dim 64: k_head at Cin 64): 1x1 Bottleneck convs up to Cin 2048, fc.0 over 2048 channels
+    # (K = 18 432), decoder inputs of 320 / 512 / 896 channels, convraw.0 reading 64 + 8 channels
+    ("r34-k9-2x64x96", Resnet34_8s, 18, 2, bs.DEEP_DIMS, (2, 64, 96)),
+    ("r34-k9-1x72x104", Resnet34_8s, 18, 2, bs.DEEP_DIMS, (1, 72, 104)),
+    ("r34-k9-1x480x640", Resnet34_8s, 18, 2, bs.DEEP_DIMS, (1, 480, 640)),
+    ("r50-k9-2x64x96", Resnet50_8s, 18, 2, bs.DEEP_DIMS, (2, 64, 96)),
+    ("r50-k9-1x72x104", Resnet50_8s, 18, 2, bs.DEEP_DIMS, (1, 72, 104)),     # Bottleneck conv2 (s2) onto 9 x 13
+    ("r50-k9-1x480x640", Resnet50_8s, 18, 2, bs.DEEP_DIMS, (1, 480, 640)),
 ]
 OUTPUT_FORMS = [(False, torch.int64), (True, torch.uint8), (False, torch.uint8), (True, torch.int64)]
 
@@ -87,8 +103,9 @@ def _fold(mods, conv, bn):
     return (w * scale[:, None, None, None]).float(), (m.bias.detach().double() - m.running_mean.detach().double() * scale).float()
 
 
-def _conv_bound(ref, rounded):
-    return (2.0 ** -11 * ref.abs() if rounded else 0) + 2e-5 * max(ref.abs().max().item(), 1.0) + 1e-5
+def _conv_bound(ref, R, K, rounded):
+    """Output rounding to TF32 (where the output is rounded) plus fp32 accumulation."""
+    return (2.0 ** -11 * ref.abs() if rounded else 0) + conv_acc_bound(ref, R, K)
 
 
 def _within(what, got, ref, bound):
@@ -146,24 +163,27 @@ class _Guarded:
 
 
 class _StageRun:
-    def __init__(self, net, x, dims, seg, ver):
-        self.net, self.x, self.dims, self.seg, self.ver = net, x, dims, seg, ver
+    def __init__(self, net, trunk, x, seg, ver):
+        self.net, self.trunk, self.x, self.seg, self.ver = net, trunk, x, seg, ver
         self.ctot = seg + ver
         self.b, _, self.h, self.w = x.shape
         self.mods = dict(net.named_modules())
-        self.table = bs.stages(dims, seg, ver, self.b, self.h, self.w)
+        self.table = bs.stages(trunk, seg, ver, self.b, self.h, self.w)
         self.L = _native.lib()
         self.handle = net._prepare_native(DEV)
+        self.num_stages = self.L.pvnet_backbone_handle_num_stages(self.handle)
+        assert [s.name for s in self.table] == [self.L.pvnet_backbone_handle_stage_name(self.handle, i).decode()
+                                                for i in range(self.num_stages)], "stage table is stale"
         n = ctypes.c_size_t()
         _native.check(self.L.pvnet_backbone_workspace_bytes(self.handle, self.b, self.h, self.w, ctypes.byref(n)),
                       "pvnet_backbone_workspace_bytes")
-        self.at, total = bs.layout(dims, self.b, self.h, self.w)
+        self.at, total = bs.layout(trunk, self.b, self.h, self.w)
         assert n.value == total + 256, "workspace layout of tests/backbone_stages.py is stale"
         self.nbytes = n.value
         raw = torch.full((self.nbytes + 256,), 0xFF, dtype=torch.uint8, device=DEV)
         shift = (-raw.data_ptr()) % 256
         self._raw, self.ws = raw, raw[shift:shift + self.nbytes]
-        self.worst = {}
+        self.worst, self.acc = {}, {}
 
     # ---------------------------------------------------------------- outputs and regions
     def set_outputs(self, pixel_major, mask_dtype):
@@ -244,7 +264,7 @@ class _StageRun:
             if not torch.equal(a[s:s + chunk], b[s:s + chunk]):
                 k = s + int(torch.nonzero(a[s:s + chunk] != b[s:s + chunk])[0, 0])
                 byte = 4 * k
-                names = [name for name in bs.BUFFERS if self.at[name] <= byte]
+                names = [name for name in self.at if self.at[name] <= byte]
                 return f"{names[-1]} at float {(byte - self.at[names[-1]]) // 4}" if names else f"byte {byte}"
         return None
 
@@ -253,19 +273,31 @@ class _StageRun:
         return torch.cat([self.f32(r, n) for r in st.reads], 3)
 
     def _conv_ref(self, st, inp, n):
+        """(the layer in fp64, R: the same sum over absolute values, before the activation)."""
         conv = self.mods[st.conv]
         w, b = _fold(self.mods, st.conv, st.bn)
-        inp = inp[..., :conv.in_channels]
-        y = F.conv2d(_nchw(_trunc(inp)).double(), _r(w).double(), None,
-                     conv.stride, conv.padding, conv.dilation)
-        y = _nhwc(y) + b.double()
+        xq, wq = _nchw(_trunc(inp[..., :conv.in_channels])).double(), _r(w).double()
+        y = _nhwc(F.conv2d(xq, wq, None, conv.stride, conv.padding, conv.dilation)) + b.double()
+        R = _nhwc(F.conv2d(xq.abs(), wq.abs(), None, conv.stride, conv.padding, conv.dilation)) + b.double().abs()
         if st.res is not None:
-            y = y + self.f32(st.res, n).double()
+            res = self.f32(st.res, n).double()
+            y, R = y + res, R + res.abs()
         if st.act == "relu":
             y = y.clamp_min(0)
         elif st.act == "leaky":
             y = torch.where(y > 0, y, 0.1 * y)
-        return y
+        return y, R
+
+    def _K(self, st):
+        """Products per output element."""
+        w = self.mods[st.conv].weight
+        return w.shape[1] * w.shape[2] * w.shape[3]
+
+    def _note_acc(self, st, got, ref, R, rounded):
+        """Records max (|got - ref| - rounding) / R: how close the accumulation comes to the R term."""
+        err = (got.double() - ref).abs() - (2.0 ** -11 * ref.abs() if rounded else 0)
+        r = float(torch.where(err > 0, err / R, torch.zeros_like(err)).max())
+        self.acc[st.name] = max(r, self.acc.get(st.name, 0.0))
 
     def _check_pack(self, st, n):
         rx = _nhwc(_r(self.x[n:n + 1]))
@@ -277,11 +309,13 @@ class _StageRun:
 
     def _check_stem(self, st, n):
         x = _nhwc(self.x[n:n + 1])
-        ref = self._conv_ref(st, _r(x), n)
-        return _within(st.name, self.f32(st.writes[0], n), ref, _conv_bound(ref, True))
+        ref, R = self._conv_ref(st, _r(x), n)
+        got = self.f32(st.writes[0], n)
+        self._note_acc(st, got, ref, R, True)
+        return _within(st.name, got, ref, _conv_bound(ref, R, self._K(st), True))
 
     def _check_pool(self, st, n):
-        ref = _nhwc(self.mods["resnet18_8s.maxpool"](_nchw(self.f32(st.reads[0], n))))
+        ref = _nhwc(self.mods[self.trunk.prefix + "maxpool"](_nchw(self.f32(st.reads[0], n))))
         return _bits_equal(st.name, self.region(st.writes[0])[n:n + 1], ref)
 
     def _check_up(self, st, n):
@@ -300,18 +334,21 @@ class _StageRun:
             f"{st.name}: mask is not torch.argmax of the stage's own logits"
 
     def _head_weights(self):
+        """convraw.3 as packed: rounded to TF32 at raw_dim 32 (the fused head's MMA reads it), fp32 at raw_dim 64."""
         w, b = _fold(self.mods, "convraw.3", None)
-        return _r(w.reshape(w.shape[0], -1)).double(), b.double()
+        w = w.reshape(w.shape[0], -1)
+        return (_r(w) if self.trunk.dims[4] == 32 else w).double(), b.double()
 
     def _check_conv(self, st, n):
-        ref = self._conv_ref(st, self._conv_input(st, n), n)
+        ref, R = self._conv_ref(st, self._conv_input(st, n), n)
         if st.writes[0].buf != "out":
-            return _within(st.name, self.f32(st.writes[0], n), ref, _conv_bound(ref, st.round_out))
+            got = self.f32(st.writes[0], n)
+            self._note_acc(st, got, ref, R, st.round_out)
+            return _within(st.name, got, ref, _conv_bound(ref, R, self._K(st), st.round_out))
         # convraw.0 with convraw.3 + argmax in its epilogue: the head MMA reads r(a)
         W, bh = self._head_weights()
         logits = _r(ref.float()).double() @ W.T + bh
-        eps = 2e-5 * max(ref.abs().max().item(), 1.0) + 1e-5
-        bound = (2.0 ** -10 * ref.abs() + eps) @ W.abs().T + 1e-6
+        bound = (2.0 ** -10 * ref.abs() + conv_acc_bound(ref, R, self._K(st))) @ W.abs().T + 1e-6
         worst = _within(f"{st.name} + fused head", self._logits_got(n), logits, bound)
         self._check_mask(st, n)
         return worst
@@ -326,19 +363,19 @@ class _StageRun:
         return worst
 
 
-def _net(ver, seg, dims, seed):
-    net = Resnet18_8s(ver, seg, *dims)
+def _net(cls, ver, seg, dims, seed):
+    net = cls(ver, seg, *dims)
     net.load_state_dict(seeded_state_dict(net, seed=seed))
     return net.to(DEV).eval()
 
 
 @pytest.mark.parametrize("case", CASES, ids=[c[0] for c in CASES])
 def test_every_stage_against_its_own_layer(case):
-    name, ver, seg, dims, (b, h, w) = case
+    name, cls, ver, seg, dims, (b, h, w) = case
     x = torch.from_numpy(np.random.default_rng(h * w + b).standard_normal((b, 3, h, w), dtype=np.float32)).to(DEV)
     try:
         with torch.no_grad():
-            run = _StageRun(_net(ver, seg, dims, seed=21), x, dims, seg, ver)
+            run = _StageRun(_net(cls, ver, seg, dims, seed=21), NETS[cls]._replace(dims=dims), x, seg, ver)
             run.set_outputs(*OUTPUT_FORMS[0])
             checked = 0
             for i, st in enumerate(run.table):
@@ -351,10 +388,19 @@ def test_every_stage_against_its_own_layer(case):
                     checked += run.run(i)
     finally:
         torch.cuda.synchronize()
-    idle = 1 if seg + ver <= 32 else 0        # the head, when convraw.0 carries it
-    assert checked == run.L.pvnet_backbone_num_stages() - idle
+    idle = 1 if dims[4] == 32 and seg + ver <= 32 else 0        # the head, when convraw.0 carries it
+    assert checked == run.num_stages - idle
     print(f"\n[stages {name}] worst |err|/bound per stage: " +
           ", ".join(f"{k}: {v:.2g}" for k, v in run.worst.items()))
+    kinds = {}
+    for st in run.table:
+        if st.name in run.worst:
+            kind = st.kind if st.kind != "conv" else "conv " + ("1x1" if run._K(st) == run.mods[st.conv].in_channels
+                                                                 else "3x3")
+            kinds[kind] = max(kinds.get(kind, 0.0), run.worst[st.name])
+    print(f"[stages {name}] worst |err|/bound per kind: " + ", ".join(f"{k}: {v:.2g}" for k, v in kinds.items()))
+    print(f"[stages {name}] max (|err| - rounding) / R per conv: " +
+          ", ".join(f"{k} (K={run._K(st)}): {run.acc[k]:.2g}" for st in run.table for k in [st.name] if k in run.acc))
 
 
 # ---------------------------------------------------------------------------------------------- argmax ties

@@ -37,7 +37,7 @@ def _case(row, b, hw, seed):
     ho, wo = hw
     cbuf = cg.buffer_channels(name, cin)
     x = pc.round_tf32(torch.randn(b, cbuf, ho * stride, wo * stride, device=DEV, generator=g))
-    if name == "convraw.0":
+    if cg.is_convraw(name):
         x[:, cin:] = 0
     dy = pc.round_tf32(torch.randn(b, cout, ho, wo, device=DEV, generator=g))
     w = torch.randn(cout, cin, k, k, device=DEV, generator=g) * 0.1
@@ -105,15 +105,21 @@ def test_layer4_full_batch16():
 
 
 def test_wgrad_workspace_stays_bounded():
-    # the split planner keeps the partial tiles to at most 128 MB and a modest split count, at the largest shapes
+    # the split planner keeps the partial tiles to at most 128 MB and a modest split count, at the largest shapes:
+    # Resnet18_8s's, and the deep networks' fc.0 over 2048 channels (a 28 MB dW), their widest 1x1 convs, the 1x1
+    # convs at 1/4 resolution (stride 2: the zero-inserted grid), the 896- and 512-channel decoder inputs and convraw.0
     import ctypes
     from pvnet_b200 import _native
-    for cin, cout, b, h, w in ((512, 512, 32, 60, 80), (40, 32, 32, 480, 640), (64, 64, 32, 120, 160)):
+    for cin, cout, b, h, w, k in ((512, 512, 32, 60, 80, 3), (40, 32, 32, 480, 640, 3), (64, 64, 32, 120, 160, 3),
+                                  (2048, 384, 32, 60, 80, 3), (2048, 512, 32, 60, 80, 1), (512, 2048, 32, 60, 80, 1),
+                                  (1024, 2048, 32, 60, 80, 1), (64, 256, 32, 120, 160, 1), (256, 64, 32, 120, 160, 1),
+                                  (256, 512, 32, 120, 160, 1), (896, 256, 32, 60, 80, 3), (512, 128, 32, 120, 160, 3),
+                                  (72, 64, 32, 480, 640, 3)):
         n = ctypes.c_size_t()
         with torch.cuda.device(DEV):
-            _native.check(_native.lib().pvnet_conv2d_nhwc_wgrad_workspace_bytes(cin, cout, b, h, w, 3, ctypes.byref(n)),
+            _native.check(_native.lib().pvnet_conv2d_nhwc_wgrad_workspace_bytes(cin, cout, b, h, w, k, ctypes.byref(n)),
                           "pvnet_conv2d_nhwc_wgrad_workspace_bytes")
-        splits = n.value // (cout * cin * 9 * 4)
+        splits = n.value // (cout * cin * k * k * 4)
         assert n.value <= 128 << 20 and 1 <= splits <= 512, (cin, cout, n.value, splits)
 
 

@@ -1,8 +1,10 @@
-"""GPU: one real Resnet18_8s.forward_train step, every native call against an fp64 restatement of its own layer.
+"""GPU: one real Resnet18_8s, Resnet34_8s or Resnet50_8s forward_train step, every native call against an fp64
+restatement of its own layer.
 
-The whole-step tests (test_gpu_conv_grad.py, test_gpu_bn_train.py) bound the network by torch's own TF32 error, up to
-1.7e-1 on a parameter gradient; a weight gradient 1 % wrong on one layer hides in that.  Here the step runs with
-capture wrappers on pvnet_b200.conv (tests/train_stages.py): each of the 52 calls records its inputs, its output, the
+The whole-step tests (test_gpu_conv_grad.py, test_gpu_bn_train.py, test_gpu_deep_backbones_train.py) bound the network
+by torch's own TF32 error, up to 1.7e-1 on a parameter gradient; a weight gradient 1 % wrong on one layer hides in
+that.  Here the step runs with capture wrappers on pvnet_b200.conv (tests/train_stages.py): each of the 52, 84 or 117
+calls records its inputs, its output, the
 gradient that reached its output and the gradient it gave each input.  Every reference below is computed from that
 call's own captured tensors, so errors do not accumulate and a failure names the layer.  trunc(.) drops the low 13
 mantissa bits (what a TF32 MMA reads from an fp32 activation or gradient), r(.) rounds to TF32 (the packed weights).
@@ -52,7 +54,7 @@ from oracle import stem_pool_head_oracle as so
 from oracle import upsample_oracle as uo
 from pvnet_b200 import conv as pc
 from pvnet_b200 import net_utils as nu
-from pvnet_b200.model_repository import Resnet18_8s
+from pvnet_b200.model_repository import Resnet18_8s, Resnet34_8s, Resnet50_8s
 from tests import train_stages as ts
 from tests.helpers import seeded_state_dict
 
@@ -62,19 +64,38 @@ ACTS = {"relu": pc.ACT_RELU, "leaky": pc.ACT_LEAKY, None: pc.ACT_NONE}
 SAMPLE_ABOVE = 65536
 
 # The paths a case must reach, asserted in _run_case: convolutions whose weight gradient is split over more than one
-# CTA per tile (layer2.0.conv1: k_conv_wgrad<2,64> on the zero-inserted grid; conv2s.0: <1,128>), and convolutions
-# whose input has a partly filled 64-channel Cin tile (channel count of the captured input).
+# CTA per tile (layer2.0.conv1: k_conv_wgrad<2,64> on the zero-inserted grid; conv2s.0: <1,128>; the deep networks'
+# 1x1 convs at 1/4 resolution and fc.0 over 512 / 2048 channels), and convolutions whose input has a partly filled
+# 64-channel Cin tile (channel count of the captured input).
+R50 = "resnet50_8s."              # Resnet34_8s keeps its trunk under the same name
 SPLIT = {"k9-2x480x640": ("resnet18_8s.layer1.0.conv1", "resnet18_8s.layer2.0.conv1", "conv4s.0", "conv2s.0",
-                          "convraw.0")}
-PARTIAL_CIN = {"k9-2x480x640": {"convraw.0": 40}, "narrow-seg3-2x72x104": {"convraw.0": 72, "conv2s.0": 96}}
+                          "convraw.0"),
+         "r34-k9-2x480x640": (R50 + "layer2.0.downsample.0", R50 + "fc.0", "convraw.0"),
+         "r50-k9-2x480x640": (R50 + "layer1.0.conv1", R50 + "layer1.1.conv3", R50 + "layer1.0.downsample.0",
+                              R50 + "layer2.0.downsample.0", R50 + "fc.0", "convraw.0")}
+PARTIAL_CIN = {"k9-2x480x640": {"convraw.0": 40}, "narrow-seg3-2x72x104": {"convraw.0": 72, "conv2s.0": 96},
+               "r34-k9-2x480x640": {"convraw.0": 72}, "r50-k9-2x480x640": {"convraw.0": 72}}
 
 CASES = [
-    # id, ver_dim, seg_dim, decoder widths, (b, h, w)
-    ("k9-2x480x640", 18, 2, ts.DEFAULT_DIMS, (2, 480, 640)),        # training resolution; wgrad splits; 150 partials
-    ("k9-3x72x104", 18, 2, ts.DEFAULT_DIMS, (3, 72, 104)),          # odd 9 x 13 grid at 1/8
-    ("k9-4x8x8", 18, 2, ts.DEFAULT_DIMS, (4, 8, 8)),                # 1 x 1 at 1/8: every dilated off-centre tap pads
-    ("k17-2x64x96", 34, 2, ts.DEFAULT_DIMS, (2, 64, 96)),           # head Cout 36
-    ("narrow-seg3-2x72x104", 18, 3, ts.NARROW_DIMS, (2, 72, 104)),  # convraw.0 reads 72 channels; conv2s.0 Cin 96
+    # id, network, trunk, ver_dim, seg_dim, decoder widths, (b, h, w)
+    # training resolution; wgrad splits; 150 partials
+    ("k9-2x480x640", Resnet18_8s, ts.RESNET18, 18, 2, ts.DEFAULT_DIMS, (2, 480, 640)),
+    ("k9-3x72x104", Resnet18_8s, ts.RESNET18, 18, 2, ts.DEFAULT_DIMS, (3, 72, 104)),   # odd 9 x 13 grid at 1/8
+    # 1 x 1 at 1/8: every dilated off-centre tap pads
+    ("k9-4x8x8", Resnet18_8s, ts.RESNET18, 18, 2, ts.DEFAULT_DIMS, (4, 8, 8)),
+    ("k17-2x64x96", Resnet18_8s, ts.RESNET18, 34, 2, ts.DEFAULT_DIMS, (2, 64, 96)),    # head Cout 36
+    # convraw.0 reads 72 channels; conv2s.0 Cin 96
+    ("narrow-seg3-2x72x104", Resnet18_8s, ts.RESNET18, 18, 3, ts.NARROW_DIMS, (2, 72, 104)),
+    # the deep networks: 1x1 Bottleneck convs up to Cin 2048, fc.0 at K = 18 432, BatchNorms of 2048 channels,
+    # head_train at Cin 64, convraw.0 reading 72 channels
+    ("r34-k9-2x64x96", Resnet34_8s, ts.RESNET34, 18, 2, ts.DEEP_DIMS, (2, 64, 96)),
+    ("r34-k9-3x72x104", Resnet34_8s, ts.RESNET34, 18, 2, ts.DEEP_DIMS, (3, 72, 104)),
+    ("r34-k9-4x8x8", Resnet34_8s, ts.RESNET34, 18, 2, ts.DEEP_DIMS, (4, 8, 8)),
+    ("r34-k9-2x480x640", Resnet34_8s, ts.RESNET34, 18, 2, ts.DEEP_DIMS, (2, 480, 640)),
+    ("r50-k9-2x64x96", Resnet50_8s, ts.RESNET50, 18, 2, ts.DEEP_DIMS, (2, 64, 96)),
+    ("r50-k9-3x72x104", Resnet50_8s, ts.RESNET50, 18, 2, ts.DEEP_DIMS, (3, 72, 104)),
+    ("r50-k9-4x8x8", Resnet50_8s, ts.RESNET50, 18, 2, ts.DEEP_DIMS, (4, 8, 8)),       # dilation 4 under Bottlenecks
+    ("r50-k9-2x480x640", Resnet50_8s, ts.RESNET50, 18, 2, ts.DEEP_DIMS, (2, 480, 640)),
 ]
 
 
@@ -124,9 +145,8 @@ class Ledger:
             self.fail.append(what)
 
 
-def _model(ver, seg, dims):
-    net = Resnet18_8s(ver_dim=ver, seg_dim=seg, fcdim=dims[0], s8dim=dims[1], s4dim=dims[2], s2dim=dims[3],
-                      raw_dim=dims[4])
+def _model(cls, ver, seg, dims):
+    net = cls(ver_dim=ver, seg_dim=seg, fcdim=dims[0], s8dim=dims[1], s4dim=dims[2], s2dim=dims[3], raw_dim=dims[4])
     net.load_state_dict(seeded_state_dict(net))
     return net.to(DEV).train()
 
@@ -331,8 +351,9 @@ def _wgrad_splits(cin, cout, b, H, W, k):
 
 # ----------------------------------------------------------------------------- the step
 def _run_case(case, monkeypatch):
-    name, ver_dim, seg_dim, dims, (b, h, w) = case
-    net = _model(ver_dim, seg_dim, dims)
+    name, cls, trunk, ver_dim, seg_dim, dims, (b, h, w) = case
+    trunk = trunk._replace(dims=dims)
+    net = _model(cls, ver_dim, seg_dim, dims)
     twin = copy.deepcopy(net)
     x = torch.randn(b, 3, h, w, device=DEV, generator=torch.Generator(device=DEV).manual_seed(b * h + w))
     mask, field, wgt = _targets(b, h, w, ver_dim // 2, h + w)
@@ -352,9 +373,9 @@ def _run_case(case, monkeypatch):
     for (k, p), (_, q) in zip(net.named_buffers(), twin.named_buffers()):
         L.exact(f"instrumented buffer {k} differs", torch.equal(p, q))
     del twin
-    rows, recs = ts.calls(dims), cap.records
+    rows, recs = ts.calls(trunk), cap.records
     assert [(r.kind, r.name or c.name) for r, c in zip(recs, rows)] == [(c.kind, c.name) for c in rows]
-    assert len(recs) == len(rows) == 52
+    assert len(recs) == len(rows)
     # (c) every parameter in exactly one call
     names = [p for c in rows for p in c.params()]
     assert sorted(names) == sorted(k for k, _ in net.named_parameters()) and len(set(names)) == len(names)
@@ -362,7 +383,8 @@ def _run_case(case, monkeypatch):
     vals = {c.name: r.output for c, r in zip(rows, recs)}
     vals["image"] = x
     vals["zeros"] = torch.zeros(b, ts.PAD_CHANNELS, h, w, device=DEV)
-    vals["cat"] = torch.cat([vals[s] for s in ts.CAT], 1)
+    cat = ts.cat_operands(trunk)
+    vals["cat"] = torch.cat([vals[s] for s in cat], 1)
     for c, r in zip(rows, recs):
         for k, s in enumerate(c.inputs):
             L.exact(f"{c.name}: input {k} is not {s}", torch.equal(r.inputs[k], vals[s]))
@@ -374,15 +396,16 @@ def _run_case(case, monkeypatch):
         if s not in index:
             continue
         terms = [recs[i].in_grads[k] for i, k in cons]
-        if s in ts.CAT:
+        if s in cat:
             g = recs[cat_call].in_grads[rows[cat_call].inputs.index("cat")]
-            terms.append(g[:, :fc] if s == ts.CAT[0] else g[:, fc:])
+            terms.append(g[:, :fc] if s == cat[0] else g[:, fc:])
         L.sums(f"gradient at {s}", recs[index[s]].out_grad, terms)
-    for s in ts.CAT:          # xfc feeds only the cat
+    for s in cat:             # xfc feeds only the cat
         if s not in ts.consumers(rows):
             g = recs[cat_call].in_grads[0]
             L.sums(f"gradient at {s}", recs[index[s]].out_grad, [g[:, :fc]])
     # the kernel paths this case is meant to reach
+    reached = set()
     for c, r in zip(rows, recs):
         if c.kind != "conv":
             continue
@@ -391,8 +414,11 @@ def _run_case(case, monkeypatch):
             splits = _wgrad_splits(x.shape[1], net.get_submodule(c.name).weight.shape[0], *x.shape[:1], *x.shape[2:],
                                    net.get_submodule(c.name).kernel_size[0])
             assert splits > 1, (c.name, splits)
+            reached.add(c.name)
         if c.name in PARTIAL_CIN.get(name, {}):
             assert x.shape[1] == PARTIAL_CIN[name][c.name] and x.shape[1] % 64 != 0, (c.name, x.shape)
+            reached.add(c.name)
+    assert reached == set(SPLIT.get(name, ())) | set(PARTIAL_CIN.get(name, {})), reached
     # per call
     mods = dict(net.named_modules())
     for c, r in zip(rows, recs):
@@ -445,7 +471,7 @@ def test_head_train_against_oracle(b, H, W):
 # ----------------------------------------------------------------------------- batch 1 at 8 x 8
 def test_single_value_per_channel_raises_like_torch():
     # layer2.0.bn1 sees one value per channel: nn.BatchNorm2d raises ValueError after counting the batch
-    net = _model(18, 2, ts.DEFAULT_DIMS)
+    net = _model(Resnet18_8s, 18, 2, ts.DEFAULT_DIMS)
     start = {k: v.clone() for k, v in net.named_buffers()}
     ref = copy.deepcopy(net)
     x = torch.randn(1, 3, 8, 8, device=DEV, generator=torch.Generator(device=DEV).manual_seed(5))
@@ -461,5 +487,5 @@ def test_single_value_per_channel_raises_like_torch():
             assert torch.equal(got[k], start[k]) == torch.equal(want[k], start[k]), k
             rel = float((got[k].double() - want[k].double()).norm() / want[k].double().norm())
             assert rel <= 1e-2, (k, rel)
-    assert int(got[ts.T + "layer2.0.bn1.num_batches_tracked"]) == 1
-    assert int(got[ts.T + "layer2.0.bn2.num_batches_tracked"]) == 0
+    assert int(got[ts.RESNET18.prefix + "layer2.0.bn1.num_batches_tracked"]) == 1
+    assert int(got[ts.RESNET18.prefix + "layer2.0.bn2.num_batches_tracked"]) == 0

@@ -1,8 +1,9 @@
-"""Resnet18_8s.forward_train as the tests see it: the graph table of its 52 native calls, and wrappers that capture
-each call's inputs, output and gradients during a real training step.
+"""Resnet*_8s.forward_train as the tests see it: the graph table of its native calls (52 for Resnet18_8s, 84 for
+Resnet34_8s, 117 for Resnet50_8s), and wrappers that capture each call's inputs, output and gradients during a real
+training step.
 
-The table is written from `Resnet18_8s._forward_torch` and pvnet_b200/resnet.py (BasicBlock.forward,
-DilatedResNet18.forward), not from `forward_train`: the CPU test (test_train_stages_cpu.py) replays it against
+The table is written from `_Resnet8s._forward_torch` and pvnet_b200/resnet.py (BasicBlock.forward, Bottleneck.forward,
+DilatedResNet.forward), not from `forward_train`: the CPU test (test_train_stages_cpu.py) replays it against
 forward hooks on a CPU model, and the GPU test (test_gpu_train_stages.py) holds every captured call to it and to an
 fp64 restatement of its own layer.
 """
@@ -13,16 +14,29 @@ from typing import NamedTuple, Optional, Tuple
 
 import torch
 
-DEFAULT_DIMS = (256, 128, 64, 32, 32)          # fcdim, s8dim, s4dim, s2dim, raw_dim of Resnet18_8s
+from tests.backbone_stages import DEEP_DIMS, DEFAULT_DIMS, RESNET18, RESNET34, RESNET50, Trunk  # noqa: F401
+
 NARROW_DIMS = (128, 64, 32, 64, 32)
-T = "resnet18_8s."
 PAD_CHANNELS = 5          # convraw.0 reads cat[fm, image, 5 zero channels] (40 = s2dim + 8 channels by default)
 
 # Sources a call can read besides the outputs of earlier calls:
 #   "image"  the input image;
 #   "zeros"  the [b, PAD_CHANNELS, H, W] zero channels behind the image;
-#   "cat"    torch.cat([xfc, x8s], 1), the one torch op of the step (CAT names its operands).
-CAT = (T + "fc.1", T + "layer2.1.bn2")
+#   "cat"    torch.cat([xfc, x8s], 1), the one torch op of the step (cat_operands names its operands).
+
+
+def _last_bn(trunk):
+    return "bn3" if trunk.bottleneck else "bn2"
+
+
+def _stage_output(trunk, layer):
+    """The call whose output is layer `layer`'s (1..4): the last block's residual BatchNorm."""
+    return f"{trunk.prefix}layer{layer}.{trunk.blocks[layer - 1] - 1}.{_last_bn(trunk)}"
+
+
+def cat_operands(trunk):
+    """The operands of the "cat" source: xfc, then x8s (layer2's output)."""
+    return (trunk.prefix + "fc.1", _stage_output(trunk, 2))
 
 
 class Call(NamedTuple):
@@ -48,30 +62,36 @@ class Call(NamedTuple):
         return [m for m in (self.name, self.bn_skip) if m is not None] if self.kind.startswith("bn_") else []
 
 
-def calls(dims=DEFAULT_DIMS):
-    """The 52 native calls of one forward_train step, in execution order."""
-    s2 = dims[3]
+def calls(trunk=RESNET18):
+    """The native calls of one forward_train step, in execution order."""
+    s2, T = trunk.dims[3], trunk.prefix
     rows = [Call("stem", T + "conv1", ("image",)),
             Call("bn_act", T + "bn1", (T + "conv1",), act="relu"),          # x2s
             Call("maxpool", T + "maxpool", (T + "bn1",))]
     x = T + "maxpool"
-    for layer in ("layer1", "layer2", "layer3", "layer4"):
-        for i in range(2):
-            blk = f"{T}{layer}.{i}"
-            rows += [Call("conv", blk + ".conv1", (x,)),
-                     Call("bn_act", blk + ".bn1", (blk + ".conv1",), act="relu"),
-                     Call("conv", blk + ".conv2", (blk + ".bn1",))]
-            if i == 0 and layer != "layer1":        # _stage: a downsample where stride or width changes
+    convs = ("conv1", "conv2", "conv3") if trunk.bottleneck else ("conv1", "conv2")
+    for layer in range(1, 5):
+        for i in range(trunk.blocks[layer - 1]):
+            blk = f"{T}layer{layer}.{i}"
+            src = x
+            # every conv but the last is followed by its BatchNorm + ReLU
+            for k, cv in enumerate(convs[:-1]):
+                rows += [Call("conv", f"{blk}.{cv}", (src,)),
+                         Call("bn_act", f"{blk}.bn{k + 1}", (f"{blk}.{cv}",), act="relu")]
+                src = f"{blk}.bn{k + 1}"
+            last, bn = f"{blk}.{convs[-1]}", f"{blk}.{_last_bn(trunk)}"
+            rows.append(Call("conv", last, (src,)))
+            # _stage: a downsample where stride or width changes (layer1 of a Bottleneck trunk widens 64 -> 256)
+            if i == 0 and (layer != 1 or trunk.bottleneck):
                 rows += [Call("conv", blk + ".downsample.0", (x,)),
-                         Call("bn_add_relu", blk + ".bn2", (blk + ".conv2", blk + ".downsample.0"),
-                              bn_skip=blk + ".downsample.1")]
+                         Call("bn_add_relu", bn, (last, blk + ".downsample.0"), bn_skip=blk + ".downsample.1")]
             else:
-                rows.append(Call("bn_add_relu", blk + ".bn2", (blk + ".conv2", x)))
-            x = blk + ".bn2"
-    # x4s = layer1.1.bn2, x8s = layer2.1.bn2, x32s = layer4.1.bn2; the decoder's cat order: upsampled features first
+                rows.append(Call("bn_add_relu", bn, (last, x)))
+            x = bn
+    # x4s, x8s, x32s: layer1 / layer2 / layer4's outputs; the decoder's cat order: upsampled features first
     rows += [Call("conv", T + "fc.0", (x,)), Call("bn_act", T + "fc.1", (T + "fc.0",), act="relu"),
              Call("conv", "conv8s.0", ("cat",)), Call("bn_act", "conv8s.1", ("conv8s.0",), act="leaky"),
-             Call("upsample_cat", "up8sto4s", ("conv8s.1", T + "layer1.1.bn2")),
+             Call("upsample_cat", "up8sto4s", ("conv8s.1", _stage_output(trunk, 1))),
              Call("conv", "conv4s.0", ("up8sto4s",)), Call("bn_act", "conv4s.1", ("conv4s.0",), act="leaky"),
              Call("upsample_cat", "up4sto2s", ("conv4s.1", T + "bn1")),
              Call("conv", "conv2s.0", ("up4sto2s",)), Call("bn_act", "conv2s.1", ("conv2s.0",), act="leaky"),
@@ -122,6 +142,7 @@ class Capture:
 
     def __init__(self, net, pc):
         self.pc = pc
+        self.maxpool = net._trunk_attr + ".maxpool"
         self.records = []
         self.param_name = {id(p): n for n, p in net.named_parameters()}
         self.module_name = {id(m): n for n, m in net.named_modules()}
@@ -182,7 +203,7 @@ class Capture:
         return self._end(rec, self.orig["bn_add_relu"](bn, av, sv, bn_skip))
 
     def maxpool_train(self, x):
-        rec, (xv,) = self._begin("maxpool", T + "maxpool", x)
+        rec, (xv,) = self._begin("maxpool", self.maxpool, x)
         return self._end(rec, self.orig["maxpool_train"](xv))
 
     def upsample2x_cat(self, low, *rest):
