@@ -1,4 +1,4 @@
-"""Resnet18_8s / Resnet34_8s / Resnet50_8s on one GPU: eval images/s (native vs the torch graph on cuDNN), per-stage
+"""Resnet18_8s / Resnet34_8s / Resnet50_8s / Resnet50_8s_2o on one GPU: eval images/s (native vs the torch graph on cuDNN), per-stage
 times of the native eval forward, and one training step (native vs the torch graph), with FLOPs per image counted
 from the layer shapes.
 
@@ -12,11 +12,13 @@ median over --iters passes; each stage's time includes the host's launch gap bef
 whole forward.  Train: forward_train + the native training losses + backward() + the native Adam, vs
 _forward_torch in channels_last + torch's cross-entropy / smooth-L1 + torch.optim.Adam, both in train mode; cuDNN TF32.
 FLOPs: 2 * MACs of every convolution (the head included) at the layer's output resolution; the train step is
-counted as 3x the forward's (forward, data and weight gradients).
+counted as 3x the forward's (forward, data and weight gradients).  Workspace: pvnet_backbone_workspace_bytes of the
+eval batch, next to the stage times.
 """
 from __future__ import annotations
 
 import argparse
+import ctypes
 import json
 import os
 import subprocess
@@ -34,7 +36,7 @@ from pvnet_b200 import net_utils as nu  # noqa: E402
 from pvnet_b200.optim import Adam  # noqa: E402
 
 H, W = 480, 640
-NETS = ("Resnet18_8s", "Resnet34_8s", "Resnet50_8s")
+NETS = ("Resnet18_8s", "Resnet34_8s", "Resnet50_8s", "Resnet50_8s_2o")
 
 
 def gpu_info():
@@ -118,7 +120,9 @@ def stage_rows(name, net, x, iters, info):
     n = L.pvnet_backbone_handle_num_stages(handle)
     names = [L.pvnet_backbone_handle_stage_name(handle, i).decode() for i in range(n)]
     b, _, h, w = x.shape
-    out = torch.empty(b, 20, h, w, device=dev)
+    out = torch.empty(b, 20, h // net._out_scale, w // net._out_scale, device=dev)
+    ws = ctypes.c_size_t()
+    _native.check(L.pvnet_backbone_workspace_bytes(handle, b, h, w, ctypes.byref(ws)), "workspace_bytes")
     net.freeze_native(True)          # no per-call walk over the weights between two stages
     with torch.no_grad():
         net.run_stages(x, out, None, 0, n)
@@ -134,7 +138,7 @@ def stage_rows(name, net, x, iters, info):
             times[it] = [ev[i].elapsed_time(ev[i + 1]) for i in range(n)]
     net.freeze_native(False)
     med = np.median(times, 0)
-    row = dict(what="stages", net=name, batch=b, total_ms=float(med.sum()),
+    row = dict(what="stages", net=name, batch=b, total_ms=float(med.sum()), workspace_bytes=ws.value,
                stages=[{"name": s, "ms": round(float(t), 4)} for s, t in zip(names, med)])
     row.update(info)
     return [row]
@@ -142,8 +146,10 @@ def stage_rows(name, net, x, iters, info):
 
 def train_rows(name, dev, batch, iters, info):
     rng = np.random.default_rng(0)
-    mask = torch.from_numpy((rng.random((batch, H, W)) < 0.3).astype(np.int64)).to(dev)
-    hc = torch.from_numpy(np.concatenate([rng.uniform([0, 0], [W, H], (batch, 9, 2)), np.ones((batch, 9, 1))], 2)).to(dev)
+    ho, wo = H // getattr(mr, name)._out_scale, W // getattr(mr, name)._out_scale    # targets on the output grid
+    mask = torch.from_numpy((rng.random((batch, ho, wo)) < 0.3).astype(np.int64)).to(dev)
+    hc = torch.from_numpy(np.concatenate([rng.uniform([0, 0], [wo, ho], (batch, 9, 2)), np.ones((batch, 9, 1))],
+                                         2)).to(dev)
     x = torch.randn(batch, 3, H, W, device=dev)
     rows = []
     net = make(name, dev).train()

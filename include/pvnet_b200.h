@@ -588,6 +588,14 @@ PVNET_API int pvnet_batchnorm_act_backward(int form, int act, const float *dy, c
 PVNET_API int pvnet_stem_s2d_nhwc(const void *image, int image_is_u8, const float *mean3, const float *std3,
                                   const float *w_s2d, const float *bias, float *s2d, float *out, float *img, int img_cs,
                                   int img_co, int b, int H, int W, pvnet_stream_t stream);
+/* pvnet_stem_s2d_half_nhwc: pvnet_stem_s2d_nhwc with img at half resolution, NHWC [b,H/2,W/2,img_cs]: channels
+ *   [img_co, img_co+3) get x_ds = F.interpolate(image, scale_factor=0.5, mode='bilinear') unrounded, bit for bit
+ *   torch's CUDA result on the NCHW float image ((0.5a + 0.5b)*0.5 + (0.5c + 0.5d)*0.5 over each 2x2 block, rows
+ *   first), and [img_co+3, img_co+8) zeros: conv2s.0's image and pad channels in Resnet50_8s_2o.  s2d and out are
+ *   those of pvnet_stem_s2d_nhwc. */
+PVNET_API int pvnet_stem_s2d_half_nhwc(const void *image, int image_is_u8, const float *mean3, const float *std3,
+                                       const float *w_s2d, const float *bias, float *s2d, float *out, float *img,
+                                       int img_cs, int img_co, int b, int H, int W, pvnet_stream_t stream);
 PVNET_API int pvnet_stem_s2d_wgrad_workspace_bytes(int b, int H, int W, size_t *bytes);
 PVNET_API int pvnet_stem_s2d_wgrad(const float *s2d, const float *dout, float *dw, int b, int H, int W,
                                    void *workspace, size_t workspace_bytes, pvnet_stream_t stream);
@@ -685,6 +693,17 @@ PVNET_API int pvnet_backbone_num_convs(void);
 enum { PVNET_BLOCK_BASIC = 0, PVNET_BLOCK_BOTTLENECK = 1 };
 PVNET_API int pvnet_backbone_create_trunk(int block_kind, const int *blocks, int ver_dim, int seg_dim, int fcdim,
                                           int s8dim, int s4dim, int s2dim, int raw_dim, pvnet_backbone_t **out);
+/* Resnet50_8s_2o's decoder (model_repository.py:158-224) over the same trunks: conv8s, conv4s, then conv2s.0 over
+ * cat[up(conv4s), x2s, x_ds] (x_ds = F.interpolate(image, scale_factor=0.5, mode='bilinear')) and the 1x1 head
+ * conv2s.3, at half resolution.  The conv slots are the trunk's, then conv8s.0, conv4s.0, conv2s.0 (packed for
+ * s4dim+64+8 input channels: s4dim upsampled, 64 x2s, 3 x_ds, 5 zeros) and conv2s.3 as [seg_dim+ver_dim][s2dim].
+ * s2dim must be 32 or 64.  The forward calls then write out [b,seg_dim+ver_dim,h/2,w/2] (or [b,h/2,w/2,C]) and the
+ * mask [b,h/2,w/2]; everything else is as for the full-resolution decoder. */
+PVNET_API int pvnet_backbone_create_trunk_2o(int block_kind, const int *blocks, int ver_dim, int seg_dim, int fcdim,
+                                             int s8dim, int s4dim, int s2dim, pvnet_backbone_t **out);
+/* The factor between the input and the output grid: 1, or 2 for a pvnet_backbone_create_trunk_2o handle; -1 for a
+ * null handle. */
+PVNET_API int pvnet_backbone_output_scale(const pvnet_backbone_t *m);
 PVNET_API int pvnet_backbone_handle_num_convs(const pvnet_backbone_t *m);   /* -1 for a null handle */
 PVNET_API void pvnet_backbone_destroy(pvnet_backbone_t *m);
 PVNET_API int pvnet_backbone_set_conv(pvnet_backbone_t *m, int slot, const float *w_packed, const float *bias);

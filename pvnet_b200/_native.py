@@ -125,6 +125,9 @@ SIGNATURES = {
     "pvnet_stem_s2d_nhwc": (c_int, [c_void_p, c_int, ctypes.POINTER(c_float), ctypes.POINTER(c_float), c_void_p,
                                     c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                     c_void_p]),
+    "pvnet_stem_s2d_half_nhwc": (c_int, [c_void_p, c_int, ctypes.POINTER(c_float), ctypes.POINTER(c_float), c_void_p,
+                                         c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
+                                         c_void_p]),
     "pvnet_stem_s2d_wgrad_workspace_bytes": (c_int, [c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
     "pvnet_stem_s2d_wgrad": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_size_t, c_void_p]),
     "pvnet_maxpool3x3s2_nhwc": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
@@ -141,6 +144,9 @@ SIGNATURES = {
     "pvnet_backbone_create": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_void_p)]),
     "pvnet_backbone_create_trunk": (c_int, [c_int, ctypes.POINTER(c_int), c_int, c_int, c_int, c_int, c_int, c_int,
                                             c_int, ctypes.POINTER(c_void_p)]),
+    "pvnet_backbone_create_trunk_2o": (c_int, [c_int, ctypes.POINTER(c_int), c_int, c_int, c_int, c_int, c_int,
+                                               c_int, ctypes.POINTER(c_void_p)]),
+    "pvnet_backbone_output_scale": (c_int, [c_void_p]),
     "pvnet_backbone_destroy": (None, [c_void_p]),
     "pvnet_backbone_num_convs": (c_int, []),
     "pvnet_backbone_handle_num_convs": (c_int, [c_void_p]),

@@ -213,10 +213,11 @@ class Upsample2xCatNHWC(torch.autograd.Function):
     atomics, so identical run to run); each rest[i] gets its channel slice of the gradient, as cat's backward gives
     it.  Runs on the input's device and its current stream.
 
-    With `buf` given (and no `rest`) the concatenated buffer is the caller's: a channels_last [b,Cb,2h,2w] float32
-    tensor that needs no gradient, whose channels behind the first C the caller has filled (forward_train: the stem
-    writes convraw.0's image and pad channels).  The upsampled channels are written into it in place, and it is
-    returned, marked dirty; its other channels are not copied in either direction."""
+    With `buf` given the concatenated buffer is the caller's: a channels_last [b,Cb,2h,2w] float32 tensor that needs
+    no gradient, whose channels behind the first C + sum Ci the caller has filled (forward_train: the stem writes
+    convraw.0's image and pad channels, or conv2s.0's x_ds and pad channels in Resnet50_8s_2o).  The upsampled
+    channels and the `rest` tensors are written into it in place, and it is returned, marked dirty; its other
+    channels are not copied in either direction."""
 
     @staticmethod
     def forward(ctx, low, buf, *rest):
@@ -239,6 +240,10 @@ class Upsample2xCatNHWC(torch.autograd.Function):
                                  f"{tuple(buf.shape)}")
             if buf.requires_grad:
                 raise ValueError("Upsample2xCatNHWC: buf gets no gradient, so it must not require one")
+            if rest and (any(r.dtype != torch.float32 or r.shape[0] != b or r.shape[2:] != (2 * h, 2 * w)
+                             for r in rest) or C % 4 or sum(widths) > buf.shape[1]):
+                raise ValueError(f"every concatenated tensor must be float32 [{b}, C, {2 * h}, {2 * w}], C a multiple "
+                                 f"of 4, and all {widths} channels must fit in buf's {buf.shape[1]}")
             ctx.mark_dirty(buf)
         dev = low.device
         lh = _nhwc(low)
@@ -281,10 +286,10 @@ def upsample2x_cat(low, *rest):
     return Upsample2xCatNHWC.apply(low, None, *rest)
 
 
-def upsample2x_into(low, buf):
-    """Upsample2xCatNHWC.apply with the caller's buffer: the upsampled `low` written into the first channels of `buf`
-    under autograd, `buf` returned."""
-    return Upsample2xCatNHWC.apply(low, buf)
+def upsample2x_into(low, buf, *rest):
+    """Upsample2xCatNHWC.apply with the caller's buffer: the upsampled `low`, then `rest`, written into the first
+    channels of `buf` under autograd, `buf` returned."""
+    return Upsample2xCatNHWC.apply(low, buf, *rest)
 
 
 # ----------------------------------------------------------------------------- train-mode BatchNorm (autograd)
@@ -551,13 +556,15 @@ class StemS2dNHWC(torch.autograd.Function):
     and the 4x4 stride-1 convolution with the weights packed by pack_stem_s2d_train -- into a channels_last
     [b,64,H/2,W/2].  In the same pass it writes the fp32 image, unrounded, into channels [co, co+3) of `img` (a
     [b,C,H,W] channels_last float32 buffer that gets no gradient; the 5 channels behind it get zeros, the others are
-    not touched): convraw.0's concatenated input.  With img None (a caller that wants conv1 alone) those channels go
-    to a scratch buffer.  Backward: the weight gradient only (pvnet_stem_s2d_wgrad: the 4x4
+    not touched): convraw.0's concatenated input.  With half=True `img` is a [b,C,H/2,W/2] buffer instead and gets
+    x_ds = F.interpolate(image, scale_factor=0.5, mode='bilinear') (torch's CUDA arithmetic, bit for bit; DESIGN.md
+    §21) in those channels: conv2s.0's input in Resnet50_8s_2o.  With img None (a caller that wants conv1 alone)
+    those channels go to a scratch buffer.  Backward: the weight gradient only (pvnet_stem_s2d_wgrad: the 4x4
     gradient on S, all 16 taps per CTA, folded back to [64,3,7,7]).  Saves S only.  Runs on the input's device and
     its current stream."""
 
     @staticmethod
-    def forward(ctx, x, weight, img, co, mean, std):
+    def forward(ctx, x, weight, img, co, mean, std, half):
         _check_float_cuda("StemS2dNHWC", weight, *([] if img is None else [img]))
         is_u8 = x.dtype == torch.uint8
         if is_u8:
@@ -582,12 +589,13 @@ class StemS2dNHWC(torch.autograd.Function):
             mean3 = std3 = None
         if tuple(weight.shape) != (64, 3, 7, 7):
             raise ValueError(f"StemS2dNHWC needs weight [64,3,7,7], got {tuple(weight.shape)}")
+        Hi, Wi = (H // 2, W // 2) if half else (H, W)
         if img is None:
-            img, co = torch.empty(b, 8, H, W, dtype=torch.float32, device=x.device,
+            img, co = torch.empty(b, 8, Hi, Wi, dtype=torch.float32, device=x.device,
                                   memory_format=torch.channels_last), 0
-        if img.dim() != 4 or img.shape[0] != b or tuple(img.shape[2:]) != (H, W) or \
+        if img.dim() != 4 or img.shape[0] != b or tuple(img.shape[2:]) != (Hi, Wi) or \
                 not img.is_contiguous(memory_format=torch.channels_last):
-            raise ValueError(f"img must be a channels_last [{b},C,{H},{W}] buffer, got {tuple(img.shape)}")
+            raise ValueError(f"img must be a channels_last [{b},C,{Hi},{Wi}] buffer, got {tuple(img.shape)}")
         if img.requires_grad:
             raise ValueError("StemS2dNHWC: img gets no gradient, so it must not require one")
         dev = x.device
@@ -597,9 +605,10 @@ class StemS2dNHWC(torch.autograd.Function):
         w4 = pack_stem_s2d_train(weight.detach())
         bias = torch.zeros(64, dtype=torch.float32, device=dev)
         with torch.cuda.device(dev):
-            _native.check(_native.lib().pvnet_stem_s2d_nhwc(
+            fn = "pvnet_stem_s2d_half_nhwc" if half else "pvnet_stem_s2d_nhwc"
+            _native.check(getattr(_native.lib(), fn)(
                 _p(xc), int(is_u8), mean3, std3, _p(w4), _p(bias), _p(s2d), _p(out), _p(img), img.shape[1], co, b, H,
-                W, _stream(dev)), "pvnet_stem_s2d_nhwc")
+                W, _stream(dev)), fn)
         ctx.save_for_backward(s2d)
         ctx.hw = (H, W)
         return out
@@ -608,7 +617,7 @@ class StemS2dNHWC(torch.autograd.Function):
     @once_differentiable
     def backward(ctx, gy):
         if not ctx.needs_input_grad[1]:
-            return None, None, None, None, None, None
+            return None, None, None, None, None, None, None
         s2d, = ctx.saved_tensors
         b = s2d.shape[0]
         H, W = ctx.hw
@@ -619,14 +628,20 @@ class StemS2dNHWC(torch.autograd.Function):
             dw = torch.empty(64, 3, 7, 7, dtype=torch.float32, device=dev)
             _native.check(_native.lib().pvnet_stem_s2d_wgrad(_p(s2d), _p(gyh), _p(dw), b, H, W, _p(ws), ws.numel(),
                                                              _stream(dev)), "pvnet_stem_s2d_wgrad")
-        return None, dw, None, None, None, None
+        return None, dw, None, None, None, None, None
 
 
 def stem_train(x, weight, img=None, co=0, mean=None, std=None):
     """StemS2dNHWC.apply: conv1 (7x7/2, pad 3, no bias) on the native kernels under autograd, of a float image or of a
     raw uint8 image normalised on the device; it also fills convraw.0's image and pad channels [co, co+8) of `img`
     when one is given (see StemS2dNHWC)."""
-    return StemS2dNHWC.apply(x, weight, img, co, mean, std)
+    return StemS2dNHWC.apply(x, weight, img, co, mean, std, False)
+
+
+def stem_train_half(x, weight, img=None, co=0, mean=None, std=None):
+    """stem_train for Resnet50_8s_2o: channels [co, co+8) of an H/2 x W/2 `img` get x_ds and 5 zeros, conv2s.0's image
+    and pad channels (see StemS2dNHWC, half=True)."""
+    return StemS2dNHWC.apply(x, weight, img, co, mean, std, True)
 
 
 class MaxPool3x3s2NHWC(torch.autograd.Function):

@@ -13,8 +13,11 @@
 //                            reads the two dense parts as its two sources (ConvDesc::in2)
 //
 // The plan -- conv slots, workspace buffers, stage list -- is generated once per handle from the trunk description
-// (block kind, blocks per stage, decoder widths) by `generate`; for the 2-2-2-2 BasicBlock trunk it is the
-// Resnet18_8s plan: slots, buffer order and sizes, and launches.
+// (block kind, blocks per stage, decoder widths) and the decoder kind by `generate`; for the 2-2-2-2 BasicBlock trunk
+// and the full-resolution decoder it is the Resnet18_8s plan: slots, buffer order and sizes, and launches.
+// The half-resolution decoder (Resnet50_8s_2o, model_repository.py:158-224) ends at conv2s: C1, R0 and the x2
+// upsampling are gone, and conv2s.0 reads C2 plus X [b,H/2,W/2,8] (x_ds, 3 channels, zeros to 8; written by the
+// image pack) as its second source, into U2, which the 1x1 head reads at H/2 x W/2.
 #include "conv_tc.cuh"
 
 #include <string>
@@ -46,18 +49,20 @@ struct Layer {
     int k, stride, dil, act;
     int round_out = 1;
     bool image_src = false;     // convraw.0: second source = the 8-channel image slice behind C1's first part
+    int in2 = -1;               // conv2s.0 of the half-resolution decoder: second source = this dense 8-channel buffer
 };
 
 }  // namespace
 
 struct pvnet_backbone {
-    int ver_dim, seg_dim, fc, s8, s4, s2, raw;
+    int ver_dim, seg_dim, fc, s8, s4, s2, raw;   // raw: the head's input width (s2 in the half-resolution decoder)
+    int half = 0;                        // decoder kind: 1 = Resnet50_8s_2o's, output at H/2 x W/2
     int nconv = 0;                       // conv slots, the head included (the last slot)
     std::vector<const float *> w, bias;
     std::vector<BufSpec> bufs;           // in carving order
     std::vector<Layer> layers;           // by slot, the head excluded
     std::vector<Stage> stages;
-    int bS2D, bC1, bR0, bC2, bU2, bP, bC4, bU4, bC8, bU8;   // buffers the non-conv stages use
+    int bS2D, bC1 = -1, bR0 = -1, bX = -1, bC2, bU2, bP, bC4, bU4, bC8, bU8;   // buffers the non-conv stages use
     int c2s, c4s, c8s;                   // channel strides of the concatenation buffers
     // cached plan for one (b,h,w,workspace,in,out) combination
     int pb = 0, ph = 0, pw = 0;
@@ -105,8 +110,12 @@ void generate(pvnet_backbone *m, int bottleneck, const int blocks[4])
     m->c4s = m->s8 + 64 * e;
     m->c8s = m->fc + 128 * e;
     m->bS2D = buf(1, 16);
-    m->bC1 = buf(0, m->s2 + 8);
-    m->bR0 = buf(0, m->raw);
+    if (m->half) {
+        m->bX = buf(1, 8);
+    } else {
+        m->bC1 = buf(0, m->s2 + 8);
+        m->bR0 = buf(0, m->raw);
+    }
     m->bC2 = buf(1, m->c2s);
     m->bU2 = buf(1, m->s2);
     m->bP = buf(2, 64);
@@ -183,6 +192,18 @@ void generate(pvnet_backbone *m, int bottleneck, const int blocks[4])
     m->stages.push_back({ST_UP8, -1, "upsample 1/8->1/4"});
     conv({m->bC4, m->c4s, 0, m->c4s, m->bU4, m->s4, 0, m->s4, -1, 0, 0, 2, 3, 1, 1, 2}, "conv4s.0");
     m->stages.push_back({ST_UP4, -1, "upsample 1/4->1/2"});
+    if (m->half) {
+        // conv2s.0 reads cat[up(conv4s), x2s, x_ds] as C2 and X; its output feeds the fp32 head unrounded
+        Layer c2{m->bC2, m->c2s, 0, m->c2s, m->bU2, m->s2, 0, m->s2, -1, 0, 0, 1, 3, 1, 1, 2};
+        c2.round_out = 0;
+        c2.in2 = m->bX;
+        conv(c2, "conv2s.0");
+        m->nconv = (int)m->layers.size() + 1;
+        m->stages.push_back({ST_HEAD, m->nconv - 1, "conv2s.3 1x1 + argmax head (fp32)"});
+        m->w.assign(m->nconv, nullptr);
+        m->bias.assign(m->nconv, nullptr);
+        return;
+    }
     conv({m->bC2, m->c2s, 0, m->c2s, m->bU2, m->s2, 0, m->s2, -1, 0, 0, 1, 3, 1, 1, 2}, "conv2s.0");
     m->stages.push_back({ST_UP2, -1, "upsample 1/2->1"});
     // convraw.0 reads cat(upsampled features [s2], image [3 -> 8]) from two dense buffers (the first p1*s2 and the
@@ -259,12 +280,21 @@ int build_plans(pvnet_backbone *m, const std::vector<float *> &B, int b, int h, 
             d.in2_cs = 8;
             d.Cin2 = 8;
         }
+        if (l.in2 >= 0) {
+            d.in2 = B[l.in2];
+            d.in2_cs = 8;
+            d.Cin2 = 8;
+        }
         void *st = m->plans.data() + ps * slot;
         const bool col = conv_col_eligible(d);
         m->use_col[slot] = col;
         int rc;
         if (!col) {
             rc = conv_plan_at(d, st);
+        } else if (l.in2 >= 0 && l.cin % 32 == 0 && l.cout == 64) {
+            // conv2s.0 of the half-resolution decoder: 32-channel chunks over C2, X as one 8-channel chunk (s2dim 32
+            // keeps the 8-channel-chunk form)
+            rc = conv_col_plan_split_at(d, st);
         } else if (l.image_src && m->raw == 32 && m->seg_dim + m->ver_dim <= 32) {
             // fuse convraw.3 + argmax into the epilogue; pointers are patched per forward call
             HeadDesc hd{m->w[head], m->bias[head], reinterpret_cast<float *>(0x10), nullptr, 8, m->seg_dim,
@@ -291,9 +321,10 @@ int check_dims(int ver_dim, int seg_dim, int fcdim, int s8dim, int s4dim, int s2
 }
 
 pvnet_backbone *make(int bottleneck, const int blocks[4], int ver_dim, int seg_dim, int fcdim, int s8dim, int s4dim,
-                     int s2dim, int raw_dim)
+                     int s2dim, int raw_dim, int half = 0)
 {
     pvnet_backbone *m = new pvnet_backbone();
+    m->half = half;
     m->ver_dim = ver_dim;
     m->seg_dim = seg_dim;
     m->fc = fcdim;
@@ -319,20 +350,39 @@ int pvnet_backbone_create(int ver_dim, int seg_dim, int fcdim, int s8dim, int s4
     return PVNET_OK;
 }
 
-int pvnet_backbone_create_trunk(int block_kind, const int *blocks, int ver_dim, int seg_dim, int fcdim, int s8dim,
-                                int s4dim, int s2dim, int raw_dim, pvnet_backbone_t **out)
+static int check_trunk(int block_kind, const int *blocks)
 {
-    if (int rc = check_dims(ver_dim, seg_dim, fcdim, s8dim, s4dim, s2dim, out)) return rc;
     PV_CHECK_ARG(block_kind == PVNET_BLOCK_BASIC || block_kind == PVNET_BLOCK_BOTTLENECK,
                  "block kind must be %d (BasicBlock) or %d (Bottleneck), got %d", PVNET_BLOCK_BASIC,
                  PVNET_BLOCK_BOTTLENECK, block_kind);
     PV_CHECK_ARG(blocks, "null block counts");
     for (int s = 0; s < 4; ++s)
         PV_CHECK_ARG(blocks[s] >= 1 && blocks[s] <= 64, "stage %d: %d blocks, must be in [1,64]", s + 1, blocks[s]);
+    return PVNET_OK;
+}
+
+int pvnet_backbone_create_trunk(int block_kind, const int *blocks, int ver_dim, int seg_dim, int fcdim, int s8dim,
+                                int s4dim, int s2dim, int raw_dim, pvnet_backbone_t **out)
+{
+    if (int rc = check_dims(ver_dim, seg_dim, fcdim, s8dim, s4dim, s2dim, out)) return rc;
+    if (int rc = check_trunk(block_kind, blocks)) return rc;
     PV_CHECK_ARG(raw_dim == 32 || raw_dim == 64, "raw_dim must be 32 or 64 (head kernel), got %d", raw_dim);
     *out = make(block_kind == PVNET_BLOCK_BOTTLENECK, blocks, ver_dim, seg_dim, fcdim, s8dim, s4dim, s2dim, raw_dim);
     return PVNET_OK;
 }
+
+int pvnet_backbone_create_trunk_2o(int block_kind, const int *blocks, int ver_dim, int seg_dim, int fcdim, int s8dim,
+                                   int s4dim, int s2dim, pvnet_backbone_t **out)
+{
+    if (int rc = check_dims(ver_dim, seg_dim, fcdim, s8dim, s4dim, s2dim, out)) return rc;
+    if (int rc = check_trunk(block_kind, blocks)) return rc;
+    PV_CHECK_ARG(s2dim == 32 || s2dim == 64, "s2dim must be 32 or 64 (the head reads conv2s.0's output), got %d",
+                 s2dim);
+    *out = make(block_kind == PVNET_BLOCK_BOTTLENECK, blocks, ver_dim, seg_dim, fcdim, s8dim, s4dim, s2dim, s2dim, 1);
+    return PVNET_OK;
+}
+
+int pvnet_backbone_output_scale(const pvnet_backbone_t *m) { return m ? (m->half ? 2 : 1) : -1; }
 
 void pvnet_backbone_destroy(pvnet_backbone_t *m) { delete m; }
 
@@ -403,11 +453,12 @@ int run_stage(pvnet_backbone *m, const Stage &st, const std::vector<float *> &B,
               int w, float *out_nchw, void *mask_out, int mask_elem_size, cudaStream_t s)
 {
     const int h2 = h / 2, w2 = w / 2, h4 = h / 4, w4 = w / 4, h8 = h / 8, w8 = w / 8;
-    float *C1 = B[m->bC1];
+    float *C1 = m->half ? nullptr : B[m->bC1];
     switch (st.kind) {
     case ST_PACK:
+        if (m->half) return launch_s2d_pack(img.ptr, img.is_u8, img.mean, img.std, B[m->bS2D], B[m->bX], b, h, w, 8, 0, 1, s);
         return launch_s2d_pack(img.ptr, img.is_u8, img.mean, img.std, B[m->bS2D], C1 + (size_t)b * h * w * m->s2, b, h,
-                               w, 8, 0, s);
+                               w, 8, 0, 0, s);
     case ST_POOL: return launch_maxpool(B[m->bC2], B[m->bP], b, h2, w2, 64, m->c2s, m->s4, s);
     case ST_CONV: {
         unsigned char *pl = m->plans.data() + plan_stride() * st.slot;
@@ -421,6 +472,9 @@ int run_stage(pvnet_backbone *m, const Stage &st, const std::vector<float *> &B,
     case ST_UP2: return launch_upsample2x(B[m->bU2], C1, b, h2, w2, m->s2, m->s2, 0, s);
     case ST_HEAD:
         if (m->head_fused) return PVNET_OK;    // already written by convraw.0's epilogue
+        if (m->half)
+            return launch_head(B[m->bU2], m->raw, m->w[st.slot], m->bias[st.slot], out_nchw, mask_out, mask_elem_size,
+                               m->seg_dim, m->seg_dim + m->ver_dim, b, h2, w2, m->out_nhwc, s);
         return launch_head(B[m->bR0], m->raw, m->w[st.slot], m->bias[st.slot], out_nchw, mask_out, mask_elem_size,
                            m->seg_dim, m->seg_dim + m->ver_dim, b, h, w, m->out_nhwc, s);
     }

@@ -22,10 +22,13 @@ namespace pvnet {
 // quarter of the input bytes.
 // RAW = true (the training stem, pvnet_stem_s2d_nhwc): the image slice gets the fp32 image values unrounded (the
 // normalised values for a uint8 input), the image convraw.0 reads in training; S stays TF32-rounded.
+// HALF = true (Resnet50_8s_2o): instead of the full-resolution image slice, `out` [b,H/2,W/2,out_cs] gets at out_co
+// x_ds = F.interpolate(image, scale_factor=0.5, mode='bilinear') (3 channels + 5 zeros), the average of the 2x2 block
+// this thread already holds, in the rounding sequence of torch's CUDA kernel (DESIGN.md §21); TF32-rounded unless RAW.
 struct Norm3 {
     float mean[3], std[3];
 };
-template <bool U8, bool RAW = false>
+template <bool U8, bool RAW = false, bool HALF = false>
 __global__ void __launch_bounds__(128)
     k_s2d_pack(const void *__restrict__ in_v, Norm3 nrm, float *__restrict__ s2d, float *__restrict__ out, int H, int W,
                int out_cs, int out_co)
@@ -64,7 +67,7 @@ __global__ void __launch_bounds__(128)
                     for (int c = 0; c < 3; ++c) {
                         const float t = __fdiv_rn(__fsub_rn(__fdiv_rn((float)bytes[px * 3 + c], 255.f), nrm.mean[c]), nrm.std[c]);
                         v[(py * 2 + px) * 3 + c] = ptx::round_tf32(t);
-                        if constexpr (RAW) raw[(py * 2 + px) * 3 + c] = t;
+                        if constexpr (RAW || HALF) raw[(py * 2 + px) * 3 + c] = t;
                     }
             }
         } else {
@@ -76,7 +79,7 @@ __global__ void __launch_bounds__(128)
                     const float2 q = __ldg(reinterpret_cast<const float2 *>(src + c * plane + py * W));
                     v[(py * 2 + 0) * 3 + c] = ptx::round_tf32(q.x);
                     v[(py * 2 + 1) * 3 + c] = ptx::round_tf32(q.y);
-                    if constexpr (RAW) {
+                    if constexpr (RAW || HALF) {
                         raw[(py * 2 + 0) * 3 + c] = q.x;
                         raw[(py * 2 + 1) * 3 + c] = q.y;
                     }
@@ -86,8 +89,23 @@ __global__ void __launch_bounds__(128)
 #pragma unroll
         for (int j = 0; j < 4; ++j)
             sS[t * 4 + (j ^ ((t >> 1) & 3))] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
+        if constexpr (HALF) {
+            // torch's upsample_bilinear2d_out_frame at source 2i + 0.5 (every weight 0.5):
+            // h0 * (w0 * a + w1 * b) + h1 * (w0 * c + w1 * d), products exact
+            float xd[3];
 #pragma unroll
-        for (int py = 0; py < 2; ++py)
+            for (int c = 0; c < 3; ++c) {
+                const float t0 = __fadd_rn(__fmul_rn(0.5f, raw[c]), __fmul_rn(0.5f, raw[3 + c]));
+                const float t1 = __fadd_rn(__fmul_rn(0.5f, raw[6 + c]), __fmul_rn(0.5f, raw[9 + c]));
+                const float m = __fadd_rn(__fmul_rn(0.5f, t0), __fmul_rn(0.5f, t1));
+                xd[c] = RAW ? m : ptx::round_tf32(m);
+            }
+            float4 *o = reinterpret_cast<float4 *>(out + ((size_t)blockIdx.y * W2 + x2) * out_cs + out_co);
+            o[0] = make_float4(xd[0], xd[1], xd[2], 0.f);
+            o[1] = make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+#pragma unroll
+        for (int py = 0; py < 2 && !HALF; ++py)
 #pragma unroll
             for (int px = 0; px < 2; ++px) {
                 const int b = (py * 2 + px) * 3;
@@ -107,7 +125,7 @@ __global__ void __launch_bounds__(128)
     }
     // image slice: lane pairs write the 32 bytes (3 channels + 5 zeros) of one full-resolution pixel
 #pragma unroll
-    for (int py = 0; py < 2; ++py) {
+    for (int py = 0; py < 2 && !HALF; ++py) {
         float *orow = out + (((size_t)n * H + 2 * y2 + py) * W + 2 * xb) * out_cs + out_co;
 #pragma unroll
         for (int r = 0; r < 4; ++r) {
@@ -120,7 +138,7 @@ __global__ void __launch_bounds__(128)
 }
 
 int launch_s2d_pack(const void *in, int in_is_u8, const float *mean3, const float *std3, float *s2d, float *out, int b,
-                    int H, int W, int out_cs, int out_co, cudaStream_t s)
+                    int H, int W, int out_cs, int out_co, int half, cudaStream_t s)
 {
     dim3 grid((unsigned)((W / 2 + 127) / 128), (unsigned)(b * (H / 2)));
     Norm3 nrm{};
@@ -129,7 +147,12 @@ int launch_s2d_pack(const void *in, int in_is_u8, const float *mean3, const floa
             nrm.mean[c] = mean3[c];
             nrm.std[c] = std3[c];
         }
-        k_s2d_pack<true><<<grid, 128, 0, s>>>(in, nrm, s2d, out, H, W, out_cs, out_co);
+        if (half)
+            k_s2d_pack<true, false, true><<<grid, 128, 0, s>>>(in, nrm, s2d, out, H, W, out_cs, out_co);
+        else
+            k_s2d_pack<true><<<grid, 128, 0, s>>>(in, nrm, s2d, out, H, W, out_cs, out_co);
+    } else if (half) {
+        k_s2d_pack<false, false, true><<<grid, 128, 0, s>>>(in, nrm, s2d, out, H, W, out_cs, out_co);
     } else {
         k_s2d_pack<false><<<grid, 128, 0, s>>>(in, nrm, s2d, out, H, W, out_cs, out_co);
     }
@@ -647,9 +670,13 @@ int pvnet_maxpool3x3s2_backward_nhwc(const float *dout, const uint8_t *code, flo
     return PVNET_OK;
 }
 
-int pvnet_stem_s2d_nhwc(const void *image, int image_is_u8, const float *mean3, const float *std3, const float *w_s2d,
-                        const float *bias, float *s2d, float *out, float *img, int img_cs, int img_co, int b, int H,
-                        int W, pvnet_stream_t stream)
+}  // extern "C"
+
+// pvnet_stem_s2d_nhwc (half = 0: the image slice of img at full resolution) and pvnet_stem_s2d_half_nhwc (half = 1:
+// x_ds of img at H/2 x W/2)
+static int stem_s2d(const void *image, int image_is_u8, const float *mean3, const float *std3, const float *w_s2d,
+                    const float *bias, float *s2d, float *out, float *img, int img_cs, int img_co, int b, int H, int W,
+                    int half, pvnet_stream_t stream)
 {
     PV_CHECK_ARG(image && w_s2d && bias && s2d && out && img, "stem: null pointer");
     PV_CHECK_ARG(image_is_u8 ? mean3 && std3 : !mean3 && !std3,
@@ -677,18 +704,40 @@ int pvnet_stem_s2d_nhwc(const void *image, int image_is_u8, const float *mean3, 
         const int nb = std::min(per, b - n0);
         const dim3 grid((unsigned)((W / 2 + 127) / 128), (unsigned)(nb * (H / 2)));
         const size_t in0 = (size_t)n0 * 3 * H * W;
-        float *s2d0 = s2d + (size_t)n0 * (H / 2) * (W / 2) * 16, *img0 = img + (size_t)n0 * H * W * img_cs;
-        if (image_is_u8)
-            pvnet::k_s2d_pack<true, true><<<grid, 128, 0, (cudaStream_t)stream>>>(
-                static_cast<const uint8_t *>(image) + in0, nrm, s2d0, img0, H, W, img_cs, img_co);
+        float *s2d0 = s2d + (size_t)n0 * (H / 2) * (W / 2) * 16;
+        float *img0 = img + (size_t)n0 * (half ? (size_t)(H / 2) * (W / 2) : (size_t)H * W) * img_cs;
+        cudaStream_t st = (cudaStream_t)stream;
+        const void *im0 = image_is_u8 ? (const void *)(static_cast<const uint8_t *>(image) + in0)
+                                      : (const void *)(static_cast<const float *>(image) + in0);
+        if (image_is_u8 && half)
+            pvnet::k_s2d_pack<true, true, true><<<grid, 128, 0, st>>>(im0, nrm, s2d0, img0, H, W, img_cs, img_co);
+        else if (image_is_u8)
+            pvnet::k_s2d_pack<true, true><<<grid, 128, 0, st>>>(im0, nrm, s2d0, img0, H, W, img_cs, img_co);
+        else if (half)
+            pvnet::k_s2d_pack<false, true, true><<<grid, 128, 0, st>>>(im0, nrm, s2d0, img0, H, W, img_cs, img_co);
         else
-            pvnet::k_s2d_pack<false, true><<<grid, 128, 0, (cudaStream_t)stream>>>(
-                static_cast<const float *>(image) + in0, nrm, s2d0, img0, H, W, img_cs, img_co);
+            pvnet::k_s2d_pack<false, true><<<grid, 128, 0, st>>>(im0, nrm, s2d0, img0, H, W, img_cs, img_co);
         PV_LAUNCHED("k_s2d_pack");
     }
     // the 7x7/2 convolution as the 4x4 stride-1 convolution on S (taps at offsets -2..1): the eval path's instantiation
     return pvnet_conv2d_nhwc(s2d, 16, 0, 16, w_s2d, bias, nullptr, 0, 0, out, 64, 0, 64, b, H / 2, W / 2, 4, 1, 1, 0,
                              0, stream);
+}
+
+extern "C" {
+
+int pvnet_stem_s2d_nhwc(const void *image, int image_is_u8, const float *mean3, const float *std3, const float *w_s2d,
+                        const float *bias, float *s2d, float *out, float *img, int img_cs, int img_co, int b, int H,
+                        int W, pvnet_stream_t stream)
+{
+    return stem_s2d(image, image_is_u8, mean3, std3, w_s2d, bias, s2d, out, img, img_cs, img_co, b, H, W, 0, stream);
+}
+
+int pvnet_stem_s2d_half_nhwc(const void *image, int image_is_u8, const float *mean3, const float *std3,
+                             const float *w_s2d, const float *bias, float *s2d, float *out, float *img, int img_cs,
+                             int img_co, int b, int H, int W, pvnet_stream_t stream)
+{
+    return stem_s2d(image, image_is_u8, mean3, std3, w_s2d, bias, s2d, out, img, img_cs, img_co, b, H, W, 1, stream);
 }
 
 }  // extern "C"

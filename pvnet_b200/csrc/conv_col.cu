@@ -18,10 +18,12 @@
 //     in shared memory and stored by the producer warpgroup's otherwise idle warps while the next tile's MMAs
 //     run -- the [b,H,W,32] intermediate never exists.
 //
-// k_conv_col<KC, HEAD, KH, BN, WIDE> is instantiated per layer form, eight in all: 3x3 taps with 32- or 8-channel
-// chunks and BN = Cout 32 or 64; the stem's 4x4 taps with 16-channel chunks, BN 32 or 64; and convraw.0's fused
+// k_conv_col<KC, HEAD, KH, BN, WIDE, SPLIT8> is instantiated per layer form, nine in all: 3x3 taps with 32- or
+// 8-channel chunks and BN = Cout 32 or 64; the stem's 4x4 taps with 16-channel chunks, BN 32 or 64; convraw.0's fused
 // head (HEAD, 8-channel chunks, BN 32), with or without WIDE, its two-source input with the 32-channel first source
-// loaded as one 128-byte-swizzled box.  conv_col_launch_at picks the instantiation a plan was made for.
+// loaded as one 128-byte-swizzled box; and SPLIT8 (32-channel chunks, BN 64): Resnet50_8s_2o's conv2s.0, whose first
+// source runs in 32-channel chunks and whose 8-channel second source is one more chunk.  conv_col_launch_at picks the
+// instantiation a plan was made for.
 #include "conv_tc.cuh"
 #include "ptx.cuh"
 
@@ -124,7 +126,10 @@ __device__ __forceinline__ void head_store_tile(const ColGeom &g, uint32_t sv, u
 // 128-byte-swizzled box, with their weights as 128-byte-swizzled [32][32] tiles, and the MMAs still run chunk by
 // chunk, tap by tap, so every output sums the same products in the same order as with 8-channel boxes.  The
 // 32-byte-swizzled operands of 8-channel chunks ran the same MMAs at about half the rate (DESIGN.md section 6).
-template <int KC, bool HEAD, int KH, int BN, bool WIDE = false>
+// SPLIT8 (KC = 32, weights not resident): chunk split_chunk, the last, is the second source's 8 channels: a box of
+// 32-byte rows from tmA2 with its KH*KH [BN][8] weight tiles (32-byte swizzle, tmBw) in the same stage.  The first
+// source keeps 128-byte rows, so a 192 + 8 channel input does not fall back to 8-channel chunks (DESIGN.md §21).
+template <int KC, bool HEAD, int KH, int BN, bool WIDE = false, bool SPLIT8 = false>
 __global__ void __launch_bounds__(COL_THREADS, 1)
     k_conv_col(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
                const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmBw, const __grid_constant__ ColGeom g,
@@ -136,6 +141,7 @@ __global__ void __launch_bounds__(COL_THREADS, 1)
     static_assert(!HEAD || KC == 8, "fused head: convraw.0's 8-channel chunks");
     static_assert((KC == 16) == (KH == 4), "16-channel chunks are the 4x4 stem's, and only its");
     static_assert(!WIDE || (HEAD && KC == 8 && KH == 3), "wide first source: convraw.0 form only");
+    static_assert(!SPLIT8 || (!HEAD && !WIDE && KC == 32 && KH == 3), "split chunks: 32-channel first source, 3x3");
     constexpr int ROWB = KC * 4;                       // bytes per K-major row
     constexpr int B_TILE = BN * ROWB;                  // one [BN][KC] weight tile (a multiple of 1024 bytes)
     constexpr int PITCH = COL_TW + KH - 1;             // box pitch in pixels (= shared-memory rows)
@@ -145,6 +151,8 @@ __global__ void __launch_bounds__(COL_THREADS, 1)
     // a box of 32-byte rows; a stage is sized for the wide box
     constexpr int WIDE_BOX = (COL_TH + KH - 1) * PITCH * 128;
     constexpr int WIDE_BYTES = (WIDE_BOX + 1023) & ~1023;
+    // SPLIT8: the 8-channel chunk's box and weight tile (32-byte rows)
+    constexpr int T_A_BOX = (COL_TH + KH - 1) * PITCH * 32, T_B_TILE = BN * 32;
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     const int n_btiles = KH * KH * g.cin_chunks;
@@ -243,6 +251,15 @@ __global__ void __launch_bounds__(COL_THREADS, 1)
                         ptx::tma_load_4d(st, cc == 0 ? &tmA : &tmA2, &full[s], 0, x0 - g.pad_l, y0 - g.pad_t, img);
                     }
                     __syncwarp();
+                } else if (SPLIT8 && cc == g.split_chunk) {
+                    if (lane == 0) {
+                        ptx::mbar_wait(&empty[s], ph ^ 1u);
+                        ptx::mbar_arrive_expect_tx(&full[s], (uint32_t)(T_A_BOX + KH * KH * T_B_TILE));
+                        ptx::tma_load_4d(st, &tmA2, &full[s], 0, x0 - g.pad_l, y0 - g.pad_t, img);
+                        for (int t = 0; t < KH * KH; ++t)
+                            ptx::tma_load_2d(st + A_BYTES + (size_t)t * T_B_TILE, &tmBw, &full[s], t * g.cin_pad + cc * KC, 0);
+                    }
+                    __syncwarp();
                 } else if (pw == 0) {
                     if (lane == 0) {
                         ptx::mbar_wait(&empty[s], ph ^ 1u);
@@ -297,6 +314,14 @@ __global__ void __launch_bounds__(COL_THREADS, 1)
                     for (int t = 0; t < KH * KH; ++t)
                         ptx::Wgmma<BN>::ss(acc, ad0 + (uint64_t)(((t / KH) * PITCH + t % KH) * 128 / 16 + 2 * ks),
                                            bd0 + (uint64_t)(t * (BN * 128) / 16 + 2 * ks), (t | ks) != 0 ? 1u : 0u);
+            } else if (SPLIT8 && cc == g.split_chunk) {
+                // the second source's 8 channels, tap by tap, after every chunk of the first
+                const uint64_t ad0 = ptx::make_kmajor_desc(a0 + (uint32_t)(8 * wg * PITCH * 32), 32, PITCH * 32);
+                const uint64_t bd0 = ptx::make_kmajor_desc(a0 + (uint32_t)A_BYTES, 32);
+#pragma unroll
+                for (int t = 0; t < KH * KH; ++t)
+                    ptx::Wgmma<BN>::ss(acc, ad0 + (uint64_t)(((t / KH) * PITCH + t % KH) * 32 / 16),
+                                       bd0 + (uint64_t)(t * T_B_TILE / 16), 1u);
             } else {
                 const int c8 = WIDE ? g.split_chunk : cc;      // the chunk's index in 8-channel units
                 const uint32_t b0 = g.resident ? sB_u + (uint32_t)(c8 * KH * KH * B_TILE) : a0 + (uint32_t)A_BYTES;
@@ -444,7 +469,7 @@ __global__ void __launch_bounds__(COL_THREADS, 1)
 struct ColPlan {
     CUtensorMap tmA, tmA2, tmB, tmBw;
     ColGeom g;
-    int kc, ksize, head, bn, wide;
+    int kc, ksize, head, bn, wide, split8;
     unsigned grid;
     size_t smem;
     const float *bias, *res;
@@ -469,15 +494,16 @@ size_t col_smem(int kc, int ksize, int cin_chunks, int bn, int stages, bool head
            (size_t)(1 + 2 * stages) * 8 + (64 + 32) * 4;
 }
 
-template <int KC, bool HEAD, int KH, int BN, bool WIDE = false>
+template <int KC, bool HEAD, int KH, int BN, bool WIDE = false, bool SPLIT8 = false>
 int col_launch(const ColPlan &p, cudaStream_t s)
 {
     // the instantiation must be the plan's: weight boxes, barrier byte counts and stores are sized by BN
-    if (p.bn != BN || p.kc != KC || p.ksize != KH || p.head != (HEAD ? 1 : 0) || p.wide != (WIDE ? 1 : 0)) {
+    if (p.bn != BN || p.kc != KC || p.ksize != KH || p.head != (HEAD ? 1 : 0) || p.wide != (WIDE ? 1 : 0) ||
+        p.split8 != (SPLIT8 ? 1 : 0)) {
         set_error("conv(col): no kernel instantiation for this plan (Cout %d, chunk %d, ksize %d)", p.bn, p.kc, p.ksize);
         return PVNET_E_STATE;
     }
-    auto fn = k_conv_col<KC, HEAD, KH, BN, WIDE>;
+    auto fn = k_conv_col<KC, HEAD, KH, BN, WIDE, SPLIT8>;
     const cudaError_t attr_err = ensure_max_smem((const void *)fn, (int)SMEM_LIMIT);
     PV_CUDA(attr_err);
     const HeadDesc &h = p.hd;
@@ -504,7 +530,9 @@ bool conv_col_eligible(const ConvDesc &d)
 
 size_t conv_col_plan_size() { return sizeof(ColPlan); }
 
-int conv_col_plan_at(const ConvDesc &d, const HeadDesc *head, void *storage)
+namespace {
+
+int plan_at(const ConvDesc &d, const HeadDesc *head, bool split8, void *storage)
 {
     ColPlan *p = new (storage) ColPlan();
     PV_CHECK_ARG(conv_col_eligible(d), "conv(col): layer not eligible for the column kernel");
@@ -515,7 +543,12 @@ int conv_col_plan_at(const ConvDesc &d, const HeadDesc *head, void *storage)
     PV_CHECK_ARG(!head || (d.Cout == 32 && col_kc(d.Cin + d.Cin2) == 8 && head->cout >= 1 && head->cout <= 32 && head->w && head->bias &&
                            head->out_nchw && (!head->mask || head->mask_esz == 1 || head->mask_esz == 8)),
                  "conv(col): bad fused-head description");
-    const int kc = col_kc(d.Cin + d.Cin2);
+    // split chunks: the first source in 32-channel chunks, the 8-channel second source as one more chunk, weights
+    // streamed with each stage (their [Cout][taps][cin_pad] packing is the single-chunk-size one: cin_pad rounds
+    // Cin + 8 up to 32, the second source's weights start at column Cin of each tap)
+    PV_CHECK_ARG(!split8 || (!head && d.in2 && d.Cin % 32 == 0 && d.Cin2 == 8 && d.Cout == 64 && d.ksize == 3),
+                 "conv(col): split chunks need a 32-channel-multiple first source, an 8-channel second, Cout 64, 3x3");
+    const int kc = split8 ? 32 : col_kc(d.Cin + d.Cin2);
     ColGeom &g = p->g;
     g.pad_l = g.pad_t = d.ksize == 4 ? 2 : 1;
     g.Ho = d.H;
@@ -523,7 +556,7 @@ int conv_col_plan_at(const ConvDesc &d, const HeadDesc *head, void *storage)
     g.tiles_x = (d.W + COL_TW - 1) / COL_TW;
     g.tiles_y = (d.H + COL_TH - 1) / COL_TH;
     g.total_tiles = g.tiles_x * g.tiles_y * d.b;
-    g.cin_chunks = (d.Cin + d.Cin2) / kc;
+    g.cin_chunks = split8 ? d.Cin / kc + 1 : (d.Cin + d.Cin2) / kc;
     g.split_chunk = d.in2 ? d.Cin / kc : g.cin_chunks;
     g.cin_pad = col_cin_pad(d.Cin + d.Cin2);   // weights are packed [Cout][KH][KW][cin_pad], zero padded
     g.out_cs = d.out_cs;
@@ -549,7 +582,7 @@ int conv_col_plan_at(const ConvDesc &d, const HeadDesc *head, void *storage)
     bool resident = true;
     while (stages > 2 && col_smem(kc, d.ksize, g.cin_chunks, d.Cout, stages, hd, true) + hs + (wide ? stages * wx : 0) > SMEM_LIMIT)
         --stages;
-    if (col_smem(kc, d.ksize, g.cin_chunks, d.Cout, stages, hd, true) + hs + (wide ? stages * wx : 0) > SMEM_LIMIT) {
+    if (split8 || col_smem(kc, d.ksize, g.cin_chunks, d.Cout, stages, hd, true) + hs + (wide ? stages * wx : 0) > SMEM_LIMIT) {
         wide = false;
         resident = false;
         stages = 8;
@@ -559,6 +592,7 @@ int conv_col_plan_at(const ConvDesc &d, const HeadDesc *head, void *storage)
     g.resident = resident ? 1 : 0;
     p->smem = col_smem(kc, d.ksize, g.cin_chunks, d.Cout, stages, hd, resident) + hs + (wide ? stages * wx : 0);
     p->wide = wide ? 1 : 0;
+    p->split8 = split8 ? 1 : 0;
     PV_CHECK_ARG(p->smem <= SMEM_LIMIT, "conv(col): layer does not fit in shared memory");
     p->kc = kc;
     p->ksize = d.ksize;
@@ -581,8 +615,9 @@ int conv_col_plan_at(const ConvDesc &d, const HeadDesc *head, void *storage)
         cuuint64_t dims[4] = {(cuuint64_t)d.Cin2, (cuuint64_t)d.W, (cuuint64_t)d.H, (cuuint64_t)d.b};
         cuuint64_t strides[3] = {(cuuint64_t)d.in2_cs * 4, (cuuint64_t)d.W * d.in2_cs * 4,
                                  (cuuint64_t)d.H * d.W * d.in2_cs * 4};
-        cuuint32_t box[4] = {(cuuint32_t)kc, (cuuint32_t)(COL_TW + d.ksize - 1), (cuuint32_t)(COL_TH + d.ksize - 1), 1};
-        int rc = tma_encode(&p->tmA2, d.in2 + d.in2_co, 4, dims, strides, box, kc * 4);
+        const int kc2 = split8 ? 8 : kc;
+        cuuint32_t box[4] = {(cuuint32_t)kc2, (cuuint32_t)(COL_TW + d.ksize - 1), (cuuint32_t)(COL_TH + d.ksize - 1), 1};
+        int rc = tma_encode(&p->tmA2, d.in2 + d.in2_co, 4, dims, strides, box, kc2 * 4);
         if (rc) return rc;
     }
     {
@@ -596,6 +631,10 @@ int conv_col_plan_at(const ConvDesc &d, const HeadDesc *head, void *storage)
             box[0] = 32;
             if ((rc = tma_encode(&p->tmBw, d.w, 2, dims, strides, box, 128))) return rc;
         }
+        if (split8) {
+            box[0] = 8;
+            if ((rc = tma_encode(&p->tmBw, d.w, 2, dims, strides, box, 32))) return rc;
+        }
     }
     PV_CHECK_ARG(!head || (uintptr_t)head->w % 16 == 0, "conv(col): head weights must be 16-byte aligned");
     long long grid = (long long)sm_count();
@@ -606,6 +645,12 @@ int conv_col_plan_at(const ConvDesc &d, const HeadDesc *head, void *storage)
     p->out = d.out;
     return PVNET_OK;
 }
+
+}  // namespace
+
+int conv_col_plan_at(const ConvDesc &d, const HeadDesc *head, void *storage) { return plan_at(d, head, false, storage); }
+
+int conv_col_plan_split_at(const ConvDesc &d, void *storage) { return plan_at(d, nullptr, true, storage); }
 
 void conv_col_set_head_ptrs(void *storage, float *out_nchw, void *mask, int mask_esz, int nhwc)
 {
@@ -621,6 +666,7 @@ int conv_col_launch_at(const void *storage, cudaStream_t s)
 {
     const ColPlan &p = *static_cast<const ColPlan *>(storage);
     if (p.wide) return col_launch<8, true, 3, 32, true>(p, s);
+    if (p.split8) return col_launch<32, false, 3, 64, false, true>(p, s);
     if (p.head) return col_launch<8, true, 3, 32>(p, s);
     const bool n64 = p.bn == 64;
     if (p.ksize == 4) return n64 ? col_launch<16, false, 4, 64>(p, s) : col_launch<16, false, 4, 32>(p, s);

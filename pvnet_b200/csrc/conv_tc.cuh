@@ -47,6 +47,9 @@ extern int g_conv_mode;
 bool conv_col_eligible(const ConvDesc &d);
 size_t conv_col_plan_size();
 int conv_col_plan_at(const ConvDesc &d, const HeadDesc *head, void *plan_storage);
+// The same for a two-source layer with Cin a multiple of 32, Cin2 == 8 and Cout 64 (Resnet50_8s_2o's conv2s.0): the
+// first source in 32-channel chunks and the second as one more 8-channel chunk, instead of 8-channel chunks throughout.
+int conv_col_plan_split_at(const ConvDesc &d, void *plan_storage);
 int conv_col_launch_at(const void *plan_storage, cudaStream_t s);
 void conv_col_set_head_ptrs(void *plan_storage, float *out, void *mask, int mask_esz, int nhwc);
 
@@ -55,8 +58,9 @@ size_t conv_plan_size();
 int conv_plan_at(const ConvDesc &d, void *plan_storage);
 int conv_launch_at(const void *plan_storage, cudaStream_t s);
 
+// half = 0: out is the full-resolution image slice [b,H,W,out_cs]; 1: x_ds [b,H/2,W/2,out_cs] (Resnet50_8s_2o)
 int launch_s2d_pack(const void *in, int in_is_u8, const float *mean3, const float *std3, float *s2d, float *out, int b,
-                    int H, int W, int out_cs, int out_co, cudaStream_t s);
+                    int H, int W, int out_cs, int out_co, int half, cudaStream_t s);
 int launch_maxpool(const float *in, float *out, int b, int H, int W, int C, int in_cs, int in_co, cudaStream_t s);
 int launch_upsample2x(const float *in, float *out, int b, int h, int w, int C, int out_cs, int out_co,
                       cudaStream_t s);

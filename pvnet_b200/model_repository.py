@@ -1,6 +1,7 @@
-"""`Resnet18_8s`, `Resnet34_8s` and `Resnet50_8s` with the reference's constructors, forward signature and
-state-dict keys (zju3dv/pvnet lib/networks/model_repository.py:7-156,226-300), backed in eval mode by the native
-sm_90a backbone (wgmma implicit-GEMM convs behind include/pvnet_b200.h).  Resnet34_8s keeps its trunk under the
+"""`Resnet18_8s`, `Resnet34_8s`, `Resnet50_8s` and `Resnet50_8s_2o` with the reference's constructors, forward
+signature and state-dict keys (zju3dv/pvnet lib/networks/model_repository.py:7-300), backed in eval mode by the native
+sm_90a backbone (wgmma implicit-GEMM convs behind include/pvnet_b200.h).  Resnet50_8s_2o ends at half resolution
+(conv2s with a 1x1 head, DESIGN.md §21).  Resnet34_8s keeps its trunk under the
 attribute `resnet50_8s`, as the reference does (model_repository.py:246), so its checkpoints load unchanged.
 The notes below are written for Resnet18_8s; the two deeper networks share every mechanism (`_Resnet8s`), with
 raw_dim 64, so their head always runs as the separate fp32 `k_head`.
@@ -35,6 +36,7 @@ import threading
 import weakref
 
 import torch
+import torch.nn.functional as F
 from torch import nn
 
 from . import _native
@@ -130,14 +132,47 @@ class _Resnet8s(nn.Module):
         self.conv4s = nn.Sequential(nn.Conv2d(x4c + s8dim, s4dim, 3, 1, 1, bias=False), nn.BatchNorm2d(s4dim),
                                     nn.LeakyReLU(0.1, True))
         self.up4sto2s = nn.UpsamplingBilinear2d(scale_factor=2)
+        self._init_tail(ver_dim, seg_dim, s4dim, s2dim, raw_dim)
+        self._nat = _NativeState()
+        self._src_key = None         # set on DataParallel replicas: the source module's weight-version key
+        self._frozen = False
+
+    # ------------------------------------------------------------------ the decoder's tail
+    # What follows conv4s differs between the full-resolution networks (conv2s, x2 upsampling, convraw) and
+    # Resnet50_8s_2o (conv2s with a 1x1 head at half resolution).  These hooks and attributes, and _create_handle, are
+    # all that differ.
+    _decoder_slots = _DECODER_SLOTS
+    _image_slot = "convraw.0"       # the convolution that reads the image slice as its second source
+    _head_slot = "convraw.3"        # the 1x1 head with bias
+    _out_scale = 1                  # the output grid is the input's divided by this
+
+    def _init_tail(self, ver_dim, seg_dim, s4dim, s2dim, raw_dim):
+        """conv2s and everything after it (model_repository.py:50-57)."""
         self.conv2s = nn.Sequential(nn.Conv2d(64 + s4dim, s2dim, 3, 1, 1, bias=False), nn.BatchNorm2d(s2dim),
                                     nn.LeakyReLU(0.1, True))
         self.up2storaw = nn.UpsamplingBilinear2d(scale_factor=2)
         self.convraw = nn.Sequential(nn.Conv2d(3 + s2dim, raw_dim, 3, 1, 1, bias=False), nn.BatchNorm2d(raw_dim),
                                      nn.LeakyReLU(0.1, True), nn.Conv2d(raw_dim, seg_dim + ver_dim, 1, 1))
-        self._nat = _NativeState()
-        self._src_key = None         # set on DataParallel replicas: the source module's weight-version key
-        self._frozen = False
+
+    def _tail_torch(self, fm, x2s, x):
+        """The PyTorch graph from conv4s's upsampled output to the head's output."""
+        fm = self.up2storaw(self.conv2s(torch.cat([fm, x2s], 1)))
+        return self.convraw(torch.cat([fm, x], 1))
+
+    def _train_tail_input(self, b, h, w, device):
+        """forward_train: the channels_last input buffer of the image-reading convolution, the channel at which the
+        stem writes the image and its 5 zero channels, and the stem that writes them.  Here convraw.0's cat[fm, image,
+        5 zeros]: pvnet_b200.conv.stem_train fills channels [s2dim, s2dim+8) now, the decoder's upsampling channels
+        [0, s2dim) at the end."""
+        s2dim = self.conv2s[0].out_channels
+        return torch.empty(b, s2dim + 8, h, w, dtype=torch.float32, device=device,
+                           memory_format=torch.channels_last), s2dim, pc.stem_train
+
+    def _train_tail(self, fm, x2s, buf):
+        """forward_train from conv4s's output to the head's input: (head input, head module)."""
+        fm = self._conv_bn_act(self.conv2s, pc.upsample2x_cat(fm, x2s))
+        y = self._conv_bn_act(self.convraw, pc.upsample2x_into(fm, buf), dgrad_channels=fm.shape[1])
+        return y, self.convraw[3]
 
     # ------------------------------------------------------------------ PyTorch graph
     def _trunk(self):
@@ -145,7 +180,7 @@ class _Resnet8s(nn.Module):
 
     def _slots(self):
         """Execution-order (conv, BatchNorm) module names of the native conv slots."""
-        return _trunk_slots(self._trunk(), self._trunk_attr + ".") + _DECODER_SLOTS
+        return _trunk_slots(self._trunk(), self._trunk_attr + ".") + self._decoder_slots
 
     def _create_handle(self, handle):
         """pvnet_backbone_create_trunk for this trunk."""
@@ -159,8 +194,7 @@ class _Resnet8s(nn.Module):
         x2s, x4s, x8s, _x16s, _x32s, xfc = self._trunk()(x)
         fm = self.up8sto4s(self.conv8s(torch.cat([xfc, x8s], 1)))
         fm = self.up4sto2s(self.conv4s(torch.cat([fm, x4s], 1)))
-        fm = self.up2storaw(self.conv2s(torch.cat([fm, x2s], 1)))
-        out = self.convraw(torch.cat([fm, x], 1))
+        out = self._tail_torch(fm, x2s, x)
         return out[:, :self.seg_dim], out[:, self.seg_dim:]
 
     # ------------------------------------------------------------------ native path
@@ -226,7 +260,7 @@ class _Resnet8s(nn.Module):
     def _pack_native(self, device, key):
         L = _native.lib()
         mods = dict(self.named_modules())
-        fcdim, s8dim, s4dim, s2dim, raw_dim = self._dims
+        raw_dim = self._dims[4]
         handle = ctypes.c_void_p()
         self._create_handle(handle)
         keep = []
@@ -243,10 +277,10 @@ class _Resnet8s(nn.Module):
                     packed = pc.pack_stem_s2d(w)
                 elif conv_name == "convraw.3" and raw_dim == 32:   # head: fp32 [cout][32]
                     packed = pc.round_tf32(w.reshape(w.shape[0], w.shape[1]))   # fused path feeds it to a tf32 MMA
-                elif conv_name == "convraw.3":        # head: fp32 [cout][64], exact in k_head
+                elif conv_name == self._head_slot:    # head: fp32 [cout][raw], exact in k_head
                     packed = w.reshape(w.shape[0], w.shape[1]).contiguous()
-                elif conv_name == "convraw.0":        # cat[fm(s2dim), image(3)] -> s2dim+8 input channels
-                    packed = pc.pack_weight(w, cin_pad=pc.cin_padded(s2dim + 8))
+                elif conv_name == self._image_slot:   # cat[features, image(3)] -> features+8 input channels
+                    packed = pc.pack_weight(w, cin_pad=pc.cin_padded(conv.in_channels + 5))
                 else:
                     packed = pc.pack_weight(w)
                 keep += [packed, b]
@@ -256,7 +290,8 @@ class _Resnet8s(nn.Module):
 
     def forward_native(self, x, with_mask=False, mask_dtype=torch.int64, mean=None, std=None, pixel_major=False):
         """x [b,3,H,W] float32 CUDA (normalised) -- or uint8 [b,H,W,3] raw images with `mean`/`std`
-        (normalised on the device) -> out [b,seg+ver,H,W] (and the fused argmax mask).
+        (normalised on the device) -> out [b,seg+ver,H,W] (and the fused argmax mask [b,H,W]); H/2 x W/2 for
+        Resnet50_8s_2o.
         pixel_major=True returns the same values as out [b,H,W,seg+ver] (one contiguous record per pixel:
         `out[..., seg:].view(b,H,W,K,2)` is the contiguous vertex tensor the voting layer likes best)."""
         if not x.is_cuda:
@@ -283,10 +318,12 @@ class _Resnet8s(nn.Module):
                           "pvnet_backbone_workspace_bytes")
             ws = self._workspace(n.value, dev)
             ctot = self.seg_dim + self.ver_dim
-            out = torch.empty([b, h, w, ctot] if pixel_major else [b, ctot, h, w], dtype=torch.float32, device=dev)
+            ho, wo = h // self._out_scale, w // self._out_scale
+            out = torch.empty([b, ho, wo, ctot] if pixel_major else [b, ctot, ho, wo], dtype=torch.float32,
+                              device=dev)
             _native.check(L.pvnet_backbone_set_output_layout(handle, 1 if pixel_major else 0),
                           "pvnet_backbone_set_output_layout")
-            mask = torch.empty([b, h, w], dtype=mask_dtype, device=dev) if with_mask else None
+            mask = torch.empty([b, ho, wo], dtype=mask_dtype, device=dev) if with_mask else None
             stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
             mptr, msz = (None, 0) if mask is None else (mask.data_ptr(), mask.element_size())
             if raw_u8:
@@ -361,10 +398,10 @@ class _Resnet8s(nn.Module):
         return pc.bn_add_relu(bn_last, y, pc.conv2d_train(x, ds[0].weight, ds[0].stride[0], 1), ds[1])
 
     def _check_train_modules(self):
-        """ValueError unless conv1, the max-pool and convraw.3 still have the shapes forward_train's kernels
-        implement."""
+        """ValueError unless conv1, the max-pool and the head (convraw.3; conv2s.3 in Resnet50_8s_2o) still have the
+        shapes forward_train's kernels implement."""
         t = self._trunk()
-        c1, mp, hd = t.conv1, t.maxpool, self.convraw[3]
+        c1, mp, hd = t.conv1, t.maxpool, self.get_submodule(self._head_slot)
         pair = lambda v: tuple(v) if isinstance(v, (tuple, list)) else (v, v)  # noqa: E731
         if not (isinstance(c1, nn.Conv2d) and tuple(c1.weight.shape) == (64, 3, 7, 7) and c1.stride == (2, 2)
                 and c1.padding == (3, 3) and c1.dilation == (1, 1) and c1.groups == 1 and c1.bias is None
@@ -376,7 +413,8 @@ class _Resnet8s(nn.Module):
             raise ValueError("forward_train: the max-pool must be 3x3, stride 2, padding 1, dilation 1, no ceil_mode")
         if not (isinstance(hd, nn.Conv2d) and hd.kernel_size == (1, 1) and hd.stride == (1, 1) and hd.padding == (0, 0)
                 and hd.dilation == (1, 1) and hd.groups == 1 and hd.bias is not None):
-            raise ValueError("forward_train: convraw[3] must be a 1x1 convolution with bias")
+            seq, i = self._head_slot.split(".")
+            raise ValueError(f"forward_train: {seq}[{i}] must be a 1x1 convolution with bias")
 
     def forward_train(self, x, mean=None, std=None):
         """The train-mode forward (`_forward_torch`) with every layer on the native kernels under autograd:
@@ -425,12 +463,8 @@ class _Resnet8s(nn.Module):
         else:
             x = x.float()
             b, h, w = x.shape[0], x.shape[-2], x.shape[-1]      # [b,3,H,W], checked by the stem
-        s2dim = self.conv2s[0].out_channels
-        # convraw.0's input cat[fm, image, 5 zeros]: the stem fills channels [s2dim, s2dim+8) now, the decoder's
-        # upsampling channels [0, s2dim) at the end
-        raw_in = torch.empty(b, s2dim + 8, h, w, dtype=torch.float32, device=x.device,
-                             memory_format=torch.channels_last)
-        x2s = pc.bn_act(t.bn1, pc.stem_train(x, t.conv1.weight, raw_in, s2dim, mean, std), pc.act_of(t.relu))
+        tail_in, co, stem = self._train_tail_input(b, h, w, x.device)
+        x2s = pc.bn_act(t.bn1, stem(x, t.conv1.weight, tail_in, co, mean, std), pc.act_of(t.relu))
         x4s = pc.maxpool_train(x2s)
         for blk in t.layer1:
             x4s = self._block_train(blk, x4s)
@@ -443,9 +477,7 @@ class _Resnet8s(nn.Module):
         xfc = self._conv_bn_act(t.fc, x32s)
         fm = self._conv_bn_act(self.conv8s, torch.cat([xfc, x8s], 1))
         fm = self._conv_bn_act(self.conv4s, pc.upsample2x_cat(fm, x4s))
-        fm = self._conv_bn_act(self.conv2s, pc.upsample2x_cat(fm, x2s))
-        y = self._conv_bn_act(self.convraw, pc.upsample2x_into(fm, raw_in), dgrad_channels=fm.shape[1])
-        head = self.convraw[3]
+        y, head = self._train_tail(fm, x2s, tail_in)
         out = pc.head_train(y, head.weight, head.bias)
         return out[:, :self.seg_dim], out[:, self.seg_dim:]
 
@@ -487,3 +519,46 @@ class Resnet50_8s(_Resnet8s):
 
     def __init__(self, ver_dim, seg_dim, fcdim=384, s8dim=256, s4dim=128, s2dim=64, raw_dim=64):
         super().__init__(resnet50(output_stride=8), ver_dim, seg_dim, fcdim, s8dim, s4dim, s2dim, raw_dim)
+
+
+class Resnet50_8s_2o(_Resnet8s):
+    """The reference's Resnet50_8s_2o (model_repository.py:158-224): Resnet50_8s's trunk, fc, conv8s and conv4s, then
+    conv2s over cat[up(conv4s), x2s, x_ds] -- x_ds = F.interpolate(x, scale_factor=0.5, mode='bilinear') -- with its
+    1x1 head conv2s.3.  The output is at half the input's resolution: [b,seg+ver,H/2,W/2] (mask [b,H/2,W/2]).  There
+    is no convraw and no x2 upsampling to full resolution.  Keypoints voted from this output are in the pixel
+    coordinates of its H/2 x W/2 grid, as the reference's voting layer gives them for this network."""
+    _trunk_attr = "resnet50_8s"
+    _decoder_slots = [("conv8s.0", "conv8s.1"), ("conv4s.0", "conv4s.1"), ("conv2s.0", "conv2s.1"),
+                      ("conv2s.3", None)]
+    _image_slot = "conv2s.0"
+    _head_slot = "conv2s.3"
+    _out_scale = 2
+
+    def __init__(self, ver_dim, seg_dim, fcdim=384, s8dim=256, s4dim=128, s2dim=64):
+        super().__init__(resnet50(output_stride=8), ver_dim, seg_dim, fcdim, s8dim, s4dim, s2dim, None)
+
+    def _init_tail(self, ver_dim, seg_dim, s4dim, s2dim, raw_dim):
+        self.conv2s = nn.Sequential(nn.Conv2d(3 + 64 + s4dim, s2dim, 3, 1, 1, bias=False), nn.BatchNorm2d(s2dim),
+                                    nn.LeakyReLU(0.1, True), nn.Conv2d(s2dim, seg_dim + ver_dim, 1, 1))
+
+    def _tail_torch(self, fm, x2s, x):
+        x_ds = F.interpolate(x, scale_factor=0.5, mode="bilinear", align_corners=False)
+        return self.conv2s(torch.cat([fm, x2s, x_ds], 1))
+
+    def _create_handle(self, handle):
+        t = self._trunk()
+        blocks = (ctypes.c_int * 4)(*(len(getattr(t, f"layer{i}")) for i in range(1, 5)))
+        _native.check(_native.lib().pvnet_backbone_create_trunk_2o(1, blocks, self.ver_dim, self.seg_dim,
+                                                                   *self._dims[:4], ctypes.byref(handle)),
+                      "pvnet_backbone_create_trunk_2o")
+
+    def _train_tail_input(self, b, h, w, device):
+        """conv2s.0's cat[up(conv4s), x2s, x_ds, 5 zeros] at H/2 x W/2: pvnet_b200.conv.stem_train_half writes x_ds
+        and the zeros into channels [s4dim+64, s4dim+72) now, the decoder the channels before them at the end."""
+        c = self.conv2s[0].in_channels + 5
+        return torch.empty(b, c, h // 2, w // 2, dtype=torch.float32, device=device,
+                           memory_format=torch.channels_last), c - 8, pc.stem_train_half
+
+    def _train_tail(self, fm, x2s, buf):
+        y = self._conv_bn_act(self.conv2s, pc.upsample2x_into(fm, buf, x2s), dgrad_channels=buf.shape[1] - 8)
+        return y, self.conv2s[3]
