@@ -609,6 +609,20 @@ PVNET_API int pvnet_head1x1_backward_workspace_bytes(int b, int H, int W, int Ci
 PVNET_API int pvnet_head1x1_backward(const float *dout, const float *y, const float *w, float *dy, float *dw,
                                      float *db, int b, int H, int W, int Cin, int Cout, void *workspace,
                                      size_t workspace_bytes, pvnet_stream_t stream);
+/* The detectors' score head (Conv2d(C, 1, 3, 1, 1) with bias; DESIGN.md §22), x NHWC [b,H,W,C] dense (C a multiple of
+ * 32, at most 512), w [9][C] (tap ky*3+kx), bias [1]:
+ * pvnet_head3x3_nchw: out [b,1,H,W] = one fp32 fmaf chain per output from bias[0]: 32-channel chunks ascending, within
+ *   a chunk the taps ascending, within a tap the channels ascending; taps outside the image are skipped.
+ * pvnet_head3x3_backward: for dout [b,1,H,W] contiguous: dx NHWC [b,H,W,C] = sum_t w[t][c]*dout[y+1-ky, x+1-kx] (an
+ *   fmaf chain, t ascending from 0, taps outside the image skipped); dw [9][C] = sum_p dout[p]*x[p+(ky-1,kx-1)][c] and
+ *   db [1] = sum_p dout[p] in fp64 over a fixed partition of the pixels, merged in a fixed order and rounded once to
+ *   fp32.  Any of dx, dw, db may be NULL (not computed); the workspace is needed only for dw / db. */
+PVNET_API int pvnet_head3x3_nchw(const float *x, const float *w, const float *bias, float *out, int b, int H, int W,
+                                 int C, pvnet_stream_t stream);
+PVNET_API int pvnet_head3x3_backward_workspace_bytes(int b, int H, int W, int C, size_t *bytes);
+PVNET_API int pvnet_head3x3_backward(const float *dout, const float *x, const float *w, float *dx, float *dw,
+                                     float *db, int b, int H, int W, int C, void *workspace, size_t workspace_bytes,
+                                     pvnet_stream_t stream);
 
 /* The optimizer step of tools/train_linemod.py:260 (optim.Adam(net.parameters(), lr=...)): one Adam step over a table
  * of fp32 tensors, in place, one pass (each element reads p, g, m, v once and writes p, m, v once).
@@ -701,8 +715,16 @@ PVNET_API int pvnet_backbone_create_trunk(int block_kind, const int *blocks, int
  * mask [b,h/2,w/2]; everything else is as for the full-resolution decoder. */
 PVNET_API int pvnet_backbone_create_trunk_2o(int block_kind, const int *blocks, int ver_dim, int seg_dim, int fcdim,
                                              int s8dim, int s4dim, int s2dim, pvnet_backbone_t **out);
-/* The factor between the input and the output grid: 1, or 2 for a pvnet_backbone_create_trunk_2o handle; -1 for a
- * null handle. */
+/* Resnet18_8s_detector / Resnet18_8s_detector_v2 (model_repository.py:302-331): no decoder.  last_stage 4: the trunk,
+ * then its fc = Conv2d(512, 1, 3, 1, 1) with bias on layer4's output; last_stage 2: the stem, layer1 and layer2, then
+ * out_conv = Conv2d(128, 1, 3, 1, 1) on layer2's output.  The conv slots are the trunk's up to that stage (no fc.0),
+ * then the score head, packed fp32 [9][C] (tap ky*3+kx, then channel; not rounded) with bias [1]; C, the stage's
+ * output channels, must be at most 512.  The forward calls write out [b,1,h/8,w/8] through pvnet_head3x3_nchw's
+ * kernel; mask_out must be NULL and the output layout setting has no effect (one channel). */
+PVNET_API int pvnet_backbone_create_detector(int block_kind, const int *blocks, int last_stage,
+                                             pvnet_backbone_t **out);
+/* The factor between the input and the output grid: 1, 2 for a pvnet_backbone_create_trunk_2o handle, 8 for a
+ * pvnet_backbone_create_detector handle; -1 for a null handle. */
 PVNET_API int pvnet_backbone_output_scale(const pvnet_backbone_t *m);
 PVNET_API int pvnet_backbone_handle_num_convs(const pvnet_backbone_t *m);   /* -1 for a null handle */
 PVNET_API void pvnet_backbone_destroy(pvnet_backbone_t *m);

@@ -137,6 +137,10 @@ SIGNATURES = {
     "pvnet_head1x1_backward_workspace_bytes": (c_int, [c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
     "pvnet_head1x1_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
                                        c_int, c_int, c_int, c_void_p, c_size_t, c_void_p]),
+    "pvnet_head3x3_nchw": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "pvnet_head3x3_backward_workspace_bytes": (c_int, [c_int, c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
+    "pvnet_head3x3_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
+                                       c_int, c_int, c_void_p, c_size_t, c_void_p]),
     "pvnet_adam_step": (c_int, [ctypes.POINTER(AdamTensor), c_int, ctypes.c_double, ctypes.c_double, ctypes.c_double,
                                 ctypes.c_double, ctypes.c_double, ctypes.c_int64, c_void_p]),
     "pvnet_adam_chunk_tensors": (c_int, []),
@@ -146,6 +150,7 @@ SIGNATURES = {
                                             c_int, ctypes.POINTER(c_void_p)]),
     "pvnet_backbone_create_trunk_2o": (c_int, [c_int, ctypes.POINTER(c_int), c_int, c_int, c_int, c_int, c_int,
                                                c_int, ctypes.POINTER(c_void_p)]),
+    "pvnet_backbone_create_detector": (c_int, [c_int, ctypes.POINTER(c_int), c_int, ctypes.POINTER(c_void_p)]),
     "pvnet_backbone_output_scale": (c_int, [c_void_p]),
     "pvnet_backbone_destroy": (None, [c_void_p]),
     "pvnet_backbone_num_convs": (c_int, []),

@@ -741,3 +741,62 @@ def head_train(y, weight, bias):
     """Head1x1NCHW.apply: convraw.3 (1x1 with bias) on the native kernels under autograd, as a contiguous NCHW
     tensor."""
     return Head1x1NCHW.apply(y, weight, bias)
+
+
+def pack_head3x3(w: torch.Tensor) -> torch.Tensor:
+    """[1,C,3,3] -> [9][C] fp32 (tap ky*3+kx, then channel; not rounded): the score head's operand
+    (pvnet_head3x3_nchw, pvnet_backbone_create_detector's last slot)."""
+    return w.detach().reshape(w.shape[1], 9).t().contiguous()
+
+
+class Head3x3NCHW(torch.autograd.Function):
+    """The detectors' score head, a 3x3 convolution with padding 1, bias and one output channel (Resnet18_8s_detector's
+    fc, Resnet18_8s_detector_v2's out_conv), of a [b,C,H,W] float32 CUDA tensor (C a multiple of 32, at most 512; made
+    channels_last if it is not) -> a contiguous [b,1,H,W].  Forward: pvnet_head3x3_nchw, exact fp32 (one fmaf chain
+    per output from the bias in a fixed (chunk, tap, channel) order).  Backward: pvnet_head3x3_backward, the input
+    gradient as fmaf chains over the taps and the weight and bias gradients as fp64 sums in a fixed order, rounded once
+    (identical run to run); the parameter gradients are skipped when the parameters need none.  Saves the input and
+    the weight."""
+
+    @staticmethod
+    def forward(ctx, y, weight, bias):
+        _check_float_cuda("Head3x3NCHW", y, weight, bias)
+        C = weight.shape[1]
+        if y.dim() != 4 or y.shape[1] != C or tuple(weight.shape) != (1, C, 3, 3) or tuple(bias.shape) != (1,):
+            raise ValueError(f"Head3x3NCHW needs y [b,{C},H,W], weight [1,C,3,3] and bias [1], got "
+                             f"{tuple(y.shape)}, {tuple(weight.shape)}, {tuple(bias.shape)}")
+        b, _, H, W = y.shape
+        dev = y.device
+        yh = _nhwc(y)
+        w9 = pack_head3x3(weight)
+        out = torch.empty(b, 1, H, W, dtype=torch.float32, device=dev)
+        with torch.cuda.device(dev):
+            _native.check(_native.lib().pvnet_head3x3_nchw(_p(yh), _p(w9), _p(bias.detach().contiguous()), _p(out), b,
+                                                           H, W, C, _stream(dev)), "pvnet_head3x3_nchw")
+        ctx.save_for_backward(yh, weight)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gout):
+        yh, weight = ctx.saved_tensors
+        b, H, W, C = yh.shape
+        dev = yh.device
+        need_y, need_w, need_b = ctx.needs_input_grad
+        g = gout.float().contiguous()
+        w9 = pack_head3x3(weight)
+        dy = torch.empty(b, C, H, W, dtype=torch.float32, device=dev,
+                         memory_format=torch.channels_last) if need_y else None
+        dw = torch.empty(9, C, dtype=torch.float32, device=dev) if need_w else None
+        db = torch.empty(1, dtype=torch.float32, device=dev) if need_b else None
+        with torch.cuda.device(dev):
+            ws = _workspace(dev, "pvnet_head3x3_backward_workspace_bytes", b, H, W, C) if need_w or need_b else None
+            _native.check(_native.lib().pvnet_head3x3_backward(
+                _p(g), _p(yh), _p(w9), _p(dy), _p(dw), _p(db), b, H, W, C, _p(ws), 0 if ws is None else ws.numel(),
+                _stream(dev)), "pvnet_head3x3_backward")
+        return dy, None if dw is None else dw.t().reshape(1, C, 3, 3), db
+
+
+def head3x3_train(y, weight, bias):
+    """Head3x3NCHW.apply: a detector's 3x3 one-channel score head on the native kernels under autograd."""
+    return Head3x3NCHW.apply(y, weight, bias)

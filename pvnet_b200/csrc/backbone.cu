@@ -18,6 +18,9 @@
 // The half-resolution decoder (Resnet50_8s_2o, model_repository.py:158-224) ends at conv2s: C1, R0 and the x2
 // upsampling are gone, and conv2s.0 reads C2 plus X [b,H/2,W/2,8] (x_ds, 3 channels, zeros to 8; written by the
 // image pack) as its second source, into U2, which the 1x1 head reads at H/2 x W/2.
+// The detector kind (Resnet18_8s_detector / _v2, model_repository.py:302-331) has no decoder: the trunk up to layer4
+// (v1) or layer2 (v2), every stage writing plain buffers (no concatenation slices), then the 3x3 one-channel score
+// head (head3x3.cu) on the last stage's output at H/8 x W/8.
 #include "conv_tc.cuh"
 
 #include <string>
@@ -27,7 +30,7 @@ using namespace pvnet;
 
 namespace {
 
-enum StageKind { ST_PACK, ST_POOL, ST_CONV, ST_UP8, ST_UP4, ST_UP2, ST_HEAD };
+enum StageKind { ST_PACK, ST_POOL, ST_CONV, ST_UP8, ST_UP4, ST_UP2, ST_HEAD, ST_SCORE };
 
 struct Stage {
     StageKind kind;
@@ -57,12 +60,14 @@ struct Layer {
 struct pvnet_backbone {
     int ver_dim, seg_dim, fc, s8, s4, s2, raw;   // raw: the head's input width (s2 in the half-resolution decoder)
     int half = 0;                        // decoder kind: 1 = Resnet50_8s_2o's, output at H/2 x W/2
+    int last_stage = 0;                  // decoder kind: 4 / 2 = the detectors' score head on layer4 / layer2's output
     int nconv = 0;                       // conv slots, the head included (the last slot)
     std::vector<const float *> w, bias;
     std::vector<BufSpec> bufs;           // in carving order
     std::vector<Layer> layers;           // by slot, the head excluded
     std::vector<Stage> stages;
-    int bS2D, bC1 = -1, bR0 = -1, bX = -1, bC2, bU2, bP, bC4, bU4, bC8, bU8;   // buffers the non-conv stages use
+    int bS2D, bC1 = -1, bR0 = -1, bX = -1, bC2, bU2 = -1, bP, bC4 = -1, bU4 = -1, bC8 = -1, bU8 = -1;   // buffers the
+    int bFeat = -1, feat_c = 0;          // non-conv stages use; the score head's input and its channels (detectors)
     int c2s, c4s, c8s;                   // channel strides of the concatenation buffers
     // cached plan for one (b,h,w,workspace,in,out) combination
     int pb = 0, ph = 0, pw = 0;
@@ -94,9 +99,11 @@ namespace {
 // conv2 (3x3) + skip + ReLU.  Bottleneck (expansion 4): conv1 (1x1) -> conv2 (3x3, the stride) -> conv3 (1x1) + skip
 // + ReLU.  The downsample runs just before the conv whose epilogue adds it.  Within a stage the block outputs
 // alternate between two buffers so that the last block writes the stage's output: layer1 / layer2 straight into
-// their concatenation slices, layer3 / layer4 into E.
+// their concatenation slices, layer3 / layer4 into E.  The detector kind stops after stage `last_stage`, and every
+// stage writes its own E.
 void generate(pvnet_backbone *m, int bottleneck, const int blocks[4])
 {
+    const bool det = m->last_stage > 0;
     auto buf = [&](int level, int ch) {
         m->bufs.push_back({level, ch});
         return (int)m->bufs.size() - 1;
@@ -106,26 +113,27 @@ void generate(pvnet_backbone *m, int bottleneck, const int blocks[4])
         m->layers.push_back(l);
     };
     const int e = bottleneck ? 4 : 1;
-    m->c2s = m->s4 + 64;
+    m->c2s = det ? 64 : m->s4 + 64;
     m->c4s = m->s8 + 64 * e;
     m->c8s = m->fc + 128 * e;
     m->bS2D = buf(1, 16);
     if (m->half) {
         m->bX = buf(1, 8);
-    } else {
+    } else if (!det) {
         m->bC1 = buf(0, m->s2 + 8);
         m->bR0 = buf(0, m->raw);
     }
     m->bC2 = buf(1, m->c2s);
-    m->bU2 = buf(1, m->s2);
+    if (!det) m->bU2 = buf(1, m->s2);
     m->bP = buf(2, 64);
-    m->stages.push_back({ST_PACK, -1, "image: space-to-depth + NHWC slice packing"});
+    m->stages.push_back({ST_PACK, -1, det ? "image: space-to-depth packing"
+                                          : "image: space-to-depth + NHWC slice packing"});
     // stem (resnet.py:201-203) as a 4x4 stride-1 conv on the 2x2 space-to-depth image
     conv({m->bS2D, 16, 0, 16, m->bC2, m->c2s, m->s4, 64, -1, 0, 0, 1, 4, 1, 1, 1}, "stem conv1+bn1+relu");
     m->stages.push_back({ST_POOL, -1, "maxpool 3x3/2"});
     int x = m->bP, x_cs = 64, x_co = 0, x_c = 64, level = 2;
     int cur_stride = 4, dil = 1;
-    for (int s = 0; s < 4; ++s) {
+    for (int s = 0; s < (det ? m->last_stage : 4); ++s) {
         const int planes = 64 << s, outc = planes * e, n = blocks[s];
         int stride = s == 0 ? 1 : 2;
         const bool has_ds = stride != 1 || x_c != outc;
@@ -142,9 +150,13 @@ void generate(pvnet_backbone *m, int bottleneck, const int blocks[4])
         const int M = bottleneck ? buf(olevel, planes) : -1;
         const int D = has_ds ? buf(olevel, outc) : -1;
         const int B = buf(olevel, outc);
-        const int E = (s >= 2 || n > 2) ? buf(olevel, outc) : -1;
+        const int E = (det || s >= 2 || n > 2) ? buf(olevel, outc) : -1;
         int out, out_cs, out_co;
-        if (s == 0) {
+        if (det) {
+            out = E;
+            out_cs = outc;
+            out_co = 0;
+        } else if (s == 0) {
             m->bC4 = out = buf(2, m->c4s);
             m->bU4 = buf(2, m->s4);
             out_cs = m->c4s;
@@ -185,6 +197,16 @@ void generate(pvnet_backbone *m, int bottleneck, const int blocks[4])
             }
             x = y, x_cs = y_cs, x_co = y_co, x_c = outc, level = olevel;
         }
+    }
+    if (det) {
+        m->bFeat = x;
+        m->feat_c = x_c;
+        m->nconv = (int)m->layers.size() + 1;
+        m->stages.push_back({ST_SCORE, m->nconv - 1, m->last_stage == 4 ? "fc 3x3 -> 1 score head (fp32)"
+                                                                        : "out_conv 3x3 -> 1 score head (fp32)"});
+        m->w.assign(m->nconv, nullptr);
+        m->bias.assign(m->nconv, nullptr);
+        return;
     }
     // fc (model_repository.py: resnet.fc = 3x3 conv + BN + ReLU) -> xfc; decoder with LeakyReLU(0.1)
     conv({x, x_cs, x_co, x_c, m->bC8, m->c8s, 0, m->fc, -1, 0, 0, 3, 3, 1, 1, 1}, "fc.0");
@@ -321,10 +343,11 @@ int check_dims(int ver_dim, int seg_dim, int fcdim, int s8dim, int s4dim, int s2
 }
 
 pvnet_backbone *make(int bottleneck, const int blocks[4], int ver_dim, int seg_dim, int fcdim, int s8dim, int s4dim,
-                     int s2dim, int raw_dim, int half = 0)
+                     int s2dim, int raw_dim, int half = 0, int last_stage = 0)
 {
     pvnet_backbone *m = new pvnet_backbone();
     m->half = half;
+    m->last_stage = last_stage;
     m->ver_dim = ver_dim;
     m->seg_dim = seg_dim;
     m->fc = fcdim;
@@ -382,7 +405,22 @@ int pvnet_backbone_create_trunk_2o(int block_kind, const int *blocks, int ver_di
     return PVNET_OK;
 }
 
-int pvnet_backbone_output_scale(const pvnet_backbone_t *m) { return m ? (m->half ? 2 : 1) : -1; }
+int pvnet_backbone_create_detector(int block_kind, const int *blocks, int last_stage, pvnet_backbone_t **out)
+{
+    PV_CHECK_ARG(out, "null out pointer");
+    if (int rc = check_trunk(block_kind, blocks)) return rc;
+    PV_CHECK_ARG(last_stage == 2 || last_stage == 4, "last_stage must be 2 (v2: layer2) or 4 (layer4), got %d",
+                 last_stage);
+    const int width = (128 << (last_stage - 2)) * (block_kind == PVNET_BLOCK_BOTTLENECK ? 4 : 1);
+    PV_CHECK_ARG(width <= 512, "the score head reads at most 512 channels, stage %d has %d", last_stage, width);
+    *out = make(block_kind == PVNET_BLOCK_BOTTLENECK, blocks, 0, 1, 0, 0, 0, 0, 0, 0, last_stage);
+    return PVNET_OK;
+}
+
+int pvnet_backbone_output_scale(const pvnet_backbone_t *m)
+{
+    return m ? (m->last_stage ? 8 : m->half ? 2 : 1) : -1;
+}
 
 void pvnet_backbone_destroy(pvnet_backbone_t *m) { delete m; }
 
@@ -427,6 +465,7 @@ int prepare(pvnet_backbone *m, const ImageSrc &img, int b, int h, int w, float *
     PV_CHECK_ARG(m && img.ptr && out_nchw && workspace, "null pointer");
     PV_CHECK_ARG(b >= 1 && h >= 16 && w >= 16 && h % 8 == 0 && w % 8 == 0, "image size must be a multiple of 8");
     PV_CHECK_ARG(!mask_out || mask_elem_size == 1 || mask_elem_size == 8, "mask element size must be 1 or 8");
+    PV_CHECK_ARG(!mask_out || !m->last_stage, "a detector has no segmentation output: mask must be NULL");
     for (int i = 0; i < m->nconv; ++i)
         if (!m->w[i] || !m->bias[i]) {
             set_error("conv slot %d has no weights (pvnet_backbone_set_conv)", i);
@@ -453,9 +492,11 @@ int run_stage(pvnet_backbone *m, const Stage &st, const std::vector<float *> &B,
               int w, float *out_nchw, void *mask_out, int mask_elem_size, cudaStream_t s)
 {
     const int h2 = h / 2, w2 = w / 2, h4 = h / 4, w4 = w / 4, h8 = h / 8, w8 = w / 8;
-    float *C1 = m->half ? nullptr : B[m->bC1];
+    float *C1 = m->bC1 >= 0 ? B[m->bC1] : nullptr;
     switch (st.kind) {
     case ST_PACK:
+        if (m->last_stage)
+            return launch_s2d_pack(img.ptr, img.is_u8, img.mean, img.std, B[m->bS2D], nullptr, b, h, w, 8, 0, 0, s);
         if (m->half) return launch_s2d_pack(img.ptr, img.is_u8, img.mean, img.std, B[m->bS2D], B[m->bX], b, h, w, 8, 0, 1, s);
         return launch_s2d_pack(img.ptr, img.is_u8, img.mean, img.std, B[m->bS2D], C1 + (size_t)b * h * w * m->s2, b, h,
                                w, 8, 0, 0, s);
@@ -477,6 +518,8 @@ int run_stage(pvnet_backbone *m, const Stage &st, const std::vector<float *> &B,
                                m->seg_dim, m->seg_dim + m->ver_dim, b, h2, w2, m->out_nhwc, s);
         return launch_head(B[m->bR0], m->raw, m->w[st.slot], m->bias[st.slot], out_nchw, mask_out, mask_elem_size,
                            m->seg_dim, m->seg_dim + m->ver_dim, b, h, w, m->out_nhwc, s);
+    case ST_SCORE:
+        return launch_head3x3(B[m->bFeat], m->feat_c, m->w[st.slot], m->bias[st.slot], out_nchw, b, h8, w8, s);
     }
     return PVNET_E_INVALID;
 }

@@ -25,10 +25,11 @@ namespace pvnet {
 // HALF = true (Resnet50_8s_2o): instead of the full-resolution image slice, `out` [b,H/2,W/2,out_cs] gets at out_co
 // x_ds = F.interpolate(image, scale_factor=0.5, mode='bilinear') (3 channels + 5 zeros), the average of the 2x2 block
 // this thread already holds, in the rounding sequence of torch's CUDA kernel (DESIGN.md §21); TF32-rounded unless RAW.
+// IMG = false (the detectors, DESIGN.md §22): S only; nothing reads the image again, so `out` is not written.
 struct Norm3 {
     float mean[3], std[3];
 };
-template <bool U8, bool RAW = false, bool HALF = false>
+template <bool U8, bool RAW = false, bool HALF = false, bool IMG = true>
 __global__ void __launch_bounds__(128)
     k_s2d_pack(const void *__restrict__ in_v, Norm3 nrm, float *__restrict__ s2d, float *__restrict__ out, int H, int W,
                int out_cs, int out_co)
@@ -89,7 +90,7 @@ __global__ void __launch_bounds__(128)
 #pragma unroll
         for (int j = 0; j < 4; ++j)
             sS[t * 4 + (j ^ ((t >> 1) & 3))] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-        if constexpr (HALF) {
+        if constexpr (HALF && IMG) {
             // torch's upsample_bilinear2d_out_frame at source 2i + 0.5 (every weight 0.5):
             // h0 * (w0 * a + w1 * b) + h1 * (w0 * c + w1 * d), products exact
             float xd[3];
@@ -105,7 +106,7 @@ __global__ void __launch_bounds__(128)
             o[1] = make_float4(0.f, 0.f, 0.f, 0.f);
         }
 #pragma unroll
-        for (int py = 0; py < 2 && !HALF; ++py)
+        for (int py = 0; py < 2 && !HALF && IMG; ++py)
 #pragma unroll
             for (int px = 0; px < 2; ++px) {
                 const int b = (py * 2 + px) * 3;
@@ -125,7 +126,7 @@ __global__ void __launch_bounds__(128)
     }
     // image slice: lane pairs write the 32 bytes (3 channels + 5 zeros) of one full-resolution pixel
 #pragma unroll
-    for (int py = 0; py < 2 && !HALF; ++py) {
+    for (int py = 0; py < 2 && !HALF && IMG; ++py) {
         float *orow = out + (((size_t)n * H + 2 * y2 + py) * W + 2 * xb) * out_cs + out_co;
 #pragma unroll
         for (int r = 0; r < 4; ++r) {
@@ -147,6 +148,13 @@ int launch_s2d_pack(const void *in, int in_is_u8, const float *mean3, const floa
             nrm.mean[c] = mean3[c];
             nrm.std[c] = std3[c];
         }
+    }
+    if (!out) {
+        if (in_is_u8)
+            k_s2d_pack<true, false, false, false><<<grid, 128, 0, s>>>(in, nrm, s2d, out, H, W, out_cs, out_co);
+        else
+            k_s2d_pack<false, false, false, false><<<grid, 128, 0, s>>>(in, nrm, s2d, out, H, W, out_cs, out_co);
+    } else if (in_is_u8) {
         if (half)
             k_s2d_pack<true, false, true><<<grid, 128, 0, s>>>(in, nrm, s2d, out, H, W, out_cs, out_co);
         else

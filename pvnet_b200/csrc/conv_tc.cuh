@@ -58,7 +58,8 @@ size_t conv_plan_size();
 int conv_plan_at(const ConvDesc &d, void *plan_storage);
 int conv_launch_at(const void *plan_storage, cudaStream_t s);
 
-// half = 0: out is the full-resolution image slice [b,H,W,out_cs]; 1: x_ds [b,H/2,W/2,out_cs] (Resnet50_8s_2o)
+// half = 0: out is the full-resolution image slice [b,H,W,out_cs]; 1: x_ds [b,H/2,W/2,out_cs] (Resnet50_8s_2o);
+// out = nullptr: s2d only (the detectors)
 int launch_s2d_pack(const void *in, int in_is_u8, const float *mean3, const float *std3, float *s2d, float *out, int b,
                     int H, int W, int out_cs, int out_co, int half, cudaStream_t s);
 int launch_maxpool(const float *in, float *out, int b, int H, int W, int C, int in_cs, int in_co, cudaStream_t s);
@@ -67,6 +68,10 @@ int launch_upsample2x(const float *in, float *out, int b, int h, int w, int C, i
 // in NHWC [b,H,W,cin], cin 32 or 64 (raw_dim)
 int launch_head(const float *in, int cin, const float *w, const float *bias, float *out, void *mask, int mask_esz,
                 int seg_dim, int Cout, int b, int H, int W, int nhwc, cudaStream_t s);
+// the detectors' 3x3 one-channel score head (head3x3.cu): in NHWC [b,H,W,C] dense, C a multiple of 32 up to 512,
+// w [9][C], bias [1] -> out [b,1,H,W]
+int launch_head3x3(const float *in, int C, const float *w, const float *bias, float *out, int b, int H, int W,
+                   cudaStream_t s);
 
 #ifdef __CUDACC__
 // Three-slot interpolation sum with a FIXED rounding sequence (one weight of the window is zero): k_upsample2x
