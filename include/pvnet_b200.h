@@ -251,12 +251,22 @@ PVNET_API int pvnet_vote_counts(const float *direct, const float *coords, const 
  *   taking a step with max |delta| < 1e-9 (pn == 4 returns the P3P pose, :90-94).
  *   out_pose f64 [b,3,4] = (R | t) like the reference's return value; out_info int32 [b,2] or NULL =
  *   (status bits: 1 = P3P found no solution and the identity start was used, 2 = the 500-iteration cap was hit and
- *   the pose is not converged;
- *   LM iterations). */
+ *   the pose is not converged, 4 = see pvnet_uncertainty_pnp_per_image_k;
+ *   LM iterations).  A zero fx or fy in camera_matrix is refused (PVNET_E_INVALID).
+ * pvnet_uncertainty_pnp_per_image_k: the same solve with one camera per image, as the truncated-LINEMOD loader
+ *   supplies them (lib/datasets/linemod_dataset.py:206-207, tools/train_linemod.py:199-205): every argument as
+ *   above except camera_matrices, a DEVICE array of doubles [b,3,3] (row-major K per image, contiguous).  Image i
+ *   is solved with its own K exactly as pvnet_uncertainty_pnp solves it with that K: same kernel, same launch, bit
+ *   for bit the same pose and info.  Both entries read fx, cx, fy, cy (K[0], K[2], K[4], K[5]) and ignore the rest.
+ *   An image whose K has fx == 0 or fy == 0 is not solved: its pose is NaN and its status is 4; the other images
+ *   are unaffected.  The K are read on the device only: the call does not synchronise and is graph-capturable. */
 PVNET_API int pvnet_covariance_to_weights(const float *cov, int n, float *weights, pvnet_stream_t stream);
 PVNET_API int pvnet_uncertainty_pnp(const float *points_2d, const float *cov, const float *weights_2d,
                                     const float *points_3d, const double camera_matrix[9], int b, int pn,
                                     double *out_pose, int32_t *out_info, pvnet_stream_t stream);
+PVNET_API int pvnet_uncertainty_pnp_per_image_k(const float *points_2d, const float *cov, const float *weights_2d,
+                                                const float *points_3d, const double *camera_matrices, int b, int pn,
+                                                double *out_pose, int32_t *out_info, pvnet_stream_t stream);
 
 /* ------------------------------------------------------------------ pose evaluation
  * The metrics tools/train_linemod.py:177-229 (`val()`) reports, computed per image on the host there

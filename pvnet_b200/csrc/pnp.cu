@@ -290,16 +290,51 @@ __device__ __forceinline__ void warp_reduce28(double (&v)[PNP_NRED], double *sm 
     __syncwarp();
 }
 
+// Where each image's camera comes from: one K passed by value for the whole batch (pvnet_uncertainty_pnp), or a
+// device array [b,3,3] with one K per image (pvnet_uncertainty_pnp_per_image_k).  Either way the solver reads
+// fx = K[0,0], cx = K[0,2], fy = K[1,1], cy = K[1,2]; skew and the last row are not used.
+struct PnpCamera {
+    double fx, fy, cx, cy;
+    const double *per_image;        // row-major [b,3,3] on the device, or null: every image uses (fx, fy, cx, cy)
+};
+
+// status bit 4: the image's K has a zero focal length (the rule pvnet_uncertainty_pnp applies to its host K); the
+// image is not solved and its pose is NaN
+constexpr int PNP_STATUS_BAD_CAMERA = 4;
+
 // one warp per image
 __global__ void __launch_bounds__(128)
     k_uncertainty_pnp(const float *__restrict__ kp, const float *__restrict__ cov, const float *__restrict__ wgt,
-                      const float *__restrict__ pts3d, double fx, double fy, double cx, double cy, int nb, int K,
+                      const float *__restrict__ pts3d, PnpCamera cam, int nb, int K,
                       double *__restrict__ out_pose, int *__restrict__ out_info)
 {
     __shared__ double s_red[4][33 * PNP_NRED];
     const int img = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int lane = threadIdx.x & 31;
     if (img >= nb) return;
+    // this image's (fx, fy, cx, cy) in this warp's slot of shared memory, read where they are used: held in
+    // registers through the LM loop they would push the kernel (at the 255-register limit) into spilling
+    __shared__ double s_cam[4][4];
+    double *cm = s_cam[threadIdx.x >> 5];
+    if (lane == 0) {
+        const double *k = cam.per_image ? cam.per_image + (size_t)img * 9 : nullptr;
+        cm[0] = k ? k[0] : cam.fx;
+        cm[1] = k ? k[4] : cam.fy;
+        cm[2] = k ? k[2] : cam.cx;
+        cm[3] = k ? k[5] : cam.cy;
+    }
+    __syncwarp();
+    const double &fx = cm[0], &fy = cm[1], &cx = cm[2], &cy = cm[3];
+    if (!(fx != 0.0 && fy != 0.0)) {                // warp-uniform: the whole warp leaves
+        if (lane == 0) {
+            for (int i = 0; i < 12; ++i) out_pose[(size_t)img * 12 + i] = __longlong_as_double(0x7ff8000000000000ll);
+            if (out_info) {
+                out_info[img * 2] = PNP_STATUS_BAD_CAMERA;
+                out_info[img * 2 + 1] = 0;
+            }
+        }
+        return;
+    }
     double *sm = s_red[threadIdx.x >> 5];
     const bool active = lane < K;
     const int li = active ? lane : 0;
@@ -536,23 +571,41 @@ int pvnet_covariance_to_weights(const float *cov, int n, float *weights, pvnet_s
     return PVNET_OK;
 }
 
-int pvnet_uncertainty_pnp(const float *points_2d, const float *cov, const float *weights_2d, const float *points_3d,
-                          const double camera_matrix[9], int b, int pn, double *out_pose, int32_t *out_info,
-                          pvnet_stream_t stream)
+static int launch_uncertainty_pnp(const float *points_2d, const float *cov, const float *weights_2d,
+                                  const float *points_3d, PnpCamera cam, int b, int pn, double *out_pose,
+                                  int32_t *out_info, pvnet_stream_t stream)
 {
-    PV_CHECK_ARG(points_2d && points_3d && camera_matrix && out_pose, "null pointer");
+    PV_CHECK_ARG(points_2d && points_3d && out_pose, "null pointer");
     PV_CHECK_ARG((cov != nullptr) != (weights_2d != nullptr), "pass exactly one of cov / weights_2d");
     PV_CHECK_ARG(b >= 1, "non-positive batch");
     PV_CHECK_ARG(pn >= 4 && pn <= 32, "point count %d outside [4,32] (one warp per image)", pn);
-    const double fx = camera_matrix[0], fy = camera_matrix[4], cx = camera_matrix[2], cy = camera_matrix[5];
-    PV_CHECK_ARG(fx != 0.0 && fy != 0.0, "zero focal length");
     // one warp per CTA: the solve is a serial fp64 chain, so images should sit on different SMs, not share
     // one SM's fp64 pipe (4 warps per CTA doubled the time at batch 16)
     const int warps_per_cta = b <= 592 ? 1 : 4;
     k_uncertainty_pnp<<<(b + warps_per_cta - 1) / warps_per_cta, 32 * warps_per_cta, 0, (cudaStream_t)stream>>>(
-        points_2d, cov, weights_2d, points_3d, fx, fy, cx, cy, b, pn, out_pose, out_info);
+        points_2d, cov, weights_2d, points_3d, cam, b, pn, out_pose, out_info);
     PV_LAUNCHED("k_uncertainty_pnp");
     return PVNET_OK;
+}
+
+int pvnet_uncertainty_pnp(const float *points_2d, const float *cov, const float *weights_2d, const float *points_3d,
+                          const double camera_matrix[9], int b, int pn, double *out_pose, int32_t *out_info,
+                          pvnet_stream_t stream)
+{
+    PV_CHECK_ARG(camera_matrix, "null pointer");
+    const double fx = camera_matrix[0], fy = camera_matrix[4], cx = camera_matrix[2], cy = camera_matrix[5];
+    PV_CHECK_ARG(fx != 0.0 && fy != 0.0, "zero focal length");
+    return launch_uncertainty_pnp(points_2d, cov, weights_2d, points_3d, PnpCamera{fx, fy, cx, cy, nullptr}, b, pn,
+                                  out_pose, out_info, stream);
+}
+
+int pvnet_uncertainty_pnp_per_image_k(const float *points_2d, const float *cov, const float *weights_2d,
+                                      const float *points_3d, const double *camera_matrices, int b, int pn,
+                                      double *out_pose, int32_t *out_info, pvnet_stream_t stream)
+{
+    PV_CHECK_ARG(camera_matrices, "null pointer");
+    return launch_uncertainty_pnp(points_2d, cov, weights_2d, points_3d, PnpCamera{0.0, 0.0, 0.0, 0.0, camera_matrices},
+                                  b, pn, out_pose, out_info, stream);
 }
 
 }  // extern "C"

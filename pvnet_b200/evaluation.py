@@ -8,7 +8,8 @@
                                                       -> float64 [b,4] = (add, proj, trans_cm, angle_deg) on the device
     pnp(points_3d, points_2d, camera_matrix, method=0)
     uncertainty_pnp_v2(points_2d, covars, points_3d, camera_matrix, type='single')
-    Evaluator                                          the reference's recorder class, plus evaluate_batch()
+    Evaluator                                          the reference's recorder class, plus evaluate_batch() and
+                                                       evaluate_keypoints_batch() (per-image cameras)
 
 Numpy inputs keep the reference's return types (one host synchronisation per call, as the reference's host loop
 has); batched CUDA tensors return CUDA tensors without synchronising.  No CPU path: without the library or a CUDA
@@ -222,6 +223,7 @@ class Evaluator(object):
         self.uncertainty_pnp_cost = []
         # evaluate_batch totals (float64, device): images, proj passes, add passes, 5cm5deg passes, proj sum, add sum
         self.batch_totals = None
+        self._points_dev = {}           # evaluate_keypoints_batch: (class, vote type, device) -> (keypoints, model)
 
     # ---- one image (numpy in, as the reference)
     @staticmethod
@@ -301,6 +303,36 @@ class Evaluator(object):
         self._all_metrics(pose_pred, pose_targets, class_type, K, sym_proj=class_type in SYMMETRIC_CLASSES)
 
     # ---- a batch on the device
+    def _device_points(self, class_type, vote_type, dev):
+        """The object's keypoints and mesh vertices as float32 device tensors, copied once per (class, vote type,
+        device): a copy from pageable host memory would synchronise every batch."""
+        key = (class_type, vote_type, dev)
+        if key not in self._points_dev:
+            vt = _VotingType.get()
+            pts = vt.get_pts_3d(vt.BB8 if vote_type is _BB8 else vote_type, class_type)
+            model = self.linemod_db.get_ply_model(class_type)
+            self._points_dev[key] = (_on(pts, dev, torch.float32), _on(model, dev, torch.float32))
+        return self._points_dev[key]
+
+    def evaluate_keypoints_batch(self, points_2d, pose_targets, class_type, K, covar=None, vote_type=_BB8):
+        """`evaluate` (covar None) or `evaluate_uncertainty` (covar [b,pn,2,2]) for a batch of images of one object
+        on the device, with one camera per image: the truncated-LINEMOD branch of val() (tools/train_linemod.py:
+        199-205) in one call per batch instead of one per image.  points_2d [b,pn,2] and pose_targets [b,3,4] CUDA
+        tensors; K a CUDA [b,3,3] (or anything `uncertainty_pnp_batched` takes).  Poses, then `evaluate_batch` with
+        the class's model, diameter and symmetry: the per-image methods' pose and metric values, bit for bit (the
+        covariances become float32 weights first, as in evaluate_uncertainty).  Does not synchronise once the
+        class's points are on the device.  Returns (pose_pred float64 [b,3,4], metrics float64 [b,4])."""
+        dev = points_2d.device
+        points_3d, model = self._device_points(class_type, vote_type, dev)
+        if covar is None:
+            pose_pred = pnp(points_3d, points_2d, K)
+        else:
+            weights = covariance_to_weights(covar.to(dev))
+            pose_pred = uncertainty_pnp_batched(points_2d, points_3d, K, weights_2d=weights)
+        m = self.evaluate_batch(pose_pred, pose_targets, model, self.linemod_db.get_diameter(class_type), K,
+                                symmetric=class_type in SYMMETRIC_CLASSES)
+        return pose_pred, m
+
     def evaluate_batch(self, pose_pred, pose_targets, model, diameter, K, symmetric=False, sym_proj=False):
         """Metrics of a batch of device poses [b,3,4] of one object; the pass counts and distance sums are added to
         `batch_totals` on the device (no synchronisation, CUDA-graph capturable).  Returns the [b,4] metrics."""

@@ -14,7 +14,8 @@ Device-side uncertainty-driven PnP: the reference's `uncertainty_pnp`
 keeps the reference's signature and return type (numpy float64) for numpy inputs -- the arrays are
 moved to the current CUDA device; batched CUDA tensors ([b,pn,2], [b,pn,3]) return a float64 CUDA
 tensor [b,3,4] with no host synchronisation, which is what `PoseKeypointPipeline(with_pose=True)` uses so
-that poses, not keypoints, are what leaves the GPU.  No CPU path: without the library or a CUDA
+that poses, not keypoints, are what leaves the GPU.  The batched form also takes one camera matrix per image as a
+CUDA tensor [b,3,3] (`pvnet_uncertainty_pnp_per_image_k`).  No CPU path: without the library or a CUDA
 device these functions raise.
 """
 from __future__ import annotations
@@ -51,9 +52,23 @@ def covariance_to_weights(cov: torch.Tensor) -> torch.Tensor:
     return out
 
 
+def check_cameras(shape, b: int):
+    """Raise ValueError unless `shape` is [3,3] (one camera for the batch) or [b,3,3] (one per image)."""
+    shape = tuple(shape)
+    if shape == (3, 3) or shape == (b, 3, 3):
+        return
+    if len(shape) == 3 and shape[1:] == (3, 3):
+        raise ValueError(f"camera_matrix holds {shape[0]} cameras for a batch of {b} images")
+    raise ValueError(f"camera_matrix must be [3,3] or [{b},3,3], got {shape}")
+
+
 def uncertainty_pnp_batched(points_2d, points_3d, camera_matrix, weights_2d=None, cov=None, return_info=False):
     """points_2d [b,pn,2] CUDA; weights_2d [b,pn,3] or cov [b,pn,2,2] (exactly one); points_3d [pn,3];
-    camera_matrix 3x3 (host).  -> poses float64 [b,3,4] on the device (and info int32 [b,2])."""
+    camera_matrix a host 3x3 (numpy, list, CPU tensor) for every image, or a CUDA tensor [b,3,3] (one camera per
+    image, the truncated-LINEMOD form) or [3,3].  A CUDA camera stays on the device (no host synchronisation) and
+    goes to `pvnet_uncertainty_pnp_per_image_k` as float64 [b,3,3]; a [3,3] one is expanded to every image, which
+    gives bit for bit the poses of the host 3x3.  -> poses float64 [b,3,4] on the device (and info int32 [b,2];
+    status bit 4 marks an image whose K has a zero focal length, its pose is NaN)."""
     if not points_2d.is_cuda:
         raise RuntimeError("pvnet_b200: `points_2d` must be a CUDA tensor (there is no CPU path)")
     if (weights_2d is None) == (cov is None):
@@ -68,11 +83,17 @@ def uncertainty_pnp_batched(points_2d, points_3d, camera_matrix, weights_2d=None
     c = None if cov is None else cov.to(dev).contiguous().float()
     out = torch.empty([b, 3, 4], dtype=torch.float64, device=dev)
     info = torch.empty([b, 2], dtype=torch.int32, device=dev) if return_info else None
+    args = (p2.data_ptr(), None if c is None else c.data_ptr(), None if w is None else w.data_ptr(), p3.data_ptr())
+    tail = (b, pn, out.data_ptr(), None if info is None else info.data_ptr(), _stream(dev))
     with torch.cuda.device(dev):
-        _native.check(_native.lib().pvnet_uncertainty_pnp(
-            p2.data_ptr(), None if c is None else c.data_ptr(), None if w is None else w.data_ptr(), p3.data_ptr(),
-            _camera(camera_matrix), b, pn, out.data_ptr(), None if info is None else info.data_ptr(), _stream(dev)),
-            "pvnet_uncertainty_pnp")
+        if isinstance(camera_matrix, torch.Tensor) and camera_matrix.is_cuda:
+            check_cameras(camera_matrix.shape, b)
+            ks = camera_matrix.to(device=dev, dtype=torch.float64).expand(b, 3, 3).contiguous()
+            _native.check(_native.lib().pvnet_uncertainty_pnp_per_image_k(*args, ks.data_ptr(), *tail),
+                          "pvnet_uncertainty_pnp_per_image_k")
+        else:
+            _native.check(_native.lib().pvnet_uncertainty_pnp(*args, _camera(camera_matrix), *tail),
+                          "pvnet_uncertainty_pnp")
     return (out, info) if return_info else out
 
 

@@ -12,7 +12,12 @@ Per batch the device work is: `pvnet_backbone_forward` (fused argmax -> uint8 ma
 
 With `points_3d` + `camera_matrix` the uncertainty-driven PnP of `Evaluator.evaluate_uncertainty`
 (lib/utils/evaluation_utils.py:165-201) runs on the device as well (`pvnet_uncertainty_pnp`), so POSES
-[b,3,4] are what leaves the GPU (and what an 8-GPU job gathers).
+[b,3,4] are what leaves the GPU (and what an 8-GPU job gathers).  Where every image has its own camera (the
+truncated-LINEMOD loader's `Ks`, tools/train_linemod.py:186-205), build the pipeline with `points_3d` alone and
+pass the cameras with the images: `step(x, camera_matrix=Ks)` with a CUDA [b,3,3], `run(host_batches,
+camera_matrices=...)` with one host [b,3,3] per batch, copied on the same side stream as its image batch (into a
+static device buffer per input buffer, so one captured graph serves every batch).  The solve is then
+`pvnet_uncertainty_pnp_per_image_k`.
 
 `graph=True`: the per-batch device work (31 backbone launches + the voting call's ~10 + PnP) is captured into one
 CUDA graph per input buffer on first use and replayed afterwards -- 4 us of host time per batch instead of
@@ -56,12 +61,16 @@ class PoseKeypointPipeline:
         self.points_3d, self.camera_matrix = points_3d, camera_matrix
         self._p3_dev = None
         self._bufs = None
+        self._kbufs = None
         self._copy_stream = None
 
-    def _setup(self, host_batch, dev):
+    def _setup(self, host_batch, dev, per_batch_k):
         if (self._bufs is None or self._bufs[0].shape != host_batch.shape or self._bufs[0].dtype != host_batch.dtype
-                or self._bufs[0].device != dev):
+                or self._bufs[0].device != dev or (self._kbufs is not None) != per_batch_k):
             self._bufs = [torch.empty(host_batch.shape, dtype=host_batch.dtype, device=dev) for _ in range(2)]
+            # per input buffer: the batch's cameras, float64 [b,3,3] (static, so a captured graph reads each batch's)
+            self._kbufs = ([torch.empty([host_batch.shape[0], 3, 3], dtype=torch.float64, device=dev) for _ in range(2)]
+                           if per_batch_k else None)
             self._ready = [torch.cuda.Event() for _ in range(2)]      # H2D of buffer i finished
             self._free = [torch.cuda.Event() for _ in range(2)]       # compute no longer reads buffer i
             self._done = torch.cuda.Event()                           # last D2H of a run() finished
@@ -71,26 +80,30 @@ class PoseKeypointPipeline:
                 e.record(torch.cuda.current_stream(dev))
 
     def _step_graph(self, j):
-        """Replay (capture on first use) the graph of `step(self._bufs[j])` on the current stream."""
+        """Replay (capture on first use) the graph of `step(self._bufs[j], self._kbufs[j])` on the current stream."""
         if self._graphs[j] is None:
             cur = torch.cuda.current_stream(self._bufs[j].device)
             side = torch.cuda.Stream(device=self._bufs[j].device)
             side.wait_stream(cur)
+            k = None if self._kbufs is None else self._kbufs[j]
             with torch.cuda.stream(side):
-                self.step(self._bufs[j])            # eager once on the capture stream: plans, workspaces, attributes
+                self.step(self._bufs[j], k)         # eager once on the capture stream: plans, workspaces, attributes
                 side.synchronize()
                 g = torch.cuda.CUDAGraph()
                 with torch.cuda.graph(g, stream=side):
-                    res = self.step(self._bufs[j])
+                    res = self.step(self._bufs[j], k)
             cur.wait_stream(side)
             self._graphs[j] = (g, res)
         g, res = self._graphs[j]
         g.replay()
         return res
 
-    def step(self, x):
+    def step(self, x, camera_matrix=None):
         """x on the device: float32 [b,3,H,W] or uint8 [b,H,W,3] -> keypoints [b,K,2]
-        (and covariances [b,K,2,2]) (and poses [b,3,4] float64)."""
+        (and covariances [b,K,2,2]) (and poses [b,3,4] float64).  camera_matrix: this batch's cameras, a CUDA
+        tensor [b,3,3] (or [3,3]), in place of the constructor's; it needs `points_3d` and `with_covariance`."""
+        if camera_matrix is not None and (self.points_3d is None or not self.with_cov):
+            raise ValueError("per-batch camera matrices need points_3d and with_covariance=True")
         # pixel-major head output: the vertex field is the contiguous [b,h,w,K,2] form of the permuted view of
         # tools/demo.py:48-50 (same values; the voting layer's gather then reads whole records, not sectors)
         if x.dtype == torch.uint8:
@@ -112,24 +125,36 @@ class PoseKeypointPipeline:
                                                                min_hyp_num=self.cov_min, inlier_thresh=self.thresh,
                                                                max_num=self.max_num, rng="batched")
             res = (kp, cov)
-        if self.with_pose:
+        if self.with_pose or camera_matrix is not None:
             if self._p3_dev is None or self._p3_dev.device != x.device:     # the model points go to the device once
                 self._p3_dev = torch.as_tensor(self.points_3d, dtype=torch.float32).to(x.device).contiguous()
-            pose = eu.uncertainty_pnp_batched(res[0], self._p3_dev, self.camera_matrix, cov=res[1])
+            K = self.camera_matrix if camera_matrix is None else camera_matrix
+            pose = eu.uncertainty_pnp_batched(res[0], self._p3_dev, K, cov=res[1])
             return res[0], res[1], pose
         return res
 
     @torch.no_grad()
-    def run(self, host_batches, out_host=None, cov_host=None, on_result=None, pose_host=None):
+    def run(self, host_batches, out_host=None, cov_host=None, on_result=None, pose_host=None, camera_matrices=None):
         """host_batches: sequence of pinned [b,3,H,W] float32 (or [b,H,W,3] uint8) tensors.  Results are
         copied device->host into out_host[i] (and cov_host[i]) -- pinned tensors -- when given; the call
         returns after the last of those copies has completed.  Returns the last device result (with graph=True a
-        static tensor that the next replay on the same input buffer overwrites)."""
+        static tensor that the next replay on the same input buffer overwrites).
+        camera_matrices: one host [b,3,3] (or [3,3]) per batch, numpy or CPU tensor (pinned float64 makes the copy as
+        asynchronous as the images'): the cameras of that batch's images, used in place of the constructor's."""
         dev = next(self.net.parameters()).device
         batches = list(host_batches)
         if not batches:
             return None
-        self._setup(batches[0], dev)
+        cams = None
+        if camera_matrices is not None:
+            cams = [torch.as_tensor(k, dtype=torch.float64) for k in camera_matrices]
+            if len(cams) != len(batches):
+                raise ValueError(f"{len(cams)} camera batches for {len(batches)} image batches")
+            for k in cams:
+                eu.check_cameras(k.shape, batches[0].shape[0])
+            if self.points_3d is None or not self.with_cov:
+                raise ValueError("per-batch camera matrices need points_3d and with_covariance=True")
+        self._setup(batches[0], dev, cams is not None)
         main = torch.cuda.current_stream(dev)
         cs = self._copy_stream
         result = None
@@ -139,6 +164,8 @@ class PoseKeypointPipeline:
             cs.wait_event(self._free[j])
             with torch.cuda.stream(cs):
                 self._bufs[j].copy_(batches[i], non_blocking=True)
+                if cams is not None:
+                    self._kbufs[j].copy_(cams[i], non_blocking=True)
                 self._ready[j].record(cs)
         upload(0)
         for i in range(len(batches)):
@@ -146,7 +173,8 @@ class PoseKeypointPipeline:
             if i + 1 < len(batches):
                 upload(i + 1)
             main.wait_event(self._ready[j])
-            result = self._step_graph(j) if self.graph else self.step(self._bufs[j])
+            k = None if cams is None else self._kbufs[j]
+            result = self._step_graph(j) if self.graph else self.step(self._bufs[j], k)
             self._free[j].record(main)
             if out_host is not None:
                 kp = result[0] if isinstance(result, tuple) else result
