@@ -268,6 +268,32 @@ PVNET_API int pvnet_uncertainty_pnp_per_image_k(const float *points_2d, const fl
                                                 const float *points_3d, const double *camera_matrices, int b, int pn,
                                                 double *out_pose, int32_t *out_info, pvnet_stream_t stream);
 
+/* ------------------------------------------------------------------ EPnP
+ * The reference's `pnp(points_3d, points_2d, camera_matrix, method=cv2.SOLVEPNP_EPNP)` (lib/utils/evaluation_utils.py:
+ * 19-52, :26-28) for a batch: Lepetit, Moreno-Noguer and Fua's closed-form EPnP (IJCV 2009), one warp per image, fp64
+ * (csrc/epnp.cu; oracle/epnp_oracle.py restates it in numpy).  Fixed work per image: no iteration count depends on
+ * the data except the Jacobi eigen-solvers', which stop after at most 30 (3x3) and 20 (12x12) sweeps.
+ * pvnet_epnp:
+ *   points_2d      f32 [b,pn,2]  image points (pixels) of every image, device
+ *   points_3d      f32 [pn,3]    object points, one object for the whole batch, device
+ *   camera_matrix  HOST array of 9 doubles (row-major K); fx, cx, fy, cy (K[0], K[2], K[4], K[5]) are read; a zero
+ *                  fx or fy is refused (PVNET_E_INVALID)
+ *   b              >= 1 images
+ *   pn             4 <= pn <= 4096 correspondences (cv2.solvePnP needs 4; every sum strides over the points)
+ *   out_pose       f64 [b,3,4] = (R | t), the reference's return value, device
+ *   out_info       int32 [b,2] or NULL = (status bits, the linearisation N in 1..3 whose pose was kept); status 1:
+ *                  the object points' PCA is rank-deficient (coplanar or collinear: smallest eigenvalue <= 1e-10 of
+ *                  the largest), the pose is still computed but is unreliable, as OpenCV's is there; 4: fx or fy is 0
+ *                  (per-image entry only), the pose is NaN
+ *   stream         CUDA stream; no workspace, no allocation, no host synchronisation: graph-capturable
+ * pvnet_epnp_per_image_k: the same with camera_matrices, a DEVICE array of doubles [b,3,3] (one K per image).  Same
+ *   kernel and launch: image i gets bit for bit the pose pvnet_epnp gives it with that K.  An image whose K has
+ *   fx == 0 or fy == 0 gets status 4 and a NaN pose; the other images are unaffected. */
+PVNET_API int pvnet_epnp(const float *points_2d, const float *points_3d, const double camera_matrix[9], int b, int pn,
+                         double *out_pose, int32_t *out_info, pvnet_stream_t stream);
+PVNET_API int pvnet_epnp_per_image_k(const float *points_2d, const float *points_3d, const double *camera_matrices,
+                                     int b, int pn, double *out_pose, int32_t *out_info, pvnet_stream_t stream);
+
 /* ------------------------------------------------------------------ pose evaluation
  * The metrics tools/train_linemod.py:177-229 (`val()`) reports, computed per image on the host there
  * (lib/utils/evaluation_utils.py:75-141).

@@ -71,6 +71,9 @@ SIGNATURES = {
                                       c_void_p, c_void_p, c_void_p]),
     "pvnet_uncertainty_pnp_per_image_k": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
                                                   c_void_p, c_void_p, c_void_p]),
+    "pvnet_epnp": (c_int, [c_void_p, c_void_p, ctypes.POINTER(ctypes.c_double), c_int, c_int, c_void_p, c_void_p,
+                           c_void_p]),
+    "pvnet_epnp_per_image_k": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "pvnet_find_nearest_point_idx": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "pvnet_pose_metrics_workspace_bytes": (c_int, [c_int, c_int, ctypes.POINTER(c_size_t)]),
     "pvnet_pose_metrics": (c_int, [c_void_p, c_void_p, c_void_p, c_int, ctypes.POINTER(ctypes.c_double), c_void_p,

@@ -1,12 +1,13 @@
 """Pose evaluation on the device: the reference's lib/utils/evaluation_utils.py (`pnp`, `find_nearest_point_distance`,
 `Evaluator`) and the nearest-point search of lib/utils/extend_utils/extend_utils.py:39-60, over the C ABI
-(`pvnet_find_nearest_point_idx`, `pvnet_pose_metrics`, `pvnet_uncertainty_pnp` in include/pvnet_b200.h).
+(`pvnet_find_nearest_point_idx`, `pvnet_pose_metrics`, `pvnet_uncertainty_pnp`, `pvnet_epnp` in include/pvnet_b200.h).
 
     find_nearest_point_idx(ref_pts, que_pts)          numpy [pn,dim] -> numpy int32 [pn2];  CUDA [b,pn,dim] -> [b,pn2]
     find_nearest_point_distance(pts1, pts2)           numpy -> numpy float64;  CUDA tensors stay on the device
     pose_metrics(pose_pred, pose_gt, model, K, symmetric=False, sym_proj=False)
                                                       -> float64 [b,4] = (add, proj, trans_cm, angle_deg) on the device
-    pnp(points_3d, points_2d, camera_matrix, method=0)
+    pnp(points_3d, points_2d, camera_matrix, method=0)    method 0 (SOLVEPNP_ITERATIVE); batched CUDA input
+                                                       also 1 (SOLVEPNP_EPNP)
     uncertainty_pnp_v2(points_2d, covars, points_3d, camera_matrix, type='single')
     Evaluator                                          the reference's recorder class, plus evaluate_batch() and
                                                        evaluate_keypoints_batch() (per-image cameras)
@@ -25,9 +26,10 @@ import numpy as np
 import torch
 
 from . import _native
-from .extend_utils import covariance_to_weights, uncertainty_pnp, uncertainty_pnp_batched
+from .extend_utils import _camera, check_cameras, covariance_to_weights, uncertainty_pnp, uncertainty_pnp_batched
 
 SOLVEPNP_ITERATIVE = 0                  # cv2.SOLVEPNP_ITERATIVE
+SOLVEPNP_EPNP = 1                       # cv2.SOLVEPNP_EPNP
 SYMMETRIC_CLASSES = ("eggbox", "glue")  # evaluation_utils.py:159,193,210
 
 
@@ -129,15 +131,59 @@ def pose_metrics(pose_pred, pose_gt, model, K, symmetric=False, sym_proj=False):
 
 
 # --------------------------------------------------------------------------------------------------------- PnP
+def _epnp_batched(points_2d, points_3d, camera_matrix, return_info=False):
+    """EPnP (`pvnet_epnp`, csrc/epnp.cu) for a batch: points_2d CUDA [b,pn,2]; points_3d [pn,3]; camera_matrix a host
+    3x3 (numpy, list, CPU tensor) or a CUDA [3,3] / [b,3,3], as `uncertainty_pnp_batched` takes it.  Inputs are read as
+    float32.  -> poses float64 [b,3,4] on the device (and info int32 [b,2] = (status, chosen linearisation N)); no
+    host synchronisation."""
+    dev = points_2d.device
+    p2 = points_2d.contiguous().float()
+    if p2.dim() != 3 or p2.shape[2] != 2:
+        raise ValueError(f"points_2d must be [b,pn,2], got {tuple(p2.shape)}")
+    b, pn, _ = p2.shape
+    if pn < 4:
+        raise ValueError(f"EPnP needs at least 4 points, got {pn}")
+    p3 = torch.as_tensor(points_3d, dtype=torch.float32, device=dev).contiguous()
+    if tuple(p3.shape) != (pn, 3):
+        raise ValueError(f"points_3d must be [{pn},3], got {tuple(p3.shape)}")
+    out = torch.empty([b, 3, 4], dtype=torch.float64, device=dev)
+    info = torch.empty([b, 2], dtype=torch.int32, device=dev) if return_info else None
+    tail = (b, pn, out.data_ptr(), None if info is None else info.data_ptr(), _stream(dev))
+    with torch.cuda.device(dev):
+        if isinstance(camera_matrix, torch.Tensor) and camera_matrix.is_cuda:
+            check_cameras(camera_matrix.shape, b)
+            ks = camera_matrix.to(device=dev, dtype=torch.float64).expand(b, 3, 3).contiguous()
+            _native.check(_native.lib().pvnet_epnp_per_image_k(p2.data_ptr(), p3.data_ptr(), ks.data_ptr(), *tail),
+                          "pvnet_epnp_per_image_k")
+        else:
+            _native.check(_native.lib().pvnet_epnp(p2.data_ptr(), p3.data_ptr(), _camera(camera_matrix), *tail),
+                          "pvnet_epnp")
+    return (out, info) if return_info else out
+
+
 def pnp(points_3d, points_2d, camera_matrix, method=SOLVEPNP_ITERATIVE):
-    """evaluation_utils.py:19-52 with cv2.SOLVEPNP_ITERATIVE, on the device solver of `uncertainty_pnp` with unit
-    weights (1, 0, 1): it then minimises the plain reprojection error, the objective of SOLVEPNP_ITERATIVE.  The
-    start differs from OpenCV's (a DLT): with equal weights the solver's stable "four largest wxx + wxy" rule takes
-    the LAST four points for its P3P start.  4 <= pn <= 32; with exactly 4 points the P3P pose is returned.
-    numpy in -> numpy [3,4] float64; CUDA points_2d [b,pn,2] -> float64 CUDA [b,3,4] without synchronising."""
+    """evaluation_utils.py:19-52.  numpy in -> numpy [3,4] float64 (method 0); CUDA points_2d [b,pn,2] -> float64 CUDA
+    [b,3,4] without synchronising (method 0 or 1).
+
+    method=0 (cv2.SOLVEPNP_ITERATIVE) runs the device solver of `uncertainty_pnp` with unit weights (1, 0, 1): it then
+    minimises the plain reprojection error, the objective of SOLVEPNP_ITERATIVE.  The start differs from OpenCV's (a
+    DLT): with equal weights the solver's stable "four largest wxx + wxy" rule takes the LAST four points for its P3P
+    start.  4 <= pn <= 32; with exactly 4 points the P3P pose is returned.
+
+    method=1 (cv2.SOLVEPNP_EPNP) runs the closed-form EPnP of `pvnet_epnp` (4 <= pn <= 4096, points read as
+    float32) on batched CUDA points_2d [b,pn,2]; the camera may be a host 3x3 or a CUDA [3,3] / [b,3,3] (one per
+    image).  The single-image numpy form keeps method 0 only, as before: it raises ValueError for method 1 too.  A
+    numpy caller gets the EPnP pose with `pnp(P, torch.from_numpy(x)[None].cuda(), K, method=1)[0].cpu().numpy()`.
+
+    Any other method raises ValueError."""
+    batched = isinstance(points_2d, torch.Tensor) and points_2d.is_cuda and points_2d.dim() == 3
+    if method == SOLVEPNP_EPNP and batched:
+        return _epnp_batched(points_2d, points_3d, camera_matrix)
     if method != SOLVEPNP_ITERATIVE:
-        raise ValueError(f"pnp: only method=0 (cv2.SOLVEPNP_ITERATIVE) is provided, got {method!r}")
-    if isinstance(points_2d, torch.Tensor) and points_2d.is_cuda and points_2d.dim() == 3:
+        raise ValueError(f"pnp: method={method!r} is not provided for this input; numpy inputs take method=0 "
+                         f"(cv2.SOLVEPNP_ITERATIVE), batched CUDA points_2d [b,pn,2] take method=0 or 1 "
+                         f"(cv2.SOLVEPNP_EPNP)")
+    if batched:
         b, pn, _ = points_2d.shape
         w = torch.zeros([b, pn, 3], dtype=torch.float32, device=points_2d.device)
         w[..., 0] = 1.0
