@@ -28,6 +28,7 @@
  *   lib/utils/evaluation_utils.py:75-141                          the pose metrics (ADD(-S), 2D projection, 5 cm 5 deg)
  *   lib/utils/extend_utils/src/farthest_point_sampling.cpp        farthest_point_sampling[_init_center]
  *   lib/utils/extend_utils/src/mesh_rasterization.cpp             mesh_binary_rasterization
+ *   lib/utils/opengl_render_backend.py:306-419                    render (depth and flat RGB)
  *   lib/utils/net_utils.py:54-80,329-348                          smooth_l1_loss, compute_precision_recall
  *   tools/train_linemod.py:83-91                                  NetWrapper's cross-entropy (nn.CrossEntropyLoss)
  *   lib/networks/model_repository.py:64-80                        Resnet18_8s.forward
@@ -452,6 +453,24 @@ PVNET_API int pvnet_farthest_point_sampling(const float *pts, const int32_t *sta
                                             pvnet_stream_t stream);
 PVNET_API int pvnet_mesh_binary_rasterization(const float *triangles, int b, int tn, int h, int w, uint8_t *mask,
                                               pvnet_stream_t stream);
+
+/* pvnet_render_mesh: depth and flat-shaded RGB of one mesh at b poses, the reference's OpenGL render backend
+ *   (lib/utils/opengl_render_backend.py:306-419, flat shading, no texture; DESIGN.md §24).
+ *   verts f32 [nv,3]; faces int32 [nf,3] (a face with an index outside [0, nv), a repeated index, a non-finite
+ *   vertex or a zero determinant covers nothing); colors f32 [nv,3] or NULL (0.5 grey); poses f32 [b,3,4] (R | t,
+ *   object to OpenCV camera); K f32 [3,3], or [b,3,3] when k_per_image != 0 (fx, s, cx, fy, cy are read).
+ *   Pixel (r, c) samples the image point (c + 0.5, r + 0.5).  A pixel is covered by the faces whose perspective-correct
+ *   barycentrics there are all >= 0 at a camera depth Z with near <= Z <= far (0 < near < far); the one with the
+ *   smallest (fp32(Z), face index) wins.  depth f32 [b,h,w] (NULL: not written) receives fp32(Z), 0 where nothing
+ *   covers the pixel; rgb uint8 [b,h,w,3] (NULL: not written) receives round(255 * fp32(light_w * colour)),
+ *   light_w = min(ambient + max(L . n, 0), 1), and the background bg (host f32 [3], NULL: black) where nothing
+ *   covers the pixel.  At least one of depth and rgb.  Workspace: pvnet_render_workspace_bytes(b, h, w), one 64-bit
+ *   key per pixel.  The output does not depend on scheduling. */
+PVNET_API int pvnet_render_workspace_bytes(int b, int h, int w, size_t *bytes);
+PVNET_API int pvnet_render_mesh(const float *verts, const int32_t *faces, const float *colors, int nv, int nf,
+                                const float *poses, const float *K, int k_per_image, int b, int h, int w,
+                                float near_clip, float far_clip, float ambient, const float *bg, float *depth,
+                                uint8_t *rgb, void *workspace, size_t workspace_bytes, pvnet_stream_t stream);
 
 /* The vanishing-point pair of the reference extension (ransac_voting.cpp:61-99 ->
  * ransac_voting_kernel.cu:170-260, :263-351; used by ransac_voting_vanish_point_layer,

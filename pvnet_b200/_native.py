@@ -102,6 +102,10 @@ SIGNATURES = {
     "pvnet_farthest_point_sampling": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_size_t,
                                               c_void_p]),
     "pvnet_mesh_binary_rasterization": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "pvnet_render_workspace_bytes": (c_int, [c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
+    "pvnet_render_mesh": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int,
+                                  c_int, c_float, c_float, c_float, ctypes.POINTER(c_float), c_void_p, c_void_p,
+                                  c_void_p, c_size_t, c_void_p]),
     "pvnet_generate_hypothesis": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "pvnet_voting_for_hypothesis": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float,
                                             c_void_p]),
