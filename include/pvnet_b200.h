@@ -29,6 +29,7 @@
  *   lib/utils/extend_utils/src/farthest_point_sampling.cpp        farthest_point_sampling[_init_center]
  *   lib/utils/extend_utils/src/mesh_rasterization.cpp             mesh_binary_rasterization
  *   lib/utils/opengl_render_backend.py:306-419                    render (depth and flat RGB)
+ *   lib/utils/data_utils.py:788-826                               get_mask_of_all_objects (label map)
  *   lib/utils/net_utils.py:54-80,329-348                          smooth_l1_loss, compute_precision_recall
  *   tools/train_linemod.py:83-91                                  NetWrapper's cross-entropy (nn.CrossEntropyLoss)
  *   lib/networks/model_repository.py:64-80                        Resnet18_8s.forward
@@ -471,6 +472,26 @@ PVNET_API int pvnet_render_mesh(const float *verts, const int32_t *faces, const 
                                 const float *poses, const float *K, int k_per_image, int b, int h, int w,
                                 float near_clip, float far_clip, float ambient, const float *bg, float *depth,
                                 uint8_t *rgb, void *workspace, size_t workspace_bytes, pvnet_stream_t stream);
+
+/* pvnet_render_label_map: the label map of several meshes at b images in one depth test, the reference's
+ *   OcclusionLineModDB.get_mask_of_all_objects (lib/utils/data_utils.py:788-826; DESIGN.md §25).
+ *   M meshes (1 <= M <= 255) packed one after the other: verts f32 [sum nv,3], faces int32 [nf_total,3] with indices
+ *   local to their mesh, and mesh_table int32 [M,4] on the device, row m = {vert_off, nv, face_off, nf}, where
+ *   face_off is the sum of the earlier meshes' nf and nf_total the sum of all.  labels uint8 [M] (host), each 1..255.
+ *   poses f32 [b,M,3,4] (R | t of slot m in image i); present uint8 [b,M] (0: the slot is absent from the image) or
+ *   NULL (all present); K f32 [3,3], or [b,3,3] when k_per_image != 0.  Coverage, clip planes and pixel convention
+ *   are pvnet_render_mesh's.  A slot's depth at a pixel is pvnet_render_mesh's depth of that mesh alone divided by
+ *   depth_divisor in one IEEE fp32 division (depth_divisor > 0 and finite, near / depth_divisor above 0).
+ *   label uint8 [b,h,w] receives the label of the slot with the smallest depth strictly below max_depth (> 0, +inf
+ *   allowed), ties to the lower slot, and 0 where there is none; depth f32 [b,h,w] (NULL: not written) receives that
+ *   depth, max_depth where the label is 0.  Workspace: pvnet_render_workspace_bytes(b, h, w).  The output does not
+ *   depend on scheduling. */
+PVNET_API int pvnet_render_label_map(const float *verts, const int32_t *faces, const int32_t *mesh_table,
+                                     const uint8_t *labels, int M, int nf_total, const float *poses,
+                                     const uint8_t *present, const float *K, int k_per_image, int b, int h, int w,
+                                     float near_clip, float far_clip, float depth_divisor, float max_depth,
+                                     uint8_t *label, float *depth, void *workspace, size_t workspace_bytes,
+                                     pvnet_stream_t stream);
 
 /* The vanishing-point pair of the reference extension (ransac_voting.cpp:61-99 ->
  * ransac_voting_kernel.cu:170-260, :263-351; used by ransac_voting_vanish_point_layer,

@@ -106,6 +106,9 @@ SIGNATURES = {
     "pvnet_render_mesh": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int,
                                   c_int, c_float, c_float, c_float, ctypes.POINTER(c_float), c_void_p, c_void_p,
                                   c_void_p, c_size_t, c_void_p]),
+    "pvnet_render_label_map": (c_int, [c_void_p, c_void_p, c_void_p, ctypes.POINTER(ctypes.c_uint8), c_int, c_int,
+                                       c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_float,
+                                       c_float, c_float, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "pvnet_generate_hypothesis": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "pvnet_voting_for_hypothesis": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float,
                                             c_void_p]),

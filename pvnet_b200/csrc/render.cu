@@ -19,9 +19,14 @@
 // Launches: the keys are set to all ones (cudaMemsetAsync); k_render_raster takes the flattened (pose, face)
 // pairs, a warp per face walking its pixel box, boxes above RD_BIG pixels deferred to the whole CTA; k_render_resolve
 // writes depth and RGB per pixel, recomputing the winner's barycentrics with the same face_setup/face_fragment.
+//
+// pvnet_render_label_map (DESIGN.md §25) runs the same raster kernel over several meshes at once (LabelScene): the
+// key holds the fp32 depth divided by a scale and the mesh's slot, so one depth test gives each pixel the nearest
+// mesh, and k_label_resolve turns the keys into a label map and its depth.
 #include "common.cuh"
 
 #include <cmath>
+#include <cstring>
 
 namespace {
 
@@ -160,17 +165,21 @@ __device__ __forceinline__ bool face_box(const Face &F, int h, int w, double nea
     return true;
 }
 
-__device__ __forceinline__ void raster_pixel(const Face &F, int f, int col, int row, int w, double nearp,
-                                             double farp, unsigned long long *__restrict__ keys)
+// The key of a fragment is bits(d) << 32 | tag: d the scene's fp32 depth of Z (positive, so its bits order like
+// the depths) and tag the scene's tie-break (the face, or the mesh slot).
+template <class S>
+__device__ __forceinline__ void raster_pixel(const S &s, const Face &F, uint32_t tag, int col, int row,
+                                             unsigned long long *__restrict__ keys)
 {
     double lam[3], Z;
-    if (!face_fragment(F, col, row, nearp, farp, lam, Z)) return;
-    const unsigned long long key =
-        (static_cast<unsigned long long>(__float_as_uint(__double2float_rn(Z))) << 32) | static_cast<uint32_t>(f);
-    unsigned long long *k = keys + static_cast<size_t>(row) * w + col;
+    if (!face_fragment(F, col, row, s.nearp, s.farp, lam, Z)) return;
+    const unsigned long long key = (static_cast<unsigned long long>(__float_as_uint(s.depth(Z))) << 32) | tag;
+    unsigned long long *k = keys + static_cast<size_t>(row) * s.w + col;
     if (*k > key) atomicMin(k, key);             // keys only decrease: a key at or below ours makes the atomic a no-op
 }
 
+// One mesh at b poses: pair t of the flattened (pose, face) pairs is face t % nf of image t / nf, and its tag is the
+// face index.
 struct Scene {
     const float *verts;
     const int32_t *faces;
@@ -180,51 +189,104 @@ struct Scene {
     int kstride;                                  // 0 or 9
     int nv, nf, h, w;
     double nearp, farp;
+
+    __device__ __forceinline__ void load_shared(int *) const {}
+    __device__ __forceinline__ bool pair(const int *, int t, int &img, uint32_t &tag, Face &F) const
+    {
+        img = t / nf;
+        const int f = t - img * nf;
+        tag = static_cast<uint32_t>(f);
+        return face_setup(verts, faces, f, nv, poses + static_cast<size_t>(img) * 12,
+                          K + static_cast<size_t>(img) * kstride, F);
+    }
+    __device__ __forceinline__ float depth(double Z) const { return __double2float_rn(Z); }
+};
+
+// Several meshes in one depth test (DESIGN.md §25): the meshes' vertices and faces are packed one after the other,
+// table[m] = {vert_off, nv, face_off, nf} with face_off the sum of the earlier meshes' nf, and pair t is global face
+// t % nf_total of image t / nf_total.  Its slot m is found in the table, which the CTA holds in shared memory; a
+// face of an absent slot covers nothing.  The tag is the slot and the depth is fp32(Z) / divisor, one IEEE fp32
+// division: with ties going to the lower slot this is the reference's sequential `depth < depth_map` update.
+struct LabelScene {
+    const float *verts;
+    const int32_t *faces;
+    const int32_t *table;                         // [M,4] device
+    const float *poses;                           // [b,M,3,4]
+    const uint8_t *present;                       // [b,M] or NULL (all present)
+    const float *K;                               // [3,3] or [b,3,3]
+    int kstride;                                  // 0 or 9
+    int M, nf, h, w;                              // nf: the faces of all the meshes
+    double nearp, farp;
+    float divisor;
+
+    __device__ __forceinline__ void load_shared(int *tab) const
+    {
+        for (int i = threadIdx.x; i < M * 4; i += blockDim.x) tab[i] = table[i];
+    }
+    __device__ __forceinline__ bool pair(const int *tab, int t, int &img, uint32_t &tag, Face &F) const
+    {
+        img = t / nf;
+        const int g = t - img * nf;
+        int lo = 0, hi = M;                       // the last slot whose faces start at or before g
+        while (hi - lo > 1) {
+            const int mid = (lo + hi) >> 1;
+            if (tab[mid * 4 + 2] <= g) lo = mid;
+            else hi = mid;
+        }
+        tag = static_cast<uint32_t>(lo);
+        const int *e = tab + lo * 4;
+        const int f = g - e[2];
+        if (f < 0 || f >= e[3]) return false;     // only a table whose face offsets are not the running sum
+        if (present && !present[static_cast<size_t>(img) * M + lo]) return false;
+        return face_setup(verts + static_cast<size_t>(e[0]) * 3, faces + static_cast<size_t>(e[2]) * 3, f, e[1],
+                          poses + (static_cast<size_t>(img) * M + lo) * 12, K + static_cast<size_t>(img) * kstride,
+                          F);
+    }
+    __device__ __forceinline__ float depth(double Z) const { return __fdiv_rn(__double2float_rn(Z), divisor); }
 };
 
 // grid: ceil(b * nf / RD_WARPS) CTAs; warp w of CTA c takes pair c * RD_WARPS + w of the flattened (pose, face)
 // pairs.  Faces whose box has more than RD_BIG pixels are handled after the others by the whole CTA, its warps
-// taking every RD_WARPS-th row.
-__global__ void __launch_bounds__(RD_THREADS)
-    k_render_raster(Scene s, int total, unsigned long long *__restrict__ keys)
+// taking every RD_WARPS-th row.  Dynamic shared memory: what the scene's load_shared writes.
+template <class S>
+__global__ void __launch_bounds__(RD_THREADS) k_render_raster(S s, int total, unsigned long long *__restrict__ keys)
 {
+    extern __shared__ int s_scene[];
     __shared__ int s_big[RD_WARPS];
     __shared__ int s_nbig;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     if (threadIdx.x == 0) s_nbig = 0;
+    s.load_shared(s_scene);
     __syncthreads();
     const int t = blockIdx.x * RD_WARPS + warp;
     const size_t hw = static_cast<size_t>(s.h) * s.w;
     if (t < total) {
-        const int img = t / s.nf, f = t - img * s.nf;
+        int img;
+        uint32_t tag;
         Face F;
         Box B;
-        if (face_setup(s.verts, s.faces, f, s.nv, s.poses + static_cast<size_t>(img) * 12,
-                       s.K + static_cast<size_t>(img) * s.kstride, F) &&
-            face_box(F, s.h, s.w, s.nearp, B)) {
+        if (s.pair(s_scene, t, img, tag, F) && face_box(F, s.h, s.w, s.nearp, B)) {
             const int bw = B.ex - B.bx + 1;
             const long long npix = static_cast<long long>(bw) * (B.ey - B.by + 1);
             if (npix > RD_BIG) {
                 if (lane == 0) s_big[atomicAdd(&s_nbig, 1)] = t;
             } else {
                 unsigned long long *k = keys + img * hw;
-                for (int p = lane; p < npix; p += 32)
-                    raster_pixel(F, f, B.bx + p % bw, B.by + p / bw, s.w, s.nearp, s.farp, k);
+                for (int p = lane; p < npix; p += 32) raster_pixel(s, F, tag, B.bx + p % bw, B.by + p / bw, k);
             }
         }
     }
     __syncthreads();
     for (int i = 0; i < s_nbig; ++i) {
-        const int tb = s_big[i];
-        const int img = tb / s.nf, f = tb - img * s.nf;
+        int img;
+        uint32_t tag;
         Face F;
         Box B;
-        face_setup(s.verts, s.faces, f, s.nv, s.poses + static_cast<size_t>(img) * 12,
-                   s.K + static_cast<size_t>(img) * s.kstride, F);
+        s.pair(s_scene, s_big[i], img, tag, F);
         face_box(F, s.h, s.w, s.nearp, B);
         unsigned long long *k = keys + img * hw;
         for (int row = B.by + warp; row <= B.ey; row += RD_WARPS)
-            for (int col = B.bx + lane; col <= B.ex; col += 32) raster_pixel(F, f, col, row, s.w, s.nearp, s.farp, k);
+            for (int col = B.bx + lane; col <= B.ex; col += 32) raster_pixel(s, F, tag, col, row, k);
     }
 }
 
@@ -316,6 +378,26 @@ __global__ void __launch_bounds__(RD_RESOLVE_THREADS)
     rgb[i * 3 + 2] = c[2];
 }
 
+struct Labels {
+    uint8_t v[256];                               // slot -> label
+};
+
+// one thread per output pixel of the batch: the winning key's slot gives the label and its high bits the divided
+// depth, unless that depth is at or above max_depth (float bits of non-negative depths order like the depths; an
+// empty key's high bits are all ones, above +inf's)
+__global__ void __launch_bounds__(RD_RESOLVE_THREADS)
+    k_label_resolve(long long npix, Labels labels, uint32_t max_bits, const unsigned long long *__restrict__ keys,
+                    uint8_t *__restrict__ label, float *__restrict__ depth)
+{
+    const long long i = static_cast<long long>(blockIdx.x) * RD_RESOLVE_THREADS + threadIdx.x;
+    if (i >= npix) return;
+    const unsigned long long key = keys[i];
+    const uint32_t hi = static_cast<uint32_t>(key >> 32);
+    const bool hit = hi < max_bits;
+    label[i] = hit ? labels.v[static_cast<uint32_t>(key) & 255u] : 0;
+    if (depth) depth[i] = __uint_as_float(hit ? hi : max_bits);
+}
+
 uint8_t host_u8(float x)
 {
     volatile float g = x * 255.f;                 // one rounded fp32 multiply
@@ -379,6 +461,68 @@ int pvnet_render_mesh(const float *verts, const int32_t *faces, const float *col
     k_render_resolve<<<static_cast<unsigned>((npix + RD_RESOLVE_THREADS - 1) / RD_RESOLVE_THREADS),
                        RD_RESOLVE_THREADS, 0, st>>>(s, npix, ambient, bgc, keys, depth, rgb);
     PV_LAUNCHED("k_render_resolve");
+    return PVNET_OK;
+}
+
+int pvnet_render_label_map(const float *verts, const int32_t *faces, const int32_t *mesh_table, const uint8_t *labels,
+                           int M, int nf_total, const float *poses, const uint8_t *present, const float *K,
+                           int k_per_image, int b, int h, int w, float near_clip, float far_clip, float depth_divisor,
+                           float max_depth, uint8_t *label, float *depth, void *workspace, size_t workspace_bytes,
+                           pvnet_stream_t stream)
+{
+    PV_CHECK_ARG(M >= 1 && M <= 255, "mesh count %d outside 1..255", M);
+    PV_CHECK_ARG(b >= 1 && h >= 1 && w >= 1 && nf_total >= 0, "bad dimension (b=%d, h=%d, w=%d, nf_total=%d)", b, h,
+                 w, nf_total);
+    PV_CHECK_ARG(static_cast<long long>(h) * w <= INT32_MAX, "image %dx%d too large", h, w);
+    PV_CHECK_ARG(static_cast<long long>(b) * nf_total <= INT32_MAX - RD_WARPS, "b * nf_total too large");
+    PV_CHECK_ARG(static_cast<long long>(b) * h * w <= static_cast<long long>(INT32_MAX) * RD_RESOLVE_THREADS,
+                 "b * h * w too large");
+    PV_CHECK_ARG(std::isfinite(near_clip) && std::isfinite(far_clip) && near_clip > 0.f && near_clip < far_clip,
+                 "clip planes must satisfy 0 < near < far (got %g, %g)", near_clip, far_clip);
+    PV_CHECK_ARG(std::isfinite(depth_divisor) && depth_divisor > 0.f, "depth_divisor must be positive and finite (got %g)",
+                 depth_divisor);
+    volatile float nearest = near_clip / depth_divisor;  // one rounded fp32 division, as on the device
+    PV_CHECK_ARG(nearest > 0.f, "near / depth_divisor underflows to 0 (near %g, depth_divisor %g)", near_clip,
+                 depth_divisor);
+    PV_CHECK_ARG(max_depth > 0.f, "max_depth must be positive (+inf allowed; got %g)", max_depth);
+    PV_CHECK_ARG(mesh_table && labels && poses && K && label && (nf_total == 0 || (faces && verts)), "null pointer");
+    Labels lt = {};
+    for (int m = 0; m < M; ++m) {
+        PV_CHECK_ARG(labels[m] != 0, "label of slot %d is 0 (the background)", m);
+        lt.v[m] = labels[m];
+    }
+    size_t need = 0;
+    pvnet_render_workspace_bytes(b, h, w, &need);
+    PV_CHECK_ARG(workspace && workspace_bytes >= need, "workspace %zu bytes < %zu", workspace_bytes, need);
+    unsigned long long *keys = static_cast<unsigned long long *>(workspace);
+    const cudaStream_t st = (cudaStream_t)stream;
+    PV_CUDA(cudaMemsetAsync(keys, 0xff, need, st));
+    LabelScene s;
+    s.verts = verts;
+    s.faces = faces;
+    s.table = mesh_table;
+    s.poses = poses;
+    s.present = present;
+    s.K = K;
+    s.kstride = k_per_image ? 9 : 0;
+    s.M = M;
+    s.nf = nf_total;
+    s.h = h;
+    s.w = w;
+    s.nearp = near_clip;
+    s.farp = far_clip;
+    s.divisor = depth_divisor;
+    const int total = b * nf_total;
+    if (total > 0) {
+        k_render_raster<<<(total + RD_WARPS - 1) / RD_WARPS, RD_THREADS, M * 4 * sizeof(int), st>>>(s, total, keys);
+        PV_LAUNCHED("k_render_raster<LabelScene>");
+    }
+    uint32_t max_bits;
+    std::memcpy(&max_bits, &max_depth, sizeof max_bits);
+    const long long npix = static_cast<long long>(b) * h * w;
+    k_label_resolve<<<static_cast<unsigned>((npix + RD_RESOLVE_THREADS - 1) / RD_RESOLVE_THREADS), RD_RESOLVE_THREADS,
+                      0, st>>>(npix, lt, max_bits, keys, label, depth);
+    PV_LAUNCHED("k_label_resolve");
     return PVNET_OK;
 }
 
