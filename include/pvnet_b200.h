@@ -493,6 +493,52 @@ PVNET_API int pvnet_render_label_map(const float *verts, const int32_t *faces, c
                                      uint8_t *label, float *depth, void *workspace, size_t workspace_bytes,
                                      pvnet_stream_t stream);
 
+/* pvnet_refine_poses: silhouette pose refinement of one mesh at b poses, the four steps of the reference's
+ *   `post_refinement` docstring (lib/utils/extend_utils/extend_utils.py:181-193, whose body is `pass`; DESIGN.md §26).
+ *   Per image and round: the depth at the current pose from pvnet_render_mesh; the silhouette (covered pixels with an
+ *   uncovered or outside 4-neighbour), back-projected through that depth to object space; the mask's contour
+ *   (nonzero pixels with a zero or outside 4-neighbour); each silhouette point's nearest contour pixel in fp32
+ *   squared pixel distance, ties to the lowest contour index, dropped beyond gate pixels; then, the pairs held fixed,
+ *   three damped Gauss-Newton steps on sum |pi(K(R X + t)) - c|^2 with R <- exp(dw) R, t <- t + dt.  Both point
+ *   sets are row-major; above max_points only every ceil(n / max_points)-th point is kept.  Each round is checked
+ *   by the next render: a round that raises the mean pair distance, or leaves no silhouette or fewer than 6 pairs, is
+ *   undone and the image stops.  So rounds + 1 renders; rounds = 0 returns the input.
+ *   mask       uint8 [b,h,w], nonzero = foreground, device
+ *   poses_in   f64 [b,3,4] (R | t, object to OpenCV camera), device
+ *   K          f32 [3,3], or [b,3,3] when k_per_image != 0, device; read as pvnet_render_mesh reads it (fx, s, cx,
+ *              fy, cy), the back-projection is the inverse of its projection
+ *   verts f32 [nv,3], faces int32 [nf,3]: the mesh, in the poses' translation units; near_clip, far_clip as for
+ *              pvnet_render_mesh
+ *   rounds >= 0; gate > 0 (pixels); max_points >= 1
+ *   poses_out  f64 [b,3,4], device (not poses_in)
+ *   info       int32 [b,2] or NULL: (status bits, pairs of the last round that took its steps); status 1: the mask
+ *              has no foreground, 2: the render at the input pose covers nothing, 4: fewer than 6 pairs at the input
+ *              pose (each of these returns the input pose), 8: a singular system (the round's starting pose is
+ *              kept), 16: a round was undone
+ *   dist       f64 [b,2] or NULL: mean pair distance in pixels at the input pose and at the returned pose (NaN
+ *              where there were no pairs)
+ *   trace      NULL, or device buffers (each nullable) that receive the input-pose round's intermediates:
+ *              sil_idx, con_idx, pair_idx int32 [b,max_points] (pixel indices r*w+c; contour index or -1), counts
+ *              int32 [b,2] (silhouette, contour points kept), sil_obj f64 [b,max_points,3], normal_eq f64 [b,27]
+ *              (the first step's 21 upper-triangle sums of J^T J row by row, then J^T r; written only when it runs)
+ *   Workspace: pvnet_refine_workspace_bytes(b, h, w, max_points).  No allocation, no host synchronisation, a fixed
+ *   number of launches for given rounds (graph capturable), and run-to-run identical output: the sums are reduced in
+ *   a fixed order, without floating-point atomics. */
+typedef struct {
+    int32_t *sil_idx;
+    int32_t *con_idx;
+    int32_t *counts;
+    double *sil_obj;
+    int32_t *pair_idx;
+    double *normal_eq;
+} pvnet_refine_trace_t;
+PVNET_API int pvnet_refine_workspace_bytes(int b, int h, int w, int max_points, size_t *bytes);
+PVNET_API int pvnet_refine_poses(const uint8_t *mask, const double *poses_in, const float *K, int k_per_image,
+                                 const float *verts, const int32_t *faces, int nv, int nf, int b, int h, int w,
+                                 float near_clip, float far_clip, int rounds, float gate, int max_points,
+                                 double *poses_out, int32_t *info, double *dist, const pvnet_refine_trace_t *trace,
+                                 void *workspace, size_t workspace_bytes, pvnet_stream_t stream);
+
 /* The vanishing-point pair of the reference extension (ransac_voting.cpp:61-99 ->
  * ransac_voting_kernel.cu:170-260, :263-351; used by ransac_voting_vanish_point_layer,
  * ransac_voting_gpu.py:408-501): hypotheses are homogeneous points hypo [hn,vn,3]; the vote sets

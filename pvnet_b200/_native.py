@@ -32,6 +32,12 @@ class BatchNormParams(ctypes.Structure):
 c_bn_p = ctypes.POINTER(BatchNormParams)
 
 
+class RefineTrace(ctypes.Structure):
+    """pvnet_refine_trace_t: device buffers for the first round's intermediates (include/pvnet_b200.h)."""
+    _fields_ = [("sil_idx", c_void_p), ("con_idx", c_void_p), ("counts", c_void_p), ("sil_obj", c_void_p),
+                ("pair_idx", c_void_p), ("normal_eq", c_void_p)]
+
+
 class AdamTensor(ctypes.Structure):
     """pvnet_adam_tensor_t: one entry of pvnet_adam_step's host table (include/pvnet_b200.h)."""
     _fields_ = [("param", c_void_p), ("grad", c_void_p), ("exp_avg", c_void_p), ("exp_avg_sq", c_void_p),
@@ -109,7 +115,11 @@ SIGNATURES = {
     "pvnet_render_label_map": (c_int, [c_void_p, c_void_p, c_void_p, ctypes.POINTER(ctypes.c_uint8), c_int, c_int,
                                        c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_float,
                                        c_float, c_float, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
-    "pvnet_generate_hypothesis": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "pvnet_refine_workspace_bytes": (c_int, [c_int, c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
+    "pvnet_refine_poses": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
+                                   c_int, c_float, c_float, c_int, c_float, c_int, c_void_p, c_void_p, c_void_p,
+                                   ctypes.POINTER(RefineTrace), c_void_p, c_size_t, c_void_p]),
+    "pvnet_generate_hypothesis":(c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "pvnet_voting_for_hypothesis": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float,
                                             c_void_p]),
     "pvnet_generate_hypothesis_vanishing_point": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,

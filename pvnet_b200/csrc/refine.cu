@@ -1,0 +1,555 @@
+// refine.cu -- silhouette pose refinement for a batch of poses (DESIGN.md §26): the four steps the reference's
+// `post_refinement` docstring lists and leaves unimplemented (lib/utils/extend_utils/extend_utils.py:181-193).
+//
+// One round, per image: render the depth at the current pose with pvnet_render_mesh (the renderer itself, not a
+// copy); take the silhouette (covered pixels with an uncovered or outside 4-neighbour) and back-project it to object
+// space; take the mask's contour (foreground pixels with a background or outside 4-neighbour; the first round only,
+// the mask does not change); pair each silhouette point with its nearest contour pixel; then, pairs held fixed, a few
+// damped Gauss-Newton steps on sum |pi(K(R X + t)) - c|^2 with R <- exp(dw) R, t <- t + dt.  The next round's render
+// evaluates the step: a round whose mean pair distance rose is undone and the image stops.  oracle/refine_oracle.py
+// restates every stage; the boundary sets, back-projection and pairs follow it bit for bit (one rounded __d*_rn /
+// __f*_rn intrinsic per operation where the order matters), the normal equations to rounding.
+//
+// Launches per evaluation: the renderer's three, k_refine_boundary (one 512-thread CTA per image and point set),
+// k_refine_pairs (a 256-point tile of one image's silhouette per CTA against its whole contour, staged through shared
+// memory) and k_refine_step (one CTA per image: the mean distance, the accept / reject decision and the
+// Gauss-Newton steps, the 6x6 sums reduced in a fixed order).  Nothing is allocated and nothing synchronises.
+#include "common.cuh"
+
+#include <cmath>
+
+namespace {
+
+constexpr int RF_BOUND_THREADS = 512;
+constexpr int RF_PER_THREAD = 16;                 // consecutive pixels per thread in the boundary scan
+constexpr int RF_CHUNK = RF_BOUND_THREADS * RF_PER_THREAD;
+constexpr int RF_PAIR_THREADS = 256;
+constexpr int RF_TILE = 2048;                     // contour points per shared-memory tile (16 KB)
+constexpr int RF_STEP_THREADS = 256;
+constexpr int RF_GN_STEPS = 3;
+constexpr double RF_DAMPING = 1e-3;
+constexpr int RF_MIN_PAIRS = 6;
+constexpr int RF_NSUM = 27;                       // 21 entries of the upper triangle of A, then g
+
+constexpr int RF_NO_CONTOUR = 1, RF_NO_SILHOUETTE = 2, RF_FEW_PAIRS = 4, RF_SINGULAR = 8, RF_REJECTED = 16;
+
+__device__ __forceinline__ double dm(double a, double b) { return __dmul_rn(a, b); }
+__device__ __forceinline__ double da(double a, double b) { return __dadd_rn(a, b); }
+__device__ __forceinline__ double ds(double a, double b) { return __dsub_rn(a, b); }
+__device__ __forceinline__ double dd(double a, double b) { return __ddiv_rn(a, b); }
+
+struct Cam {
+    double fx, s, cx, fy, cy;                     // K as the renderer reads it: fp32 widened
+};
+
+__device__ __forceinline__ Cam load_cam(const float *K)
+{
+    return {(double)K[0], (double)K[1], (double)K[2], (double)K[4], (double)K[5]};
+}
+
+// Per-image state across rounds (workspace).
+struct State {
+    double backup[12];                            // the pose the current round started from
+    double mean0, mean_prev, mean_after;
+    int status, done, pairs, pad;
+};
+
+// Projection of X at pose P (row-major [3,4] fp64), the renderer's order: p = R X, Xc = p + t,
+// u = ((fx X + s Y) + cx Z) / Z, v = (fy Y + cy Z) / Z.
+__device__ __forceinline__ void project(const double *P, const Cam &c, double x, double y, double z, double &u,
+                                        double &v)
+{
+    double Xc[3];
+#pragma unroll
+    for (int r = 0; r < 3; ++r) Xc[r] = da(da(da(dm(P[r * 4], x), dm(P[r * 4 + 1], y)), dm(P[r * 4 + 2], z)), P[r * 4 + 3]);
+    u = dd(da(da(dm(c.fx, Xc[0]), dm(c.s, Xc[1])), dm(c.cx, Xc[2])), Xc[2]);
+    v = dd(da(dm(c.fy, Xc[1]), dm(c.cy, Xc[2])), Xc[2]);
+}
+
+// Boundary of one point set of one image: blockIdx.y == 0 the silhouette (depth > 0), 1 the mask's contour (nonzero).
+// Pass 1 counts the boundary pixels; pass 2 walks them again in row-major order and keeps rank % stride == 0,
+// stride = ceil(n / max_points), writing each at rank / stride.  A silhouette point is back-projected at the pose
+// it was rendered from.  skip_done: images already stopped are left alone.
+__global__ void __launch_bounds__(RF_BOUND_THREADS, 1)
+    k_refine_boundary(const float *__restrict__ depth, const uint8_t *__restrict__ mask, const double *__restrict__ pose,
+                      const float *__restrict__ K, int kstride, int h, int w, int max_points, int skip_done,
+                      const State *__restrict__ state, int32_t *__restrict__ sil_idx, double *__restrict__ sil_obj,
+                      int32_t *__restrict__ con_idx, int32_t *__restrict__ counts)
+{
+    const int img = blockIdx.x, which = blockIdx.y;
+    if (skip_done && state[img].done) return;
+    __shared__ int s_warp[RF_BOUND_THREADS / 32];
+    __shared__ int s_total;
+    __shared__ double s_pose[12];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const long long hw = static_cast<long long>(h) * w;
+    const float *dep = depth + img * hw;
+    const uint8_t *msk = mask + img * hw;
+    if (tid == 0) s_total = 0;
+    if (tid < 12) s_pose[tid] = pose[img * 12 + tid];
+    __syncthreads();
+    auto on = [&](long long p) -> bool { return which == 0 ? dep[p] > 0.f : msk[p] != 0; };
+    auto edge = [&](long long p) -> bool {
+        if (!on(p)) return false;
+        const int r = static_cast<int>(p / w), c = static_cast<int>(p - static_cast<long long>(r) * w);
+        if (r == 0 || r == h - 1 || c == 0 || c == w - 1) return true;
+        return !on(p - 1) || !on(p + 1) || !on(p - w) || !on(p + w);
+    };
+    int local = 0;
+    for (long long base = 0; base < hw; base += RF_CHUNK)
+        for (int q = 0; q < RF_PER_THREAD; ++q) {
+            const long long p = base + static_cast<long long>(tid) * RF_PER_THREAD + q;
+            if (p < hw && edge(p)) ++local;
+        }
+    atomicAdd(&s_total, local);                   // an integer sum: the same whatever the order
+    __syncthreads();
+    const int n = s_total;
+    const int stride = n > max_points ? (n + max_points - 1) / max_points : 1;
+    int32_t *idx_out = (which == 0 ? sil_idx : con_idx) + static_cast<size_t>(img) * max_points;
+    double *obj_out = sil_obj + static_cast<size_t>(img) * max_points * 3;
+    const Cam cam = load_cam(K + static_cast<size_t>(img) * kstride);
+    int running = 0;                              // boundary pixels in earlier chunks
+    for (long long base = 0; base < hw; base += RF_CHUNK) {
+        unsigned bits = 0;
+        for (int q = 0; q < RF_PER_THREAD; ++q) {
+            const long long p = base + static_cast<long long>(tid) * RF_PER_THREAD + q;
+            if (p < hw && edge(p)) bits |= 1u << q;
+        }
+        const int cnt = __popc(bits);
+        int incl = cnt;                           // inclusive scan over the warp
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const int y = __shfl_up_sync(0xffffffffu, incl, o);
+            if (lane >= o) incl += y;
+        }
+        if (lane == 31) s_warp[warp] = incl;
+        __syncthreads();
+        if (warp == 0) {
+            int t = lane < RF_BOUND_THREADS / 32 ? s_warp[lane] : 0;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const int y = __shfl_up_sync(0xffffffffu, t, o);
+                if (lane >= o) t += y;
+            }
+            if (lane < RF_BOUND_THREADS / 32) s_warp[lane] = t;   // inclusive warp totals
+        }
+        __syncthreads();
+        int rank = running + (warp ? s_warp[warp - 1] : 0) + incl - cnt;
+        for (int q = 0; q < RF_PER_THREAD; ++q) {
+            if (!(bits >> q & 1u)) continue;
+            if (rank % stride == 0) {
+                const long long p = base + static_cast<long long>(tid) * RF_PER_THREAD + q;
+                const int j = rank / stride;
+                idx_out[j] = static_cast<int32_t>(p);
+                if (which == 0) {
+                    const int r = static_cast<int>(p / w), c = static_cast<int>(p - static_cast<long long>(r) * w);
+                    const double u = c + 0.5, v = r + 0.5, Z = dep[p];
+                    const double yn = dd(ds(v, cam.cy), cam.fy);
+                    const double xn = dd(ds(ds(u, cam.cx), dm(cam.s, yn)), cam.fx);
+                    const double d0 = ds(dm(Z, xn), s_pose[3]), d1 = ds(dm(Z, yn), s_pose[7]), d2 = ds(Z, s_pose[11]);
+#pragma unroll
+                    for (int k = 0; k < 3; ++k)
+                        obj_out[j * 3 + k] = da(da(dm(s_pose[k], d0), dm(s_pose[4 + k], d1)), dm(s_pose[8 + k], d2));
+                }
+            }
+            ++rank;
+        }
+        running += s_warp[RF_BOUND_THREADS / 32 - 1];
+        __syncthreads();                          // s_warp is rewritten by the next chunk
+    }
+    if (tid == 0) counts[img * 2 + which] = n ? (n + stride - 1) / stride : 0;
+}
+
+// Nearest contour pixel of each silhouette point: grid (ceil(max_points / 256), b).  The point is projected at the
+// current pose and rounded to fp32; d2 = (cu - pu)^2 + (cv - pv)^2 in fp32, each operation rounded; the strictly
+// smaller d2 wins while the contour is walked in order, so ties keep the lowest index.  pair = -1 when the nearest
+// d2 is above gate2 or is not a number (or there is no contour).
+__global__ void __launch_bounds__(RF_PAIR_THREADS)
+    k_refine_pairs(const double *__restrict__ pose, const float *__restrict__ K, int kstride, int w, int max_points,
+                   float gate2, int skip_done, const State *__restrict__ state, const int32_t *__restrict__ counts,
+                   const double *__restrict__ sil_obj, const int32_t *__restrict__ con_idx,
+                   int32_t *__restrict__ pair, float *__restrict__ pair_d2)
+{
+    const int img = blockIdx.y;
+    if (skip_done && state[img].done) return;
+    const int ns = counts[img * 2], nc = counts[img * 2 + 1];
+    const int i = blockIdx.x * RF_PAIR_THREADS + threadIdx.x;
+    if (static_cast<int>(blockIdx.x) * RF_PAIR_THREADS >= ns) return;
+    __shared__ float2 s_c[RF_TILE];
+    float pu = 0.f, pv = 0.f;
+    if (i < ns) {
+        const double *P = pose + img * 12;
+        const double *X = sil_obj + (static_cast<size_t>(img) * max_points + i) * 3;
+        double u, v;
+        project(P, load_cam(K + static_cast<size_t>(img) * kstride), X[0], X[1], X[2], u, v);
+        pu = __double2float_rn(u);
+        pv = __double2float_rn(v);
+    }
+    float best = INFINITY;
+    int bj = -1;
+    const int32_t *con = con_idx + static_cast<size_t>(img) * max_points;
+    for (int t0 = 0; t0 < nc; t0 += RF_TILE) {
+        const int tn = min(RF_TILE, nc - t0);
+        __syncthreads();
+        for (int j = threadIdx.x; j < tn; j += RF_PAIR_THREADS) {
+            const int p = con[t0 + j], r = p / w, c = p - r * w;
+            s_c[j] = make_float2(c + 0.5f, r + 0.5f);
+        }
+        __syncthreads();
+        for (int j = 0; j < tn; ++j) {
+            const float2 cc = s_c[j];
+            const float dx = __fsub_rn(cc.x, pu), dy = __fsub_rn(cc.y, pv);
+            const float d2 = __fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy));
+            if (d2 < best) {
+                best = d2;
+                bj = t0 + j;
+            }
+        }
+    }
+    if (i < ns) {
+        const size_t o = static_cast<size_t>(img) * max_points + i;
+        pair[o] = best <= gate2 ? bj : -1;
+        pair_d2[o] = best;
+    }
+}
+
+// Block sum of n doubles per thread into out (thread 0's view): xor butterflies within each warp, then the warps'
+// partials in warp order.  The same inputs give the same sum every run.
+template <int N>
+__device__ __forceinline__ void block_sum(double (&v)[N], double (*s_part)[N], double *out)
+{
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int k = 0; k < N; ++k)
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) v[k] += __shfl_xor_sync(0xffffffffu, v[k], o);
+    if (lane == 0)
+#pragma unroll
+        for (int k = 0; k < N; ++k) s_part[warp][k] = v[k];
+    __syncthreads();
+    if (threadIdx.x == 0)
+        for (int k = 0; k < N; ++k) {
+            double t = s_part[0][k];
+            for (int q = 1; q < RF_STEP_THREADS / 32; ++q) t += s_part[q][k];
+            out[k] = t;
+        }
+    __syncthreads();
+}
+
+// Rodrigues, pnp.cu's form: E = I + a [w]x + b [w]x^2, row-major.
+__device__ void so3_exp(double wx, double wy, double wz, double (&E)[9])
+{
+    const double th2 = wx * wx + wy * wy + wz * wz;
+    double a, b;
+    if (th2 < 1e-16) {
+        a = 1.0 - th2 / 6.0;
+        b = 0.5 - th2 / 24.0;
+    } else {
+        const double th = sqrt(th2);
+        a = sin(th) / th;
+        b = (1.0 - cos(th)) / th2;
+    }
+    E[0] = 1.0 - b * (wy * wy + wz * wz);
+    E[1] = -a * wz + b * wx * wy;
+    E[2] = a * wy + b * wx * wz;
+    E[3] = a * wz + b * wx * wy;
+    E[4] = 1.0 - b * (wx * wx + wz * wz);
+    E[5] = -a * wx + b * wy * wz;
+    E[6] = -a * wy + b * wx * wz;
+    E[7] = a * wx + b * wy * wz;
+    E[8] = 1.0 - b * (wx * wx + wy * wy);
+}
+
+// (A + RF_DAMPING diag(A)) x = -g by Cholesky, A from the 21 upper-triangle sums.  false: not positive definite.
+__device__ bool damped_solve(const double *sum, double (&x)[6])
+{
+    double L[6][6];
+    int k = 0;
+    for (int r = 0; r < 6; ++r)
+        for (int c = r; c < 6; ++c) {
+            L[c][r] = sum[k++];
+            if (c == r) L[r][r] += RF_DAMPING * L[r][r];
+        }
+    for (int j = 0; j < 6; ++j) {
+        double d = L[j][j];
+        for (int q = 0; q < j; ++q) d -= L[j][q] * L[j][q];
+        if (!(d > 0.0) || !isfinite(d)) return false;
+        d = sqrt(d);
+        L[j][j] = d;
+        for (int r = j + 1; r < 6; ++r) {
+            double t = L[r][j];
+            for (int q = 0; q < j; ++q) t -= L[r][q] * L[j][q];
+            L[r][j] = t / d;
+        }
+    }
+    double y[6];
+    for (int r = 0; r < 6; ++r) {
+        double t = -sum[21 + r];
+        for (int q = 0; q < r; ++q) t -= L[r][q] * y[q];
+        y[r] = t / L[r][r];
+    }
+    for (int r = 5; r >= 0; --r) {
+        double t = y[r];
+        for (int q = r + 1; q < 6; ++q) t -= L[q][r] * x[q];
+        x[r] = t / L[r][r];
+    }
+    for (int r = 0; r < 6; ++r)
+        if (!isfinite(x[r])) return false;
+    return true;
+}
+
+// One CTA per image: evaluation k of the pose (mean pair distance, accept or undo), then, unless k is the last
+// evaluation, RF_GN_STEPS Gauss-Newton steps on the pairs.  The pose lives in `pose` (the caller's output); pose32
+// is its fp32 copy for the next render.  normal_eq (nullable): the sums of the first step of evaluation 0.
+__global__ void __launch_bounds__(RF_STEP_THREADS)
+    k_refine_step(double *__restrict__ pose, float *__restrict__ pose32, const float *__restrict__ K, int kstride,
+                  int w, int max_points, int k, int last, State *__restrict__ state,
+                  const int32_t *__restrict__ counts, const double *__restrict__ sil_obj,
+                  const int32_t *__restrict__ con_idx, const int32_t *__restrict__ pair,
+                  const float *__restrict__ pair_d2, double *__restrict__ normal_eq)
+{
+    const int img = blockIdx.x;
+    State &S = state[img];
+    if (S.done) return;
+    __shared__ double s_part[RF_STEP_THREADS / 32][RF_NSUM];
+    __shared__ double s_sum[RF_NSUM];
+    __shared__ double s_pose[12];
+    __shared__ int s_go;
+    const int ns = counts[img * 2], nc = counts[img * 2 + 1];
+    const size_t o = static_cast<size_t>(img) * max_points;
+    double acc[2] = {0.0, 0.0};
+    for (int i = threadIdx.x; i < ns; i += RF_STEP_THREADS)
+        if (pair[o + i] >= 0) {
+            acc[0] += 1.0;
+            acc[1] += sqrt(static_cast<double>(pair_d2[o + i]));
+        }
+    block_sum<2>(acc, reinterpret_cast<double (*)[2]>(&s_part[0][0]), s_sum);
+    if (threadIdx.x == 0) {
+        const int n = static_cast<int>(s_sum[0]);
+        const double m = n ? s_sum[1] / n : NAN;
+        bool go = true;
+        if (k == 0) {
+            int st = 0;
+            if (nc == 0) st = RF_NO_CONTOUR;
+            else if (ns == 0) st = RF_NO_SILHOUETTE;
+            else if (n < RF_MIN_PAIRS) st = RF_FEW_PAIRS;
+            if (st) {
+                S.status |= st;
+                go = false;
+            } else {
+                S.mean0 = S.mean_after = m;
+            }
+        } else if (ns == 0 || n < RF_MIN_PAIRS || m > S.mean_prev) {
+            S.status |= RF_REJECTED;
+            for (int q = 0; q < 12; ++q) pose[img * 12 + q] = S.backup[q];
+            go = false;
+        } else {
+            S.mean_after = m;
+        }
+        if (!go) S.done = 1;
+        if (go && !last) {
+            S.mean_prev = m;
+            for (int q = 0; q < 12; ++q) S.backup[q] = pose[img * 12 + q];
+            S.pairs = n;
+        }
+        s_go = go && !last;
+    }
+    if (threadIdx.x < 12) s_pose[threadIdx.x] = pose[img * 12 + threadIdx.x];
+    __syncthreads();
+    if (!s_go) return;
+    const Cam cam = load_cam(K + static_cast<size_t>(img) * kstride);
+    for (int step = 0; step < RF_GN_STEPS; ++step) {
+        double v[RF_NSUM];
+#pragma unroll
+        for (int q = 0; q < RF_NSUM; ++q) v[q] = 0.0;
+        for (int i = threadIdx.x; i < ns; i += RF_STEP_THREADS) {
+            const int j = pair[o + i];
+            if (j < 0) continue;
+            const double *X = sil_obj + (o + i) * 3;
+            const int cp = con_idx[o + j], cr = cp / w, cc = cp - cr * w;
+            double p[3], Xc[3];
+#pragma unroll
+            for (int r = 0; r < 3; ++r) {
+                p[r] = s_pose[r * 4] * X[0] + s_pose[r * 4 + 1] * X[1] + s_pose[r * 4 + 2] * X[2];
+                Xc[r] = p[r] + s_pose[r * 4 + 3];
+            }
+            const double iz = 1.0 / Xc[2];
+            const double u = (cam.fx * Xc[0] + cam.s * Xc[1] + cam.cx * Xc[2]) * iz;
+            const double vv = (cam.fy * Xc[1] + cam.cy * Xc[2]) * iz;
+            const double ru = u - (cc + 0.5), rv = vv - (cr + 0.5);
+            const double du[3] = {cam.fx * iz, cam.s * iz, -(u - cam.cx) * iz};
+            const double dv[3] = {0.0, cam.fy * iz, -(vv - cam.cy) * iz};
+            // d/d(dw) of the projection for R <- exp(dw) R is p x d(proj)/dXc; d/d(dt) is d(proj)/dXc
+            const double Ju[6] = {p[1] * du[2] - p[2] * du[1], p[2] * du[0] - p[0] * du[2], p[0] * du[1] - p[1] * du[0],
+                                  du[0], du[1], du[2]};
+            const double Jv[6] = {p[1] * dv[2] - p[2] * dv[1], p[2] * dv[0] - p[0] * dv[2], p[0] * dv[1] - p[1] * dv[0],
+                                  dv[0], dv[1], dv[2]};
+            int q = 0;
+#pragma unroll
+            for (int r = 0; r < 6; ++r)
+#pragma unroll
+                for (int c = r; c < 6; ++c) v[q++] += Ju[r] * Ju[c] + Jv[r] * Jv[c];
+#pragma unroll
+            for (int r = 0; r < 6; ++r) v[21 + r] += Ju[r] * ru + Jv[r] * rv;
+        }
+        block_sum<RF_NSUM>(v, s_part, s_sum);
+        if (threadIdx.x == 0) {
+            if (normal_eq && k == 0 && step == 0)
+                for (int q = 0; q < RF_NSUM; ++q) normal_eq[img * RF_NSUM + q] = s_sum[q];
+            double x[6];
+            if (!damped_solve(s_sum, x)) {
+                S.status |= RF_SINGULAR;
+                S.done = 1;
+                for (int q = 0; q < 12; ++q) s_pose[q] = S.backup[q];
+                s_go = 0;
+            } else {
+                double E[9], R[9];
+                so3_exp(x[0], x[1], x[2], E);
+                for (int r = 0; r < 3; ++r)
+                    for (int c = 0; c < 3; ++c)
+                        R[r * 3 + c] = E[r * 3] * s_pose[c] + E[r * 3 + 1] * s_pose[4 + c] + E[r * 3 + 2] * s_pose[8 + c];
+                for (int r = 0; r < 3; ++r) {
+                    for (int c = 0; c < 3; ++c) s_pose[r * 4 + c] = R[r * 3 + c];
+                    s_pose[r * 4 + 3] += x[3 + r];
+                }
+            }
+        }
+        __syncthreads();
+        if (!s_go) break;
+    }
+    if (threadIdx.x < 12) {
+        pose[img * 12 + threadIdx.x] = s_pose[threadIdx.x];
+        pose32[img * 12 + threadIdx.x] = __double2float_rn(s_pose[threadIdx.x]);
+    }
+}
+
+__global__ void k_refine_init(const double *__restrict__ pose_in, double *__restrict__ pose, float *__restrict__ pose32,
+                              State *__restrict__ state, int b)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= b) return;
+    for (int q = 0; q < 12; ++q) {
+        pose[i * 12 + q] = pose_in[i * 12 + q];
+        pose32[i * 12 + q] = __double2float_rn(pose_in[i * 12 + q]);
+    }
+    State &S = state[i];
+    S.mean0 = S.mean_prev = S.mean_after = NAN;
+    S.status = S.done = S.pairs = S.pad = 0;
+}
+
+__global__ void k_refine_finish(const State *__restrict__ state, int b, int32_t *__restrict__ info,
+                                double *__restrict__ dist)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= b) return;
+    if (info) {
+        info[i * 2] = state[i].status;
+        info[i * 2 + 1] = state[i].pairs;
+    }
+    if (dist) {
+        dist[i * 2] = state[i].mean0;
+        dist[i * 2 + 1] = state[i].mean_after;
+    }
+}
+
+struct Layout {
+    unsigned long long *keys;
+    float *depth, *pose32, *d2;
+    int32_t *sil, *con, *pair, *counts;
+    double *obj;
+    State *state;
+    size_t bytes;
+};
+
+Layout carve(void *base, int b, int h, int w, int max_points)
+{
+    pvnet::Carver cv(base);
+    Layout L;
+    const size_t npix = static_cast<size_t>(b) * h * w, np = static_cast<size_t>(b) * max_points;
+    L.keys = cv.take<unsigned long long>(npix);
+    L.depth = cv.take<float>(npix);
+    L.pose32 = cv.take<float>(static_cast<size_t>(b) * 12);
+    L.sil = cv.take<int32_t>(np);
+    L.con = cv.take<int32_t>(np);
+    L.pair = cv.take<int32_t>(np);
+    L.d2 = cv.take<float>(np);
+    L.obj = cv.take<double>(np * 3);
+    L.counts = cv.take<int32_t>(static_cast<size_t>(b) * 2);
+    L.state = cv.take<State>(b);
+    L.bytes = pvnet::align_up(cv.off, 256);
+    return L;
+}
+
+}  // namespace
+
+extern "C" {
+
+int pvnet_refine_workspace_bytes(int b, int h, int w, int max_points, size_t *bytes)
+{
+    PV_CHECK_ARG(b >= 1 && h >= 1 && w >= 1 && max_points >= 1, "non-positive dimension (b=%d, h=%d, w=%d, "
+                 "max_points=%d)", b, h, w, max_points);
+    PV_CHECK_ARG(bytes, "null pointer");
+    *bytes = carve(nullptr, b, h, w, max_points).bytes;
+    return PVNET_OK;
+}
+
+int pvnet_refine_poses(const uint8_t *mask, const double *poses_in, const float *K, int k_per_image,
+                       const float *verts, const int32_t *faces, int nv, int nf, int b, int h, int w, float near_clip,
+                       float far_clip, int rounds, float gate, int max_points, double *poses_out, int32_t *info,
+                       double *dist, const pvnet_refine_trace_t *trace, void *workspace, size_t workspace_bytes,
+                       pvnet_stream_t stream)
+{
+    PV_CHECK_ARG(b >= 1 && h >= 1 && w >= 1 && nv >= 0 && nf >= 0, "bad dimension (b=%d, h=%d, w=%d, nv=%d, nf=%d)",
+                 b, h, w, nv, nf);
+    PV_CHECK_ARG(static_cast<long long>(h) * w <= INT32_MAX, "image %dx%d too large", h, w);
+    PV_CHECK_ARG(max_points >= 1 && static_cast<long long>(b) * max_points <= INT32_MAX / 3,
+                 "max_points %d outside 1..%d for b = %d", max_points, INT32_MAX / 3 / b, b);
+    PV_CHECK_ARG(rounds >= 0, "rounds must be >= 0 (got %d)", rounds);
+    PV_CHECK_ARG(gate > 0.f, "gate must be positive (got %g)", gate);
+    PV_CHECK_ARG(mask && poses_in && K && poses_out && (nf == 0 || faces) && (nv == 0 || verts), "null pointer");
+    size_t need = 0;
+    pvnet_refine_workspace_bytes(b, h, w, max_points, &need);
+    PV_CHECK_ARG(workspace && workspace_bytes >= need, "workspace %zu bytes < %zu", workspace_bytes, need);
+    const Layout L = carve(workspace, b, h, w, max_points);
+    size_t render_need = 0;
+    pvnet_render_workspace_bytes(b, h, w, &render_need);
+    const cudaStream_t st = (cudaStream_t)stream;
+    const int kstride = k_per_image ? 9 : 0;
+    volatile float g2v = gate * gate;             // one rounded fp32 multiply
+    const float gate2 = g2v;
+    k_refine_init<<<(b + 127) / 128, 128, 0, st>>>(poses_in, poses_out, L.pose32, L.state, b);
+    PV_LAUNCHED("k_refine_init");
+    for (int k = 0; k <= rounds; ++k) {
+        const int rc = pvnet_render_mesh(verts, faces, nullptr, nv, nf, L.pose32, K, k_per_image, b, h, w, near_clip,
+                                         far_clip, 0.5f, nullptr, L.depth, nullptr, L.keys, render_need, stream);
+        if (rc != PVNET_OK) return rc;
+        k_refine_boundary<<<dim3(b, k == 0 ? 2 : 1), RF_BOUND_THREADS, 0, st>>>(
+            L.depth, mask, poses_out, K, kstride, h, w, max_points, k > 0, L.state, L.sil, L.obj, L.con, L.counts);
+        PV_LAUNCHED("k_refine_boundary");
+        k_refine_pairs<<<dim3((max_points + RF_PAIR_THREADS - 1) / RF_PAIR_THREADS, b), RF_PAIR_THREADS, 0, st>>>(
+            poses_out, K, kstride, w, max_points, gate2, k > 0, L.state, L.counts, L.obj, L.con, L.pair, L.d2);
+        PV_LAUNCHED("k_refine_pairs");
+        if (k == 0 && trace) {
+            const size_t np = static_cast<size_t>(b) * max_points;
+            if (trace->sil_idx) PV_CUDA(cudaMemcpyAsync(trace->sil_idx, L.sil, np * 4, cudaMemcpyDeviceToDevice, st));
+            if (trace->con_idx) PV_CUDA(cudaMemcpyAsync(trace->con_idx, L.con, np * 4, cudaMemcpyDeviceToDevice, st));
+            if (trace->counts)
+                PV_CUDA(cudaMemcpyAsync(trace->counts, L.counts, static_cast<size_t>(b) * 8, cudaMemcpyDeviceToDevice,
+                                        st));
+            if (trace->sil_obj)
+                PV_CUDA(cudaMemcpyAsync(trace->sil_obj, L.obj, np * 24, cudaMemcpyDeviceToDevice, st));
+            if (trace->pair_idx) PV_CUDA(cudaMemcpyAsync(trace->pair_idx, L.pair, np * 4, cudaMemcpyDeviceToDevice, st));
+        }
+        k_refine_step<<<b, RF_STEP_THREADS, 0, st>>>(poses_out, L.pose32, K, kstride, w, max_points, k, k == rounds,
+                                                     L.state, L.counts, L.obj, L.con, L.pair, L.d2,
+                                                     trace ? trace->normal_eq : nullptr);
+        PV_LAUNCHED("k_refine_step");
+    }
+    if (info || dist) {
+        k_refine_finish<<<(b + 127) / 128, 128, 0, st>>>(L.state, b, info, dist);
+        PV_LAUNCHED("k_refine_finish");
+    }
+    return PVNET_OK;
+}
+
+}  // extern "C"

@@ -1,0 +1,126 @@
+"""Silhouette pose refinement on the device, over `pvnet_refine_poses` (csrc/refine.cu, DESIGN.md §26).
+
+The reference declares `post_refinement(mask, pose, K, pts)` (lib/utils/extend_utils/extend_utils.py:181-193) with a
+four-step docstring -- find the mask's edge, render the silhouette and back-project it, pair it with the edge,
+optimise -- and a `pass` body; the `extend_utils` shim keeps returning None for that name.  `refine_poses` is the
+device form: each round renders the mesh at the current pose with `render_mesh`'s renderer, pairs its silhouette
+with the mask's contour and takes damped Gauss-Newton steps on the pairs' pixel distances.  oracle/refine_oracle.py
+restates it.  No CPU path: without the library or a CUDA device it raises."""
+from __future__ import annotations
+
+import ctypes
+import math
+
+import torch
+
+from . import _native
+from .extend_utils import check_cameras
+
+# status bits of info["status"]
+NO_CONTOUR = 1          # the mask has no foreground: the input pose is returned
+NO_SILHOUETTE = 2       # the render at the input pose covers nothing: the input pose is returned
+FEW_PAIRS = 4           # fewer than 6 pairs at the input pose: the input pose is returned
+SINGULAR = 8            # a round's normal equations were singular: that round's starting pose is kept
+REJECTED = 16           # a round raised the mean pair distance (or lost its pairs) and was undone
+
+
+def _cuda_tensor(name, t):
+    if not isinstance(t, torch.Tensor):
+        raise ValueError(f"{name} must be a torch tensor, got {type(t).__name__}")
+    if not t.is_cuda:
+        raise RuntimeError(f"pvnet_b200: `{name}` must be a CUDA tensor (there is no CPU path)")
+
+
+def refine_poses(mask, poses, K, vertices, faces, near, far, rounds=8, gate=20.0, max_points=4096,
+                 return_info=False, trace=False):
+    """Refine b poses of one mesh so its rendered silhouette meets each mask's contour.
+
+    mask [b,H,W] (any integer dtype or bool; nonzero is foreground), poses [b,3,4] (float32 or float64, R | t object
+    to OpenCV camera), K [3,3] or [b,3,3], vertices [nv,3] and faces [nf,3] (integer): CUDA tensors on one device.
+    The mesh is in the poses' translation units, and so are near and far, the render's clip planes.  Each round
+    pairs the silhouette with the contour, drops pairs more than `gate` pixels apart, and keeps at most `max_points`
+    points of each (every ceil(n / max_points)-th).  `rounds` is a host constant: a call is a fixed sequence of
+    launches, with no host synchronisation, and can be captured in a CUDA graph.  rounds = 0 returns the input.
+
+    -> poses float64 [b,3,4] on the device.  return_info: also a dict of [b] tensors, "status" (int32 bits, see the
+    module's constants), "pairs" (int32, the pairs of the last round that took its steps), "dist_before" and
+    "dist_after" (float64, the mean pair distance in pixels at the input pose and at the returned one, NaN without
+    pairs).  trace: also a dict of the first round's intermediates ("sil_idx", "con_idx", "pair_idx" int32
+    [b,max_points], "counts" int32 [b,2], "sil_obj" float64 [b,max_points,3], "normal_eq" float64 [b,27]), for
+    checking the stages against the oracle."""
+    for name, t in (("mask", mask), ("poses", poses), ("K", K), ("vertices", vertices), ("faces", faces)):
+        _cuda_tensor(name, t)
+    dev = poses.device
+    if any(t.device != dev for t in (mask, K, vertices, faces)):
+        raise ValueError("mask, poses, K, vertices and faces must be on one device")
+    if poses.dim() != 3 or tuple(poses.shape[1:]) != (3, 4):
+        raise ValueError(f"poses must be [b,3,4], got {tuple(poses.shape)}")
+    if poses.dtype not in (torch.float32, torch.float64):
+        raise ValueError(f"poses must be float32 or float64, got {poses.dtype}")
+    b = int(poses.shape[0])
+    if b < 1:
+        raise ValueError("poses holds no pose")
+    if mask.dim() != 3 or int(mask.shape[0]) != b:
+        raise ValueError(f"mask must be [{b},H,W], got {tuple(mask.shape)}")
+    if mask.dtype.is_floating_point or mask.dtype.is_complex:
+        raise ValueError(f"mask must be an integer or bool tensor, got {mask.dtype}")
+    h, w = int(mask.shape[1]), int(mask.shape[2])
+    if h < 1 or w < 1:
+        raise ValueError(f"image size must be positive, got {h}x{w}")
+    check_cameras(K.shape, b)
+    if vertices.dim() != 2 or vertices.shape[1] != 3:
+        raise ValueError(f"vertices must be [nv,3], got {tuple(vertices.shape)}")
+    if faces.dim() != 2 or faces.shape[1] != 3:
+        raise ValueError(f"faces must be [nf,3], got {tuple(faces.shape)}")
+    if faces.dtype.is_floating_point or faces.dtype.is_complex or faces.dtype == torch.bool:
+        raise ValueError(f"faces must hold integer indices, got {faces.dtype}")
+    near, far = float(near), float(far)
+    if not 0 < near < far < math.inf:
+        raise ValueError(f"clip planes must satisfy 0 < near < far, got {near}, {far}")
+    rounds, max_points, gate = int(rounds), int(max_points), float(gate)
+    if rounds < 0:
+        raise ValueError(f"rounds must be >= 0, got {rounds}")
+    if not 0 < gate < math.inf:
+        raise ValueError(f"gate must be positive and finite, got {gate}")
+    if not 1 <= max_points <= (2 ** 31 - 1) // 3 // b:
+        raise ValueError(f"max_points must lie in 1..{(2 ** 31 - 1) // 3 // b} for b = {b}, got {max_points}")
+
+    nv, nf = int(vertices.shape[0]), int(faces.shape[0])
+    m = mask.view(torch.uint8) if mask.dtype in (torch.uint8, torch.bool) else (mask != 0).to(torch.uint8)
+    m = m.contiguous()
+    p = poses.contiguous().double()
+    k = K.contiguous().float()
+    v = vertices.contiguous().float()
+    # an index beyond int32 is out of range either way; the clamp keeps it so
+    f = faces.contiguous() if faces.dtype == torch.int32 else faces.clamp(-1, nv).to(torch.int32).contiguous()
+    out = torch.empty((b, 3, 4), dtype=torch.float64, device=dev)
+    info = torch.empty((b, 2), dtype=torch.int32, device=dev) if return_info else None
+    dist = torch.empty((b, 2), dtype=torch.float64, device=dev) if return_info else None
+    tr, tr_struct = None, None
+    if trace:
+        tr = dict(sil_idx=torch.full((b, max_points), -1, dtype=torch.int32, device=dev),
+                  con_idx=torch.full((b, max_points), -1, dtype=torch.int32, device=dev),
+                  counts=torch.zeros((b, 2), dtype=torch.int32, device=dev),
+                  sil_obj=torch.zeros((b, max_points, 3), dtype=torch.float64, device=dev),
+                  pair_idx=torch.full((b, max_points), -1, dtype=torch.int32, device=dev),
+                  normal_eq=torch.full((b, 27), math.nan, dtype=torch.float64, device=dev))
+        tr_struct = _native.RefineTrace(*(tr[n].data_ptr() for n in ("sil_idx", "con_idx", "counts", "sil_obj",
+                                                                      "pair_idx", "normal_eq")))
+    L = _native.lib()
+    with torch.cuda.device(dev):
+        need = ctypes.c_size_t()
+        _native.check(L.pvnet_refine_workspace_bytes(b, h, w, max_points, ctypes.byref(need)),
+                      "pvnet_refine_workspace_bytes")
+        ws = torch.empty(need.value, dtype=torch.uint8, device=dev)
+        _native.check(L.pvnet_refine_poses(
+            m.data_ptr(), p.data_ptr(), k.data_ptr(), int(k.dim() == 3), v.data_ptr() if nv else None,
+            f.data_ptr() if nf else None, nv, nf, b, h, w, near, far, rounds, gate, max_points, out.data_ptr(),
+            None if info is None else info.data_ptr(), None if dist is None else dist.data_ptr(),
+            None if tr_struct is None else ctypes.byref(tr_struct), ws.data_ptr(), need.value,
+            ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "pvnet_refine_poses")
+    res = (out,)
+    if return_info:
+        res += (dict(status=info[:, 0], pairs=info[:, 1], dist_before=dist[:, 0], dist_after=dist[:, 1]),)
+    if trace:
+        res += (tr,)
+    return res[0] if len(res) == 1 else res
