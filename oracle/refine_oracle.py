@@ -4,7 +4,8 @@ unimplemented.
 
 Per image and round, in the kernel's operation order where the result is compared bit for bit:
 
-1. Depth at the current pose: `render_oracle.render` (the renderer's contract, §24) with the pose rounded to fp32.
+1. Depth at the current pose: the renderer's contract (§24, `render_oracle.render`; see below) with the pose rounded
+   to fp32.
 2. Silhouette: covered pixels (depth > 0) with a 4-neighbour that is uncovered or outside the image, row-major.
    Back-projection in fp64, K read as fp32 like the renderer reads it: u = c + 0.5, v = r + 0.5,
    yn = (v - cy) / fy, xn = ((u - cx) - s yn) / fx, X_cam = (Z xn, Z yn, Z), d = X_cam - t,
@@ -15,15 +16,22 @@ Per image and round, in the kernel's operation order where the result is compare
    u = ((fx X + s Y) + cx Z) / Z, v = (fy Y + cy Z) / Z), rounded to fp32; for each contour point's centre
    (cu, cv) in fp32, dx = cu - pu, dy = cv - pv, d2 = dx dx + dy dy in fp32; the nearest is the lowest index of the
    smallest d2; the pair is dropped (index -1) when d2 > fp32(gate) * fp32(gate) or d2 is not a number.
-5. The round's mean pair distance is the mean of sqrt(d2) in fp64 over its pairs.  Round 0 records it; a later round
-   whose mean is above the previous round's, or that has no silhouette or fewer than MIN_PAIRS pairs, is rejected:
-   the previous pose is kept and the image stops.  Otherwise, unless it is the last evaluation, GN_STEPS damped
+5. The round's mean pair distance is the mean of sqrt(d2) in fp64 over its pairs, summed in k_refine_step's order
+   (`block_sum`): bit for bit the kernel's, so the accept / undo decision below is the kernel's by construction, not
+   to a tolerance.  Round 0 records it; a later round whose mean is above the previous round's, or that has no
+   silhouette or fewer than MIN_PAIRS pairs, is rejected: the previous pose is kept and the image stops.  Otherwise, unless it is the last evaluation, GN_STEPS damped
    Gauss-Newton steps with the pairs held fixed: residual pi(X_obj) - c, Jacobian in (dw, dt) for
    R <- exp(dw) R, t <- t + dt; (A + DAMPING diag(A)) delta = -g by Cholesky.  A failed factorisation keeps the
    round's starting pose and stops the image.
 
-The normal equations are summed with numpy here and in a fixed order on the device: they agree to rounding, not bit
-for bit.  CPU only; nothing here reads the reference."""
+The normal equations are summed with numpy here and in a fixed order on the device, where nvcc also contracts
+multiplies and adds into FMAs: they agree to rounding, not bit for bit.
+
+Step 1's renderer is a parameter (`render=` of `refine_image` and `refine`).  The default is `render_oracle.render`,
+which evaluates every face at every pixel and takes seconds to minutes per 480x640 image.  The device renderer,
+`pvnet_b200.render.render_mesh`, is pinned bit for bit to it for the same fp32 pose and K (tests/test_gpu_render.py),
+so passing a wrapper around it checks the refinement's own steps at full size in seconds.  CPU only by default;
+nothing here reads the reference."""
 from __future__ import annotations
 
 import numpy as np
@@ -109,10 +117,37 @@ def nearest_pairs(X, pose, K, con, w, gate, chunk=1024):
     return j, d2
 
 
+STEP_THREADS = 256                                                  # k_refine_step's CTA
+
+
+def block_sum(x, threads=STEP_THREADS):
+    """Sum of fp64 x [n] in k_refine_step's order: thread t adds x[t], x[t + threads], ... in turn from 0.0; each
+    warp of 32 combines its lanes by xor butterflies at offsets 16, 8, 4, 2, 1 (lane l adds lane l ^ o's value;
+    fp64 addition commutes, so every lane ends with lane 0's value); then warp 0's value plus warps 1, 2, ... in
+    order."""
+    x = np.asarray(x, np.float64)
+    rows = np.zeros((-(-len(x) // threads), threads))
+    rows.reshape(-1)[:len(x)] = x
+    part = np.zeros(threads)
+    for row in rows:                                                # each thread's sum, in index order
+        part = part + row
+    lanes = part.reshape(threads // 32, 32)
+    for o in (16, 8, 4, 2, 1):
+        lanes = lanes + lanes[:, np.arange(32) ^ o]
+    total = lanes[0, 0]
+    for q in range(1, threads // 32):
+        total = total + lanes[q, 0]
+    return float(total)
+
+
 def mean_distance(j, d2):
+    """-> (kept pairs, their mean distance): sqrt(fp64(d2)) of each kept pair i, summed by `block_sum` with pair i on
+    thread i % 256 (a dropped pair adds nothing), over the count."""
     keep = j >= 0
     n = int(keep.sum())
-    return n, (float(np.sqrt(d2[keep].astype(np.float64)).sum() / n) if n else float("nan"))
+    if not n:
+        return 0, float("nan")
+    return n, block_sum(np.where(keep, np.sqrt(d2.astype(np.float64)), 0.0)) / n
 
 
 def normal_equations(X, cu, cv, pose, K):
@@ -166,10 +201,18 @@ def gauss_newton_step(A, g, pose):
     return P
 
 
-def refine_image(mask, pose, K, verts, faces, near, far, rounds=8, gate=20.0, max_points=4096, trace=None):
+def oracle_depth(verts, faces, K, pose32, h, w, near, far):
+    """Step 1's default renderer: `render_oracle.render`'s depth [h,w] fp32 of one fp32 pose [3,4]."""
+    return ro.render(verts, faces, K, pose32[None], h, w, near, far)[0][0]
+
+
+def refine_image(mask, pose, K, verts, faces, near, far, rounds=8, gate=20.0, max_points=4096, trace=None,
+                 render=None):
     """One image: mask [h,w], pose [3,4], K [3,3] -> (pose fp64 [3,4], info dict).  trace (a list) receives one dict
     per evaluation: the pose it started from, the silhouette and contour sets, X_obj, the pairs, their mean distance
-    and the normal equations of each Gauss-Newton step it took."""
+    and the normal equations of each Gauss-Newton step it took.  render: step 1's renderer, called as
+    `render(verts, faces, K, pose32 [3,4] fp32, h, w, near, far) -> depth [h,w] fp32` (None: `oracle_depth`)."""
+    render = oracle_depth if render is None else render
     mask = np.asarray(mask)
     h, w = mask.shape
     P = np.asarray(pose, np.float64).reshape(3, 4).copy()
@@ -177,7 +220,7 @@ def refine_image(mask, pose, K, verts, faces, near, far, rounds=8, gate=20.0, ma
     cu_all, cv_all = centres(con, w)
     status, pairs, mean0, mean_after, mean_prev, backup = 0, 0, float("nan"), float("nan"), None, P
     for k in range(rounds + 1):
-        depth = ro.render(verts, faces, K, P.astype(np.float32)[None], h, w, near, far)[0][0]
+        depth = np.asarray(render(verts, faces, K, P.astype(np.float32), h, w, near, far), np.float32)
         sil = subsample(boundary(depth > 0), max_points)
         X = back_project(sil, depth, P, K, w)
         j, d2 = nearest_pairs(X, P, K, con, w, gate)
@@ -221,8 +264,9 @@ def refine_image(mask, pose, K, verts, faces, near, far, rounds=8, gate=20.0, ma
     return P, dict(status=status, pairs=pairs, dist_before=mean0, dist_after=mean_after)
 
 
-def refine(mask, poses, K, verts, faces, near, far, rounds=8, gate=20.0, max_points=4096):
-    """mask [b,h,w], poses [b,3,4], K [3,3] or [b,3,3] -> poses fp64 [b,3,4], info dict of [b] arrays."""
+def refine(mask, poses, K, verts, faces, near, far, rounds=8, gate=20.0, max_points=4096, render=None):
+    """mask [b,h,w], poses [b,3,4], K [3,3] or [b,3,3] -> poses fp64 [b,3,4], info dict of [b] arrays.  render: as
+    in `refine_image`."""
     mask = np.asarray(mask)
     poses = np.asarray(poses, np.float64).reshape(-1, 3, 4)
     b = len(poses)
@@ -230,6 +274,7 @@ def refine(mask, poses, K, verts, faces, near, far, rounds=8, gate=20.0, max_poi
     Ks = np.broadcast_to(K, (b, 3, 3)) if K.shape == (3, 3) else K.reshape(b, 3, 3)
     out, infos = np.empty((b, 3, 4)), []
     for i in range(b):
-        out[i], info = refine_image(mask[i], poses[i], Ks[i], verts, faces, near, far, rounds, gate, max_points)
+        out[i], info = refine_image(mask[i], poses[i], Ks[i], verts, faces, near, far, rounds, gate, max_points,
+                                     render=render)
         infos.append(info)
     return out, {key: np.array([d[key] for d in infos]) for key in infos[0]}

@@ -1,5 +1,7 @@
-"""Meshes, cameras and poses for the silhouette-refinement tests (tests/test_refine_cpu.py, tests/test_gpu_refine.py)
-and benchmarks/refine.py.  Lengths are in metres, so the perturbations read as "3 degrees and 1 cm"."""
+"""Meshes, cameras, poses and masks for the silhouette-refinement tests (tests/test_refine_cpu.py,
+tests/test_refine_edges_cpu.py, tests/test_gpu_refine.py, tests/test_gpu_refine_edges.py) and benchmarks/refine.py,
+and `device_depth`, the oracle's render step on the device.  Lengths are in metres, so the perturbations read as
+"3 degrees and 1 cm"."""
 import numpy as np
 
 from oracle import refine_oracle as rfo
@@ -71,3 +73,163 @@ def pose_error(Pa, Pb):
     """-> (rotation error in degrees, translation error in metres)."""
     Pa, Pb = np.asarray(Pa).reshape(3, 4), np.asarray(Pb).reshape(3, 4)
     return rotation_error_deg(Pa[:, :3], Pb[:, :3]), float(np.linalg.norm(Pa[:, 3] - Pb[:, 3]))
+
+
+def comb_mesh(teeth=16, length=0.2, width=0.005, gap=0.01):
+    """A spine with `teeth` thin bars hanging from it, facing +z: at 0.5 m and f = 572 px its silhouette has several
+    thousand border pixels, more than one 4 096-point cap."""
+    parts = [box((0.0, -0.01, 0.0), (teeth * (width + gap), 0.0, 0.01))]
+    for k in range(teeth):
+        x = k * (width + gap)
+        parts.append(box((x, 0.0, 0.0), (x + width, length, 0.01)))
+    verts, faces, off = [], [], 0
+    for v, f in parts:
+        verts.append(v)
+        faces.append(f + off)
+        off += len(v)
+    return np.concatenate(verts), np.concatenate(faces).astype(np.int32)
+
+
+def singular_scene():
+    """Six one-pixel triangles whose silhouette points all lie on the line through the object's origin along the
+    optical axis: mesh (verts, faces), a 40 x 40 K with fx = fy = 1 and (cx, cy) = (0.5, 0.5), the pose [3,4] and
+    the mask (the same six pixels).  Pixel (k, k), k = 1, 2, 4, ..., 32, is covered at depth 4 / k, which
+    back-projects to X_cam = (4, 4, 4 / k) exactly, so R^T (X_cam - t) = (0, 0, 4 / k) with t = (4, 4, 0): every
+    rotation about the optical axis moves no point, the dw_z row and column of the normal equations are exactly
+    zero, and so is A + 1e-3 diag(A)'s diagonal there."""
+    h = w = 40
+    K = np.array([[1, 0, 0.5], [0, 1, 0.5], [0, 0, 1]], np.float32)
+    t = np.array([4.0, 4.0, 0.0])
+    verts, faces = [], []
+    for i, k in enumerate((1, 2, 4, 8, 16, 32)):
+        Z = 4.0 / k
+        for dx, dy in ((-0.3, -0.3), (0.3, -0.3), (0.0, 0.3)):      # a third of a pixel about the centre
+            verts.append(np.array([4.0 + dx * Z, 4.0 + dy * Z, Z]) - t)
+        faces.append([3 * i, 3 * i + 2, 3 * i + 1])
+    pose = np.hstack([np.eye(3), t[:, None]])
+    mask = np.zeros((h, w), bool)
+    for k in (1, 2, 4, 8, 16, 32):
+        mask[k, k] = True
+    return (np.array(verts, np.float32), np.array(faces, np.int32)), K, pose, mask
+
+
+# ---- masks with a chosen contour: the cases PVNet's argmax masks make (speckle, holes) at exact point counts ----
+
+def _dilate4(on, k, outside=False):
+    """Pixels within 4-neighbour distance k of an on pixel, or of the outside when `outside` is True."""
+    out = on.copy()
+    for _ in range(k):
+        p = np.pad(out, 1, constant_values=outside)
+        out = out | p[:-2, 1:-1] | p[2:, 1:-1] | p[1:-1, :-2] | p[1:-1, 2:]
+    return out
+
+
+def hole_sites(on):
+    """Pixels of `on` at least two 4-steps from anything off (the outside included), on a 3-pixel grid: punching one
+    out turns exactly its four neighbours into contour pixels, and no two sites share a neighbour."""
+    h, w = on.shape
+    r, c = np.mgrid[:h, :w]
+    return np.flatnonzero(~_dilate4(~on, 2, outside=True) & (r % 3 == 0) & (c % 3 == 0))
+
+
+def speckle_sites(on, region=None):
+    """Off pixels whose 4-neighbours are all off, on a 2-pixel grid (inside `region` if given): setting one adds
+    exactly one contour pixel, itself, and changes no other pixel's status."""
+    h, w = on.shape
+    r, c = np.mgrid[:h, :w]
+    ok = ~_dilate4(on, 1) & (r % 2 == 0) & (c % 2 == 0)
+    return np.flatnonzero(ok if region is None else ok & region)
+
+
+def with_contour_count(on, n, holes=0, seed=0):
+    """A copy of the mask `on` (bool [h,w]) with `holes` one-pixel holes punched inside it and isolated pixels
+    scattered outside it, so that rfo.boundary finds exactly n points.  Both are drawn with `seed`."""
+    on = np.asarray(on, bool)
+    rng = np.random.default_rng(seed)
+    out = on.copy().reshape(-1)
+    hs = hole_sites(on)
+    assert holes <= len(hs), (holes, len(hs))
+    out[np.sort(rng.choice(hs, holes, replace=False))] = False
+    extra = n - len(rfo.boundary(on)) - 4 * holes
+    ss = speckle_sites(on)
+    assert 0 <= extra <= len(ss), (n, extra, len(ss))
+    out[np.sort(rng.choice(ss, extra, replace=False))] = True
+    out = out.reshape(on.shape)
+    assert len(rfo.boundary(out)) == n
+    return out
+
+
+def round0_d2(sil, depth, pose, K, con, w):
+    """The first round's fp32 d2 [ns, nc] of every silhouette point against every contour pixel (rfo's steps)."""
+    X = rfo.back_project(sil, depth, pose, K, w)
+    u, v = rfo.project(X, pose, K)
+    pu, pv = u.astype(np.float32), v.astype(np.float32)
+    cu, cv = rfo.centres(con, w)
+    dx, dy = cu[None, :] - pu[:, None], cv[None, :] - pv[:, None]
+    return dx * dx + dy * dy
+
+
+def straddling_tie(mask, depth, pose, K, gate=20.0, at=2047, margin=24):
+    """Pad `mask` with isolated pixels in rows above the object, so that some silhouette point's nearest contour
+    pixels are a tie between contour index `at` (the last point of the first 2 048-point tile) and a later index.
+
+    The padding precedes every object contour pixel in row-major order and lies more than `margin` (> gate) rows
+    above the object and its render, so it moves the object's contour indices up without being anyone's pair.
+    -> (padded mask, silhouette index i, lower index, higher index) of the chosen tie, indices in the padded mask."""
+    mask, h, w = np.asarray(mask, bool), *np.asarray(mask).shape
+    assert margin > gate
+    sil = rfo.boundary(depth > 0)
+    con = rfo.boundary(mask)
+    d = round0_d2(sil, depth, pose, K, con, w)
+    best = d.min(1)
+    ties = (d == best[:, None]).sum(1) >= 2
+    a = d.argmin(1)
+    cand = np.flatnonzero(ties & (best <= np.float32(gate) ** 2) & (a <= at))
+    assert len(cand), "no tie to move"
+    i = int(cand[0])
+    lo, hi = np.flatnonzero(d[i] == best[i])[:2]
+    top = min(np.nonzero(mask)[0].min(), np.nonzero(depth > 0)[0].min())
+    rows = np.zeros((h, w), bool)
+    rows[:max(0, top - margin)] = True
+    sites = speckle_sites(mask, rows)
+    pad = at - lo
+    assert pad <= len(sites), (pad, len(sites))
+    out = mask.copy().reshape(-1)
+    out[sites[:pad]] = True
+    out = out.reshape(h, w)
+    assert np.array_equal(rfo.boundary(out)[pad:], con)
+    return out, i, int(lo + pad), int(hi + pad)
+
+
+def spur(on, length=15, half=3):
+    """The mask `on` with a bar 2 half + 1 rows tall and `length` columns long stuck to its right edge at its middle
+    row: a start at the truth then pairs most silhouette points at distance 0 and a few with the bar, and the least
+    squares step towards the bar raises the mean pair distance, so the first round is undone."""
+    out = np.asarray(on, bool).copy()
+    rows, cols = np.nonzero(out)
+    r0 = int(rows.mean())
+    c1 = int(cols[rows == r0].max())
+    out[max(0, r0 - half):r0 + half + 1, c1:c1 + length] = True
+    return out
+
+
+def device_depth(dev="cuda:0"):
+    """Step 1 of oracle/refine_oracle.py on the device: `render=` for rfo.refine_image / rfo.refine that calls
+    `pvnet_b200.render.render_mesh`, which tests/test_gpu_render.py pins bit for bit to render_oracle for the same
+    fp32 pose and K.  The mesh is uploaded once per (verts, faces) pair."""
+    import torch
+
+    from pvnet_b200.render import render_mesh
+    meshes = {}
+
+    def render(verts, faces, K, pose32, h, w, near, far):
+        key = (id(verts), id(faces))
+        if key not in meshes:
+            meshes[key] = (verts, faces, torch.as_tensor(np.ascontiguousarray(verts), device=dev),
+                           torch.as_tensor(np.ascontiguousarray(faces), device=dev))
+        v, f = meshes[key][2:]
+        k = torch.as_tensor(np.asarray(K, np.float32), device=dev)
+        p = torch.as_tensor(np.asarray(pose32, np.float32)[None], device=dev)
+        return render_mesh(v, f, k, p, h, w, near, far)[0].cpu().numpy()
+
+    return render
