@@ -539,6 +539,31 @@ PVNET_API int pvnet_refine_poses(const uint8_t *mask, const double *poses_in, co
                                  double *poses_out, int32_t *info, double *dist, const pvnet_refine_trace_t *trace,
                                  void *workspace, size_t workspace_bytes, pvnet_stream_t stream);
 
+/* pvnet_refine_poses_keypoints: pvnet_refine_poses with the voted keypoints anchoring the pose (DESIGN.md §27).
+ *   Each Gauss-Newton step minimises (1/n) sum_i |pi(R X_i + t) - c_i|^2 + (lambda/nk) sum_k |W_k (pi(R P_k + t) -
+ *   x_k)|^2, n the round's pair count (the pairs held fixed as above, the keypoint term evaluated at the current
+ *   pose), with K read as fp32 by both terms.  Each round is judged by C = mean pair distance + lambda * mean_k
+ *   |W_k e_k| at the pose it reached: a round whose C rose is undone, so the returned C is never above the input's.
+ *   The gates (status 1, 2, 4), the 6-pair minimum, REJECTED and SINGULAR keep their meaning; a step is singular
+ *   only when the combined system is.  Same launches as pvnet_refine_poses, same workspace.
+ *   keypoints  f32 [b,nk,2], pixels as pvnet_uncertainty_pnp reads them, device
+ *   points_3d  f32 [nk,3], the keypoints' model points (the mesh's units), device
+ *   weights_2d f32 [b,nk,3] = (wxx, wxy, wyy) of W_k (pvnet_covariance_to_weights of the covariances), device;
+ *              a keypoint with a non-finite coordinate or weight is left out of both sums
+ *   nk in [4,32]; keypoint_weight (lambda) finite and >= 0
+ *   cost       f64 [b,2] or NULL: C at the input pose and at the returned pose (NaN where dist is)
+ *   keypoint_eq f64 [b,27] or NULL: the first step's keypoint sums, unscaled, in normal_eq's layout (written only
+ *              when that step runs); trace->normal_eq keeps the pair sums alone
+ *   The other arguments are pvnet_refine_poses's. */
+PVNET_API int pvnet_refine_poses_keypoints(const uint8_t *mask, const double *poses_in, const float *K, int k_per_image,
+                                           const float *verts, const int32_t *faces, int nv, int nf, int b, int h,
+                                           int w, float near_clip, float far_clip, int rounds, float gate,
+                                           int max_points, const float *keypoints, const float *points_3d,
+                                           const float *weights_2d, int nk, double keypoint_weight, double *poses_out,
+                                           int32_t *info, double *dist, double *cost,
+                                           const pvnet_refine_trace_t *trace, double *keypoint_eq, void *workspace,
+                                           size_t workspace_bytes, pvnet_stream_t stream);
+
 /* The vanishing-point pair of the reference extension (ransac_voting.cpp:61-99 ->
  * ransac_voting_kernel.cu:170-260, :263-351; used by ransac_voting_vanish_point_layer,
  * ransac_voting_gpu.py:408-501): hypotheses are homogeneous points hypo [hn,vn,3]; the vote sets

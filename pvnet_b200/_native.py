@@ -119,6 +119,11 @@ SIGNATURES = {
     "pvnet_refine_poses": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
                                    c_int, c_float, c_float, c_int, c_float, c_int, c_void_p, c_void_p, c_void_p,
                                    ctypes.POINTER(RefineTrace), c_void_p, c_size_t, c_void_p]),
+    "pvnet_refine_poses_keypoints": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int,
+                                             c_int, c_int, c_int, c_float, c_float, c_int, c_float, c_int, c_void_p,
+                                             c_void_p, c_void_p, c_int, ctypes.c_double, c_void_p, c_void_p, c_void_p,
+                                             c_void_p, ctypes.POINTER(RefineTrace), c_void_p, c_void_p, c_size_t,
+                                             c_void_p]),
     "pvnet_generate_hypothesis":(c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "pvnet_voting_for_hypothesis": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float,
                                             c_void_p]),

@@ -14,6 +14,11 @@
 // k_refine_pairs (a 256-point tile of one image's silhouette per CTA against its whole contour, staged through shared
 // memory) and k_refine_step (one CTA per image: the mean distance, the accept / reject decision and the
 // Gauss-Newton steps, the 6x6 sums reduced in a fixed order).  Nothing is allocated and nothing synchronises.
+//
+// Keypoint anchoring (DESIGN.md §27, pvnet_refine_poses_keypoints): k_refine_step<true> adds the voted keypoints'
+// weighted reprojection term (lambda / nk) sum_k |W_k (pi(R P_k + t) - x_k)|^2 to the pair term, which it then
+// divides by the pair count, and judges each round by mean pair distance + lambda * mean_k |W_k e_k|.  Warp 0 holds
+// one keypoint per lane; the other launches are the same as without keypoints.
 #include "common.cuh"
 
 #include <cmath>
@@ -31,6 +36,8 @@ constexpr double RF_DAMPING = 1e-3;
 constexpr int RF_MIN_PAIRS = 6;
 constexpr int RF_NSUM = 27;                       // 21 entries of the upper triangle of A, then g
 
+constexpr int RF_MAX_KP = 32;                     // keypoints: one lane of warp 0 each
+
 constexpr int RF_NO_CONTOUR = 1, RF_NO_SILHOUETTE = 2, RF_FEW_PAIRS = 4, RF_SINGULAR = 8, RF_REJECTED = 16;
 
 __device__ __forceinline__ double dm(double a, double b) { return __dmul_rn(a, b); }
@@ -47,11 +54,21 @@ __device__ __forceinline__ Cam load_cam(const float *K)
     return {(double)K[0], (double)K[1], (double)K[2], (double)K[4], (double)K[5]};
 }
 
-// Per-image state across rounds (workspace).
+// Per-image state across rounds (workspace).  cost*: the keypoint-anchored round cost (k_refine_step<true> only).
 struct State {
     double backup[12];                            // the pose the current round started from
     double mean0, mean_prev, mean_after;
+    double cost0, cost_prev, cost_after;
     int status, done, pairs, pad;
+};
+
+// The keypoint term's inputs (all device pointers; kp_eq nullable): keypoints f32 [b,nk,2] in pixels, model points
+// f32 [nk,3], weights f32 [b,nk,3] = (wxx, wxy, wyy), lambda = keypoint_weight.
+struct KpArgs {
+    const float *kp, *pts, *wgt;
+    int nk;
+    double lambda;
+    double *kp_eq;                                // trace: the first step's keypoint sums [b,27]
 };
 
 // Projection of X at pose P (row-major [3,4] fp64), the renderer's order: p = R X, Xc = p + t,
@@ -213,16 +230,23 @@ __global__ void __launch_bounds__(RF_PAIR_THREADS)
     }
 }
 
+// Xor butterflies at offsets 16, 8, 4, 2, 1 over the warp: every lane ends with the same sum of each entry.
+template <int N>
+__device__ __forceinline__ void warp_xor_sum(double (&v)[N])
+{
+#pragma unroll
+    for (int k = 0; k < N; ++k)
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) v[k] += __shfl_xor_sync(0xffffffffu, v[k], o);
+}
+
 // Block sum of n doubles per thread into out (thread 0's view): xor butterflies within each warp, then the warps'
 // partials in warp order.  The same inputs give the same sum every run.
 template <int N>
 __device__ __forceinline__ void block_sum(double (&v)[N], double (*s_part)[N], double *out)
 {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-    for (int k = 0; k < N; ++k)
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) v[k] += __shfl_xor_sync(0xffffffffu, v[k], o);
+    warp_xor_sum(v);
     if (lane == 0)
 #pragma unroll
         for (int k = 0; k < N; ++k) s_part[warp][k] = v[k];
@@ -298,15 +322,87 @@ __device__ bool damped_solve(const double *sum, double (&x)[6])
     return true;
 }
 
+// Keypoint term, warp 0: lane l < nk holds keypoint l as (x, y, X, Y, Z, wxx, wxy, wyy) in fp64.  A keypoint with a
+// non-finite coordinate or weight is left out (it adds zero to every sum).
+__device__ __forceinline__ bool load_keypoint(const KpArgs &a, int img, int lane, double (&q)[8])
+{
+    if (lane >= a.nk) return false;
+    const size_t e = static_cast<size_t>(img) * a.nk + lane;
+    q[0] = a.kp[e * 2];
+    q[1] = a.kp[e * 2 + 1];
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+        q[2 + r] = a.pts[lane * 3 + r];
+        q[5 + r] = a.wgt[e * 3 + r];
+    }
+    bool ok = true;
+#pragma unroll
+    for (int r = 0; r < 8; ++r) ok = ok && isfinite(q[r]);
+    return ok;
+}
+
+// |W (pi(R P + t) - x)| of one keypoint, each operation rounded (oracle/refine_keypoints_oracle.py restates it bit
+// for bit): the projection is `project`'s, e = (u - x, v - y), r = (wxx eu + wxy ev, wxy eu + wyy ev),
+// sqrt(r0 r0 + r1 r1).
+__device__ __forceinline__ double keypoint_distance(const double *P, const Cam &c, const double *q)
+{
+    double u, v;
+    project(P, c, q[2], q[3], q[4], u, v);
+    const double eu = ds(u, q[0]), ev = ds(v, q[1]);
+    const double r0 = da(dm(q[5], eu), dm(q[6], ev)), r1 = da(dm(q[6], eu), dm(q[7], ev));
+    return __dsqrt_rn(da(dm(r0, r0), dm(r1, r1)));
+}
+
+// One keypoint's 27 sums of the weighted residual r = W e at pose P: J_w = W [Ju; Jv] with the pairs' Jacobian,
+// the 21 upper-triangle entries of J_w^T J_w row by row, then J_w^T r.
+__device__ __forceinline__ void keypoint_sums(const double *P, const Cam &cam, const double *q, double (&v)[RF_NSUM])
+{
+    double p[3], Xc[3];
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+        p[r] = P[r * 4] * q[2] + P[r * 4 + 1] * q[3] + P[r * 4 + 2] * q[4];
+        Xc[r] = p[r] + P[r * 4 + 3];
+    }
+    const double iz = 1.0 / Xc[2];
+    const double u = (cam.fx * Xc[0] + cam.s * Xc[1] + cam.cx * Xc[2]) * iz;
+    const double vv = (cam.fy * Xc[1] + cam.cy * Xc[2]) * iz;
+    const double eu = u - q[0], ev = vv - q[1];
+    const double du[3] = {cam.fx * iz, cam.s * iz, -(u - cam.cx) * iz};
+    const double dv[3] = {0.0, cam.fy * iz, -(vv - cam.cy) * iz};
+    const double Ju[6] = {p[1] * du[2] - p[2] * du[1], p[2] * du[0] - p[0] * du[2], p[0] * du[1] - p[1] * du[0],
+                          du[0], du[1], du[2]};
+    const double Jv[6] = {p[1] * dv[2] - p[2] * dv[1], p[2] * dv[0] - p[0] * dv[2], p[0] * dv[1] - p[1] * dv[0],
+                          dv[0], dv[1], dv[2]};
+    double J0[6], J1[6];
+#pragma unroll
+    for (int r = 0; r < 6; ++r) {
+        J0[r] = q[5] * Ju[r] + q[6] * Jv[r];
+        J1[r] = q[6] * Ju[r] + q[7] * Jv[r];
+    }
+    const double r0 = q[5] * eu + q[6] * ev, r1 = q[6] * eu + q[7] * ev;
+    int k = 0;
+#pragma unroll
+    for (int r = 0; r < 6; ++r)
+#pragma unroll
+        for (int c = r; c < 6; ++c) v[k++] = J0[r] * J0[c] + J1[r] * J1[c];
+#pragma unroll
+    for (int r = 0; r < 6; ++r) v[21 + r] = J0[r] * r0 + J1[r] * r1;
+}
+
 // One CTA per image: evaluation k of the pose (mean pair distance, accept or undo), then, unless k is the last
 // evaluation, RF_GN_STEPS Gauss-Newton steps on the pairs.  The pose lives in `pose` (the caller's output); pose32
 // is its fp32 copy for the next render.  normal_eq (nullable): the sums of the first step of evaluation 0.
+// KP: the keypoint-anchored form.  Each step's pair sums (after block_sum) become, entry by entry and each
+// operation rounded, pair / n + (lambda / nk) * kp, kp the keypoints' sums combined by warp 0's xor butterflies;
+// the round's cost is C = m + lambda * (kd / nk), m the mean pair distance and kd the butterfly sum of the keypoint
+// distances at the evaluated pose, and a round whose C rose is undone.
+template <bool KP>
 __global__ void __launch_bounds__(RF_STEP_THREADS)
     k_refine_step(double *__restrict__ pose, float *__restrict__ pose32, const float *__restrict__ K, int kstride,
                   int w, int max_points, int k, int last, State *__restrict__ state,
                   const int32_t *__restrict__ counts, const double *__restrict__ sil_obj,
                   const int32_t *__restrict__ con_idx, const int32_t *__restrict__ pair,
-                  const float *__restrict__ pair_d2, double *__restrict__ normal_eq)
+                  const float *__restrict__ pair_d2, double *__restrict__ normal_eq, KpArgs kpa)
 {
     const int img = blockIdx.x;
     State &S = state[img];
@@ -315,6 +411,8 @@ __global__ void __launch_bounds__(RF_STEP_THREADS)
     __shared__ double s_sum[RF_NSUM];
     __shared__ double s_pose[12];
     __shared__ int s_go;
+    __shared__ double s_kp[KP ? RF_MAX_KP : 1][8];
+    __shared__ int s_kp_on[KP ? RF_MAX_KP : 1];
     const int ns = counts[img * 2], nc = counts[img * 2 + 1];
     const size_t o = static_cast<size_t>(img) * max_points;
     double acc[2] = {0.0, 0.0};
@@ -323,10 +421,29 @@ __global__ void __launch_bounds__(RF_STEP_THREADS)
             acc[0] += 1.0;
             acc[1] += sqrt(static_cast<double>(pair_d2[o + i]));
         }
-    block_sum<2>(acc, reinterpret_cast<double (*)[2]>(&s_part[0][0]), s_sum);
+    if constexpr (KP) {
+        if (threadIdx.x < 12) s_pose[threadIdx.x] = pose[img * 12 + threadIdx.x];
+        if (threadIdx.x < RF_MAX_KP) {
+            double q[8];
+            const bool on = load_keypoint(kpa, img, threadIdx.x, q);
+#pragma unroll
+            for (int r = 0; r < 8; ++r) s_kp[threadIdx.x][r] = on ? q[r] : 0.0;
+            s_kp_on[threadIdx.x] = on;
+        }
+    }
+    block_sum<2>(acc, reinterpret_cast<double (*)[2]>(&s_part[0][0]), s_sum);   // its barriers publish s_pose, s_kp
+    double kd[1] = {0.0};
+    if constexpr (KP) {
+        if (threadIdx.x < 32) {
+            if (s_kp_on[threadIdx.x])
+                kd[0] = keypoint_distance(s_pose, load_cam(K + static_cast<size_t>(img) * kstride), s_kp[threadIdx.x]);
+            warp_xor_sum(kd);
+        }
+    }
     if (threadIdx.x == 0) {
         const int n = static_cast<int>(s_sum[0]);
         const double m = n ? s_sum[1] / n : NAN;
+        const double cost = KP ? da(m, dm(kpa.lambda, dd(kd[0], static_cast<double>(kpa.nk)))) : m;
         bool go = true;
         if (k == 0) {
             int st = 0;
@@ -338,17 +455,20 @@ __global__ void __launch_bounds__(RF_STEP_THREADS)
                 go = false;
             } else {
                 S.mean0 = S.mean_after = m;
+                if (KP) S.cost0 = S.cost_after = cost;
             }
-        } else if (ns == 0 || n < RF_MIN_PAIRS || m > S.mean_prev) {
+        } else if (ns == 0 || n < RF_MIN_PAIRS || (KP ? cost > S.cost_prev : m > S.mean_prev)) {
             S.status |= RF_REJECTED;
             for (int q = 0; q < 12; ++q) pose[img * 12 + q] = S.backup[q];
             go = false;
         } else {
             S.mean_after = m;
+            if (KP) S.cost_after = cost;
         }
         if (!go) S.done = 1;
         if (go && !last) {
             S.mean_prev = m;
+            if (KP) S.cost_prev = cost;
             for (int q = 0; q < 12; ++q) S.backup[q] = pose[img * 12 + q];
             S.pairs = n;
         }
@@ -393,9 +513,26 @@ __global__ void __launch_bounds__(RF_STEP_THREADS)
             for (int r = 0; r < 6; ++r) v[21 + r] += Ju[r] * ru + Jv[r] * rv;
         }
         block_sum<RF_NSUM>(v, s_part, s_sum);
+        if constexpr (KP) {
+            if (threadIdx.x < 32) {                   // v is free again: warp 0 reuses it for the keypoint sums
+                if (s_kp_on[threadIdx.x]) {
+                    keypoint_sums(s_pose, cam, s_kp[threadIdx.x], v);
+                } else {
+#pragma unroll
+                    for (int q = 0; q < RF_NSUM; ++q) v[q] = 0.0;
+                }
+                warp_xor_sum(v);
+            }
+        }
         if (threadIdx.x == 0) {
             if (normal_eq && k == 0 && step == 0)
                 for (int q = 0; q < RF_NSUM; ++q) normal_eq[img * RF_NSUM + q] = s_sum[q];
+            if constexpr (KP) {
+                if (kpa.kp_eq && k == 0 && step == 0)
+                    for (int q = 0; q < RF_NSUM; ++q) kpa.kp_eq[img * RF_NSUM + q] = v[q];
+                const double n = static_cast<double>(S.pairs), lk = dd(kpa.lambda, static_cast<double>(kpa.nk));
+                for (int q = 0; q < RF_NSUM; ++q) s_sum[q] = da(dd(s_sum[q], n), dm(lk, v[q]));
+            }
             double x[6];
             if (!damped_solve(s_sum, x)) {
                 S.status |= RF_SINGULAR;
@@ -434,11 +571,12 @@ __global__ void k_refine_init(const double *__restrict__ pose_in, double *__rest
     }
     State &S = state[i];
     S.mean0 = S.mean_prev = S.mean_after = NAN;
+    S.cost0 = S.cost_prev = S.cost_after = NAN;
     S.status = S.done = S.pairs = S.pad = 0;
 }
 
 __global__ void k_refine_finish(const State *__restrict__ state, int b, int32_t *__restrict__ info,
-                                double *__restrict__ dist)
+                                double *__restrict__ dist, double *__restrict__ cost)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= b) return;
@@ -449,6 +587,10 @@ __global__ void k_refine_finish(const State *__restrict__ state, int b, int32_t 
     if (dist) {
         dist[i * 2] = state[i].mean0;
         dist[i * 2 + 1] = state[i].mean_after;
+    }
+    if (cost) {
+        cost[i * 2] = state[i].cost0;
+        cost[i * 2 + 1] = state[i].cost_after;
     }
 }
 
@@ -493,11 +635,16 @@ int pvnet_refine_workspace_bytes(int b, int h, int w, int max_points, size_t *by
     return PVNET_OK;
 }
 
-int pvnet_refine_poses(const uint8_t *mask, const double *poses_in, const float *K, int k_per_image,
-                       const float *verts, const int32_t *faces, int nv, int nf, int b, int h, int w, float near_clip,
-                       float far_clip, int rounds, float gate, int max_points, double *poses_out, int32_t *info,
-                       double *dist, const pvnet_refine_trace_t *trace, void *workspace, size_t workspace_bytes,
-                       pvnet_stream_t stream)
+}  // extern "C"
+
+namespace {
+
+// Both entry points: kpa null runs k_refine_step<false>, the silhouette objective alone.
+int refine_poses(const uint8_t *mask, const double *poses_in, const float *K, int k_per_image, const float *verts,
+                 const int32_t *faces, int nv, int nf, int b, int h, int w, float near_clip, float far_clip, int rounds,
+                 float gate, int max_points, const KpArgs *kpa, double *poses_out, int32_t *info, double *dist,
+                 double *cost, const pvnet_refine_trace_t *trace, void *workspace, size_t workspace_bytes,
+                 pvnet_stream_t stream)
 {
     PV_CHECK_ARG(b >= 1 && h >= 1 && w >= 1 && nv >= 0 && nf >= 0, "bad dimension (b=%d, h=%d, w=%d, nv=%d, nf=%d)",
                  b, h, w, nv, nf);
@@ -540,16 +687,55 @@ int pvnet_refine_poses(const uint8_t *mask, const double *poses_in, const float 
                 PV_CUDA(cudaMemcpyAsync(trace->sil_obj, L.obj, np * 24, cudaMemcpyDeviceToDevice, st));
             if (trace->pair_idx) PV_CUDA(cudaMemcpyAsync(trace->pair_idx, L.pair, np * 4, cudaMemcpyDeviceToDevice, st));
         }
-        k_refine_step<<<b, RF_STEP_THREADS, 0, st>>>(poses_out, L.pose32, K, kstride, w, max_points, k, k == rounds,
-                                                     L.state, L.counts, L.obj, L.con, L.pair, L.d2,
-                                                     trace ? trace->normal_eq : nullptr);
+        double *ne = trace ? trace->normal_eq : nullptr;
+        if (kpa)
+            k_refine_step<true><<<b, RF_STEP_THREADS, 0, st>>>(poses_out, L.pose32, K, kstride, w, max_points, k,
+                                                               k == rounds, L.state, L.counts, L.obj, L.con, L.pair,
+                                                               L.d2, ne, *kpa);
+        else
+            k_refine_step<false><<<b, RF_STEP_THREADS, 0, st>>>(poses_out, L.pose32, K, kstride, w, max_points, k,
+                                                                k == rounds, L.state, L.counts, L.obj, L.con, L.pair,
+                                                                L.d2, ne, KpArgs{});
         PV_LAUNCHED("k_refine_step");
     }
-    if (info || dist) {
-        k_refine_finish<<<(b + 127) / 128, 128, 0, st>>>(L.state, b, info, dist);
+    if (info || dist || cost) {
+        k_refine_finish<<<(b + 127) / 128, 128, 0, st>>>(L.state, b, info, dist, cost);
         PV_LAUNCHED("k_refine_finish");
     }
     return PVNET_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int pvnet_refine_poses(const uint8_t *mask, const double *poses_in, const float *K, int k_per_image,
+                       const float *verts, const int32_t *faces, int nv, int nf, int b, int h, int w, float near_clip,
+                       float far_clip, int rounds, float gate, int max_points, double *poses_out, int32_t *info,
+                       double *dist, const pvnet_refine_trace_t *trace, void *workspace, size_t workspace_bytes,
+                       pvnet_stream_t stream)
+{
+    return refine_poses(mask, poses_in, K, k_per_image, verts, faces, nv, nf, b, h, w, near_clip, far_clip, rounds,
+                        gate, max_points, nullptr, poses_out, info, dist, nullptr, trace, workspace, workspace_bytes,
+                        stream);
+}
+
+int pvnet_refine_poses_keypoints(const uint8_t *mask, const double *poses_in, const float *K, int k_per_image,
+                                 const float *verts, const int32_t *faces, int nv, int nf, int b, int h, int w,
+                                 float near_clip, float far_clip, int rounds, float gate, int max_points,
+                                 const float *keypoints, const float *points_3d, const float *weights_2d, int nk,
+                                 double keypoint_weight, double *poses_out, int32_t *info, double *dist, double *cost,
+                                 const pvnet_refine_trace_t *trace, double *keypoint_eq, void *workspace,
+                                 size_t workspace_bytes, pvnet_stream_t stream)
+{
+    PV_CHECK_ARG(keypoints && points_3d && weights_2d, "null pointer");
+    PV_CHECK_ARG(nk >= 4 && nk <= RF_MAX_KP, "keypoint count %d outside [4,%d] (one lane per keypoint)", nk,
+                 RF_MAX_KP);
+    PV_CHECK_ARG(keypoint_weight >= 0.0 && keypoint_weight < INFINITY, "keypoint_weight must be finite and >= 0 "
+                 "(got %g)", keypoint_weight);
+    const KpArgs kpa{keypoints, points_3d, weights_2d, nk, keypoint_weight, keypoint_eq};
+    return refine_poses(mask, poses_in, K, k_per_image, verts, faces, nv, nf, b, h, w, near_clip, far_clip, rounds,
+                        gate, max_points, &kpa, poses_out, info, dist, cost, trace, workspace, workspace_bytes, stream);
 }
 
 }  // extern "C"

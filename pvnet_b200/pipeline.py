@@ -24,6 +24,11 @@ CUDA graph per input buffer on first use and replayed afterwards -- 4 us of host
 0.4-5 ms of Python + launches (batch 1: 0.72 ms per image instead of 0.78; at batch 16 the GPU is the limit either
 way, the host thread is what is freed).  The device-side sampler keeps drawing fresh samples across replays.
 
+`refine=dict(vertices=, faces=, near=, far=, ...)`: the poses are then refined on the device before they are returned
+(`refine.refine_poses` with the step's own fused-argmax mask, PnP poses, keypoints and covariances and its cameras,
+the keypoint-anchored objective of DESIGN.md §27), inside the same captured graph when graph=True.  The mesh goes to
+the device once.
+
 Inputs may be float32 [b,3,H,W] (already normalised, what `ToTensor` + `Normalize` produce,
 tools/demo.py:89-95) or uint8 [b,H,W,3] raw images: the latter are normalised on the device inside
 the packing kernel (4x fewer host->device bytes).
@@ -34,6 +39,7 @@ import torch
 
 from . import extend_utils as eu
 from . import ransac_voting_gpu as rv
+from . import refine as rfn
 
 IMAGENET_MEAN = (0.485, 0.456, 0.406)      # tools/demo.py:91-94, lib/datasets/linemod_dataset.py:191-195
 IMAGENET_STD = (0.229, 0.224, 0.225)
@@ -42,7 +48,7 @@ IMAGENET_STD = (0.229, 0.224, 0.225)
 class PoseKeypointPipeline:
     def __init__(self, net, round_hyp_num=256, inlier_thresh=0.99, rng="device", with_covariance=False,
                  cov_round_hyp_num=256, cov_min_hyp_num=4096, max_num=30000, mean=IMAGENET_MEAN, std=IMAGENET_STD,
-                 points_3d=None, camera_matrix=None, graph=False):
+                 points_3d=None, camera_matrix=None, graph=False, refine=None):
         self.net = net
         self.graph = bool(graph)
         self.hn = round_hyp_num
@@ -59,6 +65,18 @@ class PoseKeypointPipeline:
         if self.graph and rng != "device":
             raise ValueError("graph=True needs rng='device' (torch's generator cannot be replayed)")
         self.points_3d, self.camera_matrix = points_3d, camera_matrix
+        self.refine = None
+        if refine is not None:
+            if points_3d is None or not with_covariance:
+                raise ValueError("refine needs points_3d and with_covariance=True")
+            cfg = dict(rounds=8, gate=20.0, max_points=4096, keypoint_weight=rfn.DEFAULT_KEYPOINT_WEIGHT)
+            unknown = set(refine) - {"vertices", "faces", "near", "far", *cfg}
+            missing = {"vertices", "faces", "near", "far"} - set(refine)
+            if unknown or missing:
+                raise ValueError(f"refine: unknown keys {sorted(unknown)}, missing keys {sorted(missing)}")
+            cfg.update(refine)
+            self.refine = cfg
+        self._mesh_dev = None                       # (device, vertices, faces, constructor K or None)
         self._p3_dev = None
         self._bufs = None
         self._kbufs = None
@@ -130,8 +148,34 @@ class PoseKeypointPipeline:
                 self._p3_dev = torch.as_tensor(self.points_3d, dtype=torch.float32).to(x.device).contiguous()
             K = self.camera_matrix if camera_matrix is None else camera_matrix
             pose = eu.uncertainty_pnp_batched(res[0], self._p3_dev, K, cov=res[1])
+            if self.refine is not None:
+                pose = self._refine(mask, pose, K, res[0], res[1])
             return res[0], res[1], pose
         return res
+
+    def _refine(self, mask, pose, K, kp, cov):
+        """refine_poses on the step's outputs; the mesh (and a host camera) go to the device on first use."""
+        dev = pose.device
+        cfg = self.refine
+        if self._mesh_dev is None or self._mesh_dev[0] != dev:
+            v = torch.as_tensor(cfg["vertices"], dtype=torch.float32).to(dev).contiguous()
+            f = torch.as_tensor(cfg["faces"]).to(dev)
+            f = f if f.dtype == torch.int32 else f.to(torch.int32)
+            k = None                                # the constructor's host camera, if any
+            if self.camera_matrix is not None and not (isinstance(self.camera_matrix, torch.Tensor)
+                                                       and self.camera_matrix.is_cuda):
+                k = torch.as_tensor(self.camera_matrix, dtype=torch.float64).reshape(3, 3).to(dev)
+            self._mesh_dev = (dev, v, f.contiguous(), k)
+        _, v, f, k_host = self._mesh_dev
+        if isinstance(K, torch.Tensor) and K.is_cuda:
+            k = K
+        elif K is self.camera_matrix and k_host is not None:
+            k = k_host
+        else:
+            k = torch.as_tensor(K, dtype=torch.float64).reshape(3, 3).to(dev)
+        return rfn.refine_poses(mask, pose, k, v, f, cfg["near"], cfg["far"], rounds=cfg["rounds"], gate=cfg["gate"],
+                                max_points=cfg["max_points"], keypoints=kp, points_3d=self._p3_dev, cov=cov,
+                                keypoint_weight=cfg["keypoint_weight"])
 
     @torch.no_grad()
     def run(self, host_batches, out_host=None, cov_host=None, on_result=None, pose_host=None, camera_matrices=None):

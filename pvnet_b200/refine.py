@@ -5,7 +5,12 @@ four-step docstring -- find the mask's edge, render the silhouette and back-proj
 optimise -- and a `pass` body; the `extend_utils` shim keeps returning None for that name.  `refine_poses` is the
 device form: each round renders the mesh at the current pose with `render_mesh`'s renderer, pairs its silhouette
 with the mask's contour and takes damped Gauss-Newton steps on the pairs' pixel distances.  oracle/refine_oracle.py
-restates it.  No CPU path: without the library or a CUDA device it raises."""
+restates it.  No CPU path: without the library or a CUDA device it raises.
+
+With `keypoints` (the voted keypoints, their model points and covariances or weights, as `uncertainty_pnp_batched`
+takes them) each step also pulls the keypoints' weighted reprojections towards the votes
+(`pvnet_refine_poses_keypoints`, DESIGN.md §27): the rotations an outline barely constrains are held by the
+keypoints."""
 from __future__ import annotations
 
 import ctypes
@@ -14,7 +19,7 @@ import math
 import torch
 
 from . import _native
-from .extend_utils import check_cameras
+from .extend_utils import check_cameras, covariance_to_weights
 
 # status bits of info["status"]
 NO_CONTOUR = 1          # the mask has no foreground: the input pose is returned
@@ -22,6 +27,10 @@ NO_SILHOUETTE = 2       # the render at the input pose covers nothing: the input
 FEW_PAIRS = 4           # fewer than 6 pairs at the input pose: the input pose is returned
 SINGULAR = 8            # a round's normal equations were singular: that round's starting pose is kept
 REJECTED = 16           # a round raised the mean pair distance (or lost its pairs) and was undone
+
+# lambda of the keypoint-anchored objective: the best of 0.25, 1 and 4 on the synthetic scenes of
+# benchmarks/refine_keypoints.py (DESIGN.md §27); real-data accuracy has not been measured
+DEFAULT_KEYPOINT_WEIGHT = 0.25
 
 
 def _cuda_tensor(name, t):
@@ -31,8 +40,43 @@ def _cuda_tensor(name, t):
         raise RuntimeError(f"pvnet_b200: `{name}` must be a CUDA tensor (there is no CPU path)")
 
 
+def _keypoint_inputs(b, dev, keypoints, points_3d, cov, weights_2d, keypoint_weight):
+    """Check the keypoint arguments -> (keypoints f32 [b,nk,2], points f32 [nk,3], weights f32 [b,nk,3], nk,
+    lambda), all contiguous on `dev`."""
+    if points_3d is None:
+        raise ValueError("keypoints need points_3d")
+    if (cov is None) == (weights_2d is None):
+        raise ValueError("pass exactly one of weights_2d / cov with keypoints")
+    for name, t in (("keypoints", keypoints), ("points_3d", points_3d), ("cov", cov), ("weights_2d", weights_2d)):
+        if t is None:
+            continue
+        if not isinstance(t, torch.Tensor):
+            raise ValueError(f"{name} must be a torch tensor, got {type(t).__name__}")
+        if t.device != dev:
+            raise ValueError(f"{name} must be on the poses' device {dev}, got {t.device}")
+        if not t.dtype.is_floating_point:
+            raise ValueError(f"{name} must be floating point, got {t.dtype}")
+    if keypoints.dim() != 3 or int(keypoints.shape[0]) != b or keypoints.shape[2] != 2:
+        raise ValueError(f"keypoints must be [{b},nk,2], got {tuple(keypoints.shape)}")
+    nk = int(keypoints.shape[1])
+    if not 4 <= nk <= 32:
+        raise ValueError(f"keypoint count must lie in 4..32, got {nk}")
+    if tuple(points_3d.shape) != (nk, 3):
+        raise ValueError(f"points_3d must be [{nk},3], got {tuple(points_3d.shape)}")
+    if cov is not None and tuple(cov.shape) != (b, nk, 2, 2):
+        raise ValueError(f"cov must be [{b},{nk},2,2], got {tuple(cov.shape)}")
+    if weights_2d is not None and tuple(weights_2d.shape) != (b, nk, 3):
+        raise ValueError(f"weights_2d must be [{b},{nk},3], got {tuple(weights_2d.shape)}")
+    lam = float(keypoint_weight)
+    if not 0.0 <= lam < math.inf:
+        raise ValueError(f"keypoint_weight must be finite and >= 0, got {keypoint_weight}")
+    wgt = covariance_to_weights(cov) if cov is not None else weights_2d.contiguous().float()
+    return keypoints.contiguous().float(), points_3d.contiguous().float(), wgt.contiguous(), nk, lam
+
+
 def refine_poses(mask, poses, K, vertices, faces, near, far, rounds=8, gate=20.0, max_points=4096,
-                 return_info=False, trace=False):
+                 return_info=False, trace=False, keypoints=None, points_3d=None, cov=None, weights_2d=None,
+                 keypoint_weight=DEFAULT_KEYPOINT_WEIGHT):
     """Refine b poses of one mesh so its rendered silhouette meets each mask's contour.
 
     mask [b,H,W] (any integer dtype or bool; nonzero is foreground), poses [b,3,4] (float32 or float64, R | t object
@@ -47,7 +91,15 @@ def refine_poses(mask, poses, K, vertices, faces, near, far, rounds=8, gate=20.0
     "dist_after" (float64, the mean pair distance in pixels at the input pose and at the returned one, NaN without
     pairs).  trace: also a dict of the first round's intermediates ("sil_idx", "con_idx", "pair_idx" int32
     [b,max_points], "counts" int32 [b,2], "sil_obj" float64 [b,max_points,3], "normal_eq" float64 [b,27]), for
-    checking the stages against the oracle."""
+    checking the stages against the oracle.
+
+    keypoints [b,nk,2] (4 <= nk <= 32, pixels as `uncertainty_pnp_batched` reads them), points_3d [nk,3] (their
+    model points, in the mesh's units) and exactly one of cov [b,nk,2,2] / weights_2d [b,nk,3] (converted through
+    `covariance_to_weights`), floating-point CUDA tensors on the poses' device: each step then minimises
+    (1/n) sum |pi(R X_i + t) - c_i|^2 + (keypoint_weight / nk) sum |W_k (pi(R P_k + t) - x_k)|^2, and a round is
+    undone when C = mean pair distance + keypoint_weight * mean_k |W_k e_k| rose (DESIGN.md §27).  return_info then
+    adds "cost_before" and "cost_after" (float64, C at the input pose and at the returned one), and trace adds
+    "keypoint_eq" (float64 [b,27], the first step's keypoint sums, unscaled)."""
     for name, t in (("mask", mask), ("poses", poses), ("K", K), ("vertices", vertices), ("faces", faces)):
         _cuda_tensor(name, t)
     dev = poses.device
@@ -85,6 +137,12 @@ def refine_poses(mask, poses, K, vertices, faces, near, far, rounds=8, gate=20.0
     if not 1 <= max_points <= (2 ** 31 - 1) // 3 // b:
         raise ValueError(f"max_points must lie in 1..{(2 ** 31 - 1) // 3 // b} for b = {b}, got {max_points}")
 
+    kpt = None
+    if keypoints is not None:
+        kpt = _keypoint_inputs(b, dev, keypoints, points_3d, cov, weights_2d, keypoint_weight)
+    elif points_3d is not None or cov is not None or weights_2d is not None:
+        raise ValueError("points_3d, cov and weights_2d go with keypoints")
+
     nv, nf = int(vertices.shape[0]), int(faces.shape[0])
     m = mask.view(torch.uint8) if mask.dtype in (torch.uint8, torch.bool) else (mask != 0).to(torch.uint8)
     m = m.contiguous()
@@ -96,6 +154,7 @@ def refine_poses(mask, poses, K, vertices, faces, near, far, rounds=8, gate=20.0
     out = torch.empty((b, 3, 4), dtype=torch.float64, device=dev)
     info = torch.empty((b, 2), dtype=torch.int32, device=dev) if return_info else None
     dist = torch.empty((b, 2), dtype=torch.float64, device=dev) if return_info else None
+    cost = torch.empty((b, 2), dtype=torch.float64, device=dev) if return_info and kpt is not None else None
     tr, tr_struct = None, None
     if trace:
         tr = dict(sil_idx=torch.full((b, max_points), -1, dtype=torch.int32, device=dev),
@@ -106,21 +165,34 @@ def refine_poses(mask, poses, K, vertices, faces, near, far, rounds=8, gate=20.0
                   normal_eq=torch.full((b, 27), math.nan, dtype=torch.float64, device=dev))
         tr_struct = _native.RefineTrace(*(tr[n].data_ptr() for n in ("sil_idx", "con_idx", "counts", "sil_obj",
                                                                       "pair_idx", "normal_eq")))
+        if kpt is not None:
+            tr["keypoint_eq"] = torch.full((b, 27), math.nan, dtype=torch.float64, device=dev)
     L = _native.lib()
     with torch.cuda.device(dev):
         need = ctypes.c_size_t()
         _native.check(L.pvnet_refine_workspace_bytes(b, h, w, max_points, ctypes.byref(need)),
                       "pvnet_refine_workspace_bytes")
         ws = torch.empty(need.value, dtype=torch.uint8, device=dev)
-        _native.check(L.pvnet_refine_poses(
-            m.data_ptr(), p.data_ptr(), k.data_ptr(), int(k.dim() == 3), v.data_ptr() if nv else None,
-            f.data_ptr() if nf else None, nv, nf, b, h, w, near, far, rounds, gate, max_points, out.data_ptr(),
-            None if info is None else info.data_ptr(), None if dist is None else dist.data_ptr(),
-            None if tr_struct is None else ctypes.byref(tr_struct), ws.data_ptr(), need.value,
-            ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "pvnet_refine_poses")
+        head = (m.data_ptr(), p.data_ptr(), k.data_ptr(), int(k.dim() == 3), v.data_ptr() if nv else None,
+                f.data_ptr() if nf else None, nv, nf, b, h, w, near, far, rounds, gate, max_points)
+        outs = (out.data_ptr(), None if info is None else info.data_ptr(), None if dist is None else dist.data_ptr())
+        trace_p = None if tr_struct is None else ctypes.byref(tr_struct)
+        stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+        if kpt is None:
+            _native.check(L.pvnet_refine_poses(*head, *outs, trace_p, ws.data_ptr(), need.value, stream),
+                          "pvnet_refine_poses")
+        else:
+            kp, pts, wgt, nk, lam = kpt
+            _native.check(L.pvnet_refine_poses_keypoints(
+                *head, kp.data_ptr(), pts.data_ptr(), wgt.data_ptr(), nk, lam, *outs,
+                None if cost is None else cost.data_ptr(), trace_p,
+                None if tr is None else tr["keypoint_eq"].data_ptr(), ws.data_ptr(), need.value, stream),
+                "pvnet_refine_poses_keypoints")
     res = (out,)
     if return_info:
         res += (dict(status=info[:, 0], pairs=info[:, 1], dist_before=dist[:, 0], dist_after=dist[:, 1]),)
+        if cost is not None:
+            res[-1].update(cost_before=cost[:, 0], cost_after=cost[:, 1])
     if trace:
         res += (tr,)
     return res[0] if len(res) == 1 else res
