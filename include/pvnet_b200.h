@@ -564,6 +564,49 @@ PVNET_API int pvnet_refine_poses_keypoints(const uint8_t *mask, const double *po
                                            const pvnet_refine_trace_t *trace, double *keypoint_eq, void *workspace,
                                            size_t workspace_bytes, pvnet_stream_t stream);
 
+/* pvnet_refine_poses_depth: depth-anchored pose refinement of one mesh at b poses, point-to-plane ICP against the
+ *   registered depth image (DESIGN.md §28).  Per image and round: the depth Zr at the current pose from
+ *   pvnet_render_mesh (the pose rounded to fp32); the pairs: every pixel (r,c) that the render covers, the mask holds
+ *   and the sensor read, whose four 4-neighbours are inside the image, in the mask and read, with ray (xn, yn, 1) at
+ *   (u,v) = (c + 0.5, r + 0.5) through K as pvnet_render_mesh reads it; model point X = R^T (Zr (xn,yn,1) - t) (fixed
+ *   for the round), observed point Y = Zo (xn,yn,1), observed normal n = (Y[c+1] - Y[c-1]) x (Y[r+1] - Y[r-1])
+ *   normalised and turned so that n . Y < 0; a pair is dropped when |R X + t - Y| > gate or its residual is not a
+ *   number.  Row-major; above max_points only every ceil(n / max_points)-th pair is kept.  Then, the pairs held
+ *   fixed, three damped Gauss-Newton steps on sum (n . (R X + t - Y))^2 with R <- exp(dw) R, t <- t + dt.  Each round
+ *   is checked by the next render: a round that raises the mean |n . (R X + t - Y)|, or leaves fewer than 6 pairs, is
+ *   undone and the image stops.  So rounds + 1 renders; rounds = 0 returns the input.
+ *   depth      f32 [b,h,w] in the poses' units, or uint16 [b,h,w] when depth_is_u16 != 0, read as
+ *              fp32(d) * depth_scale (one rounded fp32 multiply; depth_scale finite and > 0), device; a value <= 0 or
+ *              not finite is no reading
+ *   gate > 0, finite, in the poses' units; max_points >= 1 with b * max_points <= INT32_MAX / 9
+ *   info       int32 [b,2] or NULL: (status bits, pairs of the last round that took its steps); status 1: the mask
+ *              has no foreground, 2: the render at the input pose covers nothing, 4: fewer than 6 pairs at the input
+ *              pose (each of these returns the input pose), 8: a singular system, 16: a round was undone
+ *   dist       f64 [b,2] or NULL: mean |n . (R X + t - Y)| in the poses' units at the input pose and at the returned
+ *              pose (NaN where there were no pairs)
+ *   trace      NULL, or device buffers (each nullable) that receive the input-pose round's intermediates: pair_idx
+ *              int32 [b,max_points] (pixel indices r*w+c), counts int32 [b,4] (pairs kept, pairs before the stride,
+ *              mask pixels, covered pixels), X, Y, n f64 [b,max_points,3], normal_eq f64 [b,27] (the first step's 21
+ *              upper-triangle sums of J^T J row by row, then J^T e; written only when it runs)
+ *   The other arguments are pvnet_refine_poses's.  Workspace: pvnet_refine_depth_workspace_bytes(b, h, w,
+ *   max_points).  No allocation, no host synchronisation, a fixed number of launches for given rounds (graph
+ *   capturable), and run-to-run identical output. */
+typedef struct {
+    int32_t *pair_idx;
+    int32_t *counts;
+    double *X;
+    double *Y;
+    double *n;
+    double *normal_eq;
+} pvnet_refine_depth_trace_t;
+PVNET_API int pvnet_refine_depth_workspace_bytes(int b, int h, int w, int max_points, size_t *bytes);
+PVNET_API int pvnet_refine_poses_depth(const uint8_t *mask, const void *depth, int depth_is_u16, float depth_scale,
+                                       const double *poses_in, const float *K, int k_per_image, const float *verts,
+                                       const int32_t *faces, int nv, int nf, int b, int h, int w, float near_clip,
+                                       float far_clip, int rounds, double gate, int max_points, double *poses_out,
+                                       int32_t *info, double *dist, const pvnet_refine_depth_trace_t *trace,
+                                       void *workspace, size_t workspace_bytes, pvnet_stream_t stream);
+
 /* The vanishing-point pair of the reference extension (ransac_voting.cpp:61-99 ->
  * ransac_voting_kernel.cu:170-260, :263-351; used by ransac_voting_vanish_point_layer,
  * ransac_voting_gpu.py:408-501): hypotheses are homogeneous points hypo [hn,vn,3]; the vote sets

@@ -38,6 +38,12 @@ class RefineTrace(ctypes.Structure):
                 ("pair_idx", c_void_p), ("normal_eq", c_void_p)]
 
 
+class RefineDepthTrace(ctypes.Structure):
+    """pvnet_refine_depth_trace_t: device buffers for the first round's pairs (include/pvnet_b200.h)."""
+    _fields_ = [("pair_idx", c_void_p), ("counts", c_void_p), ("X", c_void_p), ("Y", c_void_p), ("n", c_void_p),
+                ("normal_eq", c_void_p)]
+
+
 class AdamTensor(ctypes.Structure):
     """pvnet_adam_tensor_t: one entry of pvnet_adam_step's host table (include/pvnet_b200.h)."""
     _fields_ = [("param", c_void_p), ("grad", c_void_p), ("exp_avg", c_void_p), ("exp_avg_sq", c_void_p),
@@ -124,6 +130,11 @@ SIGNATURES = {
                                              c_void_p, c_void_p, c_int, ctypes.c_double, c_void_p, c_void_p, c_void_p,
                                              c_void_p, ctypes.POINTER(RefineTrace), c_void_p, c_void_p, c_size_t,
                                              c_void_p]),
+    "pvnet_refine_depth_workspace_bytes": (c_int, [c_int, c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
+    "pvnet_refine_poses_depth": (c_int, [c_void_p, c_void_p, c_int, c_float, c_void_p, c_void_p, c_int, c_void_p,
+                                         c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_float, c_int,
+                                         ctypes.c_double, c_int, c_void_p, c_void_p, c_void_p,
+                                         ctypes.POINTER(RefineDepthTrace), c_void_p, c_size_t, c_void_p]),
     "pvnet_generate_hypothesis":(c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "pvnet_voting_for_hypothesis": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float,
                                             c_void_p]),

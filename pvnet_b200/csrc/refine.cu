@@ -739,3 +739,424 @@ int pvnet_refine_poses_keypoints(const uint8_t *mask, const double *poses_in, co
 }
 
 }  // extern "C"
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Depth-anchored refinement (DESIGN.md §28, pvnet_refine_poses_depth): point-to-plane ICP of the rendered surface
+// against the registered depth image, one object per image.  Per round: the render at the current pose (as above);
+// k_refine_depth_pairs (one CTA per image) takes every pixel that the render covers, the mask holds and the sensor read,
+// whose four 4-neighbours are inside the image, in the mask and read, and whose pair passes the gate; above max_points
+// every ceil(n / max_points)-th, by k_refine_boundary's count-then-rank scan.  Each pair holds the model point X (the
+// rendered point taken to object space at the round's pose), the observed point Y and the observed normal n from the
+// neighbours' cross product.  k_refine_depth_step (one CTA per image) judges the round by the mean |n . (R X + t - Y)|
+// and, pairs held fixed, takes RF_GN_STEPS damped Gauss-Newton steps on sum (n . (R X + t - Y))^2.
+// oracle/refine_depth_oracle.py restates it; the pair sets, X, Y, n and the mean are bit for bit (one rounded __d*_rn
+// per operation), the normal equations to rounding.
+namespace {
+
+constexpr int RD_PAIR_THREADS = 256;
+constexpr int RD_CHUNK = RD_PAIR_THREADS * RF_PER_THREAD;
+constexpr int RD_NCOUNT = 4;                      // per image: pairs kept, pairs, mask pixels, covered pixels
+
+struct DepthIn {
+    const void *depth;                            // f32 or u16 [b,h,w]
+    int is_u16;
+    float scale;                                  // u16 only: Z = fp32(d) * scale, one rounded multiply
+};
+
+// The observed depth of pixel p of the image at `base` (an element offset), 0 for no reading (<= 0 or not finite).
+__device__ __forceinline__ float observed_depth(const DepthIn &d, long long base, long long p)
+{
+    const float z = d.is_u16 ? __fmul_rn(static_cast<float>(static_cast<const uint16_t *>(d.depth)[base + p]), d.scale)
+                             : static_cast<const float *>(d.depth)[base + p];
+    return z > 0.f && z < INFINITY ? z : 0.f;
+}
+
+// The normalised ray (xn, yn, 1) of pixel (r, c), k_refine_boundary's back-projection.
+__device__ __forceinline__ void pixel_ray(const Cam &cam, int r, int c, double &xn, double &yn)
+{
+    const double u = c + 0.5, v = r + 0.5;
+    yn = dd(ds(v, cam.cy), cam.fy);
+    xn = dd(ds(ds(u, cam.cx), dm(cam.s, yn)), cam.fx);
+}
+
+// n . (R X + t - Y) at pose P, each operation rounded: Xc = project's R X + t, d = Xc - Y, (n0 d0 + n1 d1) + n2 d2.
+// dist (optional): |R X + t - Y| = sqrt((d0 d0 + d1 d1) + d2 d2).
+__device__ __forceinline__ double plane_residual(const double *P, const double *X, const double *Y, const double *n,
+                                                 double *dist = nullptr)
+{
+    double d[3];
+#pragma unroll
+    for (int r = 0; r < 3; ++r)
+        d[r] = ds(da(da(da(dm(P[r * 4], X[0]), dm(P[r * 4 + 1], X[1])), dm(P[r * 4 + 2], X[2])), P[r * 4 + 3]), Y[r]);
+    if (dist) *dist = __dsqrt_rn(da(da(dm(d[0], d[0]), dm(d[1], d[1])), dm(d[2], d[2])));
+    return da(da(dm(n[0], d[0]), dm(n[1], d[1])), dm(n[2], d[2]));
+}
+
+// Pairs of one image (grid b): pass 1 counts the pixels that form a pair (and the mask and covered pixels), pass 2
+// walks them again in row-major order and keeps rank % stride == 0, stride = ceil(n / max_points), writing each at
+// rank / stride.  A pixel forms a pair when it is covered (rendered Z > 0), in the mask, read, its four 4-neighbours
+// are inside the image, in the mask and read, |R X + t - Y| <= gate and the residual is a number.  skip_done: images
+// already stopped are left alone.
+__global__ void __launch_bounds__(RD_PAIR_THREADS)
+    k_refine_depth_pairs(const float *__restrict__ rdepth, const uint8_t *__restrict__ mask, DepthIn obs,
+                         const double *__restrict__ pose, const float *__restrict__ K, int kstride, int h, int w,
+                         int max_points, double gate, int skip_done, const State *__restrict__ state,
+                         int32_t *__restrict__ pix, double *__restrict__ pX, double *__restrict__ pY,
+                         double *__restrict__ pN, int32_t *__restrict__ counts)
+{
+    const int img = blockIdx.x;
+    if (skip_done && state[img].done) return;
+    __shared__ int s_warp[RD_PAIR_THREADS / 32];
+    __shared__ int s_total, s_mask, s_cover;
+    __shared__ double s_pose[12];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const long long hw = static_cast<long long>(h) * w, ibase = img * hw;
+    const float *ren = rdepth + ibase;
+    const uint8_t *msk = mask + ibase;
+    if (tid == 0) s_total = s_mask = s_cover = 0;
+    if (tid < 12) s_pose[tid] = pose[img * 12 + tid];
+    __syncthreads();
+    const Cam cam = load_cam(K + static_cast<size_t>(img) * kstride);
+    // pixel p as a pair: X (object space, round's pose), Y (observed), n (observed normal, n . Y <= 0)
+    auto pair_at = [&](long long p, double (&X)[3], double (&Y)[3], double (&nn)[3]) -> bool {
+        const float zr = ren[p];
+        if (!(zr > 0.f) || !msk[p]) return false;
+        const float zo = observed_depth(obs, ibase, p);
+        if (zo == 0.f) return false;
+        const int r = static_cast<int>(p / w), c = static_cast<int>(p - static_cast<long long>(r) * w);
+        if (r == 0 || r == h - 1 || c == 0 || c == w - 1) return false;
+        const long long nb[4] = {p + 1, p - 1, p + w, p - w};
+        float zn[4];
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            if (!msk[nb[q]]) return false;
+            zn[q] = observed_depth(obs, ibase, nb[q]);
+            if (zn[q] == 0.f) return false;
+        }
+        double xn, yn;
+        pixel_ray(cam, r, c, xn, yn);
+        const double Z = zr;
+        const double d0 = ds(dm(Z, xn), s_pose[3]), d1 = ds(dm(Z, yn), s_pose[7]), d2 = ds(Z, s_pose[11]);
+#pragma unroll
+        for (int k = 0; k < 3; ++k) X[k] = da(da(dm(s_pose[k], d0), dm(s_pose[4 + k], d1)), dm(s_pose[8 + k], d2));
+        const double zo64 = zo;
+        Y[0] = dm(zo64, xn);
+        Y[1] = dm(zo64, yn);
+        Y[2] = zo64;
+        double Q[4][3];                           // the neighbours' observed points: c + 1, c - 1, r + 1, r - 1
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            double qx, qy;
+            pixel_ray(cam, r + (q == 2) - (q == 3), c + (q == 0) - (q == 1), qx, qy);
+            const double z = zn[q];
+            Q[q][0] = dm(z, qx);
+            Q[q][1] = dm(z, qy);
+            Q[q][2] = z;
+        }
+        double a[3], bv[3];
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+            a[k] = ds(Q[0][k], Q[1][k]);
+            bv[k] = ds(Q[2][k], Q[3][k]);
+        }
+        nn[0] = ds(dm(a[1], bv[2]), dm(a[2], bv[1]));
+        nn[1] = ds(dm(a[2], bv[0]), dm(a[0], bv[2]));
+        nn[2] = ds(dm(a[0], bv[1]), dm(a[1], bv[0]));
+        const double len = __dsqrt_rn(da(da(dm(nn[0], nn[0]), dm(nn[1], nn[1])), dm(nn[2], nn[2])));
+#pragma unroll
+        for (int k = 0; k < 3; ++k) nn[k] = dd(nn[k], len);
+        if (da(da(dm(nn[0], Y[0]), dm(nn[1], Y[1])), dm(nn[2], Y[2])) > 0.0)
+#pragma unroll
+            for (int k = 0; k < 3; ++k) nn[k] = -nn[k];
+        double dist;
+        const double e = plane_residual(s_pose, X, Y, nn, &dist);
+        return dist <= gate && isfinite(e);
+    };
+    int local = 0, lmask = 0, lcover = 0;
+    for (long long base = 0; base < hw; base += RD_CHUNK)
+        for (int q = 0; q < RF_PER_THREAD; ++q) {
+            const long long p = base + static_cast<long long>(tid) * RF_PER_THREAD + q;
+            if (p >= hw) continue;
+            lmask += msk[p] != 0;
+            lcover += ren[p] > 0.f;
+            double X[3], Y[3], nn[3];
+            if (pair_at(p, X, Y, nn)) ++local;
+        }
+    atomicAdd(&s_total, local);                   // integer sums: the same whatever the order
+    atomicAdd(&s_mask, lmask);
+    atomicAdd(&s_cover, lcover);
+    __syncthreads();
+    const int n = s_total;
+    const int stride = n > max_points ? (n + max_points - 1) / max_points : 1;
+    const size_t o = static_cast<size_t>(img) * max_points;
+    int running = 0;                              // pairs in earlier chunks
+    for (long long base = 0; base < hw; base += RD_CHUNK) {
+        unsigned bits = 0;
+        for (int q = 0; q < RF_PER_THREAD; ++q) {
+            const long long p = base + static_cast<long long>(tid) * RF_PER_THREAD + q;
+            double X[3], Y[3], nn[3];
+            if (p < hw && pair_at(p, X, Y, nn)) bits |= 1u << q;
+        }
+        const int cnt = __popc(bits);
+        int incl = cnt;                           // inclusive scan over the warp
+#pragma unroll
+        for (int s = 1; s < 32; s <<= 1) {
+            const int y = __shfl_up_sync(0xffffffffu, incl, s);
+            if (lane >= s) incl += y;
+        }
+        if (lane == 31) s_warp[warp] = incl;
+        __syncthreads();
+        if (warp == 0) {
+            int t = lane < RD_PAIR_THREADS / 32 ? s_warp[lane] : 0;
+#pragma unroll
+            for (int s = 1; s < 32; s <<= 1) {
+                const int y = __shfl_up_sync(0xffffffffu, t, s);
+                if (lane >= s) t += y;
+            }
+            if (lane < RD_PAIR_THREADS / 32) s_warp[lane] = t;   // inclusive warp totals
+        }
+        __syncthreads();
+        int rank = running + (warp ? s_warp[warp - 1] : 0) + incl - cnt;
+        for (int q = 0; q < RF_PER_THREAD; ++q) {
+            if (!(bits >> q & 1u)) continue;
+            if (rank % stride == 0) {
+                const long long p = base + static_cast<long long>(tid) * RF_PER_THREAD + q;
+                const size_t j = o + rank / stride;
+                double X[3], Y[3], nn[3];
+                pair_at(p, X, Y, nn);
+                pix[j] = static_cast<int32_t>(p);
+#pragma unroll
+                for (int k = 0; k < 3; ++k) {
+                    pX[j * 3 + k] = X[k];
+                    pY[j * 3 + k] = Y[k];
+                    pN[j * 3 + k] = nn[k];
+                }
+            }
+            ++rank;
+        }
+        running += s_warp[RD_PAIR_THREADS / 32 - 1];
+        __syncthreads();                          // s_warp is rewritten by the next chunk
+    }
+    if (tid == 0) {
+        int32_t *cn = counts + img * RD_NCOUNT;
+        cn[0] = n ? (n + stride - 1) / stride : 0;
+        cn[1] = n;
+        cn[2] = s_mask;
+        cn[3] = s_cover;
+    }
+}
+
+// One CTA per image: evaluation k of the pose (mean |e| over the pairs, pair i on thread i % 256 and block_sum's
+// order; accept or undo as k_refine_step does), then, unless k is the last evaluation, RF_GN_STEPS Gauss-Newton steps
+// on sum e_i^2, e_i = n_i . (R X_i + t - Y_i), J_i = [(R X_i) x n_i ; n_i].  normal_eq (nullable): the sums of the
+// first step of evaluation 0.
+__global__ void __launch_bounds__(RF_STEP_THREADS)
+    k_refine_depth_step(double *__restrict__ pose, float *__restrict__ pose32, int max_points, int k, int last,
+                        State *__restrict__ state, const int32_t *__restrict__ counts, const double *__restrict__ pX,
+                        const double *__restrict__ pY, const double *__restrict__ pN, double *__restrict__ normal_eq)
+{
+    const int img = blockIdx.x;
+    State &S = state[img];
+    if (S.done) return;
+    __shared__ double s_part[RF_STEP_THREADS / 32][RF_NSUM];
+    __shared__ double s_sum[RF_NSUM];
+    __shared__ double s_pose[12];
+    __shared__ int s_go;
+    const int32_t *cn = counts + img * RD_NCOUNT;
+    const int ns = cn[0];
+    const size_t o = static_cast<size_t>(img) * max_points;
+    if (threadIdx.x < 12) s_pose[threadIdx.x] = pose[img * 12 + threadIdx.x];
+    __syncthreads();
+    double acc[2] = {0.0, 0.0};
+    for (int i = threadIdx.x; i < ns; i += RF_STEP_THREADS) {
+        acc[0] += 1.0;
+        acc[1] += fabs(plane_residual(s_pose, pX + (o + i) * 3, pY + (o + i) * 3, pN + (o + i) * 3));
+    }
+    block_sum<2>(acc, reinterpret_cast<double (*)[2]>(&s_part[0][0]), s_sum);
+    if (threadIdx.x == 0) {
+        const int n = static_cast<int>(s_sum[0]);
+        const double m = n ? s_sum[1] / n : NAN;
+        bool go = true;
+        if (k == 0) {
+            int st = 0;
+            if (cn[2] == 0) st = RF_NO_CONTOUR;
+            else if (cn[3] == 0) st = RF_NO_SILHOUETTE;
+            else if (n < RF_MIN_PAIRS) st = RF_FEW_PAIRS;
+            if (st) {
+                S.status |= st;
+                go = false;
+            } else {
+                S.mean0 = S.mean_after = m;
+            }
+        } else if (n < RF_MIN_PAIRS || m > S.mean_prev) {
+            S.status |= RF_REJECTED;
+            for (int q = 0; q < 12; ++q) pose[img * 12 + q] = S.backup[q];
+            go = false;
+        } else {
+            S.mean_after = m;
+        }
+        if (!go) S.done = 1;
+        if (go && !last) {
+            S.mean_prev = m;
+            for (int q = 0; q < 12; ++q) S.backup[q] = pose[img * 12 + q];
+            S.pairs = n;
+        }
+        s_go = go && !last;
+    }
+    __syncthreads();
+    if (!s_go) return;
+    for (int step = 0; step < RF_GN_STEPS; ++step) {
+        double v[RF_NSUM];
+#pragma unroll
+        for (int q = 0; q < RF_NSUM; ++q) v[q] = 0.0;
+        for (int i = threadIdx.x; i < ns; i += RF_STEP_THREADS) {
+            const double *X = pX + (o + i) * 3, *Y = pY + (o + i) * 3, *nn = pN + (o + i) * 3;
+            double p[3], d[3];
+#pragma unroll
+            for (int r = 0; r < 3; ++r) {
+                p[r] = s_pose[r * 4] * X[0] + s_pose[r * 4 + 1] * X[1] + s_pose[r * 4 + 2] * X[2];
+                d[r] = p[r] + s_pose[r * 4 + 3] - Y[r];
+            }
+            const double e = nn[0] * d[0] + nn[1] * d[1] + nn[2] * d[2];
+            // d e / d(dw) for R <- exp(dw) R is (R X) x n; d e / d(dt) is n
+            const double J[6] = {p[1] * nn[2] - p[2] * nn[1], p[2] * nn[0] - p[0] * nn[2], p[0] * nn[1] - p[1] * nn[0],
+                                 nn[0], nn[1], nn[2]};
+            int q = 0;
+#pragma unroll
+            for (int r = 0; r < 6; ++r)
+#pragma unroll
+                for (int c = r; c < 6; ++c) v[q++] += J[r] * J[c];
+#pragma unroll
+            for (int r = 0; r < 6; ++r) v[21 + r] += J[r] * e;
+        }
+        block_sum<RF_NSUM>(v, s_part, s_sum);
+        if (threadIdx.x == 0) {
+            if (normal_eq && k == 0 && step == 0)
+                for (int q = 0; q < RF_NSUM; ++q) normal_eq[img * RF_NSUM + q] = s_sum[q];
+            double x[6];
+            if (!damped_solve(s_sum, x)) {
+                S.status |= RF_SINGULAR;
+                S.done = 1;
+                for (int q = 0; q < 12; ++q) s_pose[q] = S.backup[q];
+                s_go = 0;
+            } else {
+                double E[9], R[9];
+                so3_exp(x[0], x[1], x[2], E);
+                for (int r = 0; r < 3; ++r)
+                    for (int c = 0; c < 3; ++c)
+                        R[r * 3 + c] = E[r * 3] * s_pose[c] + E[r * 3 + 1] * s_pose[4 + c] + E[r * 3 + 2] * s_pose[8 + c];
+                for (int r = 0; r < 3; ++r) {
+                    for (int c = 0; c < 3; ++c) s_pose[r * 4 + c] = R[r * 3 + c];
+                    s_pose[r * 4 + 3] += x[3 + r];
+                }
+            }
+        }
+        __syncthreads();
+        if (!s_go) break;
+    }
+    if (threadIdx.x < 12) {
+        pose[img * 12 + threadIdx.x] = s_pose[threadIdx.x];
+        pose32[img * 12 + threadIdx.x] = __double2float_rn(s_pose[threadIdx.x]);
+    }
+}
+
+struct DepthLayout {
+    unsigned long long *keys;
+    float *depth, *pose32;
+    int32_t *pix, *counts;
+    double *X, *Y, *N;
+    State *state;
+    size_t bytes;
+};
+
+DepthLayout carve_depth(void *base, int b, int h, int w, int max_points)
+{
+    pvnet::Carver cv(base);
+    DepthLayout L;
+    const size_t npix = static_cast<size_t>(b) * h * w, np = static_cast<size_t>(b) * max_points;
+    L.keys = cv.take<unsigned long long>(npix);
+    L.depth = cv.take<float>(npix);
+    L.pose32 = cv.take<float>(static_cast<size_t>(b) * 12);
+    L.pix = cv.take<int32_t>(np);
+    L.X = cv.take<double>(np * 3);
+    L.Y = cv.take<double>(np * 3);
+    L.N = cv.take<double>(np * 3);
+    L.counts = cv.take<int32_t>(static_cast<size_t>(b) * RD_NCOUNT);
+    L.state = cv.take<State>(b);
+    L.bytes = pvnet::align_up(cv.off, 256);
+    return L;
+}
+
+}  // namespace
+
+extern "C" {
+
+int pvnet_refine_depth_workspace_bytes(int b, int h, int w, int max_points, size_t *bytes)
+{
+    PV_CHECK_ARG(b >= 1 && h >= 1 && w >= 1 && max_points >= 1, "non-positive dimension (b=%d, h=%d, w=%d, "
+                 "max_points=%d)", b, h, w, max_points);
+    PV_CHECK_ARG(bytes, "null pointer");
+    *bytes = carve_depth(nullptr, b, h, w, max_points).bytes;
+    return PVNET_OK;
+}
+
+int pvnet_refine_poses_depth(const uint8_t *mask, const void *depth, int depth_is_u16, float depth_scale,
+                             const double *poses_in, const float *K, int k_per_image, const float *verts,
+                             const int32_t *faces, int nv, int nf, int b, int h, int w, float near_clip,
+                             float far_clip, int rounds, double gate, int max_points, double *poses_out, int32_t *info,
+                             double *dist, const pvnet_refine_depth_trace_t *trace, void *workspace,
+                             size_t workspace_bytes, pvnet_stream_t stream)
+{
+    PV_CHECK_ARG(b >= 1 && h >= 1 && w >= 1 && nv >= 0 && nf >= 0, "bad dimension (b=%d, h=%d, w=%d, nv=%d, nf=%d)",
+                 b, h, w, nv, nf);
+    PV_CHECK_ARG(static_cast<long long>(h) * w <= INT32_MAX, "image %dx%d too large", h, w);
+    PV_CHECK_ARG(max_points >= 1 && static_cast<long long>(b) * max_points <= INT32_MAX / 9,
+                 "max_points %d outside 1..%d for b = %d", max_points, INT32_MAX / 9 / b, b);
+    PV_CHECK_ARG(rounds >= 0, "rounds must be >= 0 (got %d)", rounds);
+    PV_CHECK_ARG(gate > 0.0 && gate < INFINITY, "gate must be positive and finite (got %g)", gate);
+    PV_CHECK_ARG(!depth_is_u16 || (depth_scale > 0.f && depth_scale < INFINITY),
+                 "depth_scale must be positive and finite (got %g)", depth_scale);
+    PV_CHECK_ARG(mask && depth && poses_in && K && poses_out && (nf == 0 || faces) && (nv == 0 || verts),
+                 "null pointer");
+    size_t need = 0;
+    pvnet_refine_depth_workspace_bytes(b, h, w, max_points, &need);
+    PV_CHECK_ARG(workspace && workspace_bytes >= need, "workspace %zu bytes < %zu", workspace_bytes, need);
+    const DepthLayout L = carve_depth(workspace, b, h, w, max_points);
+    size_t render_need = 0;
+    pvnet_render_workspace_bytes(b, h, w, &render_need);
+    const cudaStream_t st = (cudaStream_t)stream;
+    const int kstride = k_per_image ? 9 : 0;
+    const DepthIn obs{depth, depth_is_u16 ? 1 : 0, depth_is_u16 ? depth_scale : 1.f};
+    k_refine_init<<<(b + 127) / 128, 128, 0, st>>>(poses_in, poses_out, L.pose32, L.state, b);
+    PV_LAUNCHED("k_refine_init");
+    for (int k = 0; k <= rounds; ++k) {
+        const int rc = pvnet_render_mesh(verts, faces, nullptr, nv, nf, L.pose32, K, k_per_image, b, h, w, near_clip,
+                                         far_clip, 0.5f, nullptr, L.depth, nullptr, L.keys, render_need, stream);
+        if (rc != PVNET_OK) return rc;
+        k_refine_depth_pairs<<<b, RD_PAIR_THREADS, 0, st>>>(L.depth, mask, obs, poses_out, K, kstride, h, w,
+                                                            max_points, gate, k > 0, L.state, L.pix, L.X, L.Y, L.N,
+                                                            L.counts);
+        PV_LAUNCHED("k_refine_depth_pairs");
+        if (k == 0 && trace) {
+            const size_t np = static_cast<size_t>(b) * max_points;
+            if (trace->pair_idx) PV_CUDA(cudaMemcpyAsync(trace->pair_idx, L.pix, np * 4, cudaMemcpyDeviceToDevice, st));
+            if (trace->counts)
+                PV_CUDA(cudaMemcpyAsync(trace->counts, L.counts, static_cast<size_t>(b) * RD_NCOUNT * 4,
+                                        cudaMemcpyDeviceToDevice, st));
+            if (trace->X) PV_CUDA(cudaMemcpyAsync(trace->X, L.X, np * 24, cudaMemcpyDeviceToDevice, st));
+            if (trace->Y) PV_CUDA(cudaMemcpyAsync(trace->Y, L.Y, np * 24, cudaMemcpyDeviceToDevice, st));
+            if (trace->n) PV_CUDA(cudaMemcpyAsync(trace->n, L.N, np * 24, cudaMemcpyDeviceToDevice, st));
+        }
+        k_refine_depth_step<<<b, RF_STEP_THREADS, 0, st>>>(poses_out, L.pose32, max_points, k, k == rounds, L.state,
+                                                           L.counts, L.X, L.Y, L.N,
+                                                           trace ? trace->normal_eq : nullptr);
+        PV_LAUNCHED("k_refine_depth_step");
+    }
+    if (info || dist) {
+        k_refine_finish<<<(b + 127) / 128, 128, 0, st>>>(L.state, b, info, dist, nullptr);
+        PV_LAUNCHED("k_refine_finish");
+    }
+    return PVNET_OK;
+}
+
+}  // extern "C"

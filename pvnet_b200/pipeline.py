@@ -27,7 +27,11 @@ way, the host thread is what is freed).  The device-side sampler keeps drawing f
 `refine=dict(vertices=, faces=, near=, far=, ...)`: the poses are then refined on the device before they are returned
 (`refine.refine_poses` with the step's own fused-argmax mask, PnP poses, keypoints and covariances and its cameras,
 the keypoint-anchored objective of DESIGN.md §27), inside the same captured graph when graph=True.  The mesh goes to
-the device once.
+the device once.  With `refine=dict(..., depth=dict(gate=, rounds=8, max_points=4096, depth_scale=1.0))` the refined
+poses are then refined again against each image's registered depth (`refine.refine_poses_depth`, DESIGN.md §28):
+`step(x, depth=)` takes a CUDA [b,H,W] float32 or uint16, `run(..., depths=)` one host [b,H,W] per batch, copied on
+the side stream into a static device buffer per input buffer like the cameras.  The mesh, clip planes and cameras are
+refine's; depth-only refinement is `refine=dict(..., rounds=0, depth=...)`.
 
 Inputs may be float32 [b,3,H,W] (already normalised, what `ToTensor` + `Normalize` produce,
 tools/demo.py:89-95) or uint8 [b,H,W,3] raw images: the latter are normalised on the device inside
@@ -69,26 +73,44 @@ class PoseKeypointPipeline:
         if refine is not None:
             if points_3d is None or not with_covariance:
                 raise ValueError("refine needs points_3d and with_covariance=True")
-            cfg = dict(rounds=8, gate=20.0, max_points=4096, keypoint_weight=rfn.DEFAULT_KEYPOINT_WEIGHT)
+            cfg = dict(rounds=8, gate=20.0, max_points=4096, keypoint_weight=rfn.DEFAULT_KEYPOINT_WEIGHT, depth=None)
             unknown = set(refine) - {"vertices", "faces", "near", "far", *cfg}
             missing = {"vertices", "faces", "near", "far"} - set(refine)
             if unknown or missing:
                 raise ValueError(f"refine: unknown keys {sorted(unknown)}, missing keys {sorted(missing)}")
             cfg.update(refine)
+            if cfg["depth"] is not None:
+                dcfg = dict(rounds=8, max_points=4096, depth_scale=1.0)
+                unknown = set(cfg["depth"]) - {"gate", *dcfg}
+                if unknown or "gate" not in cfg["depth"]:
+                    raise ValueError(f"refine['depth']: unknown keys {sorted(unknown)}; gate is required")
+                dcfg.update(cfg["depth"])
+                cfg["depth"] = dcfg
             self.refine = cfg
         self._mesh_dev = None                       # (device, vertices, faces, constructor K or None)
         self._p3_dev = None
         self._bufs = None
         self._kbufs = None
+        self._dbufs = None
         self._copy_stream = None
 
-    def _setup(self, host_batch, dev, per_batch_k):
+    @property
+    def _with_depth(self):
+        return self.refine is not None and self.refine["depth"] is not None
+
+    def _setup(self, host_batch, dev, per_batch_k, host_depth=None):
         if (self._bufs is None or self._bufs[0].shape != host_batch.shape or self._bufs[0].dtype != host_batch.dtype
-                or self._bufs[0].device != dev or (self._kbufs is not None) != per_batch_k):
+                or self._bufs[0].device != dev or (self._kbufs is not None) != per_batch_k
+                or (self._dbufs is not None) != (host_depth is not None)
+                or (host_depth is not None and (self._dbufs[0].shape != host_depth.shape
+                                                or self._dbufs[0].dtype != host_depth.dtype))):
             self._bufs = [torch.empty(host_batch.shape, dtype=host_batch.dtype, device=dev) for _ in range(2)]
             # per input buffer: the batch's cameras, float64 [b,3,3] (static, so a captured graph reads each batch's)
             self._kbufs = ([torch.empty([host_batch.shape[0], 3, 3], dtype=torch.float64, device=dev) for _ in range(2)]
                            if per_batch_k else None)
+            # per input buffer: the batch's registered depth (static, like the cameras)
+            self._dbufs = ([torch.empty(host_depth.shape, dtype=host_depth.dtype, device=dev) for _ in range(2)]
+                           if host_depth is not None else None)
             self._ready = [torch.cuda.Event() for _ in range(2)]      # H2D of buffer i finished
             self._free = [torch.cuda.Event() for _ in range(2)]       # compute no longer reads buffer i
             self._done = torch.cuda.Event()                           # last D2H of a run() finished
@@ -98,30 +120,36 @@ class PoseKeypointPipeline:
                 e.record(torch.cuda.current_stream(dev))
 
     def _step_graph(self, j):
-        """Replay (capture on first use) the graph of `step(self._bufs[j], self._kbufs[j])` on the current stream."""
+        """Replay (capture on first use) the graph of `step(self._bufs[j], self._kbufs[j], self._dbufs[j])` on the
+        current stream."""
         if self._graphs[j] is None:
             cur = torch.cuda.current_stream(self._bufs[j].device)
             side = torch.cuda.Stream(device=self._bufs[j].device)
             side.wait_stream(cur)
             k = None if self._kbufs is None else self._kbufs[j]
+            d = None if self._dbufs is None else self._dbufs[j]
             with torch.cuda.stream(side):
-                self.step(self._bufs[j], k)         # eager once on the capture stream: plans, workspaces, attributes
+                self.step(self._bufs[j], k, d)      # eager once on the capture stream: plans, workspaces, attributes
                 side.synchronize()
                 g = torch.cuda.CUDAGraph()
                 with torch.cuda.graph(g, stream=side):
-                    res = self.step(self._bufs[j], k)
+                    res = self.step(self._bufs[j], k, d)
             cur.wait_stream(side)
             self._graphs[j] = (g, res)
         g, res = self._graphs[j]
         g.replay()
         return res
 
-    def step(self, x, camera_matrix=None):
+    def step(self, x, camera_matrix=None, depth=None):
         """x on the device: float32 [b,3,H,W] or uint8 [b,H,W,3] -> keypoints [b,K,2]
         (and covariances [b,K,2,2]) (and poses [b,3,4] float64).  camera_matrix: this batch's cameras, a CUDA
-        tensor [b,3,3] (or [3,3]), in place of the constructor's; it needs `points_3d` and `with_covariance`."""
+        tensor [b,3,3] (or [3,3]), in place of the constructor's; it needs `points_3d` and `with_covariance`.
+        depth: this batch's registered depth, a CUDA [b,H,W] float32 or uint16; required exactly when
+        refine['depth'] is set."""
         if camera_matrix is not None and (self.points_3d is None or not self.with_cov):
             raise ValueError("per-batch camera matrices need points_3d and with_covariance=True")
+        if (depth is not None) != self._with_depth:
+            raise ValueError("depth goes with refine['depth'], and refine['depth'] needs depth")
         # pixel-major head output: the vertex field is the contiguous [b,h,w,K,2] form of the permuted view of
         # tools/demo.py:48-50 (same values; the voting layer's gather then reads whole records, not sectors)
         if x.dtype == torch.uint8:
@@ -149,12 +177,13 @@ class PoseKeypointPipeline:
             K = self.camera_matrix if camera_matrix is None else camera_matrix
             pose = eu.uncertainty_pnp_batched(res[0], self._p3_dev, K, cov=res[1])
             if self.refine is not None:
-                pose = self._refine(mask, pose, K, res[0], res[1])
+                pose = self._refine(mask, pose, K, res[0], res[1], depth)
             return res[0], res[1], pose
         return res
 
-    def _refine(self, mask, pose, K, kp, cov):
-        """refine_poses on the step's outputs; the mesh (and a host camera) go to the device on first use."""
+    def _refine(self, mask, pose, K, kp, cov, depth):
+        """refine_poses on the step's outputs, then refine_poses_depth on its poses when depth is given; the mesh (and
+        a host camera) go to the device on first use."""
         dev = pose.device
         cfg = self.refine
         if self._mesh_dev is None or self._mesh_dev[0] != dev:
@@ -173,18 +202,27 @@ class PoseKeypointPipeline:
             k = k_host
         else:
             k = torch.as_tensor(K, dtype=torch.float64).reshape(3, 3).to(dev)
-        return rfn.refine_poses(mask, pose, k, v, f, cfg["near"], cfg["far"], rounds=cfg["rounds"], gate=cfg["gate"],
+        pose = rfn.refine_poses(mask, pose, k, v, f, cfg["near"], cfg["far"], rounds=cfg["rounds"], gate=cfg["gate"],
                                 max_points=cfg["max_points"], keypoints=kp, points_3d=self._p3_dev, cov=cov,
                                 keypoint_weight=cfg["keypoint_weight"])
+        if depth is not None:
+            d = cfg["depth"]
+            pose = rfn.refine_poses_depth(mask, depth, pose, k, v, f, cfg["near"], cfg["far"], gate=d["gate"],
+                                          rounds=d["rounds"], max_points=d["max_points"],
+                                          depth_scale=d["depth_scale"])
+        return pose
 
     @torch.no_grad()
-    def run(self, host_batches, out_host=None, cov_host=None, on_result=None, pose_host=None, camera_matrices=None):
+    def run(self, host_batches, out_host=None, cov_host=None, on_result=None, pose_host=None, camera_matrices=None,
+            depths=None):
         """host_batches: sequence of pinned [b,3,H,W] float32 (or [b,H,W,3] uint8) tensors.  Results are
         copied device->host into out_host[i] (and cov_host[i]) -- pinned tensors -- when given; the call
         returns after the last of those copies has completed.  Returns the last device result (with graph=True a
         static tensor that the next replay on the same input buffer overwrites).
         camera_matrices: one host [b,3,3] (or [3,3]) per batch, numpy or CPU tensor (pinned float64 makes the copy as
-        asynchronous as the images'): the cameras of that batch's images, used in place of the constructor's."""
+        asynchronous as the images'): the cameras of that batch's images, used in place of the constructor's.
+        depths: one host [b,H,W] float32 or uint16 tensor per batch (pinned, for an asynchronous copy), that batch's
+        registered depth; required exactly when refine['depth'] is set."""
         dev = next(self.net.parameters()).device
         batches = list(host_batches)
         if not batches:
@@ -198,7 +236,16 @@ class PoseKeypointPipeline:
                 eu.check_cameras(k.shape, batches[0].shape[0])
             if self.points_3d is None or not self.with_cov:
                 raise ValueError("per-batch camera matrices need points_3d and with_covariance=True")
-        self._setup(batches[0], dev, cams is not None)
+        if (depths is not None) != self._with_depth:
+            raise ValueError("depths go with refine['depth'], and refine['depth'] needs depths")
+        if depths is not None:
+            depths = list(depths)
+            if len(depths) != len(batches):
+                raise ValueError(f"{len(depths)} depth batches for {len(batches)} image batches")
+            if any(not isinstance(d, torch.Tensor) or d.shape != depths[0].shape or d.dtype != depths[0].dtype
+                   for d in depths):
+                raise ValueError("depths must be torch tensors of one shape and dtype")
+        self._setup(batches[0], dev, cams is not None, None if depths is None else depths[0])
         main = torch.cuda.current_stream(dev)
         cs = self._copy_stream
         result = None
@@ -210,6 +257,8 @@ class PoseKeypointPipeline:
                 self._bufs[j].copy_(batches[i], non_blocking=True)
                 if cams is not None:
                     self._kbufs[j].copy_(cams[i], non_blocking=True)
+                if depths is not None:
+                    self._dbufs[j].copy_(depths[i], non_blocking=True)
                 self._ready[j].record(cs)
         upload(0)
         for i in range(len(batches)):
@@ -218,7 +267,8 @@ class PoseKeypointPipeline:
                 upload(i + 1)
             main.wait_event(self._ready[j])
             k = None if cams is None else self._kbufs[j]
-            result = self._step_graph(j) if self.graph else self.step(self._bufs[j], k)
+            d = None if depths is None else self._dbufs[j]
+            result = self._step_graph(j) if self.graph else self.step(self._bufs[j], k, d)
             self._free[j].record(main)
             if out_host is not None:
                 kp = result[0] if isinstance(result, tuple) else result

@@ -10,7 +10,11 @@ restates it.  No CPU path: without the library or a CUDA device it raises.
 With `keypoints` (the voted keypoints, their model points and covariances or weights, as `uncertainty_pnp_batched`
 takes them) each step also pulls the keypoints' weighted reprojections towards the votes
 (`pvnet_refine_poses_keypoints`, DESIGN.md §27): the rotations an outline barely constrains are held by the
-keypoints."""
+keypoints.
+
+`refine_poses_depth` refines the same way against a registered depth image (`pvnet_refine_poses_depth`, DESIGN.md
+§28): point-to-plane ICP of the rendered surface against the observed one, which holds the distance along the
+viewing ray that the RGB cues barely see."""
 from __future__ import annotations
 
 import ctypes
@@ -74,32 +78,9 @@ def _keypoint_inputs(b, dev, keypoints, points_3d, cov, weights_2d, keypoint_wei
     return keypoints.contiguous().float(), points_3d.contiguous().float(), wgt.contiguous(), nk, lam
 
 
-def refine_poses(mask, poses, K, vertices, faces, near, far, rounds=8, gate=20.0, max_points=4096,
-                 return_info=False, trace=False, keypoints=None, points_3d=None, cov=None, weights_2d=None,
-                 keypoint_weight=DEFAULT_KEYPOINT_WEIGHT):
-    """Refine b poses of one mesh so its rendered silhouette meets each mask's contour.
-
-    mask [b,H,W] (any integer dtype or bool; nonzero is foreground), poses [b,3,4] (float32 or float64, R | t object
-    to OpenCV camera), K [3,3] or [b,3,3], vertices [nv,3] and faces [nf,3] (integer): CUDA tensors on one device.
-    The mesh is in the poses' translation units, and so are near and far, the render's clip planes.  Each round
-    pairs the silhouette with the contour, drops pairs more than `gate` pixels apart, and keeps at most `max_points`
-    points of each (every ceil(n / max_points)-th).  `rounds` is a host constant: a call is a fixed sequence of
-    launches, with no host synchronisation, and can be captured in a CUDA graph.  rounds = 0 returns the input.
-
-    -> poses float64 [b,3,4] on the device.  return_info: also a dict of [b] tensors, "status" (int32 bits, see the
-    module's constants), "pairs" (int32, the pairs of the last round that took its steps), "dist_before" and
-    "dist_after" (float64, the mean pair distance in pixels at the input pose and at the returned one, NaN without
-    pairs).  trace: also a dict of the first round's intermediates ("sil_idx", "con_idx", "pair_idx" int32
-    [b,max_points], "counts" int32 [b,2], "sil_obj" float64 [b,max_points,3], "normal_eq" float64 [b,27]), for
-    checking the stages against the oracle.
-
-    keypoints [b,nk,2] (4 <= nk <= 32, pixels as `uncertainty_pnp_batched` reads them), points_3d [nk,3] (their
-    model points, in the mesh's units) and exactly one of cov [b,nk,2,2] / weights_2d [b,nk,3] (converted through
-    `covariance_to_weights`), floating-point CUDA tensors on the poses' device: each step then minimises
-    (1/n) sum |pi(R X_i + t) - c_i|^2 + (keypoint_weight / nk) sum |W_k (pi(R P_k + t) - x_k)|^2, and a round is
-    undone when C = mean pair distance + keypoint_weight * mean_k |W_k e_k| rose (DESIGN.md §27).  return_info then
-    adds "cost_before" and "cost_after" (float64, C at the input pose and at the returned one), and trace adds
-    "keypoint_eq" (float64 [b,27], the first step's keypoint sums, unscaled)."""
+def _check_common(mask, poses, K, vertices, faces, near, far, rounds, gate, max_points, point_words):
+    """refine_poses's checks, shared with refine_poses_depth -> (device, b, h, w, near, far, rounds, gate,
+    max_points); point_words: the fp64 words kept per point, which bounds b * max_points."""
     for name, t in (("mask", mask), ("poses", poses), ("K", K), ("vertices", vertices), ("faces", faces)):
         _cuda_tensor(name, t)
     dev = poses.device
@@ -134,8 +115,49 @@ def refine_poses(mask, poses, K, vertices, faces, near, far, rounds=8, gate=20.0
         raise ValueError(f"rounds must be >= 0, got {rounds}")
     if not 0 < gate < math.inf:
         raise ValueError(f"gate must be positive and finite, got {gate}")
-    if not 1 <= max_points <= (2 ** 31 - 1) // 3 // b:
-        raise ValueError(f"max_points must lie in 1..{(2 ** 31 - 1) // 3 // b} for b = {b}, got {max_points}")
+    if not 1 <= max_points <= (2 ** 31 - 1) // point_words // b:
+        raise ValueError(f"max_points must lie in 1..{(2 ** 31 - 1) // point_words // b} for b = {b}, got {max_points}")
+    return dev, b, h, w, near, far, rounds, gate, max_points
+
+
+def _device_inputs(mask, poses, K, vertices, faces):
+    """-> mask uint8, poses f64, K f32, vertices f32, faces int32, all contiguous, and nv, nf."""
+    nv, nf = int(vertices.shape[0]), int(faces.shape[0])
+    m = mask.view(torch.uint8) if mask.dtype in (torch.uint8, torch.bool) else (mask != 0).to(torch.uint8)
+    # an index beyond int32 is out of range either way; the clamp keeps it so
+    f = faces.contiguous() if faces.dtype == torch.int32 else faces.clamp(-1, nv).to(torch.int32).contiguous()
+    return (m.contiguous(), poses.contiguous().double(), K.contiguous().float(), vertices.contiguous().float(), f,
+            nv, nf)
+
+
+def refine_poses(mask, poses, K, vertices, faces, near, far, rounds=8, gate=20.0, max_points=4096,
+                 return_info=False, trace=False, keypoints=None, points_3d=None, cov=None, weights_2d=None,
+                 keypoint_weight=DEFAULT_KEYPOINT_WEIGHT):
+    """Refine b poses of one mesh so its rendered silhouette meets each mask's contour.
+
+    mask [b,H,W] (any integer dtype or bool; nonzero is foreground), poses [b,3,4] (float32 or float64, R | t object
+    to OpenCV camera), K [3,3] or [b,3,3], vertices [nv,3] and faces [nf,3] (integer): CUDA tensors on one device.
+    The mesh is in the poses' translation units, and so are near and far, the render's clip planes.  Each round
+    pairs the silhouette with the contour, drops pairs more than `gate` pixels apart, and keeps at most `max_points`
+    points of each (every ceil(n / max_points)-th).  `rounds` is a host constant: a call is a fixed sequence of
+    launches, with no host synchronisation, and can be captured in a CUDA graph.  rounds = 0 returns the input.
+
+    -> poses float64 [b,3,4] on the device.  return_info: also a dict of [b] tensors, "status" (int32 bits, see the
+    module's constants), "pairs" (int32, the pairs of the last round that took its steps), "dist_before" and
+    "dist_after" (float64, the mean pair distance in pixels at the input pose and at the returned one, NaN without
+    pairs).  trace: also a dict of the first round's intermediates ("sil_idx", "con_idx", "pair_idx" int32
+    [b,max_points], "counts" int32 [b,2], "sil_obj" float64 [b,max_points,3], "normal_eq" float64 [b,27]), for
+    checking the stages against the oracle.
+
+    keypoints [b,nk,2] (4 <= nk <= 32, pixels as `uncertainty_pnp_batched` reads them), points_3d [nk,3] (their
+    model points, in the mesh's units) and exactly one of cov [b,nk,2,2] / weights_2d [b,nk,3] (converted through
+    `covariance_to_weights`), floating-point CUDA tensors on the poses' device: each step then minimises
+    (1/n) sum |pi(R X_i + t) - c_i|^2 + (keypoint_weight / nk) sum |W_k (pi(R P_k + t) - x_k)|^2, and a round is
+    undone when C = mean pair distance + keypoint_weight * mean_k |W_k e_k| rose (DESIGN.md §27).  return_info then
+    adds "cost_before" and "cost_after" (float64, C at the input pose and at the returned one), and trace adds
+    "keypoint_eq" (float64 [b,27], the first step's keypoint sums, unscaled)."""
+    dev, b, h, w, near, far, rounds, gate, max_points = _check_common(mask, poses, K, vertices, faces, near, far,
+                                                                      rounds, gate, max_points, 3)
 
     kpt = None
     if keypoints is not None:
@@ -143,14 +165,7 @@ def refine_poses(mask, poses, K, vertices, faces, near, far, rounds=8, gate=20.0
     elif points_3d is not None or cov is not None or weights_2d is not None:
         raise ValueError("points_3d, cov and weights_2d go with keypoints")
 
-    nv, nf = int(vertices.shape[0]), int(faces.shape[0])
-    m = mask.view(torch.uint8) if mask.dtype in (torch.uint8, torch.bool) else (mask != 0).to(torch.uint8)
-    m = m.contiguous()
-    p = poses.contiguous().double()
-    k = K.contiguous().float()
-    v = vertices.contiguous().float()
-    # an index beyond int32 is out of range either way; the clamp keeps it so
-    f = faces.contiguous() if faces.dtype == torch.int32 else faces.clamp(-1, nv).to(torch.int32).contiguous()
+    m, p, k, v, f, nv, nf = _device_inputs(mask, poses, K, vertices, faces)
     out = torch.empty((b, 3, 4), dtype=torch.float64, device=dev)
     info = torch.empty((b, 2), dtype=torch.int32, device=dev) if return_info else None
     dist = torch.empty((b, 2), dtype=torch.float64, device=dev) if return_info else None
@@ -193,6 +208,78 @@ def refine_poses(mask, poses, K, vertices, faces, near, far, rounds=8, gate=20.0
         res += (dict(status=info[:, 0], pairs=info[:, 1], dist_before=dist[:, 0], dist_after=dist[:, 1]),)
         if cost is not None:
             res[-1].update(cost_before=cost[:, 0], cost_after=cost[:, 1])
+    if trace:
+        res += (tr,)
+    return res[0] if len(res) == 1 else res
+
+
+def refine_poses_depth(mask, depth, poses, K, vertices, faces, near, far, gate, rounds=8, max_points=4096,
+                       depth_scale=1.0, return_info=False, trace=False):
+    """Refine b poses of one mesh so its rendered surface meets each registered depth image (DESIGN.md §28).
+
+    mask, poses, K, vertices, faces, near, far, rounds and max_points as for `refine_poses`.  depth [b,H,W] on the
+    poses' device: float32 in the poses' units, or uint16 (the LINEMOD PNG format) read as fp32(d) * fp32(depth_scale)
+    (depth_scale is only read for uint16); a value <= 0 or not finite is no reading.  Each round pairs every pixel
+    that the render covers, the mask holds and the sensor read (with its four 4-neighbours in the image, the mask and
+    read, for the observed normal), drops pairs whose rendered and observed points lie more than `gate` apart (in the
+    poses' units; there is no default, as there is none for near and far), keeps at most `max_points` (every
+    ceil(n / max_points)-th) and takes damped Gauss-Newton steps on sum (n . (R X + t - Y))^2.  A call is a fixed
+    sequence of launches, with no host synchronisation, and can be captured in a CUDA graph.  rounds = 0 returns the
+    input.
+
+    -> poses float64 [b,3,4] on the device.  return_info: also a dict of [b] tensors, "status" (int32 bits, the
+    module's constants: NO_CONTOUR is an empty mask, NO_SILHOUETTE a render that covers nothing, FEW_PAIRS fewer than
+    6 pairs at the input pose, which includes no readings), "pairs" (int32, the pairs of the last round that took its
+    steps), "dist_before" and "dist_after" (float64, the mean |n . (R X + t - Y)| in the poses' units at the input
+    pose and at the returned one, NaN without pairs).  trace: also a dict of the first round's pairs ("pair_idx"
+    int32 [b,max_points] pixel indices, "counts" int32 [b,4]: pairs kept, pairs before the stride, mask pixels,
+    covered pixels; "X", "Y", "n" float64 [b,max_points,3]; "normal_eq" float64 [b,27]), for checking the stages
+    against the oracle."""
+    dev, b, h, w, near, far, rounds, gate, max_points = _check_common(mask, poses, K, vertices, faces, near, far,
+                                                                      rounds, gate, max_points, 9)
+    if not isinstance(depth, torch.Tensor):
+        raise ValueError(f"depth must be a torch tensor, got {type(depth).__name__}")
+    if depth.device != dev:
+        raise ValueError(f"depth must be on the poses' device {dev}, got {depth.device}")
+    if tuple(depth.shape) != (b, h, w):
+        raise ValueError(f"depth must be [{b},{h},{w}], got {tuple(depth.shape)}")
+    if depth.dtype not in (torch.float32, torch.uint16):
+        raise ValueError(f"depth must be float32 or uint16, got {depth.dtype}")
+    is_u16 = depth.dtype == torch.uint16
+    scale = float(depth_scale)
+    if not 0 < scale < math.inf:
+        raise ValueError(f"depth_scale must be positive and finite, got {depth_scale}")
+    m, p, k, v, f, nv, nf = _device_inputs(mask, poses, K, vertices, faces)
+    d = depth.contiguous()
+    out = torch.empty((b, 3, 4), dtype=torch.float64, device=dev)
+    info = torch.empty((b, 2), dtype=torch.int32, device=dev) if return_info else None
+    dist = torch.empty((b, 2), dtype=torch.float64, device=dev) if return_info else None
+    tr, tr_struct = None, None
+    if trace:
+        tr = dict(pair_idx=torch.full((b, max_points), -1, dtype=torch.int32, device=dev),
+                  counts=torch.zeros((b, 4), dtype=torch.int32, device=dev),
+                  X=torch.zeros((b, max_points, 3), dtype=torch.float64, device=dev),
+                  Y=torch.zeros((b, max_points, 3), dtype=torch.float64, device=dev),
+                  n=torch.zeros((b, max_points, 3), dtype=torch.float64, device=dev),
+                  normal_eq=torch.full((b, 27), math.nan, dtype=torch.float64, device=dev))
+        tr_struct = _native.RefineDepthTrace(*(tr[x].data_ptr() for x in ("pair_idx", "counts", "X", "Y", "n",
+                                                                          "normal_eq")))
+    L = _native.lib()
+    with torch.cuda.device(dev):
+        need = ctypes.c_size_t()
+        _native.check(L.pvnet_refine_depth_workspace_bytes(b, h, w, max_points, ctypes.byref(need)),
+                      "pvnet_refine_depth_workspace_bytes")
+        ws = torch.empty(need.value, dtype=torch.uint8, device=dev)
+        stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+        _native.check(L.pvnet_refine_poses_depth(
+            m.data_ptr(), d.data_ptr(), int(is_u16), scale, p.data_ptr(), k.data_ptr(), int(k.dim() == 3),
+            v.data_ptr() if nv else None, f.data_ptr() if nf else None, nv, nf, b, h, w, near, far, rounds, gate,
+            max_points, out.data_ptr(), None if info is None else info.data_ptr(),
+            None if dist is None else dist.data_ptr(), None if tr_struct is None else ctypes.byref(tr_struct),
+            ws.data_ptr(), need.value, stream), "pvnet_refine_poses_depth")
+    res = (out,)
+    if return_info:
+        res += (dict(status=info[:, 0], pairs=info[:, 1], dist_before=dist[:, 0], dist_after=dist[:, 1]),)
     if trace:
         res += (tr,)
     return res[0] if len(res) == 1 else res
