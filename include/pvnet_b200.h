@@ -218,6 +218,72 @@ PVNET_API int pvnet_ransac_voting_pipeline(const void *mask, int mask_elem_size,
                                            int32_t *out_cov_counts, float *out_cov_hyp, int32_t *out_tn,
                                            void *workspace, size_t workspace_bytes, pvnet_stream_t stream);
 
+/* Workspace of pvnet_ransac_voting_center: O(b*h*w), independent of max_instances. */
+PVNET_API int pvnet_center_workspace_bytes(int b, int h, int w, int hn, size_t *bytes);
+
+/* ransac_voting_center (ransac_voting_gpu.py:600-667), which the reference leaves unfinished: finds up to
+ * max_instances object centres per image in a centre vector field and splits the foreground into instances
+ * (DESIGN.md section 29).  Per image, with I = max_instances:
+ *   R_0 = the foreground pixels (low byte nonzero, as v3 reads the mask) in row-major order; nothing is
+ *   subsampled.  For i = 0..I-1: t = |R_i|; stop if t < min_num.  Hypotheses of the pairs
+ *   idxs[b,i,m] mod t of R_i (v3's bit-exact sequence), counted over R_i with v3's exact predicate; the
+ *   winner is the lowest index with the highest count; stop if that count is < min_num.  Centre c_i = v3's
+ *   fp64 least-squares refit over the winner's inliers S_i, or the winning hypothesis where the refit is
+ *   not finite.  R_{i+1} = R_i without S_i, in order; num = i+1.
+ *   Then every foreground pixel gets 1 + the j < num with the highest cosine value (the reference's `ang`,
+ *   exact) among the centres it is an inlier of, lowest j on ties; 0 where it is an inlier of none, and for
+ *   background.
+ *
+ *   field        f32, logically [b,h,w,2], read in place through field_strides (elements): the last
+ *                keypoint channel of the permuted NCHW head output works without a copy
+ *   idxs         int32 [b,I,hn,2], or NULL to draw on the device from rng_state (Philox4x32-10, stream 3,
+ *                item i*hn + m; the call then advances the offset)
+ *   max_instances 1..32; min_num >= 1
+ *   out_labels   int32 [b,h,w]; out_num int32 [b]; out_centers f32 [b,I,2], zeros beyond num
+ *   out_counts int32 [b,I,hn], out_hyp f32 [b,I,hn,2], out_tn int32 [b,I] (|R_i|, 0 after a stop),
+ *   out_win_counts int32 [b,I]: optional per-iteration debug outputs, zeros where an iteration did no work.
+ * The launch count depends on (b, I) only, nothing synchronises the host, and the call can be captured in
+ * a CUDA graph.  Workspace: pvnet_center_workspace_bytes(b, h, w, hn). */
+PVNET_API int pvnet_ransac_voting_center(const void *mask, int mask_elem_size,
+                                         const float *field, const int64_t field_strides[4],
+                                         const int32_t *idxs, const unsigned long long *rng_state,
+                                         int b, int h, int w, int hn, float inlier_thresh, int min_num,
+                                         int max_instances, int32_t *out_labels, int32_t *out_num,
+                                         float *out_centers, int32_t *out_counts, float *out_hyp,
+                                         int32_t *out_tn, int32_t *out_win_counts,
+                                         void *workspace, size_t workspace_bytes, pvnet_stream_t stream);
+
+/* Workspace of pvnet_ransac_voting_labels for b images of h x w, vn keypoints, num_labels labels and hn_total =
+ * hn + cov_rounds*cov_hn hypotheses per keypoint.  The pixel and field lists are those of b images, not of
+ * b*num_labels: each image's list holds all of its labels' pixels once. */
+PVNET_API int pvnet_labels_workspace_bytes(int b, int h, int w, int vn, int num_labels, int hn_total, size_t *bytes);
+
+/* pvnet_ransac_voting_pipeline for every label of a label map (DESIGN.md section 29), e.g. the instance map of
+ * pvnet_ransac_voting_center.  For every image bi and label j < num_labels (1..32, b*num_labels <= 1024) the outputs
+ * at [bi, j] are bit-identical to those of pvnet_ransac_voting_pipeline(mask = (labels[bi] == j+1) as uint8 with
+ * PVNET_MASK_NONZERO_BYTE, vertex[bi], idxs[bi, j], cov_idxs[bi, j], selection[bi], the same parameters) on one
+ * image: the min_num skip, the max_num subsampling with max_num / (pixels of label j) and the covariance included.
+ * Each image's list is written grouped by label, row-major within a label, and the vector field is gathered once.
+ *
+ *   labels     integer [b,h,w] of any element size; value j+1 is label j, other values are ignored
+ *   idxs       int32 [b,num_labels,hn,vn,2] or NULL; cov_idxs int32 [b,num_labels,cov_rounds*cov_hn,vn,2] or NULL;
+ *              selection f32 [b,h,w] or NULL (one field for every label of an image); rng_state as for the pipeline
+ *              (the draws of (bi, j) are those of image bi*num_labels + j)
+ *   out_pts    f32 [b,num_labels,vn,2]; out_cov f32 [b,num_labels,vn,2,2] or NULL to skip the covariance
+ *   out_counts/out_hyp [b,num_labels,hn,vn(,2)], out_cov_counts/out_cov_hyp [b,num_labels,cov_rounds*cov_hn,vn(,2)],
+ *   out_tn [b,num_labels]: optional debug outputs.
+ *   Workspace: pvnet_labels_workspace_bytes(b, h, w, vn, num_labels, hn + cov_rounds*cov_hn). */
+PVNET_API int pvnet_ransac_voting_labels(const void *labels, int labels_elem_size, int num_labels,
+                                         const float *vertex, const int64_t vertex_strides[5],
+                                         const int32_t *idxs, const int32_t *cov_idxs, const float *selection,
+                                         const unsigned long long *rng_state,
+                                         int b, int h, int w, int vn, int hn, float inlier_thresh,
+                                         int cov_hn, int cov_rounds, int cov_min_hyp_num, float cov_inlier_thresh,
+                                         int min_num, int max_num, float *out_pts, float *out_cov,
+                                         int32_t *out_counts, float *out_hyp,
+                                         int32_t *out_cov_counts, float *out_cov_hyp, int32_t *out_tn,
+                                         void *workspace, size_t workspace_bytes, pvnet_stream_t stream);
+
 /* 1:1 stand-ins for the reference extension's two functions, same layouts:
  * direct [tn,vn,2] f32, coords [tn,2] f32 (x,y), idxs [hn,vn,2] i32, hypo [hn,vn,2] f32.
  * pvnet_generate_hypothesis writes every element of hypo (degenerate pairs -> (0,0),

@@ -5,7 +5,9 @@ from pvnet_b200.ransac_voting_gpu import (  # noqa: F401
     estimate_voting_distribution_with_mean,
     generate_hypothesis,
     ransac_motion_voting,
+    ransac_voting_center,
     ransac_voting_hypothesis,
+    ransac_voting_labels,
     ransac_voting_layer,
     ransac_voting_layer_v2,
     ransac_voting_layer_v3,

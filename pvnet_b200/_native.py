@@ -74,6 +74,15 @@ SIGNATURES = {
     "pvnet_vote_cov_with_mean": (c_int, [c_void_p, c_int, c_void_p, c_int64_p, c_void_p, c_void_p, c_void_p,
                                          c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_int, c_int,
                                          c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "pvnet_center_workspace_bytes": (c_int, [c_int, c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
+    "pvnet_ransac_voting_center": (c_int, [c_void_p, c_int, c_void_p, c_int64_p, c_void_p, c_void_p, c_int, c_int,
+                                           c_int, c_int, c_float, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                                           c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "pvnet_labels_workspace_bytes": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
+    "pvnet_ransac_voting_labels": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int64_p, c_void_p, c_void_p, c_void_p,
+                                           c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_int, c_int, c_int,
+                                           c_float, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                           c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "pvnet_ransac_voting_pipeline": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int64_p, c_void_p, c_void_p, c_void_p,
                                              c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_int, c_int, c_int,
                                              c_float, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,

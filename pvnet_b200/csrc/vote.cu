@@ -156,7 +156,7 @@ __device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k)
     }
     return c;
 }
-enum { RNG_SELECTION = 0, RNG_IDXS_V3 = 1, RNG_IDXS_COV = 2 };
+enum { RNG_SELECTION = 0, RNG_IDXS_V3 = 1, RNG_IDXS_COV = 2, RNG_IDXS_CENTER = 3 };
 __device__ __forceinline__ uint4 rng_draw(const unsigned long long *__restrict__ rng_state, unsigned item,
                                           unsigned image, unsigned stream)
 {
@@ -348,11 +348,19 @@ __global__ void __launch_bounds__(256)
 // ------------------------------------------------------------------ hypotheses
 // idxs [b,hn,vn,2] (or the device RNG) -> hyp [b][vn][HT] at column h_off + h (keypoint-major so a
 // vote CTA reads one row).  Samples index the compact direct list.
+// SEG (pvnet_ransac_voting_labels): b is a virtual image (field image b / seg_div, one label of it) whose list is the
+// segment starting at seg_off[b] of its field image's lists; without SEG seg_off / seg_div are unused.
+template <bool SEG>
+__device__ __forceinline__ int seg_image(int b, int seg_div) { return SEG ? b / seg_div : b; }
+template <bool SEG>
+__device__ __forceinline__ int seg_start(const int *seg_off, int b) { return SEG ? seg_off[b] : 0; }
+
+template <bool SEG>
 __global__ void __launch_bounds__(256)
     k_gen_hyp(const float2 *__restrict__ direct, const int *__restrict__ idxs,
               const unsigned long long *__restrict__ rng_state, int rng_stream, const unsigned *__restrict__ pix,
               const int *__restrict__ tn_arr, int npx, int cap, int vn, int hn, int HT, int h_off,
-              float2 *__restrict__ hyp)
+              float2 *__restrict__ hyp, const int *__restrict__ seg_off, int seg_div)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     const int b = blockIdx.y;
@@ -371,8 +379,12 @@ __global__ void __launch_bounds__(256)
             t0 = r.x % (unsigned)tn;
             t1 = r.y % (unsigned)tn;
         }
-        const unsigned p0 = pix[(size_t)b * npx + t0], p1 = pix[(size_t)b * npx + t1];
-        const float2 d0 = direct[((size_t)b * vn + vi) * cap + t0], d1 = direct[((size_t)b * vn + vi) * cap + t1];
+        const int fb = seg_image<SEG>(b, seg_div);
+        const int so = seg_start<SEG>(seg_off, b);
+        const unsigned *pb = pix + (size_t)fb * npx + so;
+        const float2 *db = direct + ((size_t)fb * vn + vi) * cap + so;
+        const unsigned p0 = pb[t0], p1 = pb[t1];
+        const float2 d0 = db[t0], d1 = db[t1];
         out = exact_hypothesis(d0.x, d0.y, (float)(p0 & 0xffff), (float)(p0 >> 16), d1.x, d1.y, (float)(p1 & 0xffff),
                                (float)(p1 >> 16));
     }
@@ -440,11 +452,12 @@ __device__ __forceinline__ float min3_nan_abs(float a, float b, float c)     // 
     return r;
 }
 
-template <int HPL>
+template <int HPL, bool SEGMENTED>
 __global__ void __launch_bounds__(VT_THREADS, HPL > 4 ? 2 : 3)
     k_vote3(const unsigned *__restrict__ pix, const float2 *__restrict__ direct, const int *__restrict__ tn_arr, int npx,
             int cap, int nb, int vn, int hn, int HT, int h0, const float2 *__restrict__ hyp, int *__restrict__ counts,
-            unsigned *__restrict__ ticket, float thresh, float sn, float cs, float beta, float b0, int items_per_warp)
+            unsigned *__restrict__ ticket, float thresh, float sn, float cs, float beta, float b0, int items_per_warp,
+            const int *__restrict__ seg_off, int seg_div)
 {
     constexpr int G = 4;                      // pixels per unrolled step of the sweep
     static_assert(G % 2 == 0 && VT_SUB % G == 0, "pixels are swept in pairs");
@@ -498,8 +511,10 @@ __global__ void __launch_bounds__(VT_THREADS, HPL > 4 ? 2 : 3)
         const int tn = tn_arr[b];
         const int t0 = (g - seg_prefix[b]) * SEG;
         const int len = min(SEG, tn - t0);
-        const unsigned *pix_t = pix + (size_t)b * npx + t0;
-        const float2 *dir_t = direct + ((size_t)b * vn + k) * cap + t0;
+        const int fb = seg_image<SEGMENTED>(b, seg_div);
+        const int so = seg_start<SEGMENTED>(seg_off, b) + t0;
+        const unsigned *pix_t = pix + (size_t)fb * npx + so;
+        const float2 *dir_t = direct + ((size_t)fb * vn + k) * cap + so;
 
         const int hbase = hc * HC;
         const float2 *hyp_row = hyp + ((size_t)b * vn + k) * HT + h0;
@@ -688,11 +703,12 @@ __device__ __forceinline__ double warp_sum_d(double v)
 // (torch.max, ransac_voting_gpu.py:562); kept only if its count is > 0 (:567).  Then the
 // inliers of the winner (:582-584) feed  sum n n^T  and  sum n (n.c),  n = (d_y,-d_x)
 // (:579-593), accumulated in fp64.
+template <bool SEG>
 __global__ void __launch_bounds__(RF_THREADS)
     k_refit(const float2 *__restrict__ direct, int cap, const unsigned *__restrict__ pix,
             const int *__restrict__ tn_arr, int npx, int vn, int hn, int HT, const float2 *__restrict__ hyp,
             const int *__restrict__ counts, float thresh, double *__restrict__ part, float2 *__restrict__ win,
-            const float2 *__restrict__ win_in)
+            const float2 *__restrict__ win_in, const int *__restrict__ seg_off, int seg_div)
 {
     __shared__ unsigned long long s_key[RF_THREADS / 32];
     __shared__ double s_acc[RF_THREADS / 32][5];
@@ -730,10 +746,15 @@ __global__ void __launch_bounds__(RF_THREADS)
     const int per = (tn + RF_CHUNKS - 1) / RF_CHUNKS;
     const int lo = rc * per, hi = min(tn, lo + per);
     const float2 *dir_k = direct + (size_t)bk * cap;
-    (void)k;
+    size_t pix_b = (size_t)b * npx;
+    if (SEG) {
+        const int so = seg_start<SEG>(seg_off, b), fb = seg_image<SEG>(b, seg_div);
+        dir_k = direct + ((size_t)fb * vn + k) * cap + so;
+        pix_b = (size_t)fb * npx + so;
+    }
     double a00 = 0, a01 = 0, a11 = 0, b0 = 0, b1 = 0;
     for (int t = lo + tid; t < hi; t += RF_THREADS) {
-        const unsigned p = pix[(size_t)b * npx + t];
+        const unsigned p = pix[pix_b + t];
         const int x = p & 0xffff, y = p >> 16;
         const float2 dv = dir_k[t];
         const float dxv = dv.x, dyv = dv.y;
@@ -1179,6 +1200,385 @@ __global__ void __launch_bounds__(256)
     }
 }
 
+// ------------------------------------------------------------------ instance centres (ransac_voting_center)
+// The centre search of DESIGN.md section 29 runs I iterations over the remaining list R_i of each image.  The
+// hypothesis, vote and refit passes are the v3 ones on a one-keypoint field (vn = 1) whose lists are R_i; the
+// kernels below make the hypotheses from the per-iteration samples, decide each image's winner and cut its
+// inliers out of R_i with a stable filter into the other of two list buffers.  An image that has stopped keeps
+// alive = 0 and a work length of 0, so every later launch skips it.
+
+// the reference's cosine value `ang` of exact_inlier's sequence; false where its norm test rejects the pair.  The
+// same instructions as exact_inlier, kept as a second copy so that the kernels built on exact_inlier compile to
+// exactly the SASS they had; tests/test_instance_vote_cpu.py and the label-map parity test pin the two together.
+__device__ __forceinline__ bool exact_cosine(float nx, float ny, float cx, float cy, float hx, float hy, float &ang)
+{
+    const float dx = __fsub_rn(hx, cx);
+    const float dy = __fsub_rn(hy, cy);
+    const float norm1 = __fsqrt_rn(__fmaf_rn(nx, nx, __fmul_rn(ny, ny)));
+    const float norm2 = __fsqrt_rn(__fmaf_rn(dx, dx, __fmul_rn(dy, dy)));
+    if (fmin((double)norm1, (double)norm2) < 1e-6) return false;
+    ang = __fdiv_rn(__fmaf_rn(dx, nx, __fmul_rn(dy, ny)), __fmul_rn(norm1, norm2));
+    return true;
+}
+
+__global__ void k_center_init(int nb, int *__restrict__ alive, int *__restrict__ num)
+{
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= nb) return;
+    alive[b] = 1;
+    num[b] = 0;
+}
+
+// iteration `it`: work[b] = |R_i| if the image still runs and |R_i| >= min_num, else 0; hypotheses of the
+// pairs idxs[b,it,m] mod |R_i| (or Philox draws, item it*hn + m of stream RNG_IDXS_CENTER)
+__global__ void __launch_bounds__(256)
+    k_center_hyp(const float2 *__restrict__ direct, const unsigned *__restrict__ pix, const int *__restrict__ tn_arr,
+                 const int *__restrict__ alive, int npx, int cap, const int *__restrict__ idxs,
+                 const unsigned long long *__restrict__ rng_state, int I, int it, int hn, int min_num,
+                 int *__restrict__ work, float2 *__restrict__ hyp, int *__restrict__ dbg_tn)
+{
+    const int m = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
+    const int t = alive[b] ? tn_arr[b] : 0;
+    const bool active = t > 0 && t >= min_num;
+    if (m == 0) {
+        work[b] = active ? t : 0;
+        if (dbg_tn) dbg_tn[b * I + it] = t;
+    }
+    if (m >= hn) return;
+    float2 out = make_float2(0.f, 0.f);
+    if (active) {
+        unsigned t0, t1;
+        if (idxs) {
+            const size_t ib = (((size_t)b * I + it) * hn + m) * 2;
+            t0 = (unsigned)idxs[ib] % (unsigned)t;
+            t1 = (unsigned)idxs[ib + 1] % (unsigned)t;
+        } else {
+            const uint4 r = rng_draw(rng_state, (unsigned)(it * hn + m), (unsigned)b, RNG_IDXS_CENTER);
+            t0 = r.x % (unsigned)t;
+            t1 = r.y % (unsigned)t;
+        }
+        const unsigned p0 = pix[(size_t)b * npx + t0], p1 = pix[(size_t)b * npx + t1];
+        const float2 d0 = direct[(size_t)b * cap + t0], d1 = direct[(size_t)b * cap + t1];
+        out = exact_hypothesis(d0.x, d0.y, (float)(p0 & 0xffff), (float)(p0 >> 16), d1.x, d1.y, (float)(p1 & 0xffff),
+                               (float)(p1 >> 16));
+    }
+    hyp[(size_t)b * hn + m] = out;
+}
+
+// block per image: the winner (highest count, lowest index), the stop rule and the centre (the refit, or the
+// winning hypothesis where the refit is not finite); copies the iteration's debug rows
+__global__ void __launch_bounds__(256)
+    k_center_decide(const int *__restrict__ counts, const float2 *__restrict__ hyp, const int *__restrict__ work,
+                    const float *__restrict__ refit, int hn, int I, int it, int min_num, int *__restrict__ alive,
+                    int *__restrict__ num, float *__restrict__ centers, int *__restrict__ dbg_counts,
+                    float *__restrict__ dbg_hyp, int *__restrict__ dbg_win)
+{
+    __shared__ unsigned long long s_key[8];
+    const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    unsigned long long key = 0;
+    for (int h = tid; h < hn; h += blockDim.x) {
+        const unsigned c = (unsigned)counts[(size_t)b * hn + h];
+        const unsigned long long kk = ((unsigned long long)c << 32) | (unsigned long long)(0xffffffffu - (unsigned)h);
+        key = kk > key ? kk : key;
+        if (dbg_counts) dbg_counts[((size_t)b * I + it) * hn + h] = (int)c;
+        if (dbg_hyp) {
+            const float2 v = hyp[(size_t)b * hn + h];
+            dbg_hyp[(((size_t)b * I + it) * hn + h) * 2] = v.x;
+            dbg_hyp[(((size_t)b * I + it) * hn + h) * 2 + 1] = v.y;
+        }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const unsigned long long other = __shfl_xor_sync(0xffffffffu, key, o);
+        key = other > key ? other : key;
+    }
+    if (lane == 0) s_key[warp] = key;
+    __syncthreads();
+    if (tid) return;
+    for (int i = 1; i < (int)(blockDim.x >> 5); ++i) key = s_key[i] > key ? s_key[i] : key;
+    const int best = (int)(key >> 32);
+    const int best_h = (int)(0xffffffffu - (unsigned)(key & 0xffffffffu));
+    if (dbg_win) dbg_win[b * I + it] = work[b] ? best : 0;
+    if (!work[b] || best < min_num) {
+        alive[b] = 0;
+        return;
+    }
+    float cx = refit[2 * b], cy = refit[2 * b + 1];
+    if (!(isfinite(cx) && isfinite(cy))) {
+        const float2 wp = hyp[(size_t)b * hn + best_h];
+        cx = wp.x;
+        cy = wp.y;
+    }
+    centers[((size_t)b * I + it) * 2] = cx;
+    centers[((size_t)b * I + it) * 2 + 1] = cy;
+    num[b] = it + 1;
+}
+
+// R_{i+1} = R_i without the winner's inliers, stable.  Pass 1: survivors per 2048-entry chunk of the list.
+__global__ void __launch_bounds__(CH_THREADS)
+    k_center_filter_count(const unsigned *__restrict__ pix, const float2 *__restrict__ direct,
+                          const int *__restrict__ work, const int *__restrict__ alive, const float2 *__restrict__ win,
+                          int npx, int cap, int nchunk, float thresh, int *__restrict__ chunk_cnt)
+{
+    __shared__ int scratch[96];
+    const int c = blockIdx.x, b = blockIdx.y;
+    const int t = alive[b] ? work[b] : 0;
+    const int base = c * CH_PX + threadIdx.x * 8;
+    if (c * CH_PX >= t) {
+        if (threadIdx.x == 0) chunk_cnt[b * nchunk + c] = 0;
+        return;
+    }
+    const float2 wp = win[b];
+    int cnt = 0, z0 = 0, z1 = 0;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        const int i = base + j;
+        if (i < t) {
+            const unsigned p = pix[(size_t)b * npx + i];
+            const float2 d = direct[(size_t)b * cap + i];
+            cnt += exact_inlier(d.x, d.y, (float)(p & 0xffff), (float)(p >> 16), wp.x, wp.y, thresh) ? 0 : 1;
+        }
+    }
+    block_sum3(cnt, z0, z1, scratch);
+    if (threadIdx.x == 0) chunk_cnt[b * nchunk + c] = cnt;
+}
+
+// pass 2: write the survivors in list order into the other buffer; tn_next[b] = their number (0 once stopped)
+__global__ void __launch_bounds__(CH_THREADS)
+    k_center_filter_write(const unsigned *__restrict__ pix, const float2 *__restrict__ direct,
+                          const int *__restrict__ work, const int *__restrict__ alive, const float2 *__restrict__ win,
+                          int npx, int cap, int nchunk, float thresh, const int *__restrict__ chunk_cnt,
+                          unsigned *__restrict__ pix_next, float2 *__restrict__ dir_next, int *__restrict__ tn_next)
+{
+    __shared__ int scratch[96];
+    __shared__ int warp_off[CH_THREADS / 32];
+    const int c = blockIdx.x, b = blockIdx.y;
+    int tot = 0, prefix = 0, z = 0;
+    for (int i = threadIdx.x; i < nchunk; i += blockDim.x) {
+        const int k = chunk_cnt[b * nchunk + i];
+        tot += k;
+        if (i < c) prefix += k;
+    }
+    block_sum3(tot, prefix, z, scratch);
+    if (c == 0 && threadIdx.x == 0) tn_next[b] = tot;
+    if (chunk_cnt[b * nchunk + c] == 0) return;
+    const int t = work[b];
+    const float2 wp = win[b];
+    const int base = c * CH_PX + threadIdx.x * 8;
+    unsigned flags = 0;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        const int i = base + j;
+        if (i < t) {
+            const unsigned p = pix[(size_t)b * npx + i];
+            const float2 d = direct[(size_t)b * cap + i];
+            if (!exact_inlier(d.x, d.y, (float)(p & 0xffff), (float)(p >> 16), wp.x, wp.y, thresh)) flags |= 1u << j;
+        }
+    }
+    const int mine = __popc(flags);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    int inc = mine;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const int v = __shfl_up_sync(0xffffffffu, inc, o);
+        if (lane >= o) inc += v;
+    }
+    if (lane == 31) warp_off[warp] = inc;
+    __syncthreads();
+    int woff = 0;
+    for (int i = 0; i < warp; ++i) woff += warp_off[i];
+    int r = prefix + woff + inc - mine;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        if (flags & (1u << j)) {
+            const int i = base + j;
+            pix_next[(size_t)b * npx + r] = pix[(size_t)b * npx + i];
+            dir_next[(size_t)b * cap + r] = direct[(size_t)b * cap + i];
+            ++r;
+        }
+    }
+}
+
+// thread per pixel: label = 1 + the centre with the highest cosine among those the pixel is an inlier of
+// (lowest index on ties), 0 for background and for a pixel that is an inlier of no centre
+template <typename T>
+__global__ void __launch_bounds__(256)
+    k_center_assign(const T *__restrict__ mask, const float *__restrict__ field, Strides st, const int *__restrict__ num,
+                    const float *__restrict__ centers, int I, int npx, int width, float thresh,
+                    int *__restrict__ labels)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
+    if (i >= npx) return;
+    int label = 0;
+    if (is_foreground(mask[(size_t)b * npx + i], PVNET_MASK_NONZERO_BYTE)) {
+        const int y = i / width, x = i - y * width;
+        const long long off = (long long)b * st.s[0] + (long long)y * st.s[1] + (long long)x * st.s[2];
+        const float nx = __ldg(field + off), ny = __ldg(field + off + st.s[4]);
+        const int n = num[b];
+        float best = 0.f;
+        for (int j = 0; j < n; ++j) {
+            float ang;
+            const float cx = centers[((size_t)b * I + j) * 2], cy = centers[((size_t)b * I + j) * 2 + 1];
+            if (exact_cosine(nx, ny, (float)x, (float)y, cx, cy, ang) && ang > thresh && (label == 0 || ang > best)) {
+                best = ang;
+                label = j + 1;
+            }
+        }
+    }
+    labels[(size_t)b * npx + i] = label;
+}
+
+// ------------------------------------------------------------------ label maps (pvnet_ransac_voting_labels)
+// Each image's list is written grouped by label, row-major within a label: label j of image b is the segment
+// [seg_off[b*L+j], seg_off[b*L+j] + tn[b*L+j]) of image b's list, kept exactly as a one-label pipeline call on
+// (labels[b] == j+1) keeps its pixels (min_num skip, max_num subsampling with max_num / fg_label).
+// pass 1: pixels of every label in every 2048-pixel chunk
+template <typename T>
+__global__ void __launch_bounds__(CH_THREADS)
+    k_label_count(const T *__restrict__ labels, int npx, int nchunk, int L, int *__restrict__ lab_cnt)
+{
+    __shared__ int s_cnt[32];
+    const int c = blockIdx.x, b = blockIdx.y;
+    if (threadIdx.x < 32) s_cnt[threadIdx.x] = 0;
+    __syncthreads();
+    const T *m = labels + (size_t)b * npx;
+    const int base = c * CH_PX + threadIdx.x * 8;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        const int i = base + j;
+        if (i < npx) {
+            const long long v = (long long)m[i];
+            if (v >= 1 && v <= L) atomicAdd(&s_cnt[v - 1], 1);
+        }
+    }
+    __syncthreads();
+    if (threadIdx.x < L) lab_cnt[((size_t)b * L + threadIdx.x) * nchunk + c] = s_cnt[threadIdx.x];
+}
+
+// per-label totals of a chunk table [b][L][nchunk] (every thread gets all L of image b), into s_tot
+__device__ __forceinline__ void label_totals(const int *__restrict__ tab, int b, int L, int nchunk, int c, int *s_tot,
+                                             int *s_pre)
+{
+    if (threadIdx.x < 32) {
+        s_tot[threadIdx.x] = 0;
+        if (s_pre) s_pre[threadIdx.x] = 0;
+    }
+    __syncthreads();
+    for (int e = threadIdx.x; e < L * nchunk; e += blockDim.x) {
+        const int j = e / nchunk, i = e - j * nchunk;
+        const int v = tab[((size_t)b * L + j) * nchunk + i];
+        if (v) {
+            atomicAdd(&s_tot[j], v);
+            if (s_pre && i < c) atomicAdd(&s_pre[j], v);
+        }
+    }
+    __syncthreads();
+}
+
+// pass 2: kept pixels of every label in every chunk
+template <typename T>
+__global__ void __launch_bounds__(CH_THREADS)
+    k_label_kept(const T *__restrict__ labels, const float *__restrict__ selection,
+                 const unsigned long long *__restrict__ rng_state, int npx, int nchunk, int L, int min_num,
+                 int max_num, const int *__restrict__ lab_cnt, int *__restrict__ lab_kept)
+{
+    __shared__ int s_fg[32], s_kept[32];
+    const int c = blockIdx.x, b = blockIdx.y;
+    label_totals(lab_cnt, b, L, nchunk, c, s_fg, nullptr);
+    const bool have_sel = selection != nullptr || rng_state != nullptr;
+    if (threadIdx.x < 32) s_kept[threadIdx.x] = 0;
+    __syncthreads();
+    const T *m = labels + (size_t)b * npx;
+    const int base = c * CH_PX + threadIdx.x * 8;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        const int i = base + j;
+        if (i < npx) {
+            const long long v = (long long)m[i];
+            if (v >= 1 && v <= L) {
+                const int fg = s_fg[v - 1];
+                bool keep = fg >= min_num;
+                if (keep && fg > max_num && have_sel)
+                    keep = selection_value(selection, rng_state, b, npx, i) < subsample_p(fg, max_num);
+                if (keep) atomicAdd(&s_kept[v - 1], 1);
+            }
+        }
+    }
+    __syncthreads();
+    if (threadIdx.x < L) lab_kept[((size_t)b * L + threadIdx.x) * nchunk + c] = s_kept[threadIdx.x];
+}
+
+// pass 3: the grouped list; block (0, b) also writes the segment table and the per-image list length
+template <typename T>
+__global__ void __launch_bounds__(CH_THREADS)
+    k_label_write(const T *__restrict__ labels, const float *__restrict__ selection,
+                  const unsigned long long *__restrict__ rng_state, int npx, int width, int nchunk, int L,
+                  int min_num, int max_num, const int *__restrict__ lab_cnt, const int *__restrict__ lab_kept,
+                  unsigned *__restrict__ pix, int *__restrict__ vtn, int *__restrict__ seg_off,
+                  int *__restrict__ tn_img)
+{
+    __shared__ int s_fg[32], s_tot[32], s_pre[32];
+    __shared__ int warp_off[CH_THREADS / 32];
+    const int c = blockIdx.x, b = blockIdx.y;
+    label_totals(lab_cnt, b, L, nchunk, c, s_fg, nullptr);
+    label_totals(lab_kept, b, L, nchunk, c, s_tot, s_pre);
+    if (c == 0 && threadIdx.x == 0) {
+        int acc = 0;
+        for (int j = 0; j < L; ++j) {
+            vtn[b * L + j] = s_tot[j];
+            seg_off[b * L + j] = acc;
+            acc += s_tot[j];
+        }
+        tn_img[b] = acc;
+    }
+    const bool have_sel = selection != nullptr || rng_state != nullptr;
+    const T *m = labels + (size_t)b * npx;
+    const int base = c * CH_PX + threadIdx.x * 8;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    int seg = 0;
+    for (int l = 0; l < L; ++l) {
+        const int kept_here = lab_kept[((size_t)b * L + l) * nchunk + c];
+        const int start = seg + s_pre[l];
+        seg += s_tot[l];
+        if (kept_here == 0) continue;                  // uniform over the block
+        const int fg = s_fg[l];
+        const bool sub = fg > max_num && have_sel;
+        const float p = sub ? subsample_p(fg, max_num) : 0.f;
+        unsigned flags = 0;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            const int i = base + j;
+            if (i < npx && (long long)m[i] == (long long)(l + 1)) {
+                bool keep = true;
+                if (sub) keep = selection_value(selection, rng_state, b, npx, i) < p;
+                flags |= (keep ? 1u : 0u) << j;
+            }
+        }
+        const int mine = __popc(flags);
+        int inc = mine;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const int v = __shfl_up_sync(0xffffffffu, inc, o);
+            if (lane >= o) inc += v;
+        }
+        __syncthreads();                               // warp_off of the previous label is consumed
+        if (lane == 31) warp_off[warp] = inc;
+        __syncthreads();
+        int woff = 0;
+        for (int i = 0; i < warp; ++i) woff += warp_off[i];
+        int r = start + woff + inc - mine;
+        unsigned *out = pix + (size_t)b * npx;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            if (flags & (1u << j)) {
+                const int i = base + j;
+                const int y = i / width, x = i - y * width;
+                out[r++] = ((unsigned)y << 16) | (unsigned)x;
+            }
+        }
+    }
+}
+
 // ------------------------------------------------------------------ host side
 struct VoteWs {
     unsigned *pix;
@@ -1188,6 +1588,10 @@ struct VoteWs {
     double *part;
     int cap, ntile;      // per-image capacity of the compact lists (pixels, multiple of VT_TILE) and tiles
     size_t bytes;
+    // label segments (pvnet_ransac_voting_labels): image b of the scoring passes is label b % seg_div of field
+    // image b / seg_div, its lists start at seg_off[b]; nullptr = one list per field image
+    const int *seg_off = nullptr;
+    int seg_div = 1;
 };
 
 VoteWs carve(void *ws, int b, int h, int w, int vn, int hn_total)
@@ -1283,8 +1687,9 @@ int launch_gen_hyp(const Samples &sm, int rng_stream, int b, int h, int w, int v
 {
     PV_CHECK_ARG(sm.idxs || sm.rng_state, "neither idxs nor an rng state given");
     dim3 ghyp((hn * vn + 255) / 256, b);
-    k_gen_hyp<<<ghyp, 256, 0, s>>>(ws.direct, sm.idxs, sm.rng_state, rng_stream, ws.pix, ws.tn, h * w, ws.cap, vn, hn, HT,
-                                   h_off, ws.hyp);
+    (ws.seg_off ? k_gen_hyp<true> : k_gen_hyp<false>)<<<ghyp, 256, 0, s>>>(
+        ws.direct, sm.idxs, sm.rng_state, rng_stream, ws.pix, ws.tn, h * w, ws.cap, vn, hn, HT, h_off, ws.hyp,
+        ws.seg_off, ws.seg_div);
     PV_LAUNCHED("k_gen_hyp");
     return PVNET_OK;
 }
@@ -1329,9 +1734,11 @@ int launch_vote(int b, int h, int w, int vn, int hn, int HT, int h0, float thres
     const unsigned grid = (unsigned)(pvnet::sm_count() * (hpl8 ? 2 : 3));
     const int items_per_warp = 16;
     PV_CUDA(cudaMemsetAsync(ws.ticket, 0, sizeof(unsigned), s));
-    (hpl8 ? k_vote3<8> : k_vote3<4>)<<<grid, VT_THREADS, 0, s>>>(ws.pix, ws.direct, ws.tn, h * w, ws.cap, b, vn, hn, HT,
-                                                                 h0, ws.hyp, ws.counts, ws.ticket, thresh, vc.sn, vc.cs,
-                                                                 vc.beta, vc.b0, items_per_warp);
+    const bool seg = ws.seg_off != nullptr;
+    auto kern = hpl8 ? (seg ? k_vote3<8, true> : k_vote3<8, false>) : (seg ? k_vote3<4, true> : k_vote3<4, false>);
+    kern<<<grid, VT_THREADS, 0, s>>>(ws.pix, ws.direct, ws.tn, h * w, ws.cap, b, vn, hn, HT, h0, ws.hyp, ws.counts,
+                                     ws.ticket, thresh, vc.sn, vc.cs, vc.beta, vc.b0, items_per_warp, ws.seg_off,
+                                     ws.seg_div);
     PV_LAUNCHED("k_vote3");
     return PVNET_OK;
 }
@@ -1340,8 +1747,9 @@ int launch_refit(int b, int h, int w, int vn, int hn, int HT, float thresh, cons
                  cudaStream_t s, const float2 *win_in = nullptr)
 {
     dim3 grf(RF_CHUNKS, b * vn);
-    k_refit<<<grf, RF_THREADS, 0, s>>>(ws.direct, ws.cap, ws.pix, ws.tn, h * w, vn, hn, HT, ws.hyp, ws.counts, thresh,
-                                       ws.part, ws.win, win_in);
+    (ws.seg_off ? k_refit<true> : k_refit<false>)<<<grf, RF_THREADS, 0, s>>>(
+        ws.direct, ws.cap, ws.pix, ws.tn, h * w, vn, hn, HT, ws.hyp, ws.counts, thresh, ws.part, ws.win, win_in,
+        ws.seg_off, ws.seg_div);
     PV_LAUNCHED("k_refit");
     k_refit_final<<<(b * vn + 127) / 128, 128, 0, s>>>(ws.part, ws.tn, b, vn, out_pts);
     PV_LAUNCHED("k_refit_final");
@@ -1384,6 +1792,83 @@ Strides to_strides(const int64_t *vs)
     Strides st;
     for (int i = 0; i < 5; ++i) st.s[i] = vs ? vs[i] : 0;
     return st;
+}
+
+// the centre search's workspace: v3's for one keypoint, plus the second list buffer and per-image state
+struct CenterWs {
+    VoteWs v;
+    unsigned *pix2;
+    float2 *dir2;
+    int *tn2, *work, *alive;
+    float *refit;
+    size_t bytes;
+};
+
+CenterWs carve_center(void *ws, int b, int h, int w, int hn)
+{
+    CenterWs c;
+    c.v = carve(ws, b, h, w, 1, hn);
+    Carver k(ws);
+    k.off = c.v.bytes;
+    c.pix2 = k.take<unsigned>((size_t)b * h * w);
+    c.dir2 = k.take<float2>((size_t)b * c.v.cap);
+    c.tn2 = k.take<int>(b);
+    c.work = k.take<int>(b);
+    c.alive = k.take<int>(b);
+    c.refit = k.take<float>((size_t)b * 2);
+    c.bytes = pvnet::align_up(k.off, 256);
+    return c;
+}
+
+// the label vote's workspace: the lists, field and hypothesis tables of b images (the tables hold L*hn_total
+// columns, so (image, label) rows fit), plus per-(image, label) lengths, segment starts, winners and refit partials
+struct LabelsWs {
+    VoteWs v;
+    int *lab_cnt, *lab_kept, *tn_img;
+    size_t bytes;
+};
+
+LabelsWs carve_labels(void *ws, int b, int h, int w, int vn, int L, int hn_total)
+{
+    LabelsWs c;
+    const VoteWs base = carve(ws, b, h, w, vn, L * hn_total);
+    const int nchunk = (h * w + CH_PX - 1) / CH_PX;
+    Carver k(ws);
+    k.off = base.bytes;
+    c.v = base;
+    c.v.tn = k.take<int>((size_t)b * L);
+    int *seg = k.take<int>((size_t)b * L);
+    c.v.seg_off = seg;
+    c.v.seg_div = L;
+    c.v.win = k.take<float2>((size_t)b * L * vn);
+    c.v.part = k.take<double>((size_t)b * L * vn * RF_CHUNKS * 5);
+    c.lab_cnt = k.take<int>((size_t)b * L * nchunk);
+    c.lab_kept = k.take<int>((size_t)b * L * nchunk);
+    c.tn_img = k.take<int>(b);
+    c.bytes = pvnet::align_up(k.off, 256);
+    return c;
+}
+
+template <typename T>
+void launch_label_compaction(const void *labels, const Samples &sm, int b, int h, int w, int L, int min_num,
+                             int max_num, const LabelsWs &lw, cudaStream_t s)
+{
+    const int npx = h * w, nchunk = (npx + CH_PX - 1) / CH_PX;
+    dim3 grid(nchunk, b);
+    k_label_count<T><<<grid, CH_THREADS, 0, s>>>((const T *)labels, npx, nchunk, L, lw.lab_cnt);
+    k_label_kept<T><<<grid, CH_THREADS, 0, s>>>((const T *)labels, sm.selection, sm.rng_state, npx, nchunk, L, min_num,
+                                               max_num, lw.lab_cnt, lw.lab_kept);
+    k_label_write<T><<<grid, CH_THREADS, 0, s>>>((const T *)labels, sm.selection, sm.rng_state, npx, w, nchunk, L, min_num,
+                                                max_num, lw.lab_cnt, lw.lab_kept, lw.v.pix, lw.v.tn,
+                                                const_cast<int *>(lw.v.seg_off), lw.tn_img);
+}
+
+template <typename T>
+void launch_center_assign(const void *mask, const float *field, const Strides &st, const int *num,
+                          const float *centers, int b, int I, int h, int w, float thresh, int *labels, cudaStream_t s)
+{
+    dim3 grid((h * w + 255) / 256, b);
+    k_center_assign<T><<<grid, 256, 0, s>>>((const T *)mask, field, st, num, centers, I, h * w, w, thresh, labels);
 }
 
 }  // namespace
@@ -1604,6 +2089,170 @@ int pvnet_ransac_voting_pipeline(const void *mask, int mask_elem_size, int mask_
     }
     if ((rc = launch_export(ws, b, vn, hn, HT, 0, out_hyp, out_counts, out_tn, s))) return rc;
     if (with_cov && (rc = launch_export(ws, b, vn, hnt, HT, hn, out_cov_hyp, out_cov_counts, nullptr, s))) return rc;
+    if (rng_state && (!idxs || (with_cov && !cov_idxs) || !selection)) return finish_rng(Samples{nullptr, nullptr, rng_state}, s);
+    return PVNET_OK;
+}
+
+int pvnet_center_workspace_bytes(int b, int h, int w, int hn, size_t *bytes)
+{
+    PV_CHECK_ARG(bytes, "null bytes pointer");
+    PV_CHECK_ARG(b >= 1 && h >= 1 && w >= 1 && hn >= 1, "non-positive dimension");
+    PV_CHECK_ARG(b <= VT_MAX_B, "batch %d outside [1,%d]", b, VT_MAX_B);
+    PV_CHECK_ARG(h <= 65535 && w <= 65535, "image size %dx%d unsupported", h, w);
+    *bytes = carve_center(nullptr, b, h, w, hn).bytes + 256;
+    return PVNET_OK;
+}
+
+// ransac_voting_center (ransac_voting_gpu.py:600-667) finished: DESIGN.md section 29, include/pvnet_b200.h
+int pvnet_ransac_voting_center(const void *mask, int mask_elem_size, const float *field,
+                               const int64_t field_strides[4], const int32_t *idxs,
+                               const unsigned long long *rng_state, int b, int h, int w, int hn, float inlier_thresh,
+                               int min_num, int max_instances, int32_t *out_labels, int32_t *out_num,
+                               float *out_centers, int32_t *out_counts, float *out_hyp, int32_t *out_tn,
+                               int32_t *out_win_counts, void *workspace, size_t workspace_bytes,
+                               pvnet_stream_t stream)
+{
+    PV_CHECK_ARG(field_strides, "null field strides");
+    const int64_t vs[5] = {field_strides[0], field_strides[1], field_strides[2], 0, field_strides[3]};
+    int rc = check_common(mask, mask_elem_size, field, (const long long *)vs, b, h, w, 1, hn);
+    if (rc) return rc;
+    PV_CHECK_ARG(idxs || rng_state, "neither idxs nor rng_state given");
+    PV_CHECK_ARG(max_instances >= 1 && max_instances <= 32, "max_instances %d outside [1,32]", max_instances);
+    PV_CHECK_ARG(min_num >= 1, "min_num %d must be positive", min_num);
+    PV_CHECK_ARG((long long)hn * max_instances <= (1LL << 30), "too many hypotheses");
+    PV_CHECK_ARG(out_labels && out_num && out_centers, "null out_labels/out_num/out_centers");
+    const int I = max_instances, npx = h * w, nchunk = (npx + CH_PX - 1) / CH_PX;
+    const Strides st = to_strides(vs);
+    CenterWs cw = carve_center(workspace, b, h, w, hn);
+    PV_CHECK_ARG(workspace, "null workspace");
+    if (workspace_bytes < cw.bytes) {
+        pvnet::set_error("workspace %zu < %zu bytes", workspace_bytes, cw.bytes);
+        return PVNET_E_WORKSPACE;
+    }
+    cudaStream_t s = (cudaStream_t)stream;
+    // R_0: every foreground pixel in row-major order, its centre vector gathered once
+    const Samples none{nullptr, nullptr, nullptr};
+    if ((rc = launch_pixels(mask, mask_elem_size, PVNET_MASK_NONZERO_BYTE, field, st, none, b, h, w, 1, 0, 0x7fffffff,
+                            cw.v, s)))
+        return rc;
+    k_center_init<<<(b + 127) / 128, 128, 0, s>>>(b, cw.alive, out_num);
+    PV_LAUNCHED("k_center_init");
+    PV_CUDA(cudaMemsetAsync(out_centers, 0, sizeof(float) * 2 * (size_t)b * I, s));
+    unsigned *pix[2] = {cw.v.pix, cw.pix2};
+    float2 *dir[2] = {cw.v.direct, cw.dir2};
+    int *tn[2] = {cw.v.tn, cw.tn2};
+    const Samples sm{idxs, nullptr, idxs ? nullptr : rng_state};
+    for (int it = 0; it < I; ++it) {
+        const int cur = it & 1, nxt = cur ^ 1;
+        VoteWs iw = cw.v;              // the v3 passes on R_i, one keypoint, the work lengths as list lengths
+        iw.pix = pix[cur];
+        iw.direct = dir[cur];
+        iw.tn = cw.work;
+        dim3 ghyp((hn + 255) / 256, b);
+        k_center_hyp<<<ghyp, 256, 0, s>>>(dir[cur], pix[cur], tn[cur], cw.alive, npx, cw.v.cap, sm.idxs, sm.rng_state,
+                                          I, it, hn, min_num, cw.work, cw.v.hyp, out_tn);
+        PV_LAUNCHED("k_center_hyp");
+        PV_CUDA(cudaMemsetAsync(cw.v.counts, 0, sizeof(int) * (size_t)b * hn, s));
+        if ((rc = launch_vote(b, h, w, 1, hn, hn, 0, inlier_thresh, iw, s))) return rc;
+        if ((rc = launch_refit(b, h, w, 1, hn, hn, inlier_thresh, iw, cw.refit, s))) return rc;
+        k_center_decide<<<b, 256, 0, s>>>(cw.v.counts, cw.v.hyp, cw.work, cw.refit, hn, I, it, min_num, cw.alive,
+                                          out_num, out_centers, out_counts, out_hyp, out_win_counts);
+        PV_LAUNCHED("k_center_decide");
+        if (it + 1 == I) break;        // R_I is never read
+        dim3 gf(nchunk, b);
+        k_center_filter_count<<<gf, CH_THREADS, 0, s>>>(pix[cur], dir[cur], cw.work, cw.alive, cw.v.win, npx, cw.v.cap,
+                                                        nchunk, inlier_thresh, cw.v.chunk_fg);
+        PV_LAUNCHED("k_center_filter_count");
+        k_center_filter_write<<<gf, CH_THREADS, 0, s>>>(pix[cur], dir[cur], cw.work, cw.alive, cw.v.win, npx, cw.v.cap,
+                                                        nchunk, inlier_thresh, cw.v.chunk_fg, pix[nxt], dir[nxt],
+                                                        tn[nxt]);
+        PV_LAUNCHED("k_center_filter_write");
+    }
+    switch (mask_elem_size) {
+    case 1: launch_center_assign<unsigned char>(mask, field, st, out_num, out_centers, b, I, h, w, inlier_thresh, out_labels, s); break;
+    case 2: launch_center_assign<short>(mask, field, st, out_num, out_centers, b, I, h, w, inlier_thresh, out_labels, s); break;
+    case 4: launch_center_assign<int>(mask, field, st, out_num, out_centers, b, I, h, w, inlier_thresh, out_labels, s); break;
+    default: launch_center_assign<long long>(mask, field, st, out_num, out_centers, b, I, h, w, inlier_thresh, out_labels, s); break;
+    }
+    PV_LAUNCHED("k_center_assign");
+    return finish_rng(sm, s);
+}
+
+int pvnet_labels_workspace_bytes(int b, int h, int w, int vn, int num_labels, int hn_total, size_t *bytes)
+{
+    PV_CHECK_ARG(bytes, "null bytes pointer");
+    PV_CHECK_ARG(b >= 1 && h >= 1 && w >= 1 && vn >= 1 && hn_total >= 1, "non-positive dimension");
+    PV_CHECK_ARG(num_labels >= 1 && num_labels <= 32, "num_labels %d outside [1,32]", num_labels);
+    PV_CHECK_ARG((long long)b * num_labels <= VT_MAX_B, "b*num_labels %lld above %d", (long long)b * num_labels, VT_MAX_B);
+    PV_CHECK_ARG(h <= 65535 && w <= 65535, "image size %dx%d unsupported", h, w);
+    *bytes = carve_labels(nullptr, b, h, w, vn, num_labels, hn_total).bytes + 256;
+    return PVNET_OK;
+}
+
+// pvnet_ransac_voting_pipeline for every label of a label map at once: include/pvnet_b200.h, DESIGN.md section 29
+int pvnet_ransac_voting_labels(const void *labels, int labels_elem_size, int num_labels, const float *vertex,
+                               const int64_t vertex_strides[5], const int32_t *idxs, const int32_t *cov_idxs,
+                               const float *selection, const unsigned long long *rng_state, int b, int h, int w,
+                               int vn, int hn, float inlier_thresh, int cov_hn, int cov_rounds, int cov_min_hyp_num,
+                               float cov_inlier_thresh, int min_num, int max_num, float *out_pts, float *out_cov,
+                               int32_t *out_counts, float *out_hyp, int32_t *out_cov_counts, float *out_cov_hyp,
+                               int32_t *out_tn, void *workspace, size_t workspace_bytes, pvnet_stream_t stream)
+{
+    const bool with_cov = out_cov != nullptr;
+    const int L = num_labels;
+    PV_CHECK_ARG(L >= 1 && L <= 32, "num_labels %d outside [1,32]", L);
+    PV_CHECK_ARG(b >= 1 && (long long)b * L <= VT_MAX_B, "b*num_labels %lld outside [1,%d]", (long long)b * L, VT_MAX_B);
+    PV_CHECK_ARG(idxs || rng_state, "neither idxs nor rng_state given");
+    PV_CHECK_ARG(!with_cov || cov_idxs || rng_state, "neither cov_idxs nor rng_state given");
+    PV_CHECK_ARG(!with_cov || (cov_hn >= 1 && cov_rounds >= 1 && cov_min_hyp_num >= 1), "bad covariance sizes");
+    const long long hnt_ll = with_cov ? (long long)cov_hn * cov_rounds : 0;
+    PV_CHECK_ARG((hnt_ll + hn) * L <= (1 << 24), "too many hypotheses");
+    const int hnt = (int)hnt_ll, HT = hn + hnt, BL = b * L;
+    int rc = check_common(labels, labels_elem_size, vertex, (const long long *)vertex_strides, b, h, w, vn, hn);
+    if (rc) return rc;
+    PV_CHECK_ARG(out_pts, "null out_pts");
+    const Strides st = to_strides(vertex_strides);
+    LabelsWs lw = carve_labels(workspace, b, h, w, vn, L, HT);
+    PV_CHECK_ARG(workspace, "null workspace");
+    if (workspace_bytes < lw.bytes) {
+        pvnet::set_error("workspace %zu < %zu bytes", workspace_bytes, lw.bytes);
+        return PVNET_E_WORKSPACE;
+    }
+    cudaStream_t s = (cudaStream_t)stream;
+    const VoteWs &ws = lw.v;
+    const Samples sm{idxs, selection, idxs ? nullptr : rng_state};
+    const Samples sel_src{nullptr, selection, selection ? nullptr : rng_state};
+    // subsampling needs a selection source and an image that can exceed max_num, as in the pipeline
+    const Samples comp = (sel_src.selection || sel_src.rng_state) && max_num < h * w ? sel_src : Samples{nullptr, nullptr, nullptr};
+    switch (labels_elem_size) {
+    case 1: launch_label_compaction<unsigned char>(labels, comp, b, h, w, L, min_num, max_num, lw, s); break;
+    case 2: launch_label_compaction<short>(labels, comp, b, h, w, L, min_num, max_num, lw, s); break;
+    case 4: launch_label_compaction<int>(labels, comp, b, h, w, L, min_num, max_num, lw, s); break;
+    default: launch_label_compaction<long long>(labels, comp, b, h, w, L, min_num, max_num, lw, s); break;
+    }
+    PV_LAUNCHED("k_label_write");
+    k_gather<<<dim3(ws.ntile, b), 256, 0, s>>>(vertex, st, ws.pix, lw.tn_img, h * w, ws.cap, vn, ws.direct);
+    PV_LAUNCHED("k_gather");
+    // from here on the scoring passes see b*L images, one per (image, label) segment
+    PV_CUDA(cudaMemsetAsync(ws.counts, 0, sizeof(int) * (size_t)BL * vn * HT, s));
+    if ((rc = launch_gen_hyp(sm, RNG_IDXS_V3, BL, h, w, vn, hn, HT, 0, ws, s))) return rc;
+    if (with_cov) {
+        const Samples smc{cov_idxs, selection, cov_idxs ? nullptr : rng_state};
+        if ((rc = launch_gen_hyp(smc, RNG_IDXS_COV, BL, h, w, vn, hnt, HT, hn, ws, s))) return rc;
+    }
+    if (with_cov && cov_inlier_thresh == inlier_thresh) {
+        if ((rc = launch_vote(BL, h, w, vn, HT, HT, 0, inlier_thresh, ws, s))) return rc;
+    } else {
+        if ((rc = launch_vote(BL, h, w, vn, hn, HT, 0, inlier_thresh, ws, s))) return rc;
+        if (with_cov && (rc = launch_vote(BL, h, w, vn, hnt, HT, hn, cov_inlier_thresh, ws, s))) return rc;
+    }
+    if ((rc = launch_refit(BL, h, w, vn, hn, HT, inlier_thresh, ws, out_pts, s))) return rc;
+    if (with_cov) {
+        k_cov<<<BL * vn, 256, 0, s>>>(ws.hyp, ws.counts, ws.tn, out_pts, vn, hnt, HT, hn, cov_min_hyp_num, out_cov);
+        PV_LAUNCHED("k_cov");
+    }
+    if ((rc = launch_export(ws, BL, vn, hn, HT, 0, out_hyp, out_counts, out_tn, s))) return rc;
+    if (with_cov && (rc = launch_export(ws, BL, vn, hnt, HT, hn, out_cov_hyp, out_cov_counts, nullptr, s))) return rc;
     if (rng_state && (!idxs || (with_cov && !cov_idxs) || !selection)) return finish_rng(Samples{nullptr, nullptr, rng_state}, s);
     return PVNET_OK;
 }

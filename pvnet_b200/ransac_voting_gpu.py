@@ -15,6 +15,9 @@ inference hot path:
     ransac_voting_vanish_point_layer         (reference :408-501)
     ransac_voting_hypothesis                 (reference :218-261)
     estimate_voting_distribution             (reference :263-331)
+    ransac_voting_center                     (reference :600-667, finished here: DESIGN.md section 29)
+
+and ``ransac_voting_labels``, ``ransac_voting_pipeline`` for every label of a label map in one call.
 
 so ``tools/demo.py`` / ``tools/train_linemod.py --test_model`` keep working when
 ``lib/ransac_voting_gpu_layer/ransac_voting_gpu.py`` is this module (the shim under
@@ -98,6 +101,10 @@ def _workspace(b, h, w, vn, hn_total, device):
     n = ctypes.c_size_t()
     _native.check(_native.lib().pvnet_vote_workspace_bytes(b, h, w, vn, hn_total, ctypes.byref(n)),
                   "pvnet_vote_workspace_bytes")
+    return _grow_workspace(n, device)
+
+
+def _grow_workspace(n, device):
     device = torch.device(device)
     key = (device.index if device.index is not None else torch.cuda.current_device(),
            torch.cuda.current_stream(device).cuda_stream)
@@ -323,6 +330,156 @@ def ransac_voting_pipeline(mask, vertex, round_hyp_num, inlier_thresh=0.99, with
         dbg.update(idxs=idxs, cov_idxs=cov_idxs, selection=selection)
         return (out, cov, dbg) if with_covariance else (out, dbg)
     return res
+
+
+def ransac_voting_center(mask, vertex, round_hyp_num, inlier_thresh=0.99, confidence=0.999, max_iter=20, min_num=100,
+                         *, max_instances=8, idxs=None, rng="device", return_debug=False):
+    """Reference signature (ransac_voting_gpu.py:600); the reference stops before its result, this returns it.
+
+    Finds up to `max_instances` object centres per image in a centre vector field and splits the
+    foreground into instances (DESIGN.md section 29; `pvnet_ransac_voting_center` in include/pvnet_b200.h):
+    each round votes on the pixels not yet taken, the winning hypothesis's inliers become one instance and
+    its centre is refitted over them; a round whose pixels or winning count fall under `min_num` ends the
+    search.  Then every foreground pixel takes the centre it agrees with best.
+
+    :param mask:      [b,h,w] integer/bool CUDA tensor; nonzero low byte = foreground, as v3 reads it
+    :param vertex:    [b,h,w,2] float32 centre field, any strides: ``vertex[..., -1, :]`` of the permuted
+                      head output (the last keypoint of the Farthest / BB8C / BB8S layouts is the centre)
+                      is read in place
+    :param confidence, max_iter: accepted for compatibility; the samples are drawn once (:630), so they
+                      change nothing, as in v3
+    :param idxs:      int32 [b,max_instances,round_hyp_num,2] injected samples; otherwise rng="device"
+                      draws them with the in-kernel Philox generator (graph-capturable)
+    :return: (instance_mask int32 [b,h,w] with 0 = none and 1.. = instance, instance_num int32 [b]);
+             with return_debug also a dict of centers [b,I,2] and the per-round counts [b,I,hn],
+             hyp [b,I,hn,2], tn [b,I] and win_counts [b,I]
+
+    Keypoints and a pose per instance::
+
+        labels, n = ransac_voting_center(mask, vertex[..., -1, :], 256, max_instances=I)
+        kp, cov = ransac_voting_labels(labels, vertex, I, 256)                      # [b,I,vn,2], [b,I,vn,2,2]
+        poses = uncertainty_pnp_batched(kp.flatten(0, 1), points_3d, K, cov=cov.flatten(0, 1))
+        # pose i of image b is an instance where i < n[b]; the caller masks the others
+    """
+    del confidence, max_iter
+    _require_cuda(mask, "mask")
+    _require_cuda(vertex, "vertex")
+    if vertex.dim() != 4 or vertex.shape[-1] != 2:
+        raise ValueError(f"vertex must be [b,h,w,2], got {tuple(vertex.shape)}")
+    if vertex.dtype != torch.float32:
+        vertex = vertex.float()
+    b, h, w, _ = vertex.shape
+    hn, I = int(round_hyp_num), int(max_instances)
+    dev = mask.device
+    m, esz = _prep_mask(mask, _MASK_NONZERO_BYTE)
+    strides = (ctypes.c_int64 * 4)(*vertex.stride())
+    with torch.cuda.device(dev):
+        state = None
+        if idxs is not None:
+            idxs = torch.as_tensor(idxs, device=dev).to(torch.int32).contiguous()
+            if tuple(idxs.shape) != (b, I, hn, 2):
+                raise ValueError(f"idxs must be [b={b},{I},{hn},2], got {tuple(idxs.shape)}")
+        elif rng == "device":
+            state = _rng_state(dev)
+        else:
+            raise ValueError(f"rng must be 'device' or idxs injected, got {rng!r}")
+        labels = torch.empty([b, h, w], dtype=torch.int32, device=dev)
+        num = torch.empty([b], dtype=torch.int32, device=dev)
+        centers = torch.empty([b, I, 2], dtype=torch.float32, device=dev)
+        dbg = {}
+        if return_debug:
+            dbg = dict(counts=torch.empty([b, I, hn], dtype=torch.int32, device=dev),
+                       hyp=torch.empty([b, I, hn, 2], dtype=torch.float32, device=dev),
+                       tn=torch.empty([b, I], dtype=torch.int32, device=dev),
+                       win_counts=torch.empty([b, I], dtype=torch.int32, device=dev))
+        n = ctypes.c_size_t()
+        _native.check(_native.lib().pvnet_center_workspace_bytes(b, h, w, hn, ctypes.byref(n)),
+                      "pvnet_center_workspace_bytes")
+        ws, ws_bytes = _grow_workspace(n, dev)
+        _native.check(_native.lib().pvnet_ransac_voting_center(
+            _ptr(m), esz, _ptr(vertex), strides, _ptr(idxs), _ptr(state), b, h, w, hn, float(inlier_thresh),
+            int(min_num), I, _ptr(labels), _ptr(num), _ptr(centers), _ptr(dbg.get("counts")), _ptr(dbg.get("hyp")),
+            _ptr(dbg.get("tn")), _ptr(dbg.get("win_counts")), _ptr(ws), ws_bytes, _stream(dev)),
+            "pvnet_ransac_voting_center")
+    if return_debug:
+        dbg.update(centers=centers, idxs=idxs)
+        return labels, num, dbg
+    return labels, num
+
+
+def ransac_voting_labels(labels, vertex, num_labels, round_hyp_num, inlier_thresh=0.99, with_covariance=True,
+                         cov_round_hyp_num=256, cov_min_hyp_num=4096, cov_inlier_thresh=0.99, min_num=5, max_num=30000,
+                         *, idxs=None, cov_idxs=None, selection=None, rng="device", return_debug=False):
+    """``ransac_voting_pipeline`` for every label j < num_labels of a label map (value j+1), in one launch sequence
+    over `pvnet_ransac_voting_labels` (DESIGN.md section 29).  Output [bi, j] is bit-identical to
+    ``ransac_voting_pipeline((labels[bi:bi+1] == j + 1).byte(), vertex[bi:bi+1], ...)`` given idxs[bi, j],
+    cov_idxs[bi, j] and selection[bi:bi+1]; a label under min_num pixels gives what that call gives for an image
+    below min_num.  The mask is compacted and the field gathered once per image, whatever num_labels is.
+
+    :param labels:    [b,h,w] integer CUDA tensor (e.g. `ransac_voting_center`'s instance map)
+    :param vertex:    [b,h,w,vn,2] float32, any strides
+    :param num_labels: 1..32, with b * num_labels <= 1024
+    :param idxs:      int32 [b,num_labels,hn,vn,2]; cov_idxs int32 [b,num_labels,cov_rounds*cov_hn,vn,2];
+                      selection f32 [b,h,w]; whatever is not given is drawn on the device (rng="device")
+    :return: keypoints [b,L,vn,2] (and cov [b,L,vn,2,2] when with_covariance); with return_debug also a dict
+    """
+    _require_cuda(labels, "labels")
+    _require_cuda(vertex, "vertex")
+    b, h, w, vn, _ = vertex.shape
+    L, hn = int(num_labels), int(round_hyp_num)
+    rounds = int(math.ceil(cov_min_hyp_num / cov_round_hyp_num)) if with_covariance else 0
+    hnt = int(cov_round_hyp_num) * rounds
+    dev = labels.device
+    if labels.dtype not in _INT_DTYPES:
+        raise ValueError(f"labels must be an integer tensor, got {labels.dtype}")
+    lab = labels if labels.is_contiguous() else labels.contiguous()
+    v, strides = _prep_vertex(vertex)
+
+    def injected(t, n, name):
+        t = torch.as_tensor(t, device=dev).to(torch.int32).contiguous()
+        if tuple(t.shape) != (b, L, n, vn, 2):
+            raise ValueError(f"{name} must be [b={b},{L},{n},{vn},2], got {tuple(t.shape)}")
+        return t
+
+    with torch.cuda.device(dev):
+        if idxs is not None:
+            idxs = injected(idxs, hn, "idxs")
+        if with_covariance and cov_idxs is not None:
+            cov_idxs = injected(cov_idxs, hnt, "cov_idxs")
+        if selection is not None:
+            selection = torch.as_tensor(selection, device=dev, dtype=torch.float32).contiguous()
+            if tuple(selection.shape) != (b, h, w):
+                raise ValueError(f"selection must be [b,h,w], got {tuple(selection.shape)}")
+        state = None
+        if rng == "device":
+            state = _rng_state(dev)
+        elif idxs is None or (with_covariance and cov_idxs is None):
+            raise ValueError(f"rng must be 'device' unless idxs (and cov_idxs) are injected, got {rng!r}")
+        out = torch.empty([b, L, vn, 2], dtype=torch.float32, device=dev)
+        cov = torch.empty([b, L, vn, 2, 2], dtype=torch.float32, device=dev) if with_covariance else None
+        dbg = {}
+        if return_debug:
+            dbg = dict(counts=torch.empty([b, L, hn, vn], dtype=torch.int32, device=dev),
+                       hyp=torch.empty([b, L, hn, vn, 2], dtype=torch.float32, device=dev),
+                       tn=torch.empty([b, L], dtype=torch.int32, device=dev))
+            if with_covariance:
+                dbg.update(cov_counts=torch.empty([b, L, hnt, vn], dtype=torch.int32, device=dev),
+                           cov_hyp=torch.empty([b, L, hnt, vn, 2], dtype=torch.float32, device=dev))
+        n = ctypes.c_size_t()
+        _native.check(_native.lib().pvnet_labels_workspace_bytes(b, h, w, vn, L, hn + hnt, ctypes.byref(n)),
+                      "pvnet_labels_workspace_bytes")
+        ws, ws_bytes = _grow_workspace(n, dev)
+        _native.check(_native.lib().pvnet_ransac_voting_labels(
+            _ptr(lab), _INT_DTYPES[lab.dtype], L, _ptr(v), strides, _ptr(idxs), _ptr(cov_idxs), _ptr(selection),
+            _ptr(state), b, h, w, vn, hn, float(inlier_thresh), int(cov_round_hyp_num), max(rounds, 1),
+            int(cov_min_hyp_num), float(cov_inlier_thresh), int(min_num), int(min(max_num, 2 ** 31 - 1)), _ptr(out),
+            _ptr(cov), _ptr(dbg.get("counts")), _ptr(dbg.get("hyp")), _ptr(dbg.get("cov_counts")),
+            _ptr(dbg.get("cov_hyp")), _ptr(dbg.get("tn")), _ptr(ws), ws_bytes, _stream(dev)),
+            "pvnet_ransac_voting_labels")
+    if return_debug:
+        dbg.update(idxs=idxs, cov_idxs=cov_idxs, selection=selection)
+        return (out, cov, dbg) if with_covariance else (out, dbg)
+    return (out, cov) if with_covariance else out
 
 
 def ransac_voting_layer_v5(mask, vertex, round_hyp_num, inlier_thresh=0.999, confidence=0.99, max_iter=20,
