@@ -137,7 +137,7 @@ def refine_image(mask, pose, K, verts, faces, near, far, keypoints, points_3d, w
             mean0 = mean_after = m
             cost0 = cost_after = c
         else:
-            if len(sil) == 0 or n < rfo.MIN_PAIRS or c > cost_prev:
+            if len(sil) == 0 or n < rfo.MIN_PAIRS or not c <= cost_prev:              # a NaN C is undone
                 status |= rfo.REJECTED
                 P = backup
                 break

@@ -457,7 +457,8 @@ __global__ void __launch_bounds__(RF_STEP_THREADS)
                 S.mean0 = S.mean_after = m;
                 if (KP) S.cost0 = S.cost_after = cost;
             }
-        } else if (ns == 0 || n < RF_MIN_PAIRS || (KP ? cost > S.cost_prev : m > S.mean_prev)) {
+        } else if (ns == 0 || n < RF_MIN_PAIRS || (KP ? !(cost <= S.cost_prev) : m > S.mean_prev)) {
+            // a cost that is not a number (a keypoint at camera depth 0) is not shown to be no higher: undone too
             S.status |= RF_REJECTED;
             for (int q = 0; q < 12; ++q) pose[img * 12 + q] = S.backup[q];
             go = false;

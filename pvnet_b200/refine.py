@@ -153,9 +153,9 @@ def refine_poses(mask, poses, K, vertices, faces, near, far, rounds=8, gate=20.0
     model points, in the mesh's units) and exactly one of cov [b,nk,2,2] / weights_2d [b,nk,3] (converted through
     `covariance_to_weights`), floating-point CUDA tensors on the poses' device: each step then minimises
     (1/n) sum |pi(R X_i + t) - c_i|^2 + (keypoint_weight / nk) sum |W_k (pi(R P_k + t) - x_k)|^2, and a round is
-    undone when C = mean pair distance + keypoint_weight * mean_k |W_k e_k| rose (DESIGN.md §27).  return_info then
-    adds "cost_before" and "cost_after" (float64, C at the input pose and at the returned one), and trace adds
-    "keypoint_eq" (float64 [b,27], the first step's keypoint sums, unscaled)."""
+    undone when C = mean pair distance + keypoint_weight * mean_k |W_k e_k| rose or is NaN (DESIGN.md §27).
+    return_info then adds "cost_before" and "cost_after" (float64, C at the input pose and at the returned one), and
+    trace adds "keypoint_eq" (float64 [b,27], the first step's keypoint sums, unscaled)."""
     dev, b, h, w, near, far, rounds, gate, max_points = _check_common(mask, poses, K, vertices, faces, near, far,
                                                                       rounds, gate, max_points, 3)
 
