@@ -327,7 +327,15 @@ PVNET_API int pvnet_vote_counts(const float *direct, const float *coords, const 
  *   is solved with its own K exactly as pvnet_uncertainty_pnp solves it with that K: same kernel, same launch, bit
  *   for bit the same pose and info.  Both entries read fx, cx, fy, cy (K[0], K[2], K[4], K[5]) and ignore the rest.
  *   An image whose K has fx == 0 or fy == 0 is not solved: its pose is NaN and its status is 4; the other images
- *   are unaffected.  The K are read on the device only: the call does not synchronise and is graph-capturable. */
+ *   are unaffected.  The K are read on the device only: the call does not synchronise and is graph-capturable.
+ * pvnet_uncertainty_pnp_instances: the same solve for every instance row of a label-map vote (DESIGN.md §30):
+ *   points_2d f32 [b,L,pn,2], cov f32 [b,L,pn,2,2] or weights_2d f32 [b,L,pn,3], as pvnet_ransac_voting_labels
+ *   writes them; camera_matrices a DEVICE array of doubles [b,3,3] (one K per image, shared by its L rows); num a
+ *   DEVICE int32 [b], the instance count pvnet_ransac_voting_center writes.  1 <= L <= 32, b*L <= 1024.  Row (i, j)
+ *   with j < num[i] is solved with K[i] exactly as pvnet_uncertainty_pnp_per_image_k solves that row: bit for bit
+ *   the same pose and info.  A row with j >= num[i] is not solved: its pose is NaN and its info (8, 0), status bit
+ *   8 = no instance.  out_pose f64 [b,L,3,4], out_info int32 [b,L,2] or NULL.  num and the K are read on the device
+ *   only: the call does not synchronise and is graph-capturable. */
 PVNET_API int pvnet_covariance_to_weights(const float *cov, int n, float *weights, pvnet_stream_t stream);
 PVNET_API int pvnet_uncertainty_pnp(const float *points_2d, const float *cov, const float *weights_2d,
                                     const float *points_3d, const double camera_matrix[9], int b, int pn,
@@ -335,6 +343,10 @@ PVNET_API int pvnet_uncertainty_pnp(const float *points_2d, const float *cov, co
 PVNET_API int pvnet_uncertainty_pnp_per_image_k(const float *points_2d, const float *cov, const float *weights_2d,
                                                 const float *points_3d, const double *camera_matrices, int b, int pn,
                                                 double *out_pose, int32_t *out_info, pvnet_stream_t stream);
+PVNET_API int pvnet_uncertainty_pnp_instances(const float *points_2d, const float *cov, const float *weights_2d,
+                                              const float *points_3d, const double *camera_matrices,
+                                              const int32_t *num, int L, int b, int pn, double *out_pose,
+                                              int32_t *out_info, pvnet_stream_t stream);
 
 /* ------------------------------------------------------------------ EPnP
  * The reference's `pnp(points_3d, points_2d, camera_matrix, method=cv2.SOLVEPNP_EPNP)` (lib/utils/evaluation_utils.py:
@@ -629,6 +641,26 @@ PVNET_API int pvnet_refine_poses_keypoints(const uint8_t *mask, const double *po
                                            int32_t *info, double *dist, double *cost,
                                            const pvnet_refine_trace_t *trace, double *keypoint_eq, void *workspace,
                                            size_t workspace_bytes, pvnet_stream_t stream);
+
+/* pvnet_refine_poses_instances: pvnet_refine_poses (keypoints NULL) or pvnet_refine_poses_keypoints for every instance
+ * of a label map (DESIGN.md §30).  labels: integer [b,h,w] of element size labels_elem_size (1, 2, 4 or 8; 0 =
+ * background, j+1 = instance j, any other nonzero value another instance), num: DEVICE int32 [b] instance counts,
+ * 1 <= L <= 32, b*L <= 1024.  Virtual image v = bi*L + j: poses_in / poses_out f64 [b*L,3,4], K f32 [b*L,3,3] (one per
+ * virtual image), keypoints f32 [b*L,nk,2] and weights_2d f32 [b*L,nk,3] when given, info / dist / cost / trace rows
+ * per virtual image; the workspace is pvnet_refine_workspace_bytes(b*L, h, w, max_points).  Only the boundary sets
+ * differ from the one-mask call: the contour of instance j is its pixels with a 4-neighbour of value 0 or on the image
+ * border; a silhouette pixel is dropped (before the max_points stride) when its 3x3 neighbourhood holds another
+ * instance.  A row with j >= num[bi] is not refined: it returns its input pose with status 32 (no instance), and its
+ * render draws nothing.  num is read on the device only: no synchronisation, graph-capturable. */
+PVNET_API int pvnet_refine_poses_instances(const void *labels, int labels_elem_size, const int32_t *num, int L,
+                                           const double *poses_in, const float *K, const float *verts,
+                                           const int32_t *faces, int nv, int nf, int b, int h, int w, float near_clip,
+                                           float far_clip, int rounds, float gate, int max_points,
+                                           const float *keypoints, const float *points_3d, const float *weights_2d,
+                                           int nk, double keypoint_weight, double *poses_out, int32_t *info,
+                                           double *dist, double *cost, const pvnet_refine_trace_t *trace,
+                                           double *keypoint_eq, void *workspace, size_t workspace_bytes,
+                                           pvnet_stream_t stream);
 
 /* pvnet_refine_poses_depth: depth-anchored pose refinement of one mesh at b poses, point-to-plane ICP against the
  *   registered depth image (DESIGN.md §28).  Per image and round: the depth Zr at the current pose from

@@ -92,6 +92,8 @@ SIGNATURES = {
                                       c_void_p, c_void_p, c_void_p]),
     "pvnet_uncertainty_pnp_per_image_k": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
                                                   c_void_p, c_void_p, c_void_p]),
+    "pvnet_uncertainty_pnp_instances": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
+                                                c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "pvnet_epnp": (c_int, [c_void_p, c_void_p, ctypes.POINTER(ctypes.c_double), c_int, c_int, c_void_p, c_void_p,
                            c_void_p]),
     "pvnet_epnp_per_image_k": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
@@ -134,6 +136,11 @@ SIGNATURES = {
     "pvnet_refine_poses": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
                                    c_int, c_float, c_float, c_int, c_float, c_int, c_void_p, c_void_p, c_void_p,
                                    ctypes.POINTER(RefineTrace), c_void_p, c_size_t, c_void_p]),
+    "pvnet_refine_poses_instances": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                                             c_int, c_int, c_int, c_int, c_int, c_float, c_float, c_int, c_float, c_int,
+                                             c_void_p, c_void_p, c_void_p, c_int, ctypes.c_double, c_void_p, c_void_p,
+                                             c_void_p, c_void_p, ctypes.POINTER(RefineTrace), c_void_p, c_void_p,
+                                             c_size_t, c_void_p]),
     "pvnet_refine_poses_keypoints": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int,
                                              c_int, c_int, c_int, c_float, c_float, c_int, c_float, c_int, c_void_p,
                                              c_void_p, c_void_p, c_int, ctypes.c_double, c_void_p, c_void_p, c_void_p,

@@ -302,22 +302,25 @@ struct PnpCamera {
 // image is not solved and its pose is NaN
 constexpr int PNP_STATUS_BAD_CAMERA = 4;
 
-// one warp per image
-__global__ void __launch_bounds__(128)
-    k_uncertainty_pnp(const float *__restrict__ kp, const float *__restrict__ cov, const float *__restrict__ wgt,
-                      const float *__restrict__ pts3d, PnpCamera cam, int nb, int K,
-                      double *__restrict__ out_pose, int *__restrict__ out_info)
+// status bit 8 (pvnet_uncertainty_pnp_instances): row j of image b with j >= num[b] holds no instance; it is not
+// solved and its pose is NaN
+constexpr int PNP_STATUS_NO_INSTANCE = 8;
+
+// The solve of one image by one warp: keypoint row `img` of kp / cov / wgt, pose and info row `img` of the outputs,
+// camera row `cam_row` of cam.per_image (when not null).  s_red, s_cam: the CTA's reduction slices and camera slots
+// in shared memory, one per warp.
+__device__ __forceinline__ void pnp_solve(const float *__restrict__ kp, const float *__restrict__ cov,
+                                          const float *__restrict__ wgt, const float *__restrict__ pts3d,
+                                          const PnpCamera &cam, int cam_row, int img, int K,
+                                          double (*s_red)[33 * PNP_NRED], double (*s_cam)[4],
+                                          double *__restrict__ out_pose, int *__restrict__ out_info)
 {
-    __shared__ double s_red[4][33 * PNP_NRED];
-    const int img = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int lane = threadIdx.x & 31;
-    if (img >= nb) return;
     // this image's (fx, fy, cx, cy) in this warp's slot of shared memory, read where they are used: held in
     // registers through the LM loop they would push the kernel (at the 255-register limit) into spilling
-    __shared__ double s_cam[4][4];
     double *cm = s_cam[threadIdx.x >> 5];
     if (lane == 0) {
-        const double *k = cam.per_image ? cam.per_image + (size_t)img * 9 : nullptr;
+        const double *k = cam.per_image ? cam.per_image + (size_t)cam_row * 9 : nullptr;
         cm[0] = k ? k[0] : cam.fx;
         cm[1] = k ? k[4] : cam.fy;
         cm[2] = k ? k[2] : cam.cx;
@@ -546,6 +549,45 @@ __global__ void __launch_bounds__(128)
     }
 }
 
+// one warp per image
+__global__ void __launch_bounds__(128)
+    k_uncertainty_pnp(const float *__restrict__ kp, const float *__restrict__ cov, const float *__restrict__ wgt,
+                      const float *__restrict__ pts3d, PnpCamera cam, int nb, int K,
+                      double *__restrict__ out_pose, int *__restrict__ out_info)
+{
+    __shared__ double s_red[4][33 * PNP_NRED];
+    const int img = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (img >= nb) return;
+    __shared__ double s_cam[4][4];
+    pnp_solve(kp, cov, wgt, pts3d, cam, img, img, K, s_red, s_cam, out_pose, out_info);
+}
+
+// One warp per (image, instance) row v = bi * L + j of [b,L] keypoints.  A row with j < num[bi] is solved with camera
+// bi by k_uncertainty_pnp's code; the others leave at once with a NaN pose and status PNP_STATUS_NO_INSTANCE.
+__global__ void __launch_bounds__(128)
+    k_uncertainty_pnp_instances(const float *__restrict__ kp, const float *__restrict__ cov,
+                                const float *__restrict__ wgt, const float *__restrict__ pts3d, PnpCamera cam,
+                                const int *__restrict__ num, int L, int nrows, int K, double *__restrict__ out_pose,
+                                int *__restrict__ out_info)
+{
+    __shared__ double s_red[4][33 * PNP_NRED];
+    __shared__ double s_cam[4][4];
+    const int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (row >= nrows) return;
+    const int bi = row / L, j = row - bi * L;
+    if (j >= num[bi]) {                             // warp-uniform
+        if ((threadIdx.x & 31) == 0) {
+            for (int i = 0; i < 12; ++i) out_pose[(size_t)row * 12 + i] = __longlong_as_double(0x7ff8000000000000ll);
+            if (out_info) {
+                out_info[row * 2] = PNP_STATUS_NO_INSTANCE;
+                out_info[row * 2 + 1] = 0;
+            }
+        }
+        return;
+    }
+    pnp_solve(kp, cov, wgt, pts3d, cam, bi, row, K, s_red, s_cam, out_pose, out_info);
+}
+
 // covariance -> (wxx, wxy, wyy), thread per keypoint
 __global__ void k_cov_to_weights(const float *__restrict__ cov, int n, float *__restrict__ wgt)
 {
@@ -606,6 +648,26 @@ int pvnet_uncertainty_pnp_per_image_k(const float *points_2d, const float *cov, 
     PV_CHECK_ARG(camera_matrices, "null pointer");
     return launch_uncertainty_pnp(points_2d, cov, weights_2d, points_3d, PnpCamera{0.0, 0.0, 0.0, 0.0, camera_matrices},
                                   b, pn, out_pose, out_info, stream);
+}
+
+int pvnet_uncertainty_pnp_instances(const float *points_2d, const float *cov, const float *weights_2d,
+                                    const float *points_3d, const double *camera_matrices, const int32_t *num, int L,
+                                    int b, int pn, double *out_pose, int32_t *out_info, pvnet_stream_t stream)
+{
+    PV_CHECK_ARG(points_2d && points_3d && out_pose && camera_matrices && num, "null pointer");
+    PV_CHECK_ARG((cov != nullptr) != (weights_2d != nullptr), "pass exactly one of cov / weights_2d");
+    PV_CHECK_ARG(b >= 1, "non-positive batch");
+    PV_CHECK_ARG(L >= 1 && L <= 32 && b * L <= 1024, "instance count %d outside 1..32 or b*L = %d above 1024", L,
+                 b * L);
+    PV_CHECK_ARG(pn >= 4 && pn <= 32, "point count %d outside [4,32] (one warp per image)", pn);
+    const int rows = b * L;
+    const int warps_per_cta = rows <= 592 ? 1 : 4;      // launch_uncertainty_pnp's rule, over the rows
+    k_uncertainty_pnp_instances<<<(rows + warps_per_cta - 1) / warps_per_cta, 32 * warps_per_cta, 0,
+                                  (cudaStream_t)stream>>>(points_2d, cov, weights_2d, points_3d,
+                                                          PnpCamera{0.0, 0.0, 0.0, 0.0, camera_matrices}, num, L, rows,
+                                                          pn, out_pose, out_info);
+    PV_LAUNCHED("k_uncertainty_pnp_instances");
+    return PVNET_OK;
 }
 
 }  // extern "C"

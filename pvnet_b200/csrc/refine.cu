@@ -39,6 +39,7 @@ constexpr int RF_NSUM = 27;                       // 21 entries of the upper tri
 constexpr int RF_MAX_KP = 32;                     // keypoints: one lane of warp 0 each
 
 constexpr int RF_NO_CONTOUR = 1, RF_NO_SILHOUETTE = 2, RF_FEW_PAIRS = 4, RF_SINGULAR = 8, RF_REJECTED = 16;
+constexpr int RF_NO_INSTANCE = 32;                // pvnet_refine_poses_instances: a row past its image's count
 
 __device__ __forceinline__ double dm(double a, double b) { return __dmul_rn(a, b); }
 __device__ __forceinline__ double da(double a, double b) { return __dadd_rn(a, b); }
@@ -87,31 +88,17 @@ __device__ __forceinline__ void project(const double *P, const Cam &c, double x,
 // Pass 1 counts the boundary pixels; pass 2 walks them again in row-major order and keeps rank % stride == 0,
 // stride = ceil(n / max_points), writing each at rank / stride.  A silhouette point is back-projected at the pose
 // it was rendered from.  skip_done: images already stopped are left alone.
-__global__ void __launch_bounds__(RF_BOUND_THREADS, 1)
-    k_refine_boundary(const float *__restrict__ depth, const uint8_t *__restrict__ mask, const double *__restrict__ pose,
-                      const float *__restrict__ K, int kstride, int h, int w, int max_points, int skip_done,
-                      const State *__restrict__ state, int32_t *__restrict__ sil_idx, double *__restrict__ sil_obj,
-                      int32_t *__restrict__ con_idx, int32_t *__restrict__ counts)
+// The count-then-rank scan of one point set of image img (the body of both boundary kernels): edge(p) says whether
+// pixel p is in the set; dep is the image's rendered depth, read for the silhouette's back-projection.
+template <class Edge>
+__device__ __forceinline__ void boundary_scan(const Edge &edge, int img, int which, const float *__restrict__ dep,
+                                              const float *__restrict__ K,
+                                              int kstride, int h, int w, int max_points, int32_t *__restrict__ sil_idx,
+                                              double *__restrict__ sil_obj, int32_t *__restrict__ con_idx,
+                                              int32_t *__restrict__ counts, int *s_warp, int &s_total, double *s_pose)
 {
-    const int img = blockIdx.x, which = blockIdx.y;
-    if (skip_done && state[img].done) return;
-    __shared__ int s_warp[RF_BOUND_THREADS / 32];
-    __shared__ int s_total;
-    __shared__ double s_pose[12];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const long long hw = static_cast<long long>(h) * w;
-    const float *dep = depth + img * hw;
-    const uint8_t *msk = mask + img * hw;
-    if (tid == 0) s_total = 0;
-    if (tid < 12) s_pose[tid] = pose[img * 12 + tid];
-    __syncthreads();
-    auto on = [&](long long p) -> bool { return which == 0 ? dep[p] > 0.f : msk[p] != 0; };
-    auto edge = [&](long long p) -> bool {
-        if (!on(p)) return false;
-        const int r = static_cast<int>(p / w), c = static_cast<int>(p - static_cast<long long>(r) * w);
-        if (r == 0 || r == h - 1 || c == 0 || c == w - 1) return true;
-        return !on(p - 1) || !on(p + 1) || !on(p - w) || !on(p + w);
-    };
     int local = 0;
     for (long long base = 0; base < hw; base += RF_CHUNK)
         for (int q = 0; q < RF_PER_THREAD; ++q) {
@@ -175,6 +162,100 @@ __global__ void __launch_bounds__(RF_BOUND_THREADS, 1)
         __syncthreads();                          // s_warp is rewritten by the next chunk
     }
     if (tid == 0) counts[img * 2 + which] = n ? (n + stride - 1) / stride : 0;
+}
+
+__global__ void __launch_bounds__(RF_BOUND_THREADS, 1)
+    k_refine_boundary(const float *__restrict__ depth, const uint8_t *__restrict__ mask, const double *__restrict__ pose,
+                      const float *__restrict__ K, int kstride, int h, int w, int max_points, int skip_done,
+                      const State *__restrict__ state, int32_t *__restrict__ sil_idx, double *__restrict__ sil_obj,
+                      int32_t *__restrict__ con_idx, int32_t *__restrict__ counts)
+{
+    const int img = blockIdx.x, which = blockIdx.y;
+    if (skip_done && state[img].done) return;
+    __shared__ int s_warp[RF_BOUND_THREADS / 32];
+    __shared__ int s_total;
+    __shared__ double s_pose[12];
+    const int tid = threadIdx.x;
+    const long long hw = static_cast<long long>(h) * w;
+    const float *dep = depth + img * hw;
+    const uint8_t *msk = mask + img * hw;
+    if (tid == 0) s_total = 0;
+    if (tid < 12) s_pose[tid] = pose[img * 12 + tid];
+    __syncthreads();
+    auto on = [&](long long p) -> bool { return which == 0 ? dep[p] > 0.f : msk[p] != 0; };
+    auto edge = [&](long long p) -> bool {
+        if (!on(p)) return false;
+        const int r = static_cast<int>(p / w), c = static_cast<int>(p - static_cast<long long>(r) * w);
+        if (r == 0 || r == h - 1 || c == 0 || c == w - 1) return true;
+        return !on(p - 1) || !on(p + 1) || !on(p - w) || !on(p + w);
+    };
+    boundary_scan(edge, img, which, dep, K, kstride, h, w, max_points, sil_idx, sil_obj, con_idx, counts, s_warp,
+                  s_total, s_pose);
+}
+
+// The boundary sets of virtual image img = bi * L + j, instance j of image bi's label map (DESIGN.md §30).  The label
+// values are read at their own width (T) and compared as integers; anything nonzero other than j+1, including values
+// above L, is another instance.  Contour (blockIdx.y == 1): pixels of value j+1 with a 4-neighbour of value 0 or on
+// the image border; a border with another instance is not outline evidence.  Silhouette (0): the rendered depth's
+// covered-boundary pixels, as k_refine_boundary takes them, less those whose 3x3 neighbourhood (inside the image) holds
+// another instance, where the outline may be hidden; they are left out before the max_points stride.  Rows already
+// done (the absent instances, from the start) are skipped.
+template <typename T>
+__global__ void __launch_bounds__(RF_BOUND_THREADS, 1)
+    k_refine_boundary_instances(const float *__restrict__ depth, const T *__restrict__ labels, int L,
+                                const double *__restrict__ pose, const float *__restrict__ K, int kstride, int h,
+                                int w, int max_points, const State *__restrict__ state, int32_t *__restrict__ sil_idx,
+                                double *__restrict__ sil_obj, int32_t *__restrict__ con_idx,
+                                int32_t *__restrict__ counts)
+{
+    const int img = blockIdx.x, which = blockIdx.y;
+    if (state[img].done) return;
+    __shared__ int s_warp[RF_BOUND_THREADS / 32];
+    __shared__ int s_total;
+    __shared__ double s_pose[12];
+    const int tid = threadIdx.x;
+    const long long hw = static_cast<long long>(h) * w;
+    const int bi = img / L;
+    const long long own = img - bi * L + 1;
+    const float *dep = depth + img * hw;
+    const T *lab = labels + bi * hw;
+    if (tid == 0) s_total = 0;
+    if (tid < 12) s_pose[tid] = pose[img * 12 + tid];
+    __syncthreads();
+    auto val = [&](long long p) -> long long { return static_cast<long long>(lab[p]); };
+    auto other = [&](long long p) -> bool { const long long v = val(p); return v != 0 && v != own; };
+    auto edge = [&](long long p) -> bool {
+        const int r = static_cast<int>(p / w), c = static_cast<int>(p - static_cast<long long>(r) * w);
+        const bool border = r == 0 || r == h - 1 || c == 0 || c == w - 1;
+        if (which == 1) {
+            if (val(p) != own) return false;
+            if (border) return true;
+            return val(p - 1) == 0 || val(p + 1) == 0 || val(p - w) == 0 || val(p + w) == 0;
+        }
+        if (!(dep[p] > 0.f)) return false;
+        if (!border && dep[p - 1] > 0.f && dep[p + 1] > 0.f && dep[p - w] > 0.f && dep[p + w] > 0.f) return false;
+        for (int dr = -1; dr <= 1; ++dr) {
+            if (r + dr < 0 || r + dr >= h) continue;
+            for (int dc = -1; dc <= 1; ++dc)
+                if (c + dc >= 0 && c + dc < w && other(p + static_cast<long long>(dr) * w + dc)) return false;
+        }
+        return true;
+    };
+    boundary_scan(edge, img, which, dep, K, kstride, h, w, max_points, sil_idx, sil_obj, con_idx, counts, s_warp,
+                  s_total, s_pose);
+}
+
+// Absent rows (j >= num[bi]) start done with status RF_NO_INSTANCE and keep their input pose.  Their fp32 render pose
+// is all zeros: every vertex then sits at camera depth 0, below the near plane, so the renderer's face box rejects
+// every face and rasterises nothing for them.
+__global__ void k_refine_absent(const int32_t *__restrict__ num, int L, int nrows, State *__restrict__ state,
+                                float *__restrict__ pose32)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= nrows || i % L < num[i / L]) return;
+    state[i].done = 1;
+    state[i].status = RF_NO_INSTANCE;
+    for (int q = 0; q < 12; ++q) pose32[i * 12 + q] = 0.f;
 }
 
 // Nearest contour pixel of each silhouette point: grid (ceil(max_points / 256), b).  The point is projected at the
@@ -640,12 +721,21 @@ int pvnet_refine_workspace_bytes(int b, int h, int w, int max_points, size_t *by
 
 namespace {
 
-// Both entry points: kpa null runs k_refine_step<false>, the silhouette objective alone.
+// The label map of pvnet_refine_poses_instances: labels [b/L,h,w] of element size esz, counts num [b/L].
+struct InstArgs {
+    const void *labels;
+    int esz;
+    const int32_t *num;
+    int L;
+};
+
+// Every entry point: kpa null runs k_refine_step<false>, the silhouette objective alone; inst non-null reads the
+// contour and silhouette rules of a label map (mask is then unused) and b counts the virtual images.
 int refine_poses(const uint8_t *mask, const double *poses_in, const float *K, int k_per_image, const float *verts,
                  const int32_t *faces, int nv, int nf, int b, int h, int w, float near_clip, float far_clip, int rounds,
                  float gate, int max_points, const KpArgs *kpa, double *poses_out, int32_t *info, double *dist,
                  double *cost, const pvnet_refine_trace_t *trace, void *workspace, size_t workspace_bytes,
-                 pvnet_stream_t stream)
+                 pvnet_stream_t stream, const InstArgs *inst = nullptr)
 {
     PV_CHECK_ARG(b >= 1 && h >= 1 && w >= 1 && nv >= 0 && nf >= 0, "bad dimension (b=%d, h=%d, w=%d, nv=%d, nf=%d)",
                  b, h, w, nv, nf);
@@ -654,7 +744,8 @@ int refine_poses(const uint8_t *mask, const double *poses_in, const float *K, in
                  "max_points %d outside 1..%d for b = %d", max_points, INT32_MAX / 3 / b, b);
     PV_CHECK_ARG(rounds >= 0, "rounds must be >= 0 (got %d)", rounds);
     PV_CHECK_ARG(gate > 0.f, "gate must be positive (got %g)", gate);
-    PV_CHECK_ARG(mask && poses_in && K && poses_out && (nf == 0 || faces) && (nv == 0 || verts), "null pointer");
+    PV_CHECK_ARG((mask || inst) && poses_in && K && poses_out && (nf == 0 || faces) && (nv == 0 || verts),
+                 "null pointer");
     size_t need = 0;
     pvnet_refine_workspace_bytes(b, h, w, max_points, &need);
     PV_CHECK_ARG(workspace && workspace_bytes >= need, "workspace %zu bytes < %zu", workspace_bytes, need);
@@ -667,15 +758,35 @@ int refine_poses(const uint8_t *mask, const double *poses_in, const float *K, in
     const float gate2 = g2v;
     k_refine_init<<<(b + 127) / 128, 128, 0, st>>>(poses_in, poses_out, L.pose32, L.state, b);
     PV_LAUNCHED("k_refine_init");
+    if (inst) {
+        k_refine_absent<<<(b + 127) / 128, 128, 0, st>>>(inst->num, inst->L, b, L.state, L.pose32);
+        PV_LAUNCHED("k_refine_absent");
+    }
     for (int k = 0; k <= rounds; ++k) {
         const int rc = pvnet_render_mesh(verts, faces, nullptr, nv, nf, L.pose32, K, k_per_image, b, h, w, near_clip,
                                          far_clip, 0.5f, nullptr, L.depth, nullptr, L.keys, render_need, stream);
         if (rc != PVNET_OK) return rc;
-        k_refine_boundary<<<dim3(b, k == 0 ? 2 : 1), RF_BOUND_THREADS, 0, st>>>(
-            L.depth, mask, poses_out, K, kstride, h, w, max_points, k > 0, L.state, L.sil, L.obj, L.con, L.counts);
+        const dim3 bgrid(b, k == 0 ? 2 : 1);
+        if (!inst) {
+            k_refine_boundary<<<bgrid, RF_BOUND_THREADS, 0, st>>>(L.depth, mask, poses_out, K, kstride, h, w, max_points,
+                                                                  k > 0, L.state, L.sil, L.obj, L.con, L.counts);
+        } else {
+#define PV_BOUNDARY_INSTANCES(T)                                                                                       \
+    k_refine_boundary_instances<T><<<bgrid, RF_BOUND_THREADS, 0, st>>>(                                                \
+        L.depth, static_cast<const T *>(inst->labels), inst->L, poses_out, K, kstride, h, w, max_points, L.state,     \
+        L.sil, L.obj, L.con, L.counts)
+            switch (inst->esz) {
+            case 1: PV_BOUNDARY_INSTANCES(unsigned char); break;
+            case 2: PV_BOUNDARY_INSTANCES(short); break;
+            case 4: PV_BOUNDARY_INSTANCES(int); break;
+            default: PV_BOUNDARY_INSTANCES(long long); break;
+            }
+#undef PV_BOUNDARY_INSTANCES
+        }
         PV_LAUNCHED("k_refine_boundary");
+        // absent instances are done from the start: their point sets were never written
         k_refine_pairs<<<dim3((max_points + RF_PAIR_THREADS - 1) / RF_PAIR_THREADS, b), RF_PAIR_THREADS, 0, st>>>(
-            poses_out, K, kstride, w, max_points, gate2, k > 0, L.state, L.counts, L.obj, L.con, L.pair, L.d2);
+            poses_out, K, kstride, w, max_points, gate2, inst || k > 0, L.state, L.counts, L.obj, L.con, L.pair, L.d2);
         PV_LAUNCHED("k_refine_pairs");
         if (k == 0 && trace) {
             const size_t np = static_cast<size_t>(b) * max_points;
@@ -737,6 +848,34 @@ int pvnet_refine_poses_keypoints(const uint8_t *mask, const double *poses_in, co
     const KpArgs kpa{keypoints, points_3d, weights_2d, nk, keypoint_weight, keypoint_eq};
     return refine_poses(mask, poses_in, K, k_per_image, verts, faces, nv, nf, b, h, w, near_clip, far_clip, rounds,
                         gate, max_points, &kpa, poses_out, info, dist, cost, trace, workspace, workspace_bytes, stream);
+}
+
+int pvnet_refine_poses_instances(const void *labels, int labels_elem_size, const int32_t *num, int L,
+                                 const double *poses_in, const float *K, const float *verts, const int32_t *faces,
+                                 int nv, int nf, int b, int h, int w, float near_clip, float far_clip, int rounds,
+                                 float gate, int max_points, const float *keypoints, const float *points_3d,
+                                 const float *weights_2d, int nk, double keypoint_weight, double *poses_out,
+                                 int32_t *info, double *dist, double *cost, const pvnet_refine_trace_t *trace,
+                                 double *keypoint_eq, void *workspace, size_t workspace_bytes, pvnet_stream_t stream)
+{
+    PV_CHECK_ARG(labels && num && K, "null pointer");
+    PV_CHECK_ARG(labels_elem_size == 1 || labels_elem_size == 2 || labels_elem_size == 4 || labels_elem_size == 8,
+                 "labels_elem_size %d not 1, 2, 4 or 8", labels_elem_size);
+    PV_CHECK_ARG(b >= 1 && L >= 1 && L <= 32 && static_cast<long long>(b) * L <= 1024,
+                 "instance count %d outside 1..32 or b*L = %lld above 1024", L, static_cast<long long>(b) * L);
+    const InstArgs inst{labels, labels_elem_size, num, L};
+    if (!keypoints && !points_3d && !weights_2d)
+        return refine_poses(nullptr, poses_in, K, 1, verts, faces, nv, nf, b * L, h, w, near_clip, far_clip, rounds,
+                            gate, max_points, nullptr, poses_out, info, dist, nullptr, trace, workspace,
+                            workspace_bytes, stream, &inst);
+    PV_CHECK_ARG(keypoints && points_3d && weights_2d, "null pointer");
+    PV_CHECK_ARG(nk >= 4 && nk <= RF_MAX_KP, "keypoint count %d outside [4,%d] (one lane per keypoint)", nk,
+                 RF_MAX_KP);
+    PV_CHECK_ARG(keypoint_weight >= 0.0 && keypoint_weight < INFINITY, "keypoint_weight must be finite and >= 0 "
+                 "(got %g)", keypoint_weight);
+    const KpArgs kpa{keypoints, points_3d, weights_2d, nk, keypoint_weight, keypoint_eq};
+    return refine_poses(nullptr, poses_in, K, 1, verts, faces, nv, nf, b * L, h, w, near_clip, far_clip, rounds, gate,
+                        max_points, &kpa, poses_out, info, dist, cost, trace, workspace, workspace_bytes, stream, &inst);
 }
 
 }  // extern "C"

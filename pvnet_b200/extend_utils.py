@@ -15,8 +15,10 @@ keeps the reference's signature and return type (numpy float64) for numpy inputs
 moved to the current CUDA device; batched CUDA tensors ([b,pn,2], [b,pn,3]) return a float64 CUDA
 tensor [b,3,4] with no host synchronisation, which is what `PoseKeypointPipeline(with_pose=True)` uses so
 that poses, not keypoints, are what leaves the GPU.  The batched form also takes one camera matrix per image as a
-CUDA tensor [b,3,3] (`pvnet_uncertainty_pnp_per_image_k`).  No CPU path: without the library or a CUDA
-device these functions raise.
+CUDA tensor [b,3,3] (`pvnet_uncertainty_pnp_per_image_k`).  `uncertainty_pnp_instances` solves the [b,L] instance
+rows of a label-map vote and leaves the rows past each image's instance count unsolved
+(`pvnet_uncertainty_pnp_instances`, DESIGN.md §30).  No CPU path: without the library or a CUDA device these
+functions raise.
 """
 from __future__ import annotations
 
@@ -94,6 +96,53 @@ def uncertainty_pnp_batched(points_2d, points_3d, camera_matrix, weights_2d=None
         else:
             _native.check(_native.lib().pvnet_uncertainty_pnp(*args, _camera(camera_matrix), *tail),
                           "pvnet_uncertainty_pnp")
+    return (out, info) if return_info else out
+
+
+def uncertainty_pnp_instances(points_2d, num, points_3d, camera_matrix, weights_2d=None, cov=None, return_info=False):
+    """One pose per instance row of a label-map vote (DESIGN.md §30): points_2d [b,L,pn,2] CUDA, as
+    `ransac_voting_labels` returns them; weights_2d [b,L,pn,3] or cov [b,L,pn,2,2] (exactly one); num the int32 [b]
+    instance count of `ransac_voting_center`, on the device; points_3d [pn,3]; camera_matrix [3,3] or [b,3,3], host or
+    CUDA (a host one is copied to the device once, with the call's other inputs).  1 <= L <= 32, b * L <= 1024.
+    Row (i, j) with j < num[i] is solved with image i's camera, bit for bit as `uncertainty_pnp_batched` solves that
+    row; a row with j >= num[i] is not solved: its pose is NaN and its info (8, 0).  num stays on the device: the call
+    does not synchronise.  -> poses float64 [b,L,3,4] on the device (and info int32 [b,L,2])."""
+    if not points_2d.is_cuda:
+        raise RuntimeError("pvnet_b200: `points_2d` must be a CUDA tensor (there is no CPU path)")
+    if (weights_2d is None) == (cov is None):
+        raise ValueError("pass exactly one of weights_2d / cov")
+    if points_2d.dim() != 4 or points_2d.shape[-1] != 2:
+        raise ValueError(f"points_2d must be [b,L,pn,2], got {tuple(points_2d.shape)}")
+    dev = points_2d.device
+    p2 = points_2d.contiguous().float()
+    b, L, pn, _ = p2.shape
+    if not 1 <= L <= 32 or b * L > 1024:
+        raise ValueError(f"L = {L} instances per image outside 1..32, or b * L = {b * L} above 1024")
+    if not 4 <= pn <= 32:
+        raise ValueError(f"point count {pn} outside [4,32]")
+    if not (isinstance(num, torch.Tensor) and num.device == dev and tuple(num.shape) == (b,)):
+        raise ValueError(f"num must be a [{b}] tensor on {dev}")
+    n = num.to(torch.int32).contiguous()
+    p3 = torch.as_tensor(points_3d, dtype=torch.float32, device=dev).contiguous()
+    if tuple(p3.shape) != (pn, 3):
+        raise ValueError(f"points_3d must be [{pn},3], got {tuple(p3.shape)}")
+    want = (b, L, pn, 3) if cov is None else (b, L, pn, 2, 2)
+    given = weights_2d if cov is None else cov
+    if tuple(given.shape) != want:
+        raise ValueError(f"{'weights_2d' if cov is None else 'cov'} must be {list(want)}, got {tuple(given.shape)}")
+    w = None if weights_2d is None else weights_2d.to(dev).contiguous().float()
+    c = None if cov is None else cov.to(dev).contiguous().float()
+    k = torch.as_tensor(camera_matrix.detach() if isinstance(camera_matrix, torch.Tensor) else
+                        np.asarray(camera_matrix, np.float64), dtype=torch.float64)
+    check_cameras(k.shape, b)
+    ks = k.to(dev).expand(b, 3, 3).contiguous()
+    out = torch.empty([b, L, 3, 4], dtype=torch.float64, device=dev)
+    info = torch.empty([b, L, 2], dtype=torch.int32, device=dev) if return_info else None
+    with torch.cuda.device(dev):
+        _native.check(_native.lib().pvnet_uncertainty_pnp_instances(
+            p2.data_ptr(), None if c is None else c.data_ptr(), None if w is None else w.data_ptr(), p3.data_ptr(),
+            ks.data_ptr(), n.data_ptr(), L, b, pn, out.data_ptr(), None if info is None else info.data_ptr(),
+            _stream(dev)), "pvnet_uncertainty_pnp_instances")
     return (out, info) if return_info else out
 
 

@@ -33,12 +33,22 @@ poses are then refined again against each image's registered depth (`refine.refi
 the side stream into a static device buffer per input buffer like the cameras.  The mesh, clip planes and cameras are
 refine's; depth-only refinement is `refine=dict(..., rounds=0, depth=...)`.
 
+`max_instances=I` (DESIGN.md §30): several objects of one class per image.  The step then splits each image's
+foreground into up to I instances with `ransac_voting_center` on the centre field (the last keypoint), votes every
+instance's keypoints and covariances with `ransac_voting_labels`, and solves one pose per instance with
+`extend_utils.uncertainty_pnp_instances`: `step` and `run` return (labels [b,H,W] int32, num [b] int32, keypoints
+[b,I,K,2], covariances [b,I,K,2,2], poses [b,I,3,4] float64), where row j of image i is an instance when j < num[i]
+(the other rows' poses are NaN).  It needs points_3d, a camera and with_covariance=True.  With `refine=` the instance
+poses are refined on the label map by `refine.refine_poses_instances` with the step's keypoints and covariances;
+`refine['depth']` is not available with max_instances.
+
 Inputs may be float32 [b,3,H,W] (already normalised, what `ToTensor` + `Normalize` produce,
 tools/demo.py:89-95) or uint8 [b,H,W,3] raw images: the latter are normalised on the device inside
 the packing kernel (4x fewer host->device bytes).
 """
 from __future__ import annotations
 
+import numpy as np
 import torch
 
 from . import extend_utils as eu
@@ -52,7 +62,7 @@ IMAGENET_STD = (0.229, 0.224, 0.225)
 class PoseKeypointPipeline:
     def __init__(self, net, round_hyp_num=256, inlier_thresh=0.99, rng="device", with_covariance=False,
                  cov_round_hyp_num=256, cov_min_hyp_num=4096, max_num=30000, mean=IMAGENET_MEAN, std=IMAGENET_STD,
-                 points_3d=None, camera_matrix=None, graph=False, refine=None):
+                 points_3d=None, camera_matrix=None, graph=False, refine=None, max_instances=None):
         self.net = net
         self.graph = bool(graph)
         self.hn = round_hyp_num
@@ -69,6 +79,17 @@ class PoseKeypointPipeline:
         if self.graph and rng != "device":
             raise ValueError("graph=True needs rng='device' (torch's generator cannot be replayed)")
         self.points_3d, self.camera_matrix = points_3d, camera_matrix
+        self.max_instances = None
+        if max_instances is not None:
+            if isinstance(max_instances, bool) or int(max_instances) != max_instances or not 1 <= max_instances <= 32:
+                raise ValueError(f"max_instances must be an integer in 1..32, got {max_instances!r}")
+            if points_3d is None or not with_covariance:
+                raise ValueError("max_instances needs points_3d and with_covariance=True")
+            if rng != "device":
+                raise ValueError("max_instances needs rng='device' (the instance split draws on the device)")
+            if refine is not None and refine.get("depth") is not None:
+                raise ValueError("refine['depth'] is not available with max_instances")
+            self.max_instances = int(max_instances)
         self.refine = None
         if refine is not None:
             if points_3d is None or not with_covariance:
@@ -89,6 +110,10 @@ class PoseKeypointPipeline:
             self.refine = cfg
         self._mesh_dev = None                       # (device, vertices, faces, constructor K or None)
         self._p3_dev = None
+        # max_instances: the constructor's host camera is snapshotted here and goes to the device once
+        host_k = camera_matrix is not None and not (isinstance(camera_matrix, torch.Tensor) and camera_matrix.is_cuda)
+        self._k_host = torch.tensor(np.asarray(camera_matrix, np.float64)).reshape(3, 3) if host_k else None
+        self._k_dev = None                          # the snapshot on the device
         self._bufs = None
         self._kbufs = None
         self._dbufs = None
@@ -160,6 +185,8 @@ class PoseKeypointPipeline:
         b, h, w, c = out.shape
         k = (c - self.net.seg_dim) // 2
         vertex = out[..., self.net.seg_dim:].unflatten(3, (k, 2))
+        if self.max_instances is not None:
+            return self._step_instances(mask, vertex, camera_matrix)
         # a 2-class argmax mask is binary: v3's `nonzero` and with_mean's `== 1` readings coincide
         if self.net.seg_dim == 2 or not self.with_cov:
             res = rv.ransac_voting_pipeline(mask, vertex, self.hn, self.thresh, self.with_cov, self.cov_hn, self.cov_min,
@@ -180,6 +207,42 @@ class PoseKeypointPipeline:
                 pose = self._refine(mask, pose, K, res[0], res[1], depth)
             return res[0], res[1], pose
         return res
+
+    def _step_instances(self, mask, vertex, camera_matrix):
+        """The max_instances step after the backbone: instance split, per-instance vote, per-instance PnP."""
+        I = self.max_instances
+        labels, num = rv.ransac_voting_center(mask, vertex[..., -1, :], self.hn, self.thresh, max_instances=I)
+        kp, cov = rv.ransac_voting_labels(labels, vertex, I, self.hn, self.thresh, True, self.cov_hn, self.cov_min,
+                                          self.thresh, max_num=self.max_num)
+        if self._p3_dev is None or self._p3_dev.device != mask.device:
+            self._p3_dev = torch.as_tensor(self.points_3d, dtype=torch.float32).to(mask.device).contiguous()
+        K = self.camera_matrix if camera_matrix is None else camera_matrix
+        if K is None:
+            raise ValueError("max_instances needs a camera: the constructor's camera_matrix or step's")
+        if not (isinstance(K, torch.Tensor) and K.is_cuda):
+            if camera_matrix is not None:
+                raise ValueError("step's camera_matrix must be a CUDA tensor")
+            if self._k_dev is None or self._k_dev.device != mask.device:
+                self._k_dev = self._k_host.to(mask.device)
+            K = self._k_dev
+        pose = eu.uncertainty_pnp_instances(kp, num, self._p3_dev, K, cov=cov)
+        if self.refine is not None:
+            cfg = self.refine
+            v, f = self._mesh(mask.device)
+            pose = rfn.refine_poses_instances(labels, num, pose, K, v, f, cfg["near"], cfg["far"], rounds=cfg["rounds"],
+                                              gate=cfg["gate"], max_points=cfg["max_points"], keypoints=kp,
+                                              points_3d=self._p3_dev, cov=cov, keypoint_weight=cfg["keypoint_weight"])
+        return labels, num, kp, cov, pose
+
+    def _mesh(self, dev):
+        """The refine mesh on the device, uploaded on first use -> (vertices f32, faces int32)."""
+        if self._mesh_dev is None or self._mesh_dev[0] != dev:
+            cfg = self.refine
+            v = torch.as_tensor(cfg["vertices"], dtype=torch.float32).to(dev).contiguous()
+            f = torch.as_tensor(cfg["faces"]).to(dev)
+            f = f if f.dtype == torch.int32 else f.to(torch.int32)
+            self._mesh_dev = (dev, v, f.contiguous(), None)
+        return self._mesh_dev[1], self._mesh_dev[2]
 
     def _refine(self, mask, pose, K, kp, cov, depth):
         """refine_poses on the step's outputs, then refine_poses_depth on its poses when depth is given; the mesh (and
@@ -270,13 +333,15 @@ class PoseKeypointPipeline:
             d = None if depths is None else self._dbufs[j]
             result = self._step_graph(j) if self.graph else self.step(self._bufs[j], k, d)
             self._free[j].record(main)
+            # max_instances: (labels, num, keypoints, cov, poses); otherwise (keypoints, cov[, poses]) or keypoints
+            res = result[2:] if self.max_instances is not None else result
             if out_host is not None:
-                kp = result[0] if isinstance(result, tuple) else result
+                kp = res[0] if isinstance(res, tuple) else res
                 out_host[i].copy_(kp, non_blocking=True)
-            if cov_host is not None and isinstance(result, tuple):
-                cov_host[i].copy_(result[1], non_blocking=True)
-            if pose_host is not None and isinstance(result, tuple) and len(result) > 2:
-                pose_host[i].copy_(result[2], non_blocking=True)
+            if cov_host is not None and isinstance(res, tuple):
+                cov_host[i].copy_(res[1], non_blocking=True)
+            if pose_host is not None and isinstance(res, tuple) and len(res) > 2:
+                pose_host[i].copy_(res[2], non_blocking=True)
             if on_result is not None:
                 on_result(i, result)
         if out_host is not None or cov_host is not None or pose_host is not None:

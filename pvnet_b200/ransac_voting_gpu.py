@@ -358,8 +358,8 @@ def ransac_voting_center(mask, vertex, round_hyp_num, inlier_thresh=0.99, confid
 
         labels, n = ransac_voting_center(mask, vertex[..., -1, :], 256, max_instances=I)
         kp, cov = ransac_voting_labels(labels, vertex, I, 256)                      # [b,I,vn,2], [b,I,vn,2,2]
-        poses = uncertainty_pnp_batched(kp.flatten(0, 1), points_3d, K, cov=cov.flatten(0, 1))
-        # pose i of image b is an instance where i < n[b]; the caller masks the others
+        poses = uncertainty_pnp_instances(kp, n, points_3d, K, cov=cov)            # [b,I,3,4]
+        # pose i of image b is an instance where i < n[b]; the others are NaN, with info status 8
     """
     del confidence, max_iter
     _require_cuda(mask, "mask")

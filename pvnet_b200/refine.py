@@ -14,7 +14,11 @@ keypoints.
 
 `refine_poses_depth` refines the same way against a registered depth image (`pvnet_refine_poses_depth`, DESIGN.md
 §28): point-to-plane ICP of the rendered surface against the observed one, which holds the distance along the
-viewing ray that the RGB cues barely see."""
+viewing ray that the RGB cues barely see.
+
+`refine_poses_instances` refines every instance of a label map (`pvnet_refine_poses_instances`, DESIGN.md §30): each
+instance is refined alone, with a contour that leaves out its borders with other instances and a silhouette that
+leaves out what another instance may hide."""
 from __future__ import annotations
 
 import ctypes
@@ -31,6 +35,7 @@ NO_SILHOUETTE = 2       # the render at the input pose covers nothing: the input
 FEW_PAIRS = 4           # fewer than 6 pairs at the input pose: the input pose is returned
 SINGULAR = 8            # a round's normal equations were singular: that round's starting pose is kept
 REJECTED = 16           # a round raised the mean pair distance (or lost its pairs) and was undone
+NO_INSTANCE = 32        # refine_poses_instances: the row is past its image's instance count; its pose is the input
 
 # lambda of the keypoint-anchored objective: the best of 0.25, 1 and 4 on the synthetic scenes of
 # benchmarks/refine_keypoints.py (DESIGN.md §27); real-data accuracy has not been measured
@@ -208,6 +213,106 @@ def refine_poses(mask, poses, K, vertices, faces, near, far, rounds=8, gate=20.0
         res += (dict(status=info[:, 0], pairs=info[:, 1], dist_before=dist[:, 0], dist_after=dist[:, 1]),)
         if cost is not None:
             res[-1].update(cost_before=cost[:, 0], cost_after=cost[:, 1])
+    if trace:
+        res += (tr,)
+    return res[0] if len(res) == 1 else res
+
+
+_INT_ELEM = {torch.uint8: 1, torch.int8: 1, torch.int16: 2, torch.int32: 4, torch.int64: 8}
+
+
+def refine_poses_instances(labels, num, poses, K, vertices, faces, near, far, rounds=8, gate=20.0, max_points=4096,
+                           return_info=False, trace=False, keypoints=None, points_3d=None, cov=None, weights_2d=None,
+                           keypoint_weight=DEFAULT_KEYPOINT_WEIGHT):
+    """`refine_poses` for every instance of a label map (DESIGN.md §30).
+
+    labels [b,H,W] integer CUDA tensor (0 background, j+1 instance j, `ransac_voting_center`'s map as it is; values
+    above L count as other instances), num int32 [b] instance counts on the device, poses [b,L,3,4] (1 <= L <= 32,
+    b * L <= 1024), K [3,3] or [b,3,3]; keypoints [b,L,nk,2] with cov [b,L,nk,2,2] or weights_2d [b,L,nk,3] as
+    `ransac_voting_labels` returns them.  Row (i, j) is refined as `refine_poses` refines one image, except for the
+    boundary sets: the contour of instance j is its pixels with a 4-neighbour of value 0 or on the image border, and
+    a silhouette pixel whose 3x3 neighbourhood holds another instance is left out.  A row with j >= num[i] keeps its
+    input pose with status NO_INSTANCE and costs no render.  Without host synchronisation; graph-capturable.
+
+    -> poses float64 [b,L,3,4]; return_info: a dict of [b,L] tensors as `refine_poses` returns; trace: the first
+    round's intermediates with one row per virtual image i * L + j."""
+    _cuda_tensor("labels", labels)
+    _cuda_tensor("num", num)
+    _cuda_tensor("poses", poses)
+    if labels.dtype not in _INT_ELEM:
+        raise ValueError(f"labels must be an integer tensor, got {labels.dtype}")
+    if labels.dim() != 3:
+        raise ValueError(f"labels must be [b,H,W], got {tuple(labels.shape)}")
+    if poses.dim() != 4 or tuple(poses.shape[2:]) != (3, 4):
+        raise ValueError(f"poses must be [b,L,3,4], got {tuple(poses.shape)}")
+    b, L = int(poses.shape[0]), int(poses.shape[1])
+    h, w = int(labels.shape[1]), int(labels.shape[2])
+    if int(labels.shape[0]) != b:
+        raise ValueError(f"labels holds {labels.shape[0]} images for {b} pose rows")
+    if not 1 <= L <= 32 or b * L > 1024:
+        raise ValueError(f"L = {L} instances per image outside 1..32, or b * L = {b * L} above 1024")
+    if tuple(num.shape) != (b,) or num.device != poses.device:
+        raise ValueError(f"num must be a [{b}] tensor on {poses.device}")
+    B = b * L
+    _cuda_tensor("K", K)
+    check_cameras(K.shape, b)
+    # the checks refine_poses makes, on the virtual images (a zero-stride stand-in for their masks)
+    stand_in = torch.zeros((), dtype=torch.uint8, device=labels.device).expand(B, h, w)
+    dev, _, _, _, near, far, rounds, gate, max_points = _check_common(
+        stand_in, poses.flatten(0, 1), K.expand(b, 3, 3).repeat_interleave(L, 0), vertices, faces, near, far, rounds,
+        gate, max_points, 3)
+    kpt = None
+    if keypoints is not None:
+        if keypoints.dim() != 4 or tuple(keypoints.shape[:2]) != (b, L):
+            raise ValueError(f"keypoints must be [{b},{L},nk,2], got {tuple(keypoints.shape)}")
+        kpt = _keypoint_inputs(B, dev, keypoints.flatten(0, 1), points_3d, None if cov is None else cov.flatten(0, 1),
+                               None if weights_2d is None else weights_2d.flatten(0, 1), keypoint_weight)
+    elif points_3d is not None or cov is not None or weights_2d is not None:
+        raise ValueError("points_3d, cov and weights_2d go with keypoints")
+    lab = labels.contiguous()
+    n32 = num.to(torch.int32).contiguous()
+    p = poses.flatten(0, 1).contiguous().double()
+    k = K.expand(b, 3, 3).float().repeat_interleave(L, 0).contiguous()        # one camera per virtual image
+    nv, nf = int(vertices.shape[0]), int(faces.shape[0])
+    v = vertices.contiguous().float()
+    f = faces.contiguous() if faces.dtype == torch.int32 else faces.clamp(-1, nv).to(torch.int32).contiguous()
+    out = torch.empty((B, 3, 4), dtype=torch.float64, device=dev)
+    info = torch.empty((B, 2), dtype=torch.int32, device=dev) if return_info else None
+    dist = torch.empty((B, 2), dtype=torch.float64, device=dev) if return_info else None
+    cost = torch.empty((B, 2), dtype=torch.float64, device=dev) if return_info and kpt is not None else None
+    tr, tr_struct = None, None
+    if trace:
+        tr = dict(sil_idx=torch.full((B, max_points), -1, dtype=torch.int32, device=dev),
+                  con_idx=torch.full((B, max_points), -1, dtype=torch.int32, device=dev),
+                  counts=torch.zeros((B, 2), dtype=torch.int32, device=dev),
+                  sil_obj=torch.zeros((B, max_points, 3), dtype=torch.float64, device=dev),
+                  pair_idx=torch.full((B, max_points), -1, dtype=torch.int32, device=dev),
+                  normal_eq=torch.full((B, 27), math.nan, dtype=torch.float64, device=dev))
+        tr_struct = _native.RefineTrace(*(tr[x].data_ptr() for x in ("sil_idx", "con_idx", "counts", "sil_obj",
+                                                                      "pair_idx", "normal_eq")))
+        if kpt is not None:
+            tr["keypoint_eq"] = torch.full((B, 27), math.nan, dtype=torch.float64, device=dev)
+    kp, pts, wgt, nk, lam = kpt if kpt is not None else (None, None, None, 0, 0.0)
+    lib = _native.lib()
+    with torch.cuda.device(dev):
+        need = ctypes.c_size_t()
+        _native.check(lib.pvnet_refine_workspace_bytes(B, h, w, max_points, ctypes.byref(need)),
+                      "pvnet_refine_workspace_bytes")
+        ws = torch.empty(need.value, dtype=torch.uint8, device=dev)
+        ptr = (lambda t: None if t is None else t.data_ptr())
+        _native.check(lib.pvnet_refine_poses_instances(
+            lab.data_ptr(), _INT_ELEM[lab.dtype], n32.data_ptr(), L, p.data_ptr(), k.data_ptr(), ptr(v) if nv else None,
+            ptr(f) if nf else None, nv, nf, b, h, w, near, far, rounds, gate, max_points, ptr(kp), ptr(pts), ptr(wgt),
+            nk, lam, out.data_ptr(), ptr(info), ptr(dist), ptr(cost),
+            None if tr_struct is None else ctypes.byref(tr_struct), None if tr is None else ptr(tr.get("keypoint_eq")),
+            ws.data_ptr(), need.value, ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
+            "pvnet_refine_poses_instances")
+    res = (out.view(b, L, 3, 4),)
+    if return_info:
+        d = dict(status=info[:, 0], pairs=info[:, 1], dist_before=dist[:, 0], dist_after=dist[:, 1])
+        if cost is not None:
+            d.update(cost_before=cost[:, 0], cost_after=cost[:, 1])
+        res += ({key: t.view(b, L) for key, t in d.items()},)
     if trace:
         res += (tr,)
     return res[0] if len(res) == 1 else res
