@@ -705,6 +705,28 @@ PVNET_API int pvnet_refine_poses_depth(const uint8_t *mask, const void *depth, i
                                        int32_t *info, double *dist, const pvnet_refine_depth_trace_t *trace,
                                        void *workspace, size_t workspace_bytes, pvnet_stream_t stream);
 
+/* pvnet_refine_poses_depth_instances: pvnet_refine_poses_depth for every instance of a label map (DESIGN.md §31).
+ *   labels: integer [b,h,w] of element size labels_elem_size (1, 2, 4 or 8; 0 = background, j+1 = instance j, any
+ *   other nonzero value another instance), read in place; num: DEVICE int32 [b] instance counts; 1 <= L <= 32,
+ *   b*L <= 1024; depth [b,h,w] as pvnet_refine_poses_depth reads it.  Virtual image v = bi*L + j: poses_in /
+ *   poses_out f64 [b*L,3,4], K f32 [b*L,3,3] (one per virtual image), info / dist / trace rows per virtual image, trace
+ *   pixel indices r*w+c in image bi's frame.  Row v with j < num[bi] is bit for bit pvnet_refine_poses_depth on the
+ *   one-image mask labels[bi] == j+1, depth[bi] and K[v]: a pixel pairs only when it and its four 4-neighbours carry
+ *   label j+1.  A row with j >= num[bi] is not refined: it returns its input pose with status 32 (no instance), pairs
+ *   0 and NaN distances, its render draws nothing and its trace counts are 0.  num is read on the device only: no
+ *   synchronisation, graph-capturable.  max_points: b*L * max_points <= INT32_MAX / 9.  Workspace:
+ *   pvnet_refine_depth_instances_workspace_bytes(b, L, h, w, max_points), pvnet_refine_depth_workspace_bytes(b*L, h,
+ *   w, max_points) plus one box per virtual image. */
+PVNET_API int pvnet_refine_depth_instances_workspace_bytes(int b, int L, int h, int w, int max_points, size_t *bytes);
+PVNET_API int pvnet_refine_poses_depth_instances(const void *labels, int labels_elem_size, const int32_t *num, int L,
+                                                 const void *depth, int depth_is_u16, float depth_scale,
+                                                 const double *poses_in, const float *K, const float *verts,
+                                                 const int32_t *faces, int nv, int nf, int b, int h, int w,
+                                                 float near_clip, float far_clip, int rounds, double gate,
+                                                 int max_points, double *poses_out, int32_t *info, double *dist,
+                                                 const pvnet_refine_depth_trace_t *trace, void *workspace,
+                                                 size_t workspace_bytes, pvnet_stream_t stream);
+
 /* The vanishing-point pair of the reference extension (ransac_voting.cpp:61-99 ->
  * ransac_voting_kernel.cu:170-260, :263-351; used by ransac_voting_vanish_point_layer,
  * ransac_voting_gpu.py:408-501): hypotheses are homogeneous points hypo [hn,vn,3]; the vote sets

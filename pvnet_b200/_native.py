@@ -151,6 +151,13 @@ SIGNATURES = {
                                          c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_float, c_int,
                                          ctypes.c_double, c_int, c_void_p, c_void_p, c_void_p,
                                          ctypes.POINTER(RefineDepthTrace), c_void_p, c_size_t, c_void_p]),
+    "pvnet_refine_depth_instances_workspace_bytes": (c_int, [c_int, c_int, c_int, c_int, c_int,
+                                                             ctypes.POINTER(c_size_t)]),
+    "pvnet_refine_poses_depth_instances": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_float,
+                                                   c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
+                                                   c_int, c_float, c_float, c_int, ctypes.c_double, c_int, c_void_p,
+                                                   c_void_p, c_void_p, ctypes.POINTER(RefineDepthTrace), c_void_p,
+                                                   c_size_t, c_void_p]),
     "pvnet_generate_hypothesis":(c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "pvnet_voting_for_hypothesis": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float,
                                             c_void_p]),

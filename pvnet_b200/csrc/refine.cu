@@ -21,6 +21,7 @@
 // one keypoint per lane; the other launches are the same as without keypoints.
 #include "common.cuh"
 
+#include <climits>
 #include <cmath>
 
 namespace {
@@ -1200,6 +1201,217 @@ __global__ void __launch_bounds__(RF_STEP_THREADS)
     }
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Depth-anchored refinement per instance (DESIGN.md §31, pvnet_refine_poses_depth_instances): virtual image
+// v = bi * L + j is instance j of image bi's label map, and row v is k_refine_depth_pairs's image v with the mask
+// labels[bi] == j+1.  The labels do not change between rounds, so each instance's bounding box is found once per call
+// and the pair scan walks only the box.
+
+constexpr int RD_BOX_THREADS = 1024;
+
+// Bounding box of each label 1..L of image blockIdx.x (grid b): boxes[bi * L + j] = (r0, c0, r1, c1), inclusive;
+// r1 < r0 when label j+1 has no pixel.  One warp per row; the lanes holding one label are grouped by
+// __match_any_sync and their lowest lane folds the group's column range into shared memory with integer atomics.
+template <typename T>
+__global__ void __launch_bounds__(RD_BOX_THREADS)
+    k_refine_label_boxes(const T *__restrict__ labels, int L, int h, int w, int4 *__restrict__ boxes)
+{
+    __shared__ int s_box[32][4];
+    const int bi = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    if (tid < 32) {
+        s_box[tid][0] = s_box[tid][1] = INT_MAX;
+        s_box[tid][2] = s_box[tid][3] = -1;
+    }
+    __syncthreads();
+    const T *lab = labels + static_cast<long long>(bi) * h * w;
+    for (int r = warp; r < h; r += RD_BOX_THREADS / 32)
+        for (int c0 = 0; c0 < w; c0 += 32) {
+            const int c = c0 + lane;
+            const long long v = c < w ? static_cast<long long>(lab[static_cast<long long>(r) * w + c]) : 0;
+            const int key = v >= 1 && v <= L ? static_cast<int>(v) : 0;
+            const unsigned grp = __match_any_sync(0xffffffffu, key);
+            const int cmin = __reduce_min_sync(grp, c), cmax = __reduce_max_sync(grp, c);
+            if (key && lane == __ffs(grp) - 1) {
+                atomicMin(&s_box[key - 1][0], r);
+                atomicMin(&s_box[key - 1][1], cmin);
+                atomicMax(&s_box[key - 1][2], r);
+                atomicMax(&s_box[key - 1][3], cmax);
+            }
+        }
+    __syncthreads();
+    if (tid < L) boxes[bi * L + tid] = make_int4(s_box[tid][0], s_box[tid][1], s_box[tid][2], s_box[tid][3]);
+}
+
+// k_refine_depth_pairs for virtual image img (grid b * L), with "in the mask" read as "carries label j+1" (labels at
+// their own width, compared as integers).  Every pixel that can pair carries label j+1, so both passes walk only the
+// instance's box, row-major: the pairs come in the image's row-major order and the ranks, stride and outputs are the
+// whole-frame scan's.  The mask count is the box's; the covered count (counts[3], the round-0 status gate) is taken
+// over the whole frame when count_cover is set (round 0) and left as it is otherwise.  Rows already done are skipped
+// from round 0 on (the absent rows: their counts are zeroed in round 0, so a trace shows them empty).
+template <typename T>
+__global__ void __launch_bounds__(RD_PAIR_THREADS, 1)
+    k_refine_depth_pairs_instances(const float *__restrict__ rdepth, const T *__restrict__ labels, int L,
+                                   const int4 *__restrict__ boxes, DepthIn obs, const double *__restrict__ pose,
+                                   const float *__restrict__ K, int h, int w, int max_points, double gate,
+                                   int count_cover, const State *__restrict__ state, int32_t *__restrict__ pix,
+                                   double *__restrict__ pX, double *__restrict__ pY, double *__restrict__ pN,
+                                   int32_t *__restrict__ counts)
+{
+    const int img = blockIdx.x;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    int32_t *cn = counts + img * RD_NCOUNT;
+    if (state[img].done) {
+        if (count_cover && tid < RD_NCOUNT) cn[tid] = 0;
+        return;
+    }
+    __shared__ int s_warp[RD_PAIR_THREADS / 32];
+    __shared__ int s_total, s_mask, s_cover;
+    __shared__ double s_pose[12];
+    const long long hw = static_cast<long long>(h) * w;
+    const int bi = img / L;
+    const long long own = img - bi * L + 1, ibase = bi * hw;
+    const float *ren = rdepth + img * hw;
+    const T *lab = labels + ibase;
+    const int4 box = boxes[img];
+    const int bw = box.w - box.y + 1;
+    const long long nbox = box.z >= box.x ? static_cast<long long>(box.z - box.x + 1) * bw : 0;
+    if (tid == 0) s_total = s_mask = s_cover = 0;
+    if (tid < 12) s_pose[tid] = pose[img * 12 + tid];
+    __syncthreads();
+    const Cam cam = load_cam(K + static_cast<size_t>(img) * 9);
+    auto mine = [&](long long p) -> bool { return static_cast<long long>(lab[p]) == own; };
+    // box position q -> image pixel
+    auto at = [&](long long q) -> long long { return (box.x + q / bw) * w + box.y + q % bw; };
+    // k_refine_depth_pairs's pair_at with mine(.) for the mask
+    auto pair_at = [&](long long p, double (&X)[3], double (&Y)[3], double (&nn)[3]) -> bool {
+        const float zr = ren[p];
+        if (!(zr > 0.f) || !mine(p)) return false;
+        const float zo = observed_depth(obs, ibase, p);
+        if (zo == 0.f) return false;
+        const int r = static_cast<int>(p / w), c = static_cast<int>(p - static_cast<long long>(r) * w);
+        if (r == 0 || r == h - 1 || c == 0 || c == w - 1) return false;
+        const long long nb[4] = {p + 1, p - 1, p + w, p - w};
+        float zn[4];
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            if (!mine(nb[q])) return false;
+            zn[q] = observed_depth(obs, ibase, nb[q]);
+            if (zn[q] == 0.f) return false;
+        }
+        double xn, yn;
+        pixel_ray(cam, r, c, xn, yn);
+        const double Z = zr;
+        const double d0 = ds(dm(Z, xn), s_pose[3]), d1 = ds(dm(Z, yn), s_pose[7]), d2 = ds(Z, s_pose[11]);
+#pragma unroll
+        for (int k = 0; k < 3; ++k) X[k] = da(da(dm(s_pose[k], d0), dm(s_pose[4 + k], d1)), dm(s_pose[8 + k], d2));
+        const double zo64 = zo;
+        Y[0] = dm(zo64, xn);
+        Y[1] = dm(zo64, yn);
+        Y[2] = zo64;
+        double Q[4][3];                           // the neighbours' observed points: c + 1, c - 1, r + 1, r - 1
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            double qx, qy;
+            pixel_ray(cam, r + (q == 2) - (q == 3), c + (q == 0) - (q == 1), qx, qy);
+            const double z = zn[q];
+            Q[q][0] = dm(z, qx);
+            Q[q][1] = dm(z, qy);
+            Q[q][2] = z;
+        }
+        double a[3], bv[3];
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+            a[k] = ds(Q[0][k], Q[1][k]);
+            bv[k] = ds(Q[2][k], Q[3][k]);
+        }
+        nn[0] = ds(dm(a[1], bv[2]), dm(a[2], bv[1]));
+        nn[1] = ds(dm(a[2], bv[0]), dm(a[0], bv[2]));
+        nn[2] = ds(dm(a[0], bv[1]), dm(a[1], bv[0]));
+        const double len = __dsqrt_rn(da(da(dm(nn[0], nn[0]), dm(nn[1], nn[1])), dm(nn[2], nn[2])));
+#pragma unroll
+        for (int k = 0; k < 3; ++k) nn[k] = dd(nn[k], len);
+        if (da(da(dm(nn[0], Y[0]), dm(nn[1], Y[1])), dm(nn[2], Y[2])) > 0.0)
+#pragma unroll
+            for (int k = 0; k < 3; ++k) nn[k] = -nn[k];
+        double dist;
+        const double e = plane_residual(s_pose, X, Y, nn, &dist);
+        return dist <= gate && isfinite(e);
+    };
+    int local = 0, lmask = 0, lcover = 0;
+    if (count_cover)
+        for (long long p = tid; p < hw; p += RD_PAIR_THREADS) lcover += ren[p] > 0.f;
+    for (long long base = 0; base < nbox; base += RD_CHUNK)
+        for (int q = 0; q < RF_PER_THREAD; ++q) {
+            const long long bq = base + static_cast<long long>(tid) * RF_PER_THREAD + q;
+            if (bq >= nbox) continue;
+            const long long p = at(bq);
+            lmask += mine(p);
+            double X[3], Y[3], nn[3];
+            if (pair_at(p, X, Y, nn)) ++local;
+        }
+    atomicAdd(&s_total, local);                   // integer sums: the same whatever the order
+    atomicAdd(&s_mask, lmask);
+    atomicAdd(&s_cover, lcover);
+    __syncthreads();
+    const int n = s_total;
+    const int stride = n > max_points ? (n + max_points - 1) / max_points : 1;
+    const size_t o = static_cast<size_t>(img) * max_points;
+    int running = 0;                              // pairs in earlier chunks
+    for (long long base = 0; base < nbox; base += RD_CHUNK) {
+        unsigned bits = 0;
+        for (int q = 0; q < RF_PER_THREAD; ++q) {
+            const long long bq = base + static_cast<long long>(tid) * RF_PER_THREAD + q;
+            double X[3], Y[3], nn[3];
+            if (bq < nbox && pair_at(at(bq), X, Y, nn)) bits |= 1u << q;
+        }
+        const int cnt = __popc(bits);
+        int incl = cnt;                           // inclusive scan over the warp
+#pragma unroll
+        for (int s = 1; s < 32; s <<= 1) {
+            const int y = __shfl_up_sync(0xffffffffu, incl, s);
+            if (lane >= s) incl += y;
+        }
+        if (lane == 31) s_warp[warp] = incl;
+        __syncthreads();
+        if (warp == 0) {
+            int t = lane < RD_PAIR_THREADS / 32 ? s_warp[lane] : 0;
+#pragma unroll
+            for (int s = 1; s < 32; s <<= 1) {
+                const int y = __shfl_up_sync(0xffffffffu, t, s);
+                if (lane >= s) t += y;
+            }
+            if (lane < RD_PAIR_THREADS / 32) s_warp[lane] = t;   // inclusive warp totals
+        }
+        __syncthreads();
+        int rank = running + (warp ? s_warp[warp - 1] : 0) + incl - cnt;
+        for (int q = 0; q < RF_PER_THREAD; ++q) {
+            if (!(bits >> q & 1u)) continue;
+            if (rank % stride == 0) {
+                const long long p = at(base + static_cast<long long>(tid) * RF_PER_THREAD + q);
+                const size_t j = o + rank / stride;
+                double X[3], Y[3], nn[3];
+                pair_at(p, X, Y, nn);
+                pix[j] = static_cast<int32_t>(p);
+#pragma unroll
+                for (int k = 0; k < 3; ++k) {
+                    pX[j * 3 + k] = X[k];
+                    pY[j * 3 + k] = Y[k];
+                    pN[j * 3 + k] = nn[k];
+                }
+            }
+            ++rank;
+        }
+        running += s_warp[RD_PAIR_THREADS / 32 - 1];
+        __syncthreads();                          // s_warp is rewritten by the next chunk
+    }
+    if (tid == 0) {
+        cn[0] = n ? (n + stride - 1) / stride : 0;
+        cn[1] = n;
+        cn[2] = s_mask;
+        if (count_cover) cn[3] = s_cover;
+    }
+}
+
 struct DepthLayout {
     unsigned long long *keys;
     float *depth, *pose32;
@@ -1240,12 +1452,18 @@ int pvnet_refine_depth_workspace_bytes(int b, int h, int w, int max_points, size
     return PVNET_OK;
 }
 
-int pvnet_refine_poses_depth(const uint8_t *mask, const void *depth, int depth_is_u16, float depth_scale,
-                             const double *poses_in, const float *K, int k_per_image, const float *verts,
-                             const int32_t *faces, int nv, int nf, int b, int h, int w, float near_clip,
-                             float far_clip, int rounds, double gate, int max_points, double *poses_out, int32_t *info,
-                             double *dist, const pvnet_refine_depth_trace_t *trace, void *workspace,
-                             size_t workspace_bytes, pvnet_stream_t stream)
+}  // extern "C"
+
+namespace {
+
+// Both depth entry points: inst null reads mask [b,h,w] with K shared or per image (k_per_image); inst non-null reads
+// its label map (mask unused), b counts the virtual images, K is per virtual image and the instances' boxes follow
+// the §28 layout in the workspace.
+int refine_depth(const uint8_t *mask, const void *depth, int depth_is_u16, float depth_scale, const double *poses_in,
+                 const float *K, int k_per_image, const float *verts, const int32_t *faces, int nv, int nf, int b, int h,
+                 int w, float near_clip, float far_clip, int rounds, double gate, int max_points, double *poses_out,
+                 int32_t *info, double *dist, const pvnet_refine_depth_trace_t *trace, void *workspace,
+                 size_t workspace_bytes, pvnet_stream_t stream, const InstArgs *inst = nullptr)
 {
     PV_CHECK_ARG(b >= 1 && h >= 1 && w >= 1 && nv >= 0 && nf >= 0, "bad dimension (b=%d, h=%d, w=%d, nv=%d, nf=%d)",
                  b, h, w, nv, nf);
@@ -1256,10 +1474,15 @@ int pvnet_refine_poses_depth(const uint8_t *mask, const void *depth, int depth_i
     PV_CHECK_ARG(gate > 0.0 && gate < INFINITY, "gate must be positive and finite (got %g)", gate);
     PV_CHECK_ARG(!depth_is_u16 || (depth_scale > 0.f && depth_scale < INFINITY),
                  "depth_scale must be positive and finite (got %g)", depth_scale);
-    PV_CHECK_ARG(mask && depth && poses_in && K && poses_out && (nf == 0 || faces) && (nv == 0 || verts),
+    PV_CHECK_ARG((mask || inst) && depth && poses_in && K && poses_out && (nf == 0 || faces) && (nv == 0 || verts),
                  "null pointer");
     size_t need = 0;
     pvnet_refine_depth_workspace_bytes(b, h, w, max_points, &need);
+    int4 *boxes = nullptr;
+    if (inst) {
+        boxes = reinterpret_cast<int4 *>(static_cast<char *>(workspace) + need);
+        need += pvnet::align_up(static_cast<size_t>(b) * sizeof(int4), 256);
+    }
     PV_CHECK_ARG(workspace && workspace_bytes >= need, "workspace %zu bytes < %zu", workspace_bytes, need);
     const DepthLayout L = carve_depth(workspace, b, h, w, max_points);
     size_t render_need = 0;
@@ -1269,13 +1492,42 @@ int pvnet_refine_poses_depth(const uint8_t *mask, const void *depth, int depth_i
     const DepthIn obs{depth, depth_is_u16 ? 1 : 0, depth_is_u16 ? depth_scale : 1.f};
     k_refine_init<<<(b + 127) / 128, 128, 0, st>>>(poses_in, poses_out, L.pose32, L.state, b);
     PV_LAUNCHED("k_refine_init");
+    if (inst) {
+        k_refine_absent<<<(b + 127) / 128, 128, 0, st>>>(inst->num, inst->L, b, L.state, L.pose32);
+        PV_LAUNCHED("k_refine_absent");
+#define PV_LABEL_BOXES(T)                                                                                              \
+    k_refine_label_boxes<T><<<b / inst->L, RD_BOX_THREADS, 0, st>>>(static_cast<const T *>(inst->labels), inst->L, h, \
+                                                                    w, boxes)
+        switch (inst->esz) {
+        case 1: PV_LABEL_BOXES(unsigned char); break;
+        case 2: PV_LABEL_BOXES(short); break;
+        case 4: PV_LABEL_BOXES(int); break;
+        default: PV_LABEL_BOXES(long long); break;
+        }
+#undef PV_LABEL_BOXES
+        PV_LAUNCHED("k_refine_label_boxes");
+    }
     for (int k = 0; k <= rounds; ++k) {
         const int rc = pvnet_render_mesh(verts, faces, nullptr, nv, nf, L.pose32, K, k_per_image, b, h, w, near_clip,
                                          far_clip, 0.5f, nullptr, L.depth, nullptr, L.keys, render_need, stream);
         if (rc != PVNET_OK) return rc;
-        k_refine_depth_pairs<<<b, RD_PAIR_THREADS, 0, st>>>(L.depth, mask, obs, poses_out, K, kstride, h, w,
-                                                            max_points, gate, k > 0, L.state, L.pix, L.X, L.Y, L.N,
-                                                            L.counts);
+        if (!inst) {
+            k_refine_depth_pairs<<<b, RD_PAIR_THREADS, 0, st>>>(L.depth, mask, obs, poses_out, K, kstride, h, w,
+                                                                max_points, gate, k > 0, L.state, L.pix, L.X, L.Y, L.N,
+                                                                L.counts);
+        } else {
+#define PV_DEPTH_PAIRS_INSTANCES(T)                                                                                    \
+    k_refine_depth_pairs_instances<T><<<b, RD_PAIR_THREADS, 0, st>>>(                                                  \
+        L.depth, static_cast<const T *>(inst->labels), inst->L, boxes, obs, poses_out, K, h, w, max_points, gate,      \
+        k == 0, L.state, L.pix, L.X, L.Y, L.N, L.counts)
+            switch (inst->esz) {
+            case 1: PV_DEPTH_PAIRS_INSTANCES(unsigned char); break;
+            case 2: PV_DEPTH_PAIRS_INSTANCES(short); break;
+            case 4: PV_DEPTH_PAIRS_INSTANCES(int); break;
+            default: PV_DEPTH_PAIRS_INSTANCES(long long); break;
+            }
+#undef PV_DEPTH_PAIRS_INSTANCES
+        }
         PV_LAUNCHED("k_refine_depth_pairs");
         if (k == 0 && trace) {
             const size_t np = static_cast<size_t>(b) * max_points;
@@ -1297,6 +1549,53 @@ int pvnet_refine_poses_depth(const uint8_t *mask, const void *depth, int depth_i
         PV_LAUNCHED("k_refine_finish");
     }
     return PVNET_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int pvnet_refine_poses_depth(const uint8_t *mask, const void *depth, int depth_is_u16, float depth_scale,
+                             const double *poses_in, const float *K, int k_per_image, const float *verts,
+                             const int32_t *faces, int nv, int nf, int b, int h, int w, float near_clip,
+                             float far_clip, int rounds, double gate, int max_points, double *poses_out, int32_t *info,
+                             double *dist, const pvnet_refine_depth_trace_t *trace, void *workspace,
+                             size_t workspace_bytes, pvnet_stream_t stream)
+{
+    return refine_depth(mask, depth, depth_is_u16, depth_scale, poses_in, K, k_per_image, verts, faces, nv, nf, b, h,
+                        w, near_clip, far_clip, rounds, gate, max_points, poses_out, info, dist, trace, workspace,
+                        workspace_bytes, stream);
+}
+
+int pvnet_refine_depth_instances_workspace_bytes(int b, int L, int h, int w, int max_points, size_t *bytes)
+{
+    PV_CHECK_ARG(b >= 1 && L >= 1 && L <= 32 && static_cast<long long>(b) * L <= 1024,
+                 "instance count %d outside 1..32 or b*L = %lld above 1024", L, static_cast<long long>(b) * L);
+    PV_CHECK_ARG(h >= 1 && w >= 1 && max_points >= 1, "non-positive dimension (h=%d, w=%d, max_points=%d)", h, w,
+                 max_points);
+    PV_CHECK_ARG(bytes, "null pointer");
+    *bytes = carve_depth(nullptr, b * L, h, w, max_points).bytes +
+             pvnet::align_up(static_cast<size_t>(b) * L * sizeof(int4), 256);
+    return PVNET_OK;
+}
+
+int pvnet_refine_poses_depth_instances(const void *labels, int labels_elem_size, const int32_t *num, int L,
+                                       const void *depth, int depth_is_u16, float depth_scale, const double *poses_in,
+                                       const float *K, const float *verts, const int32_t *faces, int nv, int nf, int b,
+                                       int h, int w, float near_clip, float far_clip, int rounds, double gate,
+                                       int max_points, double *poses_out, int32_t *info, double *dist,
+                                       const pvnet_refine_depth_trace_t *trace, void *workspace,
+                                       size_t workspace_bytes, pvnet_stream_t stream)
+{
+    PV_CHECK_ARG(labels && num && K, "null pointer");
+    PV_CHECK_ARG(labels_elem_size == 1 || labels_elem_size == 2 || labels_elem_size == 4 || labels_elem_size == 8,
+                 "labels_elem_size %d not 1, 2, 4 or 8", labels_elem_size);
+    PV_CHECK_ARG(b >= 1 && L >= 1 && L <= 32 && static_cast<long long>(b) * L <= 1024,
+                 "instance count %d outside 1..32 or b*L = %lld above 1024", L, static_cast<long long>(b) * L);
+    const InstArgs inst{labels, labels_elem_size, num, L};
+    return refine_depth(nullptr, depth, depth_is_u16, depth_scale, poses_in, K, 1, verts, faces, nv, nf, b * L, h, w,
+                        near_clip, far_clip, rounds, gate, max_points, poses_out, info, dist, trace, workspace,
+                        workspace_bytes, stream, &inst);
 }
 
 }  // extern "C"

@@ -18,7 +18,11 @@ viewing ray that the RGB cues barely see.
 
 `refine_poses_instances` refines every instance of a label map (`pvnet_refine_poses_instances`, DESIGN.md §30): each
 instance is refined alone, with a contour that leaves out its borders with other instances and a silhouette that
-leaves out what another instance may hide."""
+leaves out what another instance may hide.
+
+`refine_poses_depth_instances` refines every instance of a label map against the depth image
+(`pvnet_refine_poses_depth_instances`, DESIGN.md §31): each present row is `refine_poses_depth` on the mask of its own
+label, in one launch sequence for the whole map, without reading the instance counts on the host."""
 from __future__ import annotations
 
 import ctypes
@@ -385,6 +389,101 @@ def refine_poses_depth(mask, depth, poses, K, vertices, faces, near, far, gate, 
     res = (out,)
     if return_info:
         res += (dict(status=info[:, 0], pairs=info[:, 1], dist_before=dist[:, 0], dist_after=dist[:, 1]),)
+    if trace:
+        res += (tr,)
+    return res[0] if len(res) == 1 else res
+
+
+def refine_poses_depth_instances(labels, num, depth, poses, K, vertices, faces, near, far, gate, rounds=8,
+                                 max_points=4096, depth_scale=1.0, return_info=False, trace=False):
+    """`refine_poses_depth` for every instance of a label map (DESIGN.md §31).
+
+    labels [b,H,W] (uint8, int8, int16, int32 or int64; 0 background, j+1 instance j, any other nonzero value another
+    instance, so `ransac_voting_center`'s map works as it is), num [b] instance counts on the device, depth [b,H,W]
+    float32 or uint16 as `refine_poses_depth` reads it, poses [b,L,3,4] (1 <= L <= 32, b * L <= 1024), K [3,3] or
+    [b,3,3]: CUDA tensors on one device.  Row (i, j) with j < num[i] is bit for bit
+    `refine_poses_depth((labels[i] == j+1)[None], depth[i][None], poses[i, j][None], K[i], ...)`: a pixel pairs only
+    when it and its four 4-neighbours carry label j+1, so no pair or observed normal is taken across an instance
+    border.  A row with j >= num[i] keeps its input pose with status NO_INSTANCE, pairs 0 and NaN distances, and costs
+    no pairs or steps.  Without host synchronisation; graph-capturable.
+
+    -> poses float64 [b,L,3,4]; return_info: a dict of [b,L] tensors as `refine_poses_depth` returns; trace: its
+    first-round dict with one row per virtual image i * L + j (pixel indices r * W + c in image i; an absent row's
+    counts are 0)."""
+    _cuda_tensor("labels", labels)
+    _cuda_tensor("num", num)
+    _cuda_tensor("depth", depth)
+    _cuda_tensor("poses", poses)
+    if labels.dtype not in _INT_ELEM:
+        raise ValueError(f"labels must be an integer tensor, got {labels.dtype}")
+    if labels.dim() != 3:
+        raise ValueError(f"labels must be [b,H,W], got {tuple(labels.shape)}")
+    if poses.dim() != 4 or tuple(poses.shape[2:]) != (3, 4):
+        raise ValueError(f"poses must be [b,L,3,4], got {tuple(poses.shape)}")
+    b, L = int(poses.shape[0]), int(poses.shape[1])
+    h, w = int(labels.shape[1]), int(labels.shape[2])
+    if int(labels.shape[0]) != b:
+        raise ValueError(f"labels holds {labels.shape[0]} images for {b} pose rows")
+    if not 1 <= L <= 32 or b * L > 1024:
+        raise ValueError(f"L = {L} instances per image outside 1..32, or b * L = {b * L} above 1024")
+    if tuple(num.shape) != (b,) or num.device != poses.device:
+        raise ValueError(f"num must be a [{b}] tensor on {poses.device}")
+    B = b * L
+    _cuda_tensor("K", K)
+    check_cameras(K.shape, b)
+    # the checks refine_poses_depth makes, on the virtual images (a zero-stride stand-in for their masks)
+    stand_in = torch.zeros((), dtype=torch.uint8, device=labels.device).expand(B, h, w)
+    dev, _, _, _, near, far, rounds, gate, max_points = _check_common(
+        stand_in, poses.flatten(0, 1), K.expand(b, 3, 3).repeat_interleave(L, 0), vertices, faces, near, far, rounds,
+        gate, max_points, 9)
+    if depth.device != dev:
+        raise ValueError(f"depth must be on the poses' device {dev}, got {depth.device}")
+    if tuple(depth.shape) != (b, h, w):
+        raise ValueError(f"depth must be [{b},{h},{w}], got {tuple(depth.shape)}")
+    if depth.dtype not in (torch.float32, torch.uint16):
+        raise ValueError(f"depth must be float32 or uint16, got {depth.dtype}")
+    is_u16 = depth.dtype == torch.uint16
+    scale = float(depth_scale)
+    if not 0 < scale < math.inf:
+        raise ValueError(f"depth_scale must be positive and finite, got {depth_scale}")
+    lab = labels.contiguous()
+    d = depth.contiguous()
+    n32 = num.to(torch.int32).contiguous()
+    p = poses.flatten(0, 1).contiguous().double()
+    k = K.expand(b, 3, 3).float().repeat_interleave(L, 0).contiguous()        # one camera per virtual image
+    nv, nf = int(vertices.shape[0]), int(faces.shape[0])
+    v = vertices.contiguous().float()
+    f = faces.contiguous() if faces.dtype == torch.int32 else faces.clamp(-1, nv).to(torch.int32).contiguous()
+    out = torch.empty((B, 3, 4), dtype=torch.float64, device=dev)
+    info = torch.empty((B, 2), dtype=torch.int32, device=dev) if return_info else None
+    dist = torch.empty((B, 2), dtype=torch.float64, device=dev) if return_info else None
+    tr, tr_struct = None, None
+    if trace:
+        tr = dict(pair_idx=torch.full((B, max_points), -1, dtype=torch.int32, device=dev),
+                  counts=torch.zeros((B, 4), dtype=torch.int32, device=dev),
+                  X=torch.zeros((B, max_points, 3), dtype=torch.float64, device=dev),
+                  Y=torch.zeros((B, max_points, 3), dtype=torch.float64, device=dev),
+                  n=torch.zeros((B, max_points, 3), dtype=torch.float64, device=dev),
+                  normal_eq=torch.full((B, 27), math.nan, dtype=torch.float64, device=dev))
+        tr_struct = _native.RefineDepthTrace(*(tr[x].data_ptr() for x in ("pair_idx", "counts", "X", "Y", "n",
+                                                                          "normal_eq")))
+    lib = _native.lib()
+    with torch.cuda.device(dev):
+        need = ctypes.c_size_t()
+        _native.check(lib.pvnet_refine_depth_instances_workspace_bytes(b, L, h, w, max_points, ctypes.byref(need)),
+                      "pvnet_refine_depth_instances_workspace_bytes")
+        ws = torch.empty(need.value, dtype=torch.uint8, device=dev)
+        ptr = (lambda t: None if t is None else t.data_ptr())
+        _native.check(lib.pvnet_refine_poses_depth_instances(
+            lab.data_ptr(), _INT_ELEM[lab.dtype], n32.data_ptr(), L, d.data_ptr(), int(is_u16), scale, p.data_ptr(),
+            k.data_ptr(), ptr(v) if nv else None, ptr(f) if nf else None, nv, nf, b, h, w, near, far, rounds, gate,
+            max_points, out.data_ptr(), ptr(info), ptr(dist), None if tr_struct is None else ctypes.byref(tr_struct),
+            ws.data_ptr(), need.value, ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
+            "pvnet_refine_poses_depth_instances")
+    res = (out.view(b, L, 3, 4),)
+    if return_info:
+        fields = dict(status=info[:, 0], pairs=info[:, 1], dist_before=dist[:, 0], dist_after=dist[:, 1])
+        res += ({key: x.view(b, L) for key, x in fields.items()},)
     if trace:
         res += (tr,)
     return res[0] if len(res) == 1 else res
